@@ -80,6 +80,7 @@ int ctx_reserve(eu_ctx* c, int64_t rows, int64_t table_slots) {
   if ((rc = regrow(&c->d_blkpre, rows / 256 + 66))) return rc;
   if ((rc = regrow(&c->d_blkmul, rows / 256 + 66))) return rc;
   if ((rc = regrow(&c->d_live, rows))) return rc;
+  if ((rc = regrow(&c->d_dup, rows))) return rc;
   if (!c->d_nlive && (rc = regrow(&c->d_nlive, 4))) return rc;
   if ((rc = regrow(&c->d_front[0], rows))) return rc;
   if ((rc = regrow(&c->d_front[1], rows))) return rc;
@@ -96,6 +97,28 @@ int ctx_misc(eu_ctx* c, int64_t bytes) {
   c->d_misc = p;
   if (rc) { c->misc_bytes = 0; return rc; }
   c->misc_bytes = bytes;
+  return EU_OK;
+}
+
+int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots) {
+  if (rows <= c->agg_rows && table_slots <= c->agg_slots) return EU_OK;
+  int rc;
+  if ((rc = refuse_growth_in_capture(c, "the aggregation scratch"))) return rc;
+  EU_CUDA(cudaStreamSynchronize(c->stream));
+  if (table_slots > c->agg_slots) {
+    c->agg_slots = 0;
+    if ((rc = regrow(&c->d_agg_tab, table_slots))) return rc;
+    EU_CUDA(cudaMemsetAsync(c->d_agg_tab, 0, sizeof(unsigned long long) * (size_t)table_slots, c->stream));   // all free
+    c->agg_slots = table_slots;
+  }
+  if (rows > c->agg_rows) {
+    c->agg_rows = 0;
+    if ((rc = regrow(&c->d_agg_src, rows))) return rc;
+    if ((rc = regrow(&c->d_agg_rep, rows))) return rc;
+    if ((rc = regrow(&c->d_agg_slot, rows))) return rc;
+    if (!c->d_agg_nrep && (rc = regrow(&c->d_agg_nrep, 1))) return rc;
+    c->agg_rows = rows;
+  }
   return EU_OK;
 }
 
@@ -164,8 +187,9 @@ int eu_ctx_destroy(eu_ctx* c) {
   cudaSetDevice(c->g->device);
   cudaStreamSynchronize(c->stream);
   cudaFree(c->d_rng); cudaFree(c->d_dedup); cudaFree(c->d_first); cudaFree(c->d_rowof);
-  cudaFree(c->d_elig); cudaFree(c->d_state); cudaFree(c->d_emask); cudaFree(c->d_woff); cudaFree(c->d_blkpre); cudaFree(c->d_blkmul); cudaFree(c->d_live); cudaFree(c->d_nlive); cudaFree(c->d_front[0]); cudaFree(c->d_front[1]);
+  cudaFree(c->d_elig); cudaFree(c->d_state); cudaFree(c->d_emask); cudaFree(c->d_woff); cudaFree(c->d_blkpre); cudaFree(c->d_blkmul); cudaFree(c->d_live); cudaFree(c->d_dup); cudaFree(c->d_nlive); cudaFree(c->d_front[0]); cudaFree(c->d_front[1]);
   cudaFree(c->d_misc); cudaFree(c->d_stage); cudaFree(c->d_walkv);
+  cudaFree(c->d_agg_tab); cudaFree(c->d_agg_src); cudaFree(c->d_agg_rep); cudaFree(c->d_agg_slot); cudaFree(c->d_agg_nrep);
   for (int i = 0; i < 2; ++i) { if (c->aux[i]) cudaStreamDestroy(c->aux[i]); if (c->ev_join[i]) cudaEventDestroy(c->ev_join[i]); }
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   if (c->h_pin) cudaFreeHost(c->h_pin);

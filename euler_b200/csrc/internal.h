@@ -118,9 +118,17 @@ struct eu_ctx {
   uint32_t* d_woff = nullptr;        // [rows/32] F^(count in earlier warps of the block)
   uint32_t* d_blkpre = nullptr;      // [rows/256] count in earlier blocks
   uint32_t* d_blkmul = nullptr;      // [rows/256] F^that count
-  int32_t* d_live = nullptr;         // [rows] rows that sample, compacted by k_prepare
-  unsigned int* d_nlive = nullptr;   // their number
+  int32_t* d_live = nullptr;         // [rows] rows that draw (eligible first occurrences), compacted by k_prepare
+  int32_t* d_dup = nullptr;          // [rows] eligible duplicates, compacted by k_prepare
+  unsigned int* d_nlive = nullptr;   // [0]: rows in d_live, [1]: rows in d_dup
   unsigned long long* d_front[2] = {nullptr, nullptr};  // engine-id frontier ping-pong [rows]
+  // segment dedup of the fused SAGE aggregation (mp_ops.cu), sized for agg_rows rows and agg_slots table slots
+  int64_t agg_rows = 0, agg_slots = 0;
+  unsigned long long* d_agg_tab = nullptr;  // [agg_slots] {hash bits, representative + 1}; all-free (0) between calls
+  int32_t* d_agg_src = nullptr;      // [agg_rows] per row: itself (representative), its representative, or -1 (no neighbor)
+  int32_t* d_agg_rep = nullptr;      // [agg_rows] representatives, compacted
+  uint32_t* d_agg_slot = nullptr;    // [agg_rows] the table slot each representative claimed
+  unsigned int* d_agg_nrep = nullptr;  // their number
   // extra scratch for walks / scatter
   void* d_misc = nullptr;
   int64_t misc_bytes = 0;
@@ -156,11 +164,18 @@ struct EuProfScope {
 };
 
 namespace eu {
+// Rows from which a launch looks for repeated work (sampler: duplicate seeds copy their first occurrence's draws; fused SAGE
+// aggregation: each distinct segment is reduced once).  The extra passes have a fixed cost -- a launch and a latency-bound
+// classification -- that only a large hop repays: a fanout's repeats sit in its deeper hops, where a seed's draws with
+// replacement come back as seeds (headline step on an H100: 69 % of the live hop-2 rows repeat; its 32K-row first hop and
+// the 64K-row hops of the heterogeneous config are slower with the extra passes).
+static constexpr int64_t kRepeatMinRows = (int64_t)1 << 17;
 int ctx_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);
 int64_t hop_scratch_rows(int nb, int64_t rows_b);
 int64_t hop_table_slots(int nb, int64_t rows_b);
 int64_t hop_table_cap(int64_t rows_b);   // dedup slots per batch (region stride = cap + 1)
 int ctx_misc(eu_ctx* c, int64_t bytes);
+int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
 int ctx_stage(eu_ctx* c, int64_t host_bytes, int64_t dev_bytes);
 int graph_build_sampler(eu_graph* g);

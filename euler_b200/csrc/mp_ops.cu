@@ -15,9 +15,13 @@
 //   unsorted indices: vector atomics (red.global.add.v4.f32), order-free, within 1e-5 relative.
 #include <stdlib.h>
 
+#include <cooperative_groups.h>
+
 #include <algorithm>
 
 #include "internal.h"
+
+namespace cg = cooperative_groups;
 
 namespace eu {
 
@@ -192,19 +196,84 @@ __global__ void k_mean_div(float* __restrict__ out, int64_t D, int64_t size, con
 
 // ---------------------------------------------------------------------------- fused SAGE mean
 // out[r,:] = (sum_j feat[row(ids[r*count+j]),:]) / (count + 1e-7), j ascending (== get_dense_feature
-// followed by scatter_mean over edge_src = repeat(range(rows), count)).  One warp per output row;
-// the `count` id->row lookups run in parallel across lanes, then NV float4 per lane are accumulated.
+// followed by scatter_mean over edge_src = repeat(range(rows), count)).
+//
+// A fanout repeats segments: a seed sampled `count` times with replacement hands the same node to the next hop many times, and
+// the sampler gives every copy of a node the same draws.  Two rows whose `count` ids are equal in the same order have
+// bit-identical outputs, so each distinct segment is reduced once, in three passes:
+//   k_sage_classify   gives every row a source: itself (a representative), an earlier-claimed row with the same segment, or
+//                     none (no id exists: zeros, no feature row is read);
+//   k_sage_mean       reduces the representatives only;
+//   k_sage_broadcast  copies each representative's output to its duplicates, zero-fills the rows without a neighbor, and frees
+//                     the table slots the representatives claimed.
+// Segments are found through an open-addressing table of 64-bit slots {upper 32 bits of the segment hash, representative + 1},
+// 0 = free.  One CAS claims a slot and publishes its representative together, so no reader sees a claimed slot without its
+// row.  A hash match is confirmed id by id: the same ids in another order are another segment (float addition does not
+// associate).  The table is all-free between calls (allocated zeroed; every claimed slot is freed by the call that claimed it).
+__global__ void __launch_bounds__(256) k_sage_classify(DevGraph g, const unsigned long long* __restrict__ ids, int64_t rows,
+                                                       int32_t count, unsigned long long* tab, unsigned long long mask,
+                                                       int32_t* __restrict__ src, int32_t* __restrict__ reps,
+                                                       uint32_t* __restrict__ rep_slot, unsigned int* n_rep) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  // one thread per row: its `count` id loads are independent, and a capped grid (EU_SAGE_CTAS) keeps many rows in flight
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < rows; r += stride) {
+    const unsigned long long* seg = ids + r * count;
+    unsigned long long h = 0;
+    bool any = false;
+#pragma unroll 4
+    for (int32_t j = 0; j < count; ++j) {
+      const unsigned long long id = __ldg(seg + j);
+      any |= lookup_row(g, id) >= 0;
+      h = mix64(h + id + 1);   // a chain: the hash depends on the order of the ids
+    }
+    if (!any) { src[r] = -1; continue; }
+    const unsigned long long tag = h & 0xFFFFFFFF00000000ull;
+    unsigned long long p = h & mask;
+    while (true) {
+      unsigned long long sl = *reinterpret_cast<volatile unsigned long long*>(tab + p);   // hub segments recur: look before any CAS
+      if (sl == 0ull) {
+        sl = atomicCAS(tab + p, 0ull, tag | (unsigned long long)(r + 1));
+        if (sl == 0ull) {
+          src[r] = (int32_t)r;
+          // one counter for the whole launch: the winners that are converged here append with one atomic
+          const cg::coalesced_group grp = cg::coalesced_threads();
+          unsigned int q = 0;
+          if (grp.thread_rank() == 0) q = atomicAdd(n_rep, grp.size());
+          q = grp.shfl(q, 0) + grp.thread_rank();
+          reps[q] = (int32_t)r;
+          rep_slot[q] = (uint32_t)p;
+          break;
+        }
+      }
+      if ((sl & 0xFFFFFFFF00000000ull) == tag) {
+        const int64_t o = (int64_t)(sl & 0xFFFFFFFFull) - 1;
+        const unsigned long long* os = ids + o * count;
+        bool same = true;
+#pragma unroll 4
+        for (int32_t j = 0; j < count; ++j) same &= __ldg(seg + j) == __ldg(os + j);
+        if (same) { src[r] = (int32_t)o; break; }
+      }
+      p = (p + 1) & mask;
+    }
+  }
+}
+
+// One warp per representative (list[0 .. *n_list)), or per row when there is no list; the `count` id->row lookups run in parallel across lanes, then NV float4
+// per lane are accumulated.
 // NV float4 per lane: rows of up to NV * 128 floats.  FULL: the width is exactly NV * 128 (128 / 256: no column guards, the
 // width is a compile-time constant); otherwise any multiple of 4 up to NV * 128 (e.g. 64 of configs[4]) with guarded columns.
 template <int NV, bool FULL>
 __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned long long* __restrict__ ids,
-                                                   int64_t rows, int32_t count, bool mean, float* __restrict__ out) {
+                                                   int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
+                                                   int32_t count, bool mean, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int32_t fd = FULL ? NV * 128 : g.feat_dim;    // == dim, a multiple of 4, <= NV * 128 (checked by the launcher)
   const float* __restrict__ feat = g.feat + lane * 4;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int64_t n = list ? (int64_t)__ldg(n_list) : rows;
   // grid-stride, one warp per output row (the launcher may cap the grid: EU_SAGE_CTAS CTAs per SM)
-  for (int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; r < rows; r += nwarps) {
+  for (int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; q < n; q += nwarps) {
+  const int64_t r = list ? (int64_t)__ldg(list + q) : q;
   float4 acc[NV];
 #pragma unroll
   for (int v = 0; v < NV; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -253,15 +322,17 @@ __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned lo
   }
 }
 
-// generic width fallback: G lanes... one warp per row, scalar columns
+// generic width fallback: one warp per representative, scalar columns
 __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const unsigned long long* __restrict__ ids,
-                                                           int64_t rows, int32_t count, int32_t dim, bool mean,
-                                                           float* __restrict__ out) {
+                                                           int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
+                                                           int32_t count, int32_t dim, bool mean, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int32_t fd = g.feat_dim;
   const float denom = __fadd_rn((float)count, 1e-7f);
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t r = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; r < rows; r += nwarps)
+  const int64_t n = list ? (int64_t)__ldg(n_list) : rows;
+  for (int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; q < n; q += nwarps) {
+    const int64_t r = list ? (int64_t)__ldg(list + q) : q;
     for (int32_t d = lane; d < dim; d += 32) {
       float acc = 0.f;
       for (int32_t j = 0; j < count; ++j) {
@@ -270,6 +341,33 @@ __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const uns
       }
       out[r * (int64_t)dim + d] = mean ? __fdiv_rn(acc, denom) : acc;
     }
+  }
+}
+
+// G lanes per row (G a power of two): a duplicate gets its representative's output, a row without a neighbor gets +0.0 (what
+// the reduction writes for it: it starts at +0.0 and adds nothing); representatives are already done.  Then every slot the
+// representatives claimed is freed.
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_sage_broadcast(const int32_t* __restrict__ src, int64_t rows, int32_t dim, int G,
+                                                        const uint32_t* __restrict__ rep_slot, const unsigned int* __restrict__ n_rep,
+                                                        unsigned long long* tab, float* out) {
+  const int sh = 31 - __clz(G);
+  const int sub = (int)(threadIdx.x & (G - 1));
+  const int64_t gtid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t nthreads = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t r = gtid >> sh; r < rows; r += nthreads >> sh) {
+    const int64_t s = __ldg(src + r);
+    if (s == r) continue;
+    float* o = out + r * (int64_t)dim;
+    const float* f = s >= 0 ? out + s * (int64_t)dim : nullptr;   // a representative's row: not written by this kernel
+    if (VEC) {
+      for (int32_t d = sub * 4; d < dim; d += G * 4) st4(o + d, f ? ldg4(f + d) : make_float4(0.f, 0.f, 0.f, 0.f));
+    } else {
+      for (int32_t d = sub; d < dim; d += G) o[d] = f ? __ldg(f + d) : 0.f;
+    }
+  }
+  const int64_t n = (int64_t)__ldg(n_rep);
+  for (int64_t q = gtid; q < n; q += nthreads) tab[__ldg(rep_slot + q)] = 0ull;
 }
 
 static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
@@ -379,23 +477,46 @@ static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int
   if (!c || rows < 0 || count < 0 || dim <= 0 || (rows > 0 && (!nbr_ids || !out))) { set_error("eu_sage_mean_aggregate: bad argument"); return EU_ERR_INVALID; }
   EU_CUDA(cudaSetDevice(c->g->device));
   if (rows == 0) return EU_OK;
+  cudaStream_t s = c->stream;
   const DevGraph& d = c->g->d;
-  const unsigned blocks = capped_grid(ceil_div(rows * 32, 256), "EU_SAGE_CTAS", 0);
   const unsigned long long* ids = (const unsigned long long*)nbr_ids;
-  EuProfScope ps(c, mean ? "k_sage_mean" : "k_sage_add", rows);
+  // otherwise k_sage_mean reduces every row (reps == null); the dedup scratch holds 32-bit row indices
+  const bool dedup = rows >= kRepeatMinRows && rows < ((int64_t)1 << 31);
+  int64_t cap = 64;   // table slots of this call: a power of two >= 2 * rows
+  while (cap < 2 * rows) cap <<= 1;
+  if (dedup) {
+    int rc = agg_reserve(c, rows, cap);
+    if (rc) return rc;
+    EU_CUDA(cudaMemsetAsync(c->d_agg_nrep, 0, sizeof(unsigned int), s));
+    EuProfScope ps(c, "k_sage_classify", rows);
+    k_sage_classify<<<capped_grid(ceil_div(rows, 256), "EU_SAGE_CTAS", 0), 256, 0, s>>>(d, ids, rows, count, c->d_agg_tab, (unsigned long long)cap - 1,
+                                                                                      c->d_agg_src, c->d_agg_rep, c->d_agg_slot, c->d_agg_nrep);
+    EU_LAUNCHED();
+  }
+  const unsigned blocks = capped_grid(ceil_div(rows * 32, 256), "EU_SAGE_CTAS", 0);
+  const int32_t* reps = dedup ? c->d_agg_rep : nullptr;
+  const unsigned int* nrep = c->d_agg_nrep;
+  { EuProfScope ps(c, mean ? "k_sage_mean" : "k_sage_add", rows);
   // float4 path: one slot of the full stored width, a multiple of 4 floats up to 1024 (D = 64 of configs[4], 128, 256, ...)
   const bool v4 = d.n < ((int64_t)1 << 31) && d.n_slots == 1 && dim == d.feat_dim && (dim & 3) == 0 && dim <= 1024 && aligned16(out) && aligned16(d.feat);
-  if (v4 && dim == 128) k_sage_mean<1, true><<<blocks, 256, 0, c->stream>>>(d, ids, rows, count, mean, out);
-  else if (v4 && dim == 256) k_sage_mean<2, true><<<blocks, 256, 0, c->stream>>>(d, ids, rows, count, mean, out);
-  else if (v4 && dim <= 128) k_sage_mean<1, false><<<blocks, 256, 0, c->stream>>>(d, ids, rows, count, mean, out);
-  else if (v4 && dim <= 256) k_sage_mean<2, false><<<blocks, 256, 0, c->stream>>>(d, ids, rows, count, mean, out);
-  else if (v4 && dim <= 512) k_sage_mean<4, false><<<blocks, 256, 0, c->stream>>>(d, ids, rows, count, mean, out);
-  else if (v4) k_sage_mean<8, false><<<blocks, 256, 0, c->stream>>>(d, ids, rows, count, mean, out);
-  else k_sage_mean_generic<<<blocks, 256, 0, c->stream>>>(d, ids, rows, count, dim, mean, out);
+  if (v4 && dim == 128) k_sage_mean<1, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim == 256) k_sage_mean<2, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 128) k_sage_mean<1, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 256) k_sage_mean<2, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 512) k_sage_mean<4, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4) k_sage_mean<8, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else k_sage_mean_generic<<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, dim, mean, out); }
+  EU_LAUNCHED();
+  if (!dedup) return EU_OK;
+  { EuProfScope ps(c, "k_sage_broadcast", rows);
+    const bool vec = (dim & 3) == 0 && aligned16(out);
+    const int G = vec ? lanes_per_row(dim) : (dim >= 32 ? 32 : 1);
+    const unsigned bb = capped_grid(ceil_div(rows * G, 256), "EU_SAGE_CTAS", 0);
+    if (vec) k_sage_broadcast<true><<<bb, 256, 0, s>>>(c->d_agg_src, rows, dim, G, c->d_agg_slot, nrep, c->d_agg_tab, out);
+    else k_sage_broadcast<false><<<bb, 256, 0, s>>>(c->d_agg_src, rows, dim, G, c->d_agg_slot, nrep, c->d_agg_tab, out); }
   EU_LAUNCHED();
   return EU_OK;
 }
-
 
 int eu_sage_mean_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out) {
   return fanout_aggregate(c, nbr_ids, rows, count, dim, true, out);

@@ -15,8 +15,8 @@
 // stream is reproduced by (1) a device hash that resolves each seed's first occurrence
 // (ID_UNIQUE order), (2) a multiplicative prefix "scan" that hands every first-occurrence row the
 // engine state it would have had in the serial loop, (3) lanes jumping ahead A^(2*k*lane).
-// Duplicate seeds re-derive the identical row from the first occurrence's state, so there is no
-// gather pass and the frontier (engine ids) stays in HBM between hops.
+// Duplicate seeds re-derive the identical row from the first occurrence's state, or, in hops of at least kRepeatMinRows
+// seeds, copy the first occurrence's outputs (k_copy_dups); the frontier (engine ids) stays in HBM between hops.
 #include <algorithm>
 
 #include <stdlib.h>
@@ -114,8 +114,10 @@ struct PrepOut {
   long long default_node;
   HashSlot* next_tabs;
   int64_t next_cap_b;
-  int32_t* live;           // [nb*rows_b] global indices of rows that sample
+  int32_t* live;           // [nb*rows_b] global indices of the rows that draw: eligible first occurrences
   unsigned int* n_live;    // their number (zeroed before the launch)
+  int32_t* dup;            // [nb*rows_b] global indices of eligible duplicates (k_copy_dups fills them in); or null: they draw
+  unsigned int* n_dup;     // their number (zeroed before the launch)
 };
 
 // ---------------------------------------------------------------------------- 2. prepare
@@ -170,15 +172,23 @@ __global__ void __launch_bounds__(kPrepBlock) k_prepare(DevGraph g, const HashSl
                          li * (int64_t)po.count);
     }
   }
-  // compact the rows that do sample (order is irrelevant: a row's engine state depends only on its position)
-  {
-    const uint32_t om = __ballot_sync(0xffffffffu, own);
-    uint32_t basepos = 0;
-    if (lane == 0 && om) basepos = atomicAdd(po.n_live, (unsigned int)__popc(om));
-    basepos = __shfl_sync(0xffffffffu, basepos, 0);
-    if (own) po.live[basepos + __popc(om & ((1u << lane) - 1u))] = (int32_t)(b * gm.rows_b + li);
-  }
+  // compact the rows that draw (order is irrelevant: a row's engine state depends only on its position).  An eligible duplicate
+  // would draw exactly what its first occurrence draws (same graph row, same engine state): given a duplicate list (hops of
+  // kRepeatMinRows rows or more) it goes there and k_copy_dups hands it the first occurrence's outputs once k_sample has
+  // written them; otherwise it draws again.
   const uint32_t m = __ballot_sync(0xffffffffu, e);
+  {
+    const uint32_t lm = po.dup ? m : __ballot_sync(0xffffffffu, own);   // without a duplicate list every eligible row draws
+    const uint32_t dm = po.dup ? __ballot_sync(0xffffffffu, own && !e) : 0u;
+    uint32_t lbase = 0, dbase = 0;
+    if (lane == 0 && lm) lbase = atomicAdd(po.n_live, (unsigned int)__popc(lm));
+    if (lane == 0 && dm) dbase = atomicAdd(po.n_dup, (unsigned int)__popc(dm));
+    lbase = __shfl_sync(0xffffffffu, lbase, 0);
+    dbase = __shfl_sync(0xffffffffu, dbase, 0);
+    const uint32_t below = (1u << lane) - 1u;
+    if (e || (own && !po.dup)) po.live[lbase + __popc(lm & below)] = (int32_t)(b * gm.rows_b + li);
+    else if (own) po.dup[dbase + __popc(dm & below)] = (int32_t)(b * gm.rows_b + li);
+  }
   if (lane == 0) s_w[wid] = __popc(m);
   __syncthreads();
   if (lane == 0) {  // rows_pad is a multiple of 256: every group of the block exists in the scratch arrays
@@ -582,6 +592,34 @@ __global__ void __launch_bounds__(256, CTAS) k_sample(DevGraph g, SampleArgs a) 
   }
 }
 
+// ---------------------------------------------------------------------------- 5. duplicates
+// Eligible duplicate seeds (k_prepare's second list) take their first occurrence's outputs: engine ids, TF-packed ids, weights
+// and types.  k_sample never saw them, and nothing it does for a row depends on which of the equal rows it is, beyond addresses:
+//   * the draws, `keep` (the row's first drawn id) and the mode 1/2 `bad` fill are functions of the graph row and the engine
+//     state, and a duplicate's are its first occurrence's (same id; the state is derived from the first occurrence's position);
+//   * the next hop's dedup table keeps each id's minimum index.  A duplicate's ids are its first occurrence's ids at larger
+//     indices (li * count + j > f * count + j), so entering them would change no slot;
+//   * rows_act (sharded owners) bounds both lists alike: k_prepare lists only rows below it.
+// One lane group (SG lanes, as k_sample) per duplicate row; the grid strides over the device count.
+__global__ void __launch_bounds__(256) k_copy_dups(Geom gm, int32_t count, int sg_log, const int32_t* __restrict__ dup,
+                                                   const unsigned int* __restrict__ n_dup, const int32_t* __restrict__ first,
+                                                   unsigned long long* eng_ids, long long* out_ids, float* out_w, int32_t* out_t) {
+  const int sl = threadIdx.x & ((1 << sg_log) - 1);
+  const int64_t total = (int64_t)__ldg(n_dup);
+  const int64_t stride = ((int64_t)gridDim.x * blockDim.x) >> sg_log;
+  for (int64_t q = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> sg_log; q < total; q += stride) {
+    const int64_t w = __ldg(dup + q);
+    const int bidx = (int)(w / gm.rows_b);
+    const int64_t li = w - bidx * gm.rows_b;
+    const int64_t f = __ldg(first + bidx * gm.rows_pad + li);
+    const int64_t src = (bidx * gm.rows_b + f) * count, dst = w * (int64_t)count;
+    for (int32_t j = sl; j < count; j += 1 << sg_log) {
+      if (eng_ids) eng_ids[dst + j] = eng_ids[src + j];
+      if (out_ids) { out_ids[dst + j] = out_ids[src + j]; out_w[dst + j] = out_w[src + j]; out_t[dst + j] = out_t[src + j]; }
+    }
+  }
+}
+
 __global__ void k_bump_calls(EuRngState* rngs, int nb) {
   if (threadIdx.x < nb) rngs[threadIdx.x].calls += 1;
 }
@@ -754,7 +792,9 @@ int hop(eu_ctx* c, const unsigned long long* seeds, int64_t rows_b, const int32_
     po.count = count; po.default_node = default_node;
     if (chain) { po.next_tabs = ntabs; po.next_cap_b = ng.cap_b; }
     po.live = c->d_live; po.n_live = c->d_nlive;
-    EU_CUDA(cudaMemsetAsync(c->d_nlive, 0, sizeof(unsigned int), s));
+    // raw mode draws every occurrence: it has no duplicates
+    if (!raw && rows >= kRepeatMinRows) { po.dup = c->d_dup; po.n_dup = c->d_nlive + 1; }
+    EU_CUDA(cudaMemsetAsync(c->d_nlive, 0, 2 * sizeof(unsigned int), s));
     k_prepare<<<dim3((unsigned)gm.nblk_b, (unsigned)nb), tb, 0, s>>>(d, raw ? nullptr : tabs, gm, seeds, a.et, a.mode, F, upr, c->d_first,
                                                                      c->d_rowof, c->d_emask, c->d_woff, c->d_blkpre, c->d_blkmul,
                                                                      c->d_rng, po); }
@@ -773,6 +813,11 @@ int hop(eu_ctx* c, const unsigned long long* seeds, int64_t rows_b, const int32_
   }
   { EuProfScope ps(c, "k_sample<minstd>", rows); if (ctas == 6) k_sample<false, 6><<<blocks, 256, 0, s>>>(d, a); else k_sample<false, 8><<<blocks, 256, 0, s>>>(d, a); }
   EU_LAUNCHED();
+  if (!raw && rows >= kRepeatMinRows) {
+    EuProfScope ps(c, "k_copy_dups", rows);
+    k_copy_dups<<<blocks, 256, 0, s>>>(gm, count, a.sg_log, c->d_dup, c->d_nlive + 1, c->d_first, eng_ids, (long long*)out_ids, out_w, out_t);
+    EU_LAUNCHED();
+  }
   return EU_OK;
 }
 
