@@ -107,6 +107,7 @@ SIGNATURES = {
     "eu_get_dense_feature_host": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
     "eu_get_full_neighbor": (C.c_int, [_P, _P, _I64, _P, _I32, _I64, _P, _P, _P, _P]),
     "eu_unique": (C.c_int, [_P, _P, _I64, _P, _P, _P]),
+    "eu_full_neighbor_hop": (C.c_int, [_P, _P, _I64, _P, _I32, _I32, _I64, _P, _P, _P, _P, _P, _P, _P, _P]),
     "eu_get_node_type": (C.c_int, [_P, _P, _I64, _P]),
     "eu_get_node_type_host": (C.c_int, [_P, _P, _I64, _P]),
     "eu_get_node_weight_host": (C.c_int, [_P, _P, _I64, _P]),

@@ -36,6 +36,11 @@ extern std::atomic<uint64_t> g_launches;
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+struct ETList {           // an edge-type list passed by value to the full-neighbor kernels
+  int32_t K;
+  int32_t v[EU_MAX_ETYPES];
+};
+
 struct TypeSampler {      // FastWeightedCollection of one node type (fast_weighted_collection.h:27-100)
   int64_t n = 0;
   unsigned long long* ids = nullptr;  // device, sampler order

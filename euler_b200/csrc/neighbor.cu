@@ -16,11 +16,6 @@
 
 namespace eu {
 
-struct ETList {
-  int32_t K;
-  int32_t v[EU_MAX_ETYPES];
-};
-
 __global__ void k_full_len(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t B, ETList et,
                            long long* __restrict__ out_ptr /* [B+1]; [0] = 0, [i+1] = len(i) */) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;

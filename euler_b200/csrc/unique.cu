@@ -7,46 +7,14 @@
 #include <cub/device/device_scan.cuh>
 
 #include "internal.h"
+#include "uq.cuh"
 
 namespace eu {
-
-// slot = {id + 1, min index}; key 0 = free; id 2^64-1 (tag overflow) lives in the extra slot [mask + 1]
-__device__ __forceinline__ void uq_insert(HashSlot* tab, unsigned long long mask, unsigned long long id, unsigned long long i) {
-  const unsigned long long tag = id + 1;
-  if (tag == 0ull) { atomicMin(&tab[mask + 1].row, i); return; }
-  unsigned long long h = mix64(id) & mask;
-  while (true) {
-    const unsigned long long prev = atomicCAS(&tab[h].key, 0ull, tag);
-    if (prev == 0ull || prev == tag) { atomicMin(&tab[h].row, i); return; }
-    h = (h + 1) & mask;
-  }
-}
-
-__device__ __forceinline__ unsigned long long uq_first(const HashSlot* tab, unsigned long long mask, unsigned long long id) {
-  const unsigned long long tag = id + 1;
-  if (tag == 0ull) return tab[mask + 1].row;
-  unsigned long long h = mix64(id) & mask;
-  while (true) {
-    const ulonglong2 s = *reinterpret_cast<const ulonglong2*>(tab + h);
-    if (s.x == tag) return s.y;
-    h = (h + 1) & mask;
-  }
-}
-
-__global__ void k_uq_clear(HashSlot* tab, int64_t slots) {
-  for (int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; s < slots; s += (int64_t)gridDim.x * blockDim.x) {
-    tab[s].key = 0ull; tab[s].row = kEmptyRow;
-  }
-}
 
 __global__ void k_uq_insert(HashSlot* tab, unsigned long long mask, const unsigned long long* __restrict__ ids, int64_t n) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const unsigned long long id = ids[i];
-  // runs of equal ids (default fill, hubs) would hammer one slot: the lowest lane of each group carries the group's minimum
-  const unsigned peers = __match_any_sync(__activemask(), id);
-  if ((threadIdx.x & 31) != __ffs(peers) - 1) return;
-  uq_insert(tab, mask, id, (unsigned long long)i);
+  uq_insert_warp(tab, mask, ids[i], (unsigned long long)i);
 }
 
 __global__ void k_uq_first(const HashSlot* tab, unsigned long long mask, const unsigned long long* __restrict__ ids, int64_t n,
@@ -81,8 +49,7 @@ extern "C" int eu_unique(eu_ctx* c, const int64_t* ids, int64_t n, int64_t* uniq
     if (n_unique) EU_CUDA(cudaMemsetAsync(n_unique, 0, sizeof(int64_t), s));
     return EU_OK;
   }
-  int64_t cap = 64;
-  while (cap < 2 * n) cap <<= 1;
+  const int64_t cap = uq_table_cap(n);
   size_t tmp = 0;
   cub::DeviceScan::ExclusiveSum((void*)nullptr, tmp, (int32_t*)nullptr, (int32_t*)nullptr, (int)n, s);
   const int64_t o_tab = 256, o_first = o_tab + 16 * (cap + 1), o_flag = o_first + ((4 * n + 255) & ~(int64_t)255),

@@ -7,9 +7,11 @@ A DataFlow is the list of Blocks a convolution stack consumes, deepest hop first
     block.edge_index  [2, E]: edge_index[0] = index into the destination nodes, edge_index[1] = index into n_id
     block.size        (number of destination nodes, number of source nodes)
 
-Tensors stay on the device; the only host sync is the unique count of UniqueDataFlow (a shape, as in TF).
-`sampler` is any object with sample_neighbor(nodes, edge_types, count, default_node) -> (ids[B, count], w, t) and
-unique(ids) -> (values, inverse): euler_b200 itself on the GPU, or a CPU stand-in in the tests."""
+Tensors stay on the device; the only host syncs are shapes, as in TF: the unique count of UniqueDataFlow, and per hop of
+GCNDataFlow / RelationDataFlow the listing total and the unique count.
+`sampler` is any object with sample_neighbor(nodes, edge_types, count, default_node) -> (ids[B, count], w, t),
+unique(ids) -> (values, inverse) and full_neighbor_hop(nodes, edge_types, self_loops, with_types) -> (n_id, res_n_id,
+edge_index, types): euler_b200 itself on the GPU, or a CPU stand-in in the tests."""
 import torch
 
 
@@ -109,3 +111,37 @@ class SageDataFlow(UniqueDataFlow):
             neighbor_src.append(torch.arange(n_id.numel(), device=n_id.device).repeat_interleave(count))
             n_id, _ = self.sampler.unique(torch.cat([one, n_id]))
         return neighbors, neighbor_src
+
+
+class GCNDataFlow:
+    """gcn_dataflow.py:26-48 over UniqueDataFlow.produce_subgraph (neighbor_dataflow.py:84-110): every hop lists the full
+    neighborhood of its frontier (metapath[h]'s edge types) and the next frontier is unique(concat(neighbors, frontier)).
+    The reference computes that unique twice per hop (in get_neighbors and again in produce_subgraph, on the same input);
+    here one fused hop (sampler.full_neighbor_hop) lists, renumbers and emits the block's edges.  e_id is None."""
+    with_types = False     # e_id = the listed edge types
+
+    def __init__(self, metapath, add_self_loops=True, sampler=None):
+        self.metapath, self.add_self_loops = metapath, add_self_loops
+        self.sampler = sampler or _default_sampler()
+
+    def produce_subgraph(self, n_id):
+        n_id = n_id.reshape(-1)
+        flow = DataFlow(n_id)
+        for hop_edge_types in self.metapath:
+            n_id, res_n_id, edge_index, types = self.sampler.full_neighbor_hop(n_id, hop_edge_types, self.add_self_loops,
+                                                                                self.with_types)
+            flow.append(n_id, res_n_id, types, edge_index)
+        return flow
+
+    __call__ = produce_subgraph
+
+
+class RelationDataFlow(GCNDataFlow):
+    """relation_dataflow.py:25-71: GCNDataFlow's blocks without self loops -- whatever add_self_loops says, as in the
+    reference -- and with e_id = the edge type of every listed edge (i32), for RelationConv.  fanouts is accepted and
+    unused, as there."""
+    with_types = True
+
+    def __init__(self, fanouts, metapath, add_self_loops=True, sampler=None):
+        super().__init__(metapath, add_self_loops=False, sampler=sampler)
+        self.fanouts = fanouts

@@ -426,6 +426,76 @@ def get_top_k_neighbor(nodes, edge_types, k, default_node=-1, condition=''):
     return ids, w, t
 
 
+_HOP_APPEND_FRONTIER, _HOP_SELF_LOOPS, _HOP_SORT = 1, 2, 4     # include/euler_b200.h
+
+
+def _full_hop(nodes, edge_types, flags, rows=True, weights=False, types=False):
+    """one eu_full_neighbor_hop: two host syncs, the listing total (output shapes) and the unique count (the frontier's length)"""
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    et = get_edge_type_id(edge_types)
+    ctx = _ctx_on_stream()
+    lib = _lib.load()
+    n, dev = nodes.numel(), nodes.device
+    indptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    check(lib.eu_full_neighbor_hop(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), flags, 0, indptr.data_ptr(),
+                                   None, None, None, None, None, None, None))
+    total = int(indptr[-1].item())
+    append = bool(flags & _HOP_APPEND_FRONTIER)
+    width = total + (n if flags & _HOP_SELF_LOOPS else 0)
+    uniq = torch.empty(total + (n if append else 0), dtype=torch.int64, device=dev)
+    cnt = torch.zeros(1, dtype=torch.int64, device=dev)
+    edge_index = torch.empty((2 if rows else 1, width), dtype=torch.int64, device=dev)
+    w = torch.empty(total, dtype=torch.float32, device=dev) if weights else None
+    t = torch.empty(total, dtype=torch.int32, device=dev) if types else None
+    res = torch.empty(n, dtype=torch.int64, device=dev) if append else None
+    ptr = lambda x: None if x is None else x.data_ptr()          # noqa: E731
+    check(lib.eu_full_neighbor_hop(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), flags, total, indptr.data_ptr(),
+                                   uniq.data_ptr(), cnt.data_ptr(), edge_index[0].data_ptr() if rows else None,
+                                   edge_index[-1].data_ptr(), ptr(w), ptr(t), ptr(res)))
+    return indptr, uniq[:int(cnt.item())], res, edge_index, w, t
+
+
+def full_neighbor_hop(nodes, edge_types, self_loops=True, with_types=False):
+    """One hop of GCNDataFlow / RelationDataFlow (gcn_dataflow.py:34-48 + neighbor_dataflow.py:84-110,
+    relation_dataflow.py:31-71) in one fused device op: lists every neighbor of `nodes` (get_full_neighbor's order) and
+    numbers the listed ids and then the nodes themselves by first occurrence (tf.unique(concat(neighbors, nodes))).
+    Returns (n_id, res_n_id, edge_index, types):
+        n_id        i64[m]        the next frontier: unique(concat(neighbors, nodes))
+        res_n_id    i64[n]        the position of every node in n_id
+        edge_index  i64[2, E(+n)] [row of each listed entry, its position in n_id], followed with self_loops by the n
+                                  self loops [k, res_n_id[k]]
+        types       i32[E]        each entry's edge type (with_types), else None"""
+    flags = _HOP_APPEND_FRONTIER | (_HOP_SELF_LOOPS if self_loops else 0)
+    _, n_id, res, edge_index, _, t = _full_hop(nodes, edge_types, flags, types=with_types)
+    return n_id, res, edge_index, t
+
+
+def full_neighbor_adjacency(nodes, edge_types):
+    """One hop of get_multi_hop_neighbor (neighbor_ops.py:209-242) in one fused device op: (next_nodes, indptr, cols,
+    weights) with next_nodes = tf.unique(every listed neighbor) and row i's entries [indptr[i], indptr[i+1]) =
+    (cols, weights) ordered by column (tf.sparse_reorder; equal columns -- multi-edges, repeated types -- in listing order)."""
+    indptr, nxt, _, cols, w, _ = _full_hop(nodes, edge_types, _HOP_SORT, rows=False, weights=True)
+    return nxt, indptr, cols[0], w
+
+
+def get_multi_hop_neighbor(nodes, edge_types, sampler=None):
+    """neighbor_ops.get_multi_hop_neighbor (neighbor_ops.py:209-242): (nodes_list[L+1], adj_list[L]).  nodes_list[0] is
+    `nodes` flattened, nodes_list[h+1] the distinct neighbors of hop h in first-occurrence order.  The reference's adjacency
+    is a SparseTensor [len(nodes_list[h]), len(nodes_list[h+1])] of edge weights in (row, col) order; here it is ragged,
+    (indptr i64[n+1], cols i64[nnz], weights f32[nnz]), entry k of row i being (i, cols[k]):
+    torch.sparse_csr_tensor(indptr, cols, weights, size) builds the same matrix.  `sampler` is the object whose
+    full_neighbor_adjacency runs each hop (this module by default)."""
+    hop = full_neighbor_adjacency if sampler is None else sampler.full_neighbor_adjacency
+    nodes = (_t(nodes, torch.int64) if sampler is None else torch.as_tensor(nodes, dtype=torch.int64)).reshape(-1)
+    nodes_list, adj_list = [nodes], []
+    for et in edge_types:
+        nxt, indptr, cols, w = hop(nodes, et)
+        nodes_list.append(nxt)
+        adj_list.append((indptr, cols, w))
+        nodes = nxt
+    return nodes_list, adj_list
+
+
 def sample_neighbor_layerwise(nodes, edge_types, count, default_node=-1, weight_func=''):
     """neighbor_ops.sample_neighbor_layerwise (neighbor_ops.py:72-77): nodes [batch, n] -> (neighbors i64[batch, count],
     adj f32[batch, n, count]); adj is the dense view of the reference's SparseTensor (1.0 where neighbors[b, k] is a neighbor of

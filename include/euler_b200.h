@@ -326,6 +326,34 @@ int eu_get_node_weight_host(eu_ctx* c, const int64_t* nodes, int64_t B, float* o
  * uniq: device i64[n] (first *n_unique valid), inverse: device i32[n], n_unique: device i64[1] (may be NULL). */
 int eu_unique(eu_ctx* c, const int64_t* ids, int64_t n, int64_t* uniq, int32_t* inverse, int64_t* n_unique);
 
+/* One full-neighbor hop of the full-neighborhood minibatch constructions, fused: list every neighbor of the n frontier
+ * nodes (eu_get_full_neighbor's listing: E entries, row-major, types in the order given), renumber the listed ids by
+ * first occurrence (tf.unique) and emit the hop's edges in the new numbering.
+ *   GCNDataFlow (tf_euler/python/dataflow/gcn_dataflow.py:34-48 + neighbor_dataflow.py:84-110):
+ *       flags = EU_HOP_APPEND_FRONTIER [| EU_HOP_SELF_LOOPS]
+ *   RelationDataFlow (relation_dataflow.py:31-71): flags = EU_HOP_APPEND_FRONTIER, out_t = the block's e_id
+ *   get_multi_hop_neighbor (tf_euler/python/euler_ops/neighbor_ops.py:209-242): flags = EU_HOP_SORT, out_w = the values
+ * EU_HOP_APPEND_FRONTIER: the unique runs over concat(listing, nodes) instead of the listing alone.
+ * EU_HOP_SELF_LOOPS (needs APPEND, excludes SORT): n self-loop edges (k, position of nodes[k]) follow the E entries.
+ * EU_HOP_SORT: within each node's row the entries (cols, weights) are ordered by column, ties in listing order
+ *   (tf.sparse_reorder of the (row, col) SparseTensor); rows are unchanged.
+ * Device pointers; W = E + n with SELF_LOOPS, E otherwise:
+ *   out_ptr  i64[n+1]  listing offsets: the entries of node i are [out_ptr[i], out_ptr[i+1])
+ *   out_uniq i64[E (+n with APPEND)]  the next frontier, first *n_unique valid; n_unique i64[1]
+ *   out_rows i64[W]    each edge's row (index into nodes)                                  (may be NULL)
+ *   out_cols i64[W]    each edge's column (index into out_uniq)
+ *   out_w    f32[E]    each entry's weight                                                 (may be NULL)
+ *   out_t    i32[E]    each entry's edge type, not with SORT                               (may be NULL)
+ *   out_res  i64[n]    APPEND only: the position of every frontier node in out_uniq       (may be NULL)
+ * Two calls, like eu_get_full_neighbor: with cap = 0 and out_uniq = NULL only out_ptr is computed; read E = out_ptr[n],
+ * size the outputs and call again with cap = E (cap must equal the listing's total; the second call recomputes out_ptr).
+ * No host synchronisation.  A hop whose E (+ n with APPEND) reaches 2^31 returns EU_ERR_UNSUPPORTED (the reference's
+ * tf.unique and row indices are int32). */
+enum { EU_HOP_APPEND_FRONTIER = 1, EU_HOP_SELF_LOOPS = 2, EU_HOP_SORT = 4 };
+int eu_full_neighbor_hop(eu_ctx* c, const int64_t* nodes, int64_t n, const int32_t* etypes, int32_t K, int32_t flags,
+                         int64_t cap, int64_t* out_ptr, int64_t* out_uniq, int64_t* n_unique, int64_t* out_rows,
+                         int64_t* out_cols, float* out_w, int32_t* out_t, int64_t* out_res);
+
 /* ------------------------------------------------------------------ message-passing ops ------ */
 /* MPGather / MPScatterAdd / MPScatterMax (tf_euler/ops/mp_ops.cc:22-81; kernels
  * tf_euler/kernels/gather_op.cc:31-52, scatter_op.cc:32-92).  f32 data, i32 indices, as registered. */
