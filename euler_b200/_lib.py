@@ -90,6 +90,7 @@ SIGNATURES = {
     "eu_get_top_k_neighbor": (C.c_int, [_P, _P, _I64, _P, _I32, _I32, _I64, _P, _P, _P]),
     "eu_sample_neighbor_layerwise": (C.c_int, [_P, _P, _I64, _I32, _P, _I32, _I32, _I64, _I32, _P, _P]),
     "eu_sparse_get_adj": (C.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _I32, _P]),
+    "eu_sparse_get_adj_coo": (C.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _I32, _I64, _P, _P, _P]),
     "eu_gen_pair_count": (_I64, [_I32, _I32, _I32]),
     "eu_gen_pair": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32, _P]),
     "eu_sample_fanout": (C.c_int, [_P, _P, _I64, _P, _I32, _P, _I32, _I64, _P, _P, _P]),

@@ -14,6 +14,7 @@
 // pin (neighbor_ops_test.py:142-181 check membership and adj consistency only).  Here the candidates are ordered by
 // (dst, type): the candidate SET, every candidate's summed weight (same additions, same order) and hence the sampling
 // DISTRIBUTION are identical; which uniform maps to which candidate differs.  tests/ check exactly that.
+#include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
@@ -21,6 +22,7 @@
 #include <algorithm>
 
 #include "internal.h"
+#include "uq.cuh"
 
 namespace eu {
 
@@ -122,6 +124,127 @@ __global__ void k_lw_adj(const long long* __restrict__ ptr, int64_t batch, int32
   for (long long e = ptr[bj]; e < ptr[bj + 1]; ++e)
     if (ids[e] == want) { v = 1.f; break; }
   adj[i] = v;
+}
+
+// ---- sparse batch adjacency (eu_sparse_get_adj_coo, section 3.5 of DESIGN.md) ----
+// Row i = b * N + j of the listing, entry e.  sk / sv: each batch row's nb ids sorted, with their positions k.
+
+// segment b of the sorted nb = [b * m, (b + 1) * m)
+struct StrideSeg {
+  long long m;
+  __host__ __device__ long long operator()(long long b) const { return b * m; }
+};
+
+__global__ void k_adj_kiota(int32_t* __restrict__ v, int64_t n, int32_t m) {
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) v[p] = (int32_t)(p % m);
+}
+
+// the last i in [0, rows) with ptr[i] <= e (rows before it may be empty)
+__device__ __forceinline__ int32_t adj_row_of(const long long* __restrict__ ptr, int32_t rows, long long e) {
+  int32_t lo = 0, hi = rows - 1;
+  while (lo < hi) {
+    const int32_t mid = (int32_t)(((int64_t)lo + hi + 1) >> 1);
+    if (ptr[mid] <= e) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// One thread per listed entry, so a hub row is spread over as many threads as it has entries: the entry's id is looked up
+// in its batch row's sorted nb (the range [lo, lo + span) of equal ids), and every hit enters the first-occurrence table
+// under key (row, lo) -- an id listed several times by one row (multi-edges, repeated types) keeps its first entry only.
+__global__ void __launch_bounds__(256) k_adj_probe(const long long* __restrict__ ptr, int32_t rows, int32_t N, int32_t M,
+                                                   const unsigned long long* __restrict__ ids, int64_t total,
+                                                   const unsigned long long* __restrict__ sk, const long long* __restrict__ nb,
+                                                   HashSlot* tab, unsigned long long mask, int32_t* __restrict__ row_of,
+                                                   int32_t* __restrict__ lo_of, int32_t* __restrict__ span_of,
+                                                   int32_t* __restrict__ has_last) {
+  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  const int32_t i = adj_row_of(ptr, rows, e);
+  const int32_t b = i / N;
+  const unsigned long long id = ids[e];
+  const int32_t s0 = b * M, s1 = s0 + M;
+  int32_t lo = s0, hi = s1;
+  while (lo < hi) { const int32_t mid = (lo + hi) >> 1; if (sk[mid] < id) lo = mid + 1; else hi = mid; }
+  int32_t up = lo;
+  hi = s1;
+  while (up < hi) { const int32_t mid = (up + hi) >> 1; if (sk[mid] <= id) up = mid + 1; else hi = mid; }
+  row_of[e] = i;
+  lo_of[e] = lo;
+  span_of[e] = up - lo;
+  if (up > lo) {
+    uq_insert_warp(tab, mask, (unsigned long long)i * (unsigned long long)M + (unsigned long long)(lo - s0), (unsigned long long)e);
+    // (b, N-1, M-1) is an entry: no filler for this batch row
+    if (i - b * N == N - 1 &&id == (unsigned long long)nb[(int64_t)b * M + M - 1]) has_last[b] = 1;
+  }
+}
+
+// cnt[e] = the entries e contributes (its span if it is the first entry of its row listing that id, else 0); cnt[total] = 0
+__global__ void k_adj_keep(int64_t total, int32_t M, const int32_t* __restrict__ row_of, const int32_t* __restrict__ lo_of,
+                           const int32_t* __restrict__ span_of, const HashSlot* tab, unsigned long long mask, int32_t N,
+                           long long* __restrict__ cnt) {
+  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e > total) return;
+  long long c = 0;
+  if (e < total && span_of[e] > 0) {
+    const int32_t i = row_of[e], s0 = i / N * M;
+    if (uq_first(tab, mask, (unsigned long long)i * (unsigned long long)M + (unsigned long long)(lo_of[e] - s0)) == (unsigned long long)e)
+      c = span_of[e];
+  }
+  cnt[e] = c;
+}
+
+// fl[b] = 1 iff batch row b gets the filler (b, N-1, M-1) = 0; fl[batch] = 0
+__global__ void k_adj_fillers(const int32_t* __restrict__ has_last, int64_t batch, long long* __restrict__ fl) {
+  const int64_t b = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (b <= batch) fl[b] = b < batch && !has_last[b] ? 1 : 0;
+}
+
+// rowptr[i] = the entries before row i: the kept hits of the listing before it plus the fillers of earlier batch rows
+__global__ void k_adj_rowptr(int64_t rows, int32_t N, const long long* __restrict__ ptr, const long long* __restrict__ scan_e,
+                             const long long* __restrict__ scan_f, long long* __restrict__ rowptr) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i <= rows) rowptr[i] = scan_e[ptr[i]] + scan_f[i / N];
+}
+
+// One thread per kept (row, k) pair, so a hit of many positions (an id repeated in nb) is spread too: hit slot h is found
+// by binary search in the scanned counts, its k read from the sorted positions.  Rows are final here, k still in id order.
+__global__ void __launch_bounds__(256) k_adj_expand(int64_t total, int32_t N, const long long* __restrict__ scan_e,
+                                                    const long long* __restrict__ scan_f, const int32_t* __restrict__ row_of,
+                                                    const int32_t* __restrict__ lo_of, const int32_t* __restrict__ sv,
+                                                    long long* __restrict__ out_idx, long long* __restrict__ out_val,
+                                                    int32_t* __restrict__ kbuf) {
+  const long long hits = scan_e[total];
+  for (long long h = blockIdx.x * (long long)blockDim.x + threadIdx.x; h < hits; h += (long long)gridDim.x * blockDim.x) {
+    int64_t lo = 0, hi = total - 1;          // the last e with scan_e[e] <= h (its count is > 0)
+    while (lo < hi) {
+      const int64_t mid = (lo + hi + 1) >> 1;
+      if (scan_e[mid] <= h) lo = mid; else hi = mid - 1;
+    }
+    const int32_t i = row_of[lo], b = i / N;
+    const long long o = h + scan_f[b];
+    out_idx[3 * o] = b;
+    out_idx[3 * o + 1] = i - (long long)b * N;
+    out_val[o] = 1;
+    kbuf[o] = sv[lo_of[lo] + (int32_t)(h - scan_e[lo])];
+  }
+}
+
+// the filler of batch row b closes row (b, N-1): M-1 is the largest k and absent from that row
+__global__ void k_adj_filler(const int32_t* __restrict__ has_last, int64_t batch, int32_t N, int32_t M,
+                             const long long* __restrict__ rowptr, long long* __restrict__ out_idx, long long* __restrict__ out_val,
+                             int32_t* __restrict__ kbuf) {
+  const int64_t b = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (b >= batch || has_last[b]) return;
+  const long long o = rowptr[(b + 1) * N] - 1;
+  out_idx[3 * o] = b;
+  out_idx[3 * o + 1] = N - 1;
+  out_val[o] = 0;
+  kbuf[o] = M - 1;
+}
+
+__global__ void k_adj_col(int64_t nnz, const int32_t* __restrict__ k, long long* __restrict__ out_idx) {
+  for (int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; o < nnz; o += (int64_t)gridDim.x * blockDim.x) out_idx[3 * o + 2] = k[o];
 }
 
 }  // namespace eu
@@ -234,6 +357,122 @@ extern "C" int eu_sparse_get_adj(eu_ctx* c, const int64_t* nodes, const int64_t*
     k_lw_adj<<<(unsigned)ceil_div(batch * (int64_t)N * M, 256), 256, 0, c->stream>>>(L.ptr, batch, N, M, L.ids, (const long long*)nb_nodes, out_adj);
     g_launches++;
     if (cudaStreamSynchronize(c->stream) != cudaSuccess) { set_error("eu_sparse_get_adj: %s", cudaGetErrorString(cudaGetLastError())); rc = EU_ERR_CUDA; }
+  }
+  L.free_all();
+  return rc;
+}
+
+// tf_euler.sparse_get_adj as the reference's SparseTensor (tf_euler/kernels/sparse_get_adj_op.cc:84-117); DESIGN.md section 3.5.
+// Everything after the listing is O(listed entries + entries + M log M) per batch row: no pass over the N * M pairs.
+static int adj_coo(eu_ctx* c, const int64_t* nb_nodes, int64_t batch, int32_t N, int32_t M, int64_t cap, const LwListing& L,
+                   int64_t* out_ptr, int64_t* out_indices, int64_t* out_values) {
+  cudaStream_t s = c->stream;
+  const int64_t rows = batch * N, nbs = batch * M, E = L.total;
+  const int64_t tcap = uq_table_cap(E);
+  cub::CountingInputIterator<long long> cnt_it(0);
+  cub::TransformInputIterator<long long, StrideSeg, cub::CountingInputIterator<long long>> seg(cnt_it, StrideSeg{(long long)M});
+  size_t t_nb = 0, t_se = 0, t_sf = 0, t_sort = 0;
+  cub::DeviceSegmentedSort::SortPairs((void*)nullptr, t_nb, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                      (const int32_t*)nullptr, (int32_t*)nullptr, (int)nbs, (int)batch, seg, seg + 1, s);
+  cub::DeviceScan::ExclusiveSum((void*)nullptr, t_se, (const long long*)nullptr, (long long*)nullptr, (int)(E + 1), s);
+  cub::DeviceScan::ExclusiveSum((void*)nullptr, t_sf, (const long long*)nullptr, (long long*)nullptr, (int)(batch + 1), s);
+  if (cap > 0)
+    cub::DeviceSegmentedSort::SortKeys((void*)nullptr, t_sort, (const int32_t*)nullptr, (int32_t*)nullptr, (int)cap, (int)rows,
+                                       (const long long*)out_ptr, (const long long*)out_ptr + 1, s);
+  const size_t tmp = std::max(std::max(t_nb, t_se), std::max(t_sf, t_sort));
+  auto a256 = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  const size_t e1 = (size_t)std::max<int64_t>(E, 1);
+  // table | sorted nb ids | positions in / sorted | per entry: row, lo, span, count, scan | per batch row: has_last, filler,
+  // scan | [per entry of the output: k, sorted k] | cub temp
+  const size_t o_tab = 0, o_sk = o_tab + a256(16 * (size_t)(tcap + 1)), o_kio = o_sk + a256(8 * (size_t)nbs),
+               o_sv = o_kio + a256(4 * (size_t)nbs), o_row = o_sv + a256(4 * (size_t)nbs), o_lo = o_row + a256(4 * e1),
+               o_span = o_lo + a256(4 * e1), o_cnt = o_span + a256(4 * e1), o_se = o_cnt + a256(8 * (size_t)(E + 1)),
+               o_has = o_se + a256(8 * (size_t)(E + 1)), o_fl = o_has + a256(4 * (size_t)batch),
+               o_sf = o_fl + a256(8 * (size_t)(batch + 1)), o_k = o_sf + a256(8 * (size_t)(batch + 1)),
+               o_k2 = o_k + a256(4 * (size_t)cap), o_tmp = o_k2 + a256(4 * (size_t)cap), total = o_tmp + a256(tmp);
+  int rc = ctx_misc(c, (int64_t)total);
+  if (rc) return rc;
+  char* m = (char*)c->d_misc;
+  HashSlot* tab = (HashSlot*)(m + o_tab);
+  unsigned long long* sk = (unsigned long long*)(m + o_sk);
+  int32_t *kio = (int32_t*)(m + o_kio), *sv = (int32_t*)(m + o_sv), *row = (int32_t*)(m + o_row), *lo = (int32_t*)(m + o_lo),
+          *span = (int32_t*)(m + o_span), *has_last = (int32_t*)(m + o_has), *kbuf = (int32_t*)(m + o_k), *kbuf2 = (int32_t*)(m + o_k2);
+  long long *cnt = (long long*)(m + o_cnt), *scan_e = (long long*)(m + o_se), *fl = (long long*)(m + o_fl), *scan_f = (long long*)(m + o_sf);
+  const unsigned long long mask = (unsigned long long)tcap - 1;
+  const unsigned cap_blocks = kSMs * 8;
+
+  k_uq_clear<<<(unsigned)std::min<int64_t>(ceil_div(tcap + 1, 256), cap_blocks), 256, 0, s>>>(tab, tcap + 1);
+  EU_LAUNCHED();
+  k_adj_kiota<<<(unsigned)std::min<int64_t>(ceil_div(nbs, 256), cap_blocks), 256, 0, s>>>(kio, nbs, M);
+  EU_LAUNCHED();
+  EU_CUDA(cub::DeviceSegmentedSort::SortPairs(m + o_tmp, t_nb, (const unsigned long long*)nb_nodes, sk, (const int32_t*)kio, sv,
+                                              (int)nbs, (int)batch, seg, seg + 1, s));
+  EU_LAUNCHED();
+  EU_CUDA(cudaMemsetAsync(has_last, 0, 4 * (size_t)batch, s));
+  if (E > 0) {
+    k_adj_probe<<<(unsigned)ceil_div(E, 256), 256, 0, s>>>(L.ptr, (int32_t)rows, N, M, L.ids, E, sk, (const long long*)nb_nodes, tab,
+                                                           mask, row, lo, span, has_last);
+    EU_LAUNCHED();
+  }
+  k_adj_keep<<<(unsigned)ceil_div(E + 1, 256), 256, 0, s>>>(E, M, row, lo, span, tab, mask, N, cnt);
+  EU_LAUNCHED();
+  k_adj_fillers<<<(unsigned)ceil_div(batch + 1, 256), 256, 0, s>>>(has_last, batch, fl);
+  EU_LAUNCHED();
+  EU_CUDA(cub::DeviceScan::ExclusiveSum(m + o_tmp, t_se, (const long long*)cnt, scan_e, (int)(E + 1), s));
+  EU_LAUNCHED();
+  EU_CUDA(cub::DeviceScan::ExclusiveSum(m + o_tmp, t_sf, (const long long*)fl, scan_f, (int)(batch + 1), s));
+  EU_LAUNCHED();
+  k_adj_rowptr<<<(unsigned)ceil_div(rows + 1, 256), 256, 0, s>>>(rows, N, L.ptr, scan_e, scan_f, (long long*)out_ptr);
+  EU_LAUNCHED();
+  if (cap == 0) return EU_OK;
+
+  long long nnz = 0;
+  EU_CUDA(cudaMemcpyAsync(&nnz, out_ptr + rows, 8, cudaMemcpyDeviceToHost, s));
+  EU_CUDA(cudaStreamSynchronize(s));
+  if (nnz != cap) {
+    set_error("eu_sparse_get_adj_coo: cap %lld is not the entry count %lld (call with cap = 0 first)", (long long)cap, nnz);
+    return EU_ERR_INVALID;
+  }
+  long long* idx = (long long*)out_indices;
+  k_adj_expand<<<(unsigned)std::min<int64_t>(ceil_div(cap, 256), cap_blocks), 256, 0, s>>>(E, N, scan_e, scan_f, row, lo, sv, idx,
+                                                                                            (long long*)out_values, kbuf);
+  EU_LAUNCHED();
+  k_adj_filler<<<(unsigned)ceil_div(batch, 256), 256, 0, s>>>(has_last, batch, N, M, (const long long*)out_ptr, idx,
+                                                              (long long*)out_values, kbuf);
+  EU_LAUNCHED();
+  EU_CUDA(cub::DeviceSegmentedSort::SortKeys(m + o_tmp, t_sort, (const int32_t*)kbuf, kbuf2, (int)cap, (int)rows,
+                                             (const long long*)out_ptr, (const long long*)out_ptr + 1, s));
+  EU_LAUNCHED();
+  k_adj_col<<<(unsigned)std::min<int64_t>(ceil_div(cap, 256), cap_blocks), 256, 0, s>>>(cap, kbuf2, idx);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+extern "C" int eu_sparse_get_adj_coo(eu_ctx* c, const int64_t* nodes, const int64_t* nb_nodes, int64_t batch, int32_t N, int32_t M,
+                                     const int32_t* etypes, int32_t K, int64_t cap, int64_t* out_ptr, int64_t* out_indices,
+                                     int64_t* out_values) {
+  if (!c || batch < 0 || N < 0 || M < 0 || cap < 0 || !out_ptr || (batch > 0 && N > 0 && !nodes) || (batch > 0 && M > 0 && !nb_nodes) ||
+      (cap > 0 && (!out_indices || !out_values))) {
+    set_error("eu_sparse_get_adj_coo: bad argument");
+    return EU_ERR_INVALID;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  const int64_t rows = batch * (int64_t)N;
+  if (rows >= ((int64_t)1 << 31) || batch * (int64_t)M >= ((int64_t)1 << 31) || cap >= ((int64_t)1 << 31)) {
+    set_error("eu_sparse_get_adj_coo: 2^31 or more node rows, neighbor slots or entries are not supported");
+    return EU_ERR_UNSUPPORTED;
+  }
+  if (rows == 0 || M == 0) {            // no (b, j, k) position at all: no entry and no filler
+    if (cap > 0) { set_error("eu_sparse_get_adj_coo: cap %lld is not the entry count 0", (long long)cap); return EU_ERR_INVALID; }
+    EU_CUDA(cudaMemsetAsync(out_ptr, 0, 8 * (size_t)(rows + 1), c->stream));
+    return EU_OK;
+  }
+  LwListing L;
+  int rc = lw_listing(c, nodes, rows, etypes, K, &L);
+  if (!rc) rc = adj_coo(c, nb_nodes, batch, N, M, cap, L, out_ptr, out_indices, out_values);
+  if (!rc && cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    set_error("eu_sparse_get_adj_coo: %s", cudaGetErrorString(cudaGetLastError()));
+    rc = EU_ERR_CUDA;
   }
   L.free_all();
   return rc;

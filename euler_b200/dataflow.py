@@ -1,5 +1,6 @@
 """Minibatch subgraph construction for the message-passing convolutions: the reference's NeighborDataFlow /
-UniqueDataFlow / SageDataFlow (tf_euler/python/dataflow/{base,neighbor,sage}_dataflow.py) over this package's ops.
+UniqueDataFlow / SageDataFlow / GCNDataFlow / RelationDataFlow / LayerwiseDataFlow / LayerwiseEachDataFlow
+(tf_euler/python/dataflow/{base,neighbor,sage,gcn,relation,layerwise}_dataflow.py) over this package's ops.
 
 A DataFlow is the list of Blocks a convolution stack consumes, deepest hop first (base_dataflow.py:19-52):
     block.n_id        node ids of the block's source side (hop l+1 frontier [+ the destination nodes])
@@ -7,11 +8,13 @@ A DataFlow is the list of Blocks a convolution stack consumes, deepest hop first
     block.edge_index  [2, E]: edge_index[0] = index into the destination nodes, edge_index[1] = index into n_id
     block.size        (number of destination nodes, number of source nodes)
 
-Tensors stay on the device; the only host syncs are shapes, as in TF: the unique count of UniqueDataFlow, and per hop of
-GCNDataFlow / RelationDataFlow the listing total and the unique count.
+Tensors stay on the device; the only host syncs are shapes, as in TF: the unique count of UniqueDataFlow, per hop of
+GCNDataFlow / RelationDataFlow the listing total and the unique count, and per layer-wise hop the adjacency's entry count.
 `sampler` is any object with sample_neighbor(nodes, edge_types, count, default_node) -> (ids[B, count], w, t),
-unique(ids) -> (values, inverse) and full_neighbor_hop(nodes, edge_types, self_loops, with_types) -> (n_id, res_n_id,
-edge_index, types): euler_b200 itself on the GPU, or a CPU stand-in in the tests."""
+unique(ids) -> (values, inverse), full_neighbor_hop(nodes, edge_types, self_loops, with_types) -> (n_id, res_n_id,
+edge_index, types), get_full_neighbor(nodes, edge_types) -> (indptr, ids, w, t) and
+sample_neighbor_layerwise_coo(nodes[batch, n], edge_types, count) -> (ids[batch, count], (indices[nnz, 3], values, shape)):
+euler_b200 itself on the GPU, or a CPU stand-in in the tests."""
 import torch
 
 
@@ -145,3 +148,68 @@ class RelationDataFlow(GCNDataFlow):
     def __init__(self, fanouts, metapath, add_self_loops=True, sampler=None):
         super().__init__(metapath, add_self_loops=False, sampler=sampler)
         self.fanouts = fanouts
+
+
+def _full_listing(sampler, n_id, edge_types):
+    """get_full_neighbor(n_id)[0] as (values, indices[:, 0]): the listed ids and the row of each"""
+    indptr, ids, _w, _t = sampler.get_full_neighbor(n_id, edge_types)
+    rows = torch.arange(n_id.numel(), device=n_id.device).repeat_interleave(indptr[1:] - indptr[:-1], output_size=ids.numel())
+    return ids, rows
+
+
+class LayerwiseDataFlow(UniqueDataFlow):
+    """layerwise_dataflow.py:26-62 ('adapt', AdaptiveGCN): every hop but the last draws total_fanout = the sum of the fanouts so
+    far from the union of the whole frontier's neighbors (one batch row), and its edges are the adjacency's entries (row j ->
+    the k-th draw); the last hop lists the frontier's full neighborhoods.  As upstream, the adjacency's filler entry (value 0,
+    sparse_get_adj_coo) is an edge too, and a frontier without candidates brings default_node (-1) into n_id."""
+
+    def __init__(self, fanouts, metapath, add_self_loops=True, sampler=None):
+        super().__init__(num_hops=len(metapath), add_self_loops=add_self_loops, sampler=sampler)
+        self.fanouts, self.metapath = fanouts, metapath
+
+    def get_neighbors(self, n_id):
+        neighbors, neighbor_src = [], []
+        total_fanout = 0
+        for i, hop_edge_types in enumerate(self.metapath):
+            n_id = n_id.reshape(-1)
+            if i == len(self.metapath) - 1:
+                one, src = _full_listing(self.sampler, n_id, hop_edge_types)
+            else:
+                total_fanout += self.fanouts[i]
+                drawn, (indices, _v, _shape) = self.sampler.sample_neighbor_layerwise_coo(n_id.reshape(1, -1), hop_edge_types,
+                                                                                          total_fanout)
+                one = drawn.reshape(-1)[indices[:, 2]]
+                src = indices[:, 1]
+            neighbors.append(one)
+            neighbor_src.append(src)
+            n_id, _ = self.sampler.unique(torch.cat([one, n_id]))
+        return neighbors, neighbor_src
+
+
+class LayerwiseEachDataFlow(NeighborDataFlow):
+    """layerwise_dataflow.py:65-119 ('layerwise'), no de-duplication: hop 1 is sample_neighbor(fanouts[0]) with default_node =
+    max_id + 1; every later hop reshapes the previous hop's neighbors into rows of the previous fanout, draws fanouts[h] per row
+    from the row's union of neighbors, and takes the adjacency's entries (fillers included) as edges, numbered across rows:
+    neighbor indices[:, 2] + indices[:, 0] * count, source indices[:, 1] + indices[:, 0] * last_count.  As upstream, a third
+    hop needs the second hop's edge count to be a multiple of fanouts[1].  Upstream passes `defulat_node=` to sample_neighbor
+    and so raises TypeError; here the keyword is spelled right."""
+
+    def __init__(self, fanouts, metapath, add_self_loops=True, max_id=-1, sampler=None):
+        super().__init__(num_hops=len(metapath), add_self_loops=add_self_loops, sampler=sampler)
+        self.fanouts, self.metapath, self.max_id = fanouts, metapath, max_id
+
+    def get_neighbors(self, n_id):
+        n_id = n_id.reshape(-1)
+        count = self.fanouts[0]
+        one, _w, _t = self.sampler.sample_neighbor(n_id, self.metapath[0], count, default_node=self.max_id + 1)
+        neighbors = [one.reshape(-1)]
+        neighbor_src = [torch.arange(n_id.numel(), device=n_id.device).repeat_interleave(count)]
+        cur, last_count = neighbors[0], count
+        for hop_edge_types, count in zip(self.metapath[1:], self.fanouts[1:]):
+            drawn, (indices, _v, _shape) = self.sampler.sample_neighbor_layerwise_coo(cur.reshape(-1, last_count), hop_edge_types,
+                                                                                      count)
+            one = drawn.reshape(-1)[indices[:, 2] + indices[:, 0] * count]
+            neighbors.append(one)
+            neighbor_src.append(indices[:, 1] + indices[:, 0] * last_count)
+            cur, last_count = one, count
+        return neighbors, neighbor_src

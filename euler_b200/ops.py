@@ -531,6 +531,59 @@ def sparse_get_adj(nodes, nb_nodes, edge_types, n=-1, m=-1):
     return adj
 
 
+def _adj_coo(nd, nb, batch, N, M, et):
+    """one eu_sparse_get_adj_coo: a host sync for the entry count (the output shape)"""
+    lib, dev = _lib.load(), nd.device
+    rowptr = torch.empty(batch * N + 1, dtype=torch.int64, device=dev)
+    ctx = _ctx_on_stream()
+    args = (ctx._h, nd.data_ptr(), nb.data_ptr(), batch, N, M, et.ctypes.data, len(et))
+    check(lib.eu_sparse_get_adj_coo(*args, 0, rowptr.data_ptr(), None, None))
+    nnz = int(rowptr[-1].item())
+    indices = torch.empty((nnz, 3), dtype=torch.int64, device=dev)
+    values = torch.empty(nnz, dtype=torch.int64, device=dev)
+    if nnz:
+        check(lib.eu_sparse_get_adj_coo(*args, nnz, rowptr.data_ptr(), indices.data_ptr(), values.data_ptr()))
+    return indices, values, (batch, N, M)
+
+
+def sparse_get_adj_coo(nodes, nb_nodes, edge_types, n=-1, m=-1):
+    """neighbor_ops.sparse_get_adj (neighbor_ops.py:33-36) with the reference's SparseTensor as it is built
+    (tf_euler/kernels/sparse_get_adj_op.cc:84-117): (indices i64[nnz, 3], values i64[nnz], dense_shape (batch, n, m)).
+    Entry (b, j, k) = 1 iff nb_nodes[b, k] is a neighbor of nodes[b, j], in row-major order; a batch row without an entry
+    (b, n-1, m-1) gets it with value 0.  Same arguments as sparse_get_adj."""
+    nd = _t(nodes, torch.int64).reshape(-1).contiguous()
+    nb = _t(nb_nodes, torch.int64).reshape(-1).contiguous()
+    N = nd.numel() if n == -1 else int(n)
+    M = nb.numel() if m == -1 else int(m)
+    batch = nd.numel() // max(N, 1)
+    return _adj_coo(nd, nb, batch, N, M, get_edge_type_id(edge_types))
+
+
+def sample_neighbor_layerwise_coo(nodes, edge_types, count, default_node=-1, weight_func=''):
+    """neighbor_ops.sample_neighbor_layerwise (neighbor_ops.py:72-77) with the adjacency as the reference's SparseTensor:
+    (neighbors i64[batch, count], (indices i64[nnz, 3], values i64[nnz], dense_shape (batch, n, count))).  The draws (and the
+    engine state they consume) are sample_neighbor_layerwise's; the adjacency is sparse_get_adj_coo of (nodes, neighbors),
+    the rule sample_neighbor_layerwise_with_adj_op.cc:104-140 applies to the drawn neighbors.  A batch of zero nodes per row
+    has no candidates: its neighbors are default_node and nothing is drawn."""
+    nd = _t(nodes, torch.int64)
+    if nd.dim() != 2:
+        raise EulerError("sample_neighbor_layerwise_coo: nodes must be [batch, n]")
+    if weight_func not in ('', 'sqrt'):
+        raise EulerError("sample_neighbor_layerwise_coo: weight_func must be '' or 'sqrt' (local_sample_layer_op.cc:93-101)")
+    nd = nd.contiguous()
+    batch, n = nd.shape
+    count = int(count)
+    et = get_edge_type_id(edge_types)
+    out = torch.empty((batch, count), dtype=torch.int64, device=nd.device)
+    if n == 0:
+        out.fill_(default_node)
+    else:
+        ctx = _ctx_on_stream()
+        check(_lib.load().eu_sample_neighbor_layerwise(ctx._h, nd.data_ptr(), batch, n, et.ctypes.data, len(et), count, default_node,
+                                                       1 if weight_func == 'sqrt' else 0, out.data_ptr(), None))
+    return out, _adj_coo(nd.reshape(-1), out.reshape(-1), batch, n, count, et)
+
+
 def gen_pair(paths, left_win_size, right_win_size):
     """walk_ops.gen_pair (tf_euler/kernels/gen_pair_op.cc): skip-gram pairs i64[B, n_pairs, 2] of walks i64[B, path_len]."""
     paths = _t(paths, torch.int64)

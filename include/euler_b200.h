@@ -308,6 +308,21 @@ int eu_sample_neighbor_layerwise(eu_ctx* c, const int64_t* nodes, int64_t batch,
  * (dense view of the SparseTensor). */
 int eu_sparse_get_adj(eu_ctx* c, const int64_t* nodes, const int64_t* nb_nodes, int64_t batch, int32_t N, int32_t M,
                       const int32_t* etypes, int32_t K, float* out_adj);
+/* tf_euler.sparse_get_adj as the reference's SparseTensor itself (tf_euler/kernels/sparse_get_adj_op.cc:84-117): same inputs
+ * and membership rule as eu_sparse_get_adj.  Entry (b, j, k) with value 1 iff nb_nodes[b, k] is among the listed neighbors of
+ * nodes[b, j]: a neighbor listed several times gives one entry, an id repeated in nb_nodes[b] one entry per position k.  Every
+ * batch row without an entry (b, N-1, M-1) gets that entry with value 0 (the reference's filler, which gives the dense shape
+ * [batch, N, M]).  Entries in row-major (b, j, k) order:
+ *   out_ptr     i64[batch*N + 1]  entries of row (b, j) are [out_ptr[b*N + j], out_ptr[b*N + j + 1])
+ *   out_indices i64[nnz, 3]       (b, j, k)
+ *   out_values  i64[nnz]          1, or 0 for a filler
+ * Two calls, like eu_get_full_neighbor: cap = 0 computes out_ptr only; read nnz = out_ptr[batch*N] and call again with cap = nnz.
+ * Cost after the listing: O(listed entries + nnz + M log M) per batch row, balanced by listed entries.  Device pointers;
+ * synchronises (scratch is sized from the listing, and the second call checks cap).  2^31 or more listed entries, node rows,
+ * neighbor slots or entries return EU_ERR_UNSUPPORTED. */
+int eu_sparse_get_adj_coo(eu_ctx* c, const int64_t* nodes, const int64_t* nb_nodes, int64_t batch, int32_t N, int32_t M,
+                          const int32_t* etypes, int32_t K, int64_t cap, int64_t* out_ptr, int64_t* out_indices,
+                          int64_t* out_values);
 /* tf_euler.gen_pair (tf_euler/kernels/gen_pair_op.cc:41-100): skip-gram pairs of walks.  paths i64[B,path_len] ->
  * out i64[B, eu_gen_pair_count(path_len, lw, rw), 2] (device pointers). */
 int64_t eu_gen_pair_count(int32_t path_len, int32_t left_win_size, int32_t right_win_size);
