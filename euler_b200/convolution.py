@@ -7,10 +7,13 @@ with the framework (torch here): they are GEMMs, not part of the sampling / aggr
   relation_aggregate tf_euler/python/convolution/relation_conv.py:53-70  x_j gathered, transformed by its relation's matrix
                                                                       (unique -> gather -> matmul), scatter_mean to the targets
   sage_aggregate     tf_euler/python/convolution/sage_conv.py:33-38   gather(x, edge_index[1]) -> scatter_mean
+  gat_aggregate      tf_euler/python/convolution/gat_conv.py:53-78    per-node attention scores, then the fused softmax-weighted
+                                                                      sum over each target's edges (ops.gat_attention_aggregate)
 """
 import torch
 
 from . import ops
+from ._lib import EulerError
 
 
 def gcn_norm(edge_index, size):
@@ -48,3 +51,27 @@ def sage_aggregate(x, edge_index, size):
     """SAGEConv's neighbor mean (sage_conv.py:33-38): scatter_mean(gather(x_source, edge_index[1]), edge_index[0], size[0])"""
     x1 = x if torch.is_tensor(x) else (x[1] if x[1] is not None else x[0])
     return ops.scatter_mean(ops.gather(x1, edge_index[1].to(torch.int32)), edge_index[0].to(torch.int32), int(size[0]))
+
+
+def gat_aggregate(x, edge_index, size, att_i, att_j, improved=False, aggr='add'):
+    """GATConv.__call__ after its `fc` (gat_conv.py:53-78), for H heads of width C laid out as the concatenation of H
+    single-head convs (gat.py's calculate_conv): x = (x_target, x_source), both already projected to [n, H*C]; att_i, att_j
+    [H, C] are the weights of the two Attention layers (Dense(1) per head).  The scores att_i(x_i) and att_j(x_j) are
+    computed once per node here, in torch, so autograd reaches att_* and x through them; the softmax-weighted sum over
+    each target's edges is the fused device op.  improved adds x_target.  Head averaging (concat=False) stays with the
+    caller.  Only aggr='add' (GATConv's default) is built."""
+    if aggr != 'add':
+        raise EulerError("gat_aggregate: aggr=%r is not built here; GATConv's aggregation is 'add'" % (aggr,))
+    if torch.is_tensor(x) or x[0] is None:
+        raise EulerError("gat_aggregate: x must be (x_target, x_source): att_i scores the targets")
+    x0, x1 = x[0], x[1] if x[1] is not None else x[0]
+    if att_i.dim() != 2 or att_j.shape != att_i.shape:
+        raise EulerError("gat_aggregate: att_i and att_j must both be [H, C]; got %s, %s" % (tuple(att_i.shape), tuple(att_j.shape)))
+    H, C = att_i.shape
+    if x0.dim() != 2 or x1.dim() != 2 or x0.shape[1] != H * C or x1.shape[1] != H * C:
+        raise EulerError("gat_aggregate: x_target and x_source must be [n, H*C] = [n, %d]; got %s, %s"
+                         % (H * C, tuple(x0.shape), tuple(x1.shape)))
+    s_dst = (x0.reshape(x0.shape[0], H, C) * att_i).sum(-1)
+    s_src = (x1.reshape(x1.shape[0], H, C) * att_j).sum(-1)
+    out = ops.gat_attention_aggregate(x1, s_dst, s_src, edge_index, size)
+    return x0 + out if improved else out

@@ -1,0 +1,441 @@
+// GATConv's attention aggregation, forward and backward, over the edge lists of dataflow blocks (f32 data, i32 indices).
+//
+// Reference semantics (file:line relative to /root/reference):
+//   GATConv.__call__ / apply_edge   tf_euler/python/convolution/gat_conv.py:53-78 with aggr = 'add', after its `fc`
+//   scatter_softmax                 tf_euler/python/euler_ops/mp_ops.py:76-79 (scatter_max initialised to -1e9)
+//
+// For head h and edge e = (dst_e, src_e):
+//   u[e,h]     = leaky_relu(s_dst[dst_e,h] + s_src[src_e,h], 0.2)
+//   alpha[e,h] = scatter_softmax(u, dst, n_dst)
+//   out[i, h*C:(h+1)*C] = sum over the edges e with dst_e = i of alpha[e,h] * h_src[src_e, h*C:(h+1)*C]
+//
+// Forward: a group of G lanes per target row, as k_scatter_sorted.  The arithmetic is the composition gather -> add ->
+// leaky_relu -> scatter_softmax -> multiply -> scatter_add over the sorted path, one rounded operation at a time
+// (__fadd_rn / __fmul_rn: nvcc would contract to FMA), with the segment sums left to right in edge order; so for
+// non-decreasing dst the output and alpha are that composition's bit for bit.  Unsorted dst is ordered by a stable radix
+// sort first and the same kernel runs through the permutation.
+//
+// Backward: one kernel per target row (d_alpha, du, grad_s_dst; du to scratch), a stable radix sort of the edges by source,
+// one kernel per source row (grad_h_src, grad_s_src).  Every sum runs in edge order within its segment: deterministic, no
+// atomics.
+#include <cub/device/device_radix_sort.cuh>
+
+#include <algorithm>
+
+#include "internal.h"
+
+namespace eu {
+
+// lanes per row: 4 columns per lane with float4, 1 otherwise; a power of two <= 32
+static inline int gat_lanes(int64_t hc, bool vec) {
+  const int64_t v = vec ? hc / 4 : hc;
+  int g = 1;
+  while (g < 32 && g < v) g <<= 1;
+  return g;
+}
+
+__device__ __forceinline__ int64_t gat_lower_bound(const int32_t* __restrict__ a, int64_t n, int64_t key) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if ((int64_t)__ldg(a + mid) < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// the mask of the G-lane group this lane belongs to (G a power of two)
+__device__ __forceinline__ unsigned group_mask(int G) {
+  if (G == 32) return 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  return ((1u << G) - 1u) << (lane & ~(G - 1));
+}
+
+__device__ __forceinline__ float leaky(float x) { return x > 0.f ? x : __fmul_rn(x, 0.2f); }
+
+// the edge at position k of the order the kernels walk (sorted by the segment key)
+__device__ __forceinline__ int64_t edge_at(const int32_t* __restrict__ perm, int64_t k) { return perm ? (int64_t)__ldg(perm + k) : k; }
+
+__global__ void k_gat_iota(int32_t* __restrict__ v, int64_t n) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) v[i] = (int32_t)i;
+}
+
+constexpr int kGatUnroll = 8;   // source rows in flight per lane in the ordered column sums
+
+// G lanes per target row r; its edges are positions [lb(r), lb(r+1)) of the dst-sorted order `key` (perm: position -> edge).
+// Per head: the max of the logits (a group reduction: max is exact in any order), the exps (in parallel) and their sum (a
+// serial chain in edge order, broadcast lane by lane), then alpha = exp / sum.  alpha doubles as the scratch of u and exp.
+// Then the columns: lanes over H*C, edges in order, kGatUnroll source rows loaded ahead of the ordered adds.
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_gat_fwd(const float* __restrict__ h_src, const float* __restrict__ s_dst,
+                                                 const float* __restrict__ s_src, const int32_t* __restrict__ key,
+                                                 const int32_t* __restrict__ perm, const int32_t* __restrict__ src, int64_t E,
+                                                 int64_t n_dst, int H, int C, int G, float* __restrict__ alpha,
+                                                 float* __restrict__ out) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t r = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (r >= n_dst) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  const int64_t b = gat_lower_bound(key, E, r), e = gat_lower_bound(key, E, r + 1);
+  const int HC = H * C;   // < 2^31: checked by the launcher
+  for (int h = 0; h < H && b < e; ++h) {
+    const float sd = __ldg(s_dst + r * H + h);
+    float m = -1e9f;                                   // scatter_max's initial value; a NaN logit never wins
+    for (int64_t k = b + sub; k < e; k += G) {
+      const int64_t ed = edge_at(perm, k);
+      const float u = leaky(__fadd_rn(sd, __ldg(s_src + (int64_t)__ldg(src + ed) * H + h)));
+      alpha[ed * H + h] = u;
+      m = u > m ? u : m;
+    }
+    for (int o = G >> 1; o > 0; o >>= 1) {
+      const float v = __shfl_xor_sync(gm, m, o, G);
+      m = v > m ? v : m;
+    }
+    float s = 0.f;
+    for (int64_t k0 = b; k0 < e; k0 += G) {             // group-uniform trip count
+      const int64_t k = k0 + sub;
+      float x = 0.f;
+      if (k < e) {
+        const int64_t ed = edge_at(perm, k);
+        x = expf(__fsub_rn(alpha[ed * H + h], m));
+        alpha[ed * H + h] = x;
+      }
+      const int n = e - k0 < G ? (int)(e - k0) : G;
+      for (int j = 0; j < n; ++j) s = __fadd_rn(s, __shfl_sync(gm, x, j, G));
+    }
+    for (int64_t k = b + sub; k < e; k += G) {
+      const int64_t ed = edge_at(perm, k);
+      alpha[ed * H + h] = __fdiv_rn(alpha[ed * H + h], s);
+    }
+  }
+  __syncwarp(gm);                                      // the column pass reads alphas other lanes of the group wrote
+  float* o = out + r * (int64_t)HC;
+  if (VEC) {
+    for (int d = sub * 4; d < HC; d += G * 4) {
+      const int h0 = d / C, h1 = (d + 1) / C, h2 = (d + 2) / C, h3 = (d + 3) / C;
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int64_t k0 = b; k0 < e; k0 += kGatUnroll) {
+        float4 x[kGatUnroll], a[kGatUnroll];
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q) {
+          if (k0 + q < e) {
+            const int64_t ed = edge_at(perm, k0 + q);
+            x[q] = __ldg(reinterpret_cast<const float4*>(h_src + (int64_t)__ldg(src + ed) * HC + d));
+            const float* al = alpha + ed * H;
+            a[q] = make_float4(al[h0], al[h1], al[h2], al[h3]);
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q) {
+          if (k0 + q < e) {
+            acc.x = __fadd_rn(acc.x, __fmul_rn(x[q].x, a[q].x)); acc.y = __fadd_rn(acc.y, __fmul_rn(x[q].y, a[q].y));
+            acc.z = __fadd_rn(acc.z, __fmul_rn(x[q].z, a[q].z)); acc.w = __fadd_rn(acc.w, __fmul_rn(x[q].w, a[q].w));
+          }
+        }
+      }
+      *reinterpret_cast<float4*>(o + d) = acc;
+    }
+  } else {
+    for (int d = sub; d < HC; d += G) {
+      const int hd = d / C;
+      float acc = 0.f;
+      for (int64_t k0 = b; k0 < e; k0 += kGatUnroll) {
+        float x[kGatUnroll], a[kGatUnroll];
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q) {
+          if (k0 + q < e) {
+            const int64_t ed = edge_at(perm, k0 + q);
+            x[q] = __ldg(h_src + (int64_t)__ldg(src + ed) * HC + d);
+            a[q] = alpha[ed * H + hd];
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q)
+          if (k0 + q < e) acc = __fadd_rn(acc, __fmul_rn(x[q], a[q]));
+      }
+      o[d] = acc;
+    }
+  }
+}
+
+// G lanes per target row r (edges as in k_gat_fwd).  Per head, lanes over the segment's edges:
+//   d_alpha[e] = <g[r, h-slice], h_src[src_e, h-slice]>        (a serial dot product over the C columns)
+//   S          = sum_seg alpha * d_alpha                         (serial in edge order)
+//   du[e]      = alpha * (d_alpha - S) * (u > 0 ? 1 : 0.2)       (to scratch, indexed by edge)
+//   grad_s_dst[r, h] = sum_seg du                                (serial in edge order)
+__global__ void __launch_bounds__(256) k_gat_bwd_dst(const float* __restrict__ g, const float* __restrict__ h_src,
+                                                     const float* __restrict__ alpha, const float* __restrict__ s_dst,
+                                                     const float* __restrict__ s_src, const int32_t* __restrict__ key,
+                                                     const int32_t* __restrict__ perm, const int32_t* __restrict__ src, int64_t E,
+                                                     int64_t n_dst, int H, int C, int G, float* __restrict__ du,
+                                                     float* __restrict__ grad_s_dst) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t r = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (r >= n_dst) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  const int64_t b = gat_lower_bound(key, E, r), e = gat_lower_bound(key, E, r + 1);
+  const int HC = H * C;   // < 2^31: checked by the launcher
+  for (int h = 0; h < H; ++h) {
+    const float* gr = g + r * (int64_t)HC + h * C;
+    float S = 0.f;
+    for (int64_t k0 = b; k0 < e; k0 += G) {
+      const int64_t k = k0 + sub;
+      float v = 0.f;
+      if (k < e) {
+        const int64_t ed = edge_at(perm, k);
+        const float* xs = h_src + (int64_t)__ldg(src + ed) * HC + h * C;
+        float da = 0.f;
+        for (int c = 0; c < C; ++c) da = fmaf(__ldg(gr + c), __ldg(xs + c), da);
+        du[ed * H + h] = da;
+        v = __fmul_rn(__ldg(alpha + ed * H + h), da);
+      }
+      const int n = e - k0 < G ? (int)(e - k0) : G;
+      for (int j = 0; j < n; ++j) S = __fadd_rn(S, __shfl_sync(gm, v, j, G));
+    }
+    const float sd = b < e ? __ldg(s_dst + r * H + h) : 0.f;
+    float T = 0.f;
+    for (int64_t k0 = b; k0 < e; k0 += G) {
+      const int64_t k = k0 + sub;
+      float v = 0.f;
+      if (k < e) {
+        const int64_t ed = edge_at(perm, k);
+        const float z = __fadd_rn(sd, __ldg(s_src + (int64_t)__ldg(src + ed) * H + h));
+        v = __fmul_rn(__fmul_rn(__ldg(alpha + ed * H + h), __fsub_rn(du[ed * H + h], S)), z > 0.f ? 1.f : 0.2f);
+        du[ed * H + h] = v;
+      }
+      const int n = e - k0 < G ? (int)(e - k0) : G;
+      for (int j = 0; j < n; ++j) T = __fadd_rn(T, __shfl_sync(gm, v, j, G));
+    }
+    if (sub == 0) grad_s_dst[r * H + h] = T;
+  }
+}
+
+// G lanes per source row j; its edges are positions [lb(j), lb(j+1)) of the src-sorted order `skey` (sperm: position ->
+// edge, ascending edge index within a source: the sort is stable).  grad_h_src[j, col] = sum alpha[e, head(col)] *
+// g[dst_e, col], grad_s_src[j, h] = sum du[e, h], both in edge order; a source without edges gets zeros.
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_gat_bwd_src(const float* __restrict__ g, const float* __restrict__ alpha,
+                                                     const float* __restrict__ du, const int32_t* __restrict__ skey,
+                                                     const int32_t* __restrict__ sperm, const int32_t* __restrict__ dst, int64_t E,
+                                                     int64_t n_src, int H, int C, int G, float* __restrict__ grad_h_src,
+                                                     float* __restrict__ grad_s_src) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t j = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (j >= n_src) return;
+  const int64_t b = gat_lower_bound(skey, E, j), e = gat_lower_bound(skey, E, j + 1);
+  const int HC = H * C;   // < 2^31: checked by the launcher
+  float* o = grad_h_src + j * (int64_t)HC;
+  if (VEC) {
+    for (int d = sub * 4; d < HC; d += G * 4) {
+      const int h0 = d / C, h1 = (d + 1) / C, h2 = (d + 2) / C, h3 = (d + 3) / C;
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int64_t k0 = b; k0 < e; k0 += kGatUnroll) {
+        float4 x[kGatUnroll], a[kGatUnroll];
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q) {
+          if (k0 + q < e) {
+            const int64_t ed = __ldg(sperm + k0 + q);
+            x[q] = __ldg(reinterpret_cast<const float4*>(g + (int64_t)__ldg(dst + ed) * HC + d));
+            const float* al = alpha + ed * H;
+            a[q] = make_float4(__ldg(al + h0), __ldg(al + h1), __ldg(al + h2), __ldg(al + h3));
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q) {
+          if (k0 + q < e) {
+            acc.x = __fadd_rn(acc.x, __fmul_rn(a[q].x, x[q].x)); acc.y = __fadd_rn(acc.y, __fmul_rn(a[q].y, x[q].y));
+            acc.z = __fadd_rn(acc.z, __fmul_rn(a[q].z, x[q].z)); acc.w = __fadd_rn(acc.w, __fmul_rn(a[q].w, x[q].w));
+          }
+        }
+      }
+      *reinterpret_cast<float4*>(o + d) = acc;
+    }
+  } else {
+    for (int d = sub; d < HC; d += G) {
+      const int hd = d / C;
+      float acc = 0.f;
+      for (int64_t k0 = b; k0 < e; k0 += kGatUnroll) {
+        float x[kGatUnroll], a[kGatUnroll];
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q) {
+          if (k0 + q < e) {
+            const int64_t ed = __ldg(sperm + k0 + q);
+            x[q] = __ldg(g + (int64_t)__ldg(dst + ed) * HC + d);
+            a[q] = __ldg(alpha + ed * H + hd);
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < kGatUnroll; ++q)
+          if (k0 + q < e) acc = __fadd_rn(acc, __fmul_rn(a[q], x[q]));
+      }
+      o[d] = acc;
+    }
+  }
+  for (int h = sub; h < H; h += G) {
+    float acc = 0.f;
+    for (int64_t k = b; k < e; ++k) acc = __fadd_rn(acc, __ldg(du + (int64_t)__ldg(sperm + k) * H + h));
+    grad_s_src[j * H + h] = acc;
+  }
+}
+
+static bool gat_aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+static size_t a256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// The order the kernels walk the edges in: by `idx` (int32[E] in [0, n)), stable.
+struct GatOrder {
+  const int32_t* key = nullptr;    // idx itself when it is already non-decreasing
+  const int32_t* perm = nullptr;   // null then
+};
+
+static int sort_bits(int64_t n) {
+  int b = 1;
+  while (b < 31 && ((int64_t)1 << b) < n) ++b;
+  return b;
+}
+
+static size_t order_bytes(int64_t E, int64_t n) {
+  size_t t = 0;
+  cub::DeviceRadixSort::SortPairs((void*)nullptr, t, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
+                                  (int32_t*)nullptr, (int)E, 0, sort_bits(n));
+  return 3 * a256(4 * (size_t)E) + a256(t);
+}
+
+// Stable order of the edges by idx, in `buf` (order_bytes(E, n) bytes): keys, permutation (edge of each position).
+static int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, GatOrder* o) {
+  cudaStream_t s = c->stream;
+  int32_t* keys = (int32_t*)buf;
+  int32_t* perm = (int32_t*)(buf + a256(4 * (size_t)E));
+  int32_t* iota = (int32_t*)(buf + 2 * a256(4 * (size_t)E));
+  void* tmp = buf + 3 * a256(4 * (size_t)E);
+  size_t t = 0;
+  cub::DeviceRadixSort::SortPairs((void*)nullptr, t, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
+                                  (int32_t*)nullptr, (int)E, 0, sort_bits(n), s);
+  k_gat_iota<<<(unsigned)std::min<int64_t>(ceil_div(E, 256), kSMs * 8), 256, 0, s>>>(iota, E);
+  EU_LAUNCHED();
+  EU_CUDA(cub::DeviceRadixSort::SortPairs(tmp, t, (const uint32_t*)idx, (uint32_t*)keys, (const int32_t*)iota, perm, (int)E, 0,
+                                          sort_bits(n), s));
+  EU_LAUNCHED();
+  o->key = keys;
+  o->perm = perm;
+  return EU_OK;
+}
+
+// Is idx non-decreasing?  One flag read back to the host (a stream synchronisation).
+static int is_sorted(eu_ctx* c, const int32_t* idx, int64_t E, int* flag_dev, bool* sorted) {
+  *sorted = true;
+  if (E < 2) return EU_OK;
+  cudaStream_t s = c->stream;
+  EU_CUDA(cudaMemsetAsync(flag_dev, 0, sizeof(int), s));
+  k_check_sorted<<<(unsigned)ceil_div(E, 256), 256, 0, s>>>(idx, E, flag_dev);
+  EU_LAUNCHED();
+  int h = 0;
+  EU_CUDA(cudaMemcpyAsync(&h, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
+  EU_CUDA(cudaStreamSynchronize(s));
+  *sorted = h == 0;
+  return EU_OK;
+}
+
+}  // namespace eu
+
+using namespace eu;
+
+extern "C" {
+
+int eu_gat_aggregate(eu_ctx* c, const float* h_src, const float* s_dst, const float* s_src, const int32_t* dst, const int32_t* src,
+                     int64_t E, int64_t n_dst, int64_t n_src, int32_t heads, int32_t head_dim, float* out, float* alpha) {
+  if (!c || heads < 1 || head_dim < 1 || E < 0 || n_dst < 0 || n_src < 0 || (E > 0 && (n_dst == 0 || n_src == 0)) ||
+      (E > 0 && (!h_src || !s_dst || !s_src || !dst || !src)) || (n_dst > 0 && !out)) {
+    set_error("eu_gat_aggregate: bad argument");
+    return EU_ERR_INVALID;
+  }
+  if (E >= ((int64_t)1 << 31) || n_dst >= ((int64_t)1 << 31) || n_src >= ((int64_t)1 << 31) || (int64_t)heads * head_dim >= ((int64_t)1 << 31)) {
+    set_error("eu_gat_aggregate: 2^31 or more edges, rows or columns are not supported");
+    return EU_ERR_UNSUPPORTED;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (n_dst == 0) return EU_OK;
+  cudaStream_t s = c->stream;
+  const int64_t H = heads, HC = H * head_dim;
+  // flag | [alpha scratch when the caller wants none] | [the dst order when dst is unsorted]; sized once the flag is read, so
+  // a sorted dst holds no sort scratch (a growth reallocates: nothing but the flag has been written yet)
+  int rc = ctx_misc(c, 256);
+  if (rc) return rc;
+  bool sorted = true;
+  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
+  const size_t o_alpha = 256, o_ord = o_alpha + (alpha ? 0 : a256(4 * (size_t)(E * H)));
+  if ((rc = ctx_misc(c, (int64_t)(o_ord + (sorted ? 0 : order_bytes(E, n_dst)))))) return rc;
+  char* m = (char*)c->d_misc;
+  float* al = alpha ? alpha : (float*)(m + o_alpha);
+  GatOrder ord;
+  ord.key = dst;
+  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_ord, &ord))) return rc;
+  const bool vec = HC % 4 == 0 && gat_aligned16(h_src) && gat_aligned16(out);
+  const int G = gat_lanes(HC, vec);
+  const unsigned blocks = (unsigned)ceil_div(n_dst * G, 256);
+  EuProfScope ps(c, "gat_fwd", E);
+  if (vec) k_gat_fwd<true><<<blocks, 256, 0, s>>>(h_src, s_dst, s_src, ord.key, ord.perm, src, E, n_dst, heads, head_dim, G, al, out);
+  else k_gat_fwd<false><<<blocks, 256, 0, s>>>(h_src, s_dst, s_src, ord.key, ord.perm, src, E, n_dst, heads, head_dim, G, al, out);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+int eu_gat_aggregate_backward(eu_ctx* c, const float* grad_out, const float* h_src, const float* alpha, const float* s_dst,
+                              const float* s_src, const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src,
+                              int32_t heads, int32_t head_dim, float* grad_h_src, float* grad_s_dst, float* grad_s_src) {
+  if (!c || heads < 1 || head_dim < 1 || E < 0 || n_dst < 0 || n_src < 0 || (E > 0 && (n_dst == 0 || n_src == 0)) ||
+      (E > 0 && (!grad_out || !h_src || !alpha || !s_dst || !s_src || !dst || !src)) || (n_dst > 0 && !grad_s_dst) ||
+      (n_src > 0 && (!grad_h_src || !grad_s_src))) {
+    set_error("eu_gat_aggregate_backward: bad argument");
+    return EU_ERR_INVALID;
+  }
+  if (E >= ((int64_t)1 << 31) || n_dst >= ((int64_t)1 << 31) || n_src >= ((int64_t)1 << 31) || (int64_t)heads * head_dim >= ((int64_t)1 << 31)) {
+    set_error("eu_gat_aggregate_backward: 2^31 or more edges, rows or columns are not supported");
+    return EU_ERR_UNSUPPORTED;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  cudaStream_t s = c->stream;
+  const int64_t H = heads, HC = H * head_dim;
+  if (E == 0) {                                        // no edge: every gradient is zero
+    if (n_dst > 0) EU_CUDA(cudaMemsetAsync(grad_s_dst, 0, 4 * (size_t)(n_dst * H), s));
+    if (n_src > 0) {
+      EU_CUDA(cudaMemsetAsync(grad_h_src, 0, 4 * (size_t)(n_src * HC), s));
+      EU_CUDA(cudaMemsetAsync(grad_s_src, 0, 4 * (size_t)(n_src * H), s));
+    }
+    return EU_OK;
+  }
+  // flag | du [E, H] | [the dst order when dst is unsorted] | the src order; sized once the flag is read
+  int rc = ctx_misc(c, 256);
+  if (rc) return rc;
+  bool sorted = true;
+  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
+  const size_t o_du = 256, o_dord = o_du + a256(4 * (size_t)(E * H)), o_sord = o_dord + (sorted ? 0 : order_bytes(E, n_dst));
+  if ((rc = ctx_misc(c, (int64_t)(o_sord + order_bytes(E, n_src))))) return rc;
+  char* m = (char*)c->d_misc;
+  float* du = (float*)(m + o_du);
+  GatOrder dord, sord;
+  dord.key = dst;
+  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_dord, &dord))) return rc;
+  {
+    const int G = 32;   // lanes over a segment's edges
+    EuProfScope ps(c, "gat_bwd_dst", E);
+    k_gat_bwd_dst<<<(unsigned)ceil_div(n_dst * G, 256), 256, 0, s>>>(grad_out, h_src, alpha, s_dst, s_src, dord.key, dord.perm, src, E,
+                                                                    n_dst, heads, head_dim, G, du, grad_s_dst);
+    EU_LAUNCHED();
+  }
+  if ((rc = order_by(c, src, E, n_src, m + o_sord, &sord))) return rc;
+  {
+    const bool vec = HC % 4 == 0 && gat_aligned16(grad_out) && gat_aligned16(grad_h_src);
+    const int G = gat_lanes(HC, vec);
+    EuProfScope ps(c, "gat_bwd_src", E);
+    if (vec) k_gat_bwd_src<true><<<(unsigned)ceil_div(n_src * G, 256), 256, 0, s>>>(grad_out, alpha, du, sord.key, sord.perm, dst, E, n_src,
+                                                                                   heads, head_dim, G, grad_h_src, grad_s_src);
+    else k_gat_bwd_src<false><<<(unsigned)ceil_div(n_src * G, 256), 256, 0, s>>>(grad_out, alpha, du, sord.key, sord.perm, dst, E, n_src,
+                                                                                heads, head_dim, G, grad_h_src, grad_s_src);
+    EU_LAUNCHED();
+  }
+  return EU_OK;
+}
+
+}  // extern "C"

@@ -180,6 +180,7 @@ int64_t hop_scratch_rows(int nb, int64_t rows_b);
 int64_t hop_table_slots(int nb, int64_t rows_b);
 int64_t hop_table_cap(int64_t rows_b);   // dedup slots per batch (region stride = cap + 1)
 int ctx_misc(eu_ctx* c, int64_t bytes);
+__global__ void k_check_sorted(const int32_t* __restrict__ idx, int64_t E, int* unsorted);   // mp_ops.cu: *unsorted = 1 if idx decreases
 int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
 int ctx_stage(eu_ctx* c, int64_t host_bytes, int64_t dev_bytes);

@@ -750,3 +750,68 @@ def scatter_softmax(updates, indices, size=None):
     updates = updates - gather(scatter_max(updates, indices, size), indices)
     updates = torch.exp(updates)
     return updates / gather(scatter_add(updates, indices, size), indices)
+
+
+def _raw_gat(h_src, s_dst, s_src, dst, src, n_dst, with_alpha):
+    """one eu_gat_aggregate: (out f32[n_dst, H*C], alpha f32[E, H] or None)"""
+    n_src, H = s_src.shape
+    E = dst.numel()
+    out = torch.empty((n_dst, h_src.shape[1]), dtype=torch.float32, device=h_src.device)
+    alpha = torch.empty((E, H), dtype=torch.float32, device=h_src.device) if with_alpha else None
+    ctx = _ctx_on_stream()
+    check(_lib.load().eu_gat_aggregate(ctx._h, h_src.data_ptr(), s_dst.data_ptr(), s_src.data_ptr(), dst.data_ptr(),
+                                       src.data_ptr(), E, n_dst, n_src, H, h_src.shape[1] // H, out.data_ptr(),
+                                       alpha.data_ptr() if with_alpha else None))
+    return out, alpha
+
+
+class _GatAggregate(torch.autograd.Function):
+    """eu_gat_aggregate / eu_gat_aggregate_backward.  Saves alpha [E, H], never the [E, H*C] messages."""
+
+    @staticmethod
+    def forward(ctx, h_src, s_dst, s_src, dst, src, n_dst):
+        want_alpha = any(ctx.needs_input_grad[:3])
+        out, alpha = _raw_gat(h_src, s_dst, s_src, dst, src, n_dst, want_alpha)
+        if want_alpha:
+            ctx.save_for_backward(h_src, s_dst, s_src, dst, src, alpha)
+        ctx.dims = (n_dst, s_src.shape[0], s_src.shape[1], h_src.shape[1] // s_src.shape[1])
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        h_src, s_dst, s_src, dst, src, alpha = ctx.saved_tensors
+        n_dst, n_src, H, C = ctx.dims
+        grad = grad.contiguous()
+        dev = grad.device
+        g_h = torch.empty((n_src, H * C), dtype=torch.float32, device=dev)
+        g_sd = torch.empty((n_dst, H), dtype=torch.float32, device=dev)
+        g_ss = torch.empty((n_src, H), dtype=torch.float32, device=dev)
+        ec = _ctx_on_stream()
+        check(_lib.load().eu_gat_aggregate_backward(ec._h, grad.data_ptr(), h_src.data_ptr(), alpha.data_ptr(), s_dst.data_ptr(),
+                                                    s_src.data_ptr(), dst.data_ptr(), src.data_ptr(), dst.numel(), n_dst, n_src,
+                                                    H, C, g_h.data_ptr(), g_sd.data_ptr(), g_ss.data_ptr()))
+        return g_h, g_sd, g_ss, None, None, None
+
+
+def gat_attention_aggregate(h_src, s_dst, s_src, edge_index, size):
+    """GATConv's attention aggregation (gat_conv.py:53-78 with aggr='add', after its `fc`) in one fused device op:
+        h_src f32[n_src, H*C]   source rows, heads concatenated per row
+        s_dst f32[n_dst, H]     per-target scores att_i(x_target), s_src f32[n_src, H] per-source scores att_j(x_source)
+        edge_index [2, E]       (target, source) per edge; size = (n_dst, n_src)
+    out[i, h*C:(h+1)*C] = sum over edges (i, j) of alpha[e,h] * h_src[j, h-slice], alpha = scatter_softmax of
+    leaky_relu(s_dst[i,h] + s_src[j,h], 0.2) over the edges of each target.  For non-decreasing edge_index[0] the result
+    equals, bit for bit, the same composition of gather / scatter_softmax / scatter_add; the backward pass is deterministic.
+    Synchronises once per call (whether edge_index[0] is sorted); an unsorted one costs a radix sort."""
+    n_dst, n_src = int(size[0]), int(size[1])
+    if any(not torch.is_tensor(t) or t.dim() != 2 for t in (h_src, s_dst, s_src)):
+        raise EulerError("gat_attention_aggregate: h_src, s_dst and s_src must be 2-D tensors")
+    h_src, s_dst, s_src = _f32(h_src), _f32(s_dst), _f32(s_src)
+    H = s_dst.shape[1]
+    if H < 1 or s_src.shape != (n_src, H) or s_dst.shape[0] != n_dst or h_src.shape[0] != n_src or h_src.shape[1] % H:
+        raise EulerError("gat_attention_aggregate: need h_src [n_src, H*C], s_dst [n_dst, H], s_src [n_src, H]; got %s, %s, %s"
+                         % (tuple(h_src.shape), tuple(s_dst.shape), tuple(s_src.shape)))
+    ei = _t(edge_index, torch.int32)
+    if ei.dim() != 2 or ei.shape[0] != 2:
+        raise EulerError("gat_attention_aggregate: edge_index must be [2, E]")
+    dst, src = ei[0].contiguous(), ei[1].contiguous()
+    return _GatAggregate.apply(h_src, s_dst, s_src, dst, src, n_dst)

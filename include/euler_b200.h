@@ -390,6 +390,31 @@ int eu_sage_mean_aggregate_host(eu_ctx* c, const int64_t* nbr_ids, int64_t rows,
                                 int32_t dim, float* out);
 /* the same block with aggr = 'add' (scatter_add, tf_euler/kernels/scatter_op.cc:44-55): out[r,:] = sum_j feat[row(nbr_ids[r*count+j]),:] */
 int eu_sage_add_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out);
+/* GATConv's attention aggregation (tf_euler/python/convolution/gat_conv.py:53-78, aggr = 'add', after its `fc`), fused.
+ * H = heads, C = head_dim; inputs h_src f32[n_src, H*C] (heads concatenated per row), s_dst f32[n_dst, H] and
+ * s_src f32[n_src, H] (the per-node scores att_i(x), att_j(x)), dst / src i32[E] (edge_index[0] / [1]).  For head h:
+ *   u[e,h]     = leaky_relu(s_dst[dst_e,h] + s_src[src_e,h], 0.2)
+ *   alpha[e,h] = scatter_softmax(u, dst, n_dst)        (running max from -1e9, as scatter_max: a target whose logits are
+ *                                                       all below -1e9 gets NaN alphas)
+ *   out[i, h*C:(h+1)*C] = sum over the edges e with dst_e = i of alpha[e,h] * h_src[src_e, h*C:(h+1)*C]
+ * out f32[n_dst, H*C] (a target without edges gets a zero row); alpha f32[E, H] may be NULL (not written).
+ * For non-decreasing dst, out and alpha equal bit for bit gather -> add -> leaky_relu -> scatter_softmax -> multiply ->
+ * scatter_add composed from the ops above: every sum runs left to right in edge order.  Unsorted dst is ordered by a stable
+ * sort first: the result is bit-identical to the call on the stably sorted edge list.
+ * The backward pass takes the forward's alpha and the gradient of out, grad_out f32[n_dst, H*C], and writes
+ *   grad_h_src f32[n_src, H*C], grad_s_dst f32[n_dst, H], grad_s_src f32[n_src, H]
+ * with d_alpha = <grad_out[dst_e, h-slice], h_src[src_e, h-slice]> and du = alpha * (d_alpha - sum_seg alpha * d_alpha) *
+ * (u > 0 ? 1 : 0.2); per-target sums run over the dst order, per-source sums over a stable sort of the edges by src, each
+ * in edge order: deterministic, no atomics.  Rows without edges get zeros.
+ * heads < 1, head_dim < 1, negative sizes, edges with n_dst or n_src = 0, or a NULL pointer that is needed: EU_ERR_INVALID;
+ * 2^31 or more edges, rows or H*C columns: EU_ERR_UNSUPPORTED.  Indices are not checked (as eu_gather).  Device pointers;
+ * both calls synchronise the stream once to read whether dst is sorted (an unsorted dst costs a radix sort, a sorted one
+ * nothing more), and they use the ctx scratch. */
+int eu_gat_aggregate(eu_ctx* c, const float* h_src, const float* s_dst, const float* s_src, const int32_t* dst, const int32_t* src,
+                     int64_t E, int64_t n_dst, int64_t n_src, int32_t heads, int32_t head_dim, float* out, float* alpha);
+int eu_gat_aggregate_backward(eu_ctx* c, const float* grad_out, const float* h_src, const float* alpha, const float* s_dst,
+                              const float* s_src, const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src,
+                              int32_t heads, int32_t head_dim, float* grad_h_src, float* grad_s_dst, float* grad_s_src);
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx,
                    int64_t E, float* out);
 int eu_scatter_add_host(eu_ctx* c, const float* updates, int64_t D, const int32_t* idx, int64_t E,
