@@ -60,7 +60,7 @@ def composition(ops, F, h, sd, ss, dst, src, n_dst):
 ARMS = ("fused_fwd", "composition_fwd", "fused_fwd_bwd", "composition_fwd_bwd")
 
 
-def block_edges(args):
+def block_edges(args, self_loops=False):
     """the benchmark block: (dst, src) int32 on the device, its sizes and each target's edge count"""
     import torch
     import euler_b200 as eb
@@ -68,7 +68,7 @@ def block_edges(args):
     graph = eb.Graph.rmat(args.nodes, args.edges, seed=GRAPH_SEED, device=0)
     eb.set_graph(graph)
     seeds = torch.from_numpy(np.random.RandomState(7000).randint(1, args.nodes + 1, size=args.batch).astype(np.int64)).cuda()
-    blk = GCNDataFlow([[0], [0]], add_self_loops=False)(seeds)[0]
+    blk = GCNDataFlow([[0], [0]], add_self_loops=self_loops)(seeds)[0]
     ei = blk.edge_index.to(torch.int32)
     n_dst, n_src = blk.size
     dst, src = ei[0].contiguous(), ei[1].contiguous()

@@ -9,6 +9,8 @@ with the framework (torch here): they are GEMMs, not part of the sampling / aggr
   sage_aggregate     tf_euler/python/convolution/sage_conv.py:33-38   gather(x, edge_index[1]) -> scatter_mean
   gat_aggregate      tf_euler/python/convolution/gat_conv.py:53-78    per-node attention scores, then the fused softmax-weighted
                                                                       sum over each target's edges (ops.gat_attention_aggregate)
+  agnn_aggregate     tf_euler/python/convolution/agnn_conv.py:32-54   l2_normalize in torch, then the fused cosine logits,
+                                                                      softmax and weighted sum (ops.agnn_attention_aggregate)
 """
 import torch
 
@@ -75,3 +77,26 @@ def gat_aggregate(x, edge_index, size, att_i, att_j, improved=False, aggr='add')
     s_src = (x1.reshape(x1.shape[0], H, C) * att_j).sum(-1)
     out = ops.gat_attention_aggregate(x1, s_dst, s_src, edge_index, size)
     return x0 + out if improved else out
+
+
+def l2_normalize(x):
+    """tf.nn.l2_normalize(x, axis=-1) as TF writes it: x * rsqrt(max(sum(x * x, -1), 1e-12))"""
+    return x * torch.rsqrt(torch.clamp_min((x * x).sum(-1, keepdim=True), 1e-12))
+
+
+def agnn_aggregate(x, edge_index, size, beta):
+    """AGNNConv.__call__ (agnn_conv.py:32-54): x = (x_target, x_source), x_source None meaning x_target; beta the conv's
+    trainable scalar (a one-element tensor, upstream tf.Variable([1.])).  l2_normalize runs here, in torch, so autograd
+    reaches x through it; the cosine logits, the softmax over each target's edges and the weighted sum of the (raw) source
+    rows are the fused device op.  apply_node is the identity."""
+    if torch.is_tensor(x) or x[0] is None:
+        raise EulerError("agnn_aggregate: x must be (x_target, x_source): the logits read the normalized targets")
+    x0, x1 = x[0], x[1] if x[1] is not None else x[0]
+    if not torch.is_tensor(beta) or beta.numel() != 1:
+        raise EulerError("agnn_aggregate: beta must be a one-element tensor")
+    if x0.dim() != 2 or x1.dim() != 2 or x0.shape[1] != x1.shape[1]:
+        raise EulerError("agnn_aggregate: x_target and x_source must be [n, D] of one width; got %s, %s"
+                         % (tuple(x0.shape), tuple(x1.shape)))
+    n1 = l2_normalize(x1)
+    n0 = n1 if x0 is x1 else l2_normalize(x0)
+    return ops.agnn_attention_aggregate(x1, n0, n1, beta, edge_index, size)

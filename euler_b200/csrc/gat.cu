@@ -18,6 +18,11 @@
 // Backward: one kernel per target row (d_alpha, du, grad_s_dst; du to scratch), a stable radix sort of the edges by source,
 // one kernel per source row (grad_h_src, grad_s_src).  Every sum runs in edge order within its segment: deterministic, no
 // atomics.
+//
+// AGNNConv's aggregation (agnn_conv.py:32-54, aggr = 'add') is the same softmax and weighted sum with H = 1, C = dim and a
+// cosine logit per edge, u[e] = beta * <nrm_dst[dst_e], nrm_src[src_e]>, computed edge-parallel first (k_agnn_dot) and read
+// by k_gat_fwd<VEC, true>.  Its backward reuses k_agnn_dot (d_alpha), k_gat_bwd_src (every segmented row sum, by target and
+// by source) and the orders above; see eu_agnn_aggregate_backward.
 #include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
@@ -65,7 +70,8 @@ constexpr int kGatUnroll = 8;   // source rows in flight per lane in the ordered
 // Per head: the max of the logits (a group reduction: max is exact in any order), the exps (in parallel) and their sum (a
 // serial chain in edge order, broadcast lane by lane), then alpha = exp / sum.  alpha doubles as the scratch of u and exp.
 // Then the columns: lanes over H*C, edges in order, kGatUnroll source rows loaded ahead of the ordered adds.
-template <bool VEC>
+// PRE: the logits are already in alpha (AGNN's beta * cos); s_dst and s_src are not read.
+template <bool VEC, bool PRE>
 __global__ void __launch_bounds__(256) k_gat_fwd(const float* __restrict__ h_src, const float* __restrict__ s_dst,
                                                  const float* __restrict__ s_src, const int32_t* __restrict__ key,
                                                  const int32_t* __restrict__ perm, const int32_t* __restrict__ src, int64_t E,
@@ -79,12 +85,17 @@ __global__ void __launch_bounds__(256) k_gat_fwd(const float* __restrict__ h_src
   const int64_t b = gat_lower_bound(key, E, r), e = gat_lower_bound(key, E, r + 1);
   const int HC = H * C;   // < 2^31: checked by the launcher
   for (int h = 0; h < H && b < e; ++h) {
-    const float sd = __ldg(s_dst + r * H + h);
+    const float sd = PRE ? 0.f : __ldg(s_dst + r * H + h);
     float m = -1e9f;                                   // scatter_max's initial value; a NaN logit never wins
     for (int64_t k = b + sub; k < e; k += G) {
       const int64_t ed = edge_at(perm, k);
-      const float u = leaky(__fadd_rn(sd, __ldg(s_src + (int64_t)__ldg(src + ed) * H + h)));
-      alpha[ed * H + h] = u;
+      float u;
+      if (PRE) {
+        u = alpha[ed * H + h];
+      } else {
+        u = leaky(__fadd_rn(sd, __ldg(s_src + (int64_t)__ldg(src + ed) * H + h)));
+        alpha[ed * H + h] = u;
+      }
       m = u > m ? u : m;
     }
     for (int o = G >> 1; o > 0; o >>= 1) {
@@ -212,8 +223,10 @@ __global__ void __launch_bounds__(256) k_gat_bwd_dst(const float* __restrict__ g
 }
 
 // G lanes per source row j; its edges are positions [lb(j), lb(j+1)) of the src-sorted order `skey` (sperm: position ->
-// edge, ascending edge index within a source: the sort is stable).  grad_h_src[j, col] = sum alpha[e, head(col)] *
-// g[dst_e, col], grad_s_src[j, h] = sum du[e, h], both in edge order; a source without edges gets zeros.
+// edge, ascending edge index within a source: the sort is stable; null when skey is already sorted).
+// grad_h_src[j, col] = sum alpha[e, head(col)] * g[dst_e, col], grad_s_src[j, h] = sum du[e, h] (when grad_s_src is given),
+// both in edge order; a source without edges gets zeros.  AGNN's backward runs it as a plain segmented weighted row sum,
+// also over the dst order.
 template <bool VEC>
 __global__ void __launch_bounds__(256) k_gat_bwd_src(const float* __restrict__ g, const float* __restrict__ alpha,
                                                      const float* __restrict__ du, const int32_t* __restrict__ skey,
@@ -236,7 +249,7 @@ __global__ void __launch_bounds__(256) k_gat_bwd_src(const float* __restrict__ g
 #pragma unroll
         for (int q = 0; q < kGatUnroll; ++q) {
           if (k0 + q < e) {
-            const int64_t ed = __ldg(sperm + k0 + q);
+            const int64_t ed = edge_at(sperm, k0 + q);
             x[q] = __ldg(reinterpret_cast<const float4*>(g + (int64_t)__ldg(dst + ed) * HC + d));
             const float* al = alpha + ed * H;
             a[q] = make_float4(__ldg(al + h0), __ldg(al + h1), __ldg(al + h2), __ldg(al + h3));
@@ -261,7 +274,7 @@ __global__ void __launch_bounds__(256) k_gat_bwd_src(const float* __restrict__ g
 #pragma unroll
         for (int q = 0; q < kGatUnroll; ++q) {
           if (k0 + q < e) {
-            const int64_t ed = __ldg(sperm + k0 + q);
+            const int64_t ed = edge_at(sperm, k0 + q);
             x[q] = __ldg(g + (int64_t)__ldg(dst + ed) * HC + d);
             a[q] = __ldg(alpha + ed * H + hd);
           }
@@ -273,11 +286,106 @@ __global__ void __launch_bounds__(256) k_gat_bwd_src(const float* __restrict__ g
       o[d] = acc;
     }
   }
+  if (!grad_s_src) return;
   for (int h = sub; h < H; h += G) {
     float acc = 0.f;
-    for (int64_t k = b; k < e; ++k) acc = __fadd_rn(acc, __ldg(du + (int64_t)__ldg(sperm + k) * H + h));
+    for (int64_t k = b; k < e; ++k) acc = __fadd_rn(acc, __ldg(du + edge_at(sperm, k) * H + h));
     grad_s_src[j * H + h] = acc;
   }
+}
+
+// G lanes per edge e (a power of two <= 32): dot[e] = <a[ia_e, :], b[ib_e, :]> over dim columns, and scaled[e] =
+// beta[0] * dot[e] when scaled is given.  The order is fixed: lane l accumulates, one __fmaf_rn at a time, the columns of
+// its 4-column chunks l, l + G, l + 2G, ..., each chunk left to right; then a butterfly over the G lanes, xor distances G/2,
+// ..., 1 (both lanes of a pair add the same two values, so every lane ends with the same bits).  VEC (dim % 4 == 0,
+// 16-byte aligned rows) changes only the loads: the bits do not depend on the alignment.
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_agnn_dot(const float* __restrict__ a, const float* __restrict__ b,
+                                                  const int32_t* __restrict__ ia, const int32_t* __restrict__ ib, int64_t E,
+                                                  int dim, int G, const float* __restrict__ beta, float* __restrict__ dot,
+                                                  float* __restrict__ scaled) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t e = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (e >= E) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  const float* ar = a + (int64_t)__ldg(ia + e) * dim;
+  const float* br = b + (int64_t)__ldg(ib + e) * dim;
+  float acc = 0.f;
+#pragma unroll 4
+  for (int d = sub * 4; d < dim; d += G * 4) {
+    if (VEC) {
+      const float4 x = __ldg(reinterpret_cast<const float4*>(ar + d)), y = __ldg(reinterpret_cast<const float4*>(br + d));
+      acc = __fmaf_rn(x.x, y.x, acc); acc = __fmaf_rn(x.y, y.y, acc);
+      acc = __fmaf_rn(x.z, y.z, acc); acc = __fmaf_rn(x.w, y.w, acc);
+    } else {
+      const int n = dim - d < 4 ? dim - d : 4;
+      for (int q = 0; q < n; ++q) acc = __fmaf_rn(__ldg(ar + d + q), __ldg(br + d + q), acc);
+    }
+  }
+  for (int o = G >> 1; o > 0; o >>= 1) acc = __fadd_rn(acc, __shfl_xor_sync(gm, acc, o, G));
+  if (sub == 0) {
+    if (dot) dot[e] = acc;
+    if (scaled) scaled[e] = __fmul_rn(__ldg(beta), acc);
+  }
+}
+
+// G lanes per target row r (edges as in k_gat_fwd), H = 1.  dw holds d_alpha[e] = <grad_out[dst_e], x_src[src_e]> on entry.
+// In edge order: S = sum alpha * d_alpha; du = alpha * (d_alpha - S); dw[e] = beta * du (the gradient of cos[e]);
+// part[r] = sum du * cos (this target's share of grad_beta).
+__global__ void __launch_bounds__(256) k_agnn_bwd_dst(const float* __restrict__ alpha, const float* __restrict__ cos,
+                                                      const float* __restrict__ beta, const int32_t* __restrict__ key,
+                                                      const int32_t* __restrict__ perm, int64_t E, int64_t n_dst, int G,
+                                                      float* __restrict__ dw, float* __restrict__ part) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t r = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (r >= n_dst) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  const int64_t b = gat_lower_bound(key, E, r), e = gat_lower_bound(key, E, r + 1);
+  float S = 0.f;
+  for (int64_t k0 = b; k0 < e; k0 += G) {
+    const int64_t k = k0 + sub;
+    float v = 0.f;
+    if (k < e) {
+      const int64_t ed = edge_at(perm, k);
+      v = __fmul_rn(__ldg(alpha + ed), dw[ed]);
+    }
+    const int n = e - k0 < G ? (int)(e - k0) : G;
+    for (int j = 0; j < n; ++j) S = __fadd_rn(S, __shfl_sync(gm, v, j, G));
+  }
+  const float bt = __ldg(beta);
+  float P = 0.f;
+  for (int64_t k0 = b; k0 < e; k0 += G) {
+    const int64_t k = k0 + sub;
+    float v = 0.f;
+    if (k < e) {
+      const int64_t ed = edge_at(perm, k);
+      const float du = __fmul_rn(__ldg(alpha + ed), __fsub_rn(dw[ed], S));
+      dw[ed] = __fmul_rn(bt, du);
+      v = __fmul_rn(du, __ldg(cos + ed));
+    }
+    const int n = e - k0 < G ? (int)(e - k0) : G;
+    for (int j = 0; j < n; ++j) P = __fadd_rn(P, __shfl_sync(gm, v, j, G));
+  }
+  if (sub == 0) part[r] = P;
+}
+
+constexpr int kAgnnSumThreads = 1024;
+
+// *out = sum of v[0, n) in a fixed order: thread t adds v[t], v[t + 1024], ... left to right, then a shared-memory tree
+// (strides 512, ..., 1).  One block.
+__global__ void __launch_bounds__(kAgnnSumThreads) k_agnn_sum(const float* __restrict__ v, int64_t n, float* __restrict__ out) {
+  __shared__ float sh[kAgnnSumThreads];
+  float acc = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += kAgnnSumThreads) acc = __fadd_rn(acc, __ldg(v + i));
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int s = kAgnnSumThreads / 2; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) sh[threadIdx.x] = __fadd_rn(sh[threadIdx.x], sh[threadIdx.x + s]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *out = sh[0];
 }
 
 static bool gat_aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
@@ -337,6 +445,30 @@ static int is_sorted(eu_ctx* c, const int32_t* idx, int64_t E, int* flag_dev, bo
   return EU_OK;
 }
 
+// k_agnn_dot over E > 0 edges: dot[e] = <a[ia_e], b[ib_e]>, scaled[e] = beta * dot[e] (either output may be null)
+static int agnn_dot(eu_ctx* c, const float* a, const float* b, const int32_t* ia, const int32_t* ib, int64_t E, int dim,
+                    const float* beta, float* dot, float* scaled) {
+  const bool vec = dim % 4 == 0 && gat_aligned16(a) && gat_aligned16(b);
+  const int G = gat_lanes(ceil_div(dim, 4), false);   // one lane per 4-column chunk, both paths: the same order
+  const unsigned blocks = (unsigned)ceil_div(E * G, 256);
+  if (vec) k_agnn_dot<true><<<blocks, 256, 0, c->stream>>>(a, b, ia, ib, E, dim, G, beta, dot, scaled);
+  else k_agnn_dot<false><<<blocks, 256, 0, c->stream>>>(a, b, ia, ib, E, dim, G, beta, dot, scaled);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+// out[r, :] = sum of w[e] * rows[idx_e, :] over the edges of segment r of the order o, in edge order (k_gat_bwd_src, H = 1)
+static int agnn_row_sum(eu_ctx* c, const float* rows, const float* w, const GatOrder& o, const int32_t* idx, int64_t E,
+                        int64_t n, int dim, float* out) {
+  const bool vec = dim % 4 == 0 && gat_aligned16(rows) && gat_aligned16(out);
+  const int G = gat_lanes(dim, vec);
+  const unsigned blocks = (unsigned)ceil_div(n * G, 256);
+  if (vec) k_gat_bwd_src<true><<<blocks, 256, 0, c->stream>>>(rows, w, nullptr, o.key, o.perm, idx, E, n, 1, dim, G, out, nullptr);
+  else k_gat_bwd_src<false><<<blocks, 256, 0, c->stream>>>(rows, w, nullptr, o.key, o.perm, idx, E, n, 1, dim, G, out, nullptr);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
 }  // namespace eu
 
 using namespace eu;
@@ -375,8 +507,8 @@ int eu_gat_aggregate(eu_ctx* c, const float* h_src, const float* s_dst, const fl
   const int G = gat_lanes(HC, vec);
   const unsigned blocks = (unsigned)ceil_div(n_dst * G, 256);
   EuProfScope ps(c, "gat_fwd", E);
-  if (vec) k_gat_fwd<true><<<blocks, 256, 0, s>>>(h_src, s_dst, s_src, ord.key, ord.perm, src, E, n_dst, heads, head_dim, G, al, out);
-  else k_gat_fwd<false><<<blocks, 256, 0, s>>>(h_src, s_dst, s_src, ord.key, ord.perm, src, E, n_dst, heads, head_dim, G, al, out);
+  if (vec) k_gat_fwd<true, false><<<blocks, 256, 0, s>>>(h_src, s_dst, s_src, ord.key, ord.perm, src, E, n_dst, heads, head_dim, G, al, out);
+  else k_gat_fwd<false, false><<<blocks, 256, 0, s>>>(h_src, s_dst, s_src, ord.key, ord.perm, src, E, n_dst, heads, head_dim, G, al, out);
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -434,6 +566,118 @@ int eu_gat_aggregate_backward(eu_ctx* c, const float* grad_out, const float* h_s
     else k_gat_bwd_src<false><<<(unsigned)ceil_div(n_src * G, 256), 256, 0, s>>>(grad_out, alpha, du, sord.key, sord.perm, dst, E, n_src,
                                                                                 heads, head_dim, G, grad_h_src, grad_s_src);
     EU_LAUNCHED();
+  }
+  return EU_OK;
+}
+
+int eu_agnn_aggregate(eu_ctx* c, const float* x_src, const float* nrm_dst, const float* nrm_src, const float* beta,
+                      const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src, int32_t dim, float* out,
+                      float* alpha, float* cos) {
+  if (!c || dim < 1 || E < 0 || n_dst < 0 || n_src < 0 || (E > 0 && (n_dst == 0 || n_src == 0)) ||
+      (E > 0 && (!x_src || !nrm_dst || !nrm_src || !beta || !dst || !src)) || (n_dst > 0 && !out)) {
+    set_error("eu_agnn_aggregate: bad argument");
+    return EU_ERR_INVALID;
+  }
+  if (E >= ((int64_t)1 << 31) || n_dst >= ((int64_t)1 << 31) || n_src >= ((int64_t)1 << 31)) {
+    set_error("eu_agnn_aggregate: 2^31 or more edges or rows are not supported");
+    return EU_ERR_UNSUPPORTED;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (n_dst == 0) return EU_OK;
+  cudaStream_t s = c->stream;
+  // flag | [logit / exp / alpha scratch when the caller wants no alpha] | [the dst order when dst is unsorted]; sized once
+  // the flag is read (a growth reallocates: nothing but the flag has been written yet)
+  int rc = ctx_misc(c, 256);
+  if (rc) return rc;
+  bool sorted = true;
+  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
+  const size_t o_alpha = 256, o_ord = o_alpha + (alpha ? 0 : a256(4 * (size_t)E));
+  if ((rc = ctx_misc(c, (int64_t)(o_ord + (sorted ? 0 : order_bytes(E, n_dst)))))) return rc;
+  char* m = (char*)c->d_misc;
+  float* al = alpha ? alpha : (float*)(m + o_alpha);
+  GatOrder ord;
+  ord.key = dst;
+  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_ord, &ord))) return rc;
+  if (E > 0) {
+    EuProfScope ps(c, "agnn_cos", E);
+    if ((rc = agnn_dot(c, nrm_dst, nrm_src, dst, src, E, dim, beta, cos, al))) return rc;   // cos and the logits beta * cos
+  }
+  const bool vec = dim % 4 == 0 && gat_aligned16(x_src) && gat_aligned16(out);
+  // a warp per target whatever dim is: the softmax phase walks a segment G edges at a time, so at small dim the
+  // column-phase width (gat_lanes) would make a hub's softmax chains several times longer; the bits do not depend on G
+  const int G = 32;
+  const unsigned blocks = (unsigned)ceil_div(n_dst * G, 256);
+  EuProfScope ps(c, "agnn_fwd", E);
+  if (vec) k_gat_fwd<true, true><<<blocks, 256, 0, s>>>(x_src, nullptr, nullptr, ord.key, ord.perm, src, E, n_dst, 1, dim, G, al, out);
+  else k_gat_fwd<false, true><<<blocks, 256, 0, s>>>(x_src, nullptr, nullptr, ord.key, ord.perm, src, E, n_dst, 1, dim, G, al, out);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+int eu_agnn_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_src, const float* nrm_dst, const float* nrm_src,
+                               const float* beta, const float* alpha, const float* cos, const int32_t* dst, const int32_t* src,
+                               int64_t E, int64_t n_dst, int64_t n_src, int32_t dim, float* grad_x_src, float* grad_nrm_dst,
+                               float* grad_nrm_src, float* grad_beta) {
+  if (!c || dim < 1 || E < 0 || n_dst < 0 || n_src < 0 || (E > 0 && (n_dst == 0 || n_src == 0)) ||
+      (E > 0 && (!grad_out || !x_src || !nrm_dst || !nrm_src || !beta || !alpha || !cos || !dst || !src)) ||
+      (n_dst > 0 && !grad_nrm_dst) || (n_src > 0 && (!grad_x_src || !grad_nrm_src)) || !grad_beta) {
+    set_error("eu_agnn_aggregate_backward: bad argument");
+    return EU_ERR_INVALID;
+  }
+  if (E >= ((int64_t)1 << 31) || n_dst >= ((int64_t)1 << 31) || n_src >= ((int64_t)1 << 31)) {
+    set_error("eu_agnn_aggregate_backward: 2^31 or more edges or rows are not supported");
+    return EU_ERR_UNSUPPORTED;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  cudaStream_t s = c->stream;
+  if (E == 0) {                                        // no edge: every gradient is zero
+    if (n_dst > 0) EU_CUDA(cudaMemsetAsync(grad_nrm_dst, 0, 4 * (size_t)(n_dst * dim), s));
+    if (n_src > 0) {
+      EU_CUDA(cudaMemsetAsync(grad_x_src, 0, 4 * (size_t)(n_src * dim), s));
+      EU_CUDA(cudaMemsetAsync(grad_nrm_src, 0, 4 * (size_t)(n_src * dim), s));
+    }
+    EU_CUDA(cudaMemsetAsync(grad_beta, 0, sizeof(float), s));
+    return EU_OK;
+  }
+  // flag | d_alpha, then beta * du [E] | per-target partials of grad_beta [n_dst] | [the dst order when dst is unsorted] |
+  // the src order; sized once the flag is read
+  int rc = ctx_misc(c, 256);
+  if (rc) return rc;
+  bool sorted = true;
+  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
+  const size_t o_dw = 256, o_part = o_dw + a256(4 * (size_t)E), o_dord = o_part + a256(4 * (size_t)n_dst),
+               o_sord = o_dord + (sorted ? 0 : order_bytes(E, n_dst));
+  if ((rc = ctx_misc(c, (int64_t)(o_sord + order_bytes(E, n_src))))) return rc;
+  char* m = (char*)c->d_misc;
+  float* dw = (float*)(m + o_dw);
+  float* part = (float*)(m + o_part);
+  GatOrder dord, sord;
+  dord.key = dst;
+  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_dord, &dord))) return rc;
+  {
+    EuProfScope ps(c, "agnn_bwd_dalpha", E);
+    if ((rc = agnn_dot(c, grad_out, x_src, dst, src, E, dim, nullptr, dw, nullptr))) return rc;
+  }
+  {
+    const int G = 32;   // lanes over a segment's edges
+    EuProfScope ps(c, "agnn_bwd_dst", E);
+    k_agnn_bwd_dst<<<(unsigned)ceil_div(n_dst * G, 256), 256, 0, s>>>(alpha, cos, beta, dord.key, dord.perm, E, n_dst, G, dw, part);
+    EU_LAUNCHED();
+  }
+  {
+    EuProfScope ps(c, "agnn_bwd_nrm_dst", E);
+    if ((rc = agnn_row_sum(c, nrm_src, dw, dord, src, E, n_dst, dim, grad_nrm_dst))) return rc;
+  }
+  {
+    EuProfScope ps(c, "agnn_bwd_beta", n_dst);
+    k_agnn_sum<<<1, kAgnnSumThreads, 0, s>>>(part, n_dst, grad_beta);
+    EU_LAUNCHED();
+  }
+  if ((rc = order_by(c, src, E, n_src, m + o_sord, &sord))) return rc;
+  {
+    EuProfScope ps(c, "agnn_bwd_src", E);
+    if ((rc = agnn_row_sum(c, grad_out, alpha, sord, dst, E, n_src, dim, grad_x_src))) return rc;
+    if ((rc = agnn_row_sum(c, nrm_dst, dw, sord, dst, E, n_src, dim, grad_nrm_src))) return rc;
   }
   return EU_OK;
 }

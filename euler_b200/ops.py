@@ -815,3 +815,79 @@ def gat_attention_aggregate(h_src, s_dst, s_src, edge_index, size):
         raise EulerError("gat_attention_aggregate: edge_index must be [2, E]")
     dst, src = ei[0].contiguous(), ei[1].contiguous()
     return _GatAggregate.apply(h_src, s_dst, s_src, dst, src, n_dst)
+
+
+def _raw_agnn(x_src, nrm_dst, nrm_src, beta, dst, src, n_dst, with_alpha):
+    """one eu_agnn_aggregate: (out f32[n_dst, dim], alpha f32[E] or None, cos f32[E] or None)"""
+    n_src, dim = x_src.shape
+    E = dst.numel()
+    dev = x_src.device
+    out = torch.empty((n_dst, dim), dtype=torch.float32, device=dev)
+    alpha = torch.empty(E, dtype=torch.float32, device=dev) if with_alpha else None
+    cos = torch.empty(E, dtype=torch.float32, device=dev) if with_alpha else None
+    ctx = _ctx_on_stream()
+    check(_lib.load().eu_agnn_aggregate(ctx._h, x_src.data_ptr(), nrm_dst.data_ptr(), nrm_src.data_ptr(), beta.data_ptr(),
+                                        dst.data_ptr(), src.data_ptr(), E, n_dst, n_src, dim, out.data_ptr(),
+                                        alpha.data_ptr() if with_alpha else None, cos.data_ptr() if with_alpha else None))
+    return out, alpha, cos
+
+
+class _AgnnAggregate(torch.autograd.Function):
+    """eu_agnn_aggregate / eu_agnn_aggregate_backward.  Saves alpha and cos (8 B per edge), never [E, dim] messages."""
+
+    @staticmethod
+    def forward(ctx, x_src, nrm_dst, nrm_src, beta, dst, src, n_dst):
+        want = any(ctx.needs_input_grad[:4])
+        out, alpha, cos = _raw_agnn(x_src, nrm_dst, nrm_src, beta, dst, src, n_dst, want)
+        if want:
+            ctx.save_for_backward(x_src, nrm_dst, nrm_src, beta, dst, src, alpha, cos)
+        ctx.n_dst = n_dst
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        x_src, nrm_dst, nrm_src, beta, dst, src, alpha, cos = ctx.saved_tensors
+        n_src, dim = x_src.shape
+        grad = grad.contiguous()
+        g_x, g_ns = torch.empty_like(x_src), torch.empty_like(nrm_src)
+        g_nd = torch.empty((ctx.n_dst, dim), dtype=torch.float32, device=grad.device)
+        g_beta = torch.empty_like(beta)
+        ec = _ctx_on_stream()
+        check(_lib.load().eu_agnn_aggregate_backward(ec._h, grad.data_ptr(), x_src.data_ptr(), nrm_dst.data_ptr(), nrm_src.data_ptr(),
+                                                     beta.data_ptr(), alpha.data_ptr(), cos.data_ptr(), dst.data_ptr(),
+                                                     src.data_ptr(), dst.numel(), ctx.n_dst, n_src, dim, g_x.data_ptr(),
+                                                     g_nd.data_ptr(), g_ns.data_ptr(), g_beta.data_ptr()))
+        return g_x, g_nd, g_ns, g_beta, None, None, None
+
+
+def agnn_attention_aggregate(x_src, nrm_dst, nrm_src, beta, edge_index, size):
+    """AGNNConv's attention aggregation (agnn_conv.py:32-54 with aggr='add') in one fused device op:
+        x_src f32[n_src, D]     the source rows summed
+        nrm_dst f32[n_dst, D]   the target rows' l2_normalize, nrm_src f32[n_src, D] the source rows' (not required to be
+                                normalized: the op takes them as given)
+        beta                    the trainable scalar, a one-element f32 tensor ([] or [1]), read on the device only
+        edge_index [2, E]       (target, source) per edge; size = (n_dst, n_src)
+    out[i] = sum over edges (i, j) of alpha[e] * x_src[j], alpha = scatter_softmax of beta * <nrm_dst[i], nrm_src[j]> over the
+    edges of each target.  The cosine is summed in this op's fixed order (include/euler_b200.h); given it, for non-decreasing
+    edge_index[0] the result equals, bit for bit, scatter_softmax / scatter_add composed from the ops above.  The backward
+    pass is deterministic.  Synchronises once per call (whether edge_index[0] is sorted); an unsorted one costs a radix sort."""
+    n_dst, n_src = int(size[0]), int(size[1])
+    named = (("x_src", x_src), ("nrm_dst", nrm_dst), ("nrm_src", nrm_src), ("beta", beta))
+    for nm, t in named:
+        if not torch.is_tensor(t) or t.dtype != torch.float32:
+            raise EulerError("agnn_attention_aggregate: %s must be a float32 tensor" % nm)
+    if beta.numel() != 1:
+        raise EulerError("agnn_attention_aggregate: beta must be a scalar (one element); got shape %s" % (tuple(beta.shape),))
+    if any(t.dim() != 2 for t in (x_src, nrm_dst, nrm_src)):
+        raise EulerError("agnn_attention_aggregate: x_src, nrm_dst and nrm_src must be 2-D tensors")
+    dim = x_src.shape[1]
+    if dim < 1 or x_src.shape[0] != n_src or nrm_src.shape != (n_src, dim) or nrm_dst.shape != (n_dst, dim):
+        raise EulerError("agnn_attention_aggregate: need x_src and nrm_src [n_src, D] = [%d, D], nrm_dst [n_dst, D] = [%d, D]; "
+                         "got %s, %s, %s" % (n_src, n_dst, tuple(x_src.shape), tuple(nrm_src.shape), tuple(nrm_dst.shape)))
+    x_src, nrm_dst, nrm_src = _t(x_src, torch.float32), _t(nrm_dst, torch.float32), _t(nrm_src, torch.float32)
+    b = _t(beta, torch.float32).reshape(1)
+    ei = _t(edge_index, torch.int32)
+    if ei.dim() != 2 or ei.shape[0] != 2:
+        raise EulerError("agnn_attention_aggregate: edge_index must be [2, E]")
+    dst, src = ei[0].contiguous(), ei[1].contiguous()
+    return _AgnnAggregate.apply(x_src, nrm_dst, nrm_src, b, dst, src, n_dst)

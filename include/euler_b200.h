@@ -415,6 +415,40 @@ int eu_gat_aggregate(eu_ctx* c, const float* h_src, const float* s_dst, const fl
 int eu_gat_aggregate_backward(eu_ctx* c, const float* grad_out, const float* h_src, const float* alpha, const float* s_dst,
                               const float* s_src, const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src,
                               int32_t heads, int32_t head_dim, float* grad_h_src, float* grad_s_dst, float* grad_s_src);
+/* AGNNConv's cosine-attention aggregation (tf_euler/python/convolution/agnn_conv.py:32-54, aggr = 'add'), fused.
+ * Inputs x_src f32[n_src, dim] (the rows summed), nrm_dst f32[n_dst, dim] and nrm_src f32[n_src, dim] (the l2-normalized
+ * target and source rows; the op does not require them to be normalized), beta f32[1] (a device pointer: the trainable
+ * scalar is never read on the host), dst / src i32[E] (edge_index[0] / [1]):
+ *   cos[e]   = <nrm_dst[dst_e], nrm_src[src_e]>   (fixed order: lane l of a power-of-two group G = min(32, pow2 >=
+ *              ceil(dim/4)) accumulates its 4-column chunks l, l + G, ... left to right with one fused multiply-add per
+ *              column, then a butterfly over the lanes at xor distances G/2 .. 1; the same on every path)
+ *   u[e]     = beta * cos[e]                      (one rounded multiply)
+ *   alpha[e] = scatter_softmax(u, dst, n_dst)     (running max from -1e9, as scatter_max: a target whose logits are all
+ *                                                  below -1e9 gets NaN alphas)
+ *   out[i]   = sum over the edges e with dst_e = i of alpha[e] * x_src[src_e]
+ * out f32[n_dst, dim] (a target without edges gets a zero row); alpha f32[E] and cos f32[E] may each be NULL (not written).
+ * Given u, the softmax and the sum are those of eu_gat_aggregate with one head: for non-decreasing dst, out and alpha equal
+ * bit for bit beta * cos -> scatter_softmax -> multiply -> scatter_add composed from the ops above, fed this op's cos.  Unsorted
+ * dst is ordered by a stable sort first: bit-identical to the call on the stably sorted edge list.
+ * The backward pass takes the forward's alpha and cos and grad_out f32[n_dst, dim], and writes grad_x_src f32[n_src, dim],
+ * grad_nrm_dst f32[n_dst, dim], grad_nrm_src f32[n_src, dim] and grad_beta f32[1] (device):
+ *   d_alpha[e] = <grad_out[dst_e], x_src[src_e]> (the order of cos), du[e] = alpha[e] * (d_alpha[e] - sum_seg alpha * d_alpha),
+ *   grad_nrm_dst[i] = sum_{dst_e = i} (beta * du[e]) * nrm_src[src_e],  grad_nrm_src[j] = sum_{src_e = j} (beta * du[e]) * nrm_dst[dst_e],
+ *   grad_x_src[j]   = sum_{src_e = j} alpha[e] * grad_out[dst_e],      grad_beta = sum_i (sum_{dst_e = i} du[e] * cos[e]);
+ * per-target sums run over the dst order, per-source sums over a stable sort of the edges by src, each in edge order, and
+ * grad_beta adds the per-target sums in a fixed order: deterministic, no atomics.  Rows without edges get zeros.
+ * dim < 1, negative sizes, edges with n_dst or n_src = 0, or a NULL pointer that is needed: EU_ERR_INVALID; 2^31 or more
+ * edges or rows: EU_ERR_UNSUPPORTED.  Indices are not checked (as eu_gather).  Device pointers; both calls synchronise the
+ * stream once to read whether dst is sorted (an unsorted dst costs a radix sort), and they use the ctx scratch: forward
+ * 4 B per edge when alpha is NULL; backward 4 B per edge + 4 B per target + a sort by src (12 B per edge + cub's temporary
+ * storage), and a sort by dst as well when dst is unsorted. */
+int eu_agnn_aggregate(eu_ctx* c, const float* x_src, const float* nrm_dst, const float* nrm_src, const float* beta,
+                      const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src, int32_t dim, float* out,
+                      float* alpha, float* cos);
+int eu_agnn_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_src, const float* nrm_dst, const float* nrm_src,
+                               const float* beta, const float* alpha, const float* cos, const int32_t* dst, const int32_t* src,
+                               int64_t E, int64_t n_dst, int64_t n_src, int32_t dim, float* grad_x_src, float* grad_nrm_dst,
+                               float* grad_nrm_src, float* grad_beta);
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx,
                    int64_t E, float* out);
 int eu_scatter_add_host(eu_ctx* c, const float* updates, int64_t D, const int32_t* idx, int64_t E,
