@@ -6,6 +6,8 @@ with the framework (torch here): they are GEMMs, not part of the sampling / aggr
                                                                       edge_index, gather of x_j and of both norms, scatter_add
   relation_aggregate tf_euler/python/convolution/relation_conv.py:53-70  x_j gathered, transformed by its relation's matrix
                                                                       (unique -> gather -> matmul), scatter_mean to the targets
+  relation_aggregate_fused  the same, fused: rows summed per (target, relation) pair, one matvec per pair
+                                                                      (ops.relation_mean_aggregate)
   sage_aggregate     tf_euler/python/convolution/sage_conv.py:33-38   gather(x, edge_index[1]) -> scatter_mean
   gat_aggregate      tf_euler/python/convolution/gat_conv.py:53-78    per-node attention scores, then the fused softmax-weighted
                                                                       sum over each target's edges (ops.gat_attention_aggregate)
@@ -47,6 +49,14 @@ def relation_aggregate(x, edge_index, size, edge_attr, matrix):
     m = matrix[rel][inv]                                             # [E, dim, fea_dim]
     out = torch.matmul(m, x_j.unsqueeze(-1)).squeeze(-1)
     return ops.scatter_mean(out, idx0, int(size[0]))
+
+
+def relation_aggregate_fused(x, edge_index, size, edge_attr, matrix):
+    """relation_aggregate's signature and result, to rounding, as one fused device op (ops.relation_mean_aggregate): the edges
+    are summed per (target, relation) pair and each pair is transformed once, so no [E, dim, fea_dim] matrix and no [E, dim]
+    message is ever made."""
+    x1 = x if torch.is_tensor(x) else (x[1] if x[1] is not None else x[0])
+    return ops.relation_mean_aggregate(x1, matrix, edge_attr, edge_index, size)
 
 
 def sage_aggregate(x, edge_index, size):

@@ -389,21 +389,15 @@ __global__ void __launch_bounds__(kAgnnSumThreads) k_agnn_sum(const float* __res
 }
 
 static bool gat_aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-static size_t a256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// The order the kernels walk the edges in: by `idx` (int32[E] in [0, n)), stable.
-struct GatOrder {
-  const int32_t* key = nullptr;    // idx itself when it is already non-decreasing
-  const int32_t* perm = nullptr;   // null then
-};
-
+// The order the kernels walk the edges in (GatOrder, internal.h): by `idx` (int32[E] in [0, n)), stable.
 static int sort_bits(int64_t n) {
   int b = 1;
   while (b < 31 && ((int64_t)1 << b) < n) ++b;
   return b;
 }
 
-static size_t order_bytes(int64_t E, int64_t n) {
+size_t order_bytes(int64_t E, int64_t n) {
   size_t t = 0;
   cub::DeviceRadixSort::SortPairs((void*)nullptr, t, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
                                   (int32_t*)nullptr, (int)E, 0, sort_bits(n));
@@ -411,7 +405,7 @@ static size_t order_bytes(int64_t E, int64_t n) {
 }
 
 // Stable order of the edges by idx, in `buf` (order_bytes(E, n) bytes): keys, permutation (edge of each position).
-static int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, GatOrder* o) {
+int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, GatOrder* o) {
   cudaStream_t s = c->stream;
   int32_t* keys = (int32_t*)buf;
   int32_t* perm = (int32_t*)(buf + a256(4 * (size_t)E));
@@ -458,8 +452,8 @@ static int agnn_dot(eu_ctx* c, const float* a, const float* b, const int32_t* ia
 }
 
 // out[r, :] = sum of w[e] * rows[idx_e, :] over the edges of segment r of the order o, in edge order (k_gat_bwd_src, H = 1)
-static int agnn_row_sum(eu_ctx* c, const float* rows, const float* w, const GatOrder& o, const int32_t* idx, int64_t E,
-                        int64_t n, int dim, float* out) {
+int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const GatOrder& o, const int32_t* idx, int64_t E, int64_t n,
+                      int dim, float* out) {
   const bool vec = dim % 4 == 0 && gat_aligned16(rows) && gat_aligned16(out);
   const int G = gat_lanes(dim, vec);
   const unsigned blocks = (unsigned)ceil_div(n * G, 256);
@@ -666,7 +660,7 @@ int eu_agnn_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_
   }
   {
     EuProfScope ps(c, "agnn_bwd_nrm_dst", E);
-    if ((rc = agnn_row_sum(c, nrm_src, dw, dord, src, E, n_dst, dim, grad_nrm_dst))) return rc;
+    if ((rc = segmented_row_sum(c, nrm_src, dw, dord, src, E, n_dst, dim, grad_nrm_dst))) return rc;
   }
   {
     EuProfScope ps(c, "agnn_bwd_beta", n_dst);
@@ -676,8 +670,8 @@ int eu_agnn_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_
   if ((rc = order_by(c, src, E, n_src, m + o_sord, &sord))) return rc;
   {
     EuProfScope ps(c, "agnn_bwd_src", E);
-    if ((rc = agnn_row_sum(c, grad_out, alpha, sord, dst, E, n_src, dim, grad_x_src))) return rc;
-    if ((rc = agnn_row_sum(c, nrm_dst, dw, sord, dst, E, n_src, dim, grad_nrm_src))) return rc;
+    if ((rc = segmented_row_sum(c, grad_out, alpha, sord, dst, E, n_src, dim, grad_x_src))) return rc;
+    if ((rc = segmented_row_sum(c, nrm_dst, dw, sord, dst, E, n_src, dim, grad_nrm_src))) return rc;
   }
   return EU_OK;
 }

@@ -181,6 +181,18 @@ int64_t hop_table_slots(int nb, int64_t rows_b);
 int64_t hop_table_cap(int64_t rows_b);   // dedup slots per batch (region stride = cap + 1)
 int ctx_misc(eu_ctx* c, int64_t bytes);
 __global__ void k_check_sorted(const int32_t* __restrict__ idx, int64_t E, int* unsorted);   // mp_ops.cu: *unsorted = 1 if idx decreases
+inline size_t a256(size_t b) { return (b + 255) & ~(size_t)255; }   // scratch offsets: 256-byte aligned
+// gat.cu: the stable edge orders its kernels walk and the segmented row sum over one (shared with relation.cu)
+struct GatOrder {                  // the order of the edges by `idx` (int32[E] in [0, n)), stable
+  const int32_t* key = nullptr;    // idx itself when it is already non-decreasing
+  const int32_t* perm = nullptr;   // null then
+};
+size_t order_bytes(int64_t E, int64_t n);   // the scratch order_by needs
+int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, GatOrder* o);
+// out[r, :] = sum of w[e] * rows[row_e, :] over the edges of segment r of the order o, in edge order (k_gat_bwd_src, H = 1);
+// a segment without edges gets a zero row
+int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const GatOrder& o, const int32_t* row, int64_t E, int64_t n,
+                      int dim, float* out);
 int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
 int ctx_stage(eu_ctx* c, int64_t host_bytes, int64_t dev_bytes);

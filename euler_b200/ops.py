@@ -891,3 +891,74 @@ def agnn_attention_aggregate(x_src, nrm_dst, nrm_src, beta, edge_index, size):
         raise EulerError("agnn_attention_aggregate: edge_index must be [2, E]")
     dst, src = ei[0].contiguous(), ei[1].contiguous()
     return _AgnnAggregate.apply(x_src, nrm_dst, nrm_src, b, dst, src, n_dst)
+
+
+def _raw_relation(x_src, matrix, rel, dst, src, n_dst):
+    """one eu_relation_aggregate: out f32[n_dst, D]"""
+    n_src, F = x_src.shape
+    R, D = matrix.shape[0], matrix.shape[1]
+    out = torch.empty((n_dst, D), dtype=torch.float32, device=x_src.device)
+    ctx = _ctx_on_stream()
+    check(_lib.load().eu_relation_aggregate(ctx._h, x_src.data_ptr(), matrix.data_ptr(), rel.data_ptr(), dst.data_ptr(),
+                                            src.data_ptr(), dst.numel(), n_dst, n_src, R, D, F, out.data_ptr()))
+    return out
+
+
+class _RelationAggregate(torch.autograd.Function):
+    """eu_relation_aggregate / eu_relation_aggregate_backward.  Saves only its inputs: the backward pass finds the pairs and
+    their sums again, never an [E, D] or [E, D, F] tensor."""
+
+    @staticmethod
+    def forward(ctx, x_src, matrix, rel, dst, src, n_dst):
+        out = _raw_relation(x_src, matrix, rel, dst, src, n_dst)
+        if any(ctx.needs_input_grad[:2]):
+            ctx.save_for_backward(x_src, matrix, rel, dst, src)
+        ctx.n_dst = n_dst
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        x_src, matrix, rel, dst, src = ctx.saved_tensors
+        n_src, F = x_src.shape
+        R, D = matrix.shape[0], matrix.shape[1]
+        grad = grad.contiguous()
+        g_x, g_m = torch.empty_like(x_src), torch.empty_like(matrix)
+        ec = _ctx_on_stream()
+        check(_lib.load().eu_relation_aggregate_backward(ec._h, grad.data_ptr(), x_src.data_ptr(), matrix.data_ptr(), rel.data_ptr(),
+                                                         dst.data_ptr(), src.data_ptr(), dst.numel(), ctx.n_dst, n_src, R, D, F,
+                                                         g_x.data_ptr(), g_m.data_ptr()))
+        return g_x, g_m, None, None, None, None
+
+
+def relation_mean_aggregate(x_src, matrix, edge_attr, edge_index, size):
+    """RelationConv's typed mean aggregation (relation_conv.py:53-70 with aggr='mean', up to apply_node) in one fused device op:
+        x_src f32[n_src, F]      the source rows
+        matrix f32[R, D, F]      one transform per relation
+        edge_attr [E]            each edge's relation, in [0, R) (RelationDataFlow's e_id)
+        edge_index [2, E]        (target, source) per edge; size = (n_dst, n_src)
+    out[i] = mean over the edges e of target i of matrix[edge_attr[e]] @ x_src[edge_index[1][e]], with scatter_mean's
+    divisor (count + 1e-7).  The edges are summed per (target, relation) pair before the transform, in this op's fixed order
+    (include/euler_b200.h), so the result differs from the per-edge composition only in rounding; it is deterministic, and
+    unsorted (target, relation) keys give the bits of the stably sorted edge list.  Gradients reach x_src and matrix.
+    Synchronises once per call (twice when the keys are unsorted, which costs a radix sort)."""
+    n_dst, n_src = int(size[0]), int(size[1])
+    for nm, t in (("x_src", x_src), ("matrix", matrix)):
+        if not torch.is_tensor(t) or t.dtype != torch.float32:
+            raise EulerError("relation_mean_aggregate: %s must be a float32 tensor" % nm)
+    if x_src.dim() != 2 or matrix.dim() != 3:
+        raise EulerError("relation_mean_aggregate: need x_src [n_src, F] (2-D) and matrix [R, D, F] (3-D); got %s, %s"
+                         % (tuple(x_src.shape), tuple(matrix.shape)))
+    R, D, F = matrix.shape
+    if R < 1 or D < 1 or F < 1 or x_src.shape != (n_src, F):
+        raise EulerError("relation_mean_aggregate: need x_src [n_src, F] = [%d, %d] and a non-empty matrix [R, D, F]; got %s, %s"
+                         % (n_src, F, tuple(x_src.shape), tuple(matrix.shape)))
+    if not torch.is_tensor(edge_attr) or edge_attr.dtype.is_floating_point or edge_attr.dtype.is_complex:
+        raise EulerError("relation_mean_aggregate: edge_attr must be an integer tensor")
+    ei = _t(edge_index, torch.int32)
+    if ei.dim() != 2 or ei.shape[0] != 2:
+        raise EulerError("relation_mean_aggregate: edge_index must be [2, E]")
+    if edge_attr.numel() != ei.shape[1]:
+        raise EulerError("relation_mean_aggregate: edge_attr has %d entries for %d edges" % (edge_attr.numel(), ei.shape[1]))
+    rel = _t(edge_attr, torch.int32).reshape(-1)
+    dst, src = ei[0].contiguous(), ei[1].contiguous()
+    return _RelationAggregate.apply(_t(x_src, torch.float32), _t(matrix, torch.float32), rel, dst, src, n_dst)

@@ -449,6 +449,40 @@ int eu_agnn_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_
                                const float* beta, const float* alpha, const float* cos, const int32_t* dst, const int32_t* src,
                                int64_t E, int64_t n_dst, int64_t n_src, int32_t dim, float* grad_x_src, float* grad_nrm_dst,
                                float* grad_nrm_src, float* grad_beta);
+/* RelationConv's typed mean aggregation (tf_euler/python/convolution/relation_conv.py:53-70, aggr = 'mean', up to
+ * apply_node), fused.  R = num_relations, D = dim, F = fea_dim; inputs x_src f32[n_src, F], matrix f32[R, D, F],
+ * rel i32[E] (each edge's relation, edge_attr upstream), dst / src i32[E] (edge_index[0] / [1]):
+ *   out[i] = (sum over the edges e with dst_e = i of matrix[rel_e] . x_src[src_e]) / fl(cnt_i + 1e-7)
+ * out f32[n_dst, D]; the divisor is scatter_mean's (the f32 edge count plus 1e-7f, one rounded division), so a target without
+ * edges gets a zero row.  The edges are summed by pair p = (target, relation) before the transform, which runs once per pair:
+ *   S_p = sum over the edges of p of x_src[src_e]   (fixed order: the pair's edges in key order, in chunks of 256 counted from
+ *                                                    its first edge, each chunk left to right from +0, then the chunk sums in
+ *                                                    chunk order)
+ *   out[i, d] = (one fused multiply-add chain over the pairs of i in key order and f ascending of matrix[r_p, d, f] * S_p[f])
+ *               / fl(cnt_i + 1e-7)
+ * so the result differs from a per-edge matvec only in rounding (it is equal on inputs whose sums are exact).  Keys (dst, rel)
+ * that are non-decreasing (as RelationDataFlow lists them) are walked as given; otherwise a stable radix sort on
+ * dst * R + rel orders the edges first: the result is bit-identical to the call on the stably sorted edge list.
+ * The backward pass takes grad_out f32[n_dst, D] and writes grad_x_src f32[n_src, F] and grad_matrix f32[R, D, F]; rel gets
+ * no gradient.  With gm_i = grad_out[i] / fl(cnt_i + 1e-7):
+ *   gS_p = matrix[r_p]^T . gm_i(p) (a chain over d ascending),  grad_x_src[j] = sum over the edges e with src_e = j of gS_pair(e)
+ *   (a stable sort of the edges by src, each source's edges in order),  grad_matrix[r] = sum over the pairs p with r_p = r of
+ *   gm_i(p) (x) S_p (the pairs in stable relation order, chunks of 256 pairs, the chunk sums in chunk order).
+ * Deterministic, no atomics; sources and relations without edges get zeros.
+ * num_relations, dim or fea_dim < 1, negative sizes, edges with n_dst or n_src = 0, a NULL pointer that is needed, or a
+ * relation outside [0, R): EU_ERR_INVALID (the relations are checked in the pass that checks the order: a bad one would read
+ * outside matrix).  2^31 or more edges, rows or matrix entries: EU_ERR_UNSUPPORTED.  dst and src are not checked (as eu_gather).
+ * Device pointers; each call synchronises the stream once to read the order flags and P (the number of pairs), twice when
+ * the keys are unsorted, and uses the ctx scratch: O(E) index data (8 B per edge; the backward adds 8 B per edge and a sort
+ * by src of 12 B per edge plus cub's temporary storage; unsorted keys add a sort of 24 B per edge plus cub's) plus
+ * O(P * (F + D)) floats, (P + E / 256) * F floats of chunk sums, and for grad_matrix one D x F block per 256 pairs of a
+ * relation; never O(E * D). */
+int eu_relation_aggregate(eu_ctx* c, const float* x_src, const float* matrix, const int32_t* rel, const int32_t* dst,
+                          const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src, int32_t num_relations, int32_t dim,
+                          int32_t fea_dim, float* out);
+int eu_relation_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_src, const float* matrix, const int32_t* rel,
+                                   const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src,
+                                   int32_t num_relations, int32_t dim, int32_t fea_dim, float* grad_x_src, float* grad_matrix);
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx,
                    int64_t E, float* out);
 int eu_scatter_add_host(eu_ctx* c, const float* updates, int64_t D, const int32_t* idx, int64_t E,
