@@ -125,6 +125,8 @@ SIGNATURES = {
     "eu_agnn_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _P, _P, _P, _P]),
     "eu_relation_aggregate": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _I32, _P]),
     "eu_relation_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _I32, _P, _P]),
+    "eu_dna_aggregate": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P]),
+    "eu_dna_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P, _P]),
     "eu_gather_host": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P]),
     "eu_scatter_add_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),
     "eu_scatter_max_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),

@@ -13,6 +13,10 @@ with the framework (torch here): they are GEMMs, not part of the sampling / aggr
                                                                       sum over each target's edges (ops.gat_attention_aggregate)
   agnn_aggregate     tf_euler/python/convolution/agnn_conv.py:32-54   l2_normalize in torch, then the fused cosine logits,
                                                                       softmax and weighted sum (ops.agnn_attention_aggregate)
+  group_dense        tf_euler/python/convolution/dna_conv.py:27-69    GroupDense: a block-diagonal matmul plus bias
+  dna_aggregate      tf_euler/python/convolution/dna_conv.py:115-170  lin_q / lin_k / lin_v per node, gcn_norm, then the fused
+                                                                      head-by-head attention and scatter_mean
+                                                                      (ops.dna_attention_aggregate)
 """
 import torch
 
@@ -110,3 +114,52 @@ def agnn_aggregate(x, edge_index, size, beta):
     n1 = l2_normalize(x1)
     n0 = n1 if x0 is x1 else l2_normalize(x0)
     return ops.agnn_attention_aggregate(x1, n0, n1, beta, edge_index, size)
+
+
+def group_dense(x, kernel, bias=None):
+    """GroupDense.call (dna_conv.py:50-69) without activation: kernel [G, in/G, out/G] is a block-diagonal matmul, group g
+    mapping input columns [g*in/G, (g+1)*in/G) to output columns [g*out/G, (g+1)*out/G); bias [out] is added when given.
+    G = 1 is a plain dense layer with kernel[0] (upstream's G = 1 branch reshapes the list [kernel, bias] and fails with a
+    bias; DESIGN section 4)."""
+    if not torch.is_tensor(x) or not torch.is_tensor(kernel) or x.dtype != torch.float32 or kernel.dtype != torch.float32:
+        raise EulerError("group_dense: x and kernel must be float32 tensors")
+    if kernel.dim() != 3 or x.dim() < 1:
+        raise EulerError("group_dense: kernel must be [groups, in/groups, out/groups]; got %s" % (tuple(kernel.shape),))
+    G, fi, fo = kernel.shape
+    if G < 1 or x.shape[-1] != G * fi:
+        raise EulerError("group_dense: x's width %d is not groups * in/groups = %d * %d" % (x.shape[-1], G, fi))
+    if bias is not None and (not torch.is_tensor(bias) or bias.dtype != torch.float32 or bias.shape != (G * fo,)):
+        raise EulerError("group_dense: bias must be a float32 [%d] tensor" % (G * fo))
+    lead = x.shape[:-1]
+    if G == 1:
+        out = x.reshape(-1, fi) @ kernel[0]
+    else:
+        out = torch.matmul(x.reshape(-1, G, fi).transpose(0, 1), kernel).transpose(0, 1).reshape(-1, G * fo)
+    if bias is not None:
+        out = out + bias
+    return out.reshape(*lead, G * fo)
+
+
+def dna_aggregate(x, edge_index, size, lin_q, lin_k, lin_v, heads):
+    """DNAConv.__call__ after in_fc (dna_conv.py:149-170): x = (x_target, x_source), both already through in_fc, x_source
+    None meaning x_target; lin_q, lin_k and lin_v are (kernel, bias) pairs of GroupDense layers (bias may be None).  The
+    linear maps act on each row, so they run here once per node (q on the targets, k and v on the sources) instead of once
+    per edge; then gcn_norm and the fused attention, norm product and scatter_mean (ops.dna_attention_aggregate).
+    apply_node is the identity."""
+    if torch.is_tensor(x) or not isinstance(x, (tuple, list)) or len(x) != 2 or x[0] is None:
+        raise EulerError("dna_aggregate: x must be (x_target, x_source): the queries read the targets")
+    x0, x1 = x[0], x[1] if x[1] is not None else x[0]
+    pairs = (("lin_q", lin_q), ("lin_k", lin_k), ("lin_v", lin_v))
+    for nm, p in pairs:
+        if not isinstance(p, (tuple, list)) or len(p) != 2:
+            raise EulerError("dna_aggregate: %s must be a (kernel, bias) pair" % nm)
+    if any(not torch.is_tensor(t) or t.dim() != 2 for t in (x0, x1)) or x0.shape[1] != x1.shape[1]:
+        raise EulerError("dna_aggregate: x_target and x_source must be 2-D tensors of one width")
+    dim = lin_q[0].shape[0] * lin_q[0].shape[2] if torch.is_tensor(lin_q[0]) and lin_q[0].dim() == 3 else None
+    if dim is None or int(heads) < 1 or dim % int(heads):
+        raise EulerError("dna_aggregate: dim = %s must be a positive multiple of heads = %s" % (dim, heads))
+    q = group_dense(x0, *lin_q)
+    k = group_dense(x1, *lin_k)
+    v = group_dense(x1, *lin_v)
+    n0, n1 = gcn_norm(edge_index, size)
+    return ops.dna_attention_aggregate(q, k, v, n0, n1, edge_index, size, heads)

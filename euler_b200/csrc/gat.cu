@@ -425,7 +425,7 @@ int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, Gat
 }
 
 // Is idx non-decreasing?  One flag read back to the host (a stream synchronisation).
-static int is_sorted(eu_ctx* c, const int32_t* idx, int64_t E, int* flag_dev, bool* sorted) {
+int is_sorted(eu_ctx* c, const int32_t* idx, int64_t E, int* flag_dev, bool* sorted) {
   *sorted = true;
   if (E < 2) return EU_OK;
   cudaStream_t s = c->stream;

@@ -962,3 +962,78 @@ def relation_mean_aggregate(x_src, matrix, edge_attr, edge_index, size):
     rel = _t(edge_attr, torch.int32).reshape(-1)
     dst, src = ei[0].contiguous(), ei[1].contiguous()
     return _RelationAggregate.apply(_t(x_src, torch.float32), _t(matrix, torch.float32), rel, dst, src, n_dst)
+
+
+def _raw_dna(q, k, v, n0, n1, dst, src, n_dst, heads, with_alpha):
+    """one eu_dna_aggregate: (out f32[n_dst, dim], alpha f32[E, H, H] or None)"""
+    n_src, dim = k.shape
+    E = dst.numel()
+    out = torch.empty((n_dst, dim), dtype=torch.float32, device=q.device)
+    alpha = torch.empty((E, heads, heads), dtype=torch.float32, device=q.device) if with_alpha else None
+    ctx = _ctx_on_stream()
+    check(_lib.load().eu_dna_aggregate(ctx._h, q.data_ptr(), k.data_ptr(), v.data_ptr(), n0.data_ptr(), n1.data_ptr(),
+                                       dst.data_ptr(), src.data_ptr(), E, n_dst, n_src, heads, dim // heads, out.data_ptr(),
+                                       alpha.data_ptr() if with_alpha else None))
+    return out, alpha
+
+
+class _DnaAggregate(torch.autograd.Function):
+    """eu_dna_aggregate / eu_dna_aggregate_backward.  Saves its inputs and alpha (4 H^2 B per edge), never [E, dim] messages."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, n0, n1, dst, src, n_dst, heads):
+        want = any(ctx.needs_input_grad[:3])
+        out, alpha = _raw_dna(q, k, v, n0, n1, dst, src, n_dst, heads, want)
+        if want:
+            ctx.save_for_backward(q, k, v, n0, n1, dst, src, alpha)
+        ctx.dims = (n_dst, heads)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        q, k, v, n0, n1, dst, src, alpha = ctx.saved_tensors
+        n_dst, H = ctx.dims
+        n_src, dim = k.shape
+        grad = grad.contiguous()
+        g_q, g_k, g_v = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        ec = _ctx_on_stream()
+        check(_lib.load().eu_dna_aggregate_backward(ec._h, grad.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), n0.data_ptr(),
+                                                    n1.data_ptr(), alpha.data_ptr(), dst.data_ptr(), src.data_ptr(), dst.numel(),
+                                                    n_dst, n_src, H, dim // H, g_q.data_ptr(), g_k.data_ptr(), g_v.data_ptr()))
+        return g_q, g_k, g_v, None, None, None, None, None, None
+
+
+def dna_attention_aggregate(q, k, v, n0, n1, edge_index, size, heads):
+    """DNAConv's attention aggregation (dna_conv.py:115-170 with aggr='mean', after lin_q / lin_k / lin_v) in one fused
+    device op:
+        q f32[n_dst, dim]        lin_q of the target rows; k, v f32[n_src, dim] lin_k / lin_v of the source rows
+        n0 f32[n_dst] or [n_dst, 1], n1 f32[n_src] or [n_src, 1]   the deg^-1/2 norms of both sides (convolution.gcn_norm)
+        edge_index [2, E]        (target, source) per edge; size = (n_dst, n_src); heads H divides dim, at most 8
+    Per edge every query head is scored against every key head (<q_i[h], k_j[h']> / sqrt(C)), restricted_softmax runs over
+    the key heads, and the message n0_i * n1_j * sum_h' a * v_j[h'] is averaged over each target's edges with
+    scatter_mean's divisor.  The sums run in this op's fixed order (include/euler_b200.h): deterministic, and unsorted
+    edge_index[0] gives the bits of the stably sorted edge list.  Gradients reach q, k and v; the norms get none.
+    Synchronises once per call (whether edge_index[0] is sorted); an unsorted one costs a radix sort."""
+    n_dst, n_src = int(size[0]), int(size[1])
+    for nm, t in (("q", q), ("k", k), ("v", v), ("n0", n0), ("n1", n1)):
+        if not torch.is_tensor(t) or t.dtype != torch.float32:
+            raise EulerError("dna_attention_aggregate: %s must be a float32 tensor" % nm)
+    if any(t.dim() != 2 for t in (q, k, v)):
+        raise EulerError("dna_attention_aggregate: q, k and v must be 2-D tensors")
+    heads = int(heads)
+    dim = q.shape[1]
+    if heads < 1 or dim < 1 or dim % heads:
+        raise EulerError("dna_attention_aggregate: dim = %d must be a positive multiple of heads = %d" % (dim, heads))
+    if q.shape[0] != n_dst or k.shape != (n_src, dim) or v.shape != (n_src, dim):
+        raise EulerError("dna_attention_aggregate: need q [n_dst, dim] = [%d, %d], k and v [n_src, dim] = [%d, %d]; got %s, %s, %s"
+                         % (n_dst, dim, n_src, dim, tuple(q.shape), tuple(k.shape), tuple(v.shape)))
+    for nm, t, n in (("n0", n0, n_dst), ("n1", n1, n_src)):
+        if t.numel() != n or t.dim() not in (1, 2) or (t.dim() == 2 and t.shape[1] != 1):
+            raise EulerError("dna_attention_aggregate: %s must be [%d] or [%d, 1]; got %s" % (nm, n, n, tuple(t.shape)))
+    ei = _t(edge_index, torch.int32)
+    if ei.dim() != 2 or ei.shape[0] != 2:
+        raise EulerError("dna_attention_aggregate: edge_index must be [2, E]")
+    dst, src = ei[0].contiguous(), ei[1].contiguous()
+    q, k, v = (_t(t, torch.float32) for t in (q, k, v))
+    n0, n1 = (_t(t, torch.float32).detach().reshape(-1) for t in (n0, n1))
+    return _DnaAggregate.apply(q, k, v, n0, n1, dst, src, n_dst, heads)

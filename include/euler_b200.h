@@ -483,6 +483,43 @@ int eu_relation_aggregate(eu_ctx* c, const float* x_src, const float* matrix, co
 int eu_relation_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_src, const float* matrix, const int32_t* rel,
                                    const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src,
                                    int32_t num_relations, int32_t dim, int32_t fea_dim, float* grad_x_src, float* grad_matrix);
+/* DNAConv's attention aggregation (tf_euler/python/convolution/dna_conv.py:115-170, aggr = 'mean'), fused, after the
+ * per-node linear maps.  H = heads, C = head_dim, dim = H * C; inputs q f32[n_dst, dim] (lin_q(in_fc(x_target))), k and v
+ * f32[n_src, dim] (lin_k / lin_v(in_fc(x_source))), n0 f32[n_dst] and n1 f32[n_src] (gcn_norm's deg^-1/2 of both sides),
+ * dst / src i32[E] (edge_index[0] / [1]).  For edge e = (i, j) = (dst_e, src_e) and heads h, h':
+ *   s[e,h,h']  = <q_i[h], k_j[h']> / sqrtf(C)   (every query head against every key head; the dot in a fixed order: lane l
+ *                of a power-of-two group G = min(32, pow2 >= ceil(C/4)) accumulates its 4-column chunks l, l + G, ... left
+ *                to right with one fused multiply-add per column, then a butterfly over the lanes at xor distances G/2 .. 1,
+ *                as eu_agnn_aggregate's cos; then one rounded division)
+ *   m[e,h]     = max(0, max_h' s[e,h,h'])
+ *   a[e,h,h']  = expf(s - m) / (sum over h'' ascending of expf(s[e,h,h''] - m) + expf(-m))   (restricted_softmax)
+ *   msg[e,h,:] = fl(n0_i * n1_j) * (sum over h' ascending of a[e,h,h'] * v_j[h']: one multiply, then fused multiply-adds)
+ *   out_i      = (sum over the edges of i of msg_e) / fl(fl(cnt_i) + 1e-7f)   (scatter_mean's divisor; no edge: a zero row)
+ * A target's edges are summed in order (dst order; unsorted dst is ordered by a stable sort first, so the result is
+ * bit-identical to the call on the stably sorted edge list) in chunks of 256 counted from its first edge, each chunk left to
+ * right from +0, then the chunk sums in chunk order.  For H = 1 and targets of at most 256 edges, given alpha, out equals
+ * gather -> multiply by alpha -> multiply by the norm product -> scatter_mean composed from the ops above, bit for bit.
+ * out f32[n_dst, dim]; alpha f32[E, H, H] may be NULL (not written).
+ * The backward pass takes the forward's alpha and grad_out f32[n_dst, dim], and writes grad_q f32[n_dst, dim], grad_k and
+ * grad_v f32[n_src, dim]; n0 and n1 get no gradient.  With gm_i = grad_out[i] / fl(cnt_i + 1e-7) and w_e = fl(n0_i * n1_j):
+ *   da = w_e * <gm_i[h], v_j[h']> (the order of s),  t = a * (da - sum_h'' a * da) / sqrtf(C),
+ *   grad_q_i[h] = sum_{dst_e = i} sum_h' t * k_j[h'],  grad_k_j[h'] = sum_{src_e = j} sum_h t * q_i[h],
+ *   grad_v_j[h'] = sum_{src_e = j} w_e * sum_h a * gm_i[h]
+ * each segment sum chunked as the forward's, per-target over the dst order, per-source over a stable sort of the edges by
+ * src: deterministic, no atomics.  Rows without edges get zeros.
+ * heads or head_dim < 1, negative sizes, edges with n_dst or n_src = 0, or a NULL pointer that is needed: EU_ERR_INVALID.
+ * heads > 8 (one edge's scores of a head are held in registers), 2^31 or more edges, rows or dim columns: EU_ERR_UNSUPPORTED.
+ * Indices are not checked (as eu_gather).  Device pointers; both calls synchronise the stream once to read whether dst is
+ * sorted (an unsorted dst costs a radix sort, a sorted one nothing more), and they use the ctx scratch: forward 4 H^2 B per
+ * edge when alpha is NULL, 12 B per target and (n_dst + E / 256) * dim floats of chunk sums; backward n_dst * dim floats,
+ * 4 H^2 B per edge, a sort by src (12 B per edge plus cub's temporary storage) and the chunk sums of both sides; never
+ * O(E * dim). */
+int eu_dna_aggregate(eu_ctx* c, const float* q, const float* k, const float* v, const float* n0, const float* n1, const int32_t* dst,
+                     const int32_t* src, int64_t E, int64_t n_dst, int64_t n_src, int32_t heads, int32_t head_dim, float* out,
+                     float* alpha);
+int eu_dna_aggregate_backward(eu_ctx* c, const float* grad_out, const float* q, const float* k, const float* v, const float* n0,
+                              const float* n1, const float* alpha, const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst,
+                              int64_t n_src, int32_t heads, int32_t head_dim, float* grad_q, float* grad_k, float* grad_v);
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx,
                    int64_t E, float* out);
 int eu_scatter_add_host(eu_ctx* c, const float* updates, int64_t D, const int32_t* idx, int64_t E,
