@@ -21,9 +21,9 @@
 //     chunks l, l + G, ... with one __fmaf_rn per column, then a butterfly at xor distances G/2 .. 1), the same with float4
 //     and scalar loads; then one __fdiv_rn by sqrtf(C), the max, one expf each, the h''-ascending __fadd_rn sum plus
 //     exp(-m), one __fdiv_rn.
-//   - a segment sum (k_dna_chunk_sums): the segment's edges in order, in chunks of kDnaChunk counted from its first edge;
+//   - a segment sum (k_dna_chunk_sums): the segment's edges in order, in chunks of kSegChunk counted from its first edge;
 //     per edge the inner sum over h' ascending (one __fmul_rn, then __fmaf_rn), times the edge weight (one __fmul_rn),
-//     added left to right from +0; the chunk sums added in chunk order (k_rel_combine); the forward then divides once.
+//     added left to right from +0; the chunk sums added in chunk order (k_seg_combine); the forward then divides once.
 // Backward, with gm_i = g_i / fl(cnt_i + 1e-7) and w_e = fl(n0_i * n1_j):
 //   da[e,h,h'] = w_e * <gm_i[h], v_j[h']>,  t = a * (da - sum_h'' a * da) / sqrt(C)          (k_dna_edge<.., true>)
 //   grad_q_i[h]  = sum_{dst_e = i} sum_h' t[e,h,h'] * k_j[h']      (the dst order)
@@ -31,37 +31,16 @@
 //   grad_v_j[h'] = sum_{src_e = j} w_e * sum_h a[e,h,h'] * gm_i[h]
 // each a k_dna_chunk_sums pass.  n0 and n1 get no gradient.
 //
-// Order: unsorted dst (GCNDataFlow with self loops appends the loops) is ordered by gat.cu's stable radix sort after one
+// Order: unsorted dst (GCNDataFlow with self loops appends the loops) is ordered by segment.cu's stable radix sort after one
 // flag read-back; the result is bit-identical to the call on the stably sorted edge list.
-#include <cub/device/device_scan.cuh>
-
-#include <algorithm>
 #include <cmath>
 
-#include "internal.h"
+#include "segment.cuh"
 
 namespace eu {
 
-constexpr int kDnaChunk = 256;    // edges per chunk of a segment sum
 constexpr int kDnaMaxHeads = 8;   // the heads one edge's scores are held for in registers
 constexpr int kDnaUnroll = 4;     // edges in flight per lane in the chunk sums
-
-__device__ __forceinline__ int64_t dna_upper_bound(const int32_t* __restrict__ a, int64_t n, int64_t key) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if ((int64_t)__ldg(a + mid) <= key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-__device__ __forceinline__ int64_t dna_edge_at(const int32_t* __restrict__ perm, int64_t k) { return perm ? (int64_t)__ldg(perm + k) : k; }
-
-__device__ __forceinline__ unsigned dna_group_mask(int G) {
-  if (G == 32) return 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  return ((1u << G) - 1u) << (lane & ~(G - 1));
-}
 
 // <x[0, C), y[0, C)> in k_agnn_dot's order (see the file comment); every lane of the group returns the same bits
 template <bool VEC>
@@ -96,7 +75,7 @@ __global__ void __launch_bounds__(256) k_dna_edge(const float* __restrict__ x, c
   const int64_t e = tid >> (31 - __clz(G));
   const int sub = (int)(tid & (G - 1));
   if (e >= E) return;   // group-uniform
-  const unsigned gm = dna_group_mask(G);
+  const unsigned gm = group_mask(G);
   const int64_t HC = (int64_t)H * C;
   const int64_t i = __ldg(dst + e), j = __ldg(src + e);
   const float* xr = x + i * HC;
@@ -149,11 +128,11 @@ __global__ void __launch_bounds__(256) k_dna_edge(const float* __restrict__ x, c
 }
 
 // G lanes per chunk c of the segments of an edge order (positions key-sorted, perm: position -> edge, null = identity).
-// Chunk c - chunk_off[p] of segment p covers the positions [start[p] + (c - chunk_off[p]) * kDnaChunk, ...), up to
-// kDnaChunk of them.  For output head h and column c of the head, summed left to right from +0:
+// Chunk c - chunk_off[p] of segment p covers the positions [start[p] + (c - chunk_off[p]) * kSegChunk, ...), up to
+// kSegChunk of them.  For output head h and column c of the head, summed left to right from +0:
 //   sum over those edges of w_e * (sum over h' ascending of coef[e, h, h'] * rows[ridx_e, h' * C + c])
 // (TRANS: coef[e, h', h]; w_e = fl(n0[dst_e] * n1[src_e]) when n0 is given, else no multiply).  A segment of one chunk
-// writes seg[p]; the chunks of a longer one write partial[c] for k_rel_combine.  VEC: C % 4 == 0, 16-byte aligned rows.
+// writes seg[p]; the chunks of a longer one write partial[c] for k_seg_combine.  VEC: C % 4 == 0, 16-byte aligned rows.
 template <bool VEC, bool TRANS>
 __global__ void __launch_bounds__(256) k_dna_chunk_sums(const float* __restrict__ rows, const int32_t* __restrict__ ridx,
                                                         const float* __restrict__ coef, const float* __restrict__ n0,
@@ -166,10 +145,10 @@ __global__ void __launch_bounds__(256) k_dna_chunk_sums(const float* __restrict_
   const int64_t c = tid >> (31 - __clz(G));
   const int sub = (int)(tid & (G - 1));
   if (c >= slots || c >= __ldg(chunk_off + n)) return;
-  const int64_t p = dna_upper_bound(chunk_off, n + 1, c) - 1;
+  const int64_t p = key_upper_bound(chunk_off, n + 1, c) - 1;
   const int64_t c0 = __ldg(chunk_off + p), nch = __ldg(chunk_off + p + 1) - c0;
-  const int64_t b = __ldg(start + p) + (c - c0) * kDnaChunk;
-  const int64_t e = min(b + kDnaChunk, (int64_t)__ldg(start + p + 1));
+  const int64_t b = __ldg(start + p) + (c - c0) * kSegChunk;
+  const int64_t e = min(b + kSegChunk, (int64_t)__ldg(start + p + 1));
   const int HC = H * C;   // < 2^31: checked by the launcher
   const int64_t HH = (int64_t)H * H;
   float* o = nch == 1 ? seg + p * HC : partial + c * HC;
@@ -184,7 +163,7 @@ __global__ void __launch_bounds__(256) k_dna_chunk_sums(const float* __restrict_
         float4 in[kDnaUnroll];
 #pragma unroll
         for (int q = 0; q < kDnaUnroll; ++q) {
-          ed[q] = k0 + q < e ? dna_edge_at(perm, k0 + q) : 0;
+          ed[q] = k0 + q < e ? edge_at(perm, k0 + q) : 0;
           r[q] = rows + (int64_t)__ldg(ridx + ed[q]) * HC + cc;
         }
         for (int hp = 0; hp < H; ++hp) {
@@ -233,7 +212,7 @@ __global__ void __launch_bounds__(256) k_dna_chunk_sums(const float* __restrict_
         float in[kDnaUnroll];
 #pragma unroll
         for (int q = 0; q < kDnaUnroll; ++q) {
-          ed[q] = k0 + q < e ? dna_edge_at(perm, k0 + q) : 0;
+          ed[q] = k0 + q < e ? edge_at(perm, k0 + q) : 0;
           r[q] = rows + (int64_t)__ldg(ridx + ed[q]) * HC + cc;
         }
         for (int hp = 0; hp < H; ++hp) {
@@ -272,62 +251,14 @@ __global__ void k_dna_mean(const float* __restrict__ g, const int32_t* __restric
   v[t] = __fdiv_rn(g ? __ldg(g + t) : v[t], den);
 }
 
-static bool dna_aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-
-static int dna_lanes(int64_t n) {   // a power of two >= n, at most 32
-  int g = 1;
-  while (g < 32 && g < n) g <<= 1;
-  return g;
-}
-
-// The segments of one edge order, in the scratch at `buf` (seg_bytes(E, n)): start [n + 1] | nc [n + 1] | chunk_off [n + 1] |
-// scan temp | partial chunk sums [n + E / kDnaChunk, dim]
-struct DnaSegs {
-  int64_t n = 0, slots = 0;
-  int32_t *start = nullptr, *chunk_off = nullptr;
-  float* partial = nullptr;
-};
-
-static size_t dna_scan_bytes(int64_t n) {
-  size_t t = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, t, (const int32_t*)nullptr, (int32_t*)nullptr, (int)(n + 1));
-  return t;
-}
-
-static size_t seg_bytes(int64_t E, int64_t n, int64_t dim) {
-  return 3 * a256(4 * (size_t)(n + 1)) + a256(dna_scan_bytes(n)) + a256(4 * (size_t)(n + E / kDnaChunk) * dim);
-}
-
-// The segment starts and chunk offsets of the order o over n segments (E > 0)
-static int dna_segments(eu_ctx* c, const GatOrder& o, int64_t E, int64_t n, int64_t dim, char* buf, DnaSegs* S) {
-  cudaStream_t s = c->stream;
-  const size_t n1 = a256(4 * (size_t)(n + 1)), scan = dna_scan_bytes(n);
-  S->n = n;
-  S->slots = n + E / kDnaChunk;   // >= the chunks: sum over segments of ceil(len / K) <= n + E / K
-  S->start = (int32_t*)buf;
-  int32_t* nc = (int32_t*)(buf + n1);
-  S->chunk_off = (int32_t*)(buf + 2 * n1);
-  void* tmp = buf + 3 * n1;
-  S->partial = (float*)(buf + 3 * n1 + a256(scan));
-  const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n + 1, 256), kSMs * 8));
-  k_rel_starts<<<grid, 256, 0, s>>>(o.key, E, n, S->start);
-  EU_LAUNCHED();
-  k_rel_seg_chunks<<<grid, 256, 0, s>>>(S->start, n, kDnaChunk, nc);
-  EU_LAUNCHED();
-  size_t t = scan;
-  EU_CUDA(cub::DeviceScan::ExclusiveSum(tmp, t, nc, S->chunk_off, (int)(n + 1), s));
-  EU_LAUNCHED();
-  return EU_OK;
-}
-
 // seg[p] = the weighted segment sums of k_dna_chunk_sums over the segments S of the order o (E > 0), chunks combined
-static int dna_seg_sums(eu_ctx* c, const DnaSegs& S, const GatOrder& o, const float* rows, const int32_t* ridx, const float* coef,
+static int dna_seg_sums(eu_ctx* c, const SegPlan& S, const EdgeOrder& o, const float* rows, const int32_t* ridx, const float* coef,
                         bool trans, const float* n0, const float* n1, const int32_t* dst, const int32_t* src, int H, int C,
                         float* seg) {
   cudaStream_t s = c->stream;
   const int64_t HC = (int64_t)H * C;
-  const bool vec = C % 4 == 0 && dna_aligned16(rows) && dna_aligned16(seg);
-  const int G = dna_lanes(vec ? HC / 4 : HC);
+  const bool vec = C % 4 == 0 && aligned16(rows) && aligned16(seg);
+  const int G = group_lanes(vec ? HC / 4 : HC);
   const unsigned blocks = (unsigned)ceil_div(S.slots * G, 256);
 #define EU_DNA_SUMS(V, T)                                                                                                   \
   k_dna_chunk_sums<V, T><<<blocks, 256, 0, s>>>(rows, ridx, coef, n0, n1, dst, src, o.perm, S.start, S.chunk_off, S.n, S.slots, \
@@ -336,7 +267,7 @@ static int dna_seg_sums(eu_ctx* c, const DnaSegs& S, const GatOrder& o, const fl
   else { if (trans) EU_DNA_SUMS(false, true); else EU_DNA_SUMS(false, false); }
 #undef EU_DNA_SUMS
   EU_LAUNCHED();
-  k_rel_combine<<<(unsigned)ceil_div(S.n * HC, 256), 256, 0, s>>>(S.chunk_off, S.partial, S.n, (int)HC, seg);
+  k_seg_combine<<<(unsigned)ceil_div(S.n * HC, 256), 256, 0, s>>>(S.chunk_off, S.partial, S.n, (int)HC, seg);
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -345,8 +276,8 @@ static int dna_seg_sums(eu_ctx* c, const DnaSegs& S, const GatOrder& o, const fl
 template <bool BWD>
 static int dna_edge(eu_ctx* c, const float* x, const float* y, const float* n0, const float* n1, const int32_t* dst,
                     const int32_t* src, int64_t E, int H, int C, const float* alpha_in, float* res) {
-  const bool vec = C % 4 == 0 && dna_aligned16(x) && dna_aligned16(y);
-  const int G = dna_lanes(ceil_div(C, 4));   // one lane per 4-column chunk, both paths: the same order
+  const bool vec = C % 4 == 0 && aligned16(x) && aligned16(y);
+  const int G = group_lanes(ceil_div(C, 4));   // one lane per 4-column chunk, both paths: the same order
   const unsigned blocks = (unsigned)ceil_div(E * G, 256);
   const float sc = sqrtf((float)C);
   if (vec) k_dna_edge<true, BWD><<<blocks, 256, 0, c->stream>>>(x, y, n0, n1, dst, src, E, H, C, G, sc, alpha_in, res);
@@ -393,29 +324,19 @@ int eu_dna_aggregate(eu_ctx* c, const float* q, const float* k, const float* v, 
     EU_CUDA(cudaMemsetAsync(out, 0, 4 * (size_t)(n_dst * HC), s));
     return EU_OK;
   }
-  // flag | [alpha scratch when the caller wants none] | [the dst order when dst is unsorted] | the target segments; sized
-  // once the flag is read (a growth reallocates: nothing but the flag has been written yet)
-  if ((rc = ctx_misc(c, 256))) return rc;
-  bool sorted = true;
-  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
-  const size_t o_alpha = 256, o_ord = o_alpha + (alpha ? 0 : a256(4 * (size_t)(E * H * H))),
-               o_seg = o_ord + (sorted ? 0 : order_bytes(E, n_dst));
-  if ((rc = ctx_misc(c, (int64_t)(o_seg + seg_bytes(E, n_dst, HC))))) return rc;
-  char* m = (char*)c->d_misc;
-  float* al = alpha ? alpha : (float*)(m + o_alpha);
-  GatOrder ord;
-  ord.key = dst;
-  if (!sorted) {
-    EuProfScope ps(c, "dna_sort", E);
-    if ((rc = order_by(c, dst, E, n_dst, m + o_ord, &ord))) return rc;
-  }
+  // head: alpha scratch when the caller wants none; tail: the target segments
+  TargetOrder to;
+  if ((rc = order_targets(c, dst, E, n_dst, alpha ? 0 : a256(4 * (size_t)(E * H * H)), seg_plan_bytes(E, n_dst, HC), "dna_sort", &to)))
+    return rc;
+  const EdgeOrder& ord = to.ord;
+  float* al = alpha ? alpha : (float*)to.head;
   {
     EuProfScope ps(c, "dna_scores", E);
     if ((rc = dna_edge<false>(c, q, k, nullptr, nullptr, dst, src, E, (int)H, (int)C, nullptr, al))) return rc;
   }
   EuProfScope ps(c, "dna_sums", E);
-  DnaSegs S;
-  if ((rc = dna_segments(c, ord, E, n_dst, HC, m + o_seg, &S))) return rc;
+  SegPlan S;
+  if ((rc = plan_segments(c, ord, E, n_dst, to.tail, &S))) return rc;
   if ((rc = dna_seg_sums(c, S, ord, v, src, al, false, n0, n1, dst, src, (int)H, (int)C, out))) return rc;
   k_dna_mean<<<(unsigned)ceil_div(n_dst * HC, 256), 256, 0, s>>>(nullptr, S.start, n_dst, (int)HC, out);
   EU_LAUNCHED();
@@ -445,28 +366,20 @@ int eu_dna_aggregate_backward(eu_ctx* c, const float* grad_out, const float* q, 
     }
     return EU_OK;
   }
-  // flag | gm [n_dst, dim] | t [E, H, H] | [the dst order when dst is unsorted] | the src order | the target segments |
-  // the source segments; sized once the flag is read
-  if ((rc = ctx_misc(c, 256))) return rc;
-  bool sorted = true;
-  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
-  const size_t o_gm = 256, o_t = o_gm + a256(4 * (size_t)(n_dst * HC)), o_dord = o_t + a256(4 * (size_t)(E * H * H)),
-               o_sord = o_dord + (sorted ? 0 : order_bytes(E, n_dst)), o_dseg = o_sord + order_bytes(E, n_src),
-               o_sseg = o_dseg + seg_bytes(E, n_dst, HC);
-  if ((rc = ctx_misc(c, (int64_t)(o_sseg + seg_bytes(E, n_src, HC))))) return rc;
-  char* m = (char*)c->d_misc;
-  float* gm = (float*)(m + o_gm);
-  float* t = (float*)(m + o_t);
-  GatOrder dord, sord;
-  dord.key = dst;
-  if (!sorted) {
-    EuProfScope ps(c, "dna_sort", E);
-    if ((rc = order_by(c, dst, E, n_dst, m + o_dord, &dord))) return rc;
-  }
-  DnaSegs SD, SS;
+  // head: gm [n_dst, dim] | t [E, H, H]; tail: the src order | the target segments | the source segments
+  const size_t o_dseg = order_bytes(E, n_src), o_sseg = o_dseg + seg_plan_bytes(E, n_dst, HC);
+  TargetOrder to;
+  if ((rc = order_targets(c, dst, E, n_dst, a256(4 * (size_t)(n_dst * HC)) + a256(4 * (size_t)(E * H * H)),
+                          o_sseg + seg_plan_bytes(E, n_src, HC), "dna_sort", &to)))
+    return rc;
+  float* gm = (float*)to.head;
+  float* t = (float*)(to.head + a256(4 * (size_t)(n_dst * HC)));
+  const EdgeOrder& dord = to.ord;
+  EdgeOrder sord;
+  SegPlan SD, SS;
   {
     EuProfScope ps(c, "dna_bwd_scores", E);
-    if ((rc = dna_segments(c, dord, E, n_dst, HC, m + o_dseg, &SD))) return rc;
+    if ((rc = plan_segments(c, dord, E, n_dst, to.tail + o_dseg, &SD))) return rc;
     k_dna_mean<<<(unsigned)ceil_div(n_dst * HC, 256), 256, 0, s>>>(grad_out, SD.start, n_dst, (int)HC, gm);
     EU_LAUNCHED();
     if ((rc = dna_edge<true>(c, gm, v, n0, n1, dst, src, E, (int)H, (int)C, alpha, t))) return rc;
@@ -477,8 +390,8 @@ int eu_dna_aggregate_backward(eu_ctx* c, const float* grad_out, const float* q, 
   }
   {
     EuProfScope ps(c, "dna_bwd_sort_src", E);
-    if ((rc = order_by(c, src, E, n_src, m + o_sord, &sord))) return rc;
-    if ((rc = dna_segments(c, sord, E, n_src, HC, m + o_sseg, &SS))) return rc;
+    if ((rc = order_by(c, src, E, n_src, to.tail, &sord))) return rc;
+    if ((rc = plan_segments(c, sord, E, n_src, to.tail + o_sseg, &SS))) return rc;
   }
   {
     EuProfScope ps(c, "dna_bwd_kv", E);

@@ -23,46 +23,11 @@
 // cosine logit per edge, u[e] = beta * <nrm_dst[dst_e], nrm_src[src_e]>, computed edge-parallel first (k_agnn_dot) and read
 // by k_gat_fwd<VEC, true>.  Its backward reuses k_agnn_dot (d_alpha), k_gat_bwd_src (every segmented row sum, by target and
 // by source) and the orders above; see eu_agnn_aggregate_backward.
-#include <cub/device/device_radix_sort.cuh>
-
-#include <algorithm>
-
-#include "internal.h"
+#include "segment.cuh"
 
 namespace eu {
 
-// lanes per row: 4 columns per lane with float4, 1 otherwise; a power of two <= 32
-static inline int gat_lanes(int64_t hc, bool vec) {
-  const int64_t v = vec ? hc / 4 : hc;
-  int g = 1;
-  while (g < 32 && g < v) g <<= 1;
-  return g;
-}
-
-__device__ __forceinline__ int64_t gat_lower_bound(const int32_t* __restrict__ a, int64_t n, int64_t key) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if ((int64_t)__ldg(a + mid) < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-// the mask of the G-lane group this lane belongs to (G a power of two)
-__device__ __forceinline__ unsigned group_mask(int G) {
-  if (G == 32) return 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  return ((1u << G) - 1u) << (lane & ~(G - 1));
-}
-
 __device__ __forceinline__ float leaky(float x) { return x > 0.f ? x : __fmul_rn(x, 0.2f); }
-
-// the edge at position k of the order the kernels walk (sorted by the segment key)
-__device__ __forceinline__ int64_t edge_at(const int32_t* __restrict__ perm, int64_t k) { return perm ? (int64_t)__ldg(perm + k) : k; }
-
-__global__ void k_gat_iota(int32_t* __restrict__ v, int64_t n) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) v[i] = (int32_t)i;
-}
 
 constexpr int kGatUnroll = 8;   // source rows in flight per lane in the ordered column sums
 
@@ -82,7 +47,7 @@ __global__ void __launch_bounds__(256) k_gat_fwd(const float* __restrict__ h_src
   const int sub = (int)(tid & (G - 1));
   if (r >= n_dst) return;   // group-uniform
   const unsigned gm = group_mask(G);
-  const int64_t b = gat_lower_bound(key, E, r), e = gat_lower_bound(key, E, r + 1);
+  const int64_t b = key_lower_bound(key, E, r), e = key_lower_bound(key, E, r + 1);
   const int HC = H * C;   // < 2^31: checked by the launcher
   for (int h = 0; h < H && b < e; ++h) {
     const float sd = PRE ? 0.f : __ldg(s_dst + r * H + h);
@@ -185,7 +150,7 @@ __global__ void __launch_bounds__(256) k_gat_bwd_dst(const float* __restrict__ g
   const int sub = (int)(tid & (G - 1));
   if (r >= n_dst) return;   // group-uniform
   const unsigned gm = group_mask(G);
-  const int64_t b = gat_lower_bound(key, E, r), e = gat_lower_bound(key, E, r + 1);
+  const int64_t b = key_lower_bound(key, E, r), e = key_lower_bound(key, E, r + 1);
   const int HC = H * C;   // < 2^31: checked by the launcher
   for (int h = 0; h < H; ++h) {
     const float* gr = g + r * (int64_t)HC + h * C;
@@ -237,7 +202,7 @@ __global__ void __launch_bounds__(256) k_gat_bwd_src(const float* __restrict__ g
   const int64_t j = tid >> (31 - __clz(G));
   const int sub = (int)(tid & (G - 1));
   if (j >= n_src) return;
-  const int64_t b = gat_lower_bound(skey, E, j), e = gat_lower_bound(skey, E, j + 1);
+  const int64_t b = key_lower_bound(skey, E, j), e = key_lower_bound(skey, E, j + 1);
   const int HC = H * C;   // < 2^31: checked by the launcher
   float* o = grad_h_src + j * (int64_t)HC;
   if (VEC) {
@@ -342,7 +307,7 @@ __global__ void __launch_bounds__(256) k_agnn_bwd_dst(const float* __restrict__ 
   const int sub = (int)(tid & (G - 1));
   if (r >= n_dst) return;   // group-uniform
   const unsigned gm = group_mask(G);
-  const int64_t b = gat_lower_bound(key, E, r), e = gat_lower_bound(key, E, r + 1);
+  const int64_t b = key_lower_bound(key, E, r), e = key_lower_bound(key, E, r + 1);
   float S = 0.f;
   for (int64_t k0 = b; k0 < e; k0 += G) {
     const int64_t k = k0 + sub;
@@ -388,62 +353,11 @@ __global__ void __launch_bounds__(kAgnnSumThreads) k_agnn_sum(const float* __res
   if (threadIdx.x == 0) *out = sh[0];
 }
 
-static bool gat_aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-
-// The order the kernels walk the edges in (GatOrder, internal.h): by `idx` (int32[E] in [0, n)), stable.
-static int sort_bits(int64_t n) {
-  int b = 1;
-  while (b < 31 && ((int64_t)1 << b) < n) ++b;
-  return b;
-}
-
-size_t order_bytes(int64_t E, int64_t n) {
-  size_t t = 0;
-  cub::DeviceRadixSort::SortPairs((void*)nullptr, t, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, (int)E, 0, sort_bits(n));
-  return 3 * a256(4 * (size_t)E) + a256(t);
-}
-
-// Stable order of the edges by idx, in `buf` (order_bytes(E, n) bytes): keys, permutation (edge of each position).
-int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, GatOrder* o) {
-  cudaStream_t s = c->stream;
-  int32_t* keys = (int32_t*)buf;
-  int32_t* perm = (int32_t*)(buf + a256(4 * (size_t)E));
-  int32_t* iota = (int32_t*)(buf + 2 * a256(4 * (size_t)E));
-  void* tmp = buf + 3 * a256(4 * (size_t)E);
-  size_t t = 0;
-  cub::DeviceRadixSort::SortPairs((void*)nullptr, t, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, (int)E, 0, sort_bits(n), s);
-  k_gat_iota<<<(unsigned)std::min<int64_t>(ceil_div(E, 256), kSMs * 8), 256, 0, s>>>(iota, E);
-  EU_LAUNCHED();
-  EU_CUDA(cub::DeviceRadixSort::SortPairs(tmp, t, (const uint32_t*)idx, (uint32_t*)keys, (const int32_t*)iota, perm, (int)E, 0,
-                                          sort_bits(n), s));
-  EU_LAUNCHED();
-  o->key = keys;
-  o->perm = perm;
-  return EU_OK;
-}
-
-// Is idx non-decreasing?  One flag read back to the host (a stream synchronisation).
-int is_sorted(eu_ctx* c, const int32_t* idx, int64_t E, int* flag_dev, bool* sorted) {
-  *sorted = true;
-  if (E < 2) return EU_OK;
-  cudaStream_t s = c->stream;
-  EU_CUDA(cudaMemsetAsync(flag_dev, 0, sizeof(int), s));
-  k_check_sorted<<<(unsigned)ceil_div(E, 256), 256, 0, s>>>(idx, E, flag_dev);
-  EU_LAUNCHED();
-  int h = 0;
-  EU_CUDA(cudaMemcpyAsync(&h, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
-  EU_CUDA(cudaStreamSynchronize(s));
-  *sorted = h == 0;
-  return EU_OK;
-}
-
 // k_agnn_dot over E > 0 edges: dot[e] = <a[ia_e], b[ib_e]>, scaled[e] = beta * dot[e] (either output may be null)
 static int agnn_dot(eu_ctx* c, const float* a, const float* b, const int32_t* ia, const int32_t* ib, int64_t E, int dim,
                     const float* beta, float* dot, float* scaled) {
-  const bool vec = dim % 4 == 0 && gat_aligned16(a) && gat_aligned16(b);
-  const int G = gat_lanes(ceil_div(dim, 4), false);   // one lane per 4-column chunk, both paths: the same order
+  const bool vec = dim % 4 == 0 && aligned16(a) && aligned16(b);
+  const int G = group_lanes(ceil_div(dim, 4));   // one lane per 4-column chunk, both paths: the same order
   const unsigned blocks = (unsigned)ceil_div(E * G, 256);
   if (vec) k_agnn_dot<true><<<blocks, 256, 0, c->stream>>>(a, b, ia, ib, E, dim, G, beta, dot, scaled);
   else k_agnn_dot<false><<<blocks, 256, 0, c->stream>>>(a, b, ia, ib, E, dim, G, beta, dot, scaled);
@@ -452,10 +366,10 @@ static int agnn_dot(eu_ctx* c, const float* a, const float* b, const int32_t* ia
 }
 
 // out[r, :] = sum of w[e] * rows[idx_e, :] over the edges of segment r of the order o, in edge order (k_gat_bwd_src, H = 1)
-int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const GatOrder& o, const int32_t* idx, int64_t E, int64_t n,
+int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const EdgeOrder& o, const int32_t* idx, int64_t E, int64_t n,
                       int dim, float* out) {
-  const bool vec = dim % 4 == 0 && gat_aligned16(rows) && gat_aligned16(out);
-  const int G = gat_lanes(dim, vec);
+  const bool vec = dim % 4 == 0 && aligned16(rows) && aligned16(out);
+  const int G = group_lanes(vec ? dim / 4 : dim);
   const unsigned blocks = (unsigned)ceil_div(n * G, 256);
   if (vec) k_gat_bwd_src<true><<<blocks, 256, 0, c->stream>>>(rows, w, nullptr, o.key, o.perm, idx, E, n, 1, dim, G, out, nullptr);
   else k_gat_bwd_src<false><<<blocks, 256, 0, c->stream>>>(rows, w, nullptr, o.key, o.perm, idx, E, n, 1, dim, G, out, nullptr);
@@ -484,21 +398,14 @@ int eu_gat_aggregate(eu_ctx* c, const float* h_src, const float* s_dst, const fl
   if (n_dst == 0) return EU_OK;
   cudaStream_t s = c->stream;
   const int64_t H = heads, HC = H * head_dim;
-  // flag | [alpha scratch when the caller wants none] | [the dst order when dst is unsorted]; sized once the flag is read, so
-  // a sorted dst holds no sort scratch (a growth reallocates: nothing but the flag has been written yet)
-  int rc = ctx_misc(c, 256);
+  // head: alpha scratch when the caller wants none
+  TargetOrder t;
+  int rc = order_targets(c, dst, E, n_dst, alpha ? 0 : a256(4 * (size_t)(E * H)), 0, nullptr, &t);
   if (rc) return rc;
-  bool sorted = true;
-  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
-  const size_t o_alpha = 256, o_ord = o_alpha + (alpha ? 0 : a256(4 * (size_t)(E * H)));
-  if ((rc = ctx_misc(c, (int64_t)(o_ord + (sorted ? 0 : order_bytes(E, n_dst)))))) return rc;
-  char* m = (char*)c->d_misc;
-  float* al = alpha ? alpha : (float*)(m + o_alpha);
-  GatOrder ord;
-  ord.key = dst;
-  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_ord, &ord))) return rc;
-  const bool vec = HC % 4 == 0 && gat_aligned16(h_src) && gat_aligned16(out);
-  const int G = gat_lanes(HC, vec);
+  const EdgeOrder& ord = t.ord;
+  float* al = alpha ? alpha : (float*)t.head;
+  const bool vec = HC % 4 == 0 && aligned16(h_src) && aligned16(out);
+  const int G = group_lanes(vec ? HC / 4 : HC);
   const unsigned blocks = (unsigned)ceil_div(n_dst * G, 256);
   EuProfScope ps(c, "gat_fwd", E);
   if (vec) k_gat_fwd<true, false><<<blocks, 256, 0, s>>>(h_src, s_dst, s_src, ord.key, ord.perm, src, E, n_dst, heads, head_dim, G, al, out);
@@ -531,18 +438,13 @@ int eu_gat_aggregate_backward(eu_ctx* c, const float* grad_out, const float* h_s
     }
     return EU_OK;
   }
-  // flag | du [E, H] | [the dst order when dst is unsorted] | the src order; sized once the flag is read
-  int rc = ctx_misc(c, 256);
+  // head: du [E, H]; tail: the src order
+  TargetOrder t;
+  int rc = order_targets(c, dst, E, n_dst, a256(4 * (size_t)(E * H)), order_bytes(E, n_src), nullptr, &t);
   if (rc) return rc;
-  bool sorted = true;
-  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
-  const size_t o_du = 256, o_dord = o_du + a256(4 * (size_t)(E * H)), o_sord = o_dord + (sorted ? 0 : order_bytes(E, n_dst));
-  if ((rc = ctx_misc(c, (int64_t)(o_sord + order_bytes(E, n_src))))) return rc;
-  char* m = (char*)c->d_misc;
-  float* du = (float*)(m + o_du);
-  GatOrder dord, sord;
-  dord.key = dst;
-  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_dord, &dord))) return rc;
+  float* du = (float*)t.head;
+  const EdgeOrder& dord = t.ord;
+  EdgeOrder sord;
   {
     const int G = 32;   // lanes over a segment's edges
     EuProfScope ps(c, "gat_bwd_dst", E);
@@ -550,10 +452,10 @@ int eu_gat_aggregate_backward(eu_ctx* c, const float* grad_out, const float* h_s
                                                                     n_dst, heads, head_dim, G, du, grad_s_dst);
     EU_LAUNCHED();
   }
-  if ((rc = order_by(c, src, E, n_src, m + o_sord, &sord))) return rc;
+  if ((rc = order_by(c, src, E, n_src, t.tail, &sord))) return rc;
   {
-    const bool vec = HC % 4 == 0 && gat_aligned16(grad_out) && gat_aligned16(grad_h_src);
-    const int G = gat_lanes(HC, vec);
+    const bool vec = HC % 4 == 0 && aligned16(grad_out) && aligned16(grad_h_src);
+    const int G = group_lanes(vec ? HC / 4 : HC);
     EuProfScope ps(c, "gat_bwd_src", E);
     if (vec) k_gat_bwd_src<true><<<(unsigned)ceil_div(n_src * G, 256), 256, 0, s>>>(grad_out, alpha, du, sord.key, sord.perm, dst, E, n_src,
                                                                                    heads, head_dim, G, grad_h_src, grad_s_src);
@@ -579,26 +481,19 @@ int eu_agnn_aggregate(eu_ctx* c, const float* x_src, const float* nrm_dst, const
   EU_CUDA(cudaSetDevice(c->g->device));
   if (n_dst == 0) return EU_OK;
   cudaStream_t s = c->stream;
-  // flag | [logit / exp / alpha scratch when the caller wants no alpha] | [the dst order when dst is unsorted]; sized once
-  // the flag is read (a growth reallocates: nothing but the flag has been written yet)
-  int rc = ctx_misc(c, 256);
+  // head: logit / exp / alpha scratch when the caller wants no alpha
+  TargetOrder t;
+  int rc = order_targets(c, dst, E, n_dst, alpha ? 0 : a256(4 * (size_t)E), 0, nullptr, &t);
   if (rc) return rc;
-  bool sorted = true;
-  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
-  const size_t o_alpha = 256, o_ord = o_alpha + (alpha ? 0 : a256(4 * (size_t)E));
-  if ((rc = ctx_misc(c, (int64_t)(o_ord + (sorted ? 0 : order_bytes(E, n_dst)))))) return rc;
-  char* m = (char*)c->d_misc;
-  float* al = alpha ? alpha : (float*)(m + o_alpha);
-  GatOrder ord;
-  ord.key = dst;
-  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_ord, &ord))) return rc;
+  const EdgeOrder& ord = t.ord;
+  float* al = alpha ? alpha : (float*)t.head;
   if (E > 0) {
     EuProfScope ps(c, "agnn_cos", E);
     if ((rc = agnn_dot(c, nrm_dst, nrm_src, dst, src, E, dim, beta, cos, al))) return rc;   // cos and the logits beta * cos
   }
-  const bool vec = dim % 4 == 0 && gat_aligned16(x_src) && gat_aligned16(out);
+  const bool vec = dim % 4 == 0 && aligned16(x_src) && aligned16(out);
   // a warp per target whatever dim is: the softmax phase walks a segment G edges at a time, so at small dim the
-  // column-phase width (gat_lanes) would make a hub's softmax chains several times longer; the bits do not depend on G
+  // column-phase width (GAT's group_lanes) would make a hub's softmax chains several times longer; the bits do not depend on G
   const int G = 32;
   const unsigned blocks = (unsigned)ceil_div(n_dst * G, 256);
   EuProfScope ps(c, "agnn_fwd", E);
@@ -633,21 +528,14 @@ int eu_agnn_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_
     EU_CUDA(cudaMemsetAsync(grad_beta, 0, sizeof(float), s));
     return EU_OK;
   }
-  // flag | d_alpha, then beta * du [E] | per-target partials of grad_beta [n_dst] | [the dst order when dst is unsorted] |
-  // the src order; sized once the flag is read
-  int rc = ctx_misc(c, 256);
+  // head: d_alpha, then beta * du [E] | per-target partials of grad_beta [n_dst]; tail: the src order
+  TargetOrder t;
+  int rc = order_targets(c, dst, E, n_dst, a256(4 * (size_t)E) + a256(4 * (size_t)n_dst), order_bytes(E, n_src), nullptr, &t);
   if (rc) return rc;
-  bool sorted = true;
-  if ((rc = is_sorted(c, dst, E, (int*)c->d_misc, &sorted))) return rc;
-  const size_t o_dw = 256, o_part = o_dw + a256(4 * (size_t)E), o_dord = o_part + a256(4 * (size_t)n_dst),
-               o_sord = o_dord + (sorted ? 0 : order_bytes(E, n_dst));
-  if ((rc = ctx_misc(c, (int64_t)(o_sord + order_bytes(E, n_src))))) return rc;
-  char* m = (char*)c->d_misc;
-  float* dw = (float*)(m + o_dw);
-  float* part = (float*)(m + o_part);
-  GatOrder dord, sord;
-  dord.key = dst;
-  if (!sorted && (rc = order_by(c, dst, E, n_dst, m + o_dord, &dord))) return rc;
+  float* dw = (float*)t.head;
+  float* part = (float*)(t.head + a256(4 * (size_t)E));
+  const EdgeOrder& dord = t.ord;
+  EdgeOrder sord;
   {
     EuProfScope ps(c, "agnn_bwd_dalpha", E);
     if ((rc = agnn_dot(c, grad_out, x_src, dst, src, E, dim, nullptr, dw, nullptr))) return rc;
@@ -667,7 +555,7 @@ int eu_agnn_aggregate_backward(eu_ctx* c, const float* grad_out, const float* x_
     k_agnn_sum<<<1, kAgnnSumThreads, 0, s>>>(part, n_dst, grad_beta);
     EU_LAUNCHED();
   }
-  if ((rc = order_by(c, src, E, n_src, m + o_sord, &sord))) return rc;
+  if ((rc = order_by(c, src, E, n_src, t.tail, &sord))) return rc;
   {
     EuProfScope ps(c, "agnn_bwd_src", E);
     if ((rc = segmented_row_sum(c, grad_out, alpha, sord, dst, E, n_src, dim, grad_x_src))) return rc;

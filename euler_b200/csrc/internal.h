@@ -180,26 +180,12 @@ int64_t hop_scratch_rows(int nb, int64_t rows_b);
 int64_t hop_table_slots(int nb, int64_t rows_b);
 int64_t hop_table_cap(int64_t rows_b);   // dedup slots per batch (region stride = cap + 1)
 int ctx_misc(eu_ctx* c, int64_t bytes);
-__global__ void k_check_sorted(const int32_t* __restrict__ idx, int64_t E, int* unsorted);   // mp_ops.cu: *unsorted = 1 if idx decreases
 inline size_t a256(size_t b) { return (b + 255) & ~(size_t)255; }   // scratch offsets: 256-byte aligned
-// gat.cu: the stable edge orders its kernels walk and the segmented row sum over one (shared with relation.cu)
-struct GatOrder {                  // the order of the edges by `idx` (int32[E] in [0, n)), stable
-  const int32_t* key = nullptr;    // idx itself when it is already non-decreasing
-  const int32_t* perm = nullptr;   // null then
-};
-size_t order_bytes(int64_t E, int64_t n);   // the scratch order_by needs
-int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, GatOrder* o);
-// out[r, :] = sum of w[e] * rows[row_e, :] over the edges of segment r of the order o, in edge order (k_gat_bwd_src, H = 1);
-// a segment without edges gets a zero row
-int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const GatOrder& o, const int32_t* row, int64_t E, int64_t n,
+struct EdgeOrder;   // segment.cuh
+// gat.cu (shared with relation.cu): out[r, :] = sum of w[e] * rows[row_e, :] over the edges of segment r of the order o, in
+// edge order (k_gat_bwd_src, H = 1); a segment without edges gets a zero row
+int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const EdgeOrder& o, const int32_t* row, int64_t E, int64_t n,
                       int dim, float* out);
-// gat.cu: *sorted = whether idx (int32[E]) is non-decreasing; one flag read back through flag_dev (a stream synchronisation)
-int is_sorted(eu_ctx* c, const int32_t* idx, int64_t E, int* flag_dev, bool* sorted);
-// relation.cu: the chunk bookkeeping of fixed-order segment sums (shared with dna.cu)
-__global__ void k_rel_starts(const int32_t* __restrict__ key, int64_t P, int64_t R, int32_t* __restrict__ start);   // start[r] = lower_bound(key, r), r in [0, R]
-__global__ void k_rel_seg_chunks(const int32_t* __restrict__ start, int64_t n, int K, int32_t* __restrict__ nc);     // chunks of K per segment
-__global__ void k_rel_combine(const int32_t* __restrict__ chunk_off, const float* __restrict__ partial, int64_t P, int F,
-                              float* __restrict__ S);   // the chunk sums of each segment of several chunks, in chunk order
 int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
 int ctx_stage(eu_ctx* c, int64_t host_bytes, int64_t dev_bytes);

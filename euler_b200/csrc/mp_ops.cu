@@ -19,7 +19,7 @@
 
 #include <algorithm>
 
-#include "internal.h"
+#include "segment.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -27,14 +27,6 @@ namespace eu {
 
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
-
-// lanes per row for a row of D floats moved as float4 (D % 4 == 0): smallest power of two >= D/4, <= 32
-static inline int lanes_per_row(int64_t D) {
-  int64_t v = D / 4;
-  int g = 1;
-  while (g < 32 && g < v) g <<= 1;
-  return g;
-}
 
 // ---------------------------------------------------------------------------- feature fetch
 // out[i, 0:dim] = feat[row(ids[i]), 0:min(feat_dim,dim)], zeros elsewhere / for unknown ids.
@@ -83,20 +75,6 @@ __global__ void __launch_bounds__(256) k_gather(const float* __restrict__ params
 }
 
 // ---------------------------------------------------------------------------- scatter
-__global__ void k_check_sorted(const int32_t* __restrict__ idx, int64_t E, int* unsorted) {
-  int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (e + 1 < E && __ldg(idx + e) > __ldg(idx + e + 1)) *unsorted = 1;
-}
-
-__device__ __forceinline__ int64_t lower_bound_i32(const int32_t* __restrict__ a, int64_t n, int64_t key) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    int64_t mid = (lo + hi) >> 1;
-    if ((int64_t)__ldg(a + mid) < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
 enum { OP_ADD = 0, OP_MAX = 1, OP_MEAN = 2 };
 
 // sorted path: G lanes per OUTPUT row r; edges [lb(r), lb(r+1)) reduced in index order.
@@ -110,7 +88,7 @@ __global__ void __launch_bounds__(256) k_scatter_sorted(const float* __restrict_
   const int64_t r = tid >> (31 - __clz(G));   // G is a power of two
   const int sub = (int)(tid & (G - 1));
   if (r >= size) return;
-  const int64_t b = lower_bound_i32(idx, E, r), e = lower_bound_i32(idx, E, r + 1);
+  const int64_t b = key_lower_bound(idx, E, r), e = key_lower_bound(idx, E, r + 1);
   const float init = OP == OP_MAX ? -1e9f : 0.f;
   const float denom = __fadd_rn((float)(e - b), 1e-7f);
   float* o = out + r * D;
@@ -370,8 +348,6 @@ __global__ void __launch_bounds__(256) k_sage_broadcast(const int32_t* __restric
   for (int64_t q = gtid; q < n; q += nthreads) tab[__ldg(rep_slot + q)] = 0ull;
 }
 
-static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-
 // CTAs per SM of the HBM-bound row movers (0 = one CTA per 8 rows / as many as the rows need).  A capped, persistent grid keeps
 // the copy at HBM speed (a few warps per SM cover the bandwidth-delay product) while the issue-bound sampling kernels of the
 // other lanes stay resident beside it.
@@ -400,7 +376,7 @@ static int scatter(eu_ctx* c, const float* upd, int64_t D, const int32_t* idx, i
   EU_CUDA(cudaMemsetAsync(unsorted, 0, sizeof(int), s));
   if (OP == OP_MEAN) EU_CUDA(cudaMemsetAsync(cnt, 0, sizeof(float) * size, s));
   const bool vec = (D % 4 == 0) && aligned16(upd) && aligned16(out);
-  const int G = vec ? lanes_per_row(D) : (D >= 32 ? 32 : 1);
+  const int G = vec ? group_lanes(D / 4) : (D >= 32 ? 32 : 1);
   const int tb = 256;
   if (E > 1) {
     k_check_sorted<<<(unsigned)ceil_div(E, tb), tb, 0, s>>>(idx, E, unsorted);
@@ -440,7 +416,7 @@ int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid
   const bool have = fid >= 0 && fid < d.n_slots;
   const int32_t soff = have ? d.slot_off[fid] : 0, sdim = have ? d.slot_dim[fid] : 0;
   const bool vec = (dim % 4 == 0) && (d.feat_dim % 4 == 0) && (soff % 4 == 0) && (sdim % 4 == 0) && aligned16(out);
-  const int G = vec ? lanes_per_row(dim) : (dim >= 32 ? 32 : 1);
+  const int G = vec ? group_lanes(dim / 4) : (dim >= 32 ? 32 : 1);
   const unsigned blocks = capped_grid(ceil_div(M * G, 256), "EU_FEATURE_CTAS", 0);
   EuProfScope ps(c, "k_feature", M);
   if (vec) k_feature<true><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
@@ -455,7 +431,7 @@ int eu_gather(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_
   EU_CUDA(cudaSetDevice(c->g->device));
   if (E == 0) return EU_OK;
   const bool vec = (D % 4 == 0) && aligned16(params) && aligned16(out);
-  const int G = vec ? lanes_per_row(D) : (D >= 32 ? 32 : 1);
+  const int G = vec ? group_lanes(D / 4) : (D >= 32 ? 32 : 1);
   const unsigned blocks = (unsigned)ceil_div(E * G, 256);
   if (vec) k_gather<true><<<blocks, 256, 0, c->stream>>>(params, D, idx, E, G, out);
   else k_gather<false><<<blocks, 256, 0, c->stream>>>(params, D, idx, E, G, out);
@@ -510,7 +486,7 @@ static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int
   if (!dedup) return EU_OK;
   { EuProfScope ps(c, "k_sage_broadcast", rows);
     const bool vec = (dim & 3) == 0 && aligned16(out);
-    const int G = vec ? lanes_per_row(dim) : (dim >= 32 ? 32 : 1);
+    const int G = vec ? group_lanes(dim / 4) : (dim >= 32 ? 32 : 1);
     const unsigned bb = capped_grid(ceil_div(rows * G, 256), "EU_SAGE_CTAS", 0);
     if (vec) k_sage_broadcast<true><<<bb, 256, 0, s>>>(c->d_agg_src, rows, dim, G, c->d_agg_slot, nrep, c->d_agg_tab, out);
     else k_sage_broadcast<false><<<bb, 256, 0, s>>>(c->d_agg_src, rows, dim, G, c->d_agg_slot, nrep, c->d_agg_tab, out); }

@@ -9,10 +9,10 @@
 //   out[i] = (sum over the edges e with dst_e = i of W[rel_e] . x_src[src_e]) / fl(cnt_i + 1e-7)
 //
 // Upstream runs one matvec per edge.  The transform is linear, so the edges are grouped by pair p = (target, relation) first:
-//   S_p    = sum over the edges of p of x_src[src_e]                          (k_rel_chunk_sums, k_rel_combine)
+//   S_p    = sum over the edges of p of x_src[src_e]                          (k_rel_chunk_sums, k_seg_combine)
 //   out[i] = (sum over the pairs p of i of W[r_p] . S_p) / fl(cnt_i + 1e-7)   (k_rel_out)
 // so the matvecs drop from E to P (the distinct pairs) and nothing of size E*D is written.  Fixed orders:
-//   - S_p: the pair's edges in key order, cut into chunks of kRelChunk consecutive edges counted from the pair's first edge;
+//   - S_p: the pair's edges in key order, cut into chunks of kSegChunk consecutive edges counted from the pair's first edge;
 //     each chunk summed left to right, then the chunk sums added in chunk order.  The bits depend on the pair's own edge
 //     sequence only, never on the launch configuration or on other pairs.
 //   - out[i, d]: one __fmaf_rn chain over the pairs of i in key order and, within a pair, over f ascending; then one
@@ -20,7 +20,7 @@
 // Backward, with gm_i = g_i / fl(cnt_i + 1e-7):
 //   gS_p              = W[r_p]^T . gm_{i(p)}                      (k_rel_gs: one __fmaf_rn chain over d ascending)
 //   grad_x_src[j]     = sum over the edges e with src_e = j of gS_{pair(e)}
-//                       (gat.cu's stable order by source and k_gat_bwd_src, weight 1, the edge's pair as its row)
+//                       (the stable order by source and k_gat_bwd_src, weight 1, the edge's pair as its row)
 //   grad_matrix[r]    = sum over the pairs p with r_p = r of gm_{i(p)} (x) S_p
 //                       (the pairs in stable relation order, chunks of kRelPairChunk pairs counted from the relation's first
 //                       pair, each a __fmaf_rn chain; the chunk sums added in chunk order)
@@ -32,41 +32,18 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
-#include <algorithm>
-
-#include "internal.h"
+#include "segment.cuh"
 
 namespace eu {
 
-constexpr int kRelChunk = 256;       // edges per chunk of a pair's row sum
 constexpr int kRelPairChunk = 256;   // pairs per chunk of a relation's grad_matrix sum
 constexpr int kRelUnroll = 8;        // source rows in flight per lane in the chunk sums
-
-__device__ __forceinline__ int64_t rel_lower_bound(const int32_t* __restrict__ a, int64_t n, int64_t key) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if ((int64_t)__ldg(a + mid) < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-__device__ __forceinline__ int64_t rel_upper_bound(const int32_t* __restrict__ a, int64_t n, int64_t key) {
-  int64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) >> 1;
-    if ((int64_t)__ldg(a + mid) <= key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-__device__ __forceinline__ int64_t rel_edge_at(const int32_t* __restrict__ perm, int64_t k) { return perm ? (int64_t)__ldg(perm + k) : k; }
 
 // The pairs of target i: [*pb, *pe) (pair_dst is non-decreasing), and scatter_mean's divisor fl(fl(cnt_i) + 1e-7f).
 __device__ __forceinline__ float rel_target(const int32_t* __restrict__ pair_dst, const int32_t* __restrict__ pair_start, int64_t P,
                                             int64_t i, int64_t* pb, int64_t* pe) {
-  *pb = rel_lower_bound(pair_dst, P, i);
-  *pe = rel_lower_bound(pair_dst, P, i + 1);
+  *pb = key_lower_bound(pair_dst, P, i);
+  *pe = key_lower_bound(pair_dst, P, i + 1);
   const int64_t cnt = (int64_t)__ldg(pair_start + *pe) - __ldg(pair_start + *pb);
   return __fadd_rn((float)cnt, 1e-7f);
 }
@@ -111,7 +88,7 @@ __global__ void k_rel_pairs(const int32_t* __restrict__ head, const int32_t* __r
                             int32_t* __restrict__ pair_start, int32_t* __restrict__ pair_dst, int32_t* __restrict__ pair_rel,
                             int32_t* __restrict__ pair_of_edge) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < E; k += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t ed = rel_edge_at(perm, k);
+    const int64_t ed = edge_at(perm, k);
     const int32_t p = __ldg(pid + k) - 1;
     if (__ldg(head + k)) {
       pair_start[p] = (int32_t)k;
@@ -123,26 +100,13 @@ __global__ void k_rel_pairs(const int32_t* __restrict__ head, const int32_t* __r
   }
 }
 
-// nc[s] = the chunks of K items of segment s = [start[s], start[s + 1]), for s < n; nc[n] = 0 (an exclusive scan then gives
-// every segment's first chunk and, at n, the number of chunks)
-__global__ void k_rel_seg_chunks(const int32_t* __restrict__ start, int64_t n, int K, int32_t* __restrict__ nc) {
-  for (int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; s <= n; s += (int64_t)gridDim.x * blockDim.x)
-    nc[s] = s < n ? (int32_t)(((int64_t)__ldg(start + s + 1) - __ldg(start + s) + K - 1) / K) : 0;
-}
-
-// start[r] = the first position of relation r in the relation-sorted pair keys, for r in [0, R]
-__global__ void k_rel_starts(const int32_t* __restrict__ key, int64_t P, int64_t R, int32_t* __restrict__ start) {
-  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r <= R; r += (int64_t)gridDim.x * blockDim.x)
-    start[r] = (int32_t)rel_lower_bound(key, P, r);
-}
-
 __global__ void k_rel_fill(float* __restrict__ v, int64_t n, float x) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) v[i] = x;
 }
 
 // G lanes per chunk c (lanes over the F columns, 4 per lane with float4).  Chunk c - chunk_off[p] of pair p covers the
-// positions [pair_start[p] + (c - chunk_off[p]) * kRelChunk, ...) up to kRelChunk of them, summed left to right from +0.  A
-// pair of one chunk writes S[p]; the chunks of a longer pair write partial[c] for k_rel_combine.
+// positions [pair_start[p] + (c - chunk_off[p]) * kSegChunk, ...) up to kSegChunk of them, summed left to right from +0.  A
+// pair of one chunk writes S[p]; the chunks of a longer pair write partial[c] for k_seg_combine.
 template <bool VEC>
 __global__ void __launch_bounds__(256) k_rel_chunk_sums(const float* __restrict__ x_src, const int32_t* __restrict__ src,
                                                         const int32_t* __restrict__ perm, const int32_t* __restrict__ pair_start,
@@ -152,10 +116,10 @@ __global__ void __launch_bounds__(256) k_rel_chunk_sums(const float* __restrict_
   const int64_t c = tid >> (31 - __clz(G));
   const int sub = (int)(tid & (G - 1));
   if (c >= slots || c >= __ldg(chunk_off + P)) return;
-  const int64_t p = rel_upper_bound(chunk_off, P + 1, c) - 1;
+  const int64_t p = key_upper_bound(chunk_off, P + 1, c) - 1;
   const int64_t c0 = __ldg(chunk_off + p), nch = __ldg(chunk_off + p + 1) - c0;
-  const int64_t b = __ldg(pair_start + p) + (c - c0) * kRelChunk;
-  const int64_t e = min(b + kRelChunk, (int64_t)__ldg(pair_start + p + 1));
+  const int64_t b = __ldg(pair_start + p) + (c - c0) * kSegChunk;
+  const int64_t e = min(b + kSegChunk, (int64_t)__ldg(pair_start + p + 1));
   float* o = nch == 1 ? S + p * F : partial + c * F;
   if (VEC) {
     for (int d = sub * 4; d < F; d += G * 4) {
@@ -164,7 +128,7 @@ __global__ void __launch_bounds__(256) k_rel_chunk_sums(const float* __restrict_
         float4 x[kRelUnroll];
 #pragma unroll
         for (int q = 0; q < kRelUnroll; ++q)
-          if (k0 + q < e) x[q] = __ldg(reinterpret_cast<const float4*>(x_src + (int64_t)__ldg(src + rel_edge_at(perm, k0 + q)) * F + d));
+          if (k0 + q < e) x[q] = __ldg(reinterpret_cast<const float4*>(x_src + (int64_t)__ldg(src + edge_at(perm, k0 + q)) * F + d));
 #pragma unroll
         for (int q = 0; q < kRelUnroll; ++q) {
           if (k0 + q < e) {
@@ -182,7 +146,7 @@ __global__ void __launch_bounds__(256) k_rel_chunk_sums(const float* __restrict_
         float x[kRelUnroll];
 #pragma unroll
         for (int q = 0; q < kRelUnroll; ++q)
-          if (k0 + q < e) x[q] = __ldg(x_src + (int64_t)__ldg(src + rel_edge_at(perm, k0 + q)) * F + d);
+          if (k0 + q < e) x[q] = __ldg(x_src + (int64_t)__ldg(src + edge_at(perm, k0 + q)) * F + d);
 #pragma unroll
         for (int q = 0; q < kRelUnroll; ++q)
           if (k0 + q < e) acc = __fadd_rn(acc, x[q]);
@@ -190,19 +154,6 @@ __global__ void __launch_bounds__(256) k_rel_chunk_sums(const float* __restrict_
       o[d] = acc;
     }
   }
-}
-
-// S[p, f] = the chunk sums of a pair of several chunks, added in chunk order from +0; one thread per (p, f)
-__global__ void k_rel_combine(const int32_t* __restrict__ chunk_off, const float* __restrict__ partial, int64_t P, int F,
-                              float* __restrict__ S) {
-  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (t >= P * F) return;
-  const int64_t p = t / F, f = t - p * F;
-  const int64_t c0 = __ldg(chunk_off + p), c1 = __ldg(chunk_off + p + 1);
-  if (c1 - c0 == 1) return;
-  float acc = 0.f;
-  for (int64_t c = c0; c < c1; ++c) acc = __fadd_rn(acc, __ldg(partial + c * F + f));
-  S[t] = acc;
 }
 
 // Wt[r, f, d] = W[r, d, f]: k_rel_out's lanes (over d) then read consecutive words
@@ -267,7 +218,7 @@ __global__ void __launch_bounds__(256) k_rel_gw_partials(const float* __restrict
                                                          int64_t R, int D, int F, float* __restrict__ partial) {
   const int64_t c = blockIdx.x;
   if (c >= __ldg(roff + R)) return;   // block-uniform
-  const int64_t r = rel_upper_bound(roff, R + 1, c) - 1;
+  const int64_t r = key_upper_bound(roff, R + 1, c) - 1;
   const int64_t b = __ldg(rstart + r) + (c - __ldg(roff + r)) * kRelPairChunk;
   const int64_t e = min(b + kRelPairChunk, (int64_t)__ldg(rstart + r + 1));
   const int64_t DF = (int64_t)D * F;
@@ -294,20 +245,10 @@ __global__ void k_rel_gw_combine(const float* __restrict__ partial, const int32_
   grad_matrix[t] = acc;
 }
 
-static bool rel_aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-
-static unsigned rel_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), kSMs * 8)); }
-
-static int key_bits(unsigned long long n) {   // bits of the keys [0, n)
-  int b = 1;
-  while (b < 64 && (1ull << b) < n) ++b;
-  return b;
-}
-
 // The pairs of one call, in the ctx scratch.  Layout (offsets fixed once `sorted` is known, so a call that does not grow the
 // scratch keeps what it has computed):
 //   flags | head [E] | pid [E] | scan temp | [sort: keys in, keys out (u64 [E] each), iota, perm ([E] each), cub temp]
-//   | pair_start [P+1] | pair_dst [P] | pair_rel [P] | nc [P+1] | chunk_off [P+1] | S [P, F] | chunk sums [P + E/kRelChunk, F]
+//   | pair_start [P+1] | pair_dst [P] | pair_rel [P] | nc [P+1] | chunk_off [P+1] | S [P, F] | chunk sums [P + E/kSegChunk, F]
 //   | the backward's part (extra bytes)
 struct RelPairs {
   bool sorted = true;
@@ -321,7 +262,7 @@ struct RelPairs {
 
 static void rel_layout(RelPairs* L, int64_t E, int64_t P, int F, size_t extra) {
   L->P = P;
-  L->slots = P + E / kRelChunk;   // >= the chunks: sum over pairs of ceil(len / K) <= P + E / K
+  L->slots = P + E / kSegChunk;   // >= the chunks: sum over pairs of ceil(len / K) <= P + E / K
   L->o_head = 256;
   L->o_pid = L->o_head + a256(4 * (size_t)E);
   L->o_scan = L->o_pid + a256(4 * (size_t)E);
@@ -351,16 +292,16 @@ static int rel_heads(eu_ctx* c, const RelPairs& L, const int32_t* rel, const int
     int32_t* iota = (int32_t*)(m + L.o_sort + 2 * a256(8 * (size_t)E));
     int32_t* perm = (int32_t*)(m + L.o_sort + 2 * a256(8 * (size_t)E) + a256(4 * (size_t)E));
     void* tmp = m + L.o_sort + 2 * a256(8 * (size_t)E) + 2 * a256(4 * (size_t)E);
-    k_rel_keys<<<rel_grid(E), 256, 0, s>>>(dst, rel, E, R, kin, iota);
+    k_rel_keys<<<stride_grid(E), 256, 0, s>>>(dst, rel, E, R, kin, iota);
     EU_LAUNCHED();
     size_t t = L.sort_tmp;
     EU_CUDA(cub::DeviceRadixSort::SortPairs(tmp, t, kin, kout, iota, perm, (int)E, 0,
-                                            key_bits((unsigned long long)n_dst * (unsigned long long)R), s));
+                                            radix_bits((unsigned long long)n_dst * (unsigned long long)R), s));
     EU_LAUNCHED();
     skey = kout;
   }
   EuProfScope ps(c, "rel_heads", E);
-  k_rel_heads<<<rel_grid(E), 256, 0, s>>>(dst, rel, skey, E, R, head, (int*)m);
+  k_rel_heads<<<stride_grid(E), 256, 0, s>>>(dst, rel, skey, E, R, head, (int*)m);
   EU_LAUNCHED();
   size_t t = L.scan_bytes;
   EU_CUDA(cub::DeviceScan::InclusiveSum(m + L.o_scan, t, head, pid, (int)E, s));
@@ -397,7 +338,7 @@ static int rel_prepare(eu_ctx* c, const float* x_src, const int32_t* rel, const 
     L->sorted = false;
     EU_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, L->sort_tmp, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                             (const int32_t*)nullptr, (int32_t*)nullptr, (int)E, 0,
-                                            key_bits((unsigned long long)n_dst * (unsigned long long)R), s));
+                                            radix_bits((unsigned long long)n_dst * (unsigned long long)R), s));
     rel_layout(L, E, 0, F, 0);
     if ((rc = ctx_misc(c, (int64_t)L->total))) return rc;
     if ((rc = rel_heads(c, *L, rel, dst, E, n_dst, R))) return rc;
@@ -419,26 +360,21 @@ static int rel_prepare(eu_ctx* c, const float* x_src, const int32_t* rel, const 
   int32_t* nc = (int32_t*)(m + L->o_nc);
   {
     EuProfScope ps(c, "rel_pairs", E);
-    k_rel_pairs<<<rel_grid(E), 256, 0, s>>>((const int32_t*)(m + L->o_head), (const int32_t*)(m + L->o_pid), L->perm, dst, rel, E,
+    k_rel_pairs<<<stride_grid(E), 256, 0, s>>>((const int32_t*)(m + L->o_head), (const int32_t*)(m + L->o_pid), L->perm, dst, rel, E,
                                             L->pair_start, L->pair_dst, L->pair_rel, nullptr);
     EU_LAUNCHED();
-    k_rel_seg_chunks<<<rel_grid(P + 1), 256, 0, s>>>(L->pair_start, P, kRelChunk, nc);
-    EU_LAUNCHED();
-    size_t t = L->scan_bytes;
-    EU_CUDA(cub::DeviceScan::ExclusiveSum(m + L->o_scan, t, nc, L->chunk_off, (int)(P + 1), s));
-    EU_LAUNCHED();
+    if ((rc = seg_chunk_offsets(c, L->pair_start, P, kSegChunk, nc, m + L->o_scan, L->scan_bytes, L->chunk_off))) return rc;
   }
   {
-    const bool vec = F % 4 == 0 && rel_aligned16(x_src);
-    int G = 1;
-    while (G < 32 && G < (vec ? F / 4 : F)) G <<= 1;
+    const bool vec = F % 4 == 0 && aligned16(x_src);
+    const int G = group_lanes(vec ? F / 4 : F);
     float* part = (float*)(m + L->o_part);
     EuProfScope ps(c, "rel_pair_sums", E);
     const unsigned blocks = (unsigned)ceil_div(L->slots * G, 256);
     if (vec) k_rel_chunk_sums<true><<<blocks, 256, 0, s>>>(x_src, src, L->perm, L->pair_start, L->chunk_off, P, L->slots, F, G, L->S, part);
     else k_rel_chunk_sums<false><<<blocks, 256, 0, s>>>(x_src, src, L->perm, L->pair_start, L->chunk_off, P, L->slots, F, G, L->S, part);
     EU_LAUNCHED();
-    k_rel_combine<<<(unsigned)ceil_div(P * F, 256), 256, 0, s>>>(L->chunk_off, part, P, F, L->S);
+    k_seg_combine<<<(unsigned)ceil_div(P * F, 256), 256, 0, s>>>(L->chunk_off, part, P, F, L->S);
     EU_LAUNCHED();
   }
   return EU_OK;
@@ -482,7 +418,7 @@ int eu_relation_aggregate(eu_ctx* c, const float* x_src, const float* matrix, co
     return rc;
   float* Wt = (float*)((char*)c->d_misc + L.o_extra);
   EuProfScope ps(c, "rel_out", E);
-  k_rel_transpose<<<rel_grid(R * D * F), 256, 0, s>>>(matrix, R, (int)D, (int)F, Wt);
+  k_rel_transpose<<<stride_grid(R * D * F), 256, 0, s>>>(matrix, R, (int)D, (int)F, Wt);
   EU_LAUNCHED();
   k_rel_out<<<(unsigned)ceil_div(n_dst * D, 256), 256, 0, s>>>(Wt, L.S, L.pair_start, L.pair_dst, L.pair_rel, L.P, n_dst, (int)D,
                                                                (int)F, out);
@@ -548,26 +484,22 @@ int eu_relation_aggregate_backward(eu_ctx* c, const float* grad_out, const float
   }
   {
     EuProfScope ps(c, "rel_bwd_src", E);
-    k_rel_pairs<<<rel_grid(E), 256, 0, s>>>((const int32_t*)(m + L.o_head), (const int32_t*)(m + L.o_pid), L.perm, dst, rel, E,
+    k_rel_pairs<<<stride_grid(E), 256, 0, s>>>((const int32_t*)(m + L.o_head), (const int32_t*)(m + L.o_pid), L.perm, dst, rel, E,
                                             L.pair_start, L.pair_dst, L.pair_rel, poe);
     EU_LAUNCHED();
-    k_rel_fill<<<rel_grid(E), 256, 0, s>>>(ones, E, 1.f);
+    k_rel_fill<<<stride_grid(E), 256, 0, s>>>(ones, E, 1.f);
     EU_LAUNCHED();
-    GatOrder sord;
+    EdgeOrder sord;
     if ((rc = order_by(c, src, E, n_src, x + o_sord, &sord))) return rc;
     if ((rc = segmented_row_sum(c, gS, ones, sord, poe, E, n_src, (int)F, grad_x_src))) return rc;
   }
   {
     EuProfScope ps(c, "rel_bwd_matrix", P);
-    GatOrder rord;
+    EdgeOrder rord;
     if ((rc = order_by(c, L.pair_rel, P, R, x + o_rord, &rord))) return rc;
-    k_rel_starts<<<rel_grid(R + 1), 256, 0, s>>>(rord.key, P, R, rst);
+    k_seg_starts<<<stride_grid(R + 1), 256, 0, s>>>(rord.key, P, R, rst);
     EU_LAUNCHED();
-    k_rel_seg_chunks<<<rel_grid(R + 1), 256, 0, s>>>(rst, R, kRelPairChunk, rnc);
-    EU_LAUNCHED();
-    size_t t = L.scan_bytes;
-    EU_CUDA(cub::DeviceScan::ExclusiveSum(m + L.o_scan, t, rnc, roff, (int)(R + 1), s));
-    EU_LAUNCHED();
+    if ((rc = seg_chunk_offsets(c, rst, R, kRelPairChunk, rnc, m + L.o_scan, L.scan_bytes, roff))) return rc;
     const dim3 grid((unsigned)rslots(P), (unsigned)std::min<int64_t>(ceil_div(DF, 256), 65535));
     k_rel_gw_partials<<<grid, 256, 0, s>>>(gm, L.S, L.pair_dst, rord.perm, rst, roff, R, (int)D, (int)F, gw);
     EU_LAUNCHED();

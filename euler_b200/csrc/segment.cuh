@@ -1,0 +1,120 @@
+// Edge orders and fixed-order segment sums shared by the fused aggregations (gat.cu, relation.cu, dna.cu) and the mp scatter.
+//
+// An edge order walks the edges sorted by an int32 index (the target, the source, a relation), stably: edges with equal
+// index keep their order, so a sum over a segment in order gives the bits of the same sum over the stably sorted list.  A
+// fixed-order segment sum cuts each segment into chunks of kSegChunk positions counted from its first one; each chunk is
+// summed left to right and a segment of several chunks adds its chunk sums in chunk order.  The bits then depend on the
+// segment's own sequence only, never on the launch configuration or on other segments, and a hub is spread over many CTAs.
+#pragma once
+#include <algorithm>
+
+#include "internal.h"
+
+namespace eu {
+
+constexpr int kSegChunk = 256;   // positions per chunk of a fixed-order segment sum: it fixes the bits of those sums
+
+// ---------------------------------------------------------------------------- device helpers
+// the first position k in [0, n) with a[k] >= key (a non-decreasing), or n
+__device__ __forceinline__ int64_t key_lower_bound(const int32_t* __restrict__ a, int64_t n, int64_t key) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if ((int64_t)__ldg(a + mid) < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// the first position k in [0, n) with a[k] > key (a non-decreasing), or n
+__device__ __forceinline__ int64_t key_upper_bound(const int32_t* __restrict__ a, int64_t n, int64_t key) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if ((int64_t)__ldg(a + mid) <= key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// the edge at position k of an order (perm: position -> edge, null = the identity)
+__device__ __forceinline__ int64_t edge_at(const int32_t* __restrict__ perm, int64_t k) { return perm ? (int64_t)__ldg(perm + k) : k; }
+
+// the mask of the G-lane group this lane belongs to (G a power of two)
+__device__ __forceinline__ unsigned group_mask(int G) {
+  if (G == 32) return 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  return ((1u << G) - 1u) << (lane & ~(G - 1));
+}
+
+// ---------------------------------------------------------------------------- host helpers
+inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// lanes of a group over n items per row (n = columns, or float4s of columns): a power of two >= n, at most 32
+inline int group_lanes(int64_t n) {
+  int g = 1;
+  while (g < 32 && g < n) g <<= 1;
+  return g;
+}
+
+// the radix-sort bits of the keys [0, n)
+inline int radix_bits(unsigned long long n) {
+  int b = 1;
+  while (b < 64 && (1ull << b) < n) ++b;
+  return b;
+}
+
+// the grid of a grid-stride loop over n items, 256 threads per CTA
+inline unsigned stride_grid(int64_t n) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), kSMs * 8)); }
+
+// ---------------------------------------------------------------------------- edge orders
+__global__ void k_check_sorted(const int32_t* __restrict__ idx, int64_t E, int* unsorted);   // *unsorted = 1 if idx decreases
+
+struct EdgeOrder {                 // the order of the edges by `idx` (int32[E] in [0, n)), stable
+  const int32_t* key = nullptr;    // idx itself when it is already non-decreasing
+  const int32_t* perm = nullptr;   // null then
+};
+
+size_t order_bytes(int64_t E, int64_t n);   // the scratch order_by needs
+// the stable order of the edges by idx (a radix sort), in `buf` (order_bytes(E, n) bytes)
+int order_by(eu_ctx* c, const int32_t* idx, int64_t E, int64_t n, char* buf, EdgeOrder* o);
+
+// The prologue of an entry point that walks the edges by target: the order by dst, and the ctx scratch laid out as
+//   flag (256 B) | head (head_bytes) | [the dst order when dst is unsorted] | tail (tail_bytes)
+// The scratch is sized once the sortedness flag is read back (one stream synchronisation when E >= 2), so a sorted dst holds
+// no sort scratch; a growth reallocates, and nothing but the flag has been written by then.  An unsorted dst is sorted
+// inside the profile scope `sort_scope` (none when null).
+struct TargetOrder {
+  EdgeOrder ord;
+  char* head = nullptr;
+  char* tail = nullptr;
+};
+int order_targets(eu_ctx* c, const int32_t* dst, int64_t E, int64_t n_dst, size_t head_bytes, size_t tail_bytes,
+                  const char* sort_scope, TargetOrder* t);
+
+// ---------------------------------------------------------------------------- chunked segments
+// Segment s of an order is the positions [start[s], start[s + 1]); its chunk c - chunk_off[s] covers K positions from
+// start[s] + (c - chunk_off[s]) * K.
+
+// start[s] = the first position of segment s in the sorted keys `key` [P], for s in [0, n]
+__global__ void k_seg_starts(const int32_t* __restrict__ key, int64_t P, int64_t n, int32_t* __restrict__ start);
+// out[s, f] = the chunk sums partial[c, f] of a segment of several chunks, added in chunk order from +0; one thread per (s, f)
+__global__ void k_seg_combine(const int32_t* __restrict__ chunk_off, const float* __restrict__ partial, int64_t n, int F,
+                              float* __restrict__ out);
+
+size_t seg_scan_bytes(int64_t n);   // the scan scratch of seg_chunk_offsets over n segments
+// chunk_off [n + 1] = each segment's first chunk of K positions, and at n the number of chunks; nc [n + 1] and tmp (tmp_bytes
+// >= seg_scan_bytes(n)) are scratch
+int seg_chunk_offsets(eu_ctx* c, const int32_t* start, int64_t n, int K, int32_t* nc, void* tmp, size_t tmp_bytes,
+                      int32_t* chunk_off);
+
+// The n segments of an edge order of E positions cut into chunks of kSegChunk, in a scratch of seg_plan_bytes(E, n, width)
+// bytes: start [n + 1] | nc [n + 1] | chunk_off [n + 1] | scan temp | partial chunk sums [slots, width]
+struct SegPlan {
+  int64_t n = 0, slots = 0;   // slots = n + E / kSegChunk >= the chunks: sum over segments of ceil(len / K) <= n + E / K
+  int32_t *start = nullptr, *chunk_off = nullptr;
+  float* partial = nullptr;
+};
+size_t seg_plan_bytes(int64_t E, int64_t n, int64_t width);
+// the segment starts and chunk offsets of the order o of E > 0 edges over n segments, in buf
+int plan_segments(eu_ctx* c, const EdgeOrder& o, int64_t E, int64_t n, char* buf, SegPlan* S);
+
+}  // namespace eu
