@@ -134,7 +134,10 @@ __global__ void __launch_bounds__(kPrepBlock) k_prepare(DevGraph g, const HashSl
                                                         ETypes et, int mode, uint32_t F, unsigned long long draws_per_row,
                                                         int32_t* first, int64_t* rowof, uint32_t* emask, uint32_t* wmul,
                                                         uint32_t* blkpre, uint32_t* blkmul, EuRngState* rngs, PrepOut po) {
-  __shared__ uint32_t s_w[kPrepBlock / 32];
+  __shared__ uint32_t s_w[kPrepBlock / 32];   // per warp: eligible first occurrences
+  __shared__ uint32_t s_l[kPrepBlock / 32];   // per warp: rows for the live list, then their offset in it
+  __shared__ uint32_t s_d[kPrepBlock / 32];   // per warp: rows for the duplicate list, then their offset in it
+  __shared__ uint32_t s_z[kPrepBlock / 32];   // per warp: ballot of the rows that cannot draw
   __shared__ bool s_last;
   const int b = blockIdx.y;
   const int64_t li = blockIdx.x * (int64_t)kPrepBlock + threadIdx.x;
@@ -143,6 +146,7 @@ __global__ void __launch_bounds__(kPrepBlock) k_prepare(DevGraph g, const HashSl
   EuRngState* rng = rngs + b;
   bool e = false;      // eligible FIRST occurrence: takes a slot of the serial draw order
   bool own = false;    // this row samples (its id is eligible, whether or not it is the first occurrence)
+  bool dflt = false;   // this row exists and cannot sample: k_prepare writes its default entries
   const int64_t rows_here = gm.rows_act ? (int64_t)gm.rows_act[b] : gm.rows_b;
   // blocks past the batch's real rows (worst-case-sized sharded owner inputs) neither scan nor take a ticket: the launch
   // costs its live rows, not its capacity.  Block 0 always stays (it advances the engine of an empty batch).
@@ -159,37 +163,29 @@ __global__ void __launch_bounds__(kPrepBlock) k_prepare(DevGraph g, const HashSl
     const int64_t row = lookup_row(g, id);
     own = row_eligible(g, row, et, mode);
     e = own && f == li;
-    if (own) {
-      rowof[ii] = row;
-    } else {
-      const int64_t ob = w * (int64_t)po.count;
-      for (int32_t j = 0; j < po.count; ++j) {
-        if (po.eng_ids) po.eng_ids[ob + j] = 0ull;
-        if (po.out_ids) { po.out_ids[ob + j] = po.default_node; po.out_w[ob + j] = 0.f; po.out_t[ob + j] = -1; }
-      }
-      if (po.next_tabs)  // its `count` zeros enter the next hop's dedup table with their minimum index
-        dedup_insert_one(po.next_tabs + (int64_t)b * (po.next_cap_b + 1), (unsigned long long)po.next_cap_b - 1, 0ull,
-                         li * (int64_t)po.count);
+    dflt = !own;
+    if (own) rowof[ii] = row;
+  }
+  // The warp's 32 rows are consecutive, so their `count` output slots each form one range of 32 * count slots: the lanes
+  // stride over it together and write the slots of the rows that cannot sample (coalesced, whatever the mix of rows).
+  const uint32_t zm = __ballot_sync(0xffffffffu, dflt);
+  if (zm) {
+    const int64_t ob = (b * gm.rows_b + (li - lane)) * (int64_t)po.count;
+    const uint32_t n = 32u * (uint32_t)po.count;
+    for (uint32_t k = lane; k < n; k += 32) {
+      if (!((zm >> (k / (uint32_t)po.count)) & 1u)) continue;
+      if (po.eng_ids) po.eng_ids[ob + k] = 0ull;
+      if (po.out_ids) { po.out_ids[ob + k] = po.default_node; po.out_w[ob + k] = 0.f; po.out_t[ob + k] = -1; }
     }
   }
   // compact the rows that draw (order is irrelevant: a row's engine state depends only on its position).  An eligible duplicate
   // would draw exactly what its first occurrence draws (same graph row, same engine state): given a duplicate list (hops of
   // kRepeatMinRows rows or more) it goes there and k_copy_dups hands it the first occurrence's outputs once k_sample has
-  // written them; otherwise it draws again.
+  // written them; otherwise it draws again.  One atomic per block and list.
   const uint32_t m = __ballot_sync(0xffffffffu, e);
-  {
-    const uint32_t lm = po.dup ? m : __ballot_sync(0xffffffffu, own);   // without a duplicate list every eligible row draws
-    const uint32_t dm = po.dup ? __ballot_sync(0xffffffffu, own && !e) : 0u;
-    uint32_t lbase = 0, dbase = 0;
-    if (lane == 0 && lm) lbase = atomicAdd(po.n_live, (unsigned int)__popc(lm));
-    if (lane == 0 && dm) dbase = atomicAdd(po.n_dup, (unsigned int)__popc(dm));
-    lbase = __shfl_sync(0xffffffffu, lbase, 0);
-    dbase = __shfl_sync(0xffffffffu, dbase, 0);
-    const uint32_t below = (1u << lane) - 1u;
-    if (e || (own && !po.dup)) po.live[lbase + __popc(lm & below)] = (int32_t)(b * gm.rows_b + li);
-    else if (own) po.dup[dbase + __popc(dm & below)] = (int32_t)(b * gm.rows_b + li);
-  }
-  if (lane == 0) s_w[wid] = __popc(m);
+  const uint32_t lm = po.dup ? m : __ballot_sync(0xffffffffu, own);   // without a duplicate list every eligible row draws
+  const uint32_t dm = po.dup ? __ballot_sync(0xffffffffu, own && !e) : 0u;
+  if (lane == 0) { s_w[wid] = __popc(m); s_l[wid] = __popc(lm); s_d[wid] = __popc(dm); s_z[wid] = zm; }
   __syncthreads();
   if (lane == 0) {  // rows_pad is a multiple of 256: every group of the block exists in the scratch arrays
     uint32_t off = 0;
@@ -202,13 +198,36 @@ __global__ void __launch_bounds__(kPrepBlock) k_prepare(DevGraph g, const HashSl
   }
   uint32_t* bp = blkpre + (int64_t)b * gm.nblk_b;
   if (threadIdx.x == 0) {
-    uint32_t tot = 0;
-    for (int k = 0; k < kPrepBlock / 32; ++k) tot += s_w[k];
+    uint32_t tot = 0, lt = 0, dt = 0;
+    for (int k = 0; k < kPrepBlock / 32; ++k) {
+      tot += s_w[k];
+      const uint32_t l = s_l[k], d = s_d[k];
+      s_l[k] = lt; s_d[k] = dt;
+      lt += l; dt += d;
+    }
+    const uint32_t lbase = lt ? atomicAdd(po.n_live, lt) : 0u, dbase = dt ? atomicAdd(po.n_dup, dt) : 0u;
+    for (int k = 0; k < kPrepBlock / 32; ++k) { s_l[k] += lbase; s_d[k] += dbase; }
+    // The rows that cannot sample each enter `count` zeros into the next hop's table, at their first index li * count.  The
+    // table keeps each id's minimum index (atomicMin), so only the smallest of them can change the slot: that of the lowest
+    // such row of the block -- rows grow with the warp and the lane -- is entered alone.
+    if (po.next_tabs)
+      for (int k = 0; k < kPrepBlock / 32; ++k)
+        if (s_z[k]) {
+          const int64_t lz = blockIdx.x * (int64_t)kPrepBlock + k * 32 + (__ffs(s_z[k]) - 1);
+          dedup_insert_one(po.next_tabs + (int64_t)b * (po.next_cap_b + 1), (unsigned long long)po.next_cap_b - 1, 0ull,
+                           lz * (int64_t)po.count);
+          break;
+        }
     bp[blockIdx.x] = tot;
     __threadfence();
     s_last = atomicAdd(&rng->blocks_done, 1u) == nblk_act - 1;
   }
   __syncthreads();
+  {
+    const uint32_t below = (1u << lane) - 1u;
+    if (e || (own && !po.dup)) po.live[s_l[wid] + __popc(lm & below)] = (int32_t)(b * gm.rows_b + li);
+    else if (own) po.dup[s_d[wid] + __popc(dm & below)] = (int32_t)(b * gm.rows_b + li);
+  }
   if (!s_last) return;
   // last block of this batch: exclusive prefix over the batch's per-block counts, in place
   __threadfence();
@@ -421,7 +440,7 @@ __global__ void __launch_bounds__(256, CTAS) k_sample(DevGraph g, SampleArgs a) 
         row = -1;
       }
     }
-    if (!ok) {
+    if (!ok) {   // philox only (k_prepare finishes these rows otherwise); a row's lanes write its consecutive slots, coalesced
       for (int32_t j = sl; j < count; j += SG) {
         if (a.eng_ids) a.eng_ids[obase + j] = 0ull;
         if (a.out_ids) { a.out_ids[obase + j] = a.default_node; a.out_w[obase + j] = 0.f; a.out_t[obase + j] = -1; }
