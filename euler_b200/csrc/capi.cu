@@ -1,4 +1,4 @@
-// Contexts, host-buffer entry points and the reference's InitQueryProxy entry.
+// Contexts (scratch, engines, profiling), the default graph and the reference's InitQueryProxy entry.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -6,9 +6,7 @@
 #include <algorithm>
 #include <map>
 #include <mutex>
-#include <initializer_list>
 #include <string>
-#include <vector>
 
 #include "internal.h"
 
@@ -120,43 +118,6 @@ int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots) {
     c->agg_rows = rows;
   }
   return EU_OK;
-}
-
-int ctx_stage(eu_ctx* c, int64_t host_bytes, int64_t dev_bytes) {
-  if (host_bytes > c->pin_bytes) {
-    if (c->h_pin) cudaFreeHost(c->h_pin);
-    c->h_pin = nullptr; c->pin_bytes = 0;
-    EU_CUDA(cudaHostAlloc(&c->h_pin, (size_t)host_bytes, cudaHostAllocDefault));
-    c->pin_bytes = host_bytes;
-  }
-  if (dev_bytes > c->stage_bytes) {
-    EU_CUDA(cudaStreamSynchronize(c->stream));
-    char* p = (char*)c->d_stage;
-    int rc = regrow(&p, dev_bytes);
-    c->d_stage = p;
-    if (rc) { c->stage_bytes = 0; return rc; }
-    c->stage_bytes = dev_bytes;
-  }
-  return EU_OK;
-}
-
-static inline int64_t align256(int64_t x) { return (x + 255) & ~(int64_t)255; }
-
-// Bump allocator over the ctx staging buffers: the same offsets are used on the pinned host
-// side and on the device side.
-struct Stage {
-  int64_t off = 0;
-  int64_t take(int64_t bytes) { int64_t o = off; off += align256(bytes); return o; }
-};
-
-// A caller's host buffer that is already page-locked (cudaHostAlloc / cudaHostRegister -- e.g. a framework's pinned
-// tensor) is DMA'd directly; only pageable memory goes through the ctx's pinned staging buffer (a pageable
-// cudaMemcpyAsync would serialise against the host, and the extra memcpy costs more than PCIe for wide feature rows).
-static bool host_is_pinned(const void* p) {
-  if (!p) return false;
-  cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-  return a.type == cudaMemoryTypeHost;
 }
 
 static std::mutex g_default_mu;
@@ -292,219 +253,6 @@ int eu_ctx_profile_read(eu_ctx* c, char* buf, int64_t cap) {
   memcpy(buf, out.c_str(), out.size() + 1);
   return EU_OK;
 }
-
-// ------------------------------------------------------------------------------ host variants
-// Pattern: copy inputs into pinned memory, H2D on the ctx stream, run the device op, D2H into
-// pinned memory, synchronise, copy out.  The pinned hop keeps the copies asynchronous-capable
-// (pageable cudaMemcpyAsync would serialise against the host).
-
-// Host-buffer staging of one call: inputs go H2D, outputs come D2H, all on the ctx stream.  Pinned caller buffers are
-// DMA'd in place; pageable ones pass through the ctx's pinned stage (copied out after the final synchronise).
-struct HostIO {
-  eu_ctx* c;
-  Stage st;
-  struct Out { void* user; int64_t off; int64_t bytes; };
-  std::vector<Out> outs;
-  int64_t take(int64_t bytes) { return st.take(bytes); }
-  // size the stage: the device side always, the pinned host side only if some caller buffer is pageable
-  int begin(std::initializer_list<const void*> user_bufs) {
-    bool all = true;
-    for (const void* p : user_bufs) all = all && (!p || host_is_pinned(p));
-    return ctx_stage(c, all ? 0 : st.off, st.off);
-  }
-  // device address of stage offset `off`
-  char* dev(int64_t off) const { return (char*)c->d_stage + off; }
-  int in(int64_t off, const void* user, int64_t bytes) {
-    if (bytes <= 0) return EU_OK;
-    const void* src = user;
-    if (!host_is_pinned(user)) { memcpy((char*)c->h_pin + off, user, (size_t)bytes); src = (char*)c->h_pin + off; }
-    EU_CUDA(cudaMemcpyAsync(dev(off), src, (size_t)bytes, cudaMemcpyHostToDevice, c->stream));
-    return EU_OK;
-  }
-  int out(int64_t off, void* user, int64_t bytes) {
-    if (bytes <= 0 || !user) return EU_OK;
-    if (host_is_pinned(user)) {
-      EU_CUDA(cudaMemcpyAsync(user, dev(off), (size_t)bytes, cudaMemcpyDeviceToHost, c->stream));
-    } else {
-      EU_CUDA(cudaMemcpyAsync((char*)c->h_pin + off, dev(off), (size_t)bytes, cudaMemcpyDeviceToHost, c->stream));
-      outs.push_back({user, off, bytes});
-    }
-    return EU_OK;
-  }
-  int finish() {
-    EU_CUDA(cudaStreamSynchronize(c->stream));
-    for (auto& o : outs) memcpy(o.user, (char*)c->h_pin + o.off, (size_t)o.bytes);
-    return EU_OK;
-  }
-};
-
-int eu_sample_fanout_batched_host(eu_ctx* c, const int64_t* nodes, int32_t nb, int64_t B, const int32_t* etypes,
-                                  int32_t K, const int32_t* counts, int32_t L, int64_t default_node,
-                                  int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t) {
-  if (!c || nb < 1 || B < 0 || L < 0 || L > 16 || !counts || (B > 0 && !nodes)) { set_error("eu_sample_fanout_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  HostIO io{c};
-  const int64_t o_nodes = io.take(8 * B * nb);
-  int64_t o_ids[16], o_w[16], o_t[16], n_l[16];
-  int64_t rows = B * nb;
-  for (int l = 0; l < L; ++l) {
-    if (counts[l] < 0) { set_error("negative count"); return EU_ERR_INVALID; }
-    rows *= counts[l];
-    n_l[l] = rows;
-    o_ids[l] = io.take(8 * rows); o_w[l] = io.take(4 * rows); o_t[l] = io.take(4 * rows);
-  }
-  int rc;
-  {
-    bool all = host_is_pinned(nodes);
-    for (int l = 0; l < L && all; ++l)
-      all = (!out_ids || !out_ids[l] || host_is_pinned(out_ids[l])) && (!out_w || !out_w[l] || host_is_pinned(out_w[l])) &&
-            (!out_t || !out_t[l] || host_is_pinned(out_t[l]));
-    rc = ctx_stage(c, all ? 0 : io.st.off, io.st.off);
-  }
-  if (rc) return rc;
-  if ((rc = io.in(o_nodes, nodes, 8 * B * nb))) return rc;
-  int64_t* d_ids[16]; float* d_w[16]; int32_t* d_t[16];
-  for (int l = 0; l < L; ++l) { d_ids[l] = (int64_t*)io.dev(o_ids[l]); d_w[l] = (float*)io.dev(o_w[l]); d_t[l] = (int32_t*)io.dev(o_t[l]); }
-  rc = eu_sample_fanout_batched(c, (const int64_t*)io.dev(o_nodes), nb, B, etypes, K, counts, L, default_node, d_ids, d_w, d_t);
-  if (rc) return rc;
-  for (int l = 0; l < L; ++l) {
-    if (out_ids && (rc = io.out(o_ids[l], out_ids[l], 8 * n_l[l]))) return rc;
-    if (out_w && (rc = io.out(o_w[l], out_w[l], 4 * n_l[l]))) return rc;
-    if (out_t && (rc = io.out(o_t[l], out_t[l], 4 * n_l[l]))) return rc;
-  }
-  return io.finish();
-}
-
-int eu_sample_fanout_host(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes,
-                          int32_t K, const int32_t* counts, int32_t L, int64_t default_node,
-                          int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t) {
-  return eu_sample_fanout_batched_host(c, nodes, 1, B, etypes, K, counts, L, default_node, out_ids, out_w, out_t);
-}
-
-int eu_sample_neighbor_host(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes,
-                            int32_t K, int32_t count, int64_t default_node, int64_t* out_ids,
-                            float* out_w, int32_t* out_t) {
-  return eu_sample_fanout_host(c, nodes, B, etypes, K, &count, 1, default_node, &out_ids, &out_w, &out_t);
-}
-
-int eu_sample_neighbor_raw_host(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K, int32_t count,
-                                int64_t* out_ids, float* out_w, int32_t* out_t) {
-  if (!c || B < 0 || count < 0 || (B > 0 && (!nodes || (count > 0 && (!out_ids || !out_w || !out_t))))) { set_error("eu_sample_neighbor_raw_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  HostIO io{c};
-  const int64_t n = B * count;
-  const int64_t o_nodes = io.take(8 * B), o_ids = io.take(8 * n), o_w = io.take(4 * n), o_t = io.take(4 * n);
-  int rc = io.begin({nodes, out_ids, out_w, out_t});
-  if (rc) return rc;
-  if ((rc = io.in(o_nodes, nodes, 8 * B))) return rc;
-  rc = eu_sample_neighbor_raw(c, (const int64_t*)io.dev(o_nodes), B, etypes, K, count, (int64_t*)io.dev(o_ids), (float*)io.dev(o_w), (int32_t*)io.dev(o_t));
-  if (rc) return rc;
-  if ((rc = io.out(o_ids, out_ids, 8 * n)) || (rc = io.out(o_w, out_w, 4 * n)) || (rc = io.out(o_t, out_t, 4 * n))) return rc;
-  return io.finish();
-}
-
-int eu_sample_node_host(eu_ctx* c, int32_t count, const int32_t* types, int32_t n_types, int64_t* out) {
-  if (!c || count < 0 || (count > 0 && !out)) { set_error("eu_sample_node_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  int rc = ctx_stage(c, 8 * (int64_t)count + 256, 8 * (int64_t)count + 256);
-  if (rc) return rc;
-  rc = eu_sample_node(c, count, types, n_types, (int64_t*)c->d_stage);
-  if (rc) return rc;
-  EU_CUDA(cudaMemcpyAsync(c->h_pin, c->d_stage, 8 * (size_t)count, cudaMemcpyDeviceToHost, c->stream));
-  EU_CUDA(cudaStreamSynchronize(c->stream));
-  memcpy(out, c->h_pin, 8 * (size_t)count);
-  return EU_OK;
-}
-
-int eu_random_walk_host(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes,
-                        int32_t K, int32_t L, float p, float q, int64_t default_node, int64_t* out) {
-  if (!c || B < 0 || L < 0 || (B > 0 && (!nodes || !out))) { set_error("eu_random_walk_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  Stage st;
-  const int64_t o_nodes = st.take(8 * B), o_out = st.take(8 * B * (L + 1));
-  int rc = ctx_stage(c, st.off, st.off);
-  if (rc) return rc;
-  char* hp = (char*)c->h_pin; char* dp = (char*)c->d_stage;
-  memcpy(hp + o_nodes, nodes, 8 * (size_t)B);
-  EU_CUDA(cudaMemcpyAsync(dp + o_nodes, hp + o_nodes, 8 * (size_t)B, cudaMemcpyHostToDevice, c->stream));
-  rc = eu_random_walk(c, (const int64_t*)(dp + o_nodes), B, etypes, K, L, p, q, default_node, (int64_t*)(dp + o_out));
-  if (rc) return rc;
-  EU_CUDA(cudaMemcpyAsync(hp + o_out, dp + o_out, 8 * (size_t)(B * (L + 1)), cudaMemcpyDeviceToHost, c->stream));
-  EU_CUDA(cudaStreamSynchronize(c->stream));
-  memcpy(out, hp + o_out, 8 * (size_t)(B * (L + 1)));
-  return EU_OK;
-}
-
-int eu_get_dense_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, float* out) {
-  if (!c || M < 0 || dim < 0 || (M > 0 && (!nodes || !out))) { set_error("eu_get_dense_feature_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  HostIO io{c};
-  const int64_t o_nodes = io.take(8 * M), o_out = io.take(4 * M * dim);
-  int rc = io.begin({nodes, out});
-  if (rc) return rc;
-  if ((rc = io.in(o_nodes, nodes, 8 * M))) return rc;
-  rc = eu_get_dense_feature(c, (const int64_t*)io.dev(o_nodes), M, fid, dim, (float*)io.dev(o_out));
-  if (rc) return rc;
-  if ((rc = io.out(o_out, out, 4 * M * dim))) return rc;
-  return io.finish();
-}
-
-// eu_sage_mean_aggregate with host buffers: only the neighbor ids go up and only the [rows, dim] means come down -- the
-// rows*count feature rows the unfused composition (get_dense_feature_host + scatter_mean) would move never leave HBM.
-int eu_sage_mean_aggregate_host(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out) {
-  if (!c || rows < 0 || count < 0 || dim <= 0 || (rows > 0 && (!nbr_ids || !out))) { set_error("eu_sage_mean_aggregate_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  HostIO io{c};
-  const int64_t o_ids = io.take(8 * rows * count), o_out = io.take(4 * rows * dim);
-  int rc = io.begin({nbr_ids, out});
-  if (rc) return rc;
-  if ((rc = io.in(o_ids, nbr_ids, 8 * rows * count))) return rc;
-  rc = eu_sage_mean_aggregate(c, (const int64_t*)io.dev(o_ids), rows, count, dim, (float*)io.dev(o_out));
-  if (rc) return rc;
-  if ((rc = io.out(o_out, out, 4 * rows * dim))) return rc;
-  return io.finish();
-}
-
-int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx, int64_t E, float* out) {
-  if (!c || N < 0 || D <= 0 || E < 0) { set_error("eu_gather_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  Stage st;
-  const int64_t o_p = st.take(4 * N * D), o_i = st.take(4 * E), o_o = st.take(4 * E * D);
-  int rc = ctx_stage(c, st.off, st.off);
-  if (rc) return rc;
-  char* hp = (char*)c->h_pin; char* dp = (char*)c->d_stage;
-  memcpy(hp + o_p, params, 4 * (size_t)(N * D));
-  memcpy(hp + o_i, idx, 4 * (size_t)E);
-  EU_CUDA(cudaMemcpyAsync(dp + o_p, hp + o_p, (size_t)(o_o - o_p), cudaMemcpyHostToDevice, c->stream));
-  rc = eu_gather(c, (const float*)(dp + o_p), N, D, (const int32_t*)(dp + o_i), E, (float*)(dp + o_o));
-  if (rc) return rc;
-  EU_CUDA(cudaMemcpyAsync(hp + o_o, dp + o_o, 4 * (size_t)(E * D), cudaMemcpyDeviceToHost, c->stream));
-  EU_CUDA(cudaStreamSynchronize(c->stream));
-  memcpy(out, hp + o_o, 4 * (size_t)(E * D));
-  return EU_OK;
-}
-
-static int scatter_host(int op, eu_ctx* c, const float* u, int64_t D, const int32_t* idx, int64_t E, int64_t size, float* out) {
-  if (!c || D <= 0 || E < 0 || size < 0) { set_error("scatter_host: bad argument"); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  Stage st;
-  const int64_t o_u = st.take(4 * E * D), o_i = st.take(4 * E), o_o = st.take(4 * size * D);
-  int rc = ctx_stage(c, st.off, st.off);
-  if (rc) return rc;
-  char* hp = (char*)c->h_pin; char* dp = (char*)c->d_stage;
-  memcpy(hp + o_u, u, 4 * (size_t)(E * D));
-  memcpy(hp + o_i, idx, 4 * (size_t)E);
-  EU_CUDA(cudaMemcpyAsync(dp + o_u, hp + o_u, (size_t)(o_o - o_u), cudaMemcpyHostToDevice, c->stream));
-  const float* du = (const float*)(dp + o_u); const int32_t* di = (const int32_t*)(dp + o_i); float* dout = (float*)(dp + o_o);
-  rc = op == 0 ? eu_scatter_add(c, du, D, di, E, size, dout) : eu_scatter_max(c, du, D, di, E, size, dout);
-  if (rc) return rc;
-  EU_CUDA(cudaMemcpyAsync(hp + o_o, dp + o_o, 4 * (size_t)(size * D), cudaMemcpyDeviceToHost, c->stream));
-  EU_CUDA(cudaStreamSynchronize(c->stream));
-  memcpy(out, hp + o_o, 4 * (size_t)(size * D));
-  return EU_OK;
-}
-int eu_scatter_add_host(eu_ctx* c, const float* u, int64_t D, const int32_t* idx, int64_t E, int64_t size, float* out) { return scatter_host(0, c, u, D, idx, E, size, out); }
-int eu_scatter_max_host(eu_ctx* c, const float* u, int64_t D, const int32_t* idx, int64_t E, int64_t size, float* out) { return scatter_host(1, c, u, D, idx, E, size, out); }
 
 // ------------------------------------------------------------------------------ InitQueryProxy
 eu_graph* eu_default_graph(void) { std::lock_guard<std::mutex> l(g_default_mu); return g_default_graph; }

@@ -85,43 +85,6 @@ static int ragged_get(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, i
   return EU_OK;
 }
 
-// host buffers: lengths first (total), then the values when cap allows
-template <bool SPARSE>
-static int ragged_get_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, int64_t cap, int64_t* out_ptr,
-                           void* out_vals, int64_t* total, const char* what) {
-  if (!c || M < 0 || cap < 0 || !out_ptr || (M > 0 && !nodes)) { set_error("%s: bad argument", what); return EU_ERR_INVALID; }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  unsigned long long* d_nodes = nullptr;
-  long long* d_ptr = nullptr;
-  char* d_vals = nullptr;
-  EU_CUDA(cudaMalloc(&d_nodes, 8 * (size_t)std::max<int64_t>(M, 1)));
-  EU_CUDA(cudaMalloc(&d_ptr, 8 * (size_t)(M + 1)));
-  const size_t esz = SPARSE ? 8 : 1;
-  int rc = EU_OK;
-  do {
-    if (M > 0 && cudaMemcpyAsync(d_nodes, nodes, 8 * (size_t)M, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) { rc = EU_ERR_CUDA; break; }
-    rc = ragged_get<SPARSE>(c, (const int64_t*)d_nodes, M, fid, default_value, 0, (int64_t*)d_ptr, nullptr, nullptr, what);
-    if (rc) break;
-    if (cudaMemcpyAsync(out_ptr, d_ptr, 8 * (size_t)(M + 1), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
-        cudaStreamSynchronize(c->stream) != cudaSuccess) { rc = EU_ERR_CUDA; break; }
-    const int64_t tot = out_ptr[M];
-    if (total) *total = tot;
-    const int64_t n = std::min(cap, tot);
-    if (n > 0) {
-      if (!out_vals) { set_error("%s: null output", what); rc = EU_ERR_INVALID; break; }
-      if (cudaMalloc(&d_vals, esz * (size_t)n) != cudaSuccess) { set_error("%s: cudaMalloc failed", what); rc = EU_ERR_CUDA; break; }
-      rc = ragged_get<SPARSE>(c, (const int64_t*)d_nodes, M, fid, default_value, n, (int64_t*)d_ptr, SPARSE ? (int64_t*)d_vals : nullptr,
-                              SPARSE ? nullptr : (uint8_t*)d_vals, what);
-      if (rc) break;
-      if (cudaMemcpyAsync(out_vals, d_vals, esz * (size_t)n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
-          cudaStreamSynchronize(c->stream) != cudaSuccess) { rc = EU_ERR_CUDA; break; }
-    }
-  } while (false);
-  cudaFree(d_nodes); cudaFree(d_ptr); cudaFree(d_vals);
-  if (rc == EU_ERR_CUDA) set_error("%s: CUDA error %s", what, cudaGetErrorString(cudaGetLastError()));
-  return rc;
-}
-
 }  // namespace eu
 
 using namespace eu;
@@ -132,16 +95,8 @@ int eu_get_sparse_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fi
                           int64_t* out_values) {
   return ragged_get<true>(c, nodes, M, fid, default_value, cap, out_ptr, out_values, nullptr, "eu_get_sparse_feature");
 }
-int eu_get_sparse_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, int64_t cap, int64_t* out_ptr,
-                               int64_t* out_values, int64_t* total) {
-  return ragged_get_host<true>(c, nodes, M, fid, default_value, cap, out_ptr, out_values, total, "eu_get_sparse_feature_host");
-}
 int eu_get_binary_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t cap, int64_t* out_ptr, uint8_t* out_bytes) {
   return ragged_get<false>(c, nodes, M, fid, 0, cap, out_ptr, nullptr, out_bytes, "eu_get_binary_feature");
-}
-int eu_get_binary_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t cap, int64_t* out_ptr, uint8_t* out_bytes,
-                               int64_t* total) {
-  return ragged_get_host<false>(c, nodes, M, fid, 0, cap, out_ptr, out_bytes, total, "eu_get_binary_feature_host");
 }
 
 }  // extern "C"

@@ -188,8 +188,8 @@ int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const EdgeOr
                       int dim, float* out);
 int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
-int ctx_stage(eu_ctx* c, int64_t host_bytes, int64_t dev_bytes);
 int graph_build_sampler(eu_graph* g);
+int get_node_weight(eu_ctx* c, const int64_t* nodes, int64_t B, float* out);   // neighbor.cu, for eu_get_node_weight_host
 int launch_state_scan(eu_ctx* c, int64_t rows, unsigned long long uniforms_per_row);
 // one sampleNB hop (sample.cu): seeds u64[rows] -> engine ids u64[rows*count] (0 placeholders, may be
 // null) and TF-packed outputs (may be null)
