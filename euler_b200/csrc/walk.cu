@@ -208,13 +208,15 @@ struct WarpWalk {
       const long long vmin = __shfl_sync(FULL, cv, 0), vmax = __shfl_sync(FULL, cv, nvalid - 1);
       int cnt = 0;
       for (int64_t tk = pk; tk < pe; tk += 32) {
-        const long long pv = tk + lane < pe ? (long long)__ldg(g->nbr + tk + lane) : BIG;
+        const int np = (int)min((int64_t)32, pe - tk);  // parent lanes holding a list entry; the others are padding
+        const long long pv = lane < np ? (long long)__ldg(g->nbr + tk + lane) : BIG;
         const long long pmin = __shfl_sync(FULL, pv, 0);
-        const long long pmax = __shfl_sync(FULL, pv, (int)min((int64_t)31, pe - tk - 1));
+        const long long pmax = __shfl_sync(FULL, pv, np - 1);
         if (pmax < vmin) { pk = tk + 32; continue; }   // below every remaining child value: never needed again
         if (pmin > vmax) break;                         // above this child chunk: the next chunk restarts at pk
+        // count valid lanes only: a child id equal to the padding value (2^63-1) must not match the padding
 #pragma unroll 8
-        for (int k = 0; k < 32; ++k) cnt += (__shfl_sync(FULL, pv, k) == cv) ? 1 : 0;
+        for (int k = 0; k < 32; ++k) cnt += (__shfl_sync(FULL, pv, k) == cv && k < np) ? 1 : 0;
         if (pmax > vmax) break;
       }
       const bool shared = m < cnt;
@@ -254,10 +256,11 @@ struct WarpWalk {
 // discarded part of v exceeds u / 2 -- an INTEGER increment that does not depend on M, except (i) exact ties (discarded
 // part == u / 2: round-half-even needs M's parity), (ii) M reaching 2^24 (the binade changes) and (iii) v above S's binade.
 // So the block computes the increments of 1024 elements in parallel, prefix-sums them as integers, accepts everything
-// before the first exception, lets one thread redo the next 32 elements with real FADDs, and continues.  Exceptions are
+// before the first exception, lets one thread redo the next kPrefSer elements with real FADDs, and continues.  Exceptions are
 // common only while S is within a few binades of the addends (the first dozens of elements of a row); a 137K-edge hub row
-// of the R-MAT graph takes 143 iterations instead of 137K dependent FADDs.  Checked against the plain sequential sum on
-// random, tie-heavy, zero-laden and wide-exponent inputs (the same arithmetic in Python) and by the oracle parity tests.
+// of the R-MAT graph takes 143 iterations instead of 137K dependent FADDs.  tests/test_walk_prefix_gpu.py compares it bit for
+// bit with the oracle's sequential sum on tie-heavy, zero-laden, wide-exponent, subnormal and randomly rounding rows at
+// every length where the step switches kernels (tests/walk_rows.py builds them and counts the events each one causes).
 static constexpr int kWalkBig = 512;        // rows longer than this get a 256-thread CTA (shorter ones a warp)
 static constexpr int kWalkHuge = 16384;     // rows longer than this get a 1024-thread CTA
 static constexpr int kWalkChunk = 256;      // elements per k_walk_weights chunk
