@@ -97,6 +97,8 @@ SIGNATURES = {
     "eu_sample_fanout_batched": (C.c_int, [_P, _P, _I32, _I64, _P, _I32, _P, _I32, _I64, _P, _P, _P]),
     "eu_sample_fanout_host": (C.c_int, [_P, _P, _I64, _P, _I32, _P, _I32, _I64, _P, _P, _P]),
     "eu_sample_fanout_batched_host": (C.c_int, [_P, _P, _I32, _I64, _P, _I32, _P, _I32, _I64, _P, _P, _P]),
+    "eu_sample_fanout_with_feature": (C.c_int, [_P, _P, _I64, _P, _I32, _P, _I32, _I64, _P, _P, _P, _P, _I32, _P, _P, _P, _I32, _P, _P,
+                                                _P, _P]),
     "eu_sage_mean_aggregate_host": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
     "eu_sample_node": (C.c_int, [_P, _I32, _P, _I32, _P]),
     "eu_sample_node_host": (C.c_int, [_P, _I32, _P, _I32, _P]),
@@ -127,6 +129,8 @@ SIGNATURES = {
     "eu_relation_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _I32, _P, _P]),
     "eu_dna_aggregate": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P]),
     "eu_dna_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P, _P]),
+    "eu_sparse_embedding_lookup": (C.c_int, [_P, _P, _I64, _I32, _I64, _P, _I64, _I32, _I32, _P]),
+    "eu_sparse_embedding_lookup_backward": (C.c_int, [_P, _P, _P, _I64, _I32, _I64, _I64, _I32, _I32, _P]),
     "eu_gather_host": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P]),
     "eu_scatter_add_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),
     "eu_scatter_max_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),

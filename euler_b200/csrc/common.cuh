@@ -109,6 +109,15 @@ __device__ __forceinline__ int64_t lookup_row(const DevGraph& g, unsigned long l
   }
 }
 
+// Row `row`'s slice of ragged slot `fid` (ptr of S slots per row): [b, e) in the value array, b == e when the node / slot does
+// not exist
+__device__ __forceinline__ void ragged_slice(const int64_t* __restrict__ ptr, int32_t S, int64_t row, int32_t fid, int64_t* b, int64_t* e) {
+  *b = *e = 0;
+  if (row < 0 || fid < 0 || fid >= S || !ptr) return;
+  *b = ptr[row * S + fid];
+  *e = ptr[row * S + fid + 1];
+}
+
 // ---------------------------------------------------------------------------------- minstd_rand0
 static constexpr uint32_t kM = 2147483647u;  // 2^31-1
 static constexpr uint32_t kA = 16807u;

@@ -13,14 +13,6 @@
 
 namespace eu {
 
-// row slice of slot `fid`: [b, e) in the value array, b == e when the node / slot does not exist
-__device__ __forceinline__ void ragged_slice(const int64_t* __restrict__ ptr, int32_t S, int64_t row, int32_t fid, int64_t* b, int64_t* e) {
-  *b = *e = 0;
-  if (row < 0 || fid < 0 || fid >= S || !ptr) return;
-  *b = ptr[row * S + fid];
-  *e = ptr[row * S + fid + 1];
-}
-
 template <bool SPARSE>
 __global__ void k_ragged_len(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t M, int32_t fid,
                              long long* __restrict__ out_ptr) {
@@ -57,6 +49,28 @@ __global__ void __launch_bounds__(256) k_ragged_fill(DevGraph g, const unsigned 
   }
 }
 
+size_t ragged_scan_bytes(int64_t M) {
+  size_t tmp = 0;
+  cub::DeviceScan::InclusiveSum((void*)nullptr, tmp, (long long*)nullptr, (long long*)nullptr, (int)(M + 1));
+  return tmp;
+}
+
+// out_ptr [M + 1] = the entry offsets of the nodes (lengths, then an inclusive scan in the scratch tmp)
+template <bool SPARSE>
+static int ragged_ptr(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, void* tmp, size_t tmp_bytes, int64_t* out_ptr) {
+  cudaStream_t s = c->stream;
+  k_ragged_len<SPARSE><<<(unsigned)ceil_div(std::max<int64_t>(M, 1), 256), 256, 0, s>>>(c->g->d, (const unsigned long long*)nodes, M, fid,
+                                                                                        (long long*)out_ptr);
+  EU_LAUNCHED();
+  EU_CUDA(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, (long long*)out_ptr, (long long*)out_ptr, (int)(M + 1), s));
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+int sparse_entry_ptr(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, void* tmp, size_t tmp_bytes, int64_t* out_ptr) {
+  return ragged_ptr<true>(c, nodes, M, fid, tmp, tmp_bytes, out_ptr);
+}
+
 template <bool SPARSE>
 static int ragged_get(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, int64_t cap, int64_t* out_ptr,
                       int64_t* out_values, uint8_t* out_bytes, const char* what) {
@@ -68,14 +82,10 @@ static int ragged_get(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, i
   if (M >= ((int64_t)1 << 31)) { set_error("%s: more than 2^31 nodes", what); return EU_ERR_UNSUPPORTED; }
   const DevGraph& d = c->g->d;
   cudaStream_t s = c->stream;
-  size_t tmp = 0;
-  cub::DeviceScan::InclusiveSum((void*)nullptr, tmp, (long long*)nullptr, (long long*)nullptr, (int)(M + 1), s);
+  const size_t tmp = ragged_scan_bytes(M);
   int rc = ctx_misc(c, (int64_t)tmp + 256);
   if (rc) return rc;
-  k_ragged_len<SPARSE><<<(unsigned)ceil_div(std::max<int64_t>(M, 1), 256), 256, 0, s>>>(d, (const unsigned long long*)nodes, M, fid, (long long*)out_ptr);
-  EU_LAUNCHED();
-  EU_CUDA(cub::DeviceScan::InclusiveSum(c->d_misc, tmp, (long long*)out_ptr, (long long*)out_ptr, (int)(M + 1), s));
-  EU_LAUNCHED();
+  if ((rc = ragged_ptr<SPARSE>(c, nodes, M, fid, c->d_misc, tmp, out_ptr))) return rc;
   if (cap > 0 && M > 0) {
     const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(M * 32, 256), kSMs * 8);
     k_ragged_fill<SPARSE><<<blocks, 256, 0, s>>>(d, (const unsigned long long*)nodes, M, fid, (long long)default_value, (const long long*)out_ptr, cap,

@@ -420,6 +420,11 @@ int eu_graph_create(const eu_graph_desc* desc, int device, eu_graph** out) {
     TRY(upload(g, &d.u64_ptr, desc->u64_ptr, n * S + 1));
     TRY(upload(g, (const uint64_t**)&d.u64_val, desc->u64_val, desc->u64_ptr[n * S]));
     for (int64_t k = 0; k < S; ++k) g->sparse_feature_names.push_back("u64_" + std::to_string(k));
+    g->u64_slot_max.assign(S, 0);
+    for (int64_t r = 0; r < n; ++r)
+      for (int64_t k = 0; k < S; ++k)
+        for (int64_t j = desc->u64_ptr[r * S + k]; j < desc->u64_ptr[r * S + k + 1]; ++j)
+          g->u64_slot_max[k] = std::max<uint64_t>(g->u64_slot_max[k], desc->u64_val[j]);
   }
   if (desc->n_bin_slots > 0 && desc->bin_ptr) {
     const int64_t S = desc->n_bin_slots;

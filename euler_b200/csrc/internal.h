@@ -69,6 +69,7 @@ struct eu_graph {
   std::vector<std::string> edge_type_names, node_type_names;
   std::vector<std::string> dense_feature_names;  // per slot, without the "dense_" prefix
   std::vector<std::string> sparse_feature_names, binary_feature_names;   // per slot, without the "sparse_" / "binary_" prefix
+  std::vector<uint64_t> u64_slot_max;  // per uint64 slot: its largest value (0 when it has none); bounds embedding lookups
   // edges (eu_graph_set_edges): device store, per-type alias samplers in edge_map_ order, feature names
   eu::DevEdges e{};
   bool edges_set = false;
@@ -186,6 +187,10 @@ struct EdgeOrder;   // segment.cuh
 // edge order (k_gat_bwd_src, H = 1); a segment without edges gets a zero row
 int segmented_row_sum(eu_ctx* c, const float* rows, const float* w, const EdgeOrder& o, const int32_t* row, int64_t E, int64_t n,
                       int dim, float* out);
+// features.cu: ptr i64[M + 1] = the entry offsets of get_sparse_feature's CSR over slot fid (a node without values counts one
+// default entry), with tmp (>= ragged_scan_bytes(M) bytes) as the scan scratch; no host synchronisation
+size_t ragged_scan_bytes(int64_t M);
+int sparse_entry_ptr(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, void* tmp, size_t tmp_bytes, int64_t* ptr);
 int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
 int graph_build_sampler(eu_graph* g);

@@ -737,6 +737,15 @@ static Geom make_geom(int nb, int64_t rows_b) {
   return gm;
 }
 
+// stats[0] = ptr[rows] (the entries of a CSR over `rows` rows), stats[1] = its longest row; stats zeroed by the caller
+__global__ void k_ragged_stats(const long long* __restrict__ ptr, int64_t rows, long long* __restrict__ stats) {
+  long long mx = 0;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows; i += (int64_t)gridDim.x * blockDim.x)
+    mx = max(mx, __ldg(ptr + i + 1) - __ldg(ptr + i));
+  if (mx > 0) atomicMax(stats + 1, mx);
+  if (blockIdx.x == 0 && threadIdx.x == 0) stats[0] = __ldg(ptr + rows);
+}
+
 // scratch needed by a hop over nb batches of rows_b seeds (see ctx_reserve)
 int64_t hop_scratch_rows(int nb, int64_t rows_b) { return make_geom(nb, rows_b).rows_pad * nb; }
 int64_t hop_table_slots(int nb, int64_t rows_b) { return (make_geom(nb, rows_b).cap_b + 1) * nb; }
@@ -906,6 +915,67 @@ int eu_sample_fanout(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* 
                      const int32_t* counts, int32_t L, int64_t default_node, int64_t* const* out_ids,
                      float* const* out_w, int32_t* const* out_t) {
   return eu_sample_fanout_batched(c, nodes, 1, B, etypes, K, counts, L, default_node, out_ids, out_w, out_t);
+}
+
+int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K, const int32_t* counts,
+                                  int32_t L, int64_t default_node, int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t,
+                                  int64_t* const* eng_ids, int32_t n_dense, const int32_t* dense_fids, const int32_t* dense_dims,
+                                  float* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids, int64_t* const* sparse_ptr,
+                                  int64_t* sparse_total, int64_t* sparse_max_len) {
+  const char* who = "eu_sample_fanout_with_feature";
+  if (!c || B < 0 || L < 0 || (L > 0 && (!counts || !out_ids || !out_w || !out_t || !eng_ids)) || (K > 0 && !etypes) || n_dense < 0 ||
+      n_sparse < 0 || (n_dense > 0 && (!dense_fids || !dense_dims || !out_dense)) ||
+      (n_sparse > 0 && (!sparse_fids || !sparse_ptr || !sparse_total || !sparse_max_len))) {
+    set_error("%s: bad argument", who);
+    return EU_ERR_INVALID;
+  }
+  for (int l = 0; l < L; ++l)
+    if (counts[l] < 1) { set_error("%s: counts must be positive", who); return EU_ERR_INVALID; }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  std::vector<int64_t> rows(L + 1, B);
+  for (int l = 0; l < L; ++l) rows[l + 1] = rows[l] * counts[l];
+  // stats (total, longest row) of every ragged output | the scan scratch of the widest hop; sized before anything is enqueued
+  const int NS = (L + 1) * n_sparse;
+  const size_t tmp = ragged_scan_bytes(rows[L]), o_tmp = a256(16 * (size_t)std::max(NS, 1));
+  int rc = n_sparse > 0 ? ctx_misc(c, (int64_t)(o_tmp + tmp)) : EU_OK;
+  if (rc) return rc;
+  // the hops of eu_sample_fanout, with every hop's engine ids kept in the caller's buffers rather than the ctx frontier
+  if (B > 0 && L > 0) {
+    int64_t max_rows = hop_scratch_rows(1, B), max_slots = hop_table_slots(1, B);
+    for (int l = 0; l + 1 < L; ++l) {
+      max_rows = std::max(max_rows, hop_scratch_rows(1, rows[l + 1]));
+      max_slots = std::max(max_slots, hop_table_slots(1, rows[l + 1]));
+    }
+    if ((rc = ctx_reserve(c, std::max(max_rows, rows[L]), max_slots))) return rc;
+    const unsigned long long* seeds = (const unsigned long long*)nodes;
+    for (int l = 0; l < L; ++l) {
+      unsigned long long* eng = (unsigned long long*)eng_ids[l];
+      rc = hop(c, seeds, rows[l], etypes + (int64_t)l * K, K, counts[l], default_node, eng, out_ids[l], out_w[l], out_t[l], l,
+               /*pre_inserted=*/l > 0 && c->rng == EU_RNG_MINSTD, /*insert_next=*/l + 1 < L, 1);
+      if (rc) return rc;
+      seeds = eng;
+    }
+  }
+  // the features of hop l are those of its engine ids (hop 0: the nodes themselves)
+  char* m = (char*)c->d_misc;
+  if (n_sparse > 0) EU_CUDA(cudaMemsetAsync(m, 0, 16 * (size_t)NS, c->stream));
+  for (int l = 0; l <= L; ++l) {
+    const int64_t* ids = l == 0 ? nodes : eng_ids[l - 1];
+    for (int j = 0; j < n_dense; ++j)
+      if ((rc = eu_get_dense_feature(c, ids, rows[l], dense_fids[j], dense_dims[j], out_dense[l * n_dense + j]))) return rc;
+    for (int j = 0; j < n_sparse; ++j) {
+      const int k = l * n_sparse + j;
+      if ((rc = sparse_entry_ptr(c, ids, rows[l], sparse_fids[j], m + o_tmp, tmp, sparse_ptr[k]))) return rc;
+      k_ragged_stats<<<(unsigned)std::min<int64_t>(ceil_div(rows[l] + 1, 256), kSMs * 8), 256, 0, c->stream>>>((const long long*)sparse_ptr[k], rows[l], (long long*)m + 2 * k);
+      EU_LAUNCHED();
+    }
+  }
+  if (n_sparse == 0) return EU_OK;
+  std::vector<int64_t> st(2 * (size_t)NS);   // the one host synchronisation: every ragged total and longest row together
+  EU_CUDA(cudaMemcpyAsync(st.data(), m, 16 * (size_t)NS, cudaMemcpyDeviceToHost, c->stream));
+  EU_CUDA(cudaStreamSynchronize(c->stream));
+  for (int k = 0; k < NS; ++k) { sparse_total[k] = st[2 * k]; sparse_max_len[k] = st[2 * k + 1]; }
+  return EU_OK;
 }
 
 int eu_sample_node(eu_ctx* c, int32_t count, const int32_t* types, int32_t n_types, int64_t* out) {

@@ -133,4 +133,73 @@ int plan_segments(eu_ctx* c, const EdgeOrder& o, int64_t E, int64_t n, char* buf
   return seg_chunk_offsets(c, S->start, n, kSegChunk, nc, buf + 3 * n1, scan, S->chunk_off);
 }
 
+// head[k] = 1 where position k of the sorted keys starts a distinct key
+__global__ void k_distinct_heads(const int32_t* __restrict__ key, int64_t E, int32_t* __restrict__ head) {
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < E; k += (int64_t)gridDim.x * blockDim.x)
+    head[k] = k == 0 || __ldg(key + k) != __ldg(key + k - 1);
+}
+
+// From sid (the inclusive scan of the heads): each distinct key's first position and value, and start[s] = E for s in [D, E]
+__global__ void k_distinct_starts(const int32_t* __restrict__ key, const int32_t* __restrict__ sid, int64_t E,
+                                  int32_t* __restrict__ skey, int32_t* __restrict__ start) {
+  const int64_t D = __ldg(sid + E - 1);
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t <= E; t += (int64_t)gridDim.x * blockDim.x) {
+    if (t < E && (t == 0 || __ldg(key + t) != __ldg(key + t - 1))) {
+      const int32_t s = __ldg(sid + t) - 1;
+      start[s] = (int32_t)t;
+      skey[s] = __ldg(key + t);
+    }
+    if (t >= D) start[t] = (int32_t)E;
+  }
+}
+
+// mc[s] = the chunks of segment s when it has several, else 0 (an exclusive scan then gives part_off)
+__global__ void k_seg_multi(const int32_t* __restrict__ chunk_off, int64_t n, int32_t* __restrict__ mc) {
+  for (int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; s <= n; s += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t k = s < n ? __ldg(chunk_off + s + 1) - __ldg(chunk_off + s) : 0;
+    mc[s] = k > 1 ? k : 0;
+  }
+}
+
+static size_t distinct_scan_bytes(int64_t E) {
+  size_t t = 0;
+  cub::DeviceScan::InclusiveSum(nullptr, t, (const int32_t*)nullptr, (int32_t*)nullptr, (int)E);
+  return std::max(t, seg_scan_bytes(E));
+}
+
+size_t distinct_plan_bytes(int64_t E, int64_t width) {
+  return 6 * a256(4 * (size_t)(E + 1)) + a256(distinct_scan_bytes(E)) + a256(4 * (size_t)(2 * E / kSegChunk + 1) * width);
+}
+
+int plan_distinct(eu_ctx* c, const EdgeOrder& o, int64_t E, char* buf, DistinctPlan* P) {
+  cudaStream_t s = c->stream;
+  const size_t n1 = a256(4 * (size_t)(E + 1)), scan = distinct_scan_bytes(E);
+  int32_t* sid = (int32_t*)buf;
+  P->E = E;
+  P->part_rows = 2 * E / kSegChunk + 1;
+  P->nd = sid + E - 1;
+  P->key = (int32_t*)(buf + n1);
+  P->start = (int32_t*)(buf + 2 * n1);
+  int32_t* nc = (int32_t*)(buf + 3 * n1);
+  P->chunk_off = (int32_t*)(buf + 4 * n1);
+  P->part_off = (int32_t*)(buf + 5 * n1);
+  void* tmp = buf + 6 * n1;
+  P->partial = (float*)(buf + 6 * n1 + a256(scan));
+  k_distinct_heads<<<stride_grid(E), 256, 0, s>>>(o.key, E, sid);
+  EU_LAUNCHED();
+  size_t t = scan;
+  EU_CUDA(cub::DeviceScan::InclusiveSum(tmp, t, sid, sid, (int)E, s));
+  EU_LAUNCHED();
+  k_distinct_starts<<<stride_grid(E + 1), 256, 0, s>>>(o.key, sid, E, P->key, P->start);
+  EU_LAUNCHED();
+  int rc = seg_chunk_offsets(c, P->start, E, kSegChunk, nc, tmp, scan, P->chunk_off);
+  if (rc) return rc;
+  k_seg_multi<<<stride_grid(E + 1), 256, 0, s>>>(P->chunk_off, E, nc);
+  EU_LAUNCHED();
+  t = scan;
+  EU_CUDA(cub::DeviceScan::ExclusiveSum(tmp, t, nc, P->part_off, (int)(E + 1), s));
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
 }  // namespace eu

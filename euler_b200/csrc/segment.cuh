@@ -117,4 +117,20 @@ size_t seg_plan_bytes(int64_t E, int64_t n, int64_t width);
 // the segment starts and chunk offsets of the order o of E > 0 edges over n segments, in buf
 int plan_segments(eu_ctx* c, const EdgeOrder& o, int64_t E, int64_t n, char* buf, SegPlan* S);
 
+// The segments of the DISTINCT keys of an order of E > 0 positions, for keys drawn from a range too large to plan over (an
+// embedding table's rows): segment s < D is the s-th distinct key, D (<= E) stays on the device, so planning needs no host
+// synchronisation and its scratch is O(E) whatever the key range.  Arrays of E + 1 entries cover the worst case D = E:
+// segments s >= D are empty (start[s] = E, no chunks).  Chunk sums of the segments of several chunks go to
+// partial[part_off[s] + (c - chunk_off[s])]: fewer than 2E / kSegChunk + 1 rows, since such a segment of len positions has
+// ceil(len / K) < 2 len / K chunks.  Scratch of distinct_plan_bytes(E, width) bytes:
+//   sid [E] | key, start, nc, chunk_off, part_off [E + 1] each | scan temp | partial [part_rows, width]
+struct DistinctPlan {
+  int64_t E = 0, part_rows = 0;
+  const int32_t* nd = nullptr;   // device: D
+  int32_t *key = nullptr, *start = nullptr, *chunk_off = nullptr, *part_off = nullptr;
+  float* partial = nullptr;
+};
+size_t distinct_plan_bytes(int64_t E, int64_t width);
+int plan_distinct(eu_ctx* c, const EdgeOrder& o, int64_t E, char* buf, DistinctPlan* P);
+
 }  // namespace eu

@@ -171,6 +171,67 @@ def sample_fanout(nodes, edge_types, counts, default_node=-1):
     return [nodes] + ids, ws, ts
 
 
+def sample_fanout_with_feature(nodes, edge_types, count, default_node, dense_feature_names, dense_dimensions,
+                               sparse_feature_names, sparse_default_values):
+    """neighbor_ops.sample_fanout_with_feature (neighbor_ops.py:49-69; kernel sample_fanout_with_feature_op.cc).  The hops are
+    sample_fanout's (the same draws on the same context state); the features of hop i are those of its engine ids, as the
+    reference's v_select(nb_i) takes them (a row whose first draw is node 0 is packed as default_node but keeps the features of
+    its draws).  Returns, as the reference's wrapper does:
+        neighbors        [nodes] + L flattened hops
+        weights, types   L tensors shaped [B, c1, ..., ci]
+        dense_features   (L+1) * len(dense_feature_names) tensors f32[rows_i, dim], hop-major
+        sparse_features  (L+1) * len(sparse_feature_names) (indices, values, dense_shape) triples, hop-major, as get_sparse_feature
+    One host synchronisation per call when sparse features are asked for (all ragged totals together), none otherwise."""
+    g, lib = get_graph(), _lib.load()
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    L = len(count)
+    ets = [get_edge_type_id(e) for e in edge_types]
+    if len(ets) != L or any(len(e) != len(ets[0]) for e in ets):
+        raise EulerError("sample_fanout_with_feature: edge_types must hold one equal-length type list per hop")
+    if len(dense_feature_names) != len(dense_dimensions) or len(sparse_feature_names) != len(sparse_default_values):
+        raise EulerError("sample_fanout_with_feature: one dimension per dense feature and one default per sparse feature")
+    et = np.ascontiguousarray(np.stack(ets) if L else np.zeros((0, 0)), dtype=np.int32)
+    cs = np.ascontiguousarray(count, dtype=np.int32)
+    B, dev = nodes.numel(), nodes.device
+    shapes, rows = [], [B]
+    for c in count:
+        shapes.append((shapes[-1] if shapes else (B,)) + (int(c),))
+        rows.append(rows[-1] * int(c))
+    ids = [torch.empty(r, dtype=torch.int64, device=dev) for r in rows[1:]]
+    eng = [torch.empty(r, dtype=torch.int64, device=dev) for r in rows[1:]]
+    ws = [torch.empty(sh, dtype=torch.float32, device=dev) for sh in shapes]
+    ts = [torch.empty(sh, dtype=torch.int32, device=dev) for sh in shapes]
+    dfid = np.asarray([n if isinstance(n, (int, np.integer)) else g.dense_feature_id(str(n)) for n in dense_feature_names], np.int32)
+    ddim = np.asarray(dense_dimensions, np.int32)
+    sfid = np.asarray([g.sparse_feature_id(str(n)) for n in sparse_feature_names], np.int32)
+    nd, ns = len(dfid), len(sfid)
+    dense = [torch.empty((rows[l], int(ddim[j])), dtype=torch.float32, device=dev) for l in range(L + 1) for j in range(nd)]
+    ptrs = [torch.empty(rows[l] + 1, dtype=torch.int64, device=dev) for l in range(L + 1) for j in range(ns)]
+    total, maxlen = np.zeros(max(len(ptrs), 1), np.int64), np.zeros(max(len(ptrs), 1), np.int64)
+
+    def P(ts_):
+        return (C.c_void_p * max(len(ts_), 1))(*[t.data_ptr() for t in ts_])
+    ctx = _ctx_on_stream()
+    check(lib.eu_sample_fanout_with_feature(ctx._h, nodes.data_ptr(), B, et.ctypes.data, et.shape[1] if L else 0, cs.ctypes.data, L,
+                                            default_node, P(ids), P(ws), P(ts), P(eng), nd, dfid.ctypes.data, ddim.ctypes.data,
+                                            P(dense), ns, sfid.ctypes.data, P(ptrs), total.ctypes.data, maxlen.ctypes.data))
+    sparse = []
+    for l in range(L + 1):
+        hop_ids = nodes if l == 0 else eng[l - 1]
+        for j in range(ns):
+            k = l * ns + j
+            ptr, tot, dv = ptrs[k], int(total[k]), int(sparse_default_values[j])
+            vals = torch.empty(tot, dtype=torch.int64, device=dev)
+            if tot:
+                check(lib.eu_get_sparse_feature(ctx._h, hop_ids.data_ptr(), rows[l], int(sfid[j]), dv, tot, ptr.data_ptr(),
+                                                vals.data_ptr()))
+            lens = ptr[1:] - ptr[:-1]
+            r = torch.repeat_interleave(torch.arange(rows[l], device=dev), lens, output_size=tot)
+            cols = torch.arange(tot, device=dev) - ptr[:-1][r]
+            sparse.append((torch.stack([r, cols], dim=1), vals, (rows[l], int(maxlen[k]))))
+    return [nodes] + ids, ws, ts, dense, sparse
+
+
 def sample_fanout_batched(nodes, edge_types, counts, default_node=-1, ctx=None):
     """nb independent sample_fanout calls in one set of kernel launches.  nodes: [nb, B]; batch b runs on engine b
     of `ctx` (Context.set_engines), i.e. it returns exactly what sample_fanout(nodes[b]) returns on a context
@@ -1037,3 +1098,57 @@ def dna_attention_aggregate(q, k, v, n0, n1, edge_index, size, heads):
     q, k, v = (_t(t, torch.float32) for t in (q, k, v))
     n0, n1 = (_t(t, torch.float32).detach().reshape(-1) for t in (n0, n1))
     return _DnaAggregate.apply(q, k, v, n0, n1, dst, src, n_dst, heads)
+
+
+_COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
+
+
+def _raw_embedding(nodes, fid, table, default_value, comb):
+    """one eu_sparse_embedding_lookup: out f32[M, dim]"""
+    n_rows, dim = table.shape
+    out = torch.empty((nodes.numel(), dim), dtype=torch.float32, device=table.device)
+    ctx = _ctx_on_stream()
+    check(_lib.load().eu_sparse_embedding_lookup(ctx._h, nodes.data_ptr(), nodes.numel(), fid, default_value, table.data_ptr(), n_rows,
+                                                 dim, comb, out.data_ptr()))
+    return out
+
+
+class _SparseEmbedding(torch.autograd.Function):
+    """eu_sparse_embedding_lookup / eu_sparse_embedding_lookup_backward.  Saves only the node ids: the backward pass lists the
+    entries again from the graph."""
+
+    @staticmethod
+    def forward(ctx, table, nodes, fid, default_value, comb):
+        out = _raw_embedding(nodes, fid, table, default_value, comb)
+        if ctx.needs_input_grad[0]:
+            ctx.save_for_backward(nodes)
+        ctx.args = (fid, default_value, comb, table.shape)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        nodes, = ctx.saved_tensors
+        fid, default_value, comb, (n_rows, dim) = ctx.args
+        grad = grad.contiguous()
+        g_t = torch.empty((n_rows, dim), dtype=torch.float32, device=grad.device)
+        ec = _ctx_on_stream()
+        check(_lib.load().eu_sparse_embedding_lookup_backward(ec._h, grad.data_ptr(), nodes.data_ptr(), nodes.numel(), fid, default_value,
+                                                              n_rows, dim, comb, g_t.data_ptr()))
+        return g_t, None, None, None, None
+
+
+def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner='sum'):
+    """SparseEmbedding over get_sparse_feature in one fused device op: row i is tf.nn.embedding_lookup_sparse(table, sp_ids,
+    None, combiner) (layers.py:152-169) of the SparseTensor get_sparse_feature(nodes, [feature_name], [default_value]) returns,
+    i.e. the rows of table f32[n_rows, dim] named by node i's uint64 values of the slot, in stored order, or the one row
+    default_value for a node without values; combined by 'sum', 'mean' or 'sqrtn'.  The sum runs left to right from the first
+    row, mean / sqrtn divide once (include/euler_b200.h).  Every value of the slot and default_value must lie in [0, n_rows):
+    the call raises otherwise, before any device work.  The gradient reaches table only (deterministic, no atomics); the
+    forward does not synchronise, the backward synchronises once."""
+    if combiner not in _COMBINERS:
+        raise EulerError("sparse_feature_embedding: combiner must be one of %s, got %r" % (sorted(_COMBINERS), combiner))
+    if not torch.is_tensor(table) or table.dtype != torch.float32 or table.dim() != 2:
+        raise EulerError("sparse_feature_embedding: table must be a 2-D float32 tensor")
+    fid = feature_name if isinstance(feature_name, (int, np.integer)) else get_graph().sparse_feature_id(str(feature_name))
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    return _SparseEmbedding.apply(_t(table, torch.float32), nodes, int(fid), int(default_value), _COMBINERS[combiner])

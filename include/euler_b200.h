@@ -222,6 +222,24 @@ int eu_sample_fanout_host(eu_ctx* c, const int64_t* nodes, int64_t B, const int3
 int eu_sample_fanout_batched_host(eu_ctx* c, const int64_t* nodes, int32_t nb, int64_t B, const int32_t* etypes,
                                   int32_t K, const int32_t* counts, int32_t L, int64_t default_node,
                                   int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t);
+/* tf_euler.sample_fanout_with_feature -- TF op SampleFanoutWithFeature (tf_euler/kernels/sample_fanout_with_feature_op.cc:95-275,
+ * wrapper neighbor_ops.py:49-69): eu_sample_fanout's hops -- the same draws, outputs and draw count on the same ctx state --
+ * followed by the features of every hop.  counts i32[L] >= 1 (host).  out_ids / out_w / out_t[l] as eu_sample_fanout
+ * (B*prod(counts[0..l]) elements, TF-packed); eng_ids[l] i64[same] receives hop l's ENGINE ids (0 = DEFAULT_UINT64 where a row
+ * was filled), from which the features are taken as the reference's v_select(nb_l) does: a row whose first draw is node 0 is
+ * packed as default_node but has the features of its real draws.  Hop 0's features are those of `nodes`.  Hop-major, hop l
+ * and feature j at index l * n + j of the (L+1) * n outputs:
+ *   out_dense   f32[rows_l, dense_dims[j]]   eu_get_dense_feature of slot dense_fids[j]
+ *   sparse_ptr  i64[rows_l + 1]              eu_get_sparse_feature's offsets of slot sparse_fids[j] (one default entry per node
+ *                                            without values); sparse_total / sparse_max_len (HOST) its entry count and longest row
+ * The values are then written by eu_get_sparse_feature(c, ids_l, rows_l, fid, default, sparse_total[k], sparse_ptr[k], values)
+ * with ids_l = nodes or eng_ids[l - 1] (no synchronisation).  Device pointers except the lists and the host arrays; the call
+ * synchronises the stream once when n_sparse > 0 (every total and longest row together), never otherwise. */
+int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K, const int32_t* counts,
+                                  int32_t L, int64_t default_node, int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t,
+                                  int64_t* const* eng_ids, int32_t n_dense, const int32_t* dense_fids, const int32_t* dense_dims,
+                                  float* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids, int64_t* const* sparse_ptr,
+                                  int64_t* sparse_total, int64_t* sparse_max_len);
 /* tf_euler.sample_node -- TF op SampleNode (tf_euler/ops/sample_ops.cc:22-37, kernel
  * tf_euler/kernels/sample_node_op.cc:39-96; euler::SampleNode api.cc:32-37).  types i32[n_types]
  * (host); a single -1 means all types.  out i64[count]. */
@@ -257,6 +275,27 @@ int eu_get_sparse_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32
 int eu_get_binary_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t cap, int64_t* out_ptr, uint8_t* out_bytes);
 int eu_get_binary_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t cap, int64_t* out_ptr,
                                uint8_t* out_bytes, int64_t* total);
+/* SparseEmbedding's lookup from node ids (tf_euler/python/utils/layers.py:152-169: tf.nn.embedding_lookup_sparse(table, sp_ids,
+ * None, combiner) over the SparseTensor of get_sparse_feature), fused: row i of out f32[M, dim] combines the rows of
+ * table f32[n_rows, dim] named by node i's bag, the uint64 values of slot fid in stored order -- or the single entry
+ * default_value when the node has none (absent id, empty or unknown slot), exactly as eu_get_sparse_feature lists them.
+ * Fixed order: the sum starts from the bag's first row (a one-entry bag is that row's bits, -0.0 and NaN payloads included)
+ * and adds the others left to right, one rounded add each; mean divides once by fl(n), sqrtn once by sqrtf(fl(n)).  Nothing is
+ * materialised between the node ids and out; no synchronisation: capturable in a CUDA graph.
+ * The backward pass writes grad_table f32[n_rows, dim] (zeros where no entry points): for value v, the sum over the entries
+ * with value v of grad_out[i] (sum), grad_out[i] / fl(n_i) (mean) or grad_out[i] / sqrtf(fl(n_i)) (sqrtn), elementwise.  The
+ * entries are listed again from the graph and ordered stably by value; each distinct value's entries are summed in chunks of
+ * 256 counted from its first entry, each chunk left to right from +0, then the chunk sums in chunk order: deterministic, no
+ * atomics.  It synchronises the stream once (to read the entry count E) and uses the ctx scratch: 8 B per node, about 24 B
+ * per entry plus cub's sort storage, and (2E/256 + 1) * dim floats of chunk sums -- never O(n_rows) of index data.
+ * combiner outside eu_combiner, n_rows or dim < 1, M < 0, a NULL pointer that is needed, default_value outside [0, n_rows),
+ * or a slot whose largest value (kept on the graph since its creation) is >= n_rows: EU_ERR_INVALID, before any device work.
+ * M or n_rows >= 2^31, or 2^31 or more entries in the backward: EU_ERR_UNSUPPORTED.  Device pointers. */
+typedef enum { EU_COMBINE_SUM = 0, EU_COMBINE_MEAN = 1, EU_COMBINE_SQRTN = 2 } eu_combiner;
+int eu_sparse_embedding_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const float* table,
+                               int64_t n_rows, int32_t dim, int32_t combiner, float* out);
+int eu_sparse_embedding_lookup_backward(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
+                                        int64_t default_value, int64_t n_rows, int32_t dim, int32_t combiner, float* grad_table);
 
 /* tf_euler.sample_edge -- TF op SampleEdge (tf_euler/kernels/sample_edge_op.cc; Graph::SampleEdge graph.cc:277-301): `count`
  * edges of ONE type drawn by the alias method over the edge weights, out i64[count,3] = (src, dst, type).  Several types or
