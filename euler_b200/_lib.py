@@ -147,6 +147,13 @@ SIGNATURES = {
     "eu_sym_sample_hop_batched": (C.c_int, [_P, _P, _I32, _I64, _P, _I32, _I32, _I64, _I32, _I32]),
     "eu_sym_get_dense_feature": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32]),
     "eu_sym_sage_mean": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32, _P]),
+    "eu_graph_set_binary_feature_name": (C.c_int, [_P, _I32, C.c_char_p]),
+    "eu_graph_labels": (C.c_int, [_P, _I64, _P, _P, _P, _P]),
+    "eu_graph_labels_inspect": (C.c_int, [C.c_char_p, _I64, _P, _P, _P, _P]),
+    "eu_sample_graph_label": (C.c_int, [_P, _I32, _P]),
+    "eu_get_graph_by_label": (C.c_int, [_P, _P, _I64, _I64, _P, _P, _P, _P, _P]),
+    "eu_graph_attention_readout": (C.c_int, [_P, _P, _P, _I64, _I64, _I32, _P, _P, _P, _P]),
+    "eu_graph_attention_readout_backward": (C.c_int, [_P, _P, _P, _P, _I64, _I64, _I32, _P, _P, _P, _P, _P]),
     "InitQueryProxy": (C.c_bool, [C.c_char_p]),
     "eu_default_graph": (_P, []),
     "eu_default_ctx": (_P, []),

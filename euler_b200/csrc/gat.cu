@@ -259,7 +259,7 @@ __global__ void __launch_bounds__(256) k_gat_bwd_src(const float* __restrict__ g
   }
 }
 
-// G lanes per edge e (a power of two <= 32): dot[e] = <a[ia_e, :], b[ib_e, :]> over dim columns, and scaled[e] =
+// G lanes per edge e (a power of two <= 32): dot[e] = <a[ia_e, :], b[ib_e, :]> over dim columns (ia null: a[e, :]), and scaled[e] =
 // beta[0] * dot[e] when scaled is given.  The order is fixed: lane l accumulates, one __fmaf_rn at a time, the columns of
 // its 4-column chunks l, l + G, l + 2G, ..., each chunk left to right; then a butterfly over the G lanes, xor distances G/2,
 // ..., 1 (both lanes of a pair add the same two values, so every lane ends with the same bits).  VEC (dim % 4 == 0,
@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(256) k_agnn_dot(const float* __restrict__ a, c
   const int sub = (int)(tid & (G - 1));
   if (e >= E) return;   // group-uniform
   const unsigned gm = group_mask(G);
-  const float* ar = a + (int64_t)__ldg(ia + e) * dim;
+  const float* ar = a + (ia ? (int64_t)__ldg(ia + e) : e) * dim;
   const float* br = b + (int64_t)__ldg(ib + e) * dim;
   float acc = 0.f;
 #pragma unroll 4
@@ -354,7 +354,7 @@ __global__ void __launch_bounds__(kAgnnSumThreads) k_agnn_sum(const float* __res
 }
 
 // k_agnn_dot over E > 0 edges: dot[e] = <a[ia_e], b[ib_e]>, scaled[e] = beta * dot[e] (either output may be null)
-static int agnn_dot(eu_ctx* c, const float* a, const float* b, const int32_t* ia, const int32_t* ib, int64_t E, int dim,
+int agnn_dot(eu_ctx* c, const float* a, const float* b, const int32_t* ia, const int32_t* ib, int64_t E, int dim,
                     const float* beta, float* dot, float* scaled) {
   const bool vec = dim % 4 == 0 && aligned16(a) && aligned16(b);
   const int G = group_lanes(ceil_div(dim, 4));   // one lane per 4-column chunk, both paths: the same order

@@ -76,6 +76,12 @@ struct eu_graph {
   struct EdgeSampler { int64_t n = 0; const int64_t* order = nullptr; const float* prob = nullptr; const int32_t* alias = nullptr; float fwc_sum = 0.f; };
   std::vector<EdgeSampler> edge_samplers;
   std::vector<std::string> edge_dense_names, edge_sparse_names, edge_binary_names;
+  // graph-label table (graph_label.cu), built lazily by the first graph-label call: the label list in Graph::GetGraphLabel's
+  // order, and the rows of label l as the node ids [label_ptr[l], label_ptr[l + 1]) of label_ids, ascending
+  bool labels_built = false;
+  std::vector<std::string> labels;
+  int32_t* d_label_ptr = nullptr;                 // [L + 1]
+  unsigned long long* d_label_ids = nullptr;      // [label_ptr[L]]
 
   template <typename T>
   int alloc(T** p, int64_t count) {
@@ -194,6 +200,20 @@ int sparse_entry_ptr(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, vo
 int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
 int graph_build_sampler(eu_graph* g);
+int graph_build_labels(eu_graph* g);   // graph_label.cu: the label table (EU_ERR_STATE without a graph_label slot)
+// graph_label.cu: Graph::GetGraphLabel's list (graph.cc:439-457) from the binary slot `fid` (S slots per row) of the rows
+// visited in node_map_ order (`order`, empty = row order); row_label (may be null) gets each row's label index, or L for a
+// row without a value (the empty label lists no nodes)
+void graph_label_list(const std::vector<int64_t>& order, int64_t n, const int64_t* bin_ptr, const uint8_t* bin_val, int32_t S,
+                      int32_t fid, std::vector<std::string>* labels, std::vector<int32_t>* row_label);
+// sample.cu: the engine after `uniforms` draws of a plain op (both modes: the Philox salt advances too)
+__global__ void k_advance_engine(EuRngState* rng, unsigned long long uniforms);
+// sample.cu: stats[0] = ptr[rows], stats[1] = the longest row of the CSR ptr; stats zeroed by the caller
+__global__ void k_ragged_stats(const long long* __restrict__ ptr, int64_t rows, long long* __restrict__ stats);
+// gat.cu: dot[e] = <a[ia_e], b[ib_e]> in k_agnn_dot's fixed order over E > 0 pairs (ia null = the identity), scaled[e] =
+// beta * dot[e]; either output may be null
+int agnn_dot(eu_ctx* c, const float* a, const float* b, const int32_t* ia, const int32_t* ib, int64_t E, int dim,
+             const float* beta, float* dot, float* scaled);
 int get_node_weight(eu_ctx* c, const int64_t* nodes, int64_t B, float* out);   // neighbor.cu, for eu_get_node_weight_host
 int launch_state_scan(eu_ctx* c, int64_t rows, unsigned long long uniforms_per_row);
 // one sampleNB hop (sample.cu): seeds u64[rows] -> engine ids u64[rows*count] (0 placeholders, may be

@@ -251,6 +251,8 @@ struct LoadInspect {
   int32_t n_edge_types = 0, n_node_types = 0;
   std::vector<int64_t> order_ids;
   std::vector<int32_t> order_types;
+  bool has_labels = false;              // the graph has the binary slot graph_label
+  std::vector<std::string> labels;      // then Graph::GetGraphLabel's list
 };
 
 static int load_impl(const char* data_path, int shard_index, int shard_number, int device, int load_edges, eu_graph** out,
@@ -443,6 +445,11 @@ static int load_impl(const char* data_path, int shard_index, int shard_number, i
     inspect->n_edge_types = d.n_edge_types;
     inspect->n_node_types = d.n_node_types;
     for (int64_t r : order) { inspect->order_ids.push_back((int64_t)ids[r]); inspect->order_types.push_back(ntype[r]); }
+    for (auto& kv : binary)   // the device path's rule (graph_build_labels): the slot named graph_label once the prefix is stripped
+      if (kv.second == "binary_graph_label" || kv.second == "graph_label") {
+        inspect->has_labels = true;
+        graph_label_list(order, d.n_nodes, bin_ptr.data(), bin_all.data(), BS, kv.first, &inspect->labels, nullptr);
+      }
     return EU_OK;
   }
   int rc = eu_graph_create(&d, device, out);
@@ -490,6 +497,25 @@ extern "C" int eu_graph_load_inspect(const char* data_path, int shard_index, int
     if (order_ids) order_ids[i] = li.order_ids[i];
     if (order_types) order_types[i] = li.order_types[i];
   }
+  return EU_OK;
+}
+
+extern "C" int eu_graph_labels_inspect(const char* data_path, int64_t cap, int64_t* n_labels, int64_t* n_bytes, int64_t* ptr,
+                                       uint8_t* bytes) {
+  LoadInspect li;
+  const int rc = load_impl(data_path, 0, 1, 0, 0, nullptr, &li);
+  if (rc) return rc;
+  if (!li.has_labels || li.labels.empty()) { set_error("graph label set is empty! (%s has no binary feature graph_label)", data_path); return EU_ERR_STATE; }
+  int64_t total = 0;
+  if (ptr) ptr[0] = 0;
+  for (size_t l = 0; l < li.labels.size(); ++l) {
+    const std::string& v = li.labels[l];
+    if (bytes && total + (int64_t)v.size() <= cap) memcpy(bytes + total, v.data(), v.size());
+    total += (int64_t)v.size();
+    if (ptr) ptr[l + 1] = total;
+  }
+  if (n_labels) *n_labels = (int64_t)li.labels.size();
+  if (n_bytes) *n_bytes = total;
   return EU_OK;
 }
 

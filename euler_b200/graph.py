@@ -34,7 +34,9 @@ class Graph:
     def from_csr(cls, ids, grp_ptr, nbr, n_edge_types=1, cum_w=None, grp_cum=None, w=None,
                  node_type=None, node_w=None, n_node_types=1, feat=None, feat_slot_dims=None,
                  sampler_order=None, device=0, u64_ptr=None, u64_val=None, n_u64_slots=0, bin_ptr=None, bin_val=None,
-                 n_bin_slots=0):
+                 n_bin_slots=0, binary_feature_names=None):
+        """binary_feature_names: one name per binary slot (default bin_0, bin_1, ...); a slot named 'graph_label' holds each
+        node's graph label for sample_graph_label / get_graph_by_label."""
         ids = _np(ids, np.uint64)
         keep = [ids, _np(node_type, np.int32), _np(node_w, np.float32), _np(grp_ptr, np.int64),
                 _np(nbr, np.uint64), _np(cum_w, np.float32), _np(grp_cum, np.float32),
@@ -57,7 +59,10 @@ class Graph:
             d.n_bin_slots, d.bin_ptr, d.bin_val = int(n_bin_slots), _ptr(keep[13]), _ptr(keep[14] if len(keep[14]) else np.zeros(1, np.uint8))
         h = C.c_void_p()
         check(_lib.load().eu_graph_create(C.byref(d), device, C.byref(h)))
-        return cls(h, device)
+        g = cls(h, device)
+        for k, name in enumerate(binary_feature_names or ()):
+            check(_lib.load().eu_graph_set_binary_feature_name(h, k, str(name).encode()))
+        return g
 
     @classmethod
     def rmat(cls, n_nodes, n_edges, a=0.57, b=0.19, c=0.19, seed=42, feat_dim=0, feat_seed=7, device=0):

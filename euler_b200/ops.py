@@ -1152,3 +1152,127 @@ def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner
     fid = feature_name if isinstance(feature_name, (int, np.integer)) else get_graph().sparse_feature_id(str(feature_name))
     nodes = _t(nodes, torch.int64).reshape(-1)
     return _SparseEmbedding.apply(_t(table, torch.float32), nodes, int(fid), int(default_value), _COMBINERS[combiner])
+
+
+# ------------------------------------------------------------------------------------ graph-level minibatches
+def _labels_from(fn, *args):
+    """the label list a two-call entry point reports (counts, then offsets and bytes), as bytes"""
+    n, nb = C.c_int64(), C.c_int64()
+    check(fn(*args, 0, C.byref(n), C.byref(nb), None, None))
+    ptr = np.zeros(n.value + 1, np.int64)
+    buf = np.zeros(max(nb.value, 1), np.uint8)
+    check(fn(*args, nb.value, C.byref(n), C.byref(nb), ptr.ctypes.data, buf.ctypes.data))
+    raw = buf[:nb.value].tobytes()
+    return [raw[ptr[i]:ptr[i + 1]] for i in range(n.value)]
+
+
+def graph_labels():
+    """The graph's label list (Graph::GetGraphLabel, graph.cc:439-457) as bytes, in the reference's order: the values of the
+    binary slot 'graph_label', b'' included when a node has none.  Label indices (sample_graph_label) index this list."""
+    return _labels_from(_lib.load().eu_graph_labels, get_graph()._h)
+
+
+def inspect_graph_labels(data_path):
+    """The label list of an Euler directory, read on the host without a device (the same list and order as graph_labels)."""
+    return _labels_from(_lib.load().eu_graph_labels_inspect, str(data_path).encode())
+
+
+def sample_graph_label(count):
+    """sample_ops.sample_graph_label (kernel sample_graph_label_op.cc): i32[count] label indices into graph_labels(), drawn
+    uniformly from this thread's engine (the same stream position as the reference's ThreadLocalRandom under rng='minstd')."""
+    count = int(count)
+    out = torch.empty(count, dtype=torch.int32, device=_dev())
+    ctx = _ctx_on_stream()
+    check(_lib.load().eu_sample_graph_label(ctx._h, count, out.data_ptr()))
+    return out
+
+
+def get_graph_by_label(labels):
+    """sample_ops.get_graph_by_label (tf_euler/kernels/get_graph_by_label_op.cc).  labels: the label indices of
+    sample_graph_label (a tensor), or a sequence of label strings (mapped on the host; a label the graph does not know is -1).
+    Returns the reference's SparseTensor content as (indices i64[nnz, 2], values i64[nnz], dense_shape (B, max_len)): row i
+    lists the node ids of graph i in ascending order; an unknown label or one without nodes gets the single entry (i, 0) = 0."""
+    if not isinstance(labels, torch.Tensor):
+        index = {v: i for i, v in enumerate(graph_labels())}
+        labels = [index.get(v if isinstance(v, bytes) else str(v).encode(), -1) for v in labels]
+    labels = _t(labels, torch.int32).reshape(-1)
+    B = labels.numel()
+    lib, ctx = _lib.load(), _ctx_on_stream()
+    ptr = torch.empty(B + 1, dtype=torch.int64, device=labels.device)
+    total, max_len = C.c_int64(), C.c_int64()
+    check(lib.eu_get_graph_by_label(ctx._h, labels.data_ptr(), B, 0, ptr.data_ptr(), None, None, C.byref(total), C.byref(max_len)))
+    nnz = total.value
+    indices = torch.empty((nnz, 2), dtype=torch.int64, device=labels.device)
+    values = torch.empty(nnz, dtype=torch.int64, device=labels.device)
+    if nnz:
+        check(lib.eu_get_graph_by_label(ctx._h, labels.data_ptr(), B, nnz, ptr.data_ptr(), indices.data_ptr(), values.data_ptr(),
+                                        None, None))
+    return indices, values, (B, max_len.value)
+
+
+def _raw_readout(x, index, size, logits, q):
+    """one eu_graph_attention_readout: (out f32[size, D], alpha f32[N])"""
+    N, D = x.shape
+    out = torch.empty((size, D), dtype=torch.float32, device=x.device)
+    alpha = torch.empty(N, dtype=torch.float32, device=x.device)
+    ctx = _ctx_on_stream()
+    check(_lib.load().eu_graph_attention_readout(ctx._h, x.data_ptr(), index.data_ptr(), N, size, D,
+                                                 logits.data_ptr() if logits is not None else None,
+                                                 q.data_ptr() if q is not None else None, out.data_ptr(), alpha.data_ptr()))
+    return out, alpha
+
+
+class _GraphReadout(torch.autograd.Function):
+    """eu_graph_attention_readout / _backward.  Saves alpha [N], never an [N, D] temporary."""
+
+    @staticmethod
+    def forward(ctx, x, weight, index, size, by_query):
+        out, alpha = _raw_readout(x, index, size, None if by_query else weight, weight if by_query else None)
+        ctx.save_for_backward(x, weight, index, alpha)
+        ctx.size, ctx.by_query = size, by_query
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, weight, index, alpha = ctx.saved_tensors
+        N, D = x.shape
+        grad = grad.contiguous()
+        g_x = torch.empty_like(x)
+        g_w = torch.empty_like(weight)
+        q = weight if ctx.by_query else None
+        ec = _ctx_on_stream()
+        check(_lib.load().eu_graph_attention_readout_backward(ec._h, grad.data_ptr(), x.data_ptr(), index.data_ptr(), N, ctx.size,
+                                                              D, q.data_ptr() if q is not None else None, alpha.data_ptr(),
+                                                              g_x.data_ptr(), None if ctx.by_query else g_w.data_ptr(),
+                                                              g_w.data_ptr() if ctx.by_query else None))
+        return g_x, g_w, None, None, None
+
+
+def graph_attention_readout(x, index, size, logits=None, q=None):
+    """The attention readout of the graph pools in one fused device op (tf_euler/python/graph_pool/):
+        x f32[N, D]          the rows of every graph of the batch
+        index [N]            each row's graph, in [0, size)
+        logits f32[N] or [N, 1]   AttentionPool's gate, or
+        q f32[size, D]       Set2SetPool's query: the logit of row n is <x_n, q[index_n]>
+    out[b] = sum over the rows n of graph b of alpha_n * x_n, alpha = scatter_softmax of the logits over each graph; a graph
+    without rows gets a zero row.  The sums are fixed-order chunked sums (include/euler_b200.h): for graphs of at most 256 rows
+    and a non-decreasing index they equal scatter_softmax / scatter_add composed from the ops above bit for bit.  The backward
+    pass is deterministic.  Synchronises once per call (whether index is sorted); an unsorted one costs a radix sort."""
+    if (logits is None) == (q is None):
+        raise EulerError("graph_attention_readout: give exactly one of logits and q")
+    if not torch.is_tensor(x) or x.dim() != 2 or x.dtype != torch.float32:
+        raise EulerError("graph_attention_readout: x must be a 2-D float32 tensor")
+    size = int(size)
+    x = _f32(x)
+    index = _t(index, torch.int32).reshape(-1)
+    if index.numel() != x.shape[0]:
+        raise EulerError("graph_attention_readout: index has %d rows, x %d" % (index.numel(), x.shape[0]))
+    if q is not None:
+        w = _f32(q)
+        if tuple(w.shape) != (size, x.shape[1]):
+            raise EulerError("graph_attention_readout: q must be [size, D] = %s, got %s" % ((size, x.shape[1]), tuple(w.shape)))
+    else:
+        w = _t(logits, torch.float32).reshape(-1)
+        if w.numel() != x.shape[0]:
+            raise EulerError("graph_attention_readout: logits has %d rows, x %d" % (w.numel(), x.shape[0]))
+    return _GraphReadout.apply(x, w, index, size, q is not None)

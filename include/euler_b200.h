@@ -297,6 +297,61 @@ int eu_sparse_embedding_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32
 int eu_sparse_embedding_lookup_backward(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
                                         int64_t default_value, int64_t n_rows, int32_t dim, int32_t combiner, float* grad_table);
 
+/* Graph-level minibatches (graph classification; reference: euler/core/kernels/sample_graph_label_op.cc,
+ * get_graph_by_label_op.cc and Graph::GetGraphLabel, euler/core/graph/graph.cc:439-457).
+ * A graph's label table is built on the first graph-label call from its binary feature slot named "graph_label" (the
+ * reference's "binary_graph_label"; name a synthetic graph's slot with eu_graph_set_binary_feature_name before that call):
+ * the label list is GetGraphLabel's, in its order (an unordered_set of every node's value in node_map_ order, "" for a node
+ * without one), and each label's nodes are listed by ascending id (a chosen order: the reference's is its index file's).
+ * The label "" lists no nodes, as the converter indexes only the values present.  A graph without the slot or without nodes:
+ * every graph-label call returns EU_ERR_STATE ("graph label set is empty!", where the reference aborts).
+ * eu_graph_labels reports the list (builds the table: needs the device): n_labels, n_bytes, ptr i64[n_labels + 1] (host, may
+ * be NULL) and the concatenated bytes (host, written when n_bytes <= cap).  eu_graph_labels_inspect reports the same list for
+ * an Euler directory (shard 0 of 1) without a device.  eu_graph_set_binary_feature_name renames slot fid; EU_ERR_STATE once the
+ * label table is built. */
+int eu_graph_set_binary_feature_name(eu_graph* g, int32_t fid, const char* name);
+int eu_graph_labels(eu_graph* g, int64_t cap, int64_t* n_labels, int64_t* n_bytes, int64_t* ptr, uint8_t* bytes);
+int eu_graph_labels_inspect(const char* data_path, int64_t cap, int64_t* n_labels, int64_t* n_bytes, int64_t* ptr,
+                            uint8_t* bytes);
+/* tf_euler.sample_graph_label: out i32[count] (device) = label indices floor(u * L), u one ThreadLocalRandom() draw each
+ * (generate_canonical<double,53>: two minstd_rand0 steps), drawn from the ctx engine and counted in its draws as
+ * eu_sample_node's are, so a call followed by any other sampling op reproduces the reference's thread-local stream under
+ * EU_RNG_MINSTD; EU_RNG_PHILOX draws one Philox uniform per label.  An index that would round up to L is clamped to L - 1.
+ * count = 0 does nothing. */
+int eu_sample_graph_label(eu_ctx* c, int32_t count, int32_t* out);
+/* tf_euler.get_graph_by_label: labels i32[B] (device; label indices, -1 = a label the graph does not know).  The output is the
+ * reference's SparseTensor content: row i lists the node ids of graph i; an unknown label or one without nodes gets the single
+ * entry (i, 0) = 0.  Two passes, device pointers:
+ *   cap = 0: ptr i64[B + 1] = the row offsets; *total and *max_len (host) = the entries and the longest row (one stream
+ *            synchronisation);
+ *   cap > 0: from that ptr, indices i64[cap, 2] = (i, j) and values i64[cap] = the ids; entries at or past cap are not written. */
+int eu_get_graph_by_label(eu_ctx* c, const int32_t* labels, int64_t B, int64_t cap, int64_t* ptr, int64_t* indices,
+                          int64_t* values, int64_t* total, int64_t* max_len);
+/* The attention readout of AttentionPool (aggr = 'add') and of one Set2SetPool step (tf_euler/python/graph_pool/), fused.
+ * x f32[N, dim], index i32[N] (each row's graph in [0, B)), and exactly one of
+ *   logits f32[N]    (AttentionPool's gate), or
+ *   q f32[B, dim]    (Set2Set's query: the logit of row n is <x_n, q[index_n]>, in eu_agnn_aggregate's fixed dot order).
+ *   alpha[n] = scatter_softmax(logits, index, B)   (running max from -1e9, as scatter_max)
+ *   out[b]   = sum over the rows n of graph b of alpha[n] * x[n]     (a graph without rows gets a zero row)
+ * A graph's rows are walked in index order (unsorted index: a stable sort first, so the bits are those of the stably sorted
+ * rows); its sums (of the exps, and of the weighted rows) are fixed-order chunked segment sums: chunks of 256 rows each added
+ * left to right from +0, then the chunk sums in chunk order.  For graphs of at most 256 rows and a non-decreasing index, out
+ * and alpha equal scatter_softmax -> multiply -> scatter_add composed from the ops above bit for bit.  alpha f32[N] is
+ * required (the backward pass reads it); out f32[B, dim].
+ * The backward pass takes grad_out f32[B, dim] and alpha, and writes, with d_n = <x_n, g_b> (the order of the dot above) and
+ * S_b = sum over graph b of alpha_n * d_n (chunked):
+ *   dl_n = alpha_n * (d_n - S_b),  grad_x f32[N, dim] = alpha_n * g_b (+ dl_n * q_b),
+ *   grad_logits f32[N] = dl (logits mode; q NULL) or grad_q f32[B, dim] = sum over graph b of dl_n * x_n (chunked).
+ * Deterministic, no atomics.  dim < 1, negative sizes, rows with B = 0, both or neither of logits / q, or a NULL pointer that
+ * is needed: EU_ERR_INVALID; 2^31 or more rows or graphs: EU_ERR_UNSUPPORTED.  index is not checked (as eu_gather).  Both calls
+ * synchronise the stream once to read whether index is sorted, and use the ctx scratch: 4 B per row and graph, 12 B per
+ * graph of segment plan, (B + N / 256) * dim floats of chunk sums, and a sort of 12 B per row when index is unsorted. */
+int eu_graph_attention_readout(eu_ctx* c, const float* x, const int32_t* index, int64_t N, int64_t B, int32_t dim,
+                               const float* logits, const float* q, float* out, float* alpha);
+int eu_graph_attention_readout_backward(eu_ctx* c, const float* grad_out, const float* x, const int32_t* index, int64_t N,
+                                        int64_t B, int32_t dim, const float* q, const float* alpha, float* grad_x,
+                                        float* grad_logits, float* grad_q);
+
 /* tf_euler.sample_edge -- TF op SampleEdge (tf_euler/kernels/sample_edge_op.cc; Graph::SampleEdge graph.cc:277-301): `count`
  * edges of ONE type drawn by the alias method over the edge weights, out i64[count,3] = (src, dst, type).  Several types or
  * -1 return EU_ERR_STATE: the reference's edge_type_collection_ is never initialised and it returns nothing for them. */
