@@ -154,6 +154,10 @@ SIGNATURES = {
     "eu_get_graph_by_label": (C.c_int, [_P, _P, _I64, _I64, _P, _P, _P, _P, _P]),
     "eu_graph_attention_readout": (C.c_int, [_P, _P, _P, _I64, _I64, _I32, _P, _P, _P, _P]),
     "eu_graph_attention_readout_backward": (C.c_int, [_P, _P, _P, _P, _I64, _I64, _I32, _P, _P, _P, _P, _P]),
+    "eu_skipgram_loss": (C.c_int, [_P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P]),
+    "eu_skipgram_loss_backward": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P]),
+    "eu_skipgram_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P, _P, _P,
+                                                   _P, _P]),
     "InitQueryProxy": (C.c_bool, [C.c_char_p]),
     "eu_default_graph": (_P, []),
     "eu_default_ctx": (_P, []),

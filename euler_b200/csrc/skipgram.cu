@@ -1,0 +1,534 @@
+// The unsupervised skip-gram step of DeepWalk, node2vec and LINE, forward and backward: id embeddings, dot products with a
+// positive and K negative context rows, the sigmoid cross-entropy mean and the rank of the positive among the negatives.
+//
+// Reference semantics (file:line in the upstream alibaba/euler tree):
+//   UnsuperviseModel.__call__   tf_euler/python/mp_utils/base.py:50-91 (also solution/base_unsupervise.py)
+//   PosNegLogits                tf_euler/python/solution/logits.py (matmul of the target row with the context rows)
+//   xent_loss                   tf_euler/python/solution/losses.py (sigmoid_cross_entropy_with_logits, one reduce_mean over
+//                               the positive and negative terms together)
+//   mrr / hitk / mr             tf_euler/python/utils/metrics.py (top_k over concat([neg, pos], 2); the rank of the LAST entry)
+//
+// Pair row b has the target row t = target[src_b] and J = P + K context ids: pos[b, 0 .. P-1], then negs[b, 0 .. K-1].
+//   logits[b, j] = <t, context[ctx_bj]>, in k_agnn_dot's fixed order: lane l of a group of G lanes (G = the power of two >=
+//     ceil(dim / 4), at most 32) accumulates with __fmaf_rn from +0 the columns of its 4-column chunks l, l + G, l + 2G, ...,
+//     each chunk left to right; then a butterfly over the G lanes, xor distances G/2 .. 1.  G depends on dim only.
+//   rank[b] = #{j != P-1 : logits[b, j] >= logits[b, P-1]}: TF's top_k is stable (ties go to the lower index) and the last
+//     positive is the last entry of concat([neg, pos], 2), so it ranks behind every entry that is not smaller.
+//   loss = mean over the B J logits of max(x, 0) - x z + log1p(exp(-|x|)) (z = 1 for j < P): each term in f32, each row's
+//     terms added in j order in f64, the rows added in a fixed order in f64 (k_sg_total), one division, rounded to f32.
+// An id outside [0, n_rows) is read as row 0 and flagged; the call returns EU_ERR_INVALID after its one synchronisation.
+//
+// Backward, with g the upstream gradient (a device scalar) and N = B J: gN = g / fl(N) once, and per logit
+//   c_bj = -gN / (1 + exp(x))  (j < P: (sigmoid(x) - 1) gN)      c_bj = gN / (1 + exp(-x))  (j >= P: sigmoid(x) gN).
+// The gradients go to the tables through key lists sorted stably by row and summed per distinct row in fixed chunks of
+// kSegChunk entries (order_by, plan_distinct: segment.cuh), no atomics:
+//   the src entries:     entry b has key src_b and value gt_b = sum over j of c_bj context[ctx_bj] (fma from +0, j order)
+//   the context entries: entry (b, j) has key ctx_bj and value c_bj target[src_b], computed while it is summed
+// Each chunk adds its entries' values left to right from +0, as acc = fma(w, row, acc) with w = 1 for a src entry (so a plain
+// add) and w = c_bj for a context entry; a row of several chunks adds the chunk sums in chunk order from +0.  Separate
+// tables: one list of the B src entries for the target table, one of the B J context entries for the context table.  One
+// shared table: one list, the src entries first, then the context entries in (b, j) order.  Index scratch is O(B J) however
+// many rows the tables have; a hub negative is spread over chunks of 256 entries.
+#include "segment.cuh"
+
+namespace eu {
+
+constexpr int kSgRows = 4;     // context rows in flight per lane in the dot and target-gradient loops
+constexpr int kSgRegs = 4;     // target chunks kept in registers per lane (dim <= 512 with 32 lanes)
+constexpr int kSgUnroll = 8;   // entries in flight per lane in the chunk sums
+constexpr int kSgSumThreads = 1024;
+
+// the columns [d, d + 4) of a row (fewer than 4 at the row's end): one float4 load (VEC) or up to four scalar loads
+template <bool VEC>
+__device__ __forceinline__ float4 sg_load(const float* __restrict__ row, int d, int dim) {
+  if (VEC) return __ldg(reinterpret_cast<const float4*>(row + d));
+  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  v.x = __ldg(row + d);
+  if (d + 1 < dim) v.y = __ldg(row + d + 1);
+  if (d + 2 < dim) v.z = __ldg(row + d + 2);
+  if (d + 3 < dim) v.w = __ldg(row + d + 3);
+  return v;
+}
+
+// acc += the dot of the columns [d, min(d + 4, dim)) of a and b, one __fmaf_rn per column, left to right
+__device__ __forceinline__ float sg_fma4(float4 a, float4 b, float acc, int n) {
+  acc = __fmaf_rn(a.x, b.x, acc);
+  if (n > 1) acc = __fmaf_rn(a.y, b.y, acc);
+  if (n > 2) acc = __fmaf_rn(a.z, b.z, acc);
+  if (n > 3) acc = __fmaf_rn(a.w, b.w, acc);
+  return acc;
+}
+
+// the row of id v, or row 0 (flagged) when v lies outside [0, n_rows)
+__device__ __forceinline__ int64_t sg_row(int64_t v, int64_t n_rows, int* bad) {
+  if (v >= 0 && v < n_rows) return v;
+  *bad = 1;
+  return 0;
+}
+
+// the context id of entry (b, j): pos[b, j] for j < P, negs[b, j - P] after
+__device__ __forceinline__ int64_t sg_ctx_id(const int64_t* __restrict__ pos, const int64_t* __restrict__ negs, int64_t b, int P,
+                                             int K, int j) {
+  return j < P ? __ldg(pos + b * P + j) : __ldg(negs + b * K + (j - P));
+}
+
+// one f32 term of sigmoid_cross_entropy_with_logits (z = 1 for a positive)
+__device__ __forceinline__ float sg_xent(float x, bool positive) {
+  float r = fmaxf(x, 0.f);
+  if (positive) r = __fsub_rn(r, x);
+  return __fadd_rn(r, log1pf(expf(-fabsf(x))));
+}
+
+// G lanes per pair row b: the target row's first kSgRegs chunks of this lane in registers, kSgRows context rows in flight.
+// Lane 0 writes the logits; after them the group counts the rank and lane 0 adds the row's loss terms.
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_sg_fwd(const int64_t* __restrict__ src, const int64_t* __restrict__ pos,
+                                                const int64_t* __restrict__ negs, int64_t B, int P, int K,
+                                                const float* __restrict__ target, const float* __restrict__ context, int64_t n_rows,
+                                                int dim, int G, float* logits, int32_t* __restrict__ rank,
+                                                double* __restrict__ rowloss, int* bad) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t b = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (b >= B) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  const int J = P + K;
+  const int nck = ((dim + 3) / 4 + G - 1) / G;   // chunks of the lane with the most
+  const float* tr = target + sg_row(__ldg(src + b), n_rows, bad) * dim;
+  float4 treg[kSgRegs];
+#pragma unroll
+  for (int i = 0; i < kSgRegs; ++i) {
+    const int d = (sub + i * G) * 4;
+    treg[i] = i < nck && d < dim ? sg_load<VEC>(tr, d, dim) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  float* lrow = logits + b * J;
+  for (int j0 = 0; j0 < J; j0 += kSgRows) {
+    const float* cr[kSgRows];
+#pragma unroll
+    for (int u = 0; u < kSgRows; ++u)
+      cr[u] = j0 + u < J ? context + sg_row(sg_ctx_id(pos, negs, b, P, K, j0 + u), n_rows, bad) * dim : nullptr;
+    float acc[kSgRows];
+#pragma unroll
+    for (int u = 0; u < kSgRows; ++u) acc[u] = 0.f;
+    for (int i = 0; i < nck; ++i) {
+      const int d = (sub + i * G) * 4;
+      if (d >= dim) break;
+      float4 t;
+      if (i < kSgRegs) {
+#pragma unroll
+        for (int r = 0; r < kSgRegs; ++r)
+          if (r == i) t = treg[r];
+      } else {
+        t = sg_load<VEC>(tr, d, dim);
+      }
+      const int n = dim - d < 4 ? dim - d : 4;
+      float4 x[kSgRows];
+#pragma unroll
+      for (int u = 0; u < kSgRows; ++u)
+        if (cr[u]) x[u] = sg_load<VEC>(cr[u], d, dim);
+#pragma unroll
+      for (int u = 0; u < kSgRows; ++u)
+        if (cr[u]) acc[u] = sg_fma4(t, x[u], acc[u], n);
+    }
+#pragma unroll
+    for (int u = 0; u < kSgRows; ++u) {
+      for (int o = G >> 1; o > 0; o >>= 1) acc[u] = __fadd_rn(acc[u], __shfl_xor_sync(gm, acc[u], o, G));
+      if (sub == 0 && j0 + u < J) lrow[j0 + u] = acc[u];
+    }
+  }
+  __syncwarp(gm);   // lane 0's logits are visible to its group
+  const float xl = lrow[P - 1];
+  int cnt = 0;
+  for (int j = sub; j < J; j += G) cnt += j != P - 1 && lrow[j] >= xl;
+  for (int o = G >> 1; o > 0; o >>= 1) cnt += __shfl_xor_sync(gm, cnt, o, G);
+  if (sub != 0) return;
+  rank[b] = cnt;
+  double s = 0.0;
+  for (int j = 0; j < J; ++j) s += (double)sg_xent(lrow[j], j < P);
+  rowloss[b] = s;
+}
+
+// *loss = fl32((sum of rowloss[0, B)) / N): thread t adds rowloss[t], rowloss[t + 1024], ... in f64, then a shared-memory tree
+// (strides 512 .. 1).  One block; N = 0 gives NaN, as a mean of nothing.
+__global__ void __launch_bounds__(kSgSumThreads) k_sg_total(const double* __restrict__ rowloss, int64_t B, int64_t N,
+                                                              float* __restrict__ loss) {
+  __shared__ double sh[kSgSumThreads];
+  double acc = 0.0;
+  for (int64_t i = threadIdx.x; i < B; i += kSgSumThreads) acc += __ldg(rowloss + i);
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int s = kSgSumThreads / 2; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *loss = (float)(sh[0] / (double)N);
+}
+
+// coef[b J + j] = c_bj (see the top of the file); one thread per logit
+__global__ void k_sg_coef(const float* __restrict__ logits, const float* __restrict__ grad_loss, int64_t N, int P, int J,
+                          float* __restrict__ coef) {
+  const float gN = __fdiv_rn(__ldg(grad_loss), (float)N);
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < N; e += (int64_t)gridDim.x * blockDim.x) {
+    const float x = __ldg(logits + e);
+    coef[e] = (int)(e % J) < P ? __fdiv_rn(-gN, __fadd_rn(1.f, expf(x))) : __fdiv_rn(gN, __fadd_rn(1.f, expf(-x)));
+  }
+}
+
+// The int32 keys of the entries: key[b] = src_b for b < n_src (0 or B), then key[n_src + b J + j] = ctx_bj.  An id outside
+// [0, n_rows) becomes row 0 and sets *bad.
+__global__ void k_sg_keys(const int64_t* __restrict__ src, const int64_t* __restrict__ pos, const int64_t* __restrict__ negs,
+                          int64_t B, int P, int K, int64_t n_src, bool ctx_entries, int64_t n_rows, int32_t* __restrict__ key,
+                          int* bad) {
+  const int J = P + K;
+  const int64_t E = n_src + (ctx_entries ? B * J : 0);
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < E; e += (int64_t)gridDim.x * blockDim.x) {
+    int64_t v;
+    if (e < n_src) {
+      v = __ldg(src + e);
+    } else {
+      const int64_t t = e - n_src, b = t / J;
+      v = sg_ctx_id(pos, negs, b, P, K, (int)(t - b * J));
+    }
+    key[e] = (int32_t)sg_row(v, n_rows, bad);
+  }
+}
+
+// G lanes per pair row b: gt[b, :] = sum over j of coef[b, j] * context[ctx_bj, :], fma from +0 in j order
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_sg_target_rows(const int64_t* __restrict__ pos, const int64_t* __restrict__ negs, int64_t B,
+                                                        int P, int K, const float* __restrict__ coef,
+                                                        const float* __restrict__ context, int64_t n_rows, int dim, int G,
+                                                        float* __restrict__ gt) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t b = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (b >= B) return;
+  const int J = P + K;
+  int ignored = 0;   // the keys pass flags bad ids
+  for (int d = sub * 4; d < dim; d += G * 4) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int j0 = 0; j0 < J; j0 += kSgRows) {
+      float4 x[kSgRows];
+      float w[kSgRows];
+#pragma unroll
+      for (int u = 0; u < kSgRows; ++u) {
+        if (j0 + u < J) {
+          x[u] = sg_load<VEC>(context + sg_row(sg_ctx_id(pos, negs, b, P, K, j0 + u), n_rows, &ignored) * dim, d, dim);
+          w[u] = __ldg(coef + b * J + j0 + u);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < kSgRows; ++u) {
+        if (j0 + u < J) {
+          acc.x = __fmaf_rn(w[u], x[u].x, acc.x); acc.y = __fmaf_rn(w[u], x[u].y, acc.y);
+          acc.z = __fmaf_rn(w[u], x[u].z, acc.z); acc.w = __fmaf_rn(w[u], x[u].w, acc.w);
+        }
+      }
+    }
+    float* o = gt + b * dim + d;
+    if (VEC) {
+      *reinterpret_cast<float4*>(o) = acc;
+    } else {
+      o[0] = acc.x;
+      if (d + 1 < dim) o[1] = acc.y;
+      if (d + 2 < dim) o[2] = acc.z;
+      if (d + 3 < dim) o[3] = acc.w;
+    }
+  }
+}
+
+// One entry list (see the top of the file): entries e < n_src are src entries (value gt[e, :]), entries e >= n_src context
+// entries (value coef[t] * target[src_b, :], t = e - n_src, b = t / J)
+struct SgEntries {
+  int64_t n_src = 0;
+  int J = 1;
+  const float* gt = nullptr;
+  const float* coef = nullptr;
+  const int64_t* src = nullptr;
+  const float* target = nullptr;
+  int64_t n_rows = 0;
+};
+
+// the destination row of distinct segment p: the table row key[p] (dense) or row p of the COO values (sparse)
+__device__ __forceinline__ float* sg_out_row(float* out, const DistinctPlan& P, int64_t p, int dim, bool by_key) {
+  return out + (by_key ? (int64_t)__ldg(P.key + p) : p) * dim;
+}
+
+// G lanes per chunk of the distinct-row segments (k_emb_bwd_chunks' layout): the chunk's entries summed left to right from +0,
+// kSgUnroll of them in flight; a segment of one chunk writes its output row, the chunks of a longer one their partial rows
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_sg_chunks(SgEntries S, const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G,
+                                                   bool by_key, float* __restrict__ out) {
+  const int lg = 31 - __clz(G);
+  const int sub = (int)(threadIdx.x & (G - 1));
+  const int64_t nch_all = __ldg(P.chunk_off + P.E);
+  const int64_t step = ((int64_t)gridDim.x * blockDim.x) >> lg;
+  constexpr int U = VEC ? kSgUnroll : kSgUnroll / 2;   // the scalar path's loads take more registers
+  int ignored = 0;
+  for (int64_t c = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> lg; c < nch_all; c += step) {
+    const int64_t p = key_upper_bound(P.chunk_off, P.E + 1, c) - 1;
+    const int64_t c0 = __ldg(P.chunk_off + p), nch = __ldg(P.chunk_off + p + 1) - c0;
+    const int64_t b = __ldg(P.start + p) + (c - c0) * kSegChunk;
+    const int64_t e = min(b + kSegChunk, (int64_t)__ldg(P.start + p + 1));
+    float* o = nch == 1 ? sg_out_row(out, P, p, dim, by_key) : P.partial + (int64_t)(__ldg(P.part_off + p) + (c - c0)) * dim;
+    for (int d = sub * 4; d < dim; d += G * 4) {
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int64_t k0 = b; k0 < e; k0 += U) {
+        float4 x[U];
+        float w[U];
+#pragma unroll
+        for (int q = 0; q < U; ++q) {
+          if (k0 + q < e) {
+            const int64_t en = __ldg(perm + k0 + q);
+            if (en < S.n_src) {
+              x[q] = sg_load<VEC>(S.gt + en * dim, d, dim);
+              w[q] = 1.f;
+            } else {
+              const int64_t t = en - S.n_src;
+              x[q] = sg_load<VEC>(S.target + sg_row(__ldg(S.src + t / S.J), S.n_rows, &ignored) * dim, d, dim);
+              w[q] = __ldg(S.coef + t);
+            }
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < U; ++q) {
+          if (k0 + q < e) {
+            acc.x = __fmaf_rn(w[q], x[q].x, acc.x); acc.y = __fmaf_rn(w[q], x[q].y, acc.y);
+            acc.z = __fmaf_rn(w[q], x[q].z, acc.z); acc.w = __fmaf_rn(w[q], x[q].w, acc.w);
+          }
+        }
+      }
+      if (VEC) {
+        *reinterpret_cast<float4*>(o + d) = acc;
+      } else {
+        o[d] = acc.x;
+        if (d + 1 < dim) o[d + 1] = acc.y;
+        if (d + 2 < dim) o[d + 2] = acc.z;
+        if (d + 3 < dim) o[d + 3] = acc.w;
+      }
+    }
+  }
+}
+
+// the output row of each segment of several chunks = its partial rows added in chunk order from +0; rows (sparse, may be
+// null) gets the segments' row ids
+__global__ void k_sg_combine(DistinctPlan P, int dim, bool by_key, float* __restrict__ out, int64_t* __restrict__ rows) {
+  const int64_t D = __ldg(P.nd);
+  if (rows)
+    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D; t += (int64_t)gridDim.x * blockDim.x)
+      rows[t] = __ldg(P.key + t);
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D * dim; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = t / dim, f = t - p * dim;
+    const int64_t nch = __ldg(P.chunk_off + p + 1) - __ldg(P.chunk_off + p);
+    if (nch == 1) continue;
+    const float* part = P.partial + (int64_t)__ldg(P.part_off + p) * dim + f;
+    float acc = 0.f;
+    for (int64_t j = 0; j < nch; ++j) acc = __fadd_rn(acc, __ldg(part + j * dim));
+    sg_out_row(out, P, p, dim, by_key)[f] = acc;
+  }
+}
+
+static int sg_check(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
+                    const float* target, const float* context, int64_t n_rows, int32_t dim, const char* who) {
+  if (!c || B < 0 || P < 1 || K < 0 || n_rows < 1 || dim < 1 || !target || !context ||
+      (B > 0 && (!src || !pos || (K > 0 && !negs)))) {
+    set_error("%s: bad argument (B >= 0, P >= 1, K >= 0, n_rows and dim >= 1, tables and ids given)", who);
+    return EU_ERR_INVALID;
+  }
+  const int64_t E = B * ((int64_t)P + K + 1);   // the longest entry list (one shared table), and its chunks below
+  if (n_rows >= ((int64_t)1 << 31) || E + E / kSegChunk + 1 >= ((int64_t)1 << 31)) {
+    set_error("%s: 2^31 or more table rows, or B (P + K + 1) entries with their chunks, are not supported", who);
+    return EU_ERR_UNSUPPORTED;
+  }
+  return EU_OK;
+}
+
+// A list of E > 0 entries to sum per distinct row: its keys, order and plan in the scratch at m + off (sg_list_bytes)
+struct SgList {
+  int64_t E = 0;
+  SgEntries S;
+  bool ctx_entries = false;
+  int32_t* key = nullptr;
+  EdgeOrder ord;
+  DistinctPlan P;
+};
+
+static size_t sg_list_bytes(int64_t E, int64_t n_rows, int dim) {
+  return E ? a256(4 * (size_t)E) + order_bytes(E, n_rows) + distinct_plan_bytes(E, dim) : 0;
+}
+
+// keys, the stable order by row and the distinct-row plan of list L, from the scratch at buf
+static int sg_plan(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int P, int K, int64_t n_rows,
+                   int dim, char* buf, int* bad, SgList* L) {
+  if (!L->E) return EU_OK;
+  cudaStream_t s = c->stream;
+  L->key = (int32_t*)buf;
+  char* o_ord = buf + a256(4 * (size_t)L->E);
+  char* o_plan = o_ord + order_bytes(L->E, n_rows);
+  k_sg_keys<<<stride_grid(L->E), 256, 0, s>>>(src, pos, negs, B, P, K, L->S.n_src, L->ctx_entries, n_rows, L->key, bad);
+  EU_LAUNCHED();
+  int rc = order_by(c, L->key, L->E, n_rows, o_ord, &L->ord);
+  if (rc) return rc;
+  return plan_distinct(c, L->ord, L->E, o_plan, &L->P);
+}
+
+// the chunk sums and their combination of list L into out (by_key: a dense table; else COO values, with their row ids in rows)
+static int sg_sum(eu_ctx* c, const SgList& L, int dim, bool by_key, float* out, int64_t* rows) {
+  if (!L.E) return EU_OK;
+  cudaStream_t s = c->stream;
+  const bool vec = dim % 4 == 0 && aligned16(out) && aligned16(L.S.target) && (!L.S.gt || aligned16(L.S.gt));
+  const int G = group_lanes(ceil_div(dim, 4));
+  const unsigned blocks = stride_grid((L.E + L.E / kSegChunk + 1) * G);
+  if (vec) k_sg_chunks<true><<<blocks, 256, 0, s>>>(L.S, L.ord.perm, L.P, dim, G, by_key, out);
+  else k_sg_chunks<false><<<blocks, 256, 0, s>>>(L.S, L.ord.perm, L.P, dim, G, by_key, out);
+  EU_LAUNCHED();
+  k_sg_combine<<<stride_grid(L.E * dim), 256, 0, s>>>(L.P, dim, by_key, out, rows);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+// The backward pass both output forms share.  shared: one list into the target outputs.  sparse: the COO of
+// each list, its distinct count read back; dense: the gradient tables, zeroed first.  One synchronisation at the end.
+static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B,
+                       int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows, int32_t dim,
+                       const float* logits, bool shared, bool sparse, float* out_t, float* out_c, int64_t* rows_t,
+                       int64_t* rows_c, int64_t* n_t, int64_t* n_c, const char* who) {
+  cudaStream_t s = c->stream;
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (!sparse) {
+    EU_CUDA(cudaMemsetAsync(out_t, 0, 4 * (size_t)n_rows * dim, s));
+    if (!shared) EU_CUDA(cudaMemsetAsync(out_c, 0, 4 * (size_t)n_rows * dim, s));
+  }
+  if (n_t) *n_t = 0;
+  if (n_c) *n_c = 0;
+  const int J = P + K;
+  const int64_t N = B * J;
+  if (B == 0) return EU_OK;
+  SgList Lt, Lc;
+  Lt.S.J = Lc.S.J = J;
+  Lt.S.n_rows = Lc.S.n_rows = n_rows;
+  Lt.S.src = Lc.S.src = src;
+  Lt.S.target = Lc.S.target = target;
+  Lt.S.n_src = B;
+  Lt.ctx_entries = shared;
+  Lt.E = shared ? B + N : B;
+  Lc.E = shared ? 0 : N;
+  Lc.ctx_entries = true;
+  // flag and the two distinct counts (256 B) | coef [N] | gt [B, dim] | list t | list c
+  const size_t o_coef = 256, o_gt = o_coef + a256(4 * (size_t)N), o_lt = o_gt + a256(4 * (size_t)B * dim);
+  const size_t o_lc = o_lt + sg_list_bytes(Lt.E, n_rows, dim), total = o_lc + sg_list_bytes(Lc.E, n_rows, dim);
+  int rc = ctx_misc(c, (int64_t)total);
+  if (rc) return rc;
+  char* m = (char*)c->d_misc;
+  int* bad = (int*)m;
+  float* coef = (float*)(m + o_coef);
+  float* gt = (float*)(m + o_gt);
+  Lt.S.gt = Lc.S.gt = gt;
+  Lt.S.coef = Lc.S.coef = coef;
+  EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  {
+    EuProfScope ps(c, "skipgram_bwd_order", Lt.E + Lc.E);
+    if ((rc = sg_plan(c, src, pos, negs, B, P, K, n_rows, dim, m + o_lt, bad, &Lt))) return rc;
+    if ((rc = sg_plan(c, src, pos, negs, B, P, K, n_rows, dim, m + o_lc, bad, &Lc))) return rc;
+  }
+  EuProfScope ps(c, "skipgram_bwd_sums", Lt.E + Lc.E);
+  k_sg_coef<<<stride_grid(N), 256, 0, s>>>(logits, grad_loss, N, P, J, coef);
+  EU_LAUNCHED();
+  const bool vec = dim % 4 == 0 && aligned16(context) && aligned16(gt);
+  const int G = group_lanes(ceil_div(dim, 4));
+  const unsigned blocks = (unsigned)ceil_div(B * G, 256);
+  if (vec) k_sg_target_rows<true><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, context, n_rows, dim, G, gt);
+  else k_sg_target_rows<false><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, context, n_rows, dim, G, gt);
+  EU_LAUNCHED();
+  if ((rc = sg_sum(c, Lt, dim, !sparse, out_t, rows_t))) return rc;
+  if ((rc = sg_sum(c, Lc, dim, !sparse, out_c, rows_c))) return rc;
+  int32_t h[3] = {0, 0, 0};
+  EU_CUDA(cudaMemcpyAsync(h, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (sparse) EU_CUDA(cudaMemcpyAsync(h + 1, Lt.P.nd, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (sparse && Lc.E) EU_CUDA(cudaMemcpyAsync(h + 2, Lc.P.nd, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  EU_CUDA(cudaStreamSynchronize(s));
+  if (h[0]) {
+    set_error("%s: an id lies outside the table's rows [0, %lld)", who, (long long)n_rows);
+    return EU_ERR_INVALID;
+  }
+  if (n_t) *n_t = h[1];
+  if (n_c) *n_c = h[2];
+  return EU_OK;
+}
+
+}  // namespace eu
+
+using namespace eu;
+
+extern "C" {
+
+int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
+                     const float* target, const float* context, int64_t n_rows, int32_t dim, float* logits, int32_t* rank,
+                     float* loss) {
+  const char* who = "eu_skipgram_loss";
+  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, who);
+  if (rc) return rc;
+  if (!loss || (B > 0 && (!logits || !rank))) {
+    set_error("%s: bad argument (logits, rank and loss are required)", who);
+    return EU_ERR_INVALID;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  cudaStream_t s = c->stream;
+  // flag (256 B) | rowloss f64[B]
+  if ((rc = ctx_misc(c, 256 + (int64_t)a256(8 * (size_t)B)))) return rc;
+  int* bad = (int*)c->d_misc;
+  double* rowloss = (double*)((char*)c->d_misc + 256);
+  EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  EuProfScope ps(c, "skipgram_fwd", B);
+  if (B > 0) {
+    const bool vec = dim % 4 == 0 && aligned16(target) && aligned16(context);
+    const int G = group_lanes(ceil_div(dim, 4));   // one lane per 4-column chunk, both paths: the same order
+    const unsigned blocks = (unsigned)ceil_div(B * G, 256);
+    if (vec) k_sg_fwd<true><<<blocks, 256, 0, s>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
+    else k_sg_fwd<false><<<blocks, 256, 0, s>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
+    EU_LAUNCHED();
+  }
+  k_sg_total<<<1, kSgSumThreads, 0, s>>>(rowloss, B, B * (int64_t)(P + K), loss);
+  EU_LAUNCHED();
+  int h = 0;
+  EU_CUDA(cudaMemcpyAsync(&h, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
+  EU_CUDA(cudaStreamSynchronize(s));
+  if (h) {
+    set_error("%s: an id lies outside the table's rows [0, %lld)", who, (long long)n_rows);
+    return EU_ERR_INVALID;
+  }
+  return EU_OK;
+}
+
+int eu_skipgram_loss_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                              int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
+                              int32_t dim, const float* logits, float* grad_target, float* grad_context) {
+  const char* who = "eu_skipgram_loss_backward";
+  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, who);
+  if (rc) return rc;
+  if (!grad_loss || !grad_target || !grad_context || (B > 0 && !logits)) {
+    set_error("%s: bad argument (grad_loss, logits and both gradient tables are required)", who);
+    return EU_ERR_INVALID;
+  }
+  return sg_backward(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, logits, grad_target == grad_context, false,
+                     grad_target, grad_context, nullptr, nullptr, nullptr, nullptr, who);
+}
+
+int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                                     int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
+                                     int32_t dim, const float* logits, int64_t* rows_target, float* values_target,
+                                     int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context) {
+  const char* who = "eu_skipgram_loss_backward_sparse";
+  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, who);
+  if (rc) return rc;
+  const bool shared = !rows_context;
+  if (!grad_loss || !n_target || (B > 0 && (!logits || !rows_target || !values_target)) ||
+      (!shared && (!n_context || (B > 0 && !values_context)))) {
+    set_error("%s: bad argument", who);
+    return EU_ERR_INVALID;
+  }
+  return sg_backward(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, logits, shared, true, values_target,
+                     values_context, rows_target, rows_context, n_target, n_context, who);
+}
+
+}  // extern "C"

@@ -1276,3 +1276,121 @@ def graph_attention_readout(x, index, size, logits=None, q=None):
         if w.numel() != x.shape[0]:
             raise EulerError("graph_attention_readout: logits has %d rows, x %d" % (w.numel(), x.shape[0]))
     return _GraphReadout.apply(x, w, index, size, q is not None)
+
+
+# ------------------------------------------------------------------------------------ unsupervised skip-gram step
+SKIPGRAM_METRICS = ('mrr', 'hit1', 'hit3', 'hit10', 'mr')
+
+
+def skipgram_metric(rank, name):
+    """metrics.py's ranking metrics (utils/metrics.py mrr_score, hitk_score, mr_score) from rank [B], the position of each row's
+    last positive among its logits:
+        mrr   mean of 1 / (rank + 1), in float32
+        hitK  mean of (rank < K), K in 1, 3, 10
+        mr    tf.reduce_mean of the int64 ranks: an INTEGER mean (the sum divided by B, rounded toward zero), int64, as upstream
+    A batch of no rows gives NaN for mrr and hitK and 0 for mr."""
+    if name == 'mrr':
+        return torch.reciprocal((rank + 1).to(torch.float32)).mean()
+    if name in ('hit1', 'hit3', 'hit10'):
+        return (rank < int(name[3:])).to(torch.float32).mean()
+    if name == 'mr':
+        r = rank.to(torch.int64)
+        return torch.div(r.sum(), max(r.numel(), 1), rounding_mode='trunc')
+    raise EulerError("skipgram metric must be one of %s, got %r" % (SKIPGRAM_METRICS, name))
+
+
+def _raw_skipgram(src, pos, negs, target, context):
+    """one eu_skipgram_loss: (logits f32[B, P + K], rank i32[B], loss f32[])"""
+    B, P = pos.shape
+    K = negs.shape[1]
+    n_rows, dim = target.shape
+    logits = torch.empty((B, P + K), dtype=torch.float32, device=target.device)
+    rank = torch.empty(B, dtype=torch.int32, device=target.device)
+    loss = torch.empty((), dtype=torch.float32, device=target.device)
+    ec = _ctx_on_stream()
+    check(_lib.load().eu_skipgram_loss(ec._h, src.data_ptr(), pos.data_ptr(), negs.data_ptr(), B, P, K, target.data_ptr(),
+                                       context.data_ptr(), n_rows, dim, logits.data_ptr(), rank.data_ptr(), loss.data_ptr()))
+    return logits, rank, loss
+
+
+class _SkipgramLoss(torch.autograd.Function):
+    """eu_skipgram_loss / eu_skipgram_loss_backward(_sparse).  Saves the ids and the logits (and the tables themselves, which
+    are inputs): no [B, P + K, dim] rows are kept.  shared: target and context are one table, whose gradient is computed as
+    one list and returned for the target input only."""
+
+    @staticmethod
+    def forward(ctx, target, context, src, pos, negs, shared, sparse_grad):
+        logits, rank, loss = _raw_skipgram(src, pos, negs, target, context)
+        ctx.save_for_backward(target, context, src, pos, negs, logits)
+        ctx.shared, ctx.sparse_grad = shared, sparse_grad
+        ctx.mark_non_differentiable(rank)
+        return loss, rank
+
+    @staticmethod
+    def backward(ctx, g_loss, g_rank):
+        target, context, src, pos, negs, logits = ctx.saved_tensors
+        B, P = pos.shape
+        K = negs.shape[1]
+        n_rows, dim = target.shape
+        dev = target.device
+        g = g_loss.to(device=dev, dtype=torch.float32).reshape(1).contiguous()
+        ec, lib = _ctx_on_stream(), _lib.load()
+        args = (ec._h, g.data_ptr(), src.data_ptr(), pos.data_ptr(), negs.data_ptr(), B, P, K, target.data_ptr(), context.data_ptr(),
+                n_rows, dim, logits.data_ptr())
+        if not ctx.sparse_grad:
+            g_t = torch.empty((n_rows, dim), dtype=torch.float32, device=dev)
+            g_c = g_t if ctx.shared else torch.empty((n_rows, dim), dtype=torch.float32, device=dev)
+            check(lib.eu_skipgram_loss_backward(*args, g_t.data_ptr(), g_c.data_ptr()))
+            return g_t, None if ctx.shared else g_c, None, None, None, None, None
+
+        def coo_buffers(entries):
+            cap = min(entries, n_rows)
+            return torch.empty(cap, dtype=torch.int64, device=dev), torch.empty((cap, dim), dtype=torch.float32, device=dev)
+
+        rows_t, vals_t = coo_buffers(B * (P + K + 1) if ctx.shared else B)
+        rows_c, vals_c = (None, None) if ctx.shared else coo_buffers(B * (P + K))
+        n_t, n_c = C.c_int64(), C.c_int64()
+        check(lib.eu_skipgram_loss_backward_sparse(*args, rows_t.data_ptr(), vals_t.data_ptr(), C.byref(n_t),
+                                                   rows_c.data_ptr() if rows_c is not None else None,
+                                                   vals_c.data_ptr() if vals_c is not None else None, C.byref(n_c)))
+
+        def coo(rows, vals, n):
+            return torch.sparse_coo_tensor(rows[:n].unsqueeze(0), vals[:n], (n_rows, dim), is_coalesced=True,
+                                           check_invariants=False)
+
+        g_t = coo(rows_t, vals_t, n_t.value)
+        return g_t, None if ctx.shared else coo(rows_c, vals_c, n_c.value), None, None, None, None, None
+
+
+def skipgram_xent_loss(src, pos, negs, target, context, metric='mrr', sparse_grad=False):
+    """The skip-gram step of UnsuperviseModel.__call__ (mp_utils/base.py:50-91; PosNegLogits, xent_loss, utils/metrics.py) in
+    one fused device op, for id embeddings:
+        src [B] or [B, 1]    target-table rows        pos [B, P] or [B]   context-table rows of the positives (P >= 1)
+        negs [B, K]          context-table rows of the negatives (K >= 0)
+        target, context      f32[n_rows, dim] tables; passing one tensor twice is LINE's first order (one shared table)
+    Returns (loss, metric): loss is the mean sigmoid cross-entropy over the B (P + K) logits (positives labelled 1), metric the
+    ranking metric `metric` (skipgram_metric) of each row's last positive among its P + K logits, ties ranked as TF's stable
+    top_k ranks them.  Ids index the tables directly, as tf.nn.embedding_lookup does; one outside [0, n_rows) raises.
+    The gradient reaches the tables only: dense f32[n_rows, dim] gradients, or, with sparse_grad=True, coalesced sparse COO
+    gradients of the rows the batch touches (as nn.Embedding(sparse=True) gives).  Deterministic, no atomics; the forward and the
+    backward synchronise once each."""
+    if metric not in SKIPGRAM_METRICS:
+        raise EulerError("skipgram_xent_loss: metric must be one of %s, got %r" % (SKIPGRAM_METRICS, metric))
+    shared = context is target
+    for name, tb in (('target', target), ('context', context)):
+        if not torch.is_tensor(tb) or tb.dtype != torch.float32 or tb.dim() != 2:
+            raise EulerError("skipgram_xent_loss: %s must be a 2-D float32 tensor" % name)
+    if target.shape != context.shape:
+        raise EulerError("skipgram_xent_loss: target %s and context %s must have one shape" % (tuple(target.shape), tuple(context.shape)))
+    src = _t(src, torch.int64).reshape(-1)
+    B = src.numel()
+    pos, negs = _t(pos, torch.int64), _t(negs, torch.int64)
+    if pos.dim() == 1:
+        pos = pos.unsqueeze(1)
+    if pos.dim() != 2 or negs.dim() != 2 or pos.shape[0] != B or negs.shape[0] != B or pos.shape[1] < 1:
+        raise EulerError("skipgram_xent_loss: pos must be [B, P >= 1] and negs [B, K] with B = %d, got %s and %s"
+                         % (B, tuple(pos.shape), tuple(negs.shape)))
+    target = _t(target, torch.float32)
+    context = target if shared else _t(context, torch.float32)
+    loss, rank = _SkipgramLoss.apply(target, context, src, pos.contiguous(), negs.contiguous(), shared, bool(sparse_grad))
+    return loss, skipgram_metric(rank, metric)

@@ -352,6 +352,45 @@ int eu_graph_attention_readout_backward(eu_ctx* c, const float* grad_out, const 
                                         int64_t B, int32_t dim, const float* q, const float* alpha, float* grad_x,
                                         float* grad_logits, float* grad_q);
 
+/* The unsupervised skip-gram step of DeepWalk / node2vec / LINE, fused (reference: UnsuperviseModel.__call__,
+ * tf_euler/python/mp_utils/base.py:50-91 and solution/base_unsupervise.py, with PosNegLogits solution/logits.py, xent_loss
+ * solution/losses.py and the rank of mrr_score / hitk_score / mr_score utils/metrics.py).  Ids are table rows, as
+ * tf.nn.embedding_lookup uses them: src i64[B], pos i64[B, P] (P >= 1), negs i64[B, K] (K >= 0); target and context
+ * f32[n_rows, dim] (may be the same table).  Outputs, device pointers:
+ *   logits f32[B, P + K]: row b is <target[src_b], context[c]> for c = pos[b, 0 .. P-1], then negs[b, 0 .. K-1], each a dot in
+ *                         eu_agnn_aggregate's fixed order (per-lane fma sums over 4-column chunks, then a fixed butterfly;
+ *                         the order depends on dim only, never on the launch);
+ *   rank i32[B]:          #{j != P-1 : logits[b, j] >= logits[b, P-1]}, the position TF's stable top_k gives the last positive
+ *                         in concat([neg, pos], 2) (ties rank it behind);
+ *   loss f32[1]:          the mean over the B (P + K) logits of max(x, 0) - x z + log1p(exp(-|x|)), z = 1 for the positives:
+ *                         f32 terms summed in f64 in a fixed order, one division (B = 0: NaN).
+ * An id outside [0, n_rows) is never dereferenced: EU_ERR_INVALID after the call's one stream synchronisation.
+ * The backward passes take grad_loss (a device f32 scalar, read on the device) and the forward's logits, and recompute
+ * c_bj = (sigmoid(x) - z) g / (B (P + K)).  The gradient of the target table sums, per distinct src id, the rows
+ * sum_j c_bj context[ctx_bj] of its pairs; that of the context table sums, per distinct context id, c_bj target[src_b] over its
+ * entries (b, j).  Entries are ordered stably by row (a shared table lists the B src entries first, then the context entries
+ * in (b, j) order) and summed in chunks of 256 counted from each row's first entry, left to right from +0, then the chunk sums
+ * in chunk order: no atomics, the same bits on every run.  Scratch: O(B (P + K)) of index data plus B dim floats, never
+ * O(n_rows); one stream synchronisation per call.
+ *   eu_skipgram_loss_backward:        dense grad_target and grad_context f32[n_rows, dim], zero on untouched rows;
+ *                                     grad_context == grad_target means one shared table (both gradients summed into it).
+ *   eu_skipgram_loss_backward_sparse: the coalesced COO of each table's gradient: rows i64[D] ascending and values f32[D, dim],
+ *                                     D (host) = the distinct ids; the arrays must hold min(entries, n_rows) rows (B for the
+ *                                     target, B (P + K) for the context, B (P + K + 1) for a shared table).  rows_context
+ *                                     NULL means one shared table, written to the target outputs.
+ * P < 1, K < 0, B < 0, n_rows or dim < 1, or a NULL pointer that is needed: EU_ERR_INVALID; n_rows >= 2^31, or B (P + K + 1)
+ * entries with their 256-entry chunks reaching 2^31: EU_ERR_UNSUPPORTED. */
+int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
+                     const float* target, const float* context, int64_t n_rows, int32_t dim, float* logits, int32_t* rank,
+                     float* loss);
+int eu_skipgram_loss_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                              int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
+                              int32_t dim, const float* logits, float* grad_target, float* grad_context);
+int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                                     int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
+                                     int32_t dim, const float* logits, int64_t* rows_target, float* values_target,
+                                     int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context);
+
 /* tf_euler.sample_edge -- TF op SampleEdge (tf_euler/kernels/sample_edge_op.cc; Graph::SampleEdge graph.cc:277-301): `count`
  * edges of ONE type drawn by the alias method over the edge weights, out i64[count,3] = (src, dst, type).  Several types or
  * -1 return EU_ERR_STATE: the reference's edge_type_collection_ is never initialised and it returns nothing for them. */
