@@ -30,6 +30,26 @@ class GraphDesc(C.Structure):
     ]
 
 
+class EdgeDesc(C.Structure):
+    """eu_edge_desc"""
+    _fields_ = [
+        ("n_edges", C.c_int64), ("src", C.c_void_p), ("dst", C.c_void_p), ("type", C.c_void_p), ("w", C.c_void_p),
+        ("feat_dim", C.c_int32), ("feat", C.c_void_p), ("n_feat_slots", C.c_int32), ("feat_slot_dims", C.c_void_p),
+        ("n_u64_slots", C.c_int32), ("u64_ptr", C.c_void_p), ("u64_val", C.c_void_p),
+        ("n_bin_slots", C.c_int32), ("bin_ptr", C.c_void_p), ("bin_val", C.c_void_p),
+        ("sampler_order", C.c_void_p),
+    ]
+
+
+class KgProblem(C.Structure):
+    """eu_kg_problem"""
+    _fields_ = [
+        ("model", C.c_int32), ("l1", C.c_int32), ("corrupt", C.c_int32), ("margin", C.c_float), ("B", C.c_int64),
+        ("K", C.c_int32), ("ent_dim", C.c_int32), ("rel_dim", C.c_int32), ("n_ent", C.c_int64), ("n_rel", C.c_int64),
+        ("src", C.c_void_p), ("dst", C.c_void_p), ("rel", C.c_void_p), ("neg", C.c_void_p), ("table", C.c_void_p * 4),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/euler_b200.h declares
 _P, _I64, _I32, _U64, _F = C.c_void_p, C.c_int64, C.c_int32, C.c_uint64, C.c_float
 SIGNATURES = {
@@ -158,6 +178,10 @@ SIGNATURES = {
     "eu_skipgram_loss_backward": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P]),
     "eu_skipgram_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P, _P, _P,
                                                    _P, _P]),
+    "eu_kg_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
+    "eu_kg_loss_backward": (C.c_int, [_P, _P, _P, _P, _P]),
+    "eu_kg_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
+    "eu_graph_set_edge_dense_feature_name": (C.c_int, [_P, _I32, C.c_char_p]),
     "InitQueryProxy": (C.c_bool, [C.c_char_p]),
     "eu_default_graph": (_P, []),
     "eu_default_ctx": (_P, []),

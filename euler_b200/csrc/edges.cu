@@ -241,6 +241,14 @@ int32_t eu_graph_edge_dense_feature_id(const eu_graph* g, const char* name) {
   for (size_t i = 0; i < g->edge_dense_names.size(); ++i) if (g->edge_dense_names[i] == name) return (int32_t)i;
   return -1;
 }
+int eu_graph_set_edge_dense_feature_name(eu_graph* g, int32_t fid, const char* name) {
+  if (!g || !name || fid < 0 || fid >= (int32_t)g->edge_dense_names.size()) {
+    set_error("eu_graph_set_edge_dense_feature_name: bad argument (slot %d)", (int)fid);
+    return EU_ERR_INVALID;
+  }
+  g->edge_dense_names[fid] = name;
+  return EU_OK;
+}
 int32_t eu_graph_edge_sparse_feature_id(const eu_graph* g, const char* name) {
   if (!g || !name) return -1;
   for (size_t i = 0; i < g->edge_sparse_names.size(); ++i) if (g->edge_sparse_names[i] == name) return (int32_t)i;

@@ -202,4 +202,113 @@ int plan_distinct(eu_ctx* c, const EdgeOrder& o, int64_t E, char* buf, DistinctP
   return EU_OK;
 }
 
+constexpr int kRowSumUnroll = 8;   // entries in flight per lane in the chunk sums
+
+// the destination row of distinct segment p: the table row key[p] (dense) or row p of the COO values (sparse)
+__device__ __forceinline__ float* distinct_out_row(float* out, const DistinctPlan& P, int64_t p, int dim, bool by_key) {
+  return out + (by_key ? (int64_t)__ldg(P.key + p) : p) * dim;
+}
+
+// G lanes per chunk of the distinct-row segments (k_emb_bwd_chunks' layout): the chunk's entries summed left to right from +0,
+// kRowSumUnroll of them in flight; a segment of one chunk writes its output row, the chunks of a longer one their partial rows
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_row_chunks(RowEntries S, const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G,
+                                                    bool by_key, float* __restrict__ out) {
+  const int lg = 31 - __clz(G);
+  const int sub = (int)(threadIdx.x & (G - 1));
+  const int64_t nch_all = __ldg(P.chunk_off + P.E);
+  const int64_t step = ((int64_t)gridDim.x * blockDim.x) >> lg;
+  constexpr int U = VEC ? kRowSumUnroll : kRowSumUnroll / 2;   // the scalar path's loads take more registers
+  int ignored = 0;
+  for (int64_t c = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> lg; c < nch_all; c += step) {
+    const int64_t p = key_upper_bound(P.chunk_off, P.E + 1, c) - 1;
+    const int64_t c0 = __ldg(P.chunk_off + p), nch = __ldg(P.chunk_off + p + 1) - c0;
+    const int64_t b = __ldg(P.start + p) + (c - c0) * kSegChunk;
+    const int64_t e = min(b + kSegChunk, (int64_t)__ldg(P.start + p + 1));
+    float* o = nch == 1 ? distinct_out_row(out, P, p, dim, by_key) : P.partial + (int64_t)(__ldg(P.part_off + p) + (c - c0)) * dim;
+    for (int d = sub * 4; d < dim; d += G * 4) {
+      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int64_t k0 = b; k0 < e; k0 += U) {
+        float4 x[U];
+        float w[U];
+#pragma unroll
+        for (int q = 0; q < U; ++q) {
+          if (k0 + q < e) {
+            const int64_t en = __ldg(perm + k0 + q);
+            if (en < S.n_src) {
+              x[q] = row_load4<VEC>(S.gt + en * dim, d, dim);
+              w[q] = 1.f;
+            } else {
+              const int64_t t = en - S.n_src;
+              x[q] = row_load4<VEC>(S.target + row_of(__ldg(S.src + t / S.J), S.n_rows, &ignored) * dim, d, dim);
+              w[q] = __ldg(S.coef + t);
+            }
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < U; ++q) {
+          if (k0 + q < e) {
+            acc.x = __fmaf_rn(w[q], x[q].x, acc.x); acc.y = __fmaf_rn(w[q], x[q].y, acc.y);
+            acc.z = __fmaf_rn(w[q], x[q].z, acc.z); acc.w = __fmaf_rn(w[q], x[q].w, acc.w);
+          }
+        }
+      }
+      if (VEC) {
+        *reinterpret_cast<float4*>(o + d) = acc;
+      } else {
+        o[d] = acc.x;
+        if (d + 1 < dim) o[d + 1] = acc.y;
+        if (d + 2 < dim) o[d + 2] = acc.z;
+        if (d + 3 < dim) o[d + 3] = acc.w;
+      }
+    }
+  }
+}
+
+// the output row of each segment of several chunks = its partial rows added in chunk order from +0; rows (sparse, may be
+// null) gets the segments' row ids
+__global__ void k_row_combine(DistinctPlan P, int dim, bool by_key, float* __restrict__ out, int64_t* __restrict__ rows) {
+  const int64_t D = __ldg(P.nd);
+  if (rows)
+    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D; t += (int64_t)gridDim.x * blockDim.x)
+      rows[t] = __ldg(P.key + t);
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D * dim; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = t / dim, f = t - p * dim;
+    const int64_t nch = __ldg(P.chunk_off + p + 1) - __ldg(P.chunk_off + p);
+    if (nch == 1) continue;
+    const float* part = P.partial + (int64_t)__ldg(P.part_off + p) * dim + f;
+    float acc = 0.f;
+    for (int64_t j = 0; j < nch; ++j) acc = __fadd_rn(acc, __ldg(part + j * dim));
+    distinct_out_row(out, P, p, dim, by_key)[f] = acc;
+  }
+}
+
+int sum_distinct_rows(eu_ctx* c, const RowEntries& S, int64_t E, const int32_t* perm, const DistinctPlan& P, int dim, bool by_key,
+                      float* out, int64_t* rows) {
+  cudaStream_t s = c->stream;
+  const bool vec = dim % 4 == 0 && aligned16(out) && (!S.target || aligned16(S.target)) && (!S.gt || aligned16(S.gt));
+  const int G = group_lanes(ceil_div(dim, 4));
+  const unsigned blocks = stride_grid((E + E / kSegChunk + 1) * G);
+  if (vec) k_row_chunks<true><<<blocks, 256, 0, s>>>(S, perm, P, dim, G, by_key, out);
+  else k_row_chunks<false><<<blocks, 256, 0, s>>>(S, perm, P, dim, G, by_key, out);
+  EU_LAUNCHED();
+  k_row_combine<<<stride_grid(E * dim), 256, 0, s>>>(P, dim, by_key, out, rows);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+__global__ void __launch_bounds__(kMeanThreads) k_f64_mean(const double* __restrict__ rowloss, int64_t B, int64_t N,
+                                                           float* __restrict__ loss) {
+  __shared__ double sh[kMeanThreads];
+  double acc = 0.0;
+  for (int64_t i = threadIdx.x; i < B; i += kMeanThreads) acc += __ldg(rowloss + i);
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int s = kMeanThreads / 2; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *loss = (float)(sh[0] / (double)N);
+}
+
 }  // namespace eu

@@ -133,4 +133,51 @@ struct DistinctPlan {
 size_t distinct_plan_bytes(int64_t E, int64_t width);
 int plan_distinct(eu_ctx* c, const EdgeOrder& o, int64_t E, char* buf, DistinctPlan* P);
 
+// ---------------------------------------------------------------------------- id-table rows summed per distinct id
+// Shared by the losses over id tables (skipgram.cu, kg.cu).
+
+// the columns [d, d + 4) of a row (fewer than 4 at the row's end): one float4 load (VEC) or up to four scalar loads
+template <bool VEC>
+__device__ __forceinline__ float4 row_load4(const float* __restrict__ row, int d, int dim) {
+  if (VEC) return __ldg(reinterpret_cast<const float4*>(row + d));
+  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  v.x = __ldg(row + d);
+  if (d + 1 < dim) v.y = __ldg(row + d + 1);
+  if (d + 2 < dim) v.z = __ldg(row + d + 2);
+  if (d + 3 < dim) v.w = __ldg(row + d + 3);
+  return v;
+}
+
+// the row of id v, or row 0 (flagged) when v lies outside [0, n_rows)
+__device__ __forceinline__ int64_t row_of(int64_t v, int64_t n_rows, int* bad) {
+  if (v >= 0 && v < n_rows) return v;
+  *bad = 1;
+  return 0;
+}
+
+// The values of an entry list ordered by row: entries e < n_src have the materialised value gt[e, :]; entries e >= n_src
+// have coef[t] * target[src_b, :], t = e - n_src, b = t / J (computed while they are summed).  A list of materialised rows only
+// has n_src = its length.
+struct RowEntries {
+  int64_t n_src = 0;
+  int J = 1;
+  const float* gt = nullptr;
+  const float* coef = nullptr;
+  const int64_t* src = nullptr;
+  const float* target = nullptr;
+  int64_t n_rows = 0;
+};
+
+// The sums per distinct row of the E > 0 entries S in the order `perm` with the plan P: each 256-entry chunk adds its entries
+// left to right from +0 as acc = fma(w, row, acc) (w = 1 for a materialised row), a row of several chunks adds its chunk sums
+// in chunk order from +0.  by_key: into the dense table out (rows not in the list untouched); else into COO values out, with
+// the rows' ids in rows (may be null).  No atomics: the bits depend on each row's entry sequence only.
+int sum_distinct_rows(eu_ctx* c, const RowEntries& S, int64_t E, const int32_t* perm, const DistinctPlan& P, int dim, bool by_key,
+                      float* out, int64_t* rows);
+
+// *loss = fl32((sum of rowloss[0, B)) / N): thread t adds rowloss[t], rowloss[t + 1024], ... in f64, then a shared-memory tree
+// (strides 512 .. 1).  One block of kMeanThreads; N = 0 gives NaN, as a mean of nothing.
+constexpr int kMeanThreads = 1024;
+__global__ void k_f64_mean(const double* __restrict__ rowloss, int64_t B, int64_t N, float* __restrict__ loss);
+
 }  // namespace eu

@@ -15,7 +15,7 @@
 //   rank[b] = #{j != P-1 : logits[b, j] >= logits[b, P-1]}: TF's top_k is stable (ties go to the lower index) and the last
 //     positive is the last entry of concat([neg, pos], 2), so it ranks behind every entry that is not smaller.
 //   loss = mean over the B J logits of max(x, 0) - x z + log1p(exp(-|x|)) (z = 1 for j < P): each term in f32, each row's
-//     terms added in j order in f64, the rows added in a fixed order in f64 (k_sg_total), one division, rounded to f32.
+//     terms added in j order in f64, the rows added in a fixed order in f64 (k_f64_mean), one division, rounded to f32.
 // An id outside [0, n_rows) is read as row 0 and flagged; the call returns EU_ERR_INVALID after its one synchronisation.
 //
 // Backward, with g the upstream gradient (a device scalar) and N = B J: gN = g / fl(N) once, and per logit
@@ -35,20 +35,6 @@ namespace eu {
 
 constexpr int kSgRows = 4;     // context rows in flight per lane in the dot and target-gradient loops
 constexpr int kSgRegs = 4;     // target chunks kept in registers per lane (dim <= 512 with 32 lanes)
-constexpr int kSgUnroll = 8;   // entries in flight per lane in the chunk sums
-constexpr int kSgSumThreads = 1024;
-
-// the columns [d, d + 4) of a row (fewer than 4 at the row's end): one float4 load (VEC) or up to four scalar loads
-template <bool VEC>
-__device__ __forceinline__ float4 sg_load(const float* __restrict__ row, int d, int dim) {
-  if (VEC) return __ldg(reinterpret_cast<const float4*>(row + d));
-  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-  v.x = __ldg(row + d);
-  if (d + 1 < dim) v.y = __ldg(row + d + 1);
-  if (d + 2 < dim) v.z = __ldg(row + d + 2);
-  if (d + 3 < dim) v.w = __ldg(row + d + 3);
-  return v;
-}
 
 // acc += the dot of the columns [d, min(d + 4, dim)) of a and b, one __fmaf_rn per column, left to right
 __device__ __forceinline__ float sg_fma4(float4 a, float4 b, float acc, int n) {
@@ -57,13 +43,6 @@ __device__ __forceinline__ float sg_fma4(float4 a, float4 b, float acc, int n) {
   if (n > 2) acc = __fmaf_rn(a.z, b.z, acc);
   if (n > 3) acc = __fmaf_rn(a.w, b.w, acc);
   return acc;
-}
-
-// the row of id v, or row 0 (flagged) when v lies outside [0, n_rows)
-__device__ __forceinline__ int64_t sg_row(int64_t v, int64_t n_rows, int* bad) {
-  if (v >= 0 && v < n_rows) return v;
-  *bad = 1;
-  return 0;
 }
 
 // the context id of entry (b, j): pos[b, j] for j < P, negs[b, j - P] after
@@ -94,19 +73,19 @@ __global__ void __launch_bounds__(256) k_sg_fwd(const int64_t* __restrict__ src,
   const unsigned gm = group_mask(G);
   const int J = P + K;
   const int nck = ((dim + 3) / 4 + G - 1) / G;   // chunks of the lane with the most
-  const float* tr = target + sg_row(__ldg(src + b), n_rows, bad) * dim;
+  const float* tr = target + row_of(__ldg(src + b), n_rows, bad) * dim;
   float4 treg[kSgRegs];
 #pragma unroll
   for (int i = 0; i < kSgRegs; ++i) {
     const int d = (sub + i * G) * 4;
-    treg[i] = i < nck && d < dim ? sg_load<VEC>(tr, d, dim) : make_float4(0.f, 0.f, 0.f, 0.f);
+    treg[i] = i < nck && d < dim ? row_load4<VEC>(tr, d, dim) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
   float* lrow = logits + b * J;
   for (int j0 = 0; j0 < J; j0 += kSgRows) {
     const float* cr[kSgRows];
 #pragma unroll
     for (int u = 0; u < kSgRows; ++u)
-      cr[u] = j0 + u < J ? context + sg_row(sg_ctx_id(pos, negs, b, P, K, j0 + u), n_rows, bad) * dim : nullptr;
+      cr[u] = j0 + u < J ? context + row_of(sg_ctx_id(pos, negs, b, P, K, j0 + u), n_rows, bad) * dim : nullptr;
     float acc[kSgRows];
 #pragma unroll
     for (int u = 0; u < kSgRows; ++u) acc[u] = 0.f;
@@ -119,13 +98,13 @@ __global__ void __launch_bounds__(256) k_sg_fwd(const int64_t* __restrict__ src,
         for (int r = 0; r < kSgRegs; ++r)
           if (r == i) t = treg[r];
       } else {
-        t = sg_load<VEC>(tr, d, dim);
+        t = row_load4<VEC>(tr, d, dim);
       }
       const int n = dim - d < 4 ? dim - d : 4;
       float4 x[kSgRows];
 #pragma unroll
       for (int u = 0; u < kSgRows; ++u)
-        if (cr[u]) x[u] = sg_load<VEC>(cr[u], d, dim);
+        if (cr[u]) x[u] = row_load4<VEC>(cr[u], d, dim);
 #pragma unroll
       for (int u = 0; u < kSgRows; ++u)
         if (cr[u]) acc[u] = sg_fma4(t, x[u], acc[u], n);
@@ -146,22 +125,6 @@ __global__ void __launch_bounds__(256) k_sg_fwd(const int64_t* __restrict__ src,
   double s = 0.0;
   for (int j = 0; j < J; ++j) s += (double)sg_xent(lrow[j], j < P);
   rowloss[b] = s;
-}
-
-// *loss = fl32((sum of rowloss[0, B)) / N): thread t adds rowloss[t], rowloss[t + 1024], ... in f64, then a shared-memory tree
-// (strides 512 .. 1).  One block; N = 0 gives NaN, as a mean of nothing.
-__global__ void __launch_bounds__(kSgSumThreads) k_sg_total(const double* __restrict__ rowloss, int64_t B, int64_t N,
-                                                              float* __restrict__ loss) {
-  __shared__ double sh[kSgSumThreads];
-  double acc = 0.0;
-  for (int64_t i = threadIdx.x; i < B; i += kSgSumThreads) acc += __ldg(rowloss + i);
-  sh[threadIdx.x] = acc;
-  __syncthreads();
-  for (int s = kSgSumThreads / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *loss = (float)(sh[0] / (double)N);
 }
 
 // coef[b J + j] = c_bj (see the top of the file); one thread per logit
@@ -189,7 +152,7 @@ __global__ void k_sg_keys(const int64_t* __restrict__ src, const int64_t* __rest
       const int64_t t = e - n_src, b = t / J;
       v = sg_ctx_id(pos, negs, b, P, K, (int)(t - b * J));
     }
-    key[e] = (int32_t)sg_row(v, n_rows, bad);
+    key[e] = (int32_t)row_of(v, n_rows, bad);
   }
 }
 
@@ -213,7 +176,7 @@ __global__ void __launch_bounds__(256) k_sg_target_rows(const int64_t* __restric
 #pragma unroll
       for (int u = 0; u < kSgRows; ++u) {
         if (j0 + u < J) {
-          x[u] = sg_load<VEC>(context + sg_row(sg_ctx_id(pos, negs, b, P, K, j0 + u), n_rows, &ignored) * dim, d, dim);
+          x[u] = row_load4<VEC>(context + row_of(sg_ctx_id(pos, negs, b, P, K, j0 + u), n_rows, &ignored) * dim, d, dim);
           w[u] = __ldg(coef + b * J + j0 + u);
         }
       }
@@ -237,97 +200,6 @@ __global__ void __launch_bounds__(256) k_sg_target_rows(const int64_t* __restric
   }
 }
 
-// One entry list (see the top of the file): entries e < n_src are src entries (value gt[e, :]), entries e >= n_src context
-// entries (value coef[t] * target[src_b, :], t = e - n_src, b = t / J)
-struct SgEntries {
-  int64_t n_src = 0;
-  int J = 1;
-  const float* gt = nullptr;
-  const float* coef = nullptr;
-  const int64_t* src = nullptr;
-  const float* target = nullptr;
-  int64_t n_rows = 0;
-};
-
-// the destination row of distinct segment p: the table row key[p] (dense) or row p of the COO values (sparse)
-__device__ __forceinline__ float* sg_out_row(float* out, const DistinctPlan& P, int64_t p, int dim, bool by_key) {
-  return out + (by_key ? (int64_t)__ldg(P.key + p) : p) * dim;
-}
-
-// G lanes per chunk of the distinct-row segments (k_emb_bwd_chunks' layout): the chunk's entries summed left to right from +0,
-// kSgUnroll of them in flight; a segment of one chunk writes its output row, the chunks of a longer one their partial rows
-template <bool VEC>
-__global__ void __launch_bounds__(256) k_sg_chunks(SgEntries S, const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G,
-                                                   bool by_key, float* __restrict__ out) {
-  const int lg = 31 - __clz(G);
-  const int sub = (int)(threadIdx.x & (G - 1));
-  const int64_t nch_all = __ldg(P.chunk_off + P.E);
-  const int64_t step = ((int64_t)gridDim.x * blockDim.x) >> lg;
-  constexpr int U = VEC ? kSgUnroll : kSgUnroll / 2;   // the scalar path's loads take more registers
-  int ignored = 0;
-  for (int64_t c = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> lg; c < nch_all; c += step) {
-    const int64_t p = key_upper_bound(P.chunk_off, P.E + 1, c) - 1;
-    const int64_t c0 = __ldg(P.chunk_off + p), nch = __ldg(P.chunk_off + p + 1) - c0;
-    const int64_t b = __ldg(P.start + p) + (c - c0) * kSegChunk;
-    const int64_t e = min(b + kSegChunk, (int64_t)__ldg(P.start + p + 1));
-    float* o = nch == 1 ? sg_out_row(out, P, p, dim, by_key) : P.partial + (int64_t)(__ldg(P.part_off + p) + (c - c0)) * dim;
-    for (int d = sub * 4; d < dim; d += G * 4) {
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int64_t k0 = b; k0 < e; k0 += U) {
-        float4 x[U];
-        float w[U];
-#pragma unroll
-        for (int q = 0; q < U; ++q) {
-          if (k0 + q < e) {
-            const int64_t en = __ldg(perm + k0 + q);
-            if (en < S.n_src) {
-              x[q] = sg_load<VEC>(S.gt + en * dim, d, dim);
-              w[q] = 1.f;
-            } else {
-              const int64_t t = en - S.n_src;
-              x[q] = sg_load<VEC>(S.target + sg_row(__ldg(S.src + t / S.J), S.n_rows, &ignored) * dim, d, dim);
-              w[q] = __ldg(S.coef + t);
-            }
-          }
-        }
-#pragma unroll
-        for (int q = 0; q < U; ++q) {
-          if (k0 + q < e) {
-            acc.x = __fmaf_rn(w[q], x[q].x, acc.x); acc.y = __fmaf_rn(w[q], x[q].y, acc.y);
-            acc.z = __fmaf_rn(w[q], x[q].z, acc.z); acc.w = __fmaf_rn(w[q], x[q].w, acc.w);
-          }
-        }
-      }
-      if (VEC) {
-        *reinterpret_cast<float4*>(o + d) = acc;
-      } else {
-        o[d] = acc.x;
-        if (d + 1 < dim) o[d + 1] = acc.y;
-        if (d + 2 < dim) o[d + 2] = acc.z;
-        if (d + 3 < dim) o[d + 3] = acc.w;
-      }
-    }
-  }
-}
-
-// the output row of each segment of several chunks = its partial rows added in chunk order from +0; rows (sparse, may be
-// null) gets the segments' row ids
-__global__ void k_sg_combine(DistinctPlan P, int dim, bool by_key, float* __restrict__ out, int64_t* __restrict__ rows) {
-  const int64_t D = __ldg(P.nd);
-  if (rows)
-    for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D; t += (int64_t)gridDim.x * blockDim.x)
-      rows[t] = __ldg(P.key + t);
-  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D * dim; t += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t p = t / dim, f = t - p * dim;
-    const int64_t nch = __ldg(P.chunk_off + p + 1) - __ldg(P.chunk_off + p);
-    if (nch == 1) continue;
-    const float* part = P.partial + (int64_t)__ldg(P.part_off + p) * dim + f;
-    float acc = 0.f;
-    for (int64_t j = 0; j < nch; ++j) acc = __fadd_rn(acc, __ldg(part + j * dim));
-    sg_out_row(out, P, p, dim, by_key)[f] = acc;
-  }
-}
-
 static int sg_check(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
                     const float* target, const float* context, int64_t n_rows, int32_t dim, const char* who) {
   if (!c || B < 0 || P < 1 || K < 0 || n_rows < 1 || dim < 1 || !target || !context ||
@@ -346,7 +218,7 @@ static int sg_check(eu_ctx* c, const int64_t* src, const int64_t* pos, const int
 // A list of E > 0 entries to sum per distinct row: its keys, order and plan in the scratch at m + off (sg_list_bytes)
 struct SgList {
   int64_t E = 0;
-  SgEntries S;
+  RowEntries S;
   bool ctx_entries = false;
   int32_t* key = nullptr;
   EdgeOrder ord;
@@ -375,16 +247,7 @@ static int sg_plan(eu_ctx* c, const int64_t* src, const int64_t* pos, const int6
 // the chunk sums and their combination of list L into out (by_key: a dense table; else COO values, with their row ids in rows)
 static int sg_sum(eu_ctx* c, const SgList& L, int dim, bool by_key, float* out, int64_t* rows) {
   if (!L.E) return EU_OK;
-  cudaStream_t s = c->stream;
-  const bool vec = dim % 4 == 0 && aligned16(out) && aligned16(L.S.target) && (!L.S.gt || aligned16(L.S.gt));
-  const int G = group_lanes(ceil_div(dim, 4));
-  const unsigned blocks = stride_grid((L.E + L.E / kSegChunk + 1) * G);
-  if (vec) k_sg_chunks<true><<<blocks, 256, 0, s>>>(L.S, L.ord.perm, L.P, dim, G, by_key, out);
-  else k_sg_chunks<false><<<blocks, 256, 0, s>>>(L.S, L.ord.perm, L.P, dim, G, by_key, out);
-  EU_LAUNCHED();
-  k_sg_combine<<<stride_grid(L.E * dim), 256, 0, s>>>(L.P, dim, by_key, out, rows);
-  EU_LAUNCHED();
-  return EU_OK;
+  return sum_distinct_rows(c, L.S, L.E, L.ord.perm, L.P, dim, by_key, out, rows);
 }
 
 // The backward pass both output forms share.  shared: one list into the target outputs.  sparse: the COO of
@@ -488,7 +351,7 @@ int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const in
     else k_sg_fwd<false><<<blocks, 256, 0, s>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
     EU_LAUNCHED();
   }
-  k_sg_total<<<1, kSgSumThreads, 0, s>>>(rowloss, B, B * (int64_t)(P + K), loss);
+  k_f64_mean<<<1, kMeanThreads, 0, s>>>(rowloss, B, B * (int64_t)(P + K), loss);
   EU_LAUNCHED();
   int h = 0;
   EU_CUDA(cudaMemcpyAsync(&h, bad, sizeof(int), cudaMemcpyDeviceToHost, s));

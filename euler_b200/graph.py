@@ -156,6 +156,35 @@ class Graph:
         fn = getattr(_lib.load(), "eu_graph_edge_%s_feature_id" % kind)
         return fn(self._h, str(name).encode())
 
+    def set_edges(self, src, dst, type, weight=None, dense=None, dense_dims=None, dense_names=None):
+        """Attach edge records (eu_graph_set_edges) for sample_edge and the edge feature ops, as an Euler directory's Edge
+        files do: src, dst [E] node ids, type [E] edge types, weight [E] (default 1.0).  dense: f32[E, F], the dense slots
+        concatenated per edge, with their widths dense_dims (default one slot of F) and names dense_names (default feat0,
+        feat1, ...; the knowledge-graph models read the relation id from a slot named 'id')."""
+        src, dst, typ = _np(src, np.uint64), _np(dst, np.uint64), _np(type, np.int32)
+        n = len(src)
+        if len(dst) != n or len(typ) != n:
+            raise EulerError("set_edges: src, dst and type must have one length")
+        keep = [src, dst, typ, _np(weight, np.float32)]
+        d = _lib.EdgeDesc()
+        d.n_edges = n
+        d.src, d.dst, d.type, d.w = map(_ptr, keep)
+        names = list(dense_names or ())
+        if dense is not None:
+            feat = np.ascontiguousarray(np.asarray(dense, dtype=np.float32).reshape(n, -1))
+            dims = _np(dense_dims if dense_dims is not None else [feat.shape[1]], np.int32)
+            if int(dims.sum()) != feat.shape[1] or (names and len(names) != len(dims)):
+                raise EulerError("set_edges: dense_dims must add up to dense's width, one name per slot")
+            keep += [feat, dims]
+            d.feat_dim, d.feat, d.n_feat_slots, d.feat_slot_dims = feat.shape[1], _ptr(feat), len(dims), _ptr(dims)
+        elif names:
+            raise EulerError("set_edges: dense_names without dense")
+        lib = _lib.load()
+        check(lib.eu_graph_set_edges(self._h, C.byref(d)))
+        for k, name in enumerate(names):
+            check(lib.eu_graph_set_edge_dense_feature_name(self._h, k, str(name).encode()))
+        return self
+
     @property
     def num_edge_records(self):
         """edges attached for sample_edge / edge features (0 when the graph was built without them)"""

@@ -1394,3 +1394,145 @@ def skipgram_xent_loss(src, pos, negs, target, context, metric='mrr', sparse_gra
     context = target if shared else _t(context, torch.float32)
     loss, rank = _SkipgramLoss.apply(target, context, src, pos.contiguous(), negs.contiguous(), shared, bool(sparse_grad))
     return loss, skipgram_metric(rank, metric)
+
+
+# ------------------------------------------------------------------------------------ knowledge-graph embedding step
+KG_MODELS = {'transe': 0, 'transh': 1, 'transr': 2, 'transd': 3, 'distmult': 4}
+KG_CORRUPT = {'front': 1, 'tail': 2, 'both': 3}
+# the tables each model takes, in order, and the slot of eu_kg_problem.table each one fills
+_KG_SLOTS = {0: (0, 1), 1: (0, 1, 3), 2: (0, 1, 3), 3: (0, 1, 2, 3), 4: (0, 1)}
+
+
+def _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, rel_dim):
+    p = _lib.KgProblem()
+    p.model, p.l1, p.corrupt, p.margin = model, int(bool(l1)), corrupt, float(margin)
+    p.B, p.K = src.numel(), neg.shape[1]
+    p.ent_dim, p.rel_dim = ent_dim, rel_dim
+    p.n_ent, p.n_rel = slots[0].shape[0], slots[1].shape[0]
+    p.src, p.dst, p.rel, p.neg = src.data_ptr(), dst.data_ptr(), rel.data_ptr(), neg.data_ptr()
+    for t, tb in enumerate(slots):
+        p.table[t] = tb.data_ptr() if tb is not None else None
+    return p
+
+
+def _raw_kg(ent, relt, eaux, raux, src, dst, rel, neg, cfg):
+    """one eu_kg_loss: (scores f32[B, 1 + C K], rank i32[B], loss f32[], [src_emb, rel_emb, dst_emb] or None)"""
+    model, l1, corrupt, margin, ent_dim, rel_dim, sparse_grad, with_emb = cfg
+    B, K = neg.shape
+    dev = ent.device
+    scores = torch.empty((B, 1 + (2 if corrupt == 3 else 1) * K), dtype=torch.float32, device=dev)
+    rank = torch.empty(B, dtype=torch.int32, device=dev)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    embs = [torch.empty((B, rel_dim), dtype=torch.float32, device=dev) for _ in range(3)] if with_emb else None
+    p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, (ent, relt, eaux, raux), ent_dim, rel_dim)
+    e_ptr = [e.data_ptr() for e in embs] if embs else [None] * 3
+    check(_lib.load().eu_kg_loss(_ctx_on_stream()._h, C.byref(p), scores.data_ptr(), rank.data_ptr(), loss.data_ptr(), *e_ptr))
+    return scores, rank, loss, embs
+
+
+class _KgLoss(torch.autograd.Function):
+    """eu_kg_loss / eu_kg_loss_backward(_sparse).  Saves the ids and the scores (and the tables, which are inputs): no
+    [B, K, dim] rows are kept.  The four table slots are entity, relation, entity-side and relation-side auxiliary (None when
+    the model has none)."""
+
+    @staticmethod
+    def forward(ctx, ent, relt, eaux, raux, src, dst, rel, neg, cfg):
+        scores, rank, loss, embs = _raw_kg(ent, relt, eaux, raux, src, dst, rel, neg, cfg)
+        ctx.save_for_backward(ent, relt, eaux, raux, src, dst, rel, neg, scores)
+        ctx.cfg = cfg
+        ctx.mark_non_differentiable(rank, *(embs or []))
+        if embs:
+            return (loss, rank) + tuple(embs)
+        return loss, rank
+
+    @staticmethod
+    def backward(ctx, g_loss, *unused):
+        ent, relt, eaux, raux, src, dst, rel, neg, scores = ctx.saved_tensors
+        model, l1, corrupt, margin, ent_dim, rel_dim, sparse_grad, _ = ctx.cfg
+        slots = (ent, relt, eaux, raux)
+        dev = ent.device
+        g = g_loss.to(device=dev, dtype=torch.float32).reshape(1).contiguous()
+        p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, rel_dim)
+        ec, lib = _ctx_on_stream(), _lib.load()
+        P4 = C.c_void_p * 4
+        if not sparse_grad:
+            grads = [torch.empty_like(t) if t is not None else None for t in slots]
+            check(lib.eu_kg_loss_backward(ec._h, C.byref(p), g.data_ptr(), scores.data_ptr(),
+                                          P4(*[t.data_ptr() if t is not None else None for t in grads])))
+            return tuple(grads) + (None,) * 5
+        B, K = neg.shape
+        entries = (B * (K + 2), B, B * (K + 2), B)
+        rows, vals = [], []
+        for t, tb in enumerate(slots):
+            if tb is None:
+                rows.append(None)
+                vals.append(None)
+                continue
+            cap = min(entries[t], tb.shape[0])
+            rows.append(torch.empty(cap, dtype=torch.int64, device=dev))
+            vals.append(torch.empty((cap, tb.shape[1]), dtype=torch.float32, device=dev))
+        counts = (C.c_int64 * 4)()
+        check(lib.eu_kg_loss_backward_sparse(ec._h, C.byref(p), g.data_ptr(), scores.data_ptr(),
+                                             P4(*[r.data_ptr() if r is not None else None for r in rows]),
+                                             P4(*[v.data_ptr() if v is not None else None for v in vals]), counts))
+        grads = []
+        for t, tb in enumerate(slots):
+            if tb is None:
+                grads.append(None)
+                continue
+            n = counts[t]
+            grads.append(torch.sparse_coo_tensor(rows[t][:n].unsqueeze(0), vals[t][:n], tuple(tb.shape), is_coalesced=True,
+                                                 check_invariants=False))
+        return tuple(grads) + (None,) * 5
+
+
+def kg_margin_loss(src, dst, neg, rel, tables, model, l1=True, corrupt='both', margin=1.0, metric='mrr', sparse_grad=False,
+                   with_embeddings=False):
+    """The step after the ids of Euler's knowledge-graph models (examples/TransX TransX.call, examples/distmult) in one fused
+    device op:
+        src, dst [B] or [B, 1]   entity ids of the true triples      rel [B] or [B, 1]   their relation ids (int64)
+        neg [B, K]               entity ids of the corruptions (K >= 1)
+        tables                   f32 tables by model: 'transe' / 'distmult' (entity, relation); 'transh' (entity, relation,
+                                 hyper); 'transr' (entity, relation, transfer_matrix [n_rel, ent_dim * rel_dim]); 'transd'
+                                 (entity, relation, entity_transfer, relation_transfer)
+    Scores each triple and its corruptions ('front': (neg_k, r, d), 'tail': (s, r, neg_k), 'both': front then tail) on the
+    mapped rows (include/euler_b200.h, eu_kg_loss), and returns (loss, metric): loss = mean_b max(margin + mean_k neg - pos, 0),
+    metric the ranking metric `metric` (skipgram_metric: mrr, hit1, hit3, hit10, mr) of the true triple among its corruptions,
+    ties ranked as TF's stable top_k ranks them.  with_embeddings=True appends the mapped (src, rel, dst) rows f32[B, rel_dim]
+    (not differentiated).  The gradient reaches the tables only: dense, or with sparse_grad=True coalesced sparse COO gradients
+    of the rows the batch touches.  Deterministic, no atomics; the forward and the backward synchronise once each."""
+    name = str(model).lower()
+    if name not in KG_MODELS:
+        raise EulerError("kg_margin_loss: model must be one of %s, got %r" % (sorted(KG_MODELS), model))
+    if corrupt not in KG_CORRUPT:
+        raise EulerError("kg_margin_loss: corrupt must be one of %s, got %r" % (sorted(KG_CORRUPT), corrupt))
+    if metric not in SKIPGRAM_METRICS:
+        raise EulerError("kg_margin_loss: metric must be one of %s, got %r" % (SKIPGRAM_METRICS, metric))
+    m = KG_MODELS[name]
+    want = _KG_SLOTS[m]
+    tables = list(tables)
+    if len(tables) != len(want):
+        raise EulerError("kg_margin_loss: %s takes %d tables, got %d" % (name, len(want), len(tables)))
+    for tb in tables:
+        if not torch.is_tensor(tb) or tb.dtype != torch.float32 or tb.dim() != 2:
+            raise EulerError("kg_margin_loss: tables must be 2-D float32 tensors")
+    slots = [None] * 4
+    for t, tb in zip(want, tables):
+        slots[t] = _t(tb, torch.float32)
+    ent_dim, rel_dim = slots[0].shape[1], slots[1].shape[1]
+    aux_w = {1: ent_dim, 2: ent_dim * rel_dim, 3: rel_dim}.get(m)
+    if (slots[2] is not None and tuple(slots[2].shape) != tuple(slots[0].shape)) or \
+       (slots[3] is not None and (slots[3].shape[0] != slots[1].shape[0] or slots[3].shape[1] != aux_w)):
+        raise EulerError("kg_margin_loss: the auxiliary tables of %s must match the entity / relation tables" % name)
+    src = _t(src, torch.int64).reshape(-1)
+    dst = _t(dst, torch.int64).reshape(-1)
+    rel = _t(rel, torch.int64).reshape(-1)
+    neg = _t(neg, torch.int64)
+    B = src.numel()
+    if dst.numel() != B or rel.numel() != B or neg.dim() != 2 or neg.shape[0] != B:
+        raise EulerError("kg_margin_loss: src, dst, rel must have B = %d ids and neg be [B, K], got %s, %s, %s"
+                         % (B, dst.numel(), rel.numel(), tuple(neg.shape)))
+    cfg = (m, bool(l1), KG_CORRUPT[corrupt], float(margin), ent_dim, rel_dim, bool(sparse_grad), bool(with_embeddings))
+    out = _KgLoss.apply(slots[0], slots[1], slots[2], slots[3], src, dst, rel, neg, cfg)
+    res = (out[0], skipgram_metric(out[1], metric))
+    return res + tuple(out[2:]) if with_embeddings else res

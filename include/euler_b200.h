@@ -137,6 +137,9 @@ typedef struct {
 int eu_graph_set_edges(eu_graph* g, const eu_edge_desc* desc);
 int64_t eu_graph_num_edge_records(const eu_graph* g);
 int32_t eu_graph_edge_dense_feature_id(const eu_graph* g, const char* name);
+/* Rename dense edge slot fid (eu_graph_set_edges names them feat0, feat1, ...), e.g. to 'id' for the knowledge-graph models'
+ * relation ids.  EU_ERR_INVALID for an unknown slot. */
+int eu_graph_set_edge_dense_feature_name(eu_graph* g, int32_t fid, const char* name);
 int32_t eu_graph_edge_sparse_feature_id(const eu_graph* g, const char* name);
 int32_t eu_graph_edge_binary_feature_id(const eu_graph* g, const char* name);
 int eu_graph_destroy(eu_graph* g);
@@ -390,6 +393,58 @@ int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const in
                                      int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
                                      int32_t dim, const float* logits, int64_t* rows_target, float* values_target,
                                      int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context);
+
+/* The knowledge-graph embedding step of TransE / TransH / TransR / TransD (examples/TransX) and DistMult (examples/distmult),
+ * fused: the mapped id rows of each triple and of its corrupted triples, the scores, the margin loss and the rank.
+ * Triple b: src_b, dst_b (entity ids), rel_b (relation id), neg[b, 0 .. K-1] (entity ids); ids are table rows.
+ * Tables (device f32; table[t] for t = 0 .. 3): entity [n_ent, ent_dim], relation [n_rel, rel_dim], the entity-side
+ * auxiliary (TransD's entity_transfer [n_ent, ent_dim], else NULL) and the relation-side one (TransH's hyper [n_rel, ent_dim],
+ * TransR's transfer matrix [n_rel, ent_dim * rel_dim] read as [ent_dim, rel_dim], TransD's relation_transfer [n_rel, rel_dim],
+ * else NULL).  With n(x) = x / sqrt(max(sum x^2, 1e-12)) and r = n(relation[rel_b]), an entity row e maps to n(e) (TransE,
+ * DistMult), e - (e . h) h with h = n(hyper[rel_b]) (TransH), n(e M) (TransR), n(e + (e . et) rt) (TransD); a triple (a, r, c)
+ * scores -||(a + r) - c|| in L1 or L2 (l1) or sum a (r c) (DistMult).  Each relation row is normalised over its own rel_dim.
+ * Outputs (device):
+ *   scores f32[B, 1 + C K]: the true triple, then (corrupt 1 'front', 2 'tail', 3 'both' = C 2) the K front corruptions
+ *                           (neg_k, r, d), then the K tail corruptions (s, r, neg_k);
+ *   rank i32[B]:            #{j : neg_j >= pos}, TF's stable top_k position of the last entry of concat([neg, pos]);
+ *   loss f32[1]:            mean over b of max((margin + mean_j neg_j) - pos_b, 0): the negative mean a fixed-order f32 sum (see
+ *                           csrc/kg.cu), the row losses added in f64 and divided once by B (B = 0: NaN);
+ *   src_emb, rel_emb, dst_emb f32[B, rel_dim] (optional, all or none): the mapped rows of the triple.
+ * Every reduction has a fixed order that depends on the dims only.  No [B, K, dim] rows are formed: a block maps its triple's
+ * rows once, stages TransR's matrix in shared memory and scores a tile of 256 negatives.
+ * The backward passes take grad_loss (a device f32 scalar) and the forward's scores.  A row is active when its hinge argument
+ * is >= 0 (TF's maximum on equality); L1 differentiates |x| as sign(x) (0 at 0), L2 gives 0 where ||x|| = 0 (TF: NaN), and
+ * n(x) passes no gradient to sum x^2 below 1e-12.  One entry per (triple, table row touched): entity entries src, dst, each
+ * (b, k) with its front and tail terms summed; one relation and one relation-side entry per triple.  The entries of a table
+ * are summed per distinct row in the stable row order in 256-entry chunks (see eu_skipgram_loss_backward): no atomics, the same
+ * bits on every run.  Scratch O(B (K + 2) dim) (TransR: plus B ent_dim rel_dim floats), never O(n_rows); one synchronisation.
+ *   eu_kg_loss_backward:        grads[t] f32 dense gradient of table t (zero on untouched rows; NULL for an absent table);
+ *   eu_kg_loss_backward_sparse: the coalesced COO of table t: rows[t] i64[D] ascending, values[t] f32[D, width], counts[t] = D
+ *                               (host); arrays of min(entries, table rows) rows: B (K + 2) for the entity-side tables, B for the
+ *                               relation-side ones.
+ * K < 1, B < 0, a missing table the model needs, ent_dim != rel_dim outside TransR, or an id outside its table: EU_ERR_INVALID;
+ * a dim above 512, a TransR ent_dim * rel_dim above 16384, 2^31 table rows or B (K + 2) entries: EU_ERR_UNSUPPORTED. */
+enum { EU_KG_TRANSE = 0, EU_KG_TRANSH = 1, EU_KG_TRANSR = 2, EU_KG_TRANSD = 3, EU_KG_DISTMULT = 4 };
+typedef struct {
+  int32_t model;            /* EU_KG_* */
+  int32_t l1;               /* TransX: 1 = L1 distance, 0 = L2 */
+  int32_t corrupt;          /* 1 front, 2 tail, 3 both */
+  float margin;
+  int64_t B;
+  int32_t K;                /* negatives per triple, >= 1 */
+  int32_t ent_dim, rel_dim;
+  int64_t n_ent, n_rel;     /* rows of the entity-side and the relation-side tables */
+  const int64_t* src;       /* [B] */
+  const int64_t* dst;       /* [B] */
+  const int64_t* rel;       /* [B] */
+  const int64_t* neg;       /* [B, K] */
+  const float* table[4];    /* entity, relation, entity-side auxiliary, relation-side auxiliary */
+} eu_kg_problem;
+int eu_kg_loss(eu_ctx* c, const eu_kg_problem* p, float* scores, int32_t* rank, float* loss, float* src_emb, float* rel_emb,
+               float* dst_emb);
+int eu_kg_loss_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, float* const* grads);
+int eu_kg_loss_backward_sparse(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, int64_t* const* rows,
+                               float* const* values, int64_t* counts);
 
 /* tf_euler.sample_edge -- TF op SampleEdge (tf_euler/kernels/sample_edge_op.cc; Graph::SampleEdge graph.cc:277-301): `count`
  * edges of ONE type drawn by the alias method over the edge weights, out i64[count,3] = (src, dst, type).  Several types or
