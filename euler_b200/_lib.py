@@ -50,6 +50,30 @@ class KgProblem(C.Structure):
     ]
 
 
+SHALLOW_MAX_SLOTS = 8   # EU_SHALLOW_MAX_SLOTS
+SHALLOW_MAX_WIDTH = 16384   # EU_SHALLOW_MAX_WIDTH
+
+
+class ShallowDense(C.Structure):
+    """eu_shallow_dense"""
+    _fields_ = [("fid", C.c_int32), ("dim", C.c_int32)]
+
+
+class ShallowSparse(C.Structure):
+    """eu_shallow_sparse"""
+    _fields_ = [("fid", C.c_int32), ("dim", C.c_int32), ("combiner", C.c_int32), ("reserved", C.c_int32),
+                ("default_value", C.c_int64), ("n_rows", C.c_int64), ("table", C.c_void_p)]
+
+
+class ShallowProblem(C.Structure):
+    """eu_shallow_problem"""
+    _fields_ = [
+        ("combiner", C.c_int32), ("id_dim", C.c_int32), ("M", C.c_int64), ("nodes", C.c_void_p), ("id_table", C.c_void_p),
+        ("n_id_rows", C.c_int64), ("n_dense", C.c_int32), ("n_sparse", C.c_int32),
+        ("dense", ShallowDense * SHALLOW_MAX_SLOTS), ("sparse", ShallowSparse * SHALLOW_MAX_SLOTS),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/euler_b200.h declares
 _P, _I64, _I32, _U64, _F = C.c_void_p, C.c_int64, C.c_int32, C.c_uint64, C.c_float
 SIGNATURES = {
@@ -151,6 +175,10 @@ SIGNATURES = {
     "eu_dna_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P, _P]),
     "eu_sparse_embedding_lookup": (C.c_int, [_P, _P, _I64, _I32, _I64, _P, _I64, _I32, _I32, _P]),
     "eu_sparse_embedding_lookup_backward": (C.c_int, [_P, _P, _P, _I64, _I32, _I64, _I64, _I32, _I32, _P]),
+    "eu_sparse_embedding_lookup_backward_sparse": (C.c_int, [_P, _P, _P, _I64, _I32, _I64, _I64, _I32, _I32, _P, _P, _P]),
+    "eu_shallow_encode": (C.c_int, [_P, _P, _P, _P]),
+    "eu_shallow_encode_backward": (C.c_int, [_P, _P, _P, _P]),
+    "eu_shallow_encode_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "eu_gather_host": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P]),
     "eu_scatter_add_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),
     "eu_scatter_max_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),

@@ -1,26 +1,31 @@
 // SparseEmbedding's lookup from node ids, forward and backward: the uint64 ("sparse") slot of each node, turned into one
-// f32 row by an embedding table, with no host round trip and no intermediate COO.
+// f32 row by an embedding table, with no host round trip and no intermediate COO.  And ShallowEncoder's whole input row (an
+// id embedding, dense feature slots and several such lookups, concatenated or added) in one pass over the nodes.
 //
 // Reference semantics (file:line in the upstream alibaba/euler tree):
 //   SparseEmbedding.call      tf_euler/python/utils/layers.py:152-169  tf.nn.embedding_lookup_sparse(table, sp_ids, None,
 //                                                                       combiner), default combiner 'sum'
 //   its input                 tf_euler/kernels/get_sparse_feature_op.cc:52-130  the node's values of the slot in stored
 //                             order; a node without values (absent id, empty or unknown slot) gets one entry, the default
-//   callers                   tf_euler/python/utils/encoders.py:151-160 (ShallowEncoder), :590-612 (SageEncoderNew)
+//   ShallowEncoder.call       tf_euler/python/utils/encoders.py:134-171  [Embedding(ids), get_dense_feature, SparseEmbedding
+//                             per slot], then concat or add_n
 //
 // Forward, for node i with bag v_0 .. v_{n-1} (n >= 1):
 //   acc = table[v_0]; acc = __fadd_rn(acc, table[v_k]) for k = 1 .. n-1   (from the first row, not from +0)
 //   out_i = acc (sum), __fdiv_rn(acc, fl(n)) (mean), __fdiv_rn(acc, __fsqrt_rn(fl(n))) (sqrtn)
 // A group of G lanes per node: the bag's values are loaded G at a time, one per lane, and broadcast by shuffle; kEmbUnroll
-// table rows are loaded ahead of the ordered adds.  float4 loads when dim % 4 == 0 and table / out are 16-byte aligned,
-// scalar otherwise: the same adds in the same order, so the bits do not depend on the alignment.  No scratch, no
-// synchronisation: the forward is capturable in a CUDA graph.
+// table rows are loaded ahead of the ordered adds (emb_bag_sum, which both forward kernels call).  float4 loads when
+// dim % 4 == 0 and table / out are 16-byte aligned, scalar otherwise: the same adds in the same order, so the bits do not
+// depend on the alignment.  No scratch, no synchronisation: the forward is capturable in a CUDA graph.
 //
 // Backward, grad_table[v] = sum over the entries (i, k) with v_k = v of s_i(g_i), where s_i is the identity (sum),
-// __fdiv_rn(., fl(n_i)) (mean) or __fdiv_rn(., __fsqrt_rn(fl(n_i))) (sqrtn), elementwise.  The entries are listed again from
-// the graph, ordered stably by value (order_by) and summed per distinct value in fixed chunks of kSegChunk entries
-// (plan_distinct, segment.cuh): deterministic, no atomics, and a hot value (the default fills every empty slot) is spread
-// over many CTAs.  Rows no entry touches are zero.
+// __fdiv_rn(., fl(n_i)) (mean) or __fdiv_rn(., __fsqrt_rn(fl(n_i))) (sqrtn), elementwise.  The entries of every table are
+// listed again from the graph in one pass over the nodes, ordered stably by value (order_by) and summed per distinct value in
+// fixed chunks of kSegChunk entries (plan_distinct, segment.cuh): deterministic, no atomics, and a hot value (the default
+// fills every empty slot) is spread over many CTAs.  The sums go to a dense table (rows no entry touches are zero) or to a
+// coalesced COO of the rows touched.
+#include <cub/device/device_scan.cuh>
+
 #include "segment.cuh"
 
 namespace eu {
@@ -37,6 +42,7 @@ template <> struct EmbVec<true> {
   static constexpr int W = 4;
   static __device__ __forceinline__ T zero(float z) { return make_float4(z, z, z, z); }
   static __device__ __forceinline__ T load(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+  static __device__ __forceinline__ T load_rw(const float* p) { return *reinterpret_cast<const float4*>(p); }   // written by this kernel
   static __device__ __forceinline__ void store(float* p, T v) { *reinterpret_cast<float4*>(p) = v; }
   static __device__ __forceinline__ T add(T a, T b) {
     return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
@@ -50,28 +56,27 @@ template <> struct EmbVec<false> {
   static constexpr int W = 1;
   static __device__ __forceinline__ T zero(float z) { return z; }
   static __device__ __forceinline__ T load(const float* p) { return __ldg(p); }
+  static __device__ __forceinline__ T load_rw(const float* p) { return *p; }
   static __device__ __forceinline__ void store(float* p, T v) { *p = v; }
   static __device__ __forceinline__ T add(T a, T b) { return __fadd_rn(a, b); }
   static __device__ __forceinline__ T div(T a, float den) { return __fdiv_rn(a, den); }
 };
 
-// G lanes per node r, W columns per lane and step; blocks of G * W columns with a group-uniform trip count, so every lane of
+// The bag sum of graph row `row` (-1: absent) in slot fid, before the combiner's division: G lanes (this one is `sub`, the
+// group's mask gm), W columns per lane and step, blocks of G * W columns with a group-uniform trip count, so every lane of
 // the group takes part in the shuffles.  The sum starts from the bag's first row (its bits, -0.0 and NaN payloads included).
-template <bool VEC>
-__global__ void __launch_bounds__(256, 1) k_emb_fwd(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t M, int32_t fid,
-                                                 unsigned long long dflt, const float* __restrict__ table, int dim, int G, int comb,
-                                                 float* __restrict__ out) {
+// *n = the bag's entries (1 for the default); it is set before the first sink(d, acc) call, which hands over the lane's
+// columns [d, d + W) of the sum, for d < dim only.
+template <bool VEC, typename Sink>
+__device__ __forceinline__ void emb_bag_sum(const DevGraph& g, int64_t row, int32_t fid, unsigned long long dflt,
+                                            const float* __restrict__ table, int dim, int G, int sub, unsigned gm, int64_t* n_out,
+                                            Sink sink) {
   using V = EmbVec<VEC>;
-  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  const int64_t r = tid >> (31 - __clz(G));
-  const int sub = (int)(tid & (G - 1));
-  if (r >= M) return;   // group-uniform
-  const unsigned gm = group_mask(G);
   int64_t b, e;
-  ragged_slice(g.u64_ptr, g.n_u64_slots, lookup_row(g, __ldg(nodes + r)), fid, &b, &e);
+  ragged_slice(g.u64_ptr, g.n_u64_slots, row, fid, &b, &e);
   const bool empty = e == b;
   const int64_t n = empty ? 1 : e - b;
-  const float den = emb_den(n, comb);
+  *n_out = n;
   for (int d0 = 0; d0 < dim; d0 += G * V::W) {
     const int d = d0 + sub * V::W;
     const bool act = d < dim;
@@ -91,55 +96,188 @@ __global__ void __launch_bounds__(256, 1) k_emb_fwd(DevGraph g, const unsigned l
           if (j0 + q < cnt) acc = k0 + j0 + q == 0 ? x[q] : V::add(acc, x[q]);
       }
     }
-    if (act) V::store(out + r * (int64_t)dim + d, acc);
+    if (act) sink(d, acc);
   }
+}
+
+// G lanes per node r (a power of two)
+template <bool VEC>
+__global__ void __launch_bounds__(256, 1) k_emb_fwd(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t M, int32_t fid,
+                                                 unsigned long long dflt, const float* __restrict__ table, int dim, int G, int comb,
+                                                 float* __restrict__ out) {
+  using V = EmbVec<VEC>;
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t r = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (r >= M) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  float* o = out + r * (int64_t)dim;
+  int64_t n;
+  emb_bag_sum<VEC>(g, lookup_row(g, __ldg(nodes + r)), fid, dflt, table, dim, G, sub, gm, &n,
+                   [&](int d, typename V::T acc) { V::store(o + d, acc); });
   if (comb == EU_COMBINE_SUM) return;
   // mean / sqrtn: one division per column, in a pass of its own over the row this group just wrote (L1-resident), so that
   // nothing of the bag loop is live across the division's slow-path subroutine
   __syncwarp(gm);
-  float* o = out + r * (int64_t)dim;
+  const float den = emb_den(n, comb);
   for (int d = sub; d < dim; d += G) o[d] = __fdiv_rn(o[d], den);
 }
 
-// One warp per node i: the value (as the sort key) and the node of each of its entries, at [ptr[i], ptr[i + 1])
-__global__ void __launch_bounds__(256) k_emb_entries(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t M, int32_t fid,
-                                                     int32_t dflt, const int64_t* __restrict__ ptr, int32_t* __restrict__ key,
-                                                     int32_t* __restrict__ node) {
-  const int lane = threadIdx.x & 31;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  for (int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; i < M; i += nwarps) {
-    int64_t b, e;
-    ragged_slice(g.u64_ptr, g.n_u64_slots, lookup_row(g, __ldg(nodes + i)), fid, &b, &e);
-    const int64_t o = __ldg(ptr + i);
-    if (e == b) {
-      if (lane == 0) { key[o] = dflt; node[o] = (int32_t)i; }
-      continue;
-    }
-    for (int64_t k = lane; k < e - b; k += 32) {
-      key[o + k] = (int32_t)__ldg(g.u64_val + b + k);
-      node[o + k] = (int32_t)i;
+// ---------------------------------------------------------------------------- ShallowEncoder's row
+struct ShallowDev {   // eu_shallow_problem, resolved for the device: column offsets, and which slots take float4 loads
+  const unsigned long long* nodes;
+  int64_t M;
+  int W, add;                      // out's width; EU_SHALLOW_ADD
+  const float* id_table;
+  int64_t n_id_rows;
+  int id_dim;
+  int n_dense, dense_w;            // dense_w: dense_out's width (ADD)
+  int32_t dense_fid[EU_SHALLOW_MAX_SLOTS];
+  int dense_dim[EU_SHALLOW_MAX_SLOTS], dense_off[EU_SHALLOW_MAX_SLOTS];
+  int n_sparse;
+  unsigned vec_mask;               // bit s: slot s's table and out columns take float4 loads and stores
+  int32_t sp_fid[EU_SHALLOW_MAX_SLOTS];
+  int sp_dim[EU_SHALLOW_MAX_SLOTS], sp_comb[EU_SHALLOW_MAX_SLOTS], sp_off[EU_SHALLOW_MAX_SLOTS];
+  unsigned long long sp_dflt[EU_SHALLOW_MAX_SLOTS];
+  const float* sp_table[EU_SHALLOW_MAX_SLOTS];
+  float* out;
+  float* dense_out;
+};
+
+// slot s of node row `row` into o (its first column): stored (CONCAT, or the first term of ADD) or added to what o holds
+template <bool VEC>
+__device__ __forceinline__ void shallow_slot(const DevGraph& g, const ShallowDev& p, int s, int64_t row, float* o, bool first, int G,
+                                             int sub, unsigned gm) {
+  using V = EmbVec<VEC>;
+  const int comb = p.sp_comb[s];
+  int64_t n;
+  emb_bag_sum<VEC>(g, row, p.sp_fid[s], p.sp_dflt[s], p.sp_table[s], p.sp_dim[s], G, sub, gm, &n, [&](int d, typename V::T acc) {
+    if (comb != EU_COMBINE_SUM) acc = V::div(acc, emb_den(n, comb));
+    V::store(o + d, first ? acc : V::add(V::load_rw(o + d), acc));
+  });
+}
+
+// G lanes per node r: the id columns, the dense slots (k_feature's rule: the stored columns, zeros past them, zeros for an
+// absent node or an unknown slot), then the sparse slots.  The group syncs between parts: a part may map columns to lanes
+// differently from the one before it, and ADD reads what the previous part wrote.
+__global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, int G) {
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t r = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (r >= p.M) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  const unsigned long long id = __ldg(p.nodes + r);
+  float* o = p.out + r * (int64_t)p.W;
+  if (p.id_table) {
+    const bool ok = (long long)id >= 0 && (long long)id < p.n_id_rows;   // false only under capture (the check is skipped)
+    const float* t = p.id_table + (ok ? (int64_t)id : 0) * p.id_dim;
+    for (int d = sub; d < p.id_dim; d += G) o[d] = ok ? __ldg(t + d) : __int_as_float(0x7fc00000);
+  }
+  const int64_t row = lookup_row(g, id);
+  float* od = p.add ? p.dense_out + r * (int64_t)p.dense_w : o;
+  for (int j = 0; j < p.n_dense; ++j) {
+    const int32_t fid = p.dense_fid[j];
+    const bool have = fid >= 0 && fid < g.n_slots && row >= 0;
+    const int sdim = have ? g.slot_dim[fid] : 0;
+    const float* f = g.feat + (have ? row * (int64_t)g.feat_dim + g.slot_off[fid] : 0);
+    float* oj = od + p.dense_off[j];
+    for (int d = sub; d < p.dense_dim[j]; d += G) oj[d] = d < sdim ? __ldg(f + d) : 0.f;
+  }
+  for (int s = 0; s < p.n_sparse; ++s) {
+    __syncwarp(gm);
+    const bool first = !p.add || (s == 0 && !p.id_table);
+    float* os = o + p.sp_off[s];
+    if (p.vec_mask >> s & 1) shallow_slot<true>(g, p, s, row, os, first, G, sub, gm);
+    else shallow_slot<false>(g, p, s, row, os, first, G, sub, gm);
+  }
+}
+
+// *bad = 1 when an id lies outside [0, n_rows)
+__global__ void k_id_range(const int64_t* __restrict__ ids, int64_t M, int64_t n_rows, int* bad) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t v = __ldg(ids + i);
+    if (v < 0 || v >= n_rows) *bad = 1;
+  }
+}
+
+// ---------------------------------------------------------------------------- backward
+// The tables of one backward pass: the uint64 slots s < S (their bags), then optionally the id table (the node ids).  Each
+// one's gradient rows are grad_out[i, col .. col + dim) with row stride ld.
+struct EmbTables {
+  int S = 0;
+  int32_t fid[EU_SHALLOW_MAX_SLOTS] = {};
+  unsigned long long dflt[EU_SHALLOW_MAX_SLOTS] = {};
+  int comb[EU_SHALLOW_MAX_SLOTS] = {};
+  bool has_id = false;
+  int64_t n_rows[EU_SHALLOW_MAX_SLOTS + 1] = {}, col[EU_SHALLOW_MAX_SLOTS + 1] = {};
+  int dim[EU_SHALLOW_MAX_SLOTS + 1] = {};
+};
+struct EmbSlots {   // the device copy of the slots' ids and defaults
+  int32_t fid[EU_SHALLOW_MAX_SLOTS];
+  unsigned long long dflt[EU_SHALLOW_MAX_SLOTS];
+};
+
+// len[s * (M + 1) + i + 1] = the entries of node i in slot s (1 for the default), len[s * (M + 1)] = 0: one inclusive scan over
+// all S (M + 1) then gives slot s's entries of node i at [ptr[s (M + 1) + i], ptr[s (M + 1) + i + 1]), the slots one after another
+__global__ void k_emb_lengths(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t M, EmbSlots sl, int S,
+                              long long* __restrict__ len) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t row = lookup_row(g, __ldg(nodes + i));
+    for (int s = 0; s < S; ++s) {
+      int64_t b, e;
+      ragged_slice(g.u64_ptr, g.n_u64_slots, row, sl.fid[s], &b, &e);
+      len[s * (M + 1) + i + 1] = e == b ? 1 : e - b;
+      if (i == 0) len[s * (M + 1)] = 0;
     }
   }
 }
 
-// gs[i, d] = g[i, d] / den(n_i) (one __fdiv_rn), n_i = ptr[i + 1] - ptr[i]: the scaled gradient of the mean and sqrtn
+// One warp per node i: the key (the row) and the node of each of its entries in every slot, and its id entry at id_base + i
+// (id_base < 0: no id table)
+__global__ void __launch_bounds__(256) k_emb_entries(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t M, EmbSlots sl,
+                                                     int S, const int64_t* __restrict__ ptr, int64_t id_base, int32_t* __restrict__ key,
+                                                     int32_t* __restrict__ node) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; i < M; i += nwarps) {
+    const unsigned long long id = __ldg(nodes + i);
+    const int64_t row = lookup_row(g, id);
+    if (id_base >= 0 && lane == 0) { key[id_base + i] = (int32_t)id; node[id_base + i] = (int32_t)i; }
+    for (int s = 0; s < S; ++s) {
+      int64_t b, e;
+      ragged_slice(g.u64_ptr, g.n_u64_slots, row, sl.fid[s], &b, &e);
+      const int64_t o = __ldg(ptr + s * (M + 1) + i);
+      if (e == b) {
+        if (lane == 0) { key[o] = (int32_t)sl.dflt[s]; node[o] = (int32_t)i; }
+        continue;
+      }
+      for (int64_t k = lane; k < e - b; k += 32) {
+        key[o + k] = (int32_t)__ldg(g.u64_val + b + k);
+        node[o + k] = (int32_t)i;
+      }
+    }
+  }
+}
+
+// gs[i, d] = g[i * ld + d] / den(n_i) (one __fdiv_rn), n_i = ptr[i + 1] - ptr[i]: the scaled gradient of the mean and sqrtn
 // combiners, once per node and column rather than once per entry
-__global__ void k_emb_scale_grad(const float* __restrict__ g, const int64_t* __restrict__ ptr, int64_t M, int dim, int comb,
+__global__ void k_emb_scale_grad(const float* __restrict__ g, int64_t ld, const int64_t* __restrict__ ptr, int64_t M, int dim, int comb,
                                  float* __restrict__ gs) {
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < M * dim; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = t / dim;
-    gs[t] = __fdiv_rn(__ldg(g + t), emb_den(__ldg(ptr + i + 1) - __ldg(ptr + i), comb));
+    gs[t] = __fdiv_rn(__ldg(g + i * ld + (t - i * dim)), emb_den(__ldg(ptr + i + 1) - __ldg(ptr + i), comb));
   }
 }
 
 // G lanes per chunk c of the distinct-value segments (grid-stride over the chunks, whose number is on the device).  Chunk
 // c - chunk_off[p] of segment p covers the sorted positions [start[p] + (c - chunk_off[p]) * kSegChunk, ...), up to kSegChunk
-// of them: the sum, left to right from +0, of the (scaled) gradient rows gs of their nodes.  A segment of one chunk writes
-// its table row; the chunks of a longer one write their partial rows for k_emb_bwd_combine.
+// of them: the sum, left to right from +0, of the (scaled) gradient rows gs[node * ld] of their nodes.  A segment of one chunk
+// writes its output row (by_key: the table row key[p]; else row p of the COO values); the chunks of a longer one write their
+// partial rows for k_row_combine.
 template <bool VEC>
-__global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restrict__ gs, const int32_t* __restrict__ node,
-                                                        const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G,
-                                                        float* __restrict__ grad_table) {
+__global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restrict__ gs, int64_t ld, const int32_t* __restrict__ node,
+                                                        const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G, bool by_key,
+                                                        float* __restrict__ out) {
   using V = EmbVec<VEC>;
   const int lg = 31 - __clz(G);
   const int sub = (int)(threadIdx.x & (G - 1));
@@ -150,14 +288,14 @@ __global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restri
     const int64_t c0 = __ldg(P.chunk_off + p), nch = __ldg(P.chunk_off + p + 1) - c0;
     const int64_t b = __ldg(P.start + p) + (c - c0) * kSegChunk;
     const int64_t e = min(b + kSegChunk, (int64_t)__ldg(P.start + p + 1));
-    float* o = nch == 1 ? grad_table + (int64_t)__ldg(P.key + p) * dim : P.partial + (int64_t)(__ldg(P.part_off + p) + (c - c0)) * dim;
+    float* o = nch == 1 ? out + (by_key ? (int64_t)__ldg(P.key + p) : p) * dim : P.partial + (int64_t)(__ldg(P.part_off + p) + (c - c0)) * dim;
     for (int d = sub * V::W; d < dim; d += G * V::W) {
       typename V::T acc = V::zero(0.f);
       for (int64_t k0 = b; k0 < e; k0 += kEmbUnroll) {
         typename V::T x[kEmbUnroll];
 #pragma unroll
         for (int q = 0; q < kEmbUnroll; ++q)
-          if (k0 + q < e) x[q] = V::load(gs + (int64_t)__ldg(node + __ldg(perm + k0 + q)) * dim + d);
+          if (k0 + q < e) x[q] = V::load(gs + (int64_t)__ldg(node + __ldg(perm + k0 + q)) * ld + d);
 #pragma unroll
         for (int q = 0; q < kEmbUnroll; ++q)
           if (k0 + q < e) acc = V::add(acc, x[q]);
@@ -167,34 +305,9 @@ __global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restri
   }
 }
 
-// grad_table[key[p], f] = the partial rows of segment p added in chunk order from +0, for the segments of several chunks
-__global__ void k_emb_bwd_combine(DistinctPlan P, int dim, float* __restrict__ grad_table) {
-  const int64_t n = (int64_t)__ldg(P.nd) * dim;
-  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n; t += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t p = t / dim, f = t - p * dim;
-    const int64_t nch = __ldg(P.chunk_off + p + 1) - __ldg(P.chunk_off + p);
-    if (nch == 1) continue;
-    const float* part = P.partial + (int64_t)__ldg(P.part_off + p) * dim + f;
-    float acc = 0.f;
-    for (int64_t j = 0; j < nch; ++j) acc = __fadd_rn(acc, __ldg(part + j * dim));
-    grad_table[(int64_t)__ldg(P.key + p) * dim + f] = acc;
-  }
-}
-
-// The checks both passes share.  Every value of slot fid and the default must index the table: the slot's largest value is
-// kept on the graph, so this costs no device work.
-static int emb_check(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const float* table, int64_t n_rows,
-                     int32_t dim, int32_t combiner, const void* out, const char* who) {
-  if (!c || M < 0 || n_rows < 1 || dim < 1 || combiner < EU_COMBINE_SUM || combiner > EU_COMBINE_SQRTN || (M > 0 && (!nodes || !out)) ||
-      !table) {
-    set_error("%s: bad argument", who);
-    return EU_ERR_INVALID;
-  }
-  if (M >= ((int64_t)1 << 31) || n_rows >= ((int64_t)1 << 31)) {
-    set_error("%s: 2^31 or more nodes or table rows are not supported", who);
-    return EU_ERR_UNSUPPORTED;
-  }
-  const eu_graph* g = c->g;
+// The checks of one uint64 slot and its table.  Every value of slot fid and the default must index the table: the slot's
+// largest value is kept on the graph, so this costs no device work.
+static int emb_slot_check(const eu_graph* g, int32_t fid, int64_t default_value, int64_t n_rows, const char* who) {
   if (default_value < 0 || default_value >= n_rows) {
     set_error("%s: default_value %lld lies outside the table's rows [0, %lld)", who, (long long)default_value, (long long)n_rows);
     return EU_ERR_INVALID;
@@ -203,6 +316,249 @@ static int emb_check(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, in
     set_error("%s: slot %d holds the value %llu, outside the table's rows [0, %lld)", who, (int)fid,
               (unsigned long long)g->u64_slot_max[fid], (long long)n_rows);
     return EU_ERR_INVALID;
+  }
+  return EU_OK;
+}
+
+// The checks the passes of the single-slot op share; ok: the pass's own table / output pointers are given.
+static int emb_check(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, bool ok, int64_t n_rows,
+                     int32_t dim, int32_t combiner, const void* out, const char* who) {
+  if (!c || M < 0 || n_rows < 1 || dim < 1 || combiner < EU_COMBINE_SUM || combiner > EU_COMBINE_SQRTN || (M > 0 && (!nodes || !out)) ||
+      !ok) {
+    set_error("%s: bad argument", who);
+    return EU_ERR_INVALID;
+  }
+  if (M >= ((int64_t)1 << 31) || n_rows >= ((int64_t)1 << 31)) {
+    set_error("%s: 2^31 or more nodes or table rows are not supported", who);
+    return EU_ERR_UNSUPPORTED;
+  }
+  return emb_slot_check(c->g, fid, default_value, n_rows, who);
+}
+
+// *bad_host = whether an id of ids [M] lies outside [0, n_rows): one kernel and one synchronisation
+static int id_range_check(eu_ctx* c, const int64_t* ids, int64_t M, int64_t n_rows, bool* bad_host) {
+  int rc = ctx_misc(c, 256);
+  if (rc) return rc;
+  int* bad = (int*)c->d_misc;
+  EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), c->stream));
+  k_id_range<<<stride_grid(M), 256, 0, c->stream>>>(ids, M, n_rows, bad);
+  EU_LAUNCHED();
+  int h = 0;
+  EU_CUDA(cudaMemcpyAsync(&h, bad, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  EU_CUDA(cudaStreamSynchronize(c->stream));
+  *bad_host = h != 0;
+  return EU_OK;
+}
+
+// The gradients of the tables T over the nodes [M] (checked by the caller), from grad_out with row stride ld.  Dense
+// (rows == null): grads[t] f32[n_rows_t, dim_t], zeroed first.  Sparse: the COO rows[t] / grads[t] with counts[t] (host).
+// Table t < S is slot t, table S the id table.
+static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int64_t M, const float* grad_out, int64_t ld,
+                        float* const* grads, int64_t* const* rows, int64_t* counts, const char* who) {
+  EU_CUDA(cudaSetDevice(c->g->device));
+  cudaStream_t s = c->stream;
+  const bool sparse = rows != nullptr;
+  const int S = T.S, NT = S + (T.has_id ? 1 : 0);
+  if (!sparse)
+    for (int t = 0; t < NT; ++t) EU_CUDA(cudaMemsetAsync(grads[t], 0, 4 * (size_t)T.n_rows[t] * T.dim[t], s));
+  if (sparse)
+    for (int t = 0; t < NT; ++t) counts[t] = 0;
+  if (M == 0) return EU_OK;
+  EmbSlots sl;
+  for (int k = 0; k < S; ++k) { sl.fid[k] = T.fid[k]; sl.dflt[k] = T.dflt[k]; }
+  // flag, the distinct counts (256 B) | ptr [S (M + 1)] | scan temp | then, once the entry counts are known:
+  // key [E] | node [E] | scaled gradients [M, dim] | one table's order and plan (reused table after table)
+  const int64_t NP = (int64_t)S * (M + 1);
+  const size_t o_ptr = 256, o_tmp = o_ptr + a256(8 * (size_t)NP), tmp = S ? ragged_scan_bytes(NP - 1) : 0, o_key = o_tmp + a256(tmp);
+  auto entry_ptr = [&]() -> int {
+    if (!S) return EU_OK;
+    k_emb_lengths<<<stride_grid(M), 256, 0, s>>>(c->g->d, (const unsigned long long*)nodes, M, sl, S, (long long*)((char*)c->d_misc + o_ptr));
+    EU_LAUNCHED();
+    long long* p = (long long*)((char*)c->d_misc + o_ptr);
+    size_t t = tmp;
+    EU_CUDA(cub::DeviceScan::InclusiveSum((char*)c->d_misc + o_tmp, t, p, p, (int)NP, s));
+    EU_LAUNCHED();
+    return EU_OK;
+  };
+  int rc = ctx_misc(c, (int64_t)o_key);
+  if (rc) return rc;
+  int* bad = (int*)c->d_misc;
+  EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  if (T.has_id) {
+    k_id_range<<<stride_grid(M), 256, 0, s>>>(nodes, M, T.n_rows[S], bad);
+    EU_LAUNCHED();
+  }
+  if ((rc = entry_ptr())) return rc;
+  int64_t h_end[EU_SHALLOW_MAX_SLOTS] = {};
+  int h_bad = 0;
+  EU_CUDA(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
+  for (int k = 0; k < S; ++k)
+    EU_CUDA(cudaMemcpyAsync(h_end + k, (int64_t*)((char*)c->d_misc + o_ptr) + k * (M + 1) + M, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  EU_CUDA(cudaStreamSynchronize(s));
+  if (h_bad) {
+    set_error("%s: a node id lies outside the id table's rows [0, %lld)", who, (long long)T.n_rows[S]);
+    return EU_ERR_INVALID;
+  }
+  int64_t base[EU_SHALLOW_MAX_SLOTS + 1], E_t[EU_SHALLOW_MAX_SLOTS + 1];
+  for (int k = 0; k < S; ++k) { base[k] = k ? h_end[k - 1] : 0; E_t[k] = h_end[k] - base[k]; }
+  const int64_t E = (S ? h_end[S - 1] : 0) + (T.has_id ? M : 0);
+  if (T.has_id) { base[S] = E - M; E_t[S] = M; }
+  if (E + E / kSegChunk + 1 >= ((int64_t)1 << 31)) {
+    set_error("%s: 2^31 or more entries are not supported", who);
+    return EU_ERR_UNSUPPORTED;
+  }
+  int scaled_dim = 0;
+  size_t region = 0;
+  for (int t = 0; t < NT; ++t) {
+    if (t < S && T.comb[t] != EU_COMBINE_SUM) scaled_dim = std::max(scaled_dim, T.dim[t]);
+    region = std::max(region, order_bytes(E_t[t], T.n_rows[t]) + distinct_plan_bytes(E_t[t], T.dim[t]));
+  }
+  const size_t o_node = o_key + a256(4 * (size_t)E), o_gs = o_node + a256(4 * (size_t)E), o_reg = o_gs + a256(4 * (size_t)M * scaled_dim);
+  const size_t total = o_reg + region;
+  if ((int64_t)total > c->misc_bytes) {   // the growth reallocates: the offsets again (no read-back needed)
+    if ((rc = ctx_misc(c, (int64_t)total))) return rc;
+    if ((rc = entry_ptr())) return rc;
+  }
+  char* m = (char*)c->d_misc;
+  int32_t* nd_copy = (int32_t*)(m + 64);
+  const int64_t* ptr = (const int64_t*)(m + o_ptr);
+  int32_t* key = (int32_t*)(m + o_key);
+  int32_t* node = (int32_t*)(m + o_node);
+  {
+    EuProfScope ps(c, "emb_bwd_entries", E);
+    k_emb_entries<<<stride_grid(M * 32), 256, 0, s>>>(c->g->d, (const unsigned long long*)nodes, M, sl, S, ptr, T.has_id ? base[S] : -1,
+                                                      key, node);
+    EU_LAUNCHED();
+  }
+  for (int t = 0; t < NT; ++t) {
+    const int dim = T.dim[t];
+    EdgeOrder ord;
+    DistinctPlan P;
+    {
+      EuProfScope ps(c, "emb_bwd_order", E_t[t]);
+      if ((rc = order_by(c, key + base[t], E_t[t], T.n_rows[t], m + o_reg, &ord))) return rc;
+      if ((rc = plan_distinct(c, ord, E_t[t], m + o_reg + order_bytes(E_t[t], T.n_rows[t]), &P))) return rc;
+    }
+    EuProfScope ps(c, "emb_bwd_sums", E_t[t]);
+    const float* gs = grad_out + T.col[t];
+    int64_t gld = ld;
+    if (t < S && T.comb[t] != EU_COMBINE_SUM) {
+      float* scaled = (float*)(m + o_gs);
+      k_emb_scale_grad<<<stride_grid(M * dim), 256, 0, s>>>(gs, ld, ptr + t * (M + 1), M, dim, T.comb[t], scaled);
+      EU_LAUNCHED();
+      gs = scaled;
+      gld = dim;
+    }
+    float* out = grads[t];
+    const bool vec = dim % 4 == 0 && gld % 4 == 0 && aligned16(gs) && aligned16(out);
+    const int G = group_lanes(ceil_div(dim, vec ? 4 : 1));
+    const unsigned blocks = stride_grid((E_t[t] + E_t[t] / kSegChunk + 1) * G);   // >= one group per chunk, up to the grid cap
+    if (vec) k_emb_bwd_chunks<true><<<blocks, 256, 0, s>>>(gs, gld, node + base[t], ord.perm, P, dim, G, !sparse, out);
+    else k_emb_bwd_chunks<false><<<blocks, 256, 0, s>>>(gs, gld, node + base[t], ord.perm, P, dim, G, !sparse, out);
+    EU_LAUNCHED();
+    k_row_combine<<<stride_grid(E_t[t] * dim), 256, 0, s>>>(P, dim, !sparse, out, sparse ? rows[t] : nullptr);
+    EU_LAUNCHED();
+    if (sparse) EU_CUDA(cudaMemcpyAsync(nd_copy + t, P.nd, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+  }
+  if (!sparse) return EU_OK;
+  int32_t h_nd[EU_SHALLOW_MAX_SLOTS + 1] = {};
+  EU_CUDA(cudaMemcpyAsync(h_nd, nd_copy, sizeof(int32_t) * NT, cudaMemcpyDeviceToHost, s));
+  EU_CUDA(cudaStreamSynchronize(s));
+  for (int t = 0; t < NT; ++t) counts[t] = h_nd[t];
+  return EU_OK;
+}
+
+// The single-slot op as a one-table backward pass
+static int single_backward(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value,
+                           int64_t n_rows, int32_t dim, int32_t combiner, float* out, int64_t* rows, int64_t* n, const char* who) {
+  EmbTables T;
+  T.S = 1;
+  T.fid[0] = fid;
+  T.dflt[0] = (unsigned long long)default_value;
+  T.comb[0] = combiner;
+  T.n_rows[0] = n_rows;
+  T.dim[0] = dim;
+  float* g[1] = {out};
+  int64_t* r[1] = {rows};
+  return emb_backward(c, T, nodes, M, grad_out, dim, g, rows ? r : nullptr, n, who);
+}
+
+// The checks of a shallow problem, and its device form (out / dense_out filled in by the caller).  *T: its backward tables.
+static int shallow_resolve(eu_ctx* c, const eu_shallow_problem* p, ShallowDev* d, EmbTables* T, const char* who) {
+  if (!c || !p || p->M < 0 || (p->M > 0 && !p->nodes) || (p->combiner != EU_SHALLOW_CONCAT && p->combiner != EU_SHALLOW_ADD) ||
+      p->n_dense < 0 || p->n_sparse < 0 || (p->id_table && (p->n_id_rows < 1 || p->id_dim < 1))) {
+    set_error("%s: bad argument", who);
+    return EU_ERR_INVALID;
+  }
+  if (p->n_dense > EU_SHALLOW_MAX_SLOTS || p->n_sparse > EU_SHALLOW_MAX_SLOTS) {
+    set_error("%s: at most %d dense and %d sparse slots are supported", who, EU_SHALLOW_MAX_SLOTS, EU_SHALLOW_MAX_SLOTS);
+    return EU_ERR_UNSUPPORTED;
+  }
+  *d = ShallowDev();
+  *T = EmbTables();
+  const bool add = p->combiner == EU_SHALLOW_ADD;
+  int64_t w = p->id_table ? p->id_dim : 0, dw = 0, emb_dim = p->id_table ? p->id_dim : -1;
+  d->n_dense = p->n_dense;
+  for (int j = 0; j < p->n_dense; ++j) {
+    if (p->dense[j].dim < 0) {
+      set_error("%s: dense slot %d has dim %d", who, j, (int)p->dense[j].dim);
+      return EU_ERR_INVALID;
+    }
+    d->dense_fid[j] = p->dense[j].fid;
+    d->dense_dim[j] = p->dense[j].dim;
+    d->dense_off[j] = (int)std::min<int64_t>(add ? dw : w, EU_SHALLOW_MAX_WIDTH + 1);
+    (add ? dw : w) += p->dense[j].dim;
+  }
+  d->n_sparse = T->S = p->n_sparse;
+  for (int k = 0; k < p->n_sparse; ++k) {
+    const eu_shallow_sparse& q = p->sparse[k];
+    if (!q.table || q.n_rows < 1 || q.dim < 1 || q.combiner < EU_COMBINE_SUM || q.combiner > EU_COMBINE_SQRTN) {
+      set_error("%s: sparse slot %d: bad argument", who, k);
+      return EU_ERR_INVALID;
+    }
+    if (add && emb_dim >= 0 && q.dim != emb_dim) {
+      set_error("%s: 'add' needs one dim for every embedding, got %lld and %d", who, (long long)emb_dim, (int)q.dim);
+      return EU_ERR_INVALID;
+    }
+    emb_dim = q.dim;
+    if (q.n_rows >= ((int64_t)1 << 31)) {
+      set_error("%s: tables of 2^31 or more rows are not supported", who);
+      return EU_ERR_UNSUPPORTED;
+    }
+    int rc = emb_slot_check(c->g, q.fid, q.default_value, q.n_rows, who);
+    if (rc) return rc;
+    d->sp_fid[k] = T->fid[k] = q.fid;
+    d->sp_dflt[k] = T->dflt[k] = (unsigned long long)q.default_value;
+    d->sp_comb[k] = T->comb[k] = q.combiner;
+    d->sp_dim[k] = T->dim[k] = q.dim;
+    d->sp_table[k] = q.table;
+    d->sp_off[k] = (int)std::min<int64_t>(add ? 0 : w, EU_SHALLOW_MAX_WIDTH + 1);
+    T->n_rows[k] = q.n_rows;
+    T->col[k] = d->sp_off[k];
+    if (!add) w += q.dim;
+  }
+  if (add) w = std::max<int64_t>(emb_dim, 0);
+  if (w > EU_SHALLOW_MAX_WIDTH || dw > EU_SHALLOW_MAX_WIDTH) {
+    set_error("%s: rows of more than %d columns are not supported", who, EU_SHALLOW_MAX_WIDTH);
+    return EU_ERR_UNSUPPORTED;
+  }
+  if (p->M >= ((int64_t)1 << 31) || p->n_id_rows >= ((int64_t)1 << 31)) {
+    set_error("%s: 2^31 or more nodes or table rows are not supported", who);
+    return EU_ERR_UNSUPPORTED;
+  }
+  d->nodes = (const unsigned long long*)p->nodes;
+  d->M = p->M;
+  d->W = (int)w;
+  d->add = add;
+  d->id_table = p->id_table;
+  d->n_id_rows = p->n_id_rows;
+  d->id_dim = p->id_table ? p->id_dim : 0;
+  d->dense_w = (int)dw;
+  T->has_id = p->id_table != nullptr;
+  if (T->has_id) {
+    T->n_rows[T->S] = p->n_id_rows;
+    T->dim[T->S] = p->id_dim;
+    T->col[T->S] = 0;
   }
   return EU_OK;
 }
@@ -216,7 +572,7 @@ extern "C" {
 int eu_sparse_embedding_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const float* table,
                                int64_t n_rows, int32_t dim, int32_t combiner, float* out) {
   const char* who = "eu_sparse_embedding_lookup";
-  int rc = emb_check(c, nodes, M, fid, default_value, table, n_rows, dim, combiner, out, who);
+  int rc = emb_check(c, nodes, M, fid, default_value, table != nullptr, n_rows, dim, combiner, out, who);
   if (rc) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   if (M == 0) return EU_OK;
@@ -235,60 +591,101 @@ int eu_sparse_embedding_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32
 int eu_sparse_embedding_lookup_backward(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
                                         int64_t default_value, int64_t n_rows, int32_t dim, int32_t combiner, float* grad_table) {
   const char* who = "eu_sparse_embedding_lookup_backward";
-  int rc = emb_check(c, nodes, M, fid, default_value, grad_table, n_rows, dim, combiner, grad_out, who);
+  int rc = emb_check(c, nodes, M, fid, default_value, grad_table != nullptr, n_rows, dim, combiner, grad_out, who);
   if (rc) return rc;
+  return single_backward(c, grad_out, nodes, M, fid, default_value, n_rows, dim, combiner, grad_table, nullptr, nullptr, who);
+}
+
+int eu_sparse_embedding_lookup_backward_sparse(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
+                                               int64_t default_value, int64_t n_rows, int32_t dim, int32_t combiner, int64_t* rows,
+                                               float* values, int64_t* n) {
+  const char* who = "eu_sparse_embedding_lookup_backward_sparse";
+  int rc = emb_check(c, nodes, M, fid, default_value, n && (M == 0 || (rows && values)), n_rows, dim, combiner, grad_out, who);
+  if (rc) return rc;
+  return single_backward(c, grad_out, nodes, M, fid, default_value, n_rows, dim, combiner, values, rows, n, who);
+}
+
+int eu_shallow_encode(eu_ctx* c, const eu_shallow_problem* p, float* out, float* dense_out) {
+  const char* who = "eu_shallow_encode";
+  ShallowDev d;
+  EmbTables T;
+  int rc = shallow_resolve(c, p, &d, &T, who);
+  if (rc) return rc;
+  if (p->M > 0 && ((d.W > 0 && !out) || (d.add && d.dense_w > 0 && !dense_out))) {
+    set_error("%s: bad argument (out%s is required)", who, d.add ? " and dense_out" : "");
+    return EU_ERR_INVALID;
+  }
   EU_CUDA(cudaSetDevice(c->g->device));
-  cudaStream_t s = c->stream;
-  EU_CUDA(cudaMemsetAsync(grad_table, 0, 4 * (size_t)n_rows * dim, s));
-  if (M == 0) return EU_OK;
-  // ptr [M + 1] | scan temp | then, once the entry count E is known: key [E] | node [E] | the order by value | the plan
-  const size_t o_tmp = a256(8 * (size_t)(M + 1)), tmp = ragged_scan_bytes(M), o_key = o_tmp + a256(tmp);
-  if ((rc = ctx_misc(c, (int64_t)o_key))) return rc;
-  if ((rc = sparse_entry_ptr(c, nodes, M, fid, (char*)c->d_misc + o_tmp, tmp, (int64_t*)c->d_misc))) return rc;
-  int64_t E = 0;
-  EU_CUDA(cudaMemcpyAsync(&E, (int64_t*)c->d_misc + M, sizeof(E), cudaMemcpyDeviceToHost, s));
-  EU_CUDA(cudaStreamSynchronize(s));
-  if (E + E / kSegChunk + 1 >= ((int64_t)1 << 31)) {
-    set_error("%s: 2^31 or more entries are not supported", who);
-    return EU_ERR_UNSUPPORTED;
+  if (p->M == 0 || (d.W == 0 && d.dense_w == 0)) return EU_OK;
+  if (p->id_table) {   // outside capture: every id must index the table before anything is written
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    EU_CUDA(cudaStreamIsCapturing(c->stream, &st));
+    if (st == cudaStreamCaptureStatusNone) {
+      bool bad = false;
+      if ((rc = id_range_check(c, p->nodes, p->M, p->n_id_rows, &bad))) return rc;
+      if (bad) {
+        set_error("%s: a node id lies outside the id table's rows [0, %lld)", who, (long long)p->n_id_rows);
+        return EU_ERR_INVALID;
+      }
+    }
   }
-  const size_t o_node = o_key + a256(4 * (size_t)E), o_ord = o_node + a256(4 * (size_t)E), o_plan = o_ord + order_bytes(E, n_rows);
-  const size_t o_gs = o_plan + distinct_plan_bytes(E, dim);
-  const size_t total = o_gs + (combiner == EU_COMBINE_SUM ? 0 : a256(4 * (size_t)M * dim));
-  if ((int64_t)total > c->misc_bytes) {   // the growth reallocates: the offsets again (no read-back needed)
-    if ((rc = ctx_misc(c, (int64_t)total))) return rc;
-    if ((rc = sparse_entry_ptr(c, nodes, M, fid, (char*)c->d_misc + o_tmp, tmp, (int64_t*)c->d_misc))) return rc;
+  d.out = out;
+  d.dense_out = dense_out;
+  int widest = d.id_dim;
+  for (int j = 0; j < d.n_dense; ++j) widest = std::max(widest, d.dense_dim[j]);
+  for (int k = 0; k < d.n_sparse; ++k) {
+    widest = std::max(widest, d.sp_dim[k]);
+    if (d.sp_dim[k] % 4 == 0 && aligned16(d.sp_table[k]) && aligned16(out) && d.W % 4 == 0 && d.sp_off[k] % 4 == 0) d.vec_mask |= 1u << k;
   }
-  char* m = (char*)c->d_misc;
-  const int64_t* ptr = (const int64_t*)m;
-  int32_t* key = (int32_t*)(m + o_key);
-  int32_t* node = (int32_t*)(m + o_node);
-  EdgeOrder ord;
-  DistinctPlan P;
-  {
-    EuProfScope ps(c, "emb_bwd_order", E);
-    k_emb_entries<<<stride_grid(M * 32), 256, 0, s>>>(c->g->d, (const unsigned long long*)nodes, M, fid, (int32_t)default_value, ptr, key,
-                                                      node);
-    EU_LAUNCHED();
-    if ((rc = order_by(c, key, E, n_rows, m + o_ord, &ord))) return rc;
-    if ((rc = plan_distinct(c, ord, E, m + o_plan, &P))) return rc;
-  }
-  EuProfScope ps(c, "emb_bwd_sums", E);
-  const float* gs = grad_out;
-  if (combiner != EU_COMBINE_SUM) {
-    float* scaled = (float*)(m + o_gs);
-    k_emb_scale_grad<<<stride_grid(M * dim), 256, 0, s>>>(grad_out, ptr, M, dim, combiner, scaled);
-    EU_LAUNCHED();
-    gs = scaled;
-  }
-  const bool vec = dim % 4 == 0 && aligned16(gs) && aligned16(grad_table);
-  const int G = group_lanes(ceil_div(dim, vec ? 4 : 1));
-  const unsigned blocks = stride_grid((E + E / kSegChunk + 1) * G);   // >= one group per chunk, up to the grid cap
-  if (vec) k_emb_bwd_chunks<true><<<blocks, 256, 0, s>>>(gs, node, ord.perm, P, dim, G, grad_table);
-  else k_emb_bwd_chunks<false><<<blocks, 256, 0, s>>>(gs, node, ord.perm, P, dim, G, grad_table);
+  const int G = group_lanes(ceil_div(widest, 4));
+  EuProfScope ps(c, "shallow_fwd", p->M);
+  k_shallow_fwd<<<(unsigned)ceil_div(p->M * G, 256), 256, 0, c->stream>>>(c->g->d, d, G);
   EU_LAUNCHED();
-  k_emb_bwd_combine<<<stride_grid(E * dim), 256, 0, s>>>(P, dim, grad_table);
-  EU_LAUNCHED();
+  return EU_OK;
+}
+
+int eu_shallow_encode_backward(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, float* const* grads) {
+  const char* who = "eu_shallow_encode_backward";
+  ShallowDev d;
+  EmbTables T;
+  int rc = shallow_resolve(c, p, &d, &T, who);
+  if (rc) return rc;
+  const int NT = T.S + (T.has_id ? 1 : 0);
+  bool ok = grads && (p->M == 0 || d.W == 0 || grad_out);
+  for (int t = 0; ok && t < NT; ++t) ok = grads[t == T.S ? 0 : t + 1] != nullptr;
+  if (!ok) {
+    set_error("%s: bad argument (grad_out and a gradient per table are required)", who);
+    return EU_ERR_INVALID;
+  }
+  float* g[EU_SHALLOW_MAX_SLOTS + 1];   // the ABI's order (id, slots) to the backward's (slots, id)
+  for (int t = 0; t < NT; ++t) g[t] = grads[t == T.S ? 0 : t + 1];
+  return emb_backward(c, T, p->nodes, p->M, grad_out, d.W, g, nullptr, nullptr, who);
+}
+
+int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, int64_t* const* rows,
+                                      float* const* values, int64_t* counts) {
+  const char* who = "eu_shallow_encode_backward_sparse";
+  ShallowDev d;
+  EmbTables T;
+  int rc = shallow_resolve(c, p, &d, &T, who);
+  if (rc) return rc;
+  const int NT = T.S + (T.has_id ? 1 : 0);
+  bool ok = rows && values && counts && (p->M == 0 || d.W == 0 || grad_out);
+  for (int t = 0; ok && t < NT && p->M > 0; ++t) ok = rows[t == T.S ? 0 : t + 1] && values[t == T.S ? 0 : t + 1];
+  if (!ok) {
+    set_error("%s: bad argument (grad_out and rows, values and counts per table are required)", who);
+    return EU_ERR_INVALID;
+  }
+  float* v[EU_SHALLOW_MAX_SLOTS + 1];
+  int64_t* r[EU_SHALLOW_MAX_SLOTS + 1];
+  int64_t n[EU_SHALLOW_MAX_SLOTS + 1] = {};
+  for (int t = 0; t < NT; ++t) {
+    v[t] = values[t == T.S ? 0 : t + 1];
+    r[t] = rows[t == T.S ? 0 : t + 1];
+  }
+  if ((rc = emb_backward(c, T, p->nodes, p->M, grad_out, d.W, v, r, n, who))) return rc;
+  for (int t = 0; t < NT; ++t) counts[t == T.S ? 0 : t + 1] = n[t];
+  if (!T.has_id) counts[0] = 0;
   return EU_OK;
 }
 

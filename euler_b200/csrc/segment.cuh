@@ -174,6 +174,9 @@ struct RowEntries {
 // the rows' ids in rows (may be null).  No atomics: the bits depend on each row's entry sequence only.
 int sum_distinct_rows(eu_ctx* c, const RowEntries& S, int64_t E, const int32_t* perm, const DistinctPlan& P, int dim, bool by_key,
                       float* out, int64_t* rows);
+// The second step of such sums: the output row of each segment of several chunks = its partial rows added in chunk order from
+// +0 (by_key: table row key[p] of out; else COO row p), and rows[p] = key[p] when rows is given.  Grid-stride over E * dim.
+__global__ void k_row_combine(DistinctPlan P, int dim, bool by_key, float* __restrict__ out, int64_t* __restrict__ rows);
 
 // *loss = fl32((sum of rowloss[0, B)) / N): thread t adds rowloss[t], rowloss[t + 1024], ... in f64, then a shared-memory tree
 // (strides 512 .. 1).  One block of kMeanThreads; N = 0 gives NaN, as a mean of nothing.

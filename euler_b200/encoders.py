@@ -1,15 +1,22 @@
 """SparseEmbedding (tf_euler/python/utils/layers.py:152-169), the embedding the sparse-feature encoders apply to uint64
-feature slots (ShallowEncoder, encoders.py:151-160; SageEncoderNew, encoders.py:590-612).
+feature slots (ShallowEncoder, encoders.py:151-160; SageEncoderNew, encoders.py:590-612), and ShallowEncoder
+(encoders.py:32-171), the input layer of the node encoders: an id embedding, dense feature slots and sparse-feature
+embeddings, concatenated or added.
 
 Callers size the table as the encoders do: SparseEmbedding(max_id + 1, dim) for values in [0, max_id] and
 default = max_id + 1 for nodes without values, so the table has max_id + 2 rows and the default row is the last one.
 
-Upstream quirk: ShallowEncoder's use_hash_embedding=True names layers.HashSparseEmbedding (encoders.py:117-119), which the
-reference tree does not define, so that option fails there; it is not provided here either.
+Upstream quirk: ShallowEncoder's use_hash_embedding=True names layers.HashEmbedding / layers.HashSparseEmbedding
+(encoders.py:108-119), which the reference tree does not define, so that option fails there; it raises here too.
 """
-import torch
+import functools
 
+import torch
+import torch.nn.functional as F
+
+from . import ops
 from .ops import sparse_feature_embedding
+from .unsupervised import Embedding
 
 
 def _truncated_normal_(t, stddev):
@@ -48,3 +55,148 @@ class SparseEmbedding(torch.nn.Module):
 
     def lookup(self, nodes, feature_name, default_value):
         return sparse_feature_embedding(nodes, feature_name, self.embeddings, default_value, self.combiner)
+
+
+class Dense(torch.nn.Module):
+    """layers.Dense(dim, use_bias=False) (utils/layers.py:70-116) over inputs of in_dim columns: a kernel [in_dim, dim]
+    initialised by tf.uniform_unit_scaling_initializer(factor=0.36), uniform in +-0.36 sqrt(3 / in_dim); x @ kernel."""
+
+    def __init__(self, in_dim, dim, device=None):
+        super().__init__()
+        bound = 0.36 * (3.0 / max(in_dim, 1)) ** 0.5
+        self.kernel = torch.nn.Parameter(torch.empty(in_dim, dim, device=device).uniform_(-bound, bound))
+
+    def forward(self, x):
+        return x @ self.kernel
+
+
+class ShallowEncoder(torch.nn.Module):
+    """encoders.ShallowEncoder (tf_euler/python/utils/encoders.py:32-171), with upstream's constructor arguments and
+    ValueErrors.  Each node's row is built from
+        max_id != -1               an id embedding: unsupervised.Embedding(max_id + 1, dim), a table of max_id + 2 rows
+        feature_idx != -1          the dense slots feature_idx with widths feature_dim (get_dense_feature)
+        sparse_feature_idx != -1   one SparseEmbedding(max_id_s + 1, dim) per uint64 slot, default value max_id_s + 1
+    combined by 'concat' (then the Dense layer when dim is given) or 'add' (every table dim columns; the dense features go
+    through the Dense layer first).  Dense is layers.Dense(dim, use_bias=False) (Dense above), built when dim is given.
+    output_dim follows upstream; __call__(inputs) takes node ids of any shape and returns inputs.shape + (output_dim,).
+
+    fused=True (the default) builds the row in one device op, ops.shallow_encode: 'concat' writes [id | dense | sparse]
+    exactly as the composition does; 'add' computes (id + sparse_0 + ..) + Dense(features), which differs from upstream's
+    add_n order id + Dense(features) + sparse_0 + .. only in float rounding.  sparse_grad=True gives the tables coalesced
+    sparse COO gradients (use an optimizer that takes them, e.g. torch.optim.SGD or SparseAdam).  fused=False runs the literal
+    composition: Embedding, get_dense_feature, get_sparse_feature + SparseEmbedding.__call__, then cat or add_n."""
+
+    def __init__(self, dim=None, feature_idx='f1', feature_dim=0, max_id=-1, sparse_feature_idx=-1, sparse_feature_max_id=-1,
+                 embedding_dim=16, use_hash_embedding=False, combiner='concat', fused=True, sparse_grad=False, device=None):
+        super().__init__()
+        if combiner not in ['add', 'concat']:
+            raise ValueError('combiner must be \'add\' or \'concat\'.')
+        if combiner == 'add' and dim is None:
+            raise ValueError('add must be used with dim provided.')
+        use_feature = feature_idx != -1
+        use_id = max_id != -1
+        use_sparse_feature = sparse_feature_idx != -1
+        if not isinstance(feature_idx, list) and use_feature:
+            feature_idx = [feature_idx]
+        if isinstance(feature_dim, int) and use_feature:
+            feature_dim = [feature_dim]
+        if use_feature and len(feature_idx) != len(feature_dim):
+            raise ValueError('feature_dim must be the same length as feature'
+                             '_idx.idx:%s, dim:%s' % (str(feature_idx), str(feature_dim)))
+        if isinstance(sparse_feature_idx, int) and use_sparse_feature:
+            sparse_feature_idx = [sparse_feature_idx]
+        if isinstance(sparse_feature_max_id, int) and use_sparse_feature:
+            sparse_feature_max_id = [sparse_feature_max_id]
+        if use_sparse_feature and len(sparse_feature_idx) != len(sparse_feature_max_id):
+            raise ValueError('sparse_feature_idx must be the same length as'
+                             'sparse_feature_max_id.')
+        embedding_num = (1 if use_id else 0) + (len(sparse_feature_idx) if use_sparse_feature else 0)
+        if combiner == 'add':
+            embedding_dim = dim
+        if isinstance(embedding_dim, int) and embedding_num:
+            embedding_dim = [embedding_dim] * embedding_num
+        if embedding_num and len(embedding_dim) != embedding_num:
+            raise ValueError('length of embedding_num must be int(use_id) + '
+                             'len(sparse_feature_idx)')
+        if isinstance(use_hash_embedding, bool) and embedding_num:
+            use_hash_embedding = [use_hash_embedding] * embedding_num
+        if embedding_num and len(use_hash_embedding) != embedding_num:
+            raise ValueError('length of use_hash_embedding must be int(use_id)'
+                             ' + len(sparse_feature_idx)')
+        if embedding_num and any(use_hash_embedding):
+            raise NotImplementedError('use_hash_embedding: layers.HashEmbedding / HashSparseEmbedding are not defined upstream')
+
+        self.dim = dim
+        self.use_id = use_id
+        self.use_feature = use_feature
+        self.use_sparse_feature = use_sparse_feature
+        self.combiner = combiner
+        self.feature_idx = feature_idx
+        self.feature_dim = feature_dim
+        self.sparse_feature_idx = sparse_feature_idx
+        self.sparse_feature_max_id = sparse_feature_max_id
+        self.embedding_dim = embedding_dim
+        self.fused = fused
+        self.sparse_grad = sparse_grad
+
+        dims = list(embedding_dim) if embedding_num else []
+        if use_id:
+            self.embedding = Embedding(max_id + 1, dims.pop(0), device=device)
+        if use_sparse_feature:
+            self.sparse_embeddings = torch.nn.ModuleList(
+                [SparseEmbedding(m + 1, d, device=device) for m, d in zip(sparse_feature_max_id, dims)])
+        if dim:
+            feat_w = sum(feature_dim) if use_feature else 0
+            in_dim = feat_w if combiner == 'add' else feat_w + (sum(embedding_dim) if embedding_num else 0)
+            self.dense = Dense(in_dim, dim, device=device)
+
+    @property
+    def output_dim(self):
+        if self.dim is not None:
+            return self.dim
+        output_dim = 0
+        if self.use_feature:
+            output_dim += sum(self.feature_dim)
+        if self.use_id or self.use_sparse_feature:
+            output_dim += sum(self.embedding_dim)
+        return output_dim
+
+    def _default_values(self):
+        return [m + 1 for m in self.sparse_feature_max_id]
+
+    def forward(self, inputs):
+        shape = tuple(inputs.shape)
+        nodes = inputs.reshape(-1)
+        out = self._fused(nodes) if self.fused else self._composed(nodes)
+        return out.reshape(shape + (self.output_dim,))
+
+    def _fused(self, nodes):
+        id_table = self.embedding.embeddings if self.use_id else None
+        dense = list(zip(self.feature_idx, self.feature_dim)) if self.use_feature else []
+        sparse = [(name, e.embeddings, dv, e.combiner) for name, e, dv in
+                  zip(self.sparse_feature_idx, self.sparse_embeddings, self._default_values())] if self.use_sparse_feature else []
+        if self.combiner == 'concat':
+            emb = ops.shallow_encode(nodes, id_table, dense, sparse, 'concat', self.sparse_grad)
+            return self.dense(emb) if self.dim else emb
+        emb, feats = ops.shallow_encode(nodes, id_table, dense, sparse, 'add', self.sparse_grad)
+        if feats is None:
+            return emb
+        feats = self.dense(feats)
+        return feats if id_table is None and not sparse else emb + feats
+
+    def _composed(self, nodes):
+        embeddings = []
+        if self.use_id:
+            embeddings.append(F.embedding(nodes, self.embedding.embeddings, sparse=self.sparse_grad))
+        if self.use_feature:
+            features = torch.cat(ops.get_dense_feature(nodes, self.feature_idx, self.feature_dim), -1)
+            if self.combiner == 'add':
+                features = self.dense(features)
+            embeddings.append(features)
+        if self.use_sparse_feature:
+            sparse_features = ops.get_sparse_feature(nodes, self.sparse_feature_idx, default_values=self._default_values())
+            embeddings.extend([e(sp) for e, sp in zip(self.sparse_embeddings, sparse_features)])
+        if self.combiner == 'add':
+            return functools.reduce(torch.add, embeddings)
+        embedding = torch.cat(embeddings, -1)
+        return self.dense(embedding) if self.dim else embedding

@@ -1118,40 +1118,186 @@ class _SparseEmbedding(torch.autograd.Function):
     entries again from the graph."""
 
     @staticmethod
-    def forward(ctx, table, nodes, fid, default_value, comb):
+    def forward(ctx, table, nodes, fid, default_value, comb, sparse_grad):
         out = _raw_embedding(nodes, fid, table, default_value, comb)
         if ctx.needs_input_grad[0]:
             ctx.save_for_backward(nodes)
-        ctx.args = (fid, default_value, comb, table.shape)
+        ctx.args = (fid, default_value, comb, table.shape, sparse_grad)
         return out
 
     @staticmethod
     def backward(ctx, grad):
         nodes, = ctx.saved_tensors
-        fid, default_value, comb, (n_rows, dim) = ctx.args
+        fid, default_value, comb, (n_rows, dim), sparse_grad = ctx.args
         grad = grad.contiguous()
-        g_t = torch.empty((n_rows, dim), dtype=torch.float32, device=grad.device)
-        ec = _ctx_on_stream()
-        check(_lib.load().eu_sparse_embedding_lookup_backward(ec._h, grad.data_ptr(), nodes.data_ptr(), nodes.numel(), fid, default_value,
-                                                              n_rows, dim, comb, g_t.data_ptr()))
-        return g_t, None, None, None, None
+        ec, lib = _ctx_on_stream(), _lib.load()
+        if not sparse_grad:
+            g_t = torch.empty((n_rows, dim), dtype=torch.float32, device=grad.device)
+            check(lib.eu_sparse_embedding_lookup_backward(ec._h, grad.data_ptr(), nodes.data_ptr(), nodes.numel(), fid, default_value,
+                                                          n_rows, dim, comb, g_t.data_ptr()))
+            return g_t, None, None, None, None, None
+        # the COO arrays hold min(entries, n_rows) rows: sized from the entries, never from a large table's rows
+        cap = min(_sparse_entries(nodes, fid), n_rows)
+        rows = torch.empty(cap, dtype=torch.int64, device=grad.device)
+        vals = torch.empty((cap, dim), dtype=torch.float32, device=grad.device)
+        n = C.c_int64()
+        check(lib.eu_sparse_embedding_lookup_backward_sparse(ec._h, grad.data_ptr(), nodes.data_ptr(), nodes.numel(), fid, default_value,
+                                                             n_rows, dim, comb, rows.data_ptr(), vals.data_ptr(), C.byref(n)))
+        return _coo(rows, vals, n.value, (n_rows, dim)), None, None, None, None, None
 
 
-def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner='sum'):
+def _sparse_entries(nodes, fid):
+    """the entries get_sparse_feature lists for nodes in slot fid (a node without values counts one): one lengths pass and
+    one read back"""
+    lib, ctx = _lib.load(), _ctx_on_stream()
+    indptr = torch.empty(nodes.numel() + 1, dtype=torch.int64, device=nodes.device)
+    check(lib.eu_get_sparse_feature(ctx._h, nodes.data_ptr(), nodes.numel(), int(fid), 0, 0, indptr.data_ptr(), None))
+    return int(indptr[-1].item())
+
+
+def _coo(rows, vals, n, shape):
+    """the coalesced sparse COO gradient of the first n rows / values"""
+    return torch.sparse_coo_tensor(rows[:n].unsqueeze(0), vals[:n], shape, is_coalesced=True, check_invariants=False)
+
+
+def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner='sum', sparse_grad=False):
     """SparseEmbedding over get_sparse_feature in one fused device op: row i is tf.nn.embedding_lookup_sparse(table, sp_ids,
     None, combiner) (layers.py:152-169) of the SparseTensor get_sparse_feature(nodes, [feature_name], [default_value]) returns,
     i.e. the rows of table f32[n_rows, dim] named by node i's uint64 values of the slot, in stored order, or the one row
     default_value for a node without values; combined by 'sum', 'mean' or 'sqrtn'.  The sum runs left to right from the first
     row, mean / sqrtn divide once (include/euler_b200.h).  Every value of the slot and default_value must lie in [0, n_rows):
-    the call raises otherwise, before any device work.  The gradient reaches table only (deterministic, no atomics); the
-    forward does not synchronise, the backward synchronises once."""
+    the call raises otherwise, before any device work.  The gradient reaches table only (deterministic, no atomics): a dense
+    f32[n_rows, dim] gradient, or, with sparse_grad=True, a coalesced sparse COO gradient of the rows the batch touches (as
+    nn.Embedding(sparse=True) gives), the same values without an [n_rows, dim] buffer.  The forward does not synchronise; the
+    backward synchronises once (dense) or three times (sparse: sizing the COO, the entry count, the row count)."""
     if combiner not in _COMBINERS:
         raise EulerError("sparse_feature_embedding: combiner must be one of %s, got %r" % (sorted(_COMBINERS), combiner))
     if not torch.is_tensor(table) or table.dtype != torch.float32 or table.dim() != 2:
         raise EulerError("sparse_feature_embedding: table must be a 2-D float32 tensor")
     fid = feature_name if isinstance(feature_name, (int, np.integer)) else get_graph().sparse_feature_id(str(feature_name))
     nodes = _t(nodes, torch.int64).reshape(-1)
-    return _SparseEmbedding.apply(_t(table, torch.float32), nodes, int(fid), int(default_value), _COMBINERS[combiner])
+    return _SparseEmbedding.apply(_t(table, torch.float32), nodes, int(fid), int(default_value), _COMBINERS[combiner], bool(sparse_grad))
+
+
+# ------------------------------------------------------------------------------------ ShallowEncoder's input row
+SHALLOW_COMBINERS = {'concat': 0, 'add': 1}
+
+
+def _shallow_problem(nodes, id_table, dense, sparse, comb):
+    """eu_shallow_problem of resolved inputs: dense [(fid, dim)], sparse [(fid, table, default, combiner code)]"""
+    p = _lib.ShallowProblem()
+    p.combiner, p.M, p.nodes = comb, nodes.numel(), nodes.data_ptr()
+    if id_table is not None:
+        p.id_table, p.n_id_rows, p.id_dim = id_table.data_ptr(), id_table.shape[0], id_table.shape[1]
+    p.n_dense, p.n_sparse = len(dense), len(sparse)
+    for j, (fid, dim) in enumerate(dense):
+        p.dense[j].fid, p.dense[j].dim = fid, dim
+    for k, (fid, table, default, c) in enumerate(sparse):
+        q = p.sparse[k]
+        q.fid, q.dim, q.combiner, q.default_value = fid, table.shape[1], c, default
+        q.n_rows, q.table = table.shape[0], table.data_ptr()
+    return p
+
+
+class _ShallowEncode(torch.autograd.Function):
+    """eu_shallow_encode / eu_shallow_encode_backward(_sparse).  Saves the node ids only (and the tables, which are inputs):
+    the backward pass lists every table's entries again from the graph.  Inputs after the configuration: the id table (None
+    when absent), then one table per sparse slot."""
+
+    @staticmethod
+    def forward(ctx, nodes, cfg, id_table, *tables):
+        dense, sparse_cfg, comb, W, dense_w, sparse_grad = cfg
+        sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
+        M, dev = nodes.numel(), nodes.device
+        out = torch.empty((M, W), dtype=torch.float32, device=dev)
+        dense_out = torch.empty((M, dense_w), dtype=torch.float32, device=dev) if comb == 1 else None
+        p = _shallow_problem(nodes, id_table, dense, sparse, comb)
+        check(_lib.load().eu_shallow_encode(_ctx_on_stream()._h, C.byref(p), out.data_ptr(),
+                                            dense_out.data_ptr() if dense_out is not None else None))
+        ctx.save_for_backward(nodes, id_table, *tables)
+        ctx.cfg = cfg
+        if dense_out is None:
+            return out
+        ctx.mark_non_differentiable(dense_out)
+        return out, dense_out
+
+    @staticmethod
+    def backward(ctx, grad, *unused):
+        nodes, id_table, *tables = ctx.saved_tensors
+        dense, sparse_cfg, comb, W, dense_w, sparse_grad = ctx.cfg
+        sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
+        all_tables = [id_table] + list(tables)
+        dev = nodes.device
+        grad = grad.contiguous()
+        p = _shallow_problem(nodes, id_table, dense, sparse, comb)
+        ec, lib = _ctx_on_stream(), _lib.load()
+        NT = len(all_tables)
+        PT = C.c_void_p * NT
+        if not sparse_grad:
+            grads = [torch.empty_like(t) if t is not None else None for t in all_tables]
+            check(lib.eu_shallow_encode_backward(ec._h, C.byref(p), grad.data_ptr(),
+                                                 PT(*[g.data_ptr() if g is not None else None for g in grads])))
+            return (None, None) + tuple(grads)
+        # arrays of min(entries, n_rows) rows: the id table has M entries, a slot its get_sparse_feature entries
+        caps = [min(nodes.numel(), id_table.shape[0]) if id_table is not None else 0]
+        caps += [min(_sparse_entries(nodes, fid), t.shape[0]) for fid, t, _, _ in sparse]
+        rows = [torch.empty(cap, dtype=torch.int64, device=dev) for cap in caps]
+        vals = [torch.empty((cap, t.shape[1] if t is not None else 0), dtype=torch.float32, device=dev) for cap, t in zip(caps, all_tables)]
+        counts = (C.c_int64 * NT)()
+        check(lib.eu_shallow_encode_backward_sparse(ec._h, C.byref(p), grad.data_ptr(), PT(*[r.data_ptr() for r in rows]),
+                                                    PT(*[v.data_ptr() for v in vals]), counts))
+        grads = [_coo(r, v, counts[t], tuple(all_tables[t].shape)) if all_tables[t] is not None else None
+                 for t, (r, v) in enumerate(zip(rows, vals))]
+        return (None, None) + tuple(grads)
+
+
+def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat', sparse_grad=False):
+    """ShallowEncoder's input row (tf_euler/python/utils/encoders.py:134-171) in one fused device op, for node ids of any shape
+    (flattened to M):
+        id_table    f32[n_id_rows, id_dim] or None: row nodes[i] (tf.nn.embedding_lookup; an id outside the table raises)
+        dense       [(feature_name or slot id, dim)]: get_dense_feature(nodes, [name], [dim]) exactly (pad, clip, absent nodes)
+        sparse      [(feature_name or slot id, table, default_value[, combiner])]: sparse_feature_embedding(nodes, name,
+                    table, default_value, combiner) exactly (combiner 'sum' by default, as SparseEmbedding's)
+    combiner 'concat' returns f32[M, W] = [id | dense_0 .. | sparse_0 ..].  'add' (every table one dim) returns (emb, feats):
+    emb f32[M, dim] = id + sparse_0 + .. + sparse_last added left to right, and feats f32[M, sum of dense dims] = the dense
+    part concatenated (None without dense slots), which the caller maps through its Dense layer and adds to emb.
+    The gradient reaches the tables only (features are not trainable), deterministic, no atomics: dense gradients, or with
+    sparse_grad=True coalesced sparse COO gradients of the rows the batch touches.  The forward synchronises once to check the
+    ids when an id table is given, and not at all under CUDA-graph capture (include/euler_b200.h); the backward once (dense)
+    or 2 + the slots (sparse)."""
+    if combiner not in SHALLOW_COMBINERS:
+        raise EulerError("shallow_encode: combiner must be one of %s, got %r" % (sorted(SHALLOW_COMBINERS), combiner))
+    comb = SHALLOW_COMBINERS[combiner]
+    g = get_graph()
+    dense, sparse = list(dense), list(sparse)
+    if len(dense) > _lib.SHALLOW_MAX_SLOTS or len(sparse) > _lib.SHALLOW_MAX_SLOTS:
+        raise EulerError("shallow_encode: at most %d dense and %d sparse slots" % (_lib.SHALLOW_MAX_SLOTS, _lib.SHALLOW_MAX_SLOTS))
+    tables = ([id_table] if id_table is not None else []) + [s[1] for s in sparse]
+    for t in tables:
+        if not torch.is_tensor(t) or t.dtype != torch.float32 or t.dim() != 2:
+            raise EulerError("shallow_encode: tables must be 2-D float32 tensors")
+    d_cfg = tuple((int(n) if isinstance(n, (int, np.integer)) else g.dense_feature_id(str(n)), int(d)) for n, d in dense)
+    s_cfg = []
+    for s in sparse:
+        name, _, dv = s[:3]
+        c = s[3] if len(s) > 3 else 'sum'
+        if c not in _COMBINERS:
+            raise EulerError("shallow_encode: sparse combiner must be one of %s, got %r" % (sorted(_COMBINERS), c))
+        s_cfg.append((int(name) if isinstance(name, (int, np.integer)) else g.sparse_feature_id(str(name)), int(dv), _COMBINERS[c]))
+    emb_dims = [t.shape[1] for t in tables]
+    if comb == 1 and len(set(emb_dims)) > 1:
+        raise EulerError("shallow_encode: 'add' needs one dim for every table, got %s" % emb_dims)
+    dense_w = sum(d for _, d in d_cfg)
+    W = (emb_dims[0] if emb_dims else 0) if comb == 1 else sum(emb_dims) + dense_w
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    id_t = _t(id_table, torch.float32) if id_table is not None else None
+    ts = [_t(s[1], torch.float32) for s in sparse]
+    cfg = (d_cfg, tuple(s_cfg), comb, W, dense_w if comb == 1 else 0, bool(sparse_grad))
+    res = _ShallowEncode.apply(nodes, cfg, id_t, *ts)
+    if comb == 0:
+        return res
+    out, feats = res
+    return out, (feats if d_cfg else None)
 
 
 # ------------------------------------------------------------------------------------ graph-level minibatches

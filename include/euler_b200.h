@@ -299,6 +299,75 @@ int eu_sparse_embedding_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32
                                int64_t n_rows, int32_t dim, int32_t combiner, float* out);
 int eu_sparse_embedding_lookup_backward(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
                                         int64_t default_value, int64_t n_rows, int32_t dim, int32_t combiner, float* grad_table);
+/* The same gradient as a coalesced COO: rows i64[D] ascending and values f32[D, dim], *n (host) = D, the distinct values the
+ * entries name; the arrays must hold min(entries, n_rows) rows (M entries at least, one per node).  No [n_rows, dim] buffer is
+ * written.  Synchronises twice (the entry count, then D). */
+int eu_sparse_embedding_lookup_backward_sparse(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
+                                               int64_t default_value, int64_t n_rows, int32_t dim, int32_t combiner, int64_t* rows,
+                                               float* values, int64_t* n);
+
+/* ShallowEncoder's input row, fused (tf_euler/python/utils/encoders.py:32-171): per node an id embedding, the dense feature
+ * slots and one SparseEmbedding per uint64 slot, concatenated or added.  Node i of nodes i64[M]:
+ *   id part      id_table[nodes[i]] (tf.nn.embedding_lookup: the node id is the row); id_table NULL = no id input
+ *   dense part   dense[j]: eu_get_dense_feature(nodes, fid, dim) exactly (padded with zeros, clipped, zeros for an absent
+ *                node or an unknown slot); a dim of 0 is allowed
+ *   sparse part  sparse[s]: eu_sparse_embedding_lookup(nodes, fid, default_value, table, n_rows, dim, combiner) exactly, by the
+ *                same device code (the same adds, in the same order)
+ * EU_SHALLOW_CONCAT: out f32[M, W], row i = [id | dense_0 .. dense_{n_dense-1} | sparse_0 .. sparse_{n_sparse-1}], W the sum of
+ *   the widths; dense_out unused.
+ * EU_SHALLOW_ADD: every embedding (the id table and the slots) has one dim; out f32[M, dim] = id + sparse_0 + .. + sparse_last,
+ *   added left to right from the first present term (one rounded add each); dense_out f32[M, sum of dense dims] = the dense
+ *   part (the caller maps it through its Dense layer and adds it to out).  With no embedding, out is unused.
+ * One lane group per node looks up the node's graph row once and writes its whole row.  No scratch and no synchronisation
+ * while the stream is being captured, so the forward is capturable in a CUDA graph; outside capture an id table's ids are
+ * checked first (one small kernel and one synchronisation) and one outside [0, n_id_rows) returns EU_ERR_INVALID before out is
+ * written.  Under capture that check is skipped: such a row's id columns are NaN and the id is never dereferenced.
+ * Backward (the gradient reaches the tables only; features are not trainable): grad_out has out's shape.  Table t (0 = the id
+ * table, 1 + s = slot s) gets, for each of its rows, the sum of its entries' gradient rows: the id table's entries are the
+ * nodes (row nodes[i]); slot s's are eu_sparse_embedding_lookup_backward's (each value of the node's bag, or the default),
+ * with its combiner's division.  The gradient row of an entry of node i is grad_out[i] restricted to the table's columns
+ * (CONCAT) or grad_out[i] (ADD).  Every table's entries are listed in one pass over the nodes, ordered stably by row and summed
+ * per distinct row in 256-entry chunks (eu_sparse_embedding_lookup_backward's order): no atomics, the same bits on every run.
+ *   eu_shallow_encode_backward:        grads[t] dense f32[n_rows_t, dim_t], zero on untouched rows (NULL: no id table)
+ *   eu_shallow_encode_backward_sparse: rows[t] i64[D_t] ascending, values[t] f32[D_t, dim_t], counts[t] = D_t (host); arrays of
+ *                                      min(entries_t, n_rows_t) rows (M for the id table); no [n_rows, dim] buffer is written
+ * Both synchronise once to read the entry counts (the sparse one once more, for D_t).  Scratch: 8 B per node and slot, about
+ * 48 B per entry of the largest table, and M dim floats per mean / sqrtn slot; never O(n_rows).
+ * Bounds: at most EU_SHALLOW_MAX_SLOTS dense and sparse slots each, W at most EU_SHALLOW_MAX_WIDTH columns, M and table rows
+ * below 2^31, and (backward) fewer than 2^31 entries: EU_ERR_UNSUPPORTED beyond them.  A bad combiner, a missing table or
+ * output, a dim < 1, ADD with unequal embedding dims, a default outside its table or a slot whose largest value is outside it:
+ * EU_ERR_INVALID, before any device work.  Device pointers. */
+#define EU_SHALLOW_MAX_SLOTS 8
+#define EU_SHALLOW_MAX_WIDTH 16384
+enum { EU_SHALLOW_CONCAT = 0, EU_SHALLOW_ADD = 1 };
+typedef struct {
+  int32_t fid;              /* dense slot id (unknown: zeros) */
+  int32_t dim;              /* columns, >= 0 */
+} eu_shallow_dense;
+typedef struct {
+  int32_t fid;              /* uint64 slot id (unknown: every node gets the default) */
+  int32_t dim;              /* the table's columns, >= 1 */
+  int32_t combiner;         /* eu_combiner */
+  int32_t reserved;         /* 0 */
+  int64_t default_value;    /* in [0, n_rows) */
+  int64_t n_rows;
+  const float* table;       /* f32[n_rows, dim] */
+} eu_shallow_sparse;
+typedef struct {
+  int32_t combiner;         /* EU_SHALLOW_CONCAT or EU_SHALLOW_ADD */
+  int32_t id_dim;
+  int64_t M;
+  const int64_t* nodes;     /* [M] */
+  const float* id_table;    /* f32[n_id_rows, id_dim], or NULL */
+  int64_t n_id_rows;
+  int32_t n_dense, n_sparse;
+  eu_shallow_dense dense[EU_SHALLOW_MAX_SLOTS];
+  eu_shallow_sparse sparse[EU_SHALLOW_MAX_SLOTS];
+} eu_shallow_problem;
+int eu_shallow_encode(eu_ctx* c, const eu_shallow_problem* p, float* out, float* dense_out);
+int eu_shallow_encode_backward(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, float* const* grads);
+int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, int64_t* const* rows,
+                                      float* const* values, int64_t* counts);
 
 /* Graph-level minibatches (graph classification; reference: euler/core/kernels/sample_graph_label_op.cc,
  * get_graph_by_label_op.cc and Graph::GetGraphLabel, euler/core/graph/graph.cc:439-457).
