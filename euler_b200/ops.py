@@ -7,6 +7,8 @@ op enqueues kernels from libeuler_b200.so on the current torch stream.  Nothing 
 CPU and nothing falls back to PyTorch ops: if the library or the GPU is missing, calls raise.
 """
 import ctypes as C
+import functools
+import math
 import threading
 
 import numpy as np
@@ -94,6 +96,57 @@ def _ctx_on_stream():
     return ctx
 
 
+def _arg(x):
+    """one argument of a library call: a tensor or numpy array as its data pointer, a list of them (None for a hole) as a
+    void* array, anything else as it is"""
+    if isinstance(x, torch.Tensor):
+        return x.data_ptr()
+    if isinstance(x, np.ndarray):
+        return x.ctypes.data
+    if isinstance(x, (list, tuple)):
+        return (C.c_void_p * max(len(x), 1))(*[_arg(v) for v in x])
+    return x
+
+
+def _call(name, *args, ctx=None):
+    """the library's entry point `name` on the Context handle (this thread's, on torch's current stream, unless ctx is
+    given) and args; raises EulerError when it fails"""
+    ctx = ctx or _ctx_on_stream()
+    check(getattr(_lib.load(), name)(ctx._h, *[_arg(a) for a in args]))
+
+
+def _ragged_lengths(name, rows, *args):
+    """the first phase of include/euler_b200.h's ragged protocol, for an entry point whose arguments after args are
+    (cap, indptr, *outs): called with cap = 0 it fills indptr i64[rows + 1] only.  Returns (indptr, total = indptr[-1]),
+    read back with one host sync."""
+    n_outs = len(_lib.SIGNATURES[name][1]) - 3 - len(args)     # the context handle, cap and indptr are the other three
+    indptr = torch.empty(rows + 1, dtype=torch.int64, device=_dev())
+    _call(name, *args, 0, indptr, *[None] * n_outs)
+    return indptr, int(indptr[-1].item())
+
+
+def _ragged(name, rows, alloc, *args, lengths=None):
+    """the whole ragged protocol: the first phase (unless lengths = (indptr, total) holds its result), then the outputs
+    alloc(total) returns, filled by a second call when total > 0.  Returns (indptr, total, outputs)."""
+    indptr, total = lengths or _ragged_lengths(name, rows, *args)
+    outs = alloc(total)
+    if total:
+        _call(name, *args, total, indptr, *outs)
+    return indptr, total, outs
+
+
+def _sparse_tensor(indptr, values, n, total, max_len=None):
+    """the SparseTensor content (indices i64[total, 2], values, dense_shape (n, max_len)) of the ragged rows
+    values[indptr[i]:indptr[i+1]]; max_len=None reads the longest row back (one host sync)"""
+    dev = indptr.device
+    lens = indptr[1:] - indptr[:-1]
+    rows = torch.repeat_interleave(torch.arange(n, device=dev), lens, output_size=total)
+    cols = torch.arange(total, device=dev) - indptr[:-1][rows]
+    if max_len is None:
+        max_len = int(lens.max().item()) if n else 0
+    return torch.stack([rows, cols], dim=1), values, (n, max_len)
+
+
 def _t(x, dtype):
     if isinstance(x, torch.Tensor):
         return x.to(device=_dev(), dtype=dtype).contiguous()
@@ -104,6 +157,27 @@ def _i32_host(x):
     if isinstance(x, torch.Tensor):
         x = x.detach().cpu().numpy()
     return np.ascontiguousarray(np.asarray(x).reshape(-1), dtype=np.int32)
+
+
+def _slot(name, lookup):
+    """a feature slot: an int is the slot id, anything else a name lookup resolves"""
+    return int(name) if isinstance(name, (int, np.integer)) else lookup(str(name))
+
+
+def _neighbor_triple(shape):
+    """empty (ids i64, weights f32, types i32) neighbor outputs of one shape"""
+    dev = _dev()
+    return tuple(torch.empty(shape, dtype=dt, device=dev) for dt in (torch.int64, torch.float32, torch.int32))
+
+
+def _neighbor_rows(entry, nodes, edge_types, k, *default_node):
+    """the k (ids, weights, types) per node that sample_neighbor, get_top_k_neighbor and sample_neighbor_api return: entry
+    takes (nodes, n, types, n_types, k[, default_node], ids, weights, types)"""
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    et = get_edge_type_id(edge_types)
+    ids, w, t = _neighbor_triple((nodes.numel(), k))
+    _call(entry, nodes, nodes.numel(), et, len(et), k, *default_node, ids, w, t)
+    return ids, w, t
 
 
 # ------------------------------------------------------------------------------------ type ops
@@ -126,22 +200,35 @@ def _type_ids(v, lookup):
     return arr.astype(np.int32)
 
 
+def _hop_types(op, edge_types, hops=None):
+    """one edge-type list per hop (exactly `hops` of them when given), all of one length T: i32[L, T], [0, 0] for none"""
+    ets = [get_edge_type_id(e) for e in edge_types]
+    if (hops is not None and len(ets) != hops) or any(len(e) != len(ets[0]) for e in ets):
+        raise EulerError("%s: edge_types must hold one equal-length type list per hop" % op)
+    return np.ascontiguousarray(np.stack(ets) if ets else np.zeros((0, 0)), dtype=np.int32)
+
+
+def _fanout_args(op, B, edge_types, counts):
+    """the hop arguments of the fanout entry points, (types i32[L, T], T, counts i32[L], L), and hop i's shape
+    (B, c1, ..., ci) for each hop"""
+    et = _hop_types(op, edge_types, len(counts))
+    shapes = [(B,) + tuple(int(c) for c in counts[:i + 1]) for i in range(len(counts))]
+    return (et, et.shape[1], np.ascontiguousarray(counts, dtype=np.int32), len(counts)), shapes
+
+
+def _hop_outputs(shapes):
+    """per hop shape a neighbor triple, returned as three lists (ids, weights, types)"""
+    triples = [_neighbor_triple(sh) for sh in shapes]
+    return tuple([tr[k] for tr in triples] for k in range(3))
+
+
 # ------------------------------------------------------------------------------------ sampling
 def sample_neighbor(nodes, edge_types, count, default_node=-1, condition=''):
     """neighbor_ops.sample_neighbor (neighbor_ops.py:39-41).  Returns (neighbors i64[B,count],
     weights f32[B,count], types i32[B,count])."""
     if condition:
         raise EulerError("sample_neighbor: `condition` (index queries) is outside this path")
-    nodes = _t(nodes, torch.int64).reshape(-1)
-    et = get_edge_type_id(edge_types)
-    B = nodes.numel()
-    ids = torch.empty((B, count), dtype=torch.int64, device=nodes.device)
-    w = torch.empty((B, count), dtype=torch.float32, device=nodes.device)
-    t = torch.empty((B, count), dtype=torch.int32, device=nodes.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sample_neighbor(ctx._h, nodes.data_ptr(), B, et.ctypes.data, len(et), count,
-                                         default_node, ids.data_ptr(), w.data_ptr(), t.data_ptr()))
-    return ids, w, t
+    return _neighbor_rows("eu_sample_neighbor", nodes, edge_types, count, default_node)
 
 
 def sample_fanout(nodes, edge_types, counts, default_node=-1):
@@ -149,25 +236,10 @@ def sample_fanout(nodes, edge_types, counts, default_node=-1):
     type lists of equal length.  Returns (neighbors_list[L+1], weights_list[L], types_list[L]),
     all flattened like the reference."""
     nodes = _t(nodes, torch.int64).reshape(-1)
-    L = len(counts)
-    ets = [get_edge_type_id(e) for e in edge_types]
-    if len(ets) != L or any(len(e) != len(ets[0]) for e in ets):
-        raise EulerError("sample_fanout: edge_types must hold one equal-length type list per hop")
-    et = np.ascontiguousarray(np.stack(ets) if L else np.zeros((0, 0)), dtype=np.int32)
-    cs = np.ascontiguousarray(counts, dtype=np.int32)
     B = nodes.numel()
-    ids, ws, ts, rows = [], [], [], B
-    for c in counts:
-        rows *= int(c)
-        ids.append(torch.empty(rows, dtype=torch.int64, device=nodes.device))
-        ws.append(torch.empty(rows, dtype=torch.float32, device=nodes.device))
-        ts.append(torch.empty(rows, dtype=torch.int32, device=nodes.device))
-    P = C.c_void_p * max(L, 1)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sample_fanout(ctx._h, nodes.data_ptr(), B, et.ctypes.data,
-                                       et.shape[1] if L else 0, cs.ctypes.data, L, default_node,
-                                       P(*[x.data_ptr() for x in ids]), P(*[x.data_ptr() for x in ws]),
-                                       P(*[x.data_ptr() for x in ts])))
+    hop_args, shapes = _fanout_args("sample_fanout", B, edge_types, counts)
+    ids, ws, ts = _hop_outputs([math.prod(sh) for sh in shapes])
+    _call("eu_sample_fanout", nodes, B, *hop_args, default_node, ids, ws, ts)
     return [nodes] + ids, ws, ts
 
 
@@ -182,53 +254,34 @@ def sample_fanout_with_feature(nodes, edge_types, count, default_node, dense_fea
         dense_features   (L+1) * len(dense_feature_names) tensors f32[rows_i, dim], hop-major
         sparse_features  (L+1) * len(sparse_feature_names) (indices, values, dense_shape) triples, hop-major, as get_sparse_feature
     One host synchronisation per call when sparse features are asked for (all ragged totals together), none otherwise."""
-    g, lib = get_graph(), _lib.load()
+    g = get_graph()
     nodes = _t(nodes, torch.int64).reshape(-1)
     L = len(count)
-    ets = [get_edge_type_id(e) for e in edge_types]
-    if len(ets) != L or any(len(e) != len(ets[0]) for e in ets):
-        raise EulerError("sample_fanout_with_feature: edge_types must hold one equal-length type list per hop")
+    B, dev = nodes.numel(), nodes.device
+    hop_args, shapes = _fanout_args("sample_fanout_with_feature", B, edge_types, count)
     if len(dense_feature_names) != len(dense_dimensions) or len(sparse_feature_names) != len(sparse_default_values):
         raise EulerError("sample_fanout_with_feature: one dimension per dense feature and one default per sparse feature")
-    et = np.ascontiguousarray(np.stack(ets) if L else np.zeros((0, 0)), dtype=np.int32)
-    cs = np.ascontiguousarray(count, dtype=np.int32)
-    B, dev = nodes.numel(), nodes.device
-    shapes, rows = [], [B]
-    for c in count:
-        shapes.append((shapes[-1] if shapes else (B,)) + (int(c),))
-        rows.append(rows[-1] * int(c))
-    ids = [torch.empty(r, dtype=torch.int64, device=dev) for r in rows[1:]]
-    eng = [torch.empty(r, dtype=torch.int64, device=dev) for r in rows[1:]]
-    ws = [torch.empty(sh, dtype=torch.float32, device=dev) for sh in shapes]
-    ts = [torch.empty(sh, dtype=torch.int32, device=dev) for sh in shapes]
-    dfid = np.asarray([n if isinstance(n, (int, np.integer)) else g.dense_feature_id(str(n)) for n in dense_feature_names], np.int32)
+    rows = [B] + [math.prod(sh) for sh in shapes]
+    ids, ws, ts = _hop_outputs(shapes)
+    ids = [x.view(-1) for x in ids]
+    eng = [torch.empty_like(x) for x in ids]
+    dfid = np.asarray([_slot(n, g.dense_feature_id) for n in dense_feature_names], np.int32)
     ddim = np.asarray(dense_dimensions, np.int32)
     sfid = np.asarray([g.sparse_feature_id(str(n)) for n in sparse_feature_names], np.int32)
     nd, ns = len(dfid), len(sfid)
     dense = [torch.empty((rows[l], int(ddim[j])), dtype=torch.float32, device=dev) for l in range(L + 1) for j in range(nd)]
     ptrs = [torch.empty(rows[l] + 1, dtype=torch.int64, device=dev) for l in range(L + 1) for j in range(ns)]
     total, maxlen = np.zeros(max(len(ptrs), 1), np.int64), np.zeros(max(len(ptrs), 1), np.int64)
-
-    def P(ts_):
-        return (C.c_void_p * max(len(ts_), 1))(*[t.data_ptr() for t in ts_])
-    ctx = _ctx_on_stream()
-    check(lib.eu_sample_fanout_with_feature(ctx._h, nodes.data_ptr(), B, et.ctypes.data, et.shape[1] if L else 0, cs.ctypes.data, L,
-                                            default_node, P(ids), P(ws), P(ts), P(eng), nd, dfid.ctypes.data, ddim.ctypes.data,
-                                            P(dense), ns, sfid.ctypes.data, P(ptrs), total.ctypes.data, maxlen.ctypes.data))
+    _call("eu_sample_fanout_with_feature", nodes, B, *hop_args, default_node, ids, ws, ts, eng, nd, dfid, ddim, dense, ns, sfid,
+          ptrs, total, maxlen)
     sparse = []
     for l in range(L + 1):
         hop_ids = nodes if l == 0 else eng[l - 1]
         for j in range(ns):
             k = l * ns + j
-            ptr, tot, dv = ptrs[k], int(total[k]), int(sparse_default_values[j])
-            vals = torch.empty(tot, dtype=torch.int64, device=dev)
-            if tot:
-                check(lib.eu_get_sparse_feature(ctx._h, hop_ids.data_ptr(), rows[l], int(sfid[j]), dv, tot, ptr.data_ptr(),
-                                                vals.data_ptr()))
-            lens = ptr[1:] - ptr[:-1]
-            r = torch.repeat_interleave(torch.arange(rows[l], device=dev), lens, output_size=tot)
-            cols = torch.arange(tot, device=dev) - ptr[:-1][r]
-            sparse.append((torch.stack([r, cols], dim=1), vals, (rows[l], int(maxlen[k]))))
+            _, tot, (vals,) = _ragged("eu_get_sparse_feature", rows[l], _values_i64, hop_ids, rows[l], int(sfid[j]),
+                                      int(sparse_default_values[j]), lengths=(ptrs[k], int(total[k])))
+            sparse.append(_sparse_tensor(ptrs[k], vals, rows[l], tot, int(maxlen[k])))
     return [nodes] + ids, ws, ts, dense, sparse
 
 
@@ -238,22 +291,9 @@ def sample_fanout_batched(nodes, edge_types, counts, default_node=-1, ctx=None):
     seeded like engine b.  Returns (neighbors_list[L+1], weights_list[L], types_list[L]) with a leading nb dim."""
     nodes = _t(nodes, torch.int64)
     nb, B = nodes.shape
-    L = len(counts)
-    ets = [get_edge_type_id(e) for e in edge_types]
-    et = np.ascontiguousarray(np.stack(ets) if L else np.zeros((0, 0)), dtype=np.int32)
-    cs = np.ascontiguousarray(counts, dtype=np.int32)
-    ids, ws, ts, rows = [], [], [], B
-    for c in counts:
-        rows *= int(c)
-        ids.append(torch.empty((nb, rows), dtype=torch.int64, device=nodes.device))
-        ws.append(torch.empty((nb, rows), dtype=torch.float32, device=nodes.device))
-        ts.append(torch.empty((nb, rows), dtype=torch.int32, device=nodes.device))
-    P = C.c_void_p * max(L, 1)
-    ctx = ctx or _ctx_on_stream()
-    check(_lib.load().eu_sample_fanout_batched(ctx._h, nodes.data_ptr(), nb, B, et.ctypes.data,
-                                               et.shape[1] if L else 0, cs.ctypes.data, L, default_node,
-                                               P(*[x.data_ptr() for x in ids]), P(*[x.data_ptr() for x in ws]),
-                                               P(*[x.data_ptr() for x in ts])))
+    hop_args, shapes = _fanout_args("sample_fanout_batched", B, edge_types, counts)
+    ids, ws, ts = _hop_outputs([(nb, math.prod(sh)) for sh in shapes])
+    _call("eu_sample_fanout_batched", nodes, nb, B, *hop_args, default_node, ids, ws, ts, ctx=ctx)
     return [nodes] + ids, ws, ts
 
 
@@ -267,8 +307,7 @@ def sample_node(count, node_type, condition=''):
         types = get_node_type_id(node_type)
     count = int(count)
     out = torch.empty(count, dtype=torch.int64, device=_dev())
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sample_node(ctx._h, count, types.ctypes.data, len(types), out.data_ptr()))
+    _call("eu_sample_node", count, types, len(types), out)
     return out
 
 
@@ -276,17 +315,10 @@ def random_walk(nodes, edge_types, p=1.0, q=1.0, default_node=-1):
     """walk_ops.random_walk (walk_ops.py:29-43).  edge_types: list of L 1-D type lists.
     Returns i64[B, L+1]."""
     nodes = _t(nodes, torch.int64).reshape(-1)
-    ets = [get_edge_type_id(e) for e in edge_types]
-    L = len(ets)
-    if any(len(e) != len(ets[0]) for e in ets):
-        raise EulerError("random_walk: every step needs the same number of edge types here")
-    et = np.ascontiguousarray(np.stack(ets) if L else np.zeros((0, 0)), dtype=np.int32)
-    B = nodes.numel()
+    et = _hop_types("random_walk", edge_types)
+    L, B = et.shape[0], nodes.numel()
     out = torch.empty((B, L + 1), dtype=torch.int64, device=nodes.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_random_walk(ctx._h, nodes.data_ptr(), B, et.ctypes.data,
-                                     et.shape[1] if L else 0, L, float(p), float(q), default_node,
-                                     out.data_ptr()))
+    _call("eu_random_walk", nodes, B, et, et.shape[1], L, float(p), float(q), default_node, out)
     return out
 
 
@@ -297,61 +329,51 @@ def get_dense_feature(nodes, feature_names, dimensions, thread_num=1):
     nodes = _t(nodes, torch.int64).reshape(-1)
     g = get_graph()
     outs = []
-    ctx = _ctx_on_stream()
     for name, dim in zip(feature_names, dimensions):
-        fid = name if isinstance(name, (int, np.integer)) else g.dense_feature_id(name)
         out = torch.empty((nodes.numel(), int(dim)), dtype=torch.float32, device=nodes.device)
-        check(_lib.load().eu_get_dense_feature(ctx._h, nodes.data_ptr(), nodes.numel(), int(fid),
-                                               int(dim), out.data_ptr()))
+        _call("eu_get_dense_feature", nodes, nodes.numel(), _slot(name, g.dense_feature_id), int(dim), out)
         outs.append(out)
     return outs
 
 
-def _ragged(fn, nodes, fid, *mid):
-    """two-phase ragged fetch: lengths, then values"""
-    nodes = _t(nodes, torch.int64).reshape(-1)
-    n = nodes.numel()
-    ctx = _ctx_on_stream()
-    indptr = torch.empty(n + 1, dtype=torch.int64, device=nodes.device)
-    check(fn(ctx._h, nodes.data_ptr(), n, int(fid), *mid, 0, indptr.data_ptr(), None))
-    total = int(indptr[-1].item())
-    return nodes, n, ctx, indptr, total
+def _values_i64(total):
+    return (torch.empty(total, dtype=torch.int64, device=_dev()),)
+
+
+def _sparse_features(entry, keys, feature_names, default_values, fid_of):
+    """get_sparse_feature over keys (node ids, or edges for eu_get_edge_sparse_feature): per feature the SparseTensor content"""
+    names = [str(x) for x in feature_names]
+    defaults = [0] * len(names) if default_values is None else [int(x) for x in default_values]
+    n, outs = keys.shape[0], []
+    for name, dv in zip(names, defaults):
+        indptr, total, (vals,) = _ragged(entry, n, _values_i64, keys, n, fid_of(name), dv)
+        outs.append(_sparse_tensor(indptr, vals, n, total))
+    return outs
+
+
+def _binary_features(entry, keys, feature_names, fid_of):
+    """get_binary_feature over keys (node ids, or edges for eu_get_edge_binary_feature): per feature n byte strings"""
+    n, outs = keys.shape[0], []
+    for name in feature_names:
+        indptr, _, (buf,) = _ragged(entry, n, lambda t: (torch.empty(t, dtype=torch.uint8, device=_dev()),), keys, n,
+                                    fid_of(str(name)))
+        raw, ptr = bytes(buf.cpu().numpy().tobytes()), indptr.cpu().tolist()
+        outs.append([raw[ptr[i]:ptr[i + 1]] for i in range(n)])
+    return outs
 
 
 def get_sparse_feature(nodes, feature_names, default_values=None, thread_num=1):
     """feature_ops.get_sparse_feature (feature_ops.py:57-73; kernel get_sparse_feature_op.cc:52-130).  Per feature the
     reference returns a SparseTensor; here the same content as (indices i64[nnz, 2], values i64[nnz], dense_shape (N, max_len)):
     row i lists the uint64 values of the node, a node without values gets the single entry (i, 0) = default value."""
-    g, lib = get_graph(), _lib.load()
-    names = [str(x) for x in feature_names]
-    defaults = [0] * len(names) if default_values is None else [int(x) for x in default_values]
-    outs = []
-    for name, dv in zip(names, defaults):
-        fid = g.sparse_feature_id(name)
-        nd, n, ctx, indptr, total = _ragged(lib.eu_get_sparse_feature, nodes, fid, dv)
-        vals = torch.empty(total, dtype=torch.int64, device=nd.device)
-        if total:
-            check(lib.eu_get_sparse_feature(ctx._h, nd.data_ptr(), n, int(fid), dv, total, indptr.data_ptr(), vals.data_ptr()))
-        lens = indptr[1:] - indptr[:-1]
-        rows = torch.repeat_interleave(torch.arange(n, device=nd.device), lens)
-        cols = torch.arange(total, device=nd.device) - indptr[:-1][rows]
-        outs.append((torch.stack([rows, cols], dim=1), vals, (n, int(lens.max().item()) if n else 0)))
-    return outs
+    fid_of = get_graph().sparse_feature_id
+    return _sparse_features("eu_get_sparse_feature", _t(nodes, torch.int64).reshape(-1), feature_names, default_values, fid_of)
 
 
 def get_binary_feature(nodes, feature_names, thread_num=1):
     """feature_ops.get_binary_feature (feature_ops.py:158-171): per feature a list of N byte strings (b'' for absent nodes)."""
-    g, lib = get_graph(), _lib.load()
-    outs = []
-    for name in [str(x) for x in feature_names]:
-        fid = g.binary_feature_id(name)
-        nd, n, ctx, indptr, total = _ragged(lib.eu_get_binary_feature, nodes, fid)
-        buf = torch.empty(max(total, 1), dtype=torch.uint8, device=nd.device)
-        if total:
-            check(lib.eu_get_binary_feature(ctx._h, nd.data_ptr(), n, int(fid), total, indptr.data_ptr(), buf.data_ptr()))
-        raw, ptr = bytes(buf[:total].cpu().numpy().tobytes()), indptr.cpu().tolist()
-        outs.append([raw[ptr[i]:ptr[i + 1]] for i in range(n)])
-    return outs
+    fid_of = get_graph().binary_feature_id
+    return _binary_features("eu_get_binary_feature", _t(nodes, torch.int64).reshape(-1), feature_names, fid_of)
 
 
 def sample_edge(count, edge_type):
@@ -360,8 +382,7 @@ def sample_edge(count, edge_type):
     types = get_edge_type_id(edge_type)
     count = int(count)
     out = torch.empty((count, 3), dtype=torch.int64, device=_dev())
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sample_edge(ctx._h, count, types.ctypes.data, len(types), out.data_ptr()))
+    _call("eu_sample_edge", count, types, len(types), out)
     return out
 
 
@@ -375,11 +396,10 @@ def _edges(edges):
 def get_edge_dense_feature(edges, feature_names, dimensions, thread_num=1):
     """feature_ops.get_edge_dense_feature: list of f32[E, dim] (zeros for unknown edges / features)"""
     e = _edges(edges)
-    g, lib, outs = get_graph(), _lib.load(), []
-    ctx = _ctx_on_stream()
+    g, outs = get_graph(), []
     for name, dim in zip(feature_names, dimensions):
         out = torch.empty((e.shape[0], int(dim)), dtype=torch.float32, device=e.device)
-        check(lib.eu_get_edge_dense_feature(ctx._h, e.data_ptr(), e.shape[0], g.edge_feature_id("dense", name), int(dim), out.data_ptr()))
+        _call("eu_get_edge_dense_feature", e, e.shape[0], g.edge_feature_id("dense", name), int(dim), out)
         outs.append(out)
     return outs
 
@@ -387,43 +407,15 @@ def get_edge_dense_feature(edges, feature_names, dimensions, thread_num=1):
 def get_edge_sparse_feature(edges, feature_names, default_values=None, thread_num=1):
     """feature_ops.get_edge_sparse_feature: per feature (indices i64[nnz, 2], values i64[nnz], dense_shape)"""
     e = _edges(edges)
-    g, lib, outs = get_graph(), _lib.load(), []
-    names = [str(x) for x in feature_names]
-    defaults = [0] * len(names) if default_values is None else [int(x) for x in default_values]
-    ctx = _ctx_on_stream()
-    n = e.shape[0]
-    for name, dv in zip(names, defaults):
-        fid = g.edge_feature_id("sparse", name)
-        indptr = torch.empty(n + 1, dtype=torch.int64, device=e.device)
-        check(lib.eu_get_edge_sparse_feature(ctx._h, e.data_ptr(), n, fid, dv, 0, indptr.data_ptr(), None))
-        total = int(indptr[-1].item())
-        vals = torch.empty(total, dtype=torch.int64, device=e.device)
-        if total:
-            check(lib.eu_get_edge_sparse_feature(ctx._h, e.data_ptr(), n, fid, dv, total, indptr.data_ptr(), vals.data_ptr()))
-        lens = indptr[1:] - indptr[:-1]
-        rows = torch.repeat_interleave(torch.arange(n, device=e.device), lens)
-        cols = torch.arange(total, device=e.device) - indptr[:-1][rows]
-        outs.append((torch.stack([rows, cols], dim=1), vals, (n, int(lens.max().item()) if n else 0)))
-    return outs
+    fid_of = functools.partial(get_graph().edge_feature_id, "sparse")
+    return _sparse_features("eu_get_edge_sparse_feature", e, feature_names, default_values, fid_of)
 
 
 def get_edge_binary_feature(edges, feature_names, thread_num=1):
     """feature_ops.get_edge_binary_feature: per feature a list of E byte strings"""
     e = _edges(edges)
-    g, lib, outs = get_graph(), _lib.load(), []
-    ctx = _ctx_on_stream()
-    n = e.shape[0]
-    for name in [str(x) for x in feature_names]:
-        fid = g.edge_feature_id("binary", name)
-        indptr = torch.empty(n + 1, dtype=torch.int64, device=e.device)
-        check(lib.eu_get_edge_binary_feature(ctx._h, e.data_ptr(), n, fid, 0, indptr.data_ptr(), None))
-        total = int(indptr[-1].item())
-        buf = torch.empty(max(total, 1), dtype=torch.uint8, device=e.device)
-        if total:
-            check(lib.eu_get_edge_binary_feature(ctx._h, e.data_ptr(), n, fid, total, indptr.data_ptr(), buf.data_ptr()))
-        raw, ptr = bytes(buf[:total].cpu().numpy().tobytes()), indptr.cpu().tolist()
-        outs.append([raw[ptr[i]:ptr[i + 1]] for i in range(n)])
-    return outs
+    fid_of = functools.partial(get_graph().edge_feature_id, "binary")
+    return _binary_features("eu_get_edge_binary_feature", e, feature_names, fid_of)
 
 
 def get_full_neighbor(nodes, edge_types):
@@ -433,19 +425,8 @@ def get_full_neighbor(nodes, edge_types):
     weights f32[nnz], types i32[nnz]) -- SparseTensor indices are (i, k - indptr[i]) for k in [indptr[i], indptr[i+1])."""
     nodes = _t(nodes, torch.int64).reshape(-1)
     et = np.ascontiguousarray(edge_types, dtype=np.int32).reshape(-1)
-    ctx = _ctx_on_stream()
-    lib = _lib.load()
-    n = nodes.numel()
-    indptr = torch.empty(n + 1, dtype=torch.int64, device=nodes.device)
-    check(lib.eu_get_full_neighbor(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), 0, indptr.data_ptr(), None, None, None))
-    total = int(indptr[-1].item())
-    ids = torch.empty(total, dtype=torch.int64, device=nodes.device)
-    w = torch.empty(total, dtype=torch.float32, device=nodes.device)
-    t = torch.empty(total, dtype=torch.int32, device=nodes.device)
-    if total:
-        check(lib.eu_get_full_neighbor(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), total, indptr.data_ptr(),
-                                       ids.data_ptr(), w.data_ptr(), t.data_ptr()))
-    return indptr, ids, w, t
+    indptr, _, outs = _ragged("eu_get_full_neighbor", nodes.numel(), _neighbor_triple, nodes, nodes.numel(), et, len(et))
+    return (indptr,) + outs
 
 
 def get_sorted_full_neighbor(nodes, edge_types, condition=''):
@@ -455,19 +436,8 @@ def get_sorted_full_neighbor(nodes, edge_types, condition=''):
         raise EulerError("get_sorted_full_neighbor: `condition` (index queries) is outside this path")
     nodes = _t(nodes, torch.int64).reshape(-1)
     et = get_edge_type_id(edge_types)
-    ctx = _ctx_on_stream()
-    lib = _lib.load()
-    n = nodes.numel()
-    indptr = torch.empty(n + 1, dtype=torch.int64, device=nodes.device)
-    check(lib.eu_get_sorted_full_neighbor(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), 0, indptr.data_ptr(), None, None, None))
-    total = int(indptr[-1].item())
-    ids = torch.empty(total, dtype=torch.int64, device=nodes.device)
-    w = torch.empty(total, dtype=torch.float32, device=nodes.device)
-    t = torch.empty(total, dtype=torch.int32, device=nodes.device)
-    if total:
-        check(lib.eu_get_sorted_full_neighbor(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), total, indptr.data_ptr(),
-                                              ids.data_ptr(), w.data_ptr(), t.data_ptr()))
-    return indptr, ids, w, t
+    indptr, _, outs = _ragged("eu_get_sorted_full_neighbor", nodes.numel(), _neighbor_triple, nodes, nodes.numel(), et, len(et))
+    return (indptr,) + outs
 
 
 def get_top_k_neighbor(nodes, edge_types, k, default_node=-1, condition=''):
@@ -475,16 +445,7 @@ def get_top_k_neighbor(nodes, edge_types, k, default_node=-1, condition=''):
     heaviest edges of each node, heaviest first, filled with default_node / 0 / -1."""
     if condition:
         raise EulerError("get_top_k_neighbor: `condition` (index queries) is outside this path")
-    nodes = _t(nodes, torch.int64).reshape(-1)
-    et = get_edge_type_id(edge_types)
-    n, k = nodes.numel(), int(k)
-    ids = torch.empty((n, k), dtype=torch.int64, device=nodes.device)
-    w = torch.empty((n, k), dtype=torch.float32, device=nodes.device)
-    t = torch.empty((n, k), dtype=torch.int32, device=nodes.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_get_top_k_neighbor(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), k, default_node,
-                                            ids.data_ptr(), w.data_ptr(), t.data_ptr()))
-    return ids, w, t
+    return _neighbor_rows("eu_get_top_k_neighbor", nodes, edge_types, int(k), default_node)
 
 
 _HOP_APPEND_FRONTIER, _HOP_SELF_LOOPS, _HOP_SORT = 1, 2, 4     # include/euler_b200.h
@@ -494,13 +455,8 @@ def _full_hop(nodes, edge_types, flags, rows=True, weights=False, types=False):
     """one eu_full_neighbor_hop: two host syncs, the listing total (output shapes) and the unique count (the frontier's length)"""
     nodes = _t(nodes, torch.int64).reshape(-1)
     et = get_edge_type_id(edge_types)
-    ctx = _ctx_on_stream()
-    lib = _lib.load()
     n, dev = nodes.numel(), nodes.device
-    indptr = torch.empty(n + 1, dtype=torch.int64, device=dev)
-    check(lib.eu_full_neighbor_hop(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), flags, 0, indptr.data_ptr(),
-                                   None, None, None, None, None, None, None))
-    total = int(indptr[-1].item())
+    indptr, total = _ragged_lengths("eu_full_neighbor_hop", n, nodes, n, et, len(et), flags)
     append = bool(flags & _HOP_APPEND_FRONTIER)
     width = total + (n if flags & _HOP_SELF_LOOPS else 0)
     uniq = torch.empty(total + (n if append else 0), dtype=torch.int64, device=dev)
@@ -509,10 +465,8 @@ def _full_hop(nodes, edge_types, flags, rows=True, weights=False, types=False):
     w = torch.empty(total, dtype=torch.float32, device=dev) if weights else None
     t = torch.empty(total, dtype=torch.int32, device=dev) if types else None
     res = torch.empty(n, dtype=torch.int64, device=dev) if append else None
-    ptr = lambda x: None if x is None else x.data_ptr()          # noqa: E731
-    check(lib.eu_full_neighbor_hop(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), flags, total, indptr.data_ptr(),
-                                   uniq.data_ptr(), cnt.data_ptr(), edge_index[0].data_ptr() if rows else None,
-                                   edge_index[-1].data_ptr(), ptr(w), ptr(t), ptr(res)))
+    _call("eu_full_neighbor_hop", nodes, n, et, len(et), flags, total, indptr, uniq, cnt, edge_index[0] if rows else None,
+          edge_index[-1], w, t, res)
     return indptr, uniq[:int(cnt.item())], res, edge_index, w, t
 
 
@@ -571,9 +525,8 @@ def sample_neighbor_layerwise(nodes, edge_types, count, default_node=-1, weight_
     et = get_edge_type_id(edge_types)
     out = torch.empty((batch, int(count)), dtype=torch.int64, device=nd.device)
     adj = torch.empty((batch, n, int(count)), dtype=torch.float32, device=nd.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sample_neighbor_layerwise(ctx._h, nd.data_ptr(), batch, n, et.ctypes.data, len(et), int(count), default_node,
-                                                   1 if weight_func == 'sqrt' else 0, out.data_ptr(), adj.data_ptr()))
+    _call("eu_sample_neighbor_layerwise", nd, batch, n, et, len(et), int(count), default_node, 1 if weight_func == 'sqrt' else 0,
+          out, adj)
     return out, adj
 
 
@@ -587,23 +540,17 @@ def sparse_get_adj(nodes, nb_nodes, edge_types, n=-1, m=-1):
     batch = nd.numel() // max(N, 1)
     et = get_edge_type_id(edge_types)
     adj = torch.empty((batch, N, M), dtype=torch.float32, device=nd.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sparse_get_adj(ctx._h, nd.data_ptr(), nb.data_ptr(), batch, N, M, et.ctypes.data, len(et), adj.data_ptr()))
+    _call("eu_sparse_get_adj", nd, nb, batch, N, M, et, len(et), adj)
     return adj
 
 
 def _adj_coo(nd, nb, batch, N, M, et):
     """one eu_sparse_get_adj_coo: a host sync for the entry count (the output shape)"""
-    lib, dev = _lib.load(), nd.device
-    rowptr = torch.empty(batch * N + 1, dtype=torch.int64, device=dev)
-    ctx = _ctx_on_stream()
-    args = (ctx._h, nd.data_ptr(), nb.data_ptr(), batch, N, M, et.ctypes.data, len(et))
-    check(lib.eu_sparse_get_adj_coo(*args, 0, rowptr.data_ptr(), None, None))
-    nnz = int(rowptr[-1].item())
-    indices = torch.empty((nnz, 3), dtype=torch.int64, device=dev)
-    values = torch.empty(nnz, dtype=torch.int64, device=dev)
-    if nnz:
-        check(lib.eu_sparse_get_adj_coo(*args, nnz, rowptr.data_ptr(), indices.data_ptr(), values.data_ptr()))
+    dev = nd.device
+
+    def alloc(nnz):
+        return torch.empty((nnz, 3), dtype=torch.int64, device=dev), torch.empty(nnz, dtype=torch.int64, device=dev)
+    _, _, (indices, values) = _ragged("eu_sparse_get_adj_coo", batch * N, alloc, nd, nb, batch, N, M, et, len(et))
     return indices, values, (batch, N, M)
 
 
@@ -639,9 +586,8 @@ def sample_neighbor_layerwise_coo(nodes, edge_types, count, default_node=-1, wei
     if n == 0:
         out.fill_(default_node)
     else:
-        ctx = _ctx_on_stream()
-        check(_lib.load().eu_sample_neighbor_layerwise(ctx._h, nd.data_ptr(), batch, n, et.ctypes.data, len(et), count, default_node,
-                                                       1 if weight_func == 'sqrt' else 0, out.data_ptr(), None))
+        _call("eu_sample_neighbor_layerwise", nd, batch, n, et, len(et), count, default_node, 1 if weight_func == 'sqrt' else 0,
+              out, None)
     return out, _adj_coo(nd.reshape(-1), out.reshape(-1), batch, n, count, et)
 
 
@@ -652,27 +598,16 @@ def gen_pair(paths, left_win_size, right_win_size):
         raise EulerError("gen_pair: paths must be [batch, path_len]")
     paths = paths.contiguous()
     B, plen = paths.shape
-    lib = _lib.load()
-    pc = lib.eu_gen_pair_count(plen, int(left_win_size), int(right_win_size))
+    pc = _lib.load().eu_gen_pair_count(plen, int(left_win_size), int(right_win_size))
     out = torch.empty((B, pc, 2), dtype=torch.int64, device=paths.device)
-    ctx = _ctx_on_stream()
-    check(lib.eu_gen_pair(ctx._h, paths.data_ptr(), B, plen, int(left_win_size), int(right_win_size), out.data_ptr()))
+    _call("eu_gen_pair", paths, B, plen, int(left_win_size), int(right_win_size), out)
     return out
 
 
 def sample_neighbor_api(nodes, edge_types, count):
     """euler::SampleNeighbor of the C++ api (api.cc:223-236): NO unique / gather -- a repeated id draws again.  Returns
     engine-form (ids i64[N,count], w, t); rows without a result are (0, 0.0, -1)."""
-    nodes = _t(nodes, torch.int64).reshape(-1)
-    et = get_edge_type_id(edge_types)
-    n, count = nodes.numel(), int(count)
-    ids = torch.empty((n, count), dtype=torch.int64, device=nodes.device)
-    w = torch.empty((n, count), dtype=torch.float32, device=nodes.device)
-    t = torch.empty((n, count), dtype=torch.int32, device=nodes.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sample_neighbor_raw(ctx._h, nodes.data_ptr(), n, et.ctypes.data, len(et), count,
-                                             ids.data_ptr(), w.data_ptr(), t.data_ptr()))
-    return ids, w, t
+    return _neighbor_rows("eu_sample_neighbor_raw", nodes, edge_types, int(count))
 
 
 def unique(ids):
@@ -682,8 +617,7 @@ def unique(ids):
     vals = torch.empty(n, dtype=torch.int64, device=ids.device)
     inv = torch.empty(n, dtype=torch.int32, device=ids.device)
     cnt = torch.zeros(1, dtype=torch.int64, device=ids.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_unique(ctx._h, ids.data_ptr(), n, vals.data_ptr(), inv.data_ptr(), cnt.data_ptr()))
+    _call("eu_unique", ids, n, vals, inv, cnt)
     return vals[:int(cnt.item())], inv
 
 
@@ -693,9 +627,7 @@ def sage_mean_aggregate(neighbor_ids, count, dim):
     ids = _t(neighbor_ids, torch.int64).reshape(-1)
     rows = ids.numel() // int(count)
     out = torch.empty((rows, int(dim)), dtype=torch.float32, device=ids.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sage_mean_aggregate(ctx._h, ids.data_ptr(), rows, int(count), int(dim),
-                                             out.data_ptr()))
+    _call("eu_sage_mean_aggregate", ids, rows, int(count), int(dim), out)
     return out
 
 
@@ -703,18 +635,14 @@ def sage_mean_aggregate(neighbor_ids, count, dim):
 def _raw_gather(params, indices):
     params = params.contiguous()
     out = torch.empty((indices.numel(), params.shape[1]), dtype=torch.float32, device=params.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_gather(ctx._h, params.data_ptr(), params.shape[0], params.shape[1],
-                                indices.data_ptr(), indices.numel(), out.data_ptr()))
+    _call("eu_gather", params, params.shape[0], params.shape[1], indices, indices.numel(), out)
     return out
 
 
 def _raw_scatter(name, updates, indices, size):
     updates = updates.contiguous()
     out = torch.empty((int(size), updates.shape[1]), dtype=torch.float32, device=updates.device)
-    ctx = _ctx_on_stream()
-    check(getattr(_lib.load(), name)(ctx._h, updates.data_ptr(), updates.shape[1], indices.data_ptr(),
-                                     indices.numel(), int(size), out.data_ptr()))
+    _call(name, updates, updates.shape[1], indices, indices.numel(), int(size), out)
     return out
 
 
@@ -771,6 +699,21 @@ def _f32(x):
     return x if x.dim() == 2 else x.reshape(x.shape[0], -1)
 
 
+def _check_f32(op, named, ndim=None):
+    """raise unless every (name, value) of named is a float32 tensor (with ndim dimensions when given)"""
+    for nm, t in named:
+        if not torch.is_tensor(t) or t.dtype != torch.float32 or (ndim is not None and t.dim() != ndim):
+            raise EulerError("%s: %s must be a %sfloat32 tensor" % (op, nm, "" if ndim is None else "%d-D " % ndim))
+
+
+def _dst_src(op, edge_index):
+    """(targets, sources) i32[E] of edge_index [2, E]"""
+    ei = _t(edge_index, torch.int32)
+    if ei.dim() != 2 or ei.shape[0] != 2:
+        raise EulerError("%s: edge_index must be [2, E]" % op)
+    return ei[0].contiguous(), ei[1].contiguous()
+
+
 def gather(params, indices):
     """mp_ops.gather = MPGather (mp_ops.py:27): out[i,:] = params[indices[i],:]."""
     return _Gather.apply(_f32(params), _t(indices, torch.int32).reshape(-1))
@@ -819,10 +762,7 @@ def _raw_gat(h_src, s_dst, s_src, dst, src, n_dst, with_alpha):
     E = dst.numel()
     out = torch.empty((n_dst, h_src.shape[1]), dtype=torch.float32, device=h_src.device)
     alpha = torch.empty((E, H), dtype=torch.float32, device=h_src.device) if with_alpha else None
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_gat_aggregate(ctx._h, h_src.data_ptr(), s_dst.data_ptr(), s_src.data_ptr(), dst.data_ptr(),
-                                       src.data_ptr(), E, n_dst, n_src, H, h_src.shape[1] // H, out.data_ptr(),
-                                       alpha.data_ptr() if with_alpha else None))
+    _call("eu_gat_aggregate", h_src, s_dst, s_src, dst, src, E, n_dst, n_src, H, h_src.shape[1] // H, out, alpha)
     return out, alpha
 
 
@@ -847,10 +787,8 @@ class _GatAggregate(torch.autograd.Function):
         g_h = torch.empty((n_src, H * C), dtype=torch.float32, device=dev)
         g_sd = torch.empty((n_dst, H), dtype=torch.float32, device=dev)
         g_ss = torch.empty((n_src, H), dtype=torch.float32, device=dev)
-        ec = _ctx_on_stream()
-        check(_lib.load().eu_gat_aggregate_backward(ec._h, grad.data_ptr(), h_src.data_ptr(), alpha.data_ptr(), s_dst.data_ptr(),
-                                                    s_src.data_ptr(), dst.data_ptr(), src.data_ptr(), dst.numel(), n_dst, n_src,
-                                                    H, C, g_h.data_ptr(), g_sd.data_ptr(), g_ss.data_ptr()))
+        _call("eu_gat_aggregate_backward", grad, h_src, alpha, s_dst, s_src, dst, src, dst.numel(), n_dst, n_src, H, C,
+              g_h, g_sd, g_ss)
         return g_h, g_sd, g_ss, None, None, None
 
 
@@ -871,10 +809,7 @@ def gat_attention_aggregate(h_src, s_dst, s_src, edge_index, size):
     if H < 1 or s_src.shape != (n_src, H) or s_dst.shape[0] != n_dst or h_src.shape[0] != n_src or h_src.shape[1] % H:
         raise EulerError("gat_attention_aggregate: need h_src [n_src, H*C], s_dst [n_dst, H], s_src [n_src, H]; got %s, %s, %s"
                          % (tuple(h_src.shape), tuple(s_dst.shape), tuple(s_src.shape)))
-    ei = _t(edge_index, torch.int32)
-    if ei.dim() != 2 or ei.shape[0] != 2:
-        raise EulerError("gat_attention_aggregate: edge_index must be [2, E]")
-    dst, src = ei[0].contiguous(), ei[1].contiguous()
+    dst, src = _dst_src("gat_attention_aggregate", edge_index)
     return _GatAggregate.apply(h_src, s_dst, s_src, dst, src, n_dst)
 
 
@@ -886,10 +821,7 @@ def _raw_agnn(x_src, nrm_dst, nrm_src, beta, dst, src, n_dst, with_alpha):
     out = torch.empty((n_dst, dim), dtype=torch.float32, device=dev)
     alpha = torch.empty(E, dtype=torch.float32, device=dev) if with_alpha else None
     cos = torch.empty(E, dtype=torch.float32, device=dev) if with_alpha else None
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_agnn_aggregate(ctx._h, x_src.data_ptr(), nrm_dst.data_ptr(), nrm_src.data_ptr(), beta.data_ptr(),
-                                        dst.data_ptr(), src.data_ptr(), E, n_dst, n_src, dim, out.data_ptr(),
-                                        alpha.data_ptr() if with_alpha else None, cos.data_ptr() if with_alpha else None))
+    _call("eu_agnn_aggregate", x_src, nrm_dst, nrm_src, beta, dst, src, E, n_dst, n_src, dim, out, alpha, cos)
     return out, alpha, cos
 
 
@@ -913,11 +845,8 @@ class _AgnnAggregate(torch.autograd.Function):
         g_x, g_ns = torch.empty_like(x_src), torch.empty_like(nrm_src)
         g_nd = torch.empty((ctx.n_dst, dim), dtype=torch.float32, device=grad.device)
         g_beta = torch.empty_like(beta)
-        ec = _ctx_on_stream()
-        check(_lib.load().eu_agnn_aggregate_backward(ec._h, grad.data_ptr(), x_src.data_ptr(), nrm_dst.data_ptr(), nrm_src.data_ptr(),
-                                                     beta.data_ptr(), alpha.data_ptr(), cos.data_ptr(), dst.data_ptr(),
-                                                     src.data_ptr(), dst.numel(), ctx.n_dst, n_src, dim, g_x.data_ptr(),
-                                                     g_nd.data_ptr(), g_ns.data_ptr(), g_beta.data_ptr()))
+        _call("eu_agnn_aggregate_backward", grad, x_src, nrm_dst, nrm_src, beta, alpha, cos, dst, src, dst.numel(), ctx.n_dst,
+              n_src, dim, g_x, g_nd, g_ns, g_beta)
         return g_x, g_nd, g_ns, g_beta, None, None, None
 
 
@@ -933,10 +862,7 @@ def agnn_attention_aggregate(x_src, nrm_dst, nrm_src, beta, edge_index, size):
     edge_index[0] the result equals, bit for bit, scatter_softmax / scatter_add composed from the ops above.  The backward
     pass is deterministic.  Synchronises once per call (whether edge_index[0] is sorted); an unsorted one costs a radix sort."""
     n_dst, n_src = int(size[0]), int(size[1])
-    named = (("x_src", x_src), ("nrm_dst", nrm_dst), ("nrm_src", nrm_src), ("beta", beta))
-    for nm, t in named:
-        if not torch.is_tensor(t) or t.dtype != torch.float32:
-            raise EulerError("agnn_attention_aggregate: %s must be a float32 tensor" % nm)
+    _check_f32("agnn_attention_aggregate", (("x_src", x_src), ("nrm_dst", nrm_dst), ("nrm_src", nrm_src), ("beta", beta)))
     if beta.numel() != 1:
         raise EulerError("agnn_attention_aggregate: beta must be a scalar (one element); got shape %s" % (tuple(beta.shape),))
     if any(t.dim() != 2 for t in (x_src, nrm_dst, nrm_src)):
@@ -947,10 +873,7 @@ def agnn_attention_aggregate(x_src, nrm_dst, nrm_src, beta, edge_index, size):
                          "got %s, %s, %s" % (n_src, n_dst, tuple(x_src.shape), tuple(nrm_src.shape), tuple(nrm_dst.shape)))
     x_src, nrm_dst, nrm_src = _t(x_src, torch.float32), _t(nrm_dst, torch.float32), _t(nrm_src, torch.float32)
     b = _t(beta, torch.float32).reshape(1)
-    ei = _t(edge_index, torch.int32)
-    if ei.dim() != 2 or ei.shape[0] != 2:
-        raise EulerError("agnn_attention_aggregate: edge_index must be [2, E]")
-    dst, src = ei[0].contiguous(), ei[1].contiguous()
+    dst, src = _dst_src("agnn_attention_aggregate", edge_index)
     return _AgnnAggregate.apply(x_src, nrm_dst, nrm_src, b, dst, src, n_dst)
 
 
@@ -959,9 +882,7 @@ def _raw_relation(x_src, matrix, rel, dst, src, n_dst):
     n_src, F = x_src.shape
     R, D = matrix.shape[0], matrix.shape[1]
     out = torch.empty((n_dst, D), dtype=torch.float32, device=x_src.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_relation_aggregate(ctx._h, x_src.data_ptr(), matrix.data_ptr(), rel.data_ptr(), dst.data_ptr(),
-                                            src.data_ptr(), dst.numel(), n_dst, n_src, R, D, F, out.data_ptr()))
+    _call("eu_relation_aggregate", x_src, matrix, rel, dst, src, dst.numel(), n_dst, n_src, R, D, F, out)
     return out
 
 
@@ -984,10 +905,8 @@ class _RelationAggregate(torch.autograd.Function):
         R, D = matrix.shape[0], matrix.shape[1]
         grad = grad.contiguous()
         g_x, g_m = torch.empty_like(x_src), torch.empty_like(matrix)
-        ec = _ctx_on_stream()
-        check(_lib.load().eu_relation_aggregate_backward(ec._h, grad.data_ptr(), x_src.data_ptr(), matrix.data_ptr(), rel.data_ptr(),
-                                                         dst.data_ptr(), src.data_ptr(), dst.numel(), ctx.n_dst, n_src, R, D, F,
-                                                         g_x.data_ptr(), g_m.data_ptr()))
+        _call("eu_relation_aggregate_backward", grad, x_src, matrix, rel, dst, src, dst.numel(), ctx.n_dst, n_src, R, D, F,
+              g_x, g_m)
         return g_x, g_m, None, None, None, None
 
 
@@ -1003,9 +922,7 @@ def relation_mean_aggregate(x_src, matrix, edge_attr, edge_index, size):
     unsorted (target, relation) keys give the bits of the stably sorted edge list.  Gradients reach x_src and matrix.
     Synchronises once per call (twice when the keys are unsorted, which costs a radix sort)."""
     n_dst, n_src = int(size[0]), int(size[1])
-    for nm, t in (("x_src", x_src), ("matrix", matrix)):
-        if not torch.is_tensor(t) or t.dtype != torch.float32:
-            raise EulerError("relation_mean_aggregate: %s must be a float32 tensor" % nm)
+    _check_f32("relation_mean_aggregate", (("x_src", x_src), ("matrix", matrix)))
     if x_src.dim() != 2 or matrix.dim() != 3:
         raise EulerError("relation_mean_aggregate: need x_src [n_src, F] (2-D) and matrix [R, D, F] (3-D); got %s, %s"
                          % (tuple(x_src.shape), tuple(matrix.shape)))
@@ -1015,13 +932,10 @@ def relation_mean_aggregate(x_src, matrix, edge_attr, edge_index, size):
                          % (n_src, F, tuple(x_src.shape), tuple(matrix.shape)))
     if not torch.is_tensor(edge_attr) or edge_attr.dtype.is_floating_point or edge_attr.dtype.is_complex:
         raise EulerError("relation_mean_aggregate: edge_attr must be an integer tensor")
-    ei = _t(edge_index, torch.int32)
-    if ei.dim() != 2 or ei.shape[0] != 2:
-        raise EulerError("relation_mean_aggregate: edge_index must be [2, E]")
-    if edge_attr.numel() != ei.shape[1]:
-        raise EulerError("relation_mean_aggregate: edge_attr has %d entries for %d edges" % (edge_attr.numel(), ei.shape[1]))
+    dst, src = _dst_src("relation_mean_aggregate", edge_index)
+    if edge_attr.numel() != dst.numel():
+        raise EulerError("relation_mean_aggregate: edge_attr has %d entries for %d edges" % (edge_attr.numel(), dst.numel()))
     rel = _t(edge_attr, torch.int32).reshape(-1)
-    dst, src = ei[0].contiguous(), ei[1].contiguous()
     return _RelationAggregate.apply(_t(x_src, torch.float32), _t(matrix, torch.float32), rel, dst, src, n_dst)
 
 
@@ -1031,10 +945,7 @@ def _raw_dna(q, k, v, n0, n1, dst, src, n_dst, heads, with_alpha):
     E = dst.numel()
     out = torch.empty((n_dst, dim), dtype=torch.float32, device=q.device)
     alpha = torch.empty((E, heads, heads), dtype=torch.float32, device=q.device) if with_alpha else None
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_dna_aggregate(ctx._h, q.data_ptr(), k.data_ptr(), v.data_ptr(), n0.data_ptr(), n1.data_ptr(),
-                                       dst.data_ptr(), src.data_ptr(), E, n_dst, n_src, heads, dim // heads, out.data_ptr(),
-                                       alpha.data_ptr() if with_alpha else None))
+    _call("eu_dna_aggregate", q, k, v, n0, n1, dst, src, E, n_dst, n_src, heads, dim // heads, out, alpha)
     return out, alpha
 
 
@@ -1057,10 +968,8 @@ class _DnaAggregate(torch.autograd.Function):
         n_src, dim = k.shape
         grad = grad.contiguous()
         g_q, g_k, g_v = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        ec = _ctx_on_stream()
-        check(_lib.load().eu_dna_aggregate_backward(ec._h, grad.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), n0.data_ptr(),
-                                                    n1.data_ptr(), alpha.data_ptr(), dst.data_ptr(), src.data_ptr(), dst.numel(),
-                                                    n_dst, n_src, H, dim // H, g_q.data_ptr(), g_k.data_ptr(), g_v.data_ptr()))
+        _call("eu_dna_aggregate_backward", grad, q, k, v, n0, n1, alpha, dst, src, dst.numel(), n_dst, n_src, H, dim // H,
+              g_q, g_k, g_v)
         return g_q, g_k, g_v, None, None, None, None, None, None
 
 
@@ -1076,9 +985,7 @@ def dna_attention_aggregate(q, k, v, n0, n1, edge_index, size, heads):
     edge_index[0] gives the bits of the stably sorted edge list.  Gradients reach q, k and v; the norms get none.
     Synchronises once per call (whether edge_index[0] is sorted); an unsorted one costs a radix sort."""
     n_dst, n_src = int(size[0]), int(size[1])
-    for nm, t in (("q", q), ("k", k), ("v", v), ("n0", n0), ("n1", n1)):
-        if not torch.is_tensor(t) or t.dtype != torch.float32:
-            raise EulerError("dna_attention_aggregate: %s must be a float32 tensor" % nm)
+    _check_f32("dna_attention_aggregate", (("q", q), ("k", k), ("v", v), ("n0", n0), ("n1", n1)))
     if any(t.dim() != 2 for t in (q, k, v)):
         raise EulerError("dna_attention_aggregate: q, k and v must be 2-D tensors")
     heads = int(heads)
@@ -1091,15 +998,35 @@ def dna_attention_aggregate(q, k, v, n0, n1, edge_index, size, heads):
     for nm, t, n in (("n0", n0, n_dst), ("n1", n1, n_src)):
         if t.numel() != n or t.dim() not in (1, 2) or (t.dim() == 2 and t.shape[1] != 1):
             raise EulerError("dna_attention_aggregate: %s must be [%d] or [%d, 1]; got %s" % (nm, n, n, tuple(t.shape)))
-    ei = _t(edge_index, torch.int32)
-    if ei.dim() != 2 or ei.shape[0] != 2:
-        raise EulerError("dna_attention_aggregate: edge_index must be [2, E]")
-    dst, src = ei[0].contiguous(), ei[1].contiguous()
+    dst, src = _dst_src("dna_attention_aggregate", edge_index)
     q, k, v = (_t(t, torch.float32) for t in (q, k, v))
     n0, n1 = (_t(t, torch.float32).detach().reshape(-1) for t in (n0, n1))
     return _DnaAggregate.apply(q, k, v, n0, n1, dst, src, n_dst, heads)
 
 
+# ------------------------------------------------------------------------------------ sparse table gradients
+def _coo_buffers(entries, shape, dev):
+    """the (rows i64[cap], values f32[cap, dim]) a sparse backward pass fills for a table of shape (n_rows, dim) that the
+    batch reaches through `entries` lookups: cap = min(entries, n_rows), sized from the entries, never from a large table's
+    rows.  (None, None) for an absent table (shape None)."""
+    if shape is None:
+        return None, None
+    cap = min(entries, shape[0])
+    return torch.empty(cap, dtype=torch.int64, device=dev), torch.empty((cap, shape[1]), dtype=torch.float32, device=dev)
+
+
+def _coo(rows, vals, n, shape):
+    """the coalesced sparse COO gradient of the first n rows / values of _coo_buffers' arrays (None for an absent table)"""
+    if shape is None:
+        return None
+    return torch.sparse_coo_tensor(rows[:n].unsqueeze(0), vals[:n], tuple(shape), is_coalesced=True, check_invariants=False)
+
+
+def _shape(table):
+    return None if table is None else tuple(table.shape)
+
+
+# ------------------------------------------------------------------------------------ sparse-feature embedding
 _COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
 
 
@@ -1107,9 +1034,7 @@ def _raw_embedding(nodes, fid, table, default_value, comb):
     """one eu_sparse_embedding_lookup: out f32[M, dim]"""
     n_rows, dim = table.shape
     out = torch.empty((nodes.numel(), dim), dtype=torch.float32, device=table.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sparse_embedding_lookup(ctx._h, nodes.data_ptr(), nodes.numel(), fid, default_value, table.data_ptr(), n_rows,
-                                                 dim, comb, out.data_ptr()))
+    _call("eu_sparse_embedding_lookup", nodes, nodes.numel(), fid, default_value, table, n_rows, dim, comb, out)
     return out
 
 
@@ -1130,34 +1055,21 @@ class _SparseEmbedding(torch.autograd.Function):
         nodes, = ctx.saved_tensors
         fid, default_value, comb, (n_rows, dim), sparse_grad = ctx.args
         grad = grad.contiguous()
-        ec, lib = _ctx_on_stream(), _lib.load()
+        args = (grad, nodes, nodes.numel(), fid, default_value, n_rows, dim, comb)
         if not sparse_grad:
             g_t = torch.empty((n_rows, dim), dtype=torch.float32, device=grad.device)
-            check(lib.eu_sparse_embedding_lookup_backward(ec._h, grad.data_ptr(), nodes.data_ptr(), nodes.numel(), fid, default_value,
-                                                          n_rows, dim, comb, g_t.data_ptr()))
+            _call("eu_sparse_embedding_lookup_backward", *args, g_t)
             return g_t, None, None, None, None, None
-        # the COO arrays hold min(entries, n_rows) rows: sized from the entries, never from a large table's rows
-        cap = min(_sparse_entries(nodes, fid), n_rows)
-        rows = torch.empty(cap, dtype=torch.int64, device=grad.device)
-        vals = torch.empty((cap, dim), dtype=torch.float32, device=grad.device)
+        rows, vals = _coo_buffers(_sparse_entries(nodes, fid), (n_rows, dim), grad.device)
         n = C.c_int64()
-        check(lib.eu_sparse_embedding_lookup_backward_sparse(ec._h, grad.data_ptr(), nodes.data_ptr(), nodes.numel(), fid, default_value,
-                                                             n_rows, dim, comb, rows.data_ptr(), vals.data_ptr(), C.byref(n)))
+        _call("eu_sparse_embedding_lookup_backward_sparse", *args, rows, vals, C.byref(n))
         return _coo(rows, vals, n.value, (n_rows, dim)), None, None, None, None, None
 
 
 def _sparse_entries(nodes, fid):
     """the entries get_sparse_feature lists for nodes in slot fid (a node without values counts one): one lengths pass and
     one read back"""
-    lib, ctx = _lib.load(), _ctx_on_stream()
-    indptr = torch.empty(nodes.numel() + 1, dtype=torch.int64, device=nodes.device)
-    check(lib.eu_get_sparse_feature(ctx._h, nodes.data_ptr(), nodes.numel(), int(fid), 0, 0, indptr.data_ptr(), None))
-    return int(indptr[-1].item())
-
-
-def _coo(rows, vals, n, shape):
-    """the coalesced sparse COO gradient of the first n rows / values"""
-    return torch.sparse_coo_tensor(rows[:n].unsqueeze(0), vals[:n], shape, is_coalesced=True, check_invariants=False)
+    return _ragged_lengths("eu_get_sparse_feature", nodes.numel(), nodes, nodes.numel(), int(fid), 0)[1]
 
 
 def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner='sum', sparse_grad=False):
@@ -1172,11 +1084,10 @@ def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner
     backward synchronises once (dense) or three times (sparse: sizing the COO, the entry count, the row count)."""
     if combiner not in _COMBINERS:
         raise EulerError("sparse_feature_embedding: combiner must be one of %s, got %r" % (sorted(_COMBINERS), combiner))
-    if not torch.is_tensor(table) or table.dtype != torch.float32 or table.dim() != 2:
-        raise EulerError("sparse_feature_embedding: table must be a 2-D float32 tensor")
-    fid = feature_name if isinstance(feature_name, (int, np.integer)) else get_graph().sparse_feature_id(str(feature_name))
+    _check_f32("sparse_feature_embedding", (("table", table),), 2)
+    fid = _slot(feature_name, get_graph().sparse_feature_id)
     nodes = _t(nodes, torch.int64).reshape(-1)
-    return _SparseEmbedding.apply(_t(table, torch.float32), nodes, int(fid), int(default_value), _COMBINERS[combiner], bool(sparse_grad))
+    return _SparseEmbedding.apply(_t(table, torch.float32), nodes, fid, int(default_value), _COMBINERS[combiner], bool(sparse_grad))
 
 
 # ------------------------------------------------------------------------------------ ShallowEncoder's input row
@@ -1212,8 +1123,7 @@ class _ShallowEncode(torch.autograd.Function):
         out = torch.empty((M, W), dtype=torch.float32, device=dev)
         dense_out = torch.empty((M, dense_w), dtype=torch.float32, device=dev) if comb == 1 else None
         p = _shallow_problem(nodes, id_table, dense, sparse, comb)
-        check(_lib.load().eu_shallow_encode(_ctx_on_stream()._h, C.byref(p), out.data_ptr(),
-                                            dense_out.data_ptr() if dense_out is not None else None))
+        _call("eu_shallow_encode", C.byref(p), out, dense_out)
         ctx.save_for_backward(nodes, id_table, *tables)
         ctx.cfg = cfg
         if dense_out is None:
@@ -1227,28 +1137,19 @@ class _ShallowEncode(torch.autograd.Function):
         dense, sparse_cfg, comb, W, dense_w, sparse_grad = ctx.cfg
         sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
         all_tables = [id_table] + list(tables)
-        dev = nodes.device
         grad = grad.contiguous()
         p = _shallow_problem(nodes, id_table, dense, sparse, comb)
-        ec, lib = _ctx_on_stream(), _lib.load()
-        NT = len(all_tables)
-        PT = C.c_void_p * NT
         if not sparse_grad:
-            grads = [torch.empty_like(t) if t is not None else None for t in all_tables]
-            check(lib.eu_shallow_encode_backward(ec._h, C.byref(p), grad.data_ptr(),
-                                                 PT(*[g.data_ptr() if g is not None else None for g in grads])))
+            grads = [None if t is None else torch.empty_like(t) for t in all_tables]
+            _call("eu_shallow_encode_backward", C.byref(p), grad, grads)
             return (None, None) + tuple(grads)
-        # arrays of min(entries, n_rows) rows: the id table has M entries, a slot its get_sparse_feature entries
-        caps = [min(nodes.numel(), id_table.shape[0]) if id_table is not None else 0]
-        caps += [min(_sparse_entries(nodes, fid), t.shape[0]) for fid, t, _, _ in sparse]
-        rows = [torch.empty(cap, dtype=torch.int64, device=dev) for cap in caps]
-        vals = [torch.empty((cap, t.shape[1] if t is not None else 0), dtype=torch.float32, device=dev) for cap, t in zip(caps, all_tables)]
-        counts = (C.c_int64 * NT)()
-        check(lib.eu_shallow_encode_backward_sparse(ec._h, C.byref(p), grad.data_ptr(), PT(*[r.data_ptr() for r in rows]),
-                                                    PT(*[v.data_ptr() for v in vals]), counts))
-        grads = [_coo(r, v, counts[t], tuple(all_tables[t].shape)) if all_tables[t] is not None else None
-                 for t, (r, v) in enumerate(zip(rows, vals))]
-        return (None, None) + tuple(grads)
+        # the id table has M entries, a slot its get_sparse_feature entries
+        entries = [nodes.numel()] + [_sparse_entries(nodes, fid) for fid, _, _, _ in sparse]
+        shapes = [_shape(t) for t in all_tables]
+        bufs = [_coo_buffers(e, sh, nodes.device) for e, sh in zip(entries, shapes)]
+        counts = (C.c_int64 * len(all_tables))()
+        _call("eu_shallow_encode_backward_sparse", C.byref(p), grad, [r for r, _ in bufs], [v for _, v in bufs], counts)
+        return (None, None) + tuple(_coo(r, v, counts[t], shapes[t]) for t, (r, v) in enumerate(bufs))
 
 
 def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat', sparse_grad=False):
@@ -1273,17 +1174,16 @@ def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat',
     if len(dense) > _lib.SHALLOW_MAX_SLOTS or len(sparse) > _lib.SHALLOW_MAX_SLOTS:
         raise EulerError("shallow_encode: at most %d dense and %d sparse slots" % (_lib.SHALLOW_MAX_SLOTS, _lib.SHALLOW_MAX_SLOTS))
     tables = ([id_table] if id_table is not None else []) + [s[1] for s in sparse]
-    for t in tables:
-        if not torch.is_tensor(t) or t.dtype != torch.float32 or t.dim() != 2:
-            raise EulerError("shallow_encode: tables must be 2-D float32 tensors")
-    d_cfg = tuple((int(n) if isinstance(n, (int, np.integer)) else g.dense_feature_id(str(n)), int(d)) for n, d in dense)
+    named = [("sparse table %d" % k, s[1]) for k, s in enumerate(sparse)]
+    _check_f32("shallow_encode", ([("id_table", id_table)] if id_table is not None else []) + named, 2)
+    d_cfg = tuple((_slot(n, g.dense_feature_id), int(d)) for n, d in dense)
     s_cfg = []
     for s in sparse:
         name, _, dv = s[:3]
         c = s[3] if len(s) > 3 else 'sum'
         if c not in _COMBINERS:
             raise EulerError("shallow_encode: sparse combiner must be one of %s, got %r" % (sorted(_COMBINERS), c))
-        s_cfg.append((int(name) if isinstance(name, (int, np.integer)) else g.sparse_feature_id(str(name)), int(dv), _COMBINERS[c]))
+        s_cfg.append((_slot(name, g.sparse_feature_id), int(dv), _COMBINERS[c]))
     emb_dims = [t.shape[1] for t in tables]
     if comb == 1 and len(set(emb_dims)) > 1:
         raise EulerError("shallow_encode: 'add' needs one dim for every table, got %s" % emb_dims)
@@ -1328,8 +1228,7 @@ def sample_graph_label(count):
     uniformly from this thread's engine (the same stream position as the reference's ThreadLocalRandom under rng='minstd')."""
     count = int(count)
     out = torch.empty(count, dtype=torch.int32, device=_dev())
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_sample_graph_label(ctx._h, count, out.data_ptr()))
+    _call("eu_sample_graph_label", count, out)
     return out
 
 
@@ -1343,16 +1242,14 @@ def get_graph_by_label(labels):
         labels = [index.get(v if isinstance(v, bytes) else str(v).encode(), -1) for v in labels]
     labels = _t(labels, torch.int32).reshape(-1)
     B = labels.numel()
-    lib, ctx = _lib.load(), _ctx_on_stream()
     ptr = torch.empty(B + 1, dtype=torch.int64, device=labels.device)
     total, max_len = C.c_int64(), C.c_int64()
-    check(lib.eu_get_graph_by_label(ctx._h, labels.data_ptr(), B, 0, ptr.data_ptr(), None, None, C.byref(total), C.byref(max_len)))
+    _call("eu_get_graph_by_label", labels, B, 0, ptr, None, None, C.byref(total), C.byref(max_len))
     nnz = total.value
     indices = torch.empty((nnz, 2), dtype=torch.int64, device=labels.device)
     values = torch.empty(nnz, dtype=torch.int64, device=labels.device)
     if nnz:
-        check(lib.eu_get_graph_by_label(ctx._h, labels.data_ptr(), B, nnz, ptr.data_ptr(), indices.data_ptr(), values.data_ptr(),
-                                        None, None))
+        _call("eu_get_graph_by_label", labels, B, nnz, ptr, indices, values, None, None)
     return indices, values, (B, max_len.value)
 
 
@@ -1361,10 +1258,7 @@ def _raw_readout(x, index, size, logits, q):
     N, D = x.shape
     out = torch.empty((size, D), dtype=torch.float32, device=x.device)
     alpha = torch.empty(N, dtype=torch.float32, device=x.device)
-    ctx = _ctx_on_stream()
-    check(_lib.load().eu_graph_attention_readout(ctx._h, x.data_ptr(), index.data_ptr(), N, size, D,
-                                                 logits.data_ptr() if logits is not None else None,
-                                                 q.data_ptr() if q is not None else None, out.data_ptr(), alpha.data_ptr()))
+    _call("eu_graph_attention_readout", x, index, N, size, D, logits, q, out, alpha)
     return out, alpha
 
 
@@ -1385,12 +1279,9 @@ class _GraphReadout(torch.autograd.Function):
         grad = grad.contiguous()
         g_x = torch.empty_like(x)
         g_w = torch.empty_like(weight)
-        q = weight if ctx.by_query else None
-        ec = _ctx_on_stream()
-        check(_lib.load().eu_graph_attention_readout_backward(ec._h, grad.data_ptr(), x.data_ptr(), index.data_ptr(), N, ctx.size,
-                                                              D, q.data_ptr() if q is not None else None, alpha.data_ptr(),
-                                                              g_x.data_ptr(), None if ctx.by_query else g_w.data_ptr(),
-                                                              g_w.data_ptr() if ctx.by_query else None))
+        by_query = ctx.by_query
+        _call("eu_graph_attention_readout_backward", grad, x, index, N, ctx.size, D, weight if by_query else None, alpha, g_x,
+              None if by_query else g_w, g_w if by_query else None)
         return g_x, g_w, None, None, None
 
 
@@ -1406,8 +1297,7 @@ def graph_attention_readout(x, index, size, logits=None, q=None):
     pass is deterministic.  Synchronises once per call (whether index is sorted); an unsorted one costs a radix sort."""
     if (logits is None) == (q is None):
         raise EulerError("graph_attention_readout: give exactly one of logits and q")
-    if not torch.is_tensor(x) or x.dim() != 2 or x.dtype != torch.float32:
-        raise EulerError("graph_attention_readout: x must be a 2-D float32 tensor")
+    _check_f32("graph_attention_readout", (("x", x),), 2)
     size = int(size)
     x = _f32(x)
     index = _t(index, torch.int32).reshape(-1)
@@ -1453,9 +1343,7 @@ def _raw_skipgram(src, pos, negs, target, context):
     logits = torch.empty((B, P + K), dtype=torch.float32, device=target.device)
     rank = torch.empty(B, dtype=torch.int32, device=target.device)
     loss = torch.empty((), dtype=torch.float32, device=target.device)
-    ec = _ctx_on_stream()
-    check(_lib.load().eu_skipgram_loss(ec._h, src.data_ptr(), pos.data_ptr(), negs.data_ptr(), B, P, K, target.data_ptr(),
-                                       context.data_ptr(), n_rows, dim, logits.data_ptr(), rank.data_ptr(), loss.data_ptr()))
+    _call("eu_skipgram_loss", src, pos, negs, B, P, K, target, context, n_rows, dim, logits, rank, loss)
     return logits, rank, loss
 
 
@@ -1480,32 +1368,19 @@ class _SkipgramLoss(torch.autograd.Function):
         n_rows, dim = target.shape
         dev = target.device
         g = g_loss.to(device=dev, dtype=torch.float32).reshape(1).contiguous()
-        ec, lib = _ctx_on_stream(), _lib.load()
-        args = (ec._h, g.data_ptr(), src.data_ptr(), pos.data_ptr(), negs.data_ptr(), B, P, K, target.data_ptr(), context.data_ptr(),
-                n_rows, dim, logits.data_ptr())
+        args = (g, src, pos, negs, B, P, K, target, context, n_rows, dim, logits)
         if not ctx.sparse_grad:
             g_t = torch.empty((n_rows, dim), dtype=torch.float32, device=dev)
             g_c = g_t if ctx.shared else torch.empty((n_rows, dim), dtype=torch.float32, device=dev)
-            check(lib.eu_skipgram_loss_backward(*args, g_t.data_ptr(), g_c.data_ptr()))
+            _call("eu_skipgram_loss_backward", *args, g_t, g_c)
             return g_t, None if ctx.shared else g_c, None, None, None, None, None
-
-        def coo_buffers(entries):
-            cap = min(entries, n_rows)
-            return torch.empty(cap, dtype=torch.int64, device=dev), torch.empty((cap, dim), dtype=torch.float32, device=dev)
-
-        rows_t, vals_t = coo_buffers(B * (P + K + 1) if ctx.shared else B)
-        rows_c, vals_c = (None, None) if ctx.shared else coo_buffers(B * (P + K))
+        # a shared table takes the target and the context entries in one list
+        shape_t, shape_c = (n_rows, dim), None if ctx.shared else (n_rows, dim)
+        rows_t, vals_t = _coo_buffers(B * (P + K + 1) if ctx.shared else B, shape_t, dev)
+        rows_c, vals_c = _coo_buffers(B * (P + K), shape_c, dev)
         n_t, n_c = C.c_int64(), C.c_int64()
-        check(lib.eu_skipgram_loss_backward_sparse(*args, rows_t.data_ptr(), vals_t.data_ptr(), C.byref(n_t),
-                                                   rows_c.data_ptr() if rows_c is not None else None,
-                                                   vals_c.data_ptr() if vals_c is not None else None, C.byref(n_c)))
-
-        def coo(rows, vals, n):
-            return torch.sparse_coo_tensor(rows[:n].unsqueeze(0), vals[:n], (n_rows, dim), is_coalesced=True,
-                                           check_invariants=False)
-
-        g_t = coo(rows_t, vals_t, n_t.value)
-        return g_t, None if ctx.shared else coo(rows_c, vals_c, n_c.value), None, None, None, None, None
+        _call("eu_skipgram_loss_backward_sparse", *args, rows_t, vals_t, C.byref(n_t), rows_c, vals_c, C.byref(n_c))
+        return _coo(rows_t, vals_t, n_t.value, shape_t), _coo(rows_c, vals_c, n_c.value, shape_c), None, None, None, None, None
 
 
 def skipgram_xent_loss(src, pos, negs, target, context, metric='mrr', sparse_grad=False):
@@ -1523,9 +1398,7 @@ def skipgram_xent_loss(src, pos, negs, target, context, metric='mrr', sparse_gra
     if metric not in SKIPGRAM_METRICS:
         raise EulerError("skipgram_xent_loss: metric must be one of %s, got %r" % (SKIPGRAM_METRICS, metric))
     shared = context is target
-    for name, tb in (('target', target), ('context', context)):
-        if not torch.is_tensor(tb) or tb.dtype != torch.float32 or tb.dim() != 2:
-            raise EulerError("skipgram_xent_loss: %s must be a 2-D float32 tensor" % name)
+    _check_f32("skipgram_xent_loss", (('target', target), ('context', context)), 2)
     if target.shape != context.shape:
         raise EulerError("skipgram_xent_loss: target %s and context %s must have one shape" % (tuple(target.shape), tuple(context.shape)))
     src = _t(src, torch.int64).reshape(-1)
@@ -1557,7 +1430,8 @@ def _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, 
     p.n_ent, p.n_rel = slots[0].shape[0], slots[1].shape[0]
     p.src, p.dst, p.rel, p.neg = src.data_ptr(), dst.data_ptr(), rel.data_ptr(), neg.data_ptr()
     for t, tb in enumerate(slots):
-        p.table[t] = tb.data_ptr() if tb is not None else None
+        if tb is not None:
+            p.table[t] = tb.data_ptr()
     return p
 
 
@@ -1571,8 +1445,7 @@ def _raw_kg(ent, relt, eaux, raux, src, dst, rel, neg, cfg):
     loss = torch.empty((), dtype=torch.float32, device=dev)
     embs = [torch.empty((B, rel_dim), dtype=torch.float32, device=dev) for _ in range(3)] if with_emb else None
     p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, (ent, relt, eaux, raux), ent_dim, rel_dim)
-    e_ptr = [e.data_ptr() for e in embs] if embs else [None] * 3
-    check(_lib.load().eu_kg_loss(_ctx_on_stream()._h, C.byref(p), scores.data_ptr(), rank.data_ptr(), loss.data_ptr(), *e_ptr))
+    _call("eu_kg_loss", C.byref(p), scores, rank, loss, *(embs or [None] * 3))
     return scores, rank, loss, embs
 
 
@@ -1599,37 +1472,17 @@ class _KgLoss(torch.autograd.Function):
         dev = ent.device
         g = g_loss.to(device=dev, dtype=torch.float32).reshape(1).contiguous()
         p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, rel_dim)
-        ec, lib = _ctx_on_stream(), _lib.load()
-        P4 = C.c_void_p * 4
         if not sparse_grad:
-            grads = [torch.empty_like(t) if t is not None else None for t in slots]
-            check(lib.eu_kg_loss_backward(ec._h, C.byref(p), g.data_ptr(), scores.data_ptr(),
-                                          P4(*[t.data_ptr() if t is not None else None for t in grads])))
+            grads = [None if t is None else torch.empty_like(t) for t in slots]
+            _call("eu_kg_loss_backward", C.byref(p), g, scores, grads)
             return tuple(grads) + (None,) * 5
         B, K = neg.shape
         entries = (B * (K + 2), B, B * (K + 2), B)
-        rows, vals = [], []
-        for t, tb in enumerate(slots):
-            if tb is None:
-                rows.append(None)
-                vals.append(None)
-                continue
-            cap = min(entries[t], tb.shape[0])
-            rows.append(torch.empty(cap, dtype=torch.int64, device=dev))
-            vals.append(torch.empty((cap, tb.shape[1]), dtype=torch.float32, device=dev))
+        shapes = [_shape(t) for t in slots]
+        bufs = [_coo_buffers(e, sh, dev) for e, sh in zip(entries, shapes)]
         counts = (C.c_int64 * 4)()
-        check(lib.eu_kg_loss_backward_sparse(ec._h, C.byref(p), g.data_ptr(), scores.data_ptr(),
-                                             P4(*[r.data_ptr() if r is not None else None for r in rows]),
-                                             P4(*[v.data_ptr() if v is not None else None for v in vals]), counts))
-        grads = []
-        for t, tb in enumerate(slots):
-            if tb is None:
-                grads.append(None)
-                continue
-            n = counts[t]
-            grads.append(torch.sparse_coo_tensor(rows[t][:n].unsqueeze(0), vals[t][:n], tuple(tb.shape), is_coalesced=True,
-                                                 check_invariants=False))
-        return tuple(grads) + (None,) * 5
+        _call("eu_kg_loss_backward_sparse", C.byref(p), g, scores, [r for r, _ in bufs], [v for _, v in bufs], counts)
+        return tuple(_coo(r, v, counts[t], shapes[t]) for t, (r, v) in enumerate(bufs)) + (None,) * 5
 
 
 def kg_margin_loss(src, dst, neg, rel, tables, model, l1=True, corrupt='both', margin=1.0, metric='mrr', sparse_grad=False,
@@ -1659,9 +1512,7 @@ def kg_margin_loss(src, dst, neg, rel, tables, model, l1=True, corrupt='both', m
     tables = list(tables)
     if len(tables) != len(want):
         raise EulerError("kg_margin_loss: %s takes %d tables, got %d" % (name, len(want), len(tables)))
-    for tb in tables:
-        if not torch.is_tensor(tb) or tb.dtype != torch.float32 or tb.dim() != 2:
-            raise EulerError("kg_margin_loss: tables must be 2-D float32 tensors")
+    _check_f32("kg_margin_loss", [("table %d" % k, tb) for k, tb in enumerate(tables)], 2)
     slots = [None] * 4
     for t, tb in zip(want, tables):
         slots[t] = _t(tb, torch.float32)
