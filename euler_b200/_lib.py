@@ -52,6 +52,7 @@ class KgProblem(C.Structure):
 
 SHALLOW_MAX_SLOTS = 8   # EU_SHALLOW_MAX_SLOTS
 SHALLOW_MAX_WIDTH = 16384   # EU_SHALLOW_MAX_WIDTH
+SHALLOW_POOL_MAX_COUNT = 512   # EU_SHALLOW_POOL_MAX_COUNT
 
 
 class ShallowDense(C.Structure):
@@ -179,6 +180,9 @@ SIGNATURES = {
     "eu_shallow_encode": (C.c_int, [_P, _P, _P, _P]),
     "eu_shallow_encode_backward": (C.c_int, [_P, _P, _P, _P]),
     "eu_shallow_encode_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "eu_shallow_encode_pool": (C.c_int, [_P, _P, _I32, _I32, _P]),
+    "eu_shallow_encode_pool_backward": (C.c_int, [_P, _P, _I32, _I32, _P, _P]),
+    "eu_shallow_encode_pool_backward_sparse": (C.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P]),
     "eu_gather_host": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P]),
     "eu_scatter_add_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),
     "eu_scatter_max_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),

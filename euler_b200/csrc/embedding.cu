@@ -1,6 +1,8 @@
 // SparseEmbedding's lookup from node ids, forward and backward: the uint64 ("sparse") slot of each node, turned into one
 // f32 row by an embedding table, with no host round trip and no intermediate COO.  And ShallowEncoder's whole input row (an
-// id embedding, dense feature slots and several such lookups, concatenated or added) in one pass over the nodes.
+// id embedding, dense feature slots and several such lookups, concatenated or added) in one pass over the nodes; and those
+// rows pooled (sum or mean) over fixed segments of nodes without being written, what SageEncoder's first layer needs of the
+// deepest hop of a fanout (k_shallow_pool; its backward is the shared one, reading gradient row node / count).
 //
 // Reference semantics (file:line in the upstream alibaba/euler tree):
 //   SparseEmbedding.call      tf_euler/python/utils/layers.py:152-169  tf.nn.embedding_lookup_sparse(table, sp_ids, None,
@@ -62,9 +64,37 @@ template <> struct EmbVec<false> {
   static __device__ __forceinline__ T div(T a, float den) { return __fdiv_rn(a, den); }
 };
 
+// This lane's columns [d, d + W) of the sum of the bag [b, e) of the uint64 values (empty: the one entry dflt), whole-group
+// call (every lane of the group takes part in the shuffles; act: d < dim, an inactive lane loads nothing).  The sum starts
+// from the bag's first row (its bits, -0.0 and NaN payloads included) and adds the others left to right.
+template <bool VEC>
+__device__ __forceinline__ typename EmbVec<VEC>::T emb_bag_tile(const DevGraph& g, int64_t b, int64_t e, unsigned long long dflt,
+                                                                const float* __restrict__ table, int dim, int d, bool act, int G,
+                                                                int sub, unsigned gm) {
+  using V = EmbVec<VEC>;
+  const bool empty = e == b;
+  const int64_t n = empty ? 1 : e - b;
+  typename V::T acc = V::zero(0.f);
+  for (int64_t k0 = 0; k0 < n; k0 += G) {
+    const unsigned long long mine = k0 + sub < n ? (empty ? dflt : __ldg(g.u64_val + b + k0 + sub)) : 0ull;
+    const int cnt = n - k0 < G ? (int)(n - k0) : G;
+    for (int j0 = 0; j0 < cnt; j0 += kEmbUnroll) {
+      typename V::T x[kEmbUnroll];
+#pragma unroll
+      for (int q = 0; q < kEmbUnroll; ++q) {
+        const unsigned long long v = __shfl_sync(gm, mine, (j0 + q) & (G - 1), G);
+        x[q] = act && j0 + q < cnt ? V::load(table + (int64_t)v * dim + d) : V::zero(0.f);
+      }
+#pragma unroll
+      for (int q = 0; q < kEmbUnroll; ++q)
+        if (j0 + q < cnt) acc = k0 + j0 + q == 0 ? x[q] : V::add(acc, x[q]);
+    }
+  }
+  return acc;
+}
+
 // The bag sum of graph row `row` (-1: absent) in slot fid, before the combiner's division: G lanes (this one is `sub`, the
-// group's mask gm), W columns per lane and step, blocks of G * W columns with a group-uniform trip count, so every lane of
-// the group takes part in the shuffles.  The sum starts from the bag's first row (its bits, -0.0 and NaN payloads included).
+// group's mask gm), W columns per lane and step, blocks of G * W columns with a group-uniform trip count (emb_bag_tile).
 // *n = the bag's entries (1 for the default); it is set before the first sink(d, acc) call, which hands over the lane's
 // columns [d, d + W) of the sum, for d < dim only.
 template <bool VEC, typename Sink>
@@ -74,29 +104,11 @@ __device__ __forceinline__ void emb_bag_sum(const DevGraph& g, int64_t row, int3
   using V = EmbVec<VEC>;
   int64_t b, e;
   ragged_slice(g.u64_ptr, g.n_u64_slots, row, fid, &b, &e);
-  const bool empty = e == b;
-  const int64_t n = empty ? 1 : e - b;
-  *n_out = n;
+  *n_out = e == b ? 1 : e - b;
   for (int d0 = 0; d0 < dim; d0 += G * V::W) {
     const int d = d0 + sub * V::W;
-    const bool act = d < dim;
-    typename V::T acc = V::zero(0.f);
-    for (int64_t k0 = 0; k0 < n; k0 += G) {
-      const unsigned long long mine = k0 + sub < n ? (empty ? dflt : __ldg(g.u64_val + b + k0 + sub)) : 0ull;
-      const int cnt = n - k0 < G ? (int)(n - k0) : G;
-      for (int j0 = 0; j0 < cnt; j0 += kEmbUnroll) {
-        typename V::T x[kEmbUnroll];
-#pragma unroll
-        for (int q = 0; q < kEmbUnroll; ++q) {
-          const unsigned long long v = __shfl_sync(gm, mine, (j0 + q) & (G - 1), G);
-          x[q] = act && j0 + q < cnt ? V::load(table + (int64_t)v * dim + d) : V::zero(0.f);
-        }
-#pragma unroll
-        for (int q = 0; q < kEmbUnroll; ++q)
-          if (j0 + q < cnt) acc = k0 + j0 + q == 0 ? x[q] : V::add(acc, x[q]);
-      }
-    }
-    if (act) sink(d, acc);
+    const typename V::T acc = emb_bag_tile<VEC>(g, b, e, dflt, table, dim, d, d < dim, G, sub, gm);
+    if (d < dim) sink(d, acc);
   }
 }
 
@@ -192,6 +204,82 @@ __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, i
   }
 }
 
+// ---------------------------------------------------------------------------- ShallowEncoder's rows, pooled per segment
+// One pooled column: load(0), then load(j) added left to right for j = 1 .. count - 1, kEmbUnroll loads ahead of the adds
+template <typename Load>
+__device__ __forceinline__ float pool_column(int count, Load load) {
+  float acc = 0.f;
+  for (int j0 = 0; j0 < count; j0 += kEmbUnroll) {
+    float x[kEmbUnroll];
+#pragma unroll
+    for (int q = 0; q < kEmbUnroll; ++q)
+      if (j0 + q < count) x[q] = load(j0 + q);
+#pragma unroll
+    for (int q = 0; q < kEmbUnroll; ++q)
+      if (j0 + q < count) acc = j0 + q == 0 ? x[q] : __fadd_rn(acc, x[q]);
+  }
+  return acc;
+}
+
+// slot s of the segment's nodes (their graph rows in `rows`), pooled into o (the slot's first column of the output row):
+// per tile of G * W columns, each node's bag sum and combiner division (shallow_slot's), added across the nodes in registers
+template <bool VEC>
+__device__ __forceinline__ void shallow_pool_slot(const DevGraph& g, const ShallowDev& p, int s, const int64_t* rows, int count,
+                                                  float pool_den, float* o, int G, int sub, unsigned gm) {
+  using V = EmbVec<VEC>;
+  const int comb = p.sp_comb[s], dim = p.sp_dim[s];
+  for (int d0 = 0; d0 < dim; d0 += G * V::W) {
+    const int d = d0 + sub * V::W;
+    typename V::T acc = V::zero(0.f);
+    for (int j = 0; j < count; ++j) {
+      int64_t b, e;
+      ragged_slice(g.u64_ptr, g.n_u64_slots, rows[j], p.sp_fid[s], &b, &e);
+      typename V::T x = emb_bag_tile<VEC>(g, b, e, p.sp_dflt[s], p.sp_table[s], dim, d, d < dim, G, sub, gm);
+      if (comb != EU_COMBINE_SUM) x = V::div(x, emb_den(e == b ? 1 : e - b, comb));
+      acc = j == 0 ? x : V::add(acc, x);
+    }
+    if (pool_den != 0.f) acc = V::div(acc, pool_den);
+    if (d < dim) V::store(o + d, acc);
+  }
+}
+
+// G lanes per output row r, the pool of the `count` ShallowEncoder rows (CONCAT) of nodes[r * count ..]: k_shallow_fwd's
+// parts and rules, each column summed over the segment's nodes in a register, in node order, and divided once by pool_den
+// (fl(count); 0: the sum).  The group looks every node's graph row up once, into its `count` slots of shared memory.
+__global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev p, int count, float pool_den, int G) {
+  extern __shared__ int64_t pool_rows[];
+  const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t r = tid >> (31 - __clz(G));
+  const int sub = (int)(tid & (G - 1));
+  if (r >= p.M / count) return;   // group-uniform
+  const unsigned gm = group_mask(G);
+  const unsigned long long* nodes = p.nodes + r * count;
+  int64_t* rows = pool_rows + (threadIdx.x >> (31 - __clz(G))) * (int64_t)count;
+  for (int j = sub; j < count; j += G) rows[j] = lookup_row(g, __ldg(nodes + j));
+  __syncwarp(gm);
+  float* o = p.out + r * (int64_t)p.W;
+  auto finish = [&](float acc) { return pool_den != 0.f ? __fdiv_rn(acc, pool_den) : acc; };
+  for (int d = sub; d < p.id_dim; d += G)
+    o[d] = finish(pool_column(count, [&](int j) {
+      const long long id = (long long)__ldg(nodes + j);
+      const bool ok = id >= 0 && id < p.n_id_rows;   // false only under capture (the check is skipped)
+      return ok ? __ldg(p.id_table + id * p.id_dim + d) : __int_as_float(0x7fc00000);
+    }));
+  for (int k = 0; k < p.n_dense; ++k) {
+    const int32_t fid = p.dense_fid[k];
+    const bool known = fid >= 0 && fid < g.n_slots;
+    const int sdim = known ? g.slot_dim[fid] : 0;
+    const float* f = g.feat + (known ? g.slot_off[fid] : 0);
+    float* oj = o + p.dense_off[k];
+    for (int d = sub; d < p.dense_dim[k]; d += G)
+      oj[d] = finish(pool_column(count, [&](int j) { return d < sdim && rows[j] >= 0 ? __ldg(f + rows[j] * (int64_t)g.feat_dim + d) : 0.f; }));
+  }
+  for (int s = 0; s < p.n_sparse; ++s) {
+    if (p.vec_mask >> s & 1) shallow_pool_slot<true>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
+    else shallow_pool_slot<false>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
+  }
+}
+
 // *bad = 1 when an id lies outside [0, n_rows)
 __global__ void k_id_range(const int64_t* __restrict__ ids, int64_t M, int64_t n_rows, int* bad) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M; i += (int64_t)gridDim.x * blockDim.x) {
@@ -259,23 +347,33 @@ __global__ void __launch_bounds__(256) k_emb_entries(DevGraph g, const unsigned 
   }
 }
 
-// gs[i, d] = g[i * ld + d] / den(n_i) (one __fdiv_rn), n_i = ptr[i + 1] - ptr[i]: the scaled gradient of the mean and sqrtn
-// combiners, once per node and column rather than once per entry
-__global__ void k_emb_scale_grad(const float* __restrict__ g, int64_t ld, const int64_t* __restrict__ ptr, int64_t M, int dim, int comb,
-                                 float* __restrict__ gs) {
+// How the nodes share gradient rows: node i reads row i / group of grad_out, divided first by pool_den (one __fdiv_rn per
+// element read) unless that is 0.  {1, 0}: a row per node, as it is -- the ops that do not pool.
+struct GradRows {
+  int group = 1;
+  float pool_den = 0.f;
+};
+
+// gs[i, d] = g[(i / group) * ld + d] (pooled: / pool_den) / den(n_i) (one __fdiv_rn), n_i = ptr[i + 1] - ptr[i]: the scaled
+// gradient of the mean and sqrtn combiners, once per node and column rather than once per entry
+__global__ void k_emb_scale_grad(const float* __restrict__ g, int64_t ld, GradRows gr, const int64_t* __restrict__ ptr, int64_t M, int dim,
+                                 int comb, float* __restrict__ gs) {
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < M * dim; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = t / dim;
-    gs[t] = __fdiv_rn(__ldg(g + i * ld + (t - i * dim)), emb_den(__ldg(ptr + i + 1) - __ldg(ptr + i), comb));
+    float x = __ldg(g + (i / gr.group) * ld + (t - i * dim));
+    if (gr.pool_den != 0.f) x = __fdiv_rn(x, gr.pool_den);
+    gs[t] = __fdiv_rn(x, emb_den(__ldg(ptr + i + 1) - __ldg(ptr + i), comb));
   }
 }
 
 // G lanes per chunk c of the distinct-value segments (grid-stride over the chunks, whose number is on the device).  Chunk
 // c - chunk_off[p] of segment p covers the sorted positions [start[p] + (c - chunk_off[p]) * kSegChunk, ...), up to kSegChunk
-// of them: the sum, left to right from +0, of the (scaled) gradient rows gs[node * ld] of their nodes.  A segment of one chunk
+// of them: the sum, left to right from +0, of the (scaled) gradient rows gs[(node / group) * ld] of their nodes, each divided
+// by pool_den first when that is not 0 (GradRows).  A segment of one chunk
 // writes its output row (by_key: the table row key[p]; else row p of the COO values); the chunks of a longer one write their
 // partial rows for k_row_combine.
 template <bool VEC>
-__global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restrict__ gs, int64_t ld, const int32_t* __restrict__ node,
+__global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restrict__ gs, int64_t ld, GradRows gr, const int32_t* __restrict__ node,
                                                         const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G, bool by_key,
                                                         float* __restrict__ out) {
   using V = EmbVec<VEC>;
@@ -295,10 +393,10 @@ __global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restri
         typename V::T x[kEmbUnroll];
 #pragma unroll
         for (int q = 0; q < kEmbUnroll; ++q)
-          if (k0 + q < e) x[q] = V::load(gs + (int64_t)__ldg(node + __ldg(perm + k0 + q)) * ld + d);
+          if (k0 + q < e) x[q] = V::load(gs + (int64_t)(__ldg(node + __ldg(perm + k0 + q)) / gr.group) * ld + d);
 #pragma unroll
         for (int q = 0; q < kEmbUnroll; ++q)
-          if (k0 + q < e) acc = V::add(acc, x[q]);
+          if (k0 + q < e) acc = V::add(acc, gr.pool_den != 0.f ? V::div(x[q], gr.pool_den) : x[q]);
       }
       V::store(o + d, acc);
     }
@@ -350,10 +448,11 @@ static int id_range_check(eu_ctx* c, const int64_t* ids, int64_t M, int64_t n_ro
   return EU_OK;
 }
 
-// The gradients of the tables T over the nodes [M] (checked by the caller), from grad_out with row stride ld.  Dense
+// The gradients of the tables T over the nodes [M] (checked by the caller), from grad_out with row stride ld, node i's row
+// being row i / gr.group of it (GradRows).  Dense
 // (rows == null): grads[t] f32[n_rows_t, dim_t], zeroed first.  Sparse: the COO rows[t] / grads[t] with counts[t] (host).
 // Table t < S is slot t, table S the id table.
-static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int64_t M, const float* grad_out, int64_t ld,
+static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int64_t M, const float* grad_out, int64_t ld, GradRows gr,
                         float* const* grads, int64_t* const* rows, int64_t* counts, const char* who) {
   EU_CUDA(cudaSetDevice(c->g->device));
   cudaStream_t s = c->stream;
@@ -442,19 +541,21 @@ static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int
     EuProfScope ps(c, "emb_bwd_sums", E_t[t]);
     const float* gs = grad_out + T.col[t];
     int64_t gld = ld;
-    if (t < S && T.comb[t] != EU_COMBINE_SUM) {
+    GradRows tr = gr;
+    if (t < S && T.comb[t] != EU_COMBINE_SUM) {   // a row per node, the pool's division done
       float* scaled = (float*)(m + o_gs);
-      k_emb_scale_grad<<<stride_grid(M * dim), 256, 0, s>>>(gs, ld, ptr + t * (M + 1), M, dim, T.comb[t], scaled);
+      k_emb_scale_grad<<<stride_grid(M * dim), 256, 0, s>>>(gs, ld, gr, ptr + t * (M + 1), M, dim, T.comb[t], scaled);
       EU_LAUNCHED();
       gs = scaled;
       gld = dim;
+      tr = GradRows();
     }
     float* out = grads[t];
     const bool vec = dim % 4 == 0 && gld % 4 == 0 && aligned16(gs) && aligned16(out);
     const int G = group_lanes(ceil_div(dim, vec ? 4 : 1));
     const unsigned blocks = stride_grid((E_t[t] + E_t[t] / kSegChunk + 1) * G);   // >= one group per chunk, up to the grid cap
-    if (vec) k_emb_bwd_chunks<true><<<blocks, 256, 0, s>>>(gs, gld, node + base[t], ord.perm, P, dim, G, !sparse, out);
-    else k_emb_bwd_chunks<false><<<blocks, 256, 0, s>>>(gs, gld, node + base[t], ord.perm, P, dim, G, !sparse, out);
+    if (vec) k_emb_bwd_chunks<true><<<blocks, 256, 0, s>>>(gs, gld, tr, node + base[t], ord.perm, P, dim, G, !sparse, out);
+    else k_emb_bwd_chunks<false><<<blocks, 256, 0, s>>>(gs, gld, tr, node + base[t], ord.perm, P, dim, G, !sparse, out);
     EU_LAUNCHED();
     k_row_combine<<<stride_grid(E_t[t] * dim), 256, 0, s>>>(P, dim, !sparse, out, sparse ? rows[t] : nullptr);
     EU_LAUNCHED();
@@ -480,7 +581,7 @@ static int single_backward(eu_ctx* c, const float* grad_out, const int64_t* node
   T.dim[0] = dim;
   float* g[1] = {out};
   int64_t* r[1] = {rows};
-  return emb_backward(c, T, nodes, M, grad_out, dim, g, rows ? r : nullptr, n, who);
+  return emb_backward(c, T, nodes, M, grad_out, dim, GradRows(), g, rows ? r : nullptr, n, who);
 }
 
 // The checks of a shallow problem, and its device form (out / dense_out filled in by the caller).  *T: its backward tables.
@@ -563,6 +664,92 @@ static int shallow_resolve(eu_ctx* c, const eu_shallow_problem* p, ShallowDev* d
   return EU_OK;
 }
 
+// The pooled op's own checks, after shallow_resolve's; *gr: how its backward reads grad_out f32[M / count, W]
+static int pool_check(const eu_shallow_problem* p, int32_t count, int32_t pool, GradRows* gr, const char* who) {
+  if (count < 1 || p->M % count || (pool != EU_POOL_SUM && pool != EU_POOL_MEAN)) {
+    set_error("%s: count = %d must be at least 1 and divide M = %lld, pool must be EU_POOL_SUM or EU_POOL_MEAN", who, (int)count,
+              (long long)p->M);
+    return EU_ERR_INVALID;
+  }
+  if (p->combiner != EU_SHALLOW_CONCAT) {
+    set_error("%s: only EU_SHALLOW_CONCAT rows are pooled", who);
+    return EU_ERR_UNSUPPORTED;
+  }
+  if (count > EU_SHALLOW_POOL_MAX_COUNT) {
+    set_error("%s: segments of more than %d nodes are not supported", who, EU_SHALLOW_POOL_MAX_COUNT);
+    return EU_ERR_UNSUPPORTED;
+  }
+  gr->group = count;
+  gr->pool_den = pool == EU_POOL_MEAN ? (float)count : 0.f;
+  return EU_OK;
+}
+
+// outside capture: every id must index the id table before anything is written
+static int shallow_id_check(eu_ctx* c, const eu_shallow_problem* p, const char* who) {
+  if (!p->id_table) return EU_OK;
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  EU_CUDA(cudaStreamIsCapturing(c->stream, &st));
+  if (st != cudaStreamCaptureStatusNone) return EU_OK;
+  bool bad = false;
+  int rc = id_range_check(c, p->nodes, p->M, p->n_id_rows, &bad);
+  if (rc) return rc;
+  if (bad) {
+    set_error("%s: a node id lies outside the id table's rows [0, %lld)", who, (long long)p->n_id_rows);
+    return EU_ERR_INVALID;
+  }
+  return EU_OK;
+}
+
+// the lane group of a row whose widest part has `widest` columns, and the slots that take float4 loads and stores
+static int shallow_lanes(ShallowDev* d, const float* out) {
+  int widest = d->id_dim;
+  for (int j = 0; j < d->n_dense; ++j) widest = std::max(widest, d->dense_dim[j]);
+  for (int k = 0; k < d->n_sparse; ++k) {
+    widest = std::max(widest, d->sp_dim[k]);
+    if (d->sp_dim[k] % 4 == 0 && aligned16(d->sp_table[k]) && aligned16(out) && d->W % 4 == 0 && d->sp_off[k] % 4 == 0) d->vec_mask |= 1u << k;
+  }
+  return group_lanes(ceil_div(widest, 4));
+}
+
+// eu_shallow_encode_backward and its pooled form (gr)
+static int shallow_backward(eu_ctx* c, const eu_shallow_problem* p, const ShallowDev& d, const EmbTables& T, GradRows gr,
+                            const float* grad_out, float* const* grads, const char* who) {
+  const int NT = T.S + (T.has_id ? 1 : 0);
+  bool ok = grads && (p->M == 0 || d.W == 0 || grad_out);
+  for (int t = 0; ok && t < NT; ++t) ok = grads[t == T.S ? 0 : t + 1] != nullptr;
+  if (!ok) {
+    set_error("%s: bad argument (grad_out and a gradient per table are required)", who);
+    return EU_ERR_INVALID;
+  }
+  float* g[EU_SHALLOW_MAX_SLOTS + 1];   // the ABI's order (id, slots) to the backward's (slots, id)
+  for (int t = 0; t < NT; ++t) g[t] = grads[t == T.S ? 0 : t + 1];
+  return emb_backward(c, T, p->nodes, p->M, grad_out, d.W, gr, g, nullptr, nullptr, who);
+}
+
+// eu_shallow_encode_backward_sparse and its pooled form (gr)
+static int shallow_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const ShallowDev& d, const EmbTables& T, GradRows gr,
+                                   const float* grad_out, int64_t* const* rows, float* const* values, int64_t* counts, const char* who) {
+  const int NT = T.S + (T.has_id ? 1 : 0);
+  bool ok = rows && values && counts && (p->M == 0 || d.W == 0 || grad_out);
+  for (int t = 0; ok && t < NT && p->M > 0; ++t) ok = rows[t == T.S ? 0 : t + 1] && values[t == T.S ? 0 : t + 1];
+  if (!ok) {
+    set_error("%s: bad argument (grad_out and rows, values and counts per table are required)", who);
+    return EU_ERR_INVALID;
+  }
+  float* v[EU_SHALLOW_MAX_SLOTS + 1];
+  int64_t* r[EU_SHALLOW_MAX_SLOTS + 1];
+  int64_t n[EU_SHALLOW_MAX_SLOTS + 1] = {};
+  for (int t = 0; t < NT; ++t) {
+    v[t] = values[t == T.S ? 0 : t + 1];
+    r[t] = rows[t == T.S ? 0 : t + 1];
+  }
+  int rc = emb_backward(c, T, p->nodes, p->M, grad_out, d.W, gr, v, r, n, who);
+  if (rc) return rc;
+  for (int t = 0; t < NT; ++t) counts[t == T.S ? 0 : t + 1] = n[t];
+  if (!T.has_id) counts[0] = 0;
+  return EU_OK;
+}
+
 }  // namespace eu
 
 using namespace eu;
@@ -617,27 +804,10 @@ int eu_shallow_encode(eu_ctx* c, const eu_shallow_problem* p, float* out, float*
   }
   EU_CUDA(cudaSetDevice(c->g->device));
   if (p->M == 0 || (d.W == 0 && d.dense_w == 0)) return EU_OK;
-  if (p->id_table) {   // outside capture: every id must index the table before anything is written
-    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
-    EU_CUDA(cudaStreamIsCapturing(c->stream, &st));
-    if (st == cudaStreamCaptureStatusNone) {
-      bool bad = false;
-      if ((rc = id_range_check(c, p->nodes, p->M, p->n_id_rows, &bad))) return rc;
-      if (bad) {
-        set_error("%s: a node id lies outside the id table's rows [0, %lld)", who, (long long)p->n_id_rows);
-        return EU_ERR_INVALID;
-      }
-    }
-  }
+  if ((rc = shallow_id_check(c, p, who))) return rc;
   d.out = out;
   d.dense_out = dense_out;
-  int widest = d.id_dim;
-  for (int j = 0; j < d.n_dense; ++j) widest = std::max(widest, d.dense_dim[j]);
-  for (int k = 0; k < d.n_sparse; ++k) {
-    widest = std::max(widest, d.sp_dim[k]);
-    if (d.sp_dim[k] % 4 == 0 && aligned16(d.sp_table[k]) && aligned16(out) && d.W % 4 == 0 && d.sp_off[k] % 4 == 0) d.vec_mask |= 1u << k;
-  }
-  const int G = group_lanes(ceil_div(widest, 4));
+  const int G = shallow_lanes(&d, out);
   EuProfScope ps(c, "shallow_fwd", p->M);
   k_shallow_fwd<<<(unsigned)ceil_div(p->M * G, 256), 256, 0, c->stream>>>(c->g->d, d, G);
   EU_LAUNCHED();
@@ -650,16 +820,7 @@ int eu_shallow_encode_backward(eu_ctx* c, const eu_shallow_problem* p, const flo
   EmbTables T;
   int rc = shallow_resolve(c, p, &d, &T, who);
   if (rc) return rc;
-  const int NT = T.S + (T.has_id ? 1 : 0);
-  bool ok = grads && (p->M == 0 || d.W == 0 || grad_out);
-  for (int t = 0; ok && t < NT; ++t) ok = grads[t == T.S ? 0 : t + 1] != nullptr;
-  if (!ok) {
-    set_error("%s: bad argument (grad_out and a gradient per table are required)", who);
-    return EU_ERR_INVALID;
-  }
-  float* g[EU_SHALLOW_MAX_SLOTS + 1];   // the ABI's order (id, slots) to the backward's (slots, id)
-  for (int t = 0; t < NT; ++t) g[t] = grads[t == T.S ? 0 : t + 1];
-  return emb_backward(c, T, p->nodes, p->M, grad_out, d.W, g, nullptr, nullptr, who);
+  return shallow_backward(c, p, d, T, GradRows(), grad_out, grads, who);
 }
 
 int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, int64_t* const* rows,
@@ -669,24 +830,55 @@ int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, co
   EmbTables T;
   int rc = shallow_resolve(c, p, &d, &T, who);
   if (rc) return rc;
-  const int NT = T.S + (T.has_id ? 1 : 0);
-  bool ok = rows && values && counts && (p->M == 0 || d.W == 0 || grad_out);
-  for (int t = 0; ok && t < NT && p->M > 0; ++t) ok = rows[t == T.S ? 0 : t + 1] && values[t == T.S ? 0 : t + 1];
-  if (!ok) {
-    set_error("%s: bad argument (grad_out and rows, values and counts per table are required)", who);
+  return shallow_backward_sparse(c, p, d, T, GradRows(), grad_out, rows, values, counts, who);
+}
+
+int eu_shallow_encode_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, float* out) {
+  const char* who = "eu_shallow_encode_pool";
+  ShallowDev d;
+  EmbTables T;
+  GradRows gr;
+  int rc = shallow_resolve(c, p, &d, &T, who);
+  if (rc || (rc = pool_check(p, count, pool, &gr, who))) return rc;
+  if (p->M > 0 && d.W > 0 && !out) {
+    set_error("%s: bad argument (out is required)", who);
     return EU_ERR_INVALID;
   }
-  float* v[EU_SHALLOW_MAX_SLOTS + 1];
-  int64_t* r[EU_SHALLOW_MAX_SLOTS + 1];
-  int64_t n[EU_SHALLOW_MAX_SLOTS + 1] = {};
-  for (int t = 0; t < NT; ++t) {
-    v[t] = values[t == T.S ? 0 : t + 1];
-    r[t] = rows[t == T.S ? 0 : t + 1];
-  }
-  if ((rc = emb_backward(c, T, p->nodes, p->M, grad_out, d.W, v, r, n, who))) return rc;
-  for (int t = 0; t < NT; ++t) counts[t == T.S ? 0 : t + 1] = n[t];
-  if (!T.has_id) counts[0] = 0;
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (p->M == 0 || d.W == 0) return EU_OK;
+  if ((rc = shallow_id_check(c, p, who))) return rc;
+  d.out = out;
+  // the group's graph rows live in shared memory: wider groups until a block's fit in the default 48 KB
+  int G = shallow_lanes(&d, out);
+  while ((256 / G) * (size_t)count * sizeof(int64_t) > 48 * 1024) G *= 2;
+  const int64_t R = p->M / count;
+  EuProfScope ps(c, "shallow_pool", p->M);
+  k_shallow_pool<<<(unsigned)ceil_div(R * G, 256), 256, (256 / G) * (size_t)count * sizeof(int64_t), c->stream>>>(c->g->d, d, count,
+                                                                                                              gr.pool_den, G);
+  EU_LAUNCHED();
   return EU_OK;
+}
+
+int eu_shallow_encode_pool_backward(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, const float* grad_out,
+                                    float* const* grads) {
+  const char* who = "eu_shallow_encode_pool_backward";
+  ShallowDev d;
+  EmbTables T;
+  GradRows gr;
+  int rc = shallow_resolve(c, p, &d, &T, who);
+  if (rc || (rc = pool_check(p, count, pool, &gr, who))) return rc;
+  return shallow_backward(c, p, d, T, gr, grad_out, grads, who);
+}
+
+int eu_shallow_encode_pool_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, const float* grad_out,
+                                           int64_t* const* rows, float* const* values, int64_t* counts) {
+  const char* who = "eu_shallow_encode_pool_backward_sparse";
+  ShallowDev d;
+  EmbTables T;
+  GradRows gr;
+  int rc = shallow_resolve(c, p, &d, &T, who);
+  if (rc || (rc = pool_check(p, count, pool, &gr, who))) return rc;
+  return shallow_backward_sparse(c, p, d, T, gr, grad_out, rows, values, counts, who);
 }
 
 }  // extern "C"

@@ -1,7 +1,8 @@
 """SparseEmbedding (tf_euler/python/utils/layers.py:152-169), the embedding the sparse-feature encoders apply to uint64
 feature slots (ShallowEncoder, encoders.py:151-160; SageEncoderNew, encoders.py:590-612), and ShallowEncoder
 (encoders.py:32-171), the input layer of the node encoders: an id embedding, dense feature slots and sparse-feature
-embeddings, concatenated or added.
+embeddings, concatenated or added.  And SageEncoder / ShuffleSageEncoder (encoders.py:411-541), GraphSAGE over
+sample_fanout's sample tree with that input layer and the aggregators of aggregators.py.
 
 Callers size the table as the encoders do: SparseEmbedding(max_id + 1, dim) for values in [0, max_id] and
 default = max_id + 1 for nodes without values, so the table has max_id + 2 rows and the default row is the last one.
@@ -14,7 +15,7 @@ import functools
 import torch
 import torch.nn.functional as F
 
-from . import ops
+from . import _lib, ops
 from .ops import sparse_feature_embedding
 from .unsupervised import Embedding
 
@@ -58,16 +59,23 @@ class SparseEmbedding(torch.nn.Module):
 
 
 class Dense(torch.nn.Module):
-    """layers.Dense(dim, use_bias=False) (utils/layers.py:70-116) over inputs of in_dim columns: a kernel [in_dim, dim]
-    initialised by tf.uniform_unit_scaling_initializer(factor=0.36), uniform in +-0.36 sqrt(3 / in_dim); x @ kernel."""
+    """layers.Dense(dim, activation=None, use_bias) (utils/layers.py:70-116) over inputs of in_dim columns: a kernel
+    [in_dim, dim] initialised by tf.uniform_unit_scaling_initializer(factor=0.36), uniform in +-0.36 sqrt(3 / in_dim), and
+    with use_bias a bias [dim] initialised to 0.0002; activation(x @ kernel + bias).  use_bias defaults to False here (the
+    encoders' use); upstream's default is True, which the pool aggregators rely on and pass explicitly."""
 
-    def __init__(self, in_dim, dim, device=None):
+    def __init__(self, in_dim, dim, activation=None, use_bias=False, device=None):
         super().__init__()
         bound = 0.36 * (3.0 / max(in_dim, 1)) ** 0.5
         self.kernel = torch.nn.Parameter(torch.empty(in_dim, dim, device=device).uniform_(-bound, bound))
+        self.bias = torch.nn.Parameter(torch.full((dim,), 0.0002, device=device)) if use_bias else None
+        self.activation = activation
 
     def forward(self, x):
-        return x @ self.kernel
+        out = x @ self.kernel
+        if self.bias is not None:
+            out = out + self.bias
+        return self.activation(out) if self.activation else out
 
 
 class ShallowEncoder(torch.nn.Module):
@@ -170,11 +178,27 @@ class ShallowEncoder(torch.nn.Module):
         out = self._fused(nodes) if self.fused else self._composed(nodes)
         return out.reshape(shape + (self.output_dim,))
 
-    def _fused(self, nodes):
+    def _op_inputs(self):
+        """(id_table, dense, sparse) as ops.shallow_encode takes them"""
         id_table = self.embedding.embeddings if self.use_id else None
         dense = list(zip(self.feature_idx, self.feature_dim)) if self.use_feature else []
         sparse = [(name, e.embeddings, dv, e.combiner) for name, e, dv in
                   zip(self.sparse_feature_idx, self.sparse_embeddings, self._default_values())] if self.use_sparse_feature else []
+        return id_table, dense, sparse
+
+    @property
+    def poolable(self):
+        """whether pooled() applies: the row is the fused op's 'concat' row itself, with no Dense layer after it"""
+        return self.fused and self.combiner == 'concat' and not self.dim
+
+    def pooled(self, nodes, count, pool):
+        """the 'sum' or 'mean' of this encoder's rows over consecutive segments of `count` nodes, f32[nodes.numel() / count,
+        output_dim], in one device op that never writes the rows (ops.shallow_encode_pool); needs poolable"""
+        id_table, dense, sparse = self._op_inputs()
+        return ops.shallow_encode_pool(nodes, count, id_table, dense, sparse, pool, self.sparse_grad)
+
+    def _fused(self, nodes):
+        id_table, dense, sparse = self._op_inputs()
         if self.combiner == 'concat':
             emb = ops.shallow_encode(nodes, id_table, dense, sparse, 'concat', self.sparse_grad)
             return self.dense(emb) if self.dim else emb
@@ -200,3 +224,106 @@ class ShallowEncoder(torch.nn.Module):
             return functools.reduce(torch.add, embeddings)
         embedding = torch.cat(embeddings, -1)
         return self.dense(embedding) if self.dim else embedding
+
+
+class SageEncoder(torch.nn.Module):
+    """encoders.SageEncoder (tf_euler/python/utils/encoders.py:411-493): GraphSAGE over the sample tree of
+    sample_fanout(inputs, metapath, fanouts, default_node=max_id + 1), with upstream's constructor arguments, ValueErrors and
+    dims.  The node encoder is ShallowEncoder(feature_idx, feature_dim, max_id if use_id else -1, sparse_feature_idx, ..)
+    with 'concat' and no dim (or shared_node_encoder), the aggregators aggregators.get(aggregator)(dim, relu on all but the last
+    layer, concat=concat) (or shared_aggregators).  use_feature is deprecated upstream and has no effect; use_residual is
+    ignored, as upstream's SageEncoder ignores it.  __call__(inputs) returns inputs.shape + (dim,).
+
+    fused=True (the default): the deepest hop, which only ever reaches layer 0's aggregator as the neighbours of hop L - 1, is
+    not encoded row by row when that aggregator is linear in its neighbours ('mean', 'gcn': it has forward_pooled) and the
+    node encoder can pool (ShallowEncoder.poolable, and a fanout within the op's bound): the aggregator then receives
+    ops.shallow_encode_pool's [n, W] rows and the [n * fanout, W] matrix is never written, forward or backward.  Every other
+    combination takes the composition.  fused=False is the literal composition everywhere: the node encoder's composed path
+    per hop, then upstream's layer / hop loop.  sparse_grad=True gives the node encoder's tables sparse COO gradients."""
+
+    @staticmethod
+    def create_aggregators(in_dim, dim, num_layers, aggregator, **kwargs):
+        """upstream's create_aggregators, with the input width of layer 0 (every later layer reads dim columns)"""
+        from . import aggregators
+        aggregator_class = aggregators.get(aggregator)
+        return torch.nn.ModuleList([
+            aggregator_class(in_dim if layer == 0 else dim, dim, activation=torch.relu if layer < num_layers - 1 else None, **kwargs)
+            for layer in range(num_layers)])
+
+    def __init__(self, metapath, fanouts, dim, aggregator='mean', concat=False, shared_aggregators=None, feature_idx=-1,
+                 feature_dim=0, max_id=-1, use_feature=None, use_id=None, sparse_feature_idx=-1, sparse_feature_max_id=-1,
+                 embedding_dim=16, use_hash_embedding=False, use_residual=False, shared_node_encoder=None, fused=True,
+                 sparse_grad=False, device=None):
+        super().__init__()
+        if len(metapath) != len(fanouts):
+            raise ValueError('Len of metapath must be the same as fanouts.')
+        self.metapath = metapath
+        self.fanouts = list(fanouts)
+        self.num_layers = len(metapath)
+        self.concat = concat
+        self.fused = fused
+        if shared_node_encoder:
+            self._node_encoder = shared_node_encoder
+        else:
+            self._node_encoder = ShallowEncoder(
+                feature_idx=feature_idx, feature_dim=feature_dim, max_id=max_id if use_id else -1,
+                sparse_feature_idx=sparse_feature_idx, sparse_feature_max_id=sparse_feature_max_id, embedding_dim=embedding_dim,
+                use_hash_embedding=use_hash_embedding, fused=fused, sparse_grad=sparse_grad, device=device)
+        self.dims = [self._node_encoder.output_dim] + [dim] * self.num_layers
+        if shared_aggregators is not None:
+            self.aggregators = shared_aggregators
+        else:
+            self.aggregators = self.create_aggregators(self.dims[0], dim, self.num_layers, aggregator, concat=concat, device=device)
+        self._max_id = max_id
+
+    def node_encoder(self, inputs):
+        return self._node_encoder(inputs)
+
+    def _pools_deepest_hop(self):
+        fanout = self.fanouts[-1]
+        return (self.fused and hasattr(self.aggregators[0], 'forward_pooled') and getattr(self._node_encoder, 'poolable', False)
+                and 1 <= fanout <= _lib.SHALLOW_POOL_MAX_COUNT)
+
+    def sample(self, inputs):
+        return ops.sample_fanout(inputs, self.metapath, self.fanouts, default_node=self._max_id + 1)[0]
+
+    def agg(self, inputs, samples):
+        """upstream's layer / hop loop over the ids of the sample tree (samples[hop], flat)"""
+        L = self.num_layers
+        pooled = None
+        if self._pools_deepest_hop():
+            pooled = self._node_encoder.pooled(samples[L], self.fanouts[-1], self.aggregators[0].pooled_input)
+        hidden = [self.node_encoder(sample) for sample in (samples[:L] if pooled is not None else samples)]
+        for layer in range(L):
+            aggregator = self.aggregators[layer]
+            next_hidden = []
+            for hop in range(L - layer):
+                if layer == 0 and hop == L - 1 and pooled is not None:
+                    h = aggregator.forward_pooled(hidden[hop], pooled, self.fanouts[hop])
+                else:
+                    h = aggregator((hidden[hop], hidden[hop + 1].reshape(-1, self.fanouts[hop], self.dims[layer])))
+                next_hidden.append(h)
+            hidden = next_hidden
+        return hidden[0].reshape(tuple(inputs.shape) + (self.dims[-1],))
+
+    def forward(self, inputs):
+        return self.agg(inputs, self.sample(inputs))
+
+
+class ShuffleSageEncoder(SageEncoder):
+    """encoders.ShuffleSageEncoder (encoders.py:496-541), DGI's encoder: returns [h, h_neg], h_neg aggregated over the same
+    sample tree with its rows shuffled.  Upstream's shuffle_tensors lays the encoded rows out as [batch, tree position, dim]
+    (the 1 + f1 + f1 f2 + .. positions of each seed's tree), permutes the positions by one permutation for the whole batch,
+    flattens and splits by the hops' sizes.  The node encoder is row-wise, so that equals encoding the sample ids moved the
+    same way (shuffle_samples), which keeps the deepest hop of the negative pass on the pooled op.  forward takes the
+    torch.Generator of the permutation."""
+
+    def shuffle_samples(self, samples, generator=None):
+        batch = samples[0].numel()
+        tree = torch.cat([s.reshape(batch, -1) for s in samples], 1)
+        perm = torch.randperm(tree.shape[1], generator=generator).to(tree.device)
+        return list(torch.split(tree[:, perm].reshape(-1), [s.numel() for s in samples]))
+
+    def forward(self, inputs, generator=None):
+        samples = self.sample(inputs)
+        return [self.agg(inputs, samples), self.agg(inputs, self.shuffle_samples(samples, generator))]

@@ -1110,6 +1110,55 @@ def _shallow_problem(nodes, id_table, dense, sparse, comb):
     return p
 
 
+def _shallow_inputs(who, nodes, id_table, dense, sparse, comb, sparse_grad):
+    """shallow_encode's arguments checked and resolved: (nodes i64[M], _ShallowEncode's cfg, the id table, the slots' tables)"""
+    g = get_graph()
+    dense, sparse = list(dense), list(sparse)
+    if len(dense) > _lib.SHALLOW_MAX_SLOTS or len(sparse) > _lib.SHALLOW_MAX_SLOTS:
+        raise EulerError("%s: at most %d dense and %d sparse slots" % (who, _lib.SHALLOW_MAX_SLOTS, _lib.SHALLOW_MAX_SLOTS))
+    tables = ([id_table] if id_table is not None else []) + [s[1] for s in sparse]
+    named = [("sparse table %d" % k, s[1]) for k, s in enumerate(sparse)]
+    _check_f32(who, ([("id_table", id_table)] if id_table is not None else []) + named, 2)
+    d_cfg = tuple((_slot(n, g.dense_feature_id), int(d)) for n, d in dense)
+    s_cfg = []
+    for s in sparse:
+        name, _, dv = s[:3]
+        c = s[3] if len(s) > 3 else 'sum'
+        if c not in _COMBINERS:
+            raise EulerError("%s: sparse combiner must be one of %s, got %r" % (who, sorted(_COMBINERS), c))
+        s_cfg.append((_slot(name, g.sparse_feature_id), int(dv), _COMBINERS[c]))
+    emb_dims = [t.shape[1] for t in tables]
+    if comb == 1 and len(set(emb_dims)) > 1:
+        raise EulerError("%s: 'add' needs one dim for every table, got %s" % (who, emb_dims))
+    dense_w = sum(d for _, d in d_cfg)
+    W = (emb_dims[0] if emb_dims else 0) if comb == 1 else sum(emb_dims) + dense_w
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    id_t = _t(id_table, torch.float32) if id_table is not None else None
+    ts = [_t(s[1], torch.float32) for s in sparse]
+    return nodes, (d_cfg, tuple(s_cfg), comb, W, dense_w if comb == 1 else 0, bool(sparse_grad)), id_t, ts
+
+
+def _shallow_backward(sym, extra, nodes, cfg, grad, id_table, tables):
+    """the table gradients of a shallow problem through sym (dense) or sym + '_sparse' (cfg's sparse_grad), `extra` being the
+    arguments between the problem and grad_out; in the order (id table, slots), None for an absent id table"""
+    dense, sparse_cfg, comb, W, dense_w, sparse_grad = cfg
+    sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
+    all_tables = [id_table] + list(tables)
+    grad = grad.contiguous()
+    p = _shallow_problem(nodes, id_table, dense, sparse, comb)
+    if not sparse_grad:
+        grads = [None if t is None else torch.empty_like(t) for t in all_tables]
+        _call(sym, C.byref(p), *extra, grad, grads)
+        return tuple(grads)
+    # the id table has M entries, a slot its get_sparse_feature entries
+    entries = [nodes.numel()] + [_sparse_entries(nodes, fid) for fid, _, _, _ in sparse]
+    shapes = [_shape(t) for t in all_tables]
+    bufs = [_coo_buffers(e, sh, nodes.device) for e, sh in zip(entries, shapes)]
+    counts = (C.c_int64 * len(all_tables))()
+    _call(sym + "_sparse", C.byref(p), *extra, grad, [r for r, _ in bufs], [v for _, v in bufs], counts)
+    return tuple(_coo(r, v, counts[t], shapes[t]) for t, (r, v) in enumerate(bufs))
+
+
 class _ShallowEncode(torch.autograd.Function):
     """eu_shallow_encode / eu_shallow_encode_backward(_sparse).  Saves the node ids only (and the tables, which are inputs):
     the backward pass lists every table's entries again from the graph.  Inputs after the configuration: the id table (None
@@ -1134,22 +1183,7 @@ class _ShallowEncode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad, *unused):
         nodes, id_table, *tables = ctx.saved_tensors
-        dense, sparse_cfg, comb, W, dense_w, sparse_grad = ctx.cfg
-        sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
-        all_tables = [id_table] + list(tables)
-        grad = grad.contiguous()
-        p = _shallow_problem(nodes, id_table, dense, sparse, comb)
-        if not sparse_grad:
-            grads = [None if t is None else torch.empty_like(t) for t in all_tables]
-            _call("eu_shallow_encode_backward", C.byref(p), grad, grads)
-            return (None, None) + tuple(grads)
-        # the id table has M entries, a slot its get_sparse_feature entries
-        entries = [nodes.numel()] + [_sparse_entries(nodes, fid) for fid, _, _, _ in sparse]
-        shapes = [_shape(t) for t in all_tables]
-        bufs = [_coo_buffers(e, sh, nodes.device) for e, sh in zip(entries, shapes)]
-        counts = (C.c_int64 * len(all_tables))()
-        _call("eu_shallow_encode_backward_sparse", C.byref(p), grad, [r for r, _ in bufs], [v for _, v in bufs], counts)
-        return (None, None) + tuple(_coo(r, v, counts[t], shapes[t]) for t, (r, v) in enumerate(bufs))
+        return (None, None) + _shallow_backward("eu_shallow_encode_backward", (), nodes, ctx.cfg, grad, id_table, tables)
 
 
 def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat', sparse_grad=False):
@@ -1169,35 +1203,54 @@ def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat',
     if combiner not in SHALLOW_COMBINERS:
         raise EulerError("shallow_encode: combiner must be one of %s, got %r" % (sorted(SHALLOW_COMBINERS), combiner))
     comb = SHALLOW_COMBINERS[combiner]
-    g = get_graph()
-    dense, sparse = list(dense), list(sparse)
-    if len(dense) > _lib.SHALLOW_MAX_SLOTS or len(sparse) > _lib.SHALLOW_MAX_SLOTS:
-        raise EulerError("shallow_encode: at most %d dense and %d sparse slots" % (_lib.SHALLOW_MAX_SLOTS, _lib.SHALLOW_MAX_SLOTS))
-    tables = ([id_table] if id_table is not None else []) + [s[1] for s in sparse]
-    named = [("sparse table %d" % k, s[1]) for k, s in enumerate(sparse)]
-    _check_f32("shallow_encode", ([("id_table", id_table)] if id_table is not None else []) + named, 2)
-    d_cfg = tuple((_slot(n, g.dense_feature_id), int(d)) for n, d in dense)
-    s_cfg = []
-    for s in sparse:
-        name, _, dv = s[:3]
-        c = s[3] if len(s) > 3 else 'sum'
-        if c not in _COMBINERS:
-            raise EulerError("shallow_encode: sparse combiner must be one of %s, got %r" % (sorted(_COMBINERS), c))
-        s_cfg.append((_slot(name, g.sparse_feature_id), int(dv), _COMBINERS[c]))
-    emb_dims = [t.shape[1] for t in tables]
-    if comb == 1 and len(set(emb_dims)) > 1:
-        raise EulerError("shallow_encode: 'add' needs one dim for every table, got %s" % emb_dims)
-    dense_w = sum(d for _, d in d_cfg)
-    W = (emb_dims[0] if emb_dims else 0) if comb == 1 else sum(emb_dims) + dense_w
-    nodes = _t(nodes, torch.int64).reshape(-1)
-    id_t = _t(id_table, torch.float32) if id_table is not None else None
-    ts = [_t(s[1], torch.float32) for s in sparse]
-    cfg = (d_cfg, tuple(s_cfg), comb, W, dense_w if comb == 1 else 0, bool(sparse_grad))
+    nodes, cfg, id_t, ts = _shallow_inputs("shallow_encode", nodes, id_table, dense, sparse, comb, sparse_grad)
+    d_cfg = cfg[0]
     res = _ShallowEncode.apply(nodes, cfg, id_t, *ts)
     if comb == 0:
         return res
     out, feats = res
     return out, (feats if d_cfg else None)
+
+
+POOLS = {'sum': 0, 'mean': 1}
+
+
+class _ShallowEncodePool(torch.autograd.Function):
+    """eu_shallow_encode_pool / eu_shallow_encode_pool_backward(_sparse): _ShallowEncode's inputs ('concat'), with the
+    segment length and the pool code.  Saves the node ids only (and the tables, which are inputs)."""
+
+    @staticmethod
+    def forward(ctx, nodes, cfg, count, pool, id_table, *tables):
+        dense, sparse_cfg, comb, W = cfg[:4]
+        sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
+        out = torch.empty((nodes.numel() // max(count, 1), W), dtype=torch.float32, device=nodes.device)   # count < 1 is refused below
+        p = _shallow_problem(nodes, id_table, dense, sparse, comb)
+        _call("eu_shallow_encode_pool", C.byref(p), count, pool, out)
+        ctx.save_for_backward(nodes, id_table, *tables)
+        ctx.cfg = (cfg, count, pool)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        nodes, id_table, *tables = ctx.saved_tensors
+        cfg, count, pool = ctx.cfg
+        return (None, None, None, None) + _shallow_backward("eu_shallow_encode_pool_backward", (count, pool), nodes, cfg, grad,
+                                                            id_table, tables)
+
+
+def shallow_encode_pool(nodes, count, id_table=None, dense=(), sparse=(), pool='mean', sparse_grad=False):
+    """The 'concat' rows of shallow_encode pooled over consecutive segments of `count` nodes, in one fused device op: what
+    SageEncoder's first layer needs of the deepest hop of sample_fanout (count = the last fanout).  nodes (any shape, M =
+    R * count ids when flattened), id_table, dense and sparse are shallow_encode's; returns f32[R, W], row r the 'sum' or
+    'mean' of the rows shallow_encode(nodes)[r * count : (r + 1) * count], every node counted (absent ones and default_node
+    too, as reduce_mean(axis=1) counts them).  The [M, W] matrix is never written, in either direction.  Fixed order
+    (include/euler_b200.h): each column is added left to right from the segment's first row, mean divides once by count.
+    Gradients reach the tables only, as shallow_encode's (dense, or coalesced sparse COO with sparse_grad=True), with the
+    same synchronisations.  count is at least 1, divides M and is at most 512 (EU_SHALLOW_POOL_MAX_COUNT)."""
+    if pool not in POOLS:
+        raise EulerError("shallow_encode_pool: pool must be one of %s, got %r" % (sorted(POOLS), pool))
+    nodes, cfg, id_t, ts = _shallow_inputs("shallow_encode_pool", nodes, id_table, dense, sparse, 0, sparse_grad)
+    return _ShallowEncodePool.apply(nodes, cfg, int(count), POOLS[pool], id_t, *ts)
 
 
 # ------------------------------------------------------------------------------------ graph-level minibatches

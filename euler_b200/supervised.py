@@ -1,0 +1,49 @@
+"""SuperviseModel (tf_euler/python/mp_utils/base.py:24-47): the supervised training step over any node encoder, and f1_score
+(tf_euler/python/utils/metrics.py:35-48)."""
+import torch
+import torch.nn.functional as F
+
+from . import ops
+
+
+def f1_score(labels, predict):
+    """metrics.f1_score for one batch: predictions = floor(predict + 0.5), true / false positives and false negatives counted
+    over every element, precision = tp / (1e-7 + tp + fp), recall = tp / (1e-7 + tp + fn),
+    f1 = 2 precision recall / (precision + recall + 1e-7).  Upstream's metric is streaming (tf.metrics accumulates the counts
+    over the session's batches); this one is the batch's own value."""
+    predictions = torch.floor(predict + 0.5) != 0
+    labels = labels != 0
+    epsilon = 1e-7
+    tp = (labels & predictions).sum().to(torch.float32)
+    fn = (labels & ~predictions).sum().to(torch.float32)
+    fp = (~labels & predictions).sum().to(torch.float32)
+    precision = tp / (epsilon + tp + fp)
+    recall = tp / (epsilon + tp + fn)
+    return 2.0 * precision * recall / (precision + recall + epsilon)
+
+
+class SuperviseModel(torch.nn.Module):
+    """SuperviseModel(label_idx, label_dim, metric_name='f1'): __call__(inputs) reads the label slot
+    (get_dense_feature(inputs, [label_idx], [label_dim])), embeds the nodes (embed, the subclass's encoder), maps the
+    embedding through a bias-free out_fc (tf.layers.Dense: glorot-uniform kernel) and returns
+    (embedding, mean sigmoid cross entropy, metric_name, metric of (label, sigmoid(logit))).  dim is the width of embed's
+    rows, which torch needs to build out_fc.  Only 'f1' is provided; see f1_score for how it differs from upstream's."""
+
+    def __init__(self, label_idx, label_dim, metric_name='f1', *, dim, device=None):
+        super().__init__()
+        if metric_name != 'f1':
+            raise ValueError("metric_name must be 'f1', got %r" % (metric_name,))
+        self.label_idx, self.label_dim, self.metric_name = label_idx, label_dim, metric_name
+        self.out_fc = torch.nn.Linear(dim, label_dim, bias=False, device=device)
+        torch.nn.init.xavier_uniform_(self.out_fc.weight)
+
+    def embed(self, n_id):
+        raise NotImplementedError
+
+    def forward(self, inputs):
+        label, = ops.get_dense_feature(inputs, [self.label_idx], [self.label_dim])
+        embedding = self.embed(inputs)
+        logit = self.out_fc(embedding)
+        metric = f1_score(label, torch.sigmoid(logit.detach()))
+        loss = F.binary_cross_entropy_with_logits(logit, label.reshape(logit.shape))
+        return embedding, loss, self.metric_name, metric

@@ -10,8 +10,11 @@ fused op is measured and tested against.
 
 The encoders here are id tables, ShallowEncoder(max_id=max_id) with ids only: layers.Embedding(max_id + 1, dim), a table of
 max_id + 2 rows, so the default node max_id + 1 that random_walk and sample_neighbor pad with is a row of its own.
-ShallowEncoder's feature inputs (dense features, sparse-feature embeddings) and the unsupervised GraphSage / GCN encoders are
-not provided by this module.  Upstream's neg_condition (sample_node with an index query) is not supported.
+Upstream's neg_condition (sample_node with an index query) is not supported.
+
+DGI (examples/dgi/dgi.py) is the one model here over a GraphSAGE encoder: encoders.ShuffleSageEncoder with ShallowEncoder's
+feature inputs, a bilinear decoder against the batch's readout, and the same rank metrics (composed_metric).  The
+unsupervised GraphSage / GCN models are not provided by this module.
 """
 import torch
 import torch.nn.functional as F
@@ -165,3 +168,51 @@ class Line(UnsuperviseModel):
         super().__init__(node_type, edge_type, max_id, dim, num_negs=num_negs, metric_name=metric_name,
                          share_context=order == 'first', **kwargs)
         self.order = order
+
+
+class DGI(torch.nn.Module):
+    """DGI (examples/dgi/dgi.py:24-90), upstream's arguments: the target encoder is ShuffleSageEncoder(metapath, fanouts, dim,
+    aggregator, concat, ..), which embeds the batch over its sample tree and over the tree with shuffled rows (the negatives).
+    decoder scores kernel(embedding) and kernel(embedding_negs) (a bias-free Dense(dim)) against the readout, the sigmoid of
+    the batch's mean embedding, with sigmoid cross entropy (ones for the true rows, zeros for the shuffled ones) and
+    composed_metric for the rank metric.  __call__(inputs, generator=None) returns upstream's
+    (embedding, loss, metric_name, metric), the embedding from a second pass of the encoder with fresh samples, as upstream;
+    generator fixes the shuffles.  num_negs is kept and unused, as upstream.  fused / sparse_grad are SageEncoder's."""
+
+    def __init__(self, node_type, edge_type, max_id, metapath, fanouts, dim, aggregator='mean', concat=False, feature_idx=-1,
+                 feature_dim=0, use_feature=None, use_id=False, sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16,
+                 use_hash_embedding=False, use_residual=False, num_negs=5, metric='mrr', fused=True, sparse_grad=False, device=None):
+        super().__init__()
+        from .encoders import Dense, ShuffleSageEncoder   # encoders builds on Embedding above
+        if metric not in SKIPGRAM_METRICS:
+            raise ValueError("metric must be one of %s, got %r" % (SKIPGRAM_METRICS, metric))
+        self.node_type, self.edge_type, self.max_id = node_type, edge_type, max_id
+        self.num_negs, self.dim, self.metric_name = num_negs, dim, metric
+        self.kernel = Dense(dim, dim, device=device)
+        self._target_encoder = ShuffleSageEncoder(
+            metapath, fanouts, dim, aggregator, concat, feature_idx=feature_idx, feature_dim=feature_dim, max_id=max_id,
+            use_id=use_id, sparse_feature_idx=sparse_feature_idx, sparse_feature_max_id=sparse_feature_max_id,
+            embedding_dim=embedding_dim, use_hash_embedding=use_hash_embedding, use_residual=use_residual, fused=fused,
+            sparse_grad=sparse_grad, device=device)
+
+    def target_encoder(self, inputs, generator=None):
+        return self._target_encoder(inputs, generator)
+
+    def readout_func(self, inputs):
+        return torch.sigmoid(inputs.mean(0, keepdim=True)).expand(inputs.shape[0], -1, -1)
+
+    def decoder(self, embedding, embedding_pos, embedding_negs):
+        logits = torch.matmul(self.kernel(embedding), embedding_pos.transpose(1, 2))
+        neg_logits = torch.matmul(self.kernel(embedding_negs), embedding_pos.transpose(1, 2))
+        metric = composed_metric(logits.detach(), neg_logits.detach(), self.metric_name)
+        true_xent = F.binary_cross_entropy_with_logits(logits, torch.ones_like(logits), reduction='none')
+        negative_xent = F.binary_cross_entropy_with_logits(neg_logits, torch.zeros_like(neg_logits), reduction='none')
+        loss = torch.cat([true_xent.reshape(-1, 1), negative_xent.reshape(-1, 1)], 0).mean()
+        return loss, metric
+
+    def forward(self, inputs, generator=None):
+        src = inputs.unsqueeze(-1)
+        embedding, embedding_negs = self.target_encoder(src, generator)
+        loss, metric = self.decoder(embedding, self.readout_func(embedding), embedding_negs)
+        embedding = self.target_encoder(inputs, generator)[0]
+        return embedding, loss, self.metric_name, metric

@@ -369,6 +369,32 @@ int eu_shallow_encode_backward(eu_ctx* c, const eu_shallow_problem* p, const flo
 int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, int64_t* const* rows,
                                       float* const* values, int64_t* counts);
 
+/* ShallowEncoder's rows pooled over fixed segments: what SageEncoder's first layer needs of the deepest hop of a fanout
+ * (tf_euler/python/utils/encoders.py:475-491: the hop's rows reshaped to [R, count, W] reach the mean / gcn aggregator only
+ * through a reduction over the count axis).  p is an EU_SHALLOW_CONCAT problem with M = R * count nodes; row r of
+ * out f32[R, W] pools the count rows eu_shallow_encode would write for nodes[r * count .. r * count + count - 1], every one
+ * of them by eu_shallow_encode's rules (an absent node, sample_fanout's default_node, an empty bag: rows like any other, and
+ * they count in the divisor, as tf.reduce_mean(axis=1) counts them).  The [M, W] matrix is never written.
+ * Fixed order, per column: acc = row_0's value; acc = __fadd_rn(acc, row_j's value) for j = 1 .. count - 1, where a sparse
+ * slot's value is the bag sum after its combiner's division, as eu_sparse_embedding_lookup rounds it.  EU_POOL_SUM: out = acc.
+ * EU_POOL_MEAN: out = __fdiv_rn(acc, fl(count)).  The bits do not depend on the alignment of the tables or of out.
+ * One lane group per output row looks each node's graph row up once (shared memory) and sums a tile of columns in registers.
+ * No scratch, no synchronisation while the stream is being captured; outside capture the id check of eu_shallow_encode.
+ * Backward: grad_out f32[R, W]; the gradient row of node k is grad_out[k / count], for EU_POOL_MEAN with every element
+ * divided by fl(count) as it is read (one __fdiv_rn, before a mean / sqrtn slot's own division by its bag's divisor, which
+ * is a second __fdiv_rn exactly as autograd through eu_shallow_encode and a mean over the segment would do).  Everything else
+ * is eu_shallow_encode_backward(_sparse): the same entries, order, chunks, outputs, synchronisations and scratch (the M dim
+ * floats of a mean / sqrtn slot included; no [M, W] gradient exists anywhere).
+ * Bounds: eu_shallow_encode's, and count at most EU_SHALLOW_POOL_MAX_COUNT; EU_SHALLOW_ADD is EU_ERR_UNSUPPORTED.  count < 1,
+ * M % count != 0 or a pool outside the enum: EU_ERR_INVALID.  Device pointers. */
+#define EU_SHALLOW_POOL_MAX_COUNT 512
+enum { EU_POOL_SUM = 0, EU_POOL_MEAN = 1 };
+int eu_shallow_encode_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, float* out);
+int eu_shallow_encode_pool_backward(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, const float* grad_out,
+                                    float* const* grads);
+int eu_shallow_encode_pool_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool,
+                                           const float* grad_out, int64_t* const* rows, float* const* values, int64_t* counts);
+
 /* Graph-level minibatches (graph classification; reference: euler/core/kernels/sample_graph_label_op.cc,
  * get_graph_by_label_op.cc and Graph::GetGraphLabel, euler/core/graph/graph.cc:439-457).
  * A graph's label table is built on the first graph-label call from its binary feature slot named "graph_label" (the
