@@ -22,10 +22,12 @@
 //
 // Backward, grad_table[v] = sum over the entries (i, k) with v_k = v of s_i(g_i), where s_i is the identity (sum),
 // __fdiv_rn(., fl(n_i)) (mean) or __fdiv_rn(., __fsqrt_rn(fl(n_i))) (sqrtn), elementwise.  The entries of every table are
-// listed again from the graph in one pass over the nodes, ordered stably by value (order_by) and summed per distinct value in
-// fixed chunks of kSegChunk entries (plan_distinct, segment.cuh): deterministic, no atomics, and a hot value (the default
-// fills every empty slot) is spread over many CTAs.  The sums go to a dense table (rows no entry touches are zero) or to a
-// coalesced COO of the rows touched.
+// listed again from the graph in one pass over the nodes (k_emb_entries: each entry's value and node), then go through the
+// id-table gradient path of segment.cuh that the skip-gram and KG losses share: ordered stably by value and planned
+// (plan_rows), summed per distinct value in fixed chunks of kSegChunk entries (sum_distinct_rows, reading each entry's
+// gradient row in place, row node / group of grad_out): deterministic, no atomics, and a hot value (the default fills every
+// empty slot) is spread over many CTAs.  The sums go to a dense table (rows no entry touches are zero) or to a coalesced COO
+// of the rows touched.
 #include <cub/device/device_scan.cuh>
 
 #include "segment.cuh"
@@ -366,43 +368,6 @@ __global__ void k_emb_scale_grad(const float* __restrict__ g, int64_t ld, GradRo
   }
 }
 
-// G lanes per chunk c of the distinct-value segments (grid-stride over the chunks, whose number is on the device).  Chunk
-// c - chunk_off[p] of segment p covers the sorted positions [start[p] + (c - chunk_off[p]) * kSegChunk, ...), up to kSegChunk
-// of them: the sum, left to right from +0, of the (scaled) gradient rows gs[(node / group) * ld] of their nodes, each divided
-// by pool_den first when that is not 0 (GradRows).  A segment of one chunk
-// writes its output row (by_key: the table row key[p]; else row p of the COO values); the chunks of a longer one write their
-// partial rows for k_row_combine.
-template <bool VEC>
-__global__ void __launch_bounds__(256, 1) k_emb_bwd_chunks(const float* __restrict__ gs, int64_t ld, GradRows gr, const int32_t* __restrict__ node,
-                                                        const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G, bool by_key,
-                                                        float* __restrict__ out) {
-  using V = EmbVec<VEC>;
-  const int lg = 31 - __clz(G);
-  const int sub = (int)(threadIdx.x & (G - 1));
-  const int64_t nch_all = __ldg(P.chunk_off + P.E);
-  const int64_t step = ((int64_t)gridDim.x * blockDim.x) >> lg;
-  for (int64_t c = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> lg; c < nch_all; c += step) {
-    const int64_t p = key_upper_bound(P.chunk_off, P.E + 1, c) - 1;
-    const int64_t c0 = __ldg(P.chunk_off + p), nch = __ldg(P.chunk_off + p + 1) - c0;
-    const int64_t b = __ldg(P.start + p) + (c - c0) * kSegChunk;
-    const int64_t e = min(b + kSegChunk, (int64_t)__ldg(P.start + p + 1));
-    float* o = nch == 1 ? out + (by_key ? (int64_t)__ldg(P.key + p) : p) * dim : P.partial + (int64_t)(__ldg(P.part_off + p) + (c - c0)) * dim;
-    for (int d = sub * V::W; d < dim; d += G * V::W) {
-      typename V::T acc = V::zero(0.f);
-      for (int64_t k0 = b; k0 < e; k0 += kEmbUnroll) {
-        typename V::T x[kEmbUnroll];
-#pragma unroll
-        for (int q = 0; q < kEmbUnroll; ++q)
-          if (k0 + q < e) x[q] = V::load(gs + (int64_t)(__ldg(node + __ldg(perm + k0 + q)) / gr.group) * ld + d);
-#pragma unroll
-        for (int q = 0; q < kEmbUnroll; ++q)
-          if (k0 + q < e) acc = V::add(acc, gr.pool_den != 0.f ? V::div(x[q], gr.pool_den) : x[q]);
-      }
-      V::store(o + d, acc);
-    }
-  }
-}
-
 // The checks of one uint64 slot and its table.  Every value of slot fid and the default must index the table: the slot's
 // largest value is kept on the graph, so this costs no device work.
 static int emb_slot_check(const eu_graph* g, int32_t fid, int64_t default_value, int64_t n_rows, const char* who) {
@@ -502,7 +467,7 @@ static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int
   for (int k = 0; k < S; ++k) { base[k] = k ? h_end[k - 1] : 0; E_t[k] = h_end[k] - base[k]; }
   const int64_t E = (S ? h_end[S - 1] : 0) + (T.has_id ? M : 0);
   if (T.has_id) { base[S] = E - M; E_t[S] = M; }
-  if (E + E / kSegChunk + 1 >= ((int64_t)1 << 31)) {
+  if (!entries_fit(E)) {
     set_error("%s: 2^31 or more entries are not supported", who);
     return EU_ERR_UNSUPPORTED;
   }
@@ -510,7 +475,7 @@ static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int
   size_t region = 0;
   for (int t = 0; t < NT; ++t) {
     if (t < S && T.comb[t] != EU_COMBINE_SUM) scaled_dim = std::max(scaled_dim, T.dim[t]);
-    region = std::max(region, order_bytes(E_t[t], T.n_rows[t]) + distinct_plan_bytes(E_t[t], T.dim[t]));
+    region = std::max(region, row_plan_bytes(E_t[t], T.n_rows[t], T.dim[t]));
   }
   const size_t o_node = o_key + a256(4 * (size_t)E), o_gs = o_node + a256(4 * (size_t)E), o_reg = o_gs + a256(4 * (size_t)M * scaled_dim);
   const size_t total = o_reg + region;
@@ -519,7 +484,7 @@ static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int
     if ((rc = entry_ptr())) return rc;
   }
   char* m = (char*)c->d_misc;
-  int32_t* nd_copy = (int32_t*)(m + 64);
+  int32_t* hdr = (int32_t*)m;   // read_back's header: the (spent) flag, then each table's distinct count
   const int64_t* ptr = (const int64_t*)(m + o_ptr);
   int32_t* key = (int32_t*)(m + o_key);
   int32_t* node = (int32_t*)(m + o_node);
@@ -529,44 +494,39 @@ static int emb_backward(eu_ctx* c, const EmbTables& T, const int64_t* nodes, int
                                                       key, node);
     EU_LAUNCHED();
   }
+  const int32_t* nd[kReadBackMax];   // each table's count, copied to its header slot before the plan's scratch is reused
   for (int t = 0; t < NT; ++t) {
     const int dim = T.dim[t];
-    EdgeOrder ord;
-    DistinctPlan P;
+    RowList L;
+    L.E = E_t[t];
+    L.n_rows = T.n_rows[t];
+    L.key = key + base[t];
     {
-      EuProfScope ps(c, "emb_bwd_order", E_t[t]);
-      if ((rc = order_by(c, key + base[t], E_t[t], T.n_rows[t], m + o_reg, &ord))) return rc;
-      if ((rc = plan_distinct(c, ord, E_t[t], m + o_reg + order_bytes(E_t[t], T.n_rows[t]), &P))) return rc;
+      EuProfScope ps(c, "emb_bwd_order", L.E);
+      if ((rc = plan_rows(c, m + o_reg, &L))) return rc;
     }
-    EuProfScope ps(c, "emb_bwd_sums", E_t[t]);
-    const float* gs = grad_out + T.col[t];
-    int64_t gld = ld;
-    GradRows tr = gr;
+    EuProfScope ps(c, "emb_bwd_sums", L.E);
+    RowEntries R;   // the gathered kind: entry e's row is grad_out's row node[e] / group, from the table's column
+    R.n_src = L.E;
+    R.gt = grad_out + T.col[t];
+    R.ld = (int)ld;   // a row of at most EU_SHALLOW_MAX_WIDTH columns
+    R.node = node + base[t];
+    R.group = gr.group;
+    R.pool_den = gr.pool_den;
     if (t < S && T.comb[t] != EU_COMBINE_SUM) {   // a row per node, the pool's division done
       float* scaled = (float*)(m + o_gs);
-      k_emb_scale_grad<<<stride_grid(M * dim), 256, 0, s>>>(gs, ld, gr, ptr + t * (M + 1), M, dim, T.comb[t], scaled);
+      k_emb_scale_grad<<<stride_grid(M * dim), 256, 0, s>>>(R.gt, ld, gr, ptr + t * (M + 1), M, dim, T.comb[t], scaled);
       EU_LAUNCHED();
-      gs = scaled;
-      gld = dim;
-      tr = GradRows();
+      R.gt = scaled;
+      R.ld = dim;
+      R.group = 1;
+      R.pool_den = 0.f;
     }
-    float* out = grads[t];
-    const bool vec = dim % 4 == 0 && gld % 4 == 0 && aligned16(gs) && aligned16(out);
-    const int G = group_lanes(ceil_div(dim, vec ? 4 : 1));
-    const unsigned blocks = stride_grid((E_t[t] + E_t[t] / kSegChunk + 1) * G);   // >= one group per chunk, up to the grid cap
-    if (vec) k_emb_bwd_chunks<true><<<blocks, 256, 0, s>>>(gs, gld, tr, node + base[t], ord.perm, P, dim, G, !sparse, out);
-    else k_emb_bwd_chunks<false><<<blocks, 256, 0, s>>>(gs, gld, tr, node + base[t], ord.perm, P, dim, G, !sparse, out);
-    EU_LAUNCHED();
-    k_row_combine<<<stride_grid(E_t[t] * dim), 256, 0, s>>>(P, dim, !sparse, out, sparse ? rows[t] : nullptr);
-    EU_LAUNCHED();
-    if (sparse) EU_CUDA(cudaMemcpyAsync(nd_copy + t, P.nd, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+    if ((rc = sum_distinct_rows(c, R, L, dim, !sparse, grads[t], sparse ? rows[t] : nullptr))) return rc;
+    nd[t] = hdr + 1 + t;
+    if (sparse) EU_CUDA(cudaMemcpyAsync(hdr + 1 + t, L.P.nd, sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
   }
-  if (!sparse) return EU_OK;
-  int32_t h_nd[EU_SHALLOW_MAX_SLOTS + 1] = {};
-  EU_CUDA(cudaMemcpyAsync(h_nd, nd_copy, sizeof(int32_t) * NT, cudaMemcpyDeviceToHost, s));
-  EU_CUDA(cudaStreamSynchronize(s));
-  for (int t = 0; t < NT; ++t) counts[t] = h_nd[t];
-  return EU_OK;
+  return sparse ? read_back(c, hdr, nullptr, NT, nd, counts) : EU_OK;
 }
 
 // The single-slot op as a one-table backward pass

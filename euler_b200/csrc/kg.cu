@@ -39,8 +39,9 @@
 //   k_kg_bwd_raux    per triple: hyper (TransH), relation_transfer (TransD) or M (TransR) summed over src, dst, negatives in
 //                    that order in f64, rounded once: one relation-side entry per triple.  (These sums run over K + 2 terms,
 //                    4 099 at K = 4 097, where f32 would lose about 1e-5 of the largest entry.)
-// The entries are then summed per distinct table row by sum_distinct_rows (segment.cuh: stable order by row, 256-entry chunks
-// left to right, chunk sums in chunk order): no atomics, the same bits on every run.  Entity entries are listed src (B), dst
+// The entries are then summed per distinct table row by segment.cuh's id-table gradient path, the one the embedding and
+// skip-gram backward passes share (plan_rows: stable order by row; sum_distinct_rows: 256-entry chunks left to right, chunk
+// sums in chunk order): no atomics, the same bits on every run.  Entity entries are listed src (B), dst
 // (B), then negatives (b, k); relation entries by triple.  Scratch is O(B (2 + K) dim) (TransR: plus B ent_dim rel_dim), never
 // O(n_rows).  An id outside its table is read as row 0 and flagged: EU_ERR_INVALID after the call's one synchronisation.
 #include <atomic>
@@ -667,8 +668,7 @@ static int kg_args(eu_ctx* c, const eu_kg_problem* p, KgArgs* A, const char* who
     set_error("%s: dims above %d, or a TransR ent_dim * rel_dim above %d, are not supported", who, kKgMaxDim, kKgMaxMat);
     return EU_ERR_UNSUPPORTED;
   }
-  const int64_t E = p->B * ((int64_t)p->K + 2);
-  if (p->n_ent >= ((int64_t)1 << 31) || p->n_rel >= ((int64_t)1 << 31) || E + E / kSegChunk + 1 >= ((int64_t)1 << 31) ||
+  if (p->n_ent >= ((int64_t)1 << 31) || p->n_rel >= ((int64_t)1 << 31) || !entries_fit(p->B * ((int64_t)p->K + 2)) ||
       p->B * ceil_div(p->K, kKgTile) >= ((int64_t)1 << 31)) {
     set_error("%s: 2^31 or more table rows, or B (K + 2) entries with their chunks, are not supported", who);
     return EU_ERR_UNSUPPORTED;
@@ -746,38 +746,6 @@ static int kg_dispatch_bwd(eu_ctx* c, const KgArgs& A, const KgBwd& W, int* bad)
   return kg_vec(M, A) ? kg_launch_bwd<M, true>(c, A, W, bad) : kg_launch_bwd<M, false>(c, A, W, bad);
 }
 
-// A list of E entries to sum per distinct row: keys, order and plan in the scratch at buf
-struct KgList {
-  int64_t E = 0, n_rows = 0;
-  int32_t* key = nullptr;
-  EdgeOrder ord;
-  DistinctPlan P;
-};
-
-static size_t kg_list_bytes(int64_t E, int64_t n_rows, int width) {
-  return E ? a256(4 * (size_t)E) + order_bytes(E, n_rows) + distinct_plan_bytes(E, width) : 0;
-}
-
-static int kg_plan(eu_ctx* c, const KgArgs& A, bool entity, char* buf, int* bad, KgList* L) {
-  if (!L->E) return EU_OK;
-  L->key = (int32_t*)buf;
-  char* o_ord = buf + a256(4 * (size_t)L->E);
-  char* o_plan = o_ord + order_bytes(L->E, L->n_rows);
-  k_kg_keys<<<stride_grid(L->E), 256, 0, c->stream>>>(A, entity, L->E, L->key, bad);
-  EU_LAUNCHED();
-  int rc = order_by(c, L->key, L->E, L->n_rows, o_ord, &L->ord);
-  if (rc) return rc;
-  return plan_distinct(c, L->ord, L->E, o_plan, &L->P);
-}
-
-static int kg_sum(eu_ctx* c, const KgList& L, const float* vals, int dim, bool by_key, float* out, int64_t* rows) {
-  if (!L.E) return EU_OK;
-  RowEntries S;
-  S.n_src = L.E;
-  S.gt = vals;
-  return sum_distinct_rows(c, S, L.E, L.ord.perm, L.P, dim, by_key, out, rows);
-}
-
 // The backward pass both output forms share: out[t] is table t's dense gradient or COO values, rows[t] its COO rows
 static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, bool sparse, float* const* out,
                        int64_t* const* rows, int64_t* counts, const char* who) {
@@ -808,11 +776,11 @@ static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss
   }
   if (A.B == 0) return EU_OK;
   const int64_t B = A.B, N = A.K + 2, E1 = B * N, D = A.rel_dim;
-  KgList Le, Lr;
+  RowList Le, Lr;   // the entity entries (src, dst, negatives), the relation entries (one per triple)
   Le.E = E1; Le.n_rows = A.n_ent;
   Lr.E = B; Lr.n_rows = A.n_rel;
   // flag and counts (256 B) | coef [B] | F | T [B K D] | U [B N D] | sc [B N] | Gent | Gea [E1 ent] | Grel [B rel] | Graux [B aw]
-  // | entity list | relation list
+  // | entity list: keys, plan | relation list: keys, plan
   size_t o = 256;
   const size_t o_coef = o; o += a256(8 * (size_t)B);
   const size_t o_F = o; o += A.front ? a256(4 * (size_t)(B * A.K * D)) : 0;
@@ -823,8 +791,10 @@ static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss
   const size_t o_Gea = o; o += has[2] ? a256(4 * (size_t)E1 * A.ent_dim) : 0;
   const size_t o_Gr = o; o += a256(4 * (size_t)B * A.rel_dim);
   const size_t o_Gra = o; o += has[3] ? a256(4 * (size_t)B * aw) : 0;
-  const size_t o_Le = o; o += kg_list_bytes(E1, A.n_ent, A.ent_dim);
-  const size_t o_Lr = o; o += kg_list_bytes(B, A.n_rel, std::max(A.rel_dim, aw));
+  const size_t o_Ke = o; o += a256(4 * (size_t)E1);
+  const size_t o_Pe = o; o += row_plan_bytes(E1, A.n_ent, A.ent_dim);
+  const size_t o_Kr = o; o += a256(4 * (size_t)B);
+  const size_t o_Pr = o; o += row_plan_bytes(B, A.n_rel, std::max(A.rel_dim, aw));
   if ((rc = ctx_misc(c, (int64_t)o))) return rc;
   char* m = (char*)c->d_misc;
   int* bad = (int*)m;
@@ -838,11 +808,17 @@ static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss
   W.Gea = (float*)(m + o_Gea);
   W.Grel = (float*)(m + o_Gr);
   W.Graux = (float*)(m + o_Gra);
+  Le.key = (int32_t*)(m + o_Ke);
+  Lr.key = (int32_t*)(m + o_Kr);
   EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), s));
   {
     EuProfScope ps(c, "kg_bwd_order", E1 + B);
-    if ((rc = kg_plan(c, A, true, m + o_Le, bad, &Le))) return rc;
-    if ((rc = kg_plan(c, A, false, m + o_Lr, bad, &Lr))) return rc;
+    k_kg_keys<<<stride_grid(E1), 256, 0, s>>>(A, true, E1, Le.key, bad);
+    EU_LAUNCHED();
+    if ((rc = plan_rows(c, m + o_Pe, &Le))) return rc;
+    k_kg_keys<<<stride_grid(B), 256, 0, s>>>(A, false, B, Lr.key, bad);
+    EU_LAUNCHED();
+    if ((rc = plan_rows(c, m + o_Pr, &Lr))) return rc;
   }
   {
     EuProfScope ps(c, "kg_bwd_rows", E1);
@@ -861,22 +837,22 @@ static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss
   const float* vals[4] = {W.Gent, W.Grel, W.Gea, W.Graux};
   for (int t = 0; t < 4; ++t) {
     if (!has[t]) continue;
-    if ((rc = kg_sum(c, t % 2 == 0 ? Le : Lr, vals[t], width[t], !sparse, out[t], sparse ? rows[t] : nullptr))) return rc;
+    RowEntries R;   // one stored row per entry
+    R.n_src = t % 2 == 0 ? E1 : B;
+    R.gt = vals[t];
+    if ((rc = sum_distinct_rows(c, R, t % 2 == 0 ? Le : Lr, width[t], !sparse, out[t], sparse ? rows[t] : nullptr))) return rc;
   }
-  int32_t h[3] = {0, 0, 0};
-  EU_CUDA(cudaMemcpyAsync(h, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
-  if (sparse) {
-    EU_CUDA(cudaMemcpyAsync(h + 1, Le.P.nd, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    EU_CUDA(cudaMemcpyAsync(h + 2, Lr.P.nd, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  }
-  EU_CUDA(cudaStreamSynchronize(s));
-  if (h[0]) {
+  bool h_bad = false;
+  const int32_t* nd[2] = {Le.P.nd, Lr.P.nd};
+  int64_t n[2] = {0, 0};
+  if ((rc = read_back(c, bad, &h_bad, sparse ? 2 : 0, nd, n))) return rc;
+  if (h_bad) {
     set_error("%s: an id lies outside its table's rows", who);
     return EU_ERR_INVALID;
   }
   if (sparse)
     for (int t = 0; t < 4; ++t)
-      if (has[t]) counts[t] = h[1 + t % 2];
+      if (has[t]) counts[t] = n[t % 2];
   return EU_OK;
 }
 
@@ -897,31 +873,24 @@ int eu_kg_loss(eu_ctx* c, const eu_kg_problem* p, float* scores, int32_t* rank, 
     return EU_ERR_INVALID;
   }
   EU_CUDA(cudaSetDevice(c->g->device));
-  cudaStream_t s = c->stream;
-  // flag (256 B) | rowloss f64[B]
-  if ((rc = ctx_misc(c, 256 + (int64_t)a256(8 * (size_t)A.B)))) return rc;
-  int* bad = (int*)c->d_misc;
-  double* rowloss = (double*)((char*)c->d_misc + 256);
-  EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), s));
   EuProfScope ps(c, "kg_fwd", A.B);
-  if (A.B > 0) {
+  bool h_bad = false;
+  rc = mean_loss(c, A.B, A.B, loss, &h_bad, [&](int* bad, double* rowloss) -> int {
+    int rc2;
     switch (p->model) {
-      case KG_TRANSE: rc = kg_dispatch_fwd<KG_TRANSE>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      case KG_TRANSH: rc = kg_dispatch_fwd<KG_TRANSH>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      case KG_TRANSR: rc = kg_dispatch_fwd<KG_TRANSR>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      case KG_TRANSD: rc = kg_dispatch_fwd<KG_TRANSD>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      default: rc = kg_dispatch_fwd<KG_DISTMULT>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSE: rc2 = kg_dispatch_fwd<KG_TRANSE>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSH: rc2 = kg_dispatch_fwd<KG_TRANSH>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSR: rc2 = kg_dispatch_fwd<KG_TRANSR>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSD: rc2 = kg_dispatch_fwd<KG_TRANSD>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
+      default: rc2 = kg_dispatch_fwd<KG_DISTMULT>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
     }
-    if (rc) return rc;
-    k_kg_rows<<<(unsigned)A.B, kKgThreads, 0, s>>>(scores, A.B, A.C * A.K, A.margin, rank, rowloss, nullptr, nullptr);
+    if (rc2) return rc2;
+    k_kg_rows<<<(unsigned)A.B, kKgThreads, 0, c->stream>>>(scores, A.B, A.C * A.K, A.margin, rank, rowloss, nullptr, nullptr);
     EU_LAUNCHED();
-  }
-  k_f64_mean<<<1, kMeanThreads, 0, s>>>(rowloss, A.B, A.B, loss);
-  EU_LAUNCHED();
-  int h = 0;
-  EU_CUDA(cudaMemcpyAsync(&h, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
-  EU_CUDA(cudaStreamSynchronize(s));
-  if (h) {
+    return EU_OK;
+  });
+  if (rc) return rc;
+  if (h_bad) {
     set_error("%s: an id lies outside its table's rows", who);
     return EU_ERR_INVALID;
   }

@@ -202,6 +202,17 @@ int plan_distinct(eu_ctx* c, const EdgeOrder& o, int64_t E, char* buf, DistinctP
   return EU_OK;
 }
 
+size_t row_plan_bytes(int64_t E, int64_t n_rows, int64_t width) {
+  return E ? order_bytes(E, n_rows) + distinct_plan_bytes(E, width) : 0;
+}
+
+int plan_rows(eu_ctx* c, char* buf, RowList* L) {
+  if (!L->E) return EU_OK;
+  int rc = order_by(c, L->key, L->E, L->n_rows, buf, &L->ord);
+  if (rc) return rc;
+  return plan_distinct(c, L->ord, L->E, buf + order_bytes(L->E, L->n_rows), &L->P);
+}
+
 constexpr int kRowSumUnroll = 8;   // entries in flight per lane in the chunk sums
 
 // the destination row of distinct segment p: the table row key[p] (dense) or row p of the COO values (sparse)
@@ -209,11 +220,16 @@ __device__ __forceinline__ float* distinct_out_row(float* out, const DistinctPla
   return out + (by_key ? (int64_t)__ldg(P.key + p) : p) * dim;
 }
 
-// G lanes per chunk of the distinct-row segments (k_emb_bwd_chunks' layout): the chunk's entries summed left to right from +0,
-// kRowSumUnroll of them in flight; a segment of one chunk writes its output row, the chunks of a longer one their partial rows
-template <bool VEC>
-__global__ void __launch_bounds__(256) k_row_chunks(RowEntries S, const int32_t* __restrict__ perm, DistinctPlan P, int dim, int G,
-                                                    bool by_key, float* __restrict__ out) {
+// G lanes per chunk of the distinct-row segments, 4 columns per lane and step: the chunk's entries summed left to right from
+// +0, kRowSumUnroll of them in flight; a segment of one chunk writes its output row, the chunks of a longer one their partial
+// rows.  GATHER: the entries are RowEntries' gathered kind (a template parameter, so the other kinds carry none of its division).
+// A column's adds are fma(w, x, acc) in entry order whatever the lane mapping, and fma(1, x, acc) is __fadd_rn(acc, x).  The
+// gathered kind asks for one block per SM: under the default bound ptxas spilled around the scalar path's division subroutine.
+// The other kinds keep the default (a minimum of 0 emits none); one block per SM would raise them from 63 / 80 registers to
+// 70 / 82, and the float4 form would then fit two blocks per SM instead of three.
+template <bool VEC, bool GATHER>
+__global__ void __launch_bounds__(256, GATHER ? 1 : 0) k_row_chunks(RowEntries S, const int32_t* __restrict__ perm, DistinctPlan P,
+                                                                    int dim, int G, bool by_key, float* __restrict__ out) {
   const int lg = 31 - __clz(G);
   const int sub = (int)(threadIdx.x & (G - 1));
   const int64_t nch_all = __ldg(P.chunk_off + P.E);
@@ -235,8 +251,9 @@ __global__ void __launch_bounds__(256) k_row_chunks(RowEntries S, const int32_t*
         for (int q = 0; q < U; ++q) {
           if (k0 + q < e) {
             const int64_t en = __ldg(perm + k0 + q);
-            if (en < S.n_src) {
-              x[q] = row_load4<VEC>(S.gt + en * dim, d, dim);
+            if (GATHER || en < S.n_src) {
+              const float* row = GATHER ? S.gt + (int64_t)(__ldg(S.node + en) / S.group) * S.ld : S.gt + en * dim;
+              x[q] = row_load4<VEC>(row, d, dim);
               w[q] = 1.f;
             } else {
               const int64_t t = en - S.n_src;
@@ -248,6 +265,10 @@ __global__ void __launch_bounds__(256) k_row_chunks(RowEntries S, const int32_t*
 #pragma unroll
         for (int q = 0; q < U; ++q) {
           if (k0 + q < e) {
+            if (GATHER && S.pool_den != 0.f) {
+              x[q].x = __fdiv_rn(x[q].x, S.pool_den); x[q].y = __fdiv_rn(x[q].y, S.pool_den);
+              x[q].z = __fdiv_rn(x[q].z, S.pool_den); x[q].w = __fdiv_rn(x[q].w, S.pool_den);
+            }
             acc.x = __fmaf_rn(w[q], x[q].x, acc.x); acc.y = __fmaf_rn(w[q], x[q].y, acc.y);
             acc.z = __fmaf_rn(w[q], x[q].z, acc.z); acc.w = __fmaf_rn(w[q], x[q].w, acc.w);
           }
@@ -283,17 +304,31 @@ __global__ void k_row_combine(DistinctPlan P, int dim, bool by_key, float* __res
   }
 }
 
-int sum_distinct_rows(eu_ctx* c, const RowEntries& S, int64_t E, const int32_t* perm, const DistinctPlan& P, int dim, bool by_key,
-                      float* out, int64_t* rows) {
+int sum_distinct_rows(eu_ctx* c, const RowEntries& S, const RowList& L, int dim, bool by_key, float* out, int64_t* rows) {
+  if (!L.E) return EU_OK;
   cudaStream_t s = c->stream;
-  const bool vec = dim % 4 == 0 && aligned16(out) && (!S.target || aligned16(S.target)) && (!S.gt || aligned16(S.gt));
+  const bool vec = dim % 4 == 0 && (!S.node || S.ld % 4 == 0) && aligned16(out) && (!S.gt || aligned16(S.gt)) &&
+                   (!S.target || aligned16(S.target));
   const int G = group_lanes(ceil_div(dim, 4));
-  const unsigned blocks = stride_grid((E + E / kSegChunk + 1) * G);
-  if (vec) k_row_chunks<true><<<blocks, 256, 0, s>>>(S, perm, P, dim, G, by_key, out);
-  else k_row_chunks<false><<<blocks, 256, 0, s>>>(S, perm, P, dim, G, by_key, out);
+  const unsigned blocks = stride_grid((L.E + L.E / kSegChunk + 1) * G);   // >= one group per chunk, up to the grid cap
+  auto chunks = vec ? (S.node ? k_row_chunks<true, true> : k_row_chunks<true, false>)
+                    : (S.node ? k_row_chunks<false, true> : k_row_chunks<false, false>);
+  chunks<<<blocks, 256, 0, s>>>(S, L.ord.perm, L.P, dim, G, by_key, out);
   EU_LAUNCHED();
-  k_row_combine<<<stride_grid(E * dim), 256, 0, s>>>(P, dim, by_key, out, rows);
+  k_row_combine<<<stride_grid(L.E * dim), 256, 0, s>>>(L.P, dim, by_key, out, rows);
   EU_LAUNCHED();
+  return EU_OK;
+}
+
+int read_back(eu_ctx* c, int32_t* hdr, bool* bad, int n, const int32_t* const* nd, int64_t* counts) {
+  cudaStream_t s = c->stream;
+  int32_t h[kReadBackMax + 1] = {};
+  for (int i = 0; i < n; ++i)
+    if (nd[i] && nd[i] != hdr + 1 + i) EU_CUDA(cudaMemcpyAsync(hdr + 1 + i, nd[i], sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
+  EU_CUDA(cudaMemcpyAsync(h, hdr, sizeof(int32_t) * (1 + n), cudaMemcpyDeviceToHost, s));
+  EU_CUDA(cudaStreamSynchronize(s));
+  if (bad) *bad = h[0] != 0;
+  for (int i = 0; i < n; ++i) counts[i] = nd[i] ? h[1 + i] : 0;
   return EU_OK;
 }
 

@@ -1,4 +1,5 @@
-// Edge orders and fixed-order segment sums shared by the fused aggregations (gat.cu, relation.cu, dna.cu) and the mp scatter.
+// Edge orders and fixed-order segment sums shared by the fused aggregations (gat.cu, relation.cu, dna.cu), the mp scatter and
+// the id-table gradients (embedding.cu, skipgram.cu, kg.cu).
 //
 // An edge order walks the edges sorted by an int32 index (the target, the source, a relation), stably: edges with equal
 // index keep their order, so a sum over a segment in order gives the bits of the same sum over the stably sorted list.  A
@@ -134,7 +135,25 @@ size_t distinct_plan_bytes(int64_t E, int64_t width);
 int plan_distinct(eu_ctx* c, const EdgeOrder& o, int64_t E, char* buf, DistinctPlan* P);
 
 // ---------------------------------------------------------------------------- id-table rows summed per distinct id
-// Shared by the losses over id tables (skipgram.cu, kg.cu).
+// Every backward pass that trains id tables (embedding.cu's SparseEmbedding and ShallowEncoder, skipgram.cu, kg.cu) reduces its
+// table gradients this one way, which fixes their bits: the op's own key kernel lists one int32 key (a table row) per entry;
+// plan_rows orders the entries stably by key and plans the distinct rows; sum_distinct_rows sums each 256-entry chunk from +0
+// and adds a row's chunk sums in chunk order, into a dense table or a coalesced COO; read_back then reads the bad-id flag and
+// the distinct counts in one synchronisation.  Deterministic, no atomics, O(entries) scratch whatever the table's rows.
+
+// a list of E entries and their chunks is indexed by int32 positions: E + E / kSegChunk + 1 < 2^31
+inline bool entries_fit(int64_t E) { return E + E / kSegChunk + 1 < ((int64_t)1 << 31); }
+
+struct RowList {                   // E entries over a table of n_rows rows
+  int64_t E = 0, n_rows = 0;
+  int32_t* key = nullptr;          // [E]: each entry's row, written by the caller
+  EdgeOrder ord;
+  DistinctPlan P;
+};
+// the scratch plan_rows needs for a list of E entries with width columns of chunk sums (its keys are the caller's); 0 when E = 0
+size_t row_plan_bytes(int64_t E, int64_t n_rows, int64_t width);
+// L's stable order by key and its distinct-row plan, in buf (row_plan_bytes), once L->key is written; nothing when E = 0
+int plan_rows(eu_ctx* c, char* buf, RowList* L);
 
 // the columns [d, d + 4) of a row (fewer than 4 at the row's end): one float4 load (VEC) or up to four scalar loads
 template <bool VEC>
@@ -155,32 +174,56 @@ __device__ __forceinline__ int64_t row_of(int64_t v, int64_t n_rows, int* bad) {
   return 0;
 }
 
-// The values of an entry list ordered by row: entries e < n_src have the materialised value gt[e, :]; entries e >= n_src
-// have coef[t] * target[src_b, :], t = e - n_src, b = t / J (computed while they are summed).  A list of materialised rows only
-// has n_src = its length.
+// The values of an entry list ordered by row.  Entries e < n_src are stored rows gt[e, :], or, when node is given (the
+// gathered kind: every entry stored), rows gt[r * ld, :] with r = node[e] / group, each element divided by pool_den first
+// unless that is 0.  Entries e >= n_src have coef[t] * target[src_b, :], t = e - n_src, b = t / J (computed while they are
+// summed).  A list of stored rows only has n_src = its length.
 struct RowEntries {
   int64_t n_src = 0;
-  int J = 1;
   const float* gt = nullptr;
+  const int32_t* node = nullptr;
+  int ld = 0;
+  int group = 1;
+  float pool_den = 0.f;
+  int J = 1;
   const float* coef = nullptr;
   const int64_t* src = nullptr;
   const float* target = nullptr;
   int64_t n_rows = 0;
 };
 
-// The sums per distinct row of the E > 0 entries S in the order `perm` with the plan P: each 256-entry chunk adds its entries
-// left to right from +0 as acc = fma(w, row, acc) (w = 1 for a materialised row), a row of several chunks adds its chunk sums
-// in chunk order from +0.  by_key: into the dense table out (rows not in the list untouched); else into COO values out, with
-// the rows' ids in rows (may be null).  No atomics: the bits depend on each row's entry sequence only.
-int sum_distinct_rows(eu_ctx* c, const RowEntries& S, int64_t E, const int32_t* perm, const DistinctPlan& P, int dim, bool by_key,
-                      float* out, int64_t* rows);
-// The second step of such sums: the output row of each segment of several chunks = its partial rows added in chunk order from
-// +0 (by_key: table row key[p] of out; else COO row p), and rows[p] = key[p] when rows is given.  Grid-stride over E * dim.
-__global__ void k_row_combine(DistinctPlan P, int dim, bool by_key, float* __restrict__ out, int64_t* __restrict__ rows);
+// The sums per distinct row of list L's entries S (nothing when L.E = 0): each 256-entry chunk adds its entries left to
+// right from +0 as acc = fma(w, row, acc) (w = 1 for a stored row, so a plain add), a row of several chunks adds its chunk
+// sums in chunk order from +0.  by_key: into the dense table out (rows not in the list untouched); else into COO values out,
+// with the rows' ids in rows (may be null).  No atomics: the bits depend on each row's entry sequence only.
+int sum_distinct_rows(eu_ctx* c, const RowEntries& S, const RowList& L, int dim, bool by_key, float* out, int64_t* rows);
+
+// One stream synchronisation over a header of 1 + n int32 of device scratch: *bad = (hdr[0] != 0), the bad-id flag (bad
+// null: no flag), and counts[i] = *nd[i], the distinct rows of a plan's list, for i < n <= kReadBackMax (a null nd[i], a list
+// never planned, reads 0).  The counts are first copied to hdr[1 + i] on the device (unless nd[i] is that slot already), so
+// the header comes back in one copy.
+constexpr int kReadBackMax = EU_SHALLOW_MAX_SLOTS + 1;
+int read_back(eu_ctx* c, int32_t* hdr, bool* bad, int n, const int32_t* const* nd, int64_t* counts);
 
 // *loss = fl32((sum of rowloss[0, B)) / N): thread t adds rowloss[t], rowloss[t + 1024], ... in f64, then a shared-memory tree
 // (strides 512 .. 1).  One block of kMeanThreads; N = 0 gives NaN, as a mean of nothing.
 constexpr int kMeanThreads = 1024;
 __global__ void k_f64_mean(const double* __restrict__ rowloss, int64_t B, int64_t N, float* __restrict__ loss);
+
+// The forward tail of a loss over B rows (skipgram.cu, kg.cu), in the ctx scratch flag (256 B) | rowloss f64[B]: when B > 0,
+// rows(flag, rowloss) launches the op's kernels, which write each row's loss and set *flag on an id outside its table; then
+// *loss = the k_f64_mean of the rows over N, and *bad = the flag, read back in the call's one synchronisation.
+template <class Rows>
+int mean_loss(eu_ctx* c, int64_t B, int64_t N, float* loss, bool* bad, Rows rows) {
+  int rc = ctx_misc(c, 256 + (int64_t)a256(8 * (size_t)B));
+  if (rc) return rc;
+  int32_t* flag = (int32_t*)c->d_misc;
+  double* rowloss = (double*)((char*)c->d_misc + 256);
+  EU_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), c->stream));
+  if (B > 0 && (rc = rows(flag, rowloss))) return rc;
+  k_f64_mean<<<1, kMeanThreads, 0, c->stream>>>(rowloss, B, N, loss);
+  EU_LAUNCHED();
+  return read_back(c, flag, bad, 0, nullptr, nullptr);
+}
 
 }  // namespace eu

@@ -20,8 +20,9 @@
 //
 // Backward, with g the upstream gradient (a device scalar) and N = B J: gN = g / fl(N) once, and per logit
 //   c_bj = -gN / (1 + exp(x))  (j < P: (sigmoid(x) - 1) gN)      c_bj = gN / (1 + exp(-x))  (j >= P: sigmoid(x) gN).
-// The gradients go to the tables through key lists sorted stably by row and summed per distinct row in fixed chunks of
-// kSegChunk entries (order_by, plan_distinct: segment.cuh), no atomics:
+// The gradients go to the tables through segment.cuh's id-table gradient path, the one the embedding and KG backward passes
+// share: key lists sorted stably by row (plan_rows) and summed per distinct row in fixed chunks of kSegChunk entries
+// (sum_distinct_rows), no atomics:
 //   the src entries:     entry b has key src_b and value gt_b = sum over j of c_bj context[ctx_bj] (fma from +0, j order)
 //   the context entries: entry (b, j) has key ctx_bj and value c_bj target[src_b], computed while it is summed
 // Each chunk adds its entries' values left to right from +0, as acc = fma(w, row, acc) with w = 1 for a src entry (so a plain
@@ -207,47 +208,11 @@ static int sg_check(eu_ctx* c, const int64_t* src, const int64_t* pos, const int
     set_error("%s: bad argument (B >= 0, P >= 1, K >= 0, n_rows and dim >= 1, tables and ids given)", who);
     return EU_ERR_INVALID;
   }
-  const int64_t E = B * ((int64_t)P + K + 1);   // the longest entry list (one shared table), and its chunks below
-  if (n_rows >= ((int64_t)1 << 31) || E + E / kSegChunk + 1 >= ((int64_t)1 << 31)) {
+  if (n_rows >= ((int64_t)1 << 31) || !entries_fit(B * ((int64_t)P + K + 1))) {   // the longest list: one shared table's
     set_error("%s: 2^31 or more table rows, or B (P + K + 1) entries with their chunks, are not supported", who);
     return EU_ERR_UNSUPPORTED;
   }
   return EU_OK;
-}
-
-// A list of E > 0 entries to sum per distinct row: its keys, order and plan in the scratch at m + off (sg_list_bytes)
-struct SgList {
-  int64_t E = 0;
-  RowEntries S;
-  bool ctx_entries = false;
-  int32_t* key = nullptr;
-  EdgeOrder ord;
-  DistinctPlan P;
-};
-
-static size_t sg_list_bytes(int64_t E, int64_t n_rows, int dim) {
-  return E ? a256(4 * (size_t)E) + order_bytes(E, n_rows) + distinct_plan_bytes(E, dim) : 0;
-}
-
-// keys, the stable order by row and the distinct-row plan of list L, from the scratch at buf
-static int sg_plan(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int P, int K, int64_t n_rows,
-                   int dim, char* buf, int* bad, SgList* L) {
-  if (!L->E) return EU_OK;
-  cudaStream_t s = c->stream;
-  L->key = (int32_t*)buf;
-  char* o_ord = buf + a256(4 * (size_t)L->E);
-  char* o_plan = o_ord + order_bytes(L->E, n_rows);
-  k_sg_keys<<<stride_grid(L->E), 256, 0, s>>>(src, pos, negs, B, P, K, L->S.n_src, L->ctx_entries, n_rows, L->key, bad);
-  EU_LAUNCHED();
-  int rc = order_by(c, L->key, L->E, n_rows, o_ord, &L->ord);
-  if (rc) return rc;
-  return plan_distinct(c, L->ord, L->E, o_plan, &L->P);
-}
-
-// the chunk sums and their combination of list L into out (by_key: a dense table; else COO values, with their row ids in rows)
-static int sg_sum(eu_ctx* c, const SgList& L, int dim, bool by_key, float* out, int64_t* rows) {
-  if (!L.E) return EU_OK;
-  return sum_distinct_rows(c, L.S, L.E, L.ord.perm, L.P, dim, by_key, out, rows);
 }
 
 // The backward pass both output forms share.  shared: one list into the target outputs.  sparse: the COO of
@@ -267,32 +232,33 @@ static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, co
   const int J = P + K;
   const int64_t N = B * J;
   if (B == 0) return EU_OK;
-  SgList Lt, Lc;
-  Lt.S.J = Lc.S.J = J;
-  Lt.S.n_rows = Lc.S.n_rows = n_rows;
-  Lt.S.src = Lc.S.src = src;
-  Lt.S.target = Lc.S.target = target;
-  Lt.S.n_src = B;
-  Lt.ctx_entries = shared;
+  RowList Lt, Lc;   // the target table's entries (shared: every entry) and the context table's
   Lt.E = shared ? B + N : B;
   Lc.E = shared ? 0 : N;
-  Lc.ctx_entries = true;
-  // flag and the two distinct counts (256 B) | coef [N] | gt [B, dim] | list t | list c
-  const size_t o_coef = 256, o_gt = o_coef + a256(4 * (size_t)N), o_lt = o_gt + a256(4 * (size_t)B * dim);
-  const size_t o_lc = o_lt + sg_list_bytes(Lt.E, n_rows, dim), total = o_lc + sg_list_bytes(Lc.E, n_rows, dim);
+  Lt.n_rows = Lc.n_rows = n_rows;
+  // flag and the two distinct counts (256 B) | coef [N] | gt [B, dim] | list t: keys, plan | list c: keys, plan
+  const size_t o_coef = 256, o_gt = o_coef + a256(4 * (size_t)N), o_kt = o_gt + a256(4 * (size_t)B * dim);
+  const size_t o_pt = o_kt + a256(4 * (size_t)Lt.E), o_kc = o_pt + row_plan_bytes(Lt.E, n_rows, dim);
+  const size_t o_pc = o_kc + a256(4 * (size_t)Lc.E), total = o_pc + row_plan_bytes(Lc.E, n_rows, dim);
   int rc = ctx_misc(c, (int64_t)total);
   if (rc) return rc;
   char* m = (char*)c->d_misc;
   int* bad = (int*)m;
   float* coef = (float*)(m + o_coef);
   float* gt = (float*)(m + o_gt);
-  Lt.S.gt = Lc.S.gt = gt;
-  Lt.S.coef = Lc.S.coef = coef;
+  Lt.key = (int32_t*)(m + o_kt);
+  Lc.key = (int32_t*)(m + o_kc);
   EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), s));
   {
     EuProfScope ps(c, "skipgram_bwd_order", Lt.E + Lc.E);
-    if ((rc = sg_plan(c, src, pos, negs, B, P, K, n_rows, dim, m + o_lt, bad, &Lt))) return rc;
-    if ((rc = sg_plan(c, src, pos, negs, B, P, K, n_rows, dim, m + o_lc, bad, &Lc))) return rc;
+    k_sg_keys<<<stride_grid(Lt.E), 256, 0, s>>>(src, pos, negs, B, P, K, B, shared, n_rows, Lt.key, bad);
+    EU_LAUNCHED();
+    if ((rc = plan_rows(c, m + o_pt, &Lt))) return rc;
+    if (Lc.E) {
+      k_sg_keys<<<stride_grid(Lc.E), 256, 0, s>>>(src, pos, negs, B, P, K, 0, true, n_rows, Lc.key, bad);
+      EU_LAUNCHED();
+      if ((rc = plan_rows(c, m + o_pc, &Lc))) return rc;
+    }
   }
   EuProfScope ps(c, "skipgram_bwd_sums", Lt.E + Lc.E);
   k_sg_coef<<<stride_grid(N), 256, 0, s>>>(logits, grad_loss, N, P, J, coef);
@@ -303,19 +269,27 @@ static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, co
   if (vec) k_sg_target_rows<true><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, context, n_rows, dim, G, gt);
   else k_sg_target_rows<false><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, context, n_rows, dim, G, gt);
   EU_LAUNCHED();
-  if ((rc = sg_sum(c, Lt, dim, !sparse, out_t, rows_t))) return rc;
-  if ((rc = sg_sum(c, Lc, dim, !sparse, out_c, rows_c))) return rc;
-  int32_t h[3] = {0, 0, 0};
-  EU_CUDA(cudaMemcpyAsync(h, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
-  if (sparse) EU_CUDA(cudaMemcpyAsync(h + 1, Lt.P.nd, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (sparse && Lc.E) EU_CUDA(cudaMemcpyAsync(h + 2, Lc.P.nd, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  EU_CUDA(cudaStreamSynchronize(s));
-  if (h[0]) {
+  RowEntries R;   // the target list: the B src entries (gt rows), then the context entries; the context list: those only
+  R.n_src = B;
+  R.gt = gt;
+  R.J = J;
+  R.coef = coef;
+  R.src = src;
+  R.target = target;
+  R.n_rows = n_rows;
+  if ((rc = sum_distinct_rows(c, R, Lt, dim, !sparse, out_t, rows_t))) return rc;
+  R.n_src = 0;
+  if ((rc = sum_distinct_rows(c, R, Lc, dim, !sparse, out_c, rows_c))) return rc;
+  bool h_bad = false;
+  const int32_t* nd[2] = {Lt.P.nd, Lc.P.nd};
+  int64_t n[2] = {0, 0};
+  if ((rc = read_back(c, bad, &h_bad, sparse ? 2 : 0, nd, n))) return rc;
+  if (h_bad) {
     set_error("%s: an id lies outside the table's rows [0, %lld)", who, (long long)n_rows);
     return EU_ERR_INVALID;
   }
-  if (n_t) *n_t = h[1];
-  if (n_c) *n_c = h[2];
+  if (n_t) *n_t = n[0];
+  if (n_c) *n_c = n[1];
   return EU_OK;
 }
 
@@ -336,27 +310,19 @@ int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const in
     return EU_ERR_INVALID;
   }
   EU_CUDA(cudaSetDevice(c->g->device));
-  cudaStream_t s = c->stream;
-  // flag (256 B) | rowloss f64[B]
-  if ((rc = ctx_misc(c, 256 + (int64_t)a256(8 * (size_t)B)))) return rc;
-  int* bad = (int*)c->d_misc;
-  double* rowloss = (double*)((char*)c->d_misc + 256);
-  EU_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), s));
   EuProfScope ps(c, "skipgram_fwd", B);
-  if (B > 0) {
+  bool h_bad = false;
+  rc = mean_loss(c, B, B * (int64_t)(P + K), loss, &h_bad, [&](int* bad, double* rowloss) -> int {
     const bool vec = dim % 4 == 0 && aligned16(target) && aligned16(context);
     const int G = group_lanes(ceil_div(dim, 4));   // one lane per 4-column chunk, both paths: the same order
     const unsigned blocks = (unsigned)ceil_div(B * G, 256);
-    if (vec) k_sg_fwd<true><<<blocks, 256, 0, s>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
-    else k_sg_fwd<false><<<blocks, 256, 0, s>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
+    if (vec) k_sg_fwd<true><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
+    else k_sg_fwd<false><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
     EU_LAUNCHED();
-  }
-  k_f64_mean<<<1, kMeanThreads, 0, s>>>(rowloss, B, B * (int64_t)(P + K), loss);
-  EU_LAUNCHED();
-  int h = 0;
-  EU_CUDA(cudaMemcpyAsync(&h, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
-  EU_CUDA(cudaStreamSynchronize(s));
-  if (h) {
+    return EU_OK;
+  });
+  if (rc) return rc;
+  if (h_bad) {
     set_error("%s: an id lies outside the table's rows [0, %lld)", who, (long long)n_rows);
     return EU_ERR_INVALID;
   }
