@@ -2,7 +2,9 @@
 feature slots (ShallowEncoder, encoders.py:151-160; SageEncoderNew, encoders.py:590-612), and ShallowEncoder
 (encoders.py:32-171), the input layer of the node encoders: an id embedding, dense feature slots and sparse-feature
 embeddings, concatenated or added.  And SageEncoder / ShuffleSageEncoder (encoders.py:411-541), GraphSAGE over
-sample_fanout's sample tree with that input layer and the aggregators of aggregators.py.
+sample_fanout's sample tree with that input layer and the aggregators of aggregators.py.  And GCNEncoder / GenieEncoder
+(encoders.py:174-291), the full-neighbourhood encoders over get_multi_hop_neighbor's hops and the aggregators of
+sparse_aggregators.py.
 
 Callers size the table as the encoders do: SparseEmbedding(max_id + 1, dim) for values in [0, max_id] and
 default = max_id + 1 for nodes without values, so the table has max_id + 2 rows and the default row is the last one.
@@ -327,3 +329,111 @@ class ShuffleSageEncoder(SageEncoder):
     def forward(self, inputs, generator=None):
         samples = self.sample(inputs)
         return [self.agg(inputs, samples), self.agg(inputs, self.shuffle_samples(samples, generator))]
+
+
+class GCNEncoder(torch.nn.Module):
+    """encoders.GCNEncoder (tf_euler/python/utils/encoders.py:174-233): the full-neighbourhood encoder over
+    get_multi_hop_neighbor(inputs, metapath), with upstream's constructor arguments and head_num handling (an int, or a list
+    of one per layer).  The node encoder is ShallowEncoder(dim if use_residual else None, .., combiner='add' if use_residual
+    else 'concat'); layer l is sparse_aggregators.get(aggregator)(width of its inputs, dim, relu on all but the last layer,
+    head_num=head_num[l]).  Layer 0 reads the node encoder's output_dim columns, every later layer the previous layer's
+    output width (head_num * (dim // head_num) for 'attention'); self.dims lists them.  With use_residual each hop's output
+    is hidden[hop] + aggregator(..).  __call__(inputs) returns inputs.shape + (width of the last layer,).
+
+    Difference from upstream: under use_residual an aggregator whose width is not dim ('attention' with dim not a multiple of
+    head_num) fails upstream when the residual is added, at run time; here it raises ValueError at construction.
+
+    fused=True (the default) gives the aggregators their device paths (sparse_aggregators: ops.adjacency_mean for 'gcn' /
+    'mean', ops.gat_attention_aggregate for 'attention') and the node encoder its fused op; fused=False is the literal
+    composition everywhere.  sparse_grad=True gives the node encoder's tables sparse COO gradients."""
+
+    def __init__(self, metapath, dim, aggregator='mean', feature_idx=-1, feature_dim=0, max_id=-1, use_id=False,
+                 sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
+                 use_residual=False, head_num=4, fused=True, sparse_grad=False, device=None):
+        super().__init__()
+        from . import sparse_aggregators
+        self.metapath = metapath
+        self.num_layers = len(metapath)
+        if isinstance(head_num, int):
+            self.head_num = [head_num] * self.num_layers
+        elif isinstance(head_num, list):
+            assert len(head_num) == self.num_layers
+            self.head_num = head_num
+        else:
+            raise ValueError('head_num error: expect int or'
+                             ' list, got {}'.format(str(head_num)))
+        self.use_residual = use_residual
+        self._node_encoder = ShallowEncoder(
+            dim=dim if use_residual else None, feature_idx=feature_idx, feature_dim=feature_dim,
+            max_id=max_id if use_id else -1, sparse_feature_idx=sparse_feature_idx, sparse_feature_max_id=sparse_feature_max_id,
+            embedding_dim=embedding_dim, use_hash_embedding=use_hash_embedding, combiner='add' if use_residual else 'concat',
+            fused=fused, sparse_grad=sparse_grad, device=device)
+        aggregator_class = sparse_aggregators.get(aggregator)
+        self.dims = [self._node_encoder.output_dim]
+        aggs = []
+        for layer in range(self.num_layers):
+            activation = torch.relu if layer < self.num_layers - 1 else None
+            aggs.append(aggregator_class(self.dims[-1], dim, activation=activation, head_num=self.head_num[layer], fused=fused,
+                                         device=device))
+            self.dims.append(aggs[-1].output_dim)
+        if use_residual and any(d != dim for d in self.dims[1:]):
+            raise ValueError('use_residual needs every aggregator to be dim = %d wide, got widths %s' % (dim, self.dims[1:]))
+        self.aggregators = torch.nn.ModuleList(aggs)
+
+    def node_encoder(self, inputs):
+        return self._node_encoder(inputs)
+
+    def _layers(self, hidden, adjs, each_layer=None):
+        """upstream's layer / hop loop; each_layer(layer, hidden[0]) after every layer"""
+        for layer in range(self.num_layers):
+            aggregator = self.aggregators[layer]
+            next_hidden = []
+            for hop in range(self.num_layers - layer):
+                h = aggregator((hidden[hop], hidden[hop + 1], adjs[hop]))
+                next_hidden.append(hidden[hop] + h if self.use_residual else h)
+            hidden = next_hidden
+            if each_layer:
+                each_layer(layer, hidden[0])
+        return hidden[0]
+
+    def forward(self, inputs):
+        nodes, adjs = ops.get_multi_hop_neighbor(inputs, self.metapath)
+        out = self._layers([self.node_encoder(node) for node in nodes], adjs)
+        return out.reshape(tuple(inputs.shape) + (self.dims[-1],))
+
+
+class GenieEncoder(GCNEncoder):
+    """encoders.GenieEncoder (encoders.py:236-291), GeniePath's encoder: GCNEncoder's layers ('attention' by default), then
+    depth_fc[0] of the seeds' node-encoder rows and depth_fc[l + 1] of layer l's seed rows (depth_fc: Dense(dim) with a bias,
+    upstream's layers.Dense default), run as a sequence of L + 1 steps through TF's LSTMCell(dim) (graph_pool.LSTMCell) from a
+    zero state.  __call__(inputs) returns inputs.shape + (dim,).
+
+    Upstream returns outputs[:, 0, :] (encoders.py:287), the LSTM's output at the FIRST step: the result depends on the seeds'
+    own node-encoder rows only, and the aggregators, the later depth_fc layers and the later steps never reach it (they get
+    no gradient).  This restates that exactly, for parity with the geniepath example; it computes every layer and step, as
+    upstream does."""
+
+    def __init__(self, metapath, dim, aggregator='attention', feature_idx=-1, feature_dim=0, max_id=-1, use_id=False,
+                 sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
+                 use_residual=False, head_num=4, fused=True, sparse_grad=False, device=None):
+        super().__init__(metapath, dim, aggregator, feature_idx, feature_dim, max_id, use_id, sparse_feature_idx,
+                         sparse_feature_max_id, embedding_dim, use_hash_embedding, use_residual, head_num, fused=fused,
+                         sparse_grad=sparse_grad, device=device)
+        from .graph_pool import LSTMCell
+        self.dim = dim
+        self.depth_fc = torch.nn.ModuleList([Dense(d, dim, use_bias=True, device=device) for d in self.dims])
+        self.lstm_cell = LSTMCell(dim, dim)
+        if device is not None:
+            self.lstm_cell.to(device)
+
+    def forward(self, inputs):
+        nodes, adjs = ops.get_multi_hop_neighbor(inputs, self.metapath)
+        hidden = [self.node_encoder(node) for node in nodes]
+        h_t = [self.depth_fc[0](hidden[0])]
+        self._layers(hidden, adjs, lambda layer, h: h_t.append(self.depth_fc[layer + 1](h)))
+        zero = h_t[0].new_zeros((h_t[0].shape[0], self.dim))
+        state, outputs = (zero, zero), []
+        for x in h_t:
+            out, state = self.lstm_cell(x, state)
+            outputs.append(out)
+        return outputs[0].reshape(tuple(inputs.shape) + (self.dim,))

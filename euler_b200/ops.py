@@ -813,6 +813,47 @@ def gat_attention_aggregate(h_src, s_dst, s_src, edge_index, size):
     return _GatAggregate.apply(h_src, s_dst, s_src, dst, src, n_dst)
 
 
+class _AdjacencyMean(torch.autograd.Function):
+    """eu_adjacency_mean / eu_adjacency_mean_backward.  Saves its inputs only (the indices and x_neigh's row count)."""
+
+    @staticmethod
+    def forward(ctx, x_neigh, indptr, cols):
+        m, D = x_neigh.shape
+        n = indptr.numel() - 1
+        out = torch.empty((n, D), dtype=torch.float32, device=x_neigh.device)
+        _call("eu_adjacency_mean", x_neigh, m, indptr, cols, n, cols.numel(), D, out)
+        ctx.save_for_backward(indptr, cols)
+        ctx.m = m
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        indptr, cols = ctx.saved_tensors
+        grad = grad.contiguous()
+        n, D = grad.shape
+        g = torch.empty((ctx.m, D), dtype=torch.float32, device=grad.device)
+        _call("eu_adjacency_mean_backward", grad, indptr, cols, n, cols.numel(), ctx.m, D, g)
+        return g, None, None
+
+
+def adjacency_mean(x_neigh, adj):
+    """The neighbour mean of the dense-combining sparse aggregators (sparse_aggregators.py:37-84) in one fused device op:
+        x_neigh f32[m, D]    the neighbour rows
+        adj                  (indptr i64[n+1], cols i64[nnz] [, weights]) as get_multi_hop_neighbor returns per hop; the
+                             weights are ignored (upstream's _sparse_ones_like)
+    out[i] = (sum of x_neigh[cols[k]] over row i's entries) / max(deg_i, 1e-7), f32[n, D]; a row without entries gives zeros.
+    The sum runs in a fixed order (include/euler_b200.h): a row of at most 256 entries gives the bits of the plain
+    left-to-right float32 sum.  The backward pass is deterministic.  Neither pass synchronises with the host."""
+    indptr, cols = adj[0], adj[1]
+    if not torch.is_tensor(x_neigh) or x_neigh.dim() != 2:
+        raise EulerError("adjacency_mean: x_neigh must be a 2-D tensor")
+    x_neigh = _f32(x_neigh)
+    indptr, cols = _t(indptr, torch.int64).reshape(-1), _t(cols, torch.int64).reshape(-1)
+    if indptr.numel() < 1:
+        raise EulerError("adjacency_mean: indptr must hold n + 1 offsets")
+    return _AdjacencyMean.apply(x_neigh, indptr, cols)
+
+
 def _raw_agnn(x_src, nrm_dst, nrm_src, beta, dst, src, n_dst, with_alpha):
     """one eu_agnn_aggregate: (out f32[n_dst, dim], alpha f32[E] or None, cos f32[E] or None)"""
     n_src, dim = x_src.shape

@@ -803,6 +803,32 @@ int eu_dna_aggregate(eu_ctx* c, const float* q, const float* k, const float* v, 
 int eu_dna_aggregate_backward(eu_ctx* c, const float* grad_out, const float* q, const float* k, const float* v, const float* n0,
                               const float* n1, const float* alpha, const int32_t* dst, const int32_t* src, int64_t E, int64_t n_dst,
                               int64_t n_src, int32_t heads, int32_t head_dim, float* grad_q, float* grad_k, float* grad_v);
+/* The neighbour mean over a CSR adjacency: what GCNAggregator and MeanAggregator of the sparse aggregators compute before
+ * their dense layers (tf_euler/python/utils/sparse_aggregators.py:37-84: the weights replaced by ones, sparse_reduce_sum,
+ * sparse_tensor_dense_matmul, maximum(degree, 1e-7)).  Inputs x_neigh f32[m, dim] and the adjacency of n rows as
+ * eu_full_neighbor_hop's EU_HOP_SORT outputs give it, indptr i64[n+1] (indptr[0] = 0, indptr[n] = nnz) and cols i64[nnz]
+ * (the weights are not read).  For row i with deg_i = indptr[i+1] - indptr[i] entries (multi-edges counted):
+ *   S_i    = sum over k in [indptr[i], indptr[i+1]) of x_neigh[cols[k], :]   (fixed order: the row cut into chunks of 256
+ *            entries counted from its first one, each chunk summed left to right from +0, the chunk sums of a row of
+ *            several chunks added in chunk order from +0)
+ *   out[i] = __fdiv_rn(S_i, max(fl(deg_i), 1e-7f))   (one IEEE-rounded division; a row without entries gives a zero row)
+ * out f32[n, dim].  A row of at most 256 entries thus gets the bits of the plain left-to-right float32 sum.  The float4 and
+ * scalar paths (dim % 4 == 0 with x_neigh and out 16-byte aligned, or not) give the same bits.  No host synchronisation;
+ * ctx scratch of 12 B per row and (n + nnz / 256) * dim floats of chunk sums, which grows only with the sizes (a forward
+ * at sizes already seen is capturable in a CUDA graph).
+ * The backward pass takes grad_out f32[n, dim] and writes grad_x f32[m, dim] (zeroed first; columns without entries stay
+ * zero): with gs_i = __fdiv_rn(grad_out[i], max(fl(deg_i), 1e-7f)),
+ *   grad_x[j] = sum over the entries k with cols[k] = j of gs[row of k]
+ * summed as the id-table gradients of eu_sparse_embedding_lookup_backward are: the entries of column j in stable row
+ * order, chunks of 256 from +0, the chunk sums in chunk order.  Deterministic, no atomics, no host synchronisation; ctx
+ * scratch of n * dim floats, 8 B per entry and a stable sort of the entries by column (O(nnz)).
+ * Negative sizes, dim < 1, entries with n or m = 0, or a NULL pointer that is needed: EU_ERR_INVALID; n, m or nnz of 2^31
+ * or more (or nnz entries whose 256-entry chunks reach 2^31): EU_ERR_UNSUPPORTED.  indptr and cols are not checked (as
+ * eu_gather): indptr must be non-decreasing from 0 to nnz and cols must lie in [0, m).  Device pointers. */
+int eu_adjacency_mean(eu_ctx* c, const float* x_neigh, int64_t m, const int64_t* indptr, const int64_t* cols, int64_t n,
+                      int64_t nnz, int32_t dim, float* out);
+int eu_adjacency_mean_backward(eu_ctx* c, const float* grad_out, const int64_t* indptr, const int64_t* cols, int64_t n,
+                               int64_t nnz, int64_t m, int32_t dim, float* grad_x);
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx,
                    int64_t E, float* out);
 int eu_scatter_add_host(eu_ctx* c, const float* updates, int64_t D, const int32_t* idx, int64_t E,
