@@ -4,7 +4,8 @@ feature slots (ShallowEncoder, encoders.py:151-160; SageEncoderNew, encoders.py:
 embeddings, concatenated or added.  And SageEncoder / ShuffleSageEncoder (encoders.py:411-541), GraphSAGE over
 sample_fanout's sample tree with that input layer and the aggregators of aggregators.py.  And GCNEncoder / GenieEncoder
 (encoders.py:174-291), the full-neighbourhood encoders over get_multi_hop_neighbor's hops and the aggregators of
-sparse_aggregators.py.
+sparse_aggregators.py.  And ScalableSageEncoder / ScalableGCNEncoder (encoders.py:294-408, 629-748), which train every layer
+from one hop over per-layer embedding stores (_ScalableStores).
 
 Callers size the table as the encoders do: SparseEmbedding(max_id + 1, dim) for values in [0, max_id] and
 default = max_id + 1 for nodes without values, so the table has max_id + 2 rows and the default row is the last one.
@@ -437,3 +438,213 @@ class GenieEncoder(GCNEncoder):
             out, state = self.lstm_cell(x, state)
             outputs.append(out)
         return outputs[0].reshape(tuple(inputs.shape) + (self.dim,))
+
+
+def _exchange_composed(store, grad_store, ids, rows):
+    """ops.store_exchange as the literal composition (any dtype and device): the pre-clear gather, then index_put_ of the
+    ids deduplicated in Python, keeping each id's last occurrence"""
+    taken = grad_store[ids]
+    last = {v: i for i, v in enumerate(ids.tolist())}
+    keys = torch.as_tensor(list(last.keys()), dtype=torch.int64, device=store.device)
+    store.index_put_((keys,), rows.detach()[torch.as_tensor(list(last.values()), dtype=torch.int64, device=store.device)])
+    grad_store.index_put_((keys,), torch.zeros((), dtype=grad_store.dtype, device=grad_store.device))
+    return taken
+
+
+class _ScalableStores(torch.nn.Module):
+    """The per-layer stores of ScalableSageEncoder / ScalableGCNEncoder and the training step over them.
+
+    One step (the order upstream leaves open, fixed here):
+      1. forward(inputs, training=True) samples one hop, encodes the node rows and runs every layer; layer l >= 1 reads its
+         neighbours' rows from stores[l - 1] as they were at the start of the step (a leaf tensor that requires grad).
+      2. After the last layer, one exchange per store: stores[l][node] = node_embeddings[l] (detached, the last occurrence of
+         a repeated node wins), taken_l = gradient_stores[l][node] as it was, then those rows zeroed; store_loss =
+         sum over l of sum(node_embeddings[l] * taken_l).  Reading and clearing before the backward pass means that a node
+         that is also a neighbour in this step keeps the gradient it receives in this step.
+      3. train_step(loss, optimizer) adds d(loss + store_loss) / d(each layer's neighbour store rows) into gradient_stores
+         (every id gets the fixed-order sum of its entries, added with one rounding), computes d loss / d params for
+         `optimizer` and d store_loss / d params for store_optimizer from the same parameters, then steps both.
+    """
+
+    def _init_stores(self, widths, max_id, store_learning_rate, store_init_maxval, generator, device):
+        self.max_id = max_id
+        self.store_learning_rate = store_learning_rate
+        self.store_init_maxval = store_init_maxval
+        self._n_stores = len(widths)
+        for l, w in enumerate(widths):
+            # upstream's tables are LOCAL_VARIABLES, which its Saver does not checkpoint: non-persistent buffers
+            store = torch.empty((max_id + 2, w), device=device).uniform_(0, store_init_maxval, generator=generator)
+            self.register_buffer('store_%d' % l, store, persistent=False)
+            self.register_buffer('gradient_store_%d' % l, torch.zeros((max_id + 2, w), device=device), persistent=False)
+        self.store_optimizer = torch.optim.Adam(self.parameters(), lr=store_learning_rate)
+        self.store_loss = None
+        self._neigh_rows = []
+
+    @property
+    def stores(self):
+        return [getattr(self, 'store_%d' % l) for l in range(self._n_stores)]
+
+    @property
+    def gradient_stores(self):
+        return [getattr(self, 'gradient_store_%d' % l) for l in range(self._n_stores)]
+
+    def _store_rows(self, l, neighbor, count=1, pool=None):
+        """stores[l]'s rows of the neighbours as a leaf that requires grad: pooled over segments of `count` ('sum' or
+        'mean', [n / count, w]) when pool is given, else gathered ([n, w]); recorded for train_step"""
+        store = self.stores[l]
+        with torch.no_grad():
+            if not self.fused:
+                rows = store[neighbor]
+            elif pool is not None:
+                rows = ops.shallow_encode_pool(neighbor, count, id_table=store, pool=pool)
+            else:
+                rows = ops.shallow_encode(neighbor, id_table=store)
+        rows.requires_grad_()
+        self._neigh_rows.append((l, neighbor, rows, count, pool))
+        return rows
+
+    def _exchange(self, node, node_embeddings):
+        """step 2: the stores' exchanges in layer order, and store_loss"""
+        losses = []
+        for store, grad_store, h in zip(self.stores, self.gradient_stores, node_embeddings):
+            if self.fused:
+                taken = ops.store_exchange(store, grad_store, node, h.detach())
+            else:
+                with torch.no_grad():
+                    taken = _exchange_composed(store, grad_store, node, h)
+            losses.append((h * taken).sum())
+        self.store_loss = functools.reduce(torch.add, losses) if losses else torch.zeros((), device=node.device)
+
+    def train_step(self, loss, optimizer):
+        """step 3 for the last forward(training=True): accumulate the neighbour store rows' gradients of loss + store_loss
+        into gradient_stores, then step `optimizer` on d loss and store_optimizer (Adam, store_learning_rate) on
+        d store_loss, both taken from the parameters before either step.  Sparse table gradients (sparse_grad=True) reach
+        store_optimizer densified."""
+        neigh, self._neigh_rows = self._neigh_rows, []
+        params = [p for p in self.parameters() if p.requires_grad]
+        store_grads = [None] * len(params)
+        if self.store_loss.requires_grad:
+            store_grads = torch.autograd.grad(self.store_loss, params, retain_graph=True, allow_unused=True)
+        if neigh:
+            grads = torch.autograd.grad(loss + self.store_loss, [r for _, _, r, _, _ in neigh], retain_graph=True, allow_unused=True)
+            for (l, neighbor, _, count, pool), g in zip(neigh, grads):
+                if g is None:
+                    continue
+                if self.fused:
+                    ops.store_accumulate(self.gradient_stores[l], neighbor, g, count, pool or 'sum')
+                else:
+                    self.gradient_stores[l].index_add_(0, neighbor, g)
+        optimizer.zero_grad()
+        loss.backward()
+        optimizer.step()
+        self.store_optimizer.zero_grad()
+        for p, g in zip(params, store_grads):
+            p.grad = None if g is None else (g.to_dense() if g.is_sparse else g)
+        self.store_optimizer.step()
+
+
+class ScalableSageEncoder(SageEncoder, _ScalableStores):
+    """encoders.ScalableSageEncoder (tf_euler/python/utils/encoders.py:629-748): SageEncoder over metapath [edge_type] *
+    num_layers and fanouts [fanout] * num_layers, trained from ONE hop.  With training=False, forward is SageEncoder's.
+    With training=True it samples sample_fanout(inputs, [edge_type], [fanout], default_node=max_id + 1) once; layer 0
+    aggregates the hop's node-encoder rows, layer l >= 1 the neighbours' rows of stores[l - 1] (f32[max_id + 2, dims[l]],
+    initialised uniform(0, store_init_maxval) from `generator`; gradient_stores alike, zeros).  The step's order and
+    train_step are _ScalableStores'; store_optimizer is torch.optim.Adam(self.parameters(), store_learning_rate).
+
+    fused=True (the default): layer 0 pools the hop through ShallowEncoder.pooled by SageEncoder's rule; layers >= 1 read
+    the stores through ops.shallow_encode_pool(neighbor, fanout, id_table=store) when the aggregator has forward_pooled
+    ('mean', 'gcn'), else ops.shallow_encode and a reshape ('meanpool', 'maxpool'); the exchanges are ops.store_exchange and
+    the accumulations ops.store_accumulate, deterministic.  fused=False is the literal composition: store[ids],
+    index_put_ with the ids deduplicated keep-last, index_add_.
+
+    Differences from upstream:
+      - upstream's __init__ passes shared_node_encoder, use_residual positionally into SageEncoder's use_residual,
+        shared_node_encoder slots, so a shared node encoder is silently ignored there; here both keywords mean what they say.
+      - the stores are initialised from `generator`, not TF's seeded random_uniform_initializer(seed=1) stream.
+      - store_optimizer is torch's Adam, which applies epsilon to sqrt(v_hat), where TF's applies "epsilon hat" to sqrt(v).
+    """
+
+    def __init__(self, edge_type, fanout, num_layers, dim, aggregator='mean', concat=False, shared_aggregators=None,
+                 feature_idx=-1, feature_dim=0, max_id=-1, use_feature=True, use_id=False, sparse_feature_idx=-1,
+                 sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False, shared_node_encoder=None,
+                 use_residual=False, store_learning_rate=0.001, store_init_maxval=0.05, fused=True, sparse_grad=False,
+                 device=None, generator=None):
+        super().__init__([edge_type] * num_layers, [fanout] * num_layers, dim, aggregator, concat, shared_aggregators,
+                         feature_idx, feature_dim, max_id, use_feature, use_id, sparse_feature_idx, sparse_feature_max_id,
+                         embedding_dim, use_hash_embedding, use_residual=use_residual,
+                         shared_node_encoder=shared_node_encoder, fused=fused, sparse_grad=sparse_grad, device=device)
+        self.edge_type = edge_type
+        self.fanout = fanout
+        self._init_stores(self.dims[1:-1], max_id, store_learning_rate, store_init_maxval, generator, device)
+
+    def _pools_store(self, aggregator):
+        return self.fused and hasattr(aggregator, 'forward_pooled') and 1 <= self.fanout <= _lib.SHALLOW_POOL_MAX_COUNT
+
+    def forward(self, inputs, training=False):
+        if not training:
+            return super().forward(inputs)
+        f, L = self.fanout, self.num_layers
+        node, neighbor = ops.sample_fanout(inputs, [self.edge_type], [f], default_node=self.max_id + 1)[0]
+        self._neigh_rows = []
+        a = self.aggregators[0]
+        if self._pools_deepest_hop():
+            h = a.forward_pooled(self.node_encoder(node), self._node_encoder.pooled(neighbor, f, a.pooled_input), f)
+        else:
+            h = a((self.node_encoder(node), self.node_encoder(neighbor).reshape(-1, f, self.dims[0])))
+        node_embeddings = [h]
+        for layer in range(1, L):
+            a = self.aggregators[layer]
+            if self._pools_store(a):
+                h = a.forward_pooled(h, self._store_rows(layer - 1, neighbor, f, a.pooled_input), f)
+            else:
+                h = a((h, self._store_rows(layer - 1, neighbor).reshape(-1, f, self.dims[layer])))
+            node_embeddings.append(h)
+        self._exchange(node, node_embeddings[:-1])
+        return h.reshape(tuple(inputs.shape) + (self.dims[-1],))
+
+
+class ScalableGCNEncoder(GCNEncoder, _ScalableStores):
+    """encoders.ScalableGCNEncoder (tf_euler/python/utils/encoders.py:294-408): GCNEncoder over metapath [edge_type] *
+    num_layers, trained from ONE full hop.  With training=False, forward is GCNEncoder's.  With training=True,
+    (node, neighbor), (adj,) = get_multi_hop_neighbor(inputs, [edge_type]); layer 0 aggregates the node-encoder rows of both,
+    layer l >= 1 the distinct neighbours' rows of stores[l - 1] (f32[max_id + 2, dim], uniform(0, store_init_maxval) from
+    `generator`; gradient_stores alike, zeros), each layer's output plus its input under use_residual.  The step's order and
+    train_step are _ScalableStores'.  fused=True reads the stores through ops.shallow_encode and updates them through
+    ops.store_exchange / ops.store_accumulate, the aggregators taking their own fused paths; fused=False is the literal
+    composition (store[ids], index_put_ keep-last, index_add_).
+
+    Differences from upstream:
+      - an aggregator whose output is stored must be dim wide, the stores' width; 'attention' with dim % head_num != 0 is
+        not, and fails upstream at the first store write: here the constructor raises ValueError.
+      - store initialisation and Adam's epsilon as ScalableSageEncoder's.
+    """
+
+    def __init__(self, edge_type, num_layers, dim, aggregator='mean', feature_idx=-1, feature_dim=0, max_id=-1, use_id=False,
+                 sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
+                 use_residual=False, store_learning_rate=0.001, store_init_maxval=0.05, head_num=4, fused=True,
+                 sparse_grad=False, device=None, generator=None):
+        super().__init__([edge_type] * num_layers, dim, aggregator, feature_idx, feature_dim, max_id, use_id,
+                         sparse_feature_idx, sparse_feature_max_id, embedding_dim, use_hash_embedding, use_residual,
+                         head_num, fused=fused, sparse_grad=sparse_grad, device=device)
+        if any(w != dim for w in self.dims[1:-1]):
+            raise ValueError('the stores are dim = %d wide; the stored layers are %s wide' % (dim, self.dims[1:-1]))
+        self.dim = dim
+        self.edge_type = edge_type
+        self.fused = fused
+        self._init_stores([dim] * (num_layers - 1), max_id, store_learning_rate, store_init_maxval, generator, device)
+
+    def forward(self, inputs, training=False):
+        if not training:
+            return super().forward(inputs)
+        (node, neighbor), (adj,) = ops.get_multi_hop_neighbor(inputs, [self.edge_type])
+        self._neigh_rows = []
+        h, nb = self.node_encoder(node), self.node_encoder(neighbor)
+        node_embeddings = []
+        for layer in range(self.num_layers):
+            out = self.aggregators[layer]((h, nb, adj))
+            h = h + out if self.use_residual else out
+            node_embeddings.append(h)
+            if layer < self.num_layers - 1:
+                nb = self._store_rows(layer, neighbor)
+        self._exchange(node, node_embeddings[:-1])
+        return h.reshape(tuple(inputs.shape) + (self.dims[-1],))

@@ -1294,6 +1294,56 @@ def shallow_encode_pool(nodes, count, id_table=None, dense=(), sparse=(), pool='
     return _ShallowEncodePool.apply(nodes, cfg, int(count), POOLS[pool], id_t, *ts)
 
 
+# ------------------------------------------------------------------------------------ embedding stores
+def _store_table(op, named):
+    """the tables a store op updates in place: float32 2-D, contiguous, on the graph's device"""
+    _check_f32(op, named, 2)
+    for nm, t in named:
+        if not t.is_contiguous() or t.device != _dev():
+            raise EulerError("%s: %s must be contiguous on %s" % (op, nm, _dev()))
+
+
+def store_exchange(store, grad_store, ids, rows):
+    """The store update of ScalableSageEncoder / ScalableGCNEncoder's training step (encoders.py:370-408, 710-748), in place
+    and in one device op, for ids i64[M] (any shape) in [0, n_rows) and rows f32[M, dim]:
+        store[ids[i]] = rows[i]   the LAST occurrence of a repeated id wins
+        taken[i] = grad_store[ids[i]] as it was before the call, for every i; then grad_store[ids[i]] = 0
+    store and grad_store are f32[n_rows, dim].  Returns taken f32[M, dim].  No autograd: rows is read detached.  An id
+    outside the tables raises before either is written (one host synchronisation; none under CUDA-graph capture)."""
+    _store_table("store_exchange", (("store", store), ("grad_store", grad_store)))
+    _check_f32("store_exchange", (("rows", rows),), 2)
+    ids = _t(ids, torch.int64).reshape(-1)
+    n_rows, dim = store.shape
+    if tuple(grad_store.shape) != (n_rows, dim) or tuple(rows.shape) != (ids.numel(), dim):
+        raise EulerError("store_exchange: need store and grad_store [n_rows, dim], rows [M, dim]; got %s, %s, %s for M = %d"
+                         % (tuple(store.shape), tuple(grad_store.shape), tuple(rows.shape), ids.numel()))
+    rows = _t(rows.detach(), torch.float32)
+    taken = torch.empty((ids.numel(), dim), dtype=torch.float32, device=store.device)
+    _call("eu_store_exchange", store, grad_store, n_rows, dim, ids, ids.numel(), rows, taken)
+    return taken
+
+
+def store_accumulate(grad_store, ids, grad, count=1, pool='mean'):
+    """The gradient-store update of ScalableSageEncoder / ScalableGCNEncoder (tf.scatter_add, encoders.py:382-389), in place
+    and in one device op: grad_store[ids[e]] += grad[e // count] (divided by count under pool='mean'), for ids i64[M] (any
+    shape) in [0, n_rows), grad f32[M / count, dim] and grad_store f32[n_rows, dim].  That is the gradient of
+    shallow_encode_pool(ids, count, id_table=store, pool=pool) (count = 1: of shallow_encode(ids, id_table=store)), summed per
+    distinct id in that op's fixed order and added to the stored row with one rounding: deterministic, no atomics.  No
+    autograd.  An id outside the table raises before it is written (one host synchronisation; none under capture)."""
+    if pool not in POOLS:
+        raise EulerError("store_accumulate: pool must be one of %s, got %r" % (sorted(POOLS), pool))
+    _store_table("store_accumulate", (("grad_store", grad_store),))
+    _check_f32("store_accumulate", (("grad", grad),), 2)
+    ids = _t(ids, torch.int64).reshape(-1)
+    n_rows, dim = grad_store.shape
+    count = int(count)
+    if count < 1 or ids.numel() % count or tuple(grad.shape) != (ids.numel() // count, dim):
+        raise EulerError("store_accumulate: need count >= 1 dividing M = %d and grad [M / count, %d]; got count %d, grad %s"
+                         % (ids.numel(), dim, count, tuple(grad.shape)))
+    grad = _t(grad.detach(), torch.float32)
+    _call("eu_store_accumulate", grad_store, n_rows, dim, ids, ids.numel(), count, POOLS[pool], grad)
+
+
 # ------------------------------------------------------------------------------------ graph-level minibatches
 def _labels_from(fn, *args):
     """the label list a two-call entry point reports (counts, then offsets and bytes), as bytes"""

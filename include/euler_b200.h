@@ -829,6 +829,30 @@ int eu_adjacency_mean(eu_ctx* c, const float* x_neigh, int64_t m, const int64_t*
                       int64_t nnz, int32_t dim, float* out);
 int eu_adjacency_mean_backward(eu_ctx* c, const float* grad_out, const int64_t* indptr, const int64_t* cols, int64_t n,
                                int64_t nnz, int64_t m, int32_t dim, float* grad_x);
+/* The per-layer embedding stores of ScalableSageEncoder / ScalableGCNEncoder (tf_euler/python/utils/encoders.py:294-408,
+ * 629-748): a store f32[n_rows, dim] and its gradient store f32[n_rows, dim], updated in place with fixed meanings for
+ * repeated ids.  ids i64[M] must lie in [0, n_rows).
+ * eu_store_exchange: rows f32[M, dim] in, taken f32[M, dim] out:
+ *   store[ids[i]]   = rows[the LAST i with that id]      (tf.scatter_update, whose winner is unspecified upstream)
+ *   taken[i]        = grad_store[ids[i]] as it was before this call, for every i (repeats included)
+ *   grad_store[v]   = 0 for every id v of ids
+ *   The ids are ordered stably and planned once (the id-table gradient path's plan); one lane group per distinct id then
+ *   reads, copies, writes and clears its row: no atomics.  Rows no id names are untouched.
+ * eu_store_accumulate: grad f32[M / count, dim]; count >= 1 divides M; pool EU_POOL_SUM or EU_POOL_MEAN:
+ *   grad_store[v] = __fadd_rn(grad_store[v], S_v),  S_v = sum over the i with ids[i] = v of grad[i / count] (EU_POOL_MEAN:
+ *   each element __fdiv_rn'd by fl(count) as it is read), summed as eu_shallow_encode_pool_backward sums a table gradient
+ *   (stable id order, chunks of 256 from +0, the chunk sums in chunk order); S_v is the gradient of eu_shallow_encode_pool
+ *   over the store as id table (count = 1: of eu_shallow_encode), added to the stored row with one rounding.
+ * Both calls first check the ids (one small kernel, one stream synchronisation): an id outside [0, n_rows) returns
+ * EU_ERR_INVALID before either table is written.  Under CUDA-graph capture the check is skipped and such an id touches no
+ * table row (exchange: its taken row is NaN).  No other synchronisation; ctx scratch O(M) index data (plus M * dim floats
+ * for eu_store_accumulate), never O(n_rows).  M = 0 does nothing.  dim < 1, n_rows < 1, negative M, a bad count or pool or a
+ * NULL pointer that is needed: EU_ERR_INVALID; n_rows of 2^31 - 1 or more, or M ids whose 256-entry chunks reach 2^31:
+ * EU_ERR_UNSUPPORTED.  Device pointers. */
+int eu_store_exchange(eu_ctx* c, float* store, float* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
+                      const float* rows, float* taken);
+int eu_store_accumulate(eu_ctx* c, float* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M, int32_t count,
+                        int32_t pool, const float* grad);
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx,
                    int64_t E, float* out);
 int eu_scatter_add_host(eu_ctx* c, const float* updates, int64_t D, const int32_t* idx, int64_t E,
