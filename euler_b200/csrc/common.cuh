@@ -273,9 +273,8 @@ __device__ __forceinline__ float gt_threshold(double r) {
 // Search over a row slice in global memory; `base` points at the slice, offsets are 32-bit (a row has
 // < 2^31 edges), thr = gt_threshold(r).  Returns the offset in [lo, hi].
 // Invariant: the answer lies in [lo, hi]; hi is the clamp or an offset with base[hi] >= thr.
-// 8-ary descent: 7 independent probes per round trip.  The rows that land here are hubs (a hop-2 frontier is
-// degree-biased) whose slices live in L2; a profile of the kernel shows it stalled on exactly this
-// load-compare chain, with issue slots to spare for the extra probes.
+// 8-ary descent: 7 independent probes per round trip, for a search whose round trips are its cost.  Where the loads
+// themselves are (the fanout sampler's deep hop), sample.cu bisects instead: same answer, a seventh of the probes per round.
 __device__ __forceinline__ int32_t upper_bound_clamped(const float* __restrict__ base, int32_t lo, int32_t hi,
                                                        float thr) {
   while (hi - lo >= 8) {

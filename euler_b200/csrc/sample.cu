@@ -355,9 +355,22 @@ __device__ __forceinline__ int lane_upper_bound(float c, int lo, int hi, float t
   return lo;
 }
 
+// First offset in [lo, hi] with base[offset] >= thr, else hi: the answer of upper_bound_clamped (common.cuh), found by
+// bisection.  k_sample's rows that are neither lane-resident nor staged search this way.  At the fanout's deep hop those
+// are most of the rows that draw (57 % at the headline shape, median 1.3 K edges).  There the launch is bound by its loads,
+// not by their round trips: every row class takes about the same time per row, and a fuller grid is slower.  Bisection
+// issues 2.4x fewer probes than the 8-ary descent, and the launch is 6 % faster with it (DESIGN §3.1).
+__device__ __forceinline__ int32_t bisect_clamped(const float* __restrict__ base, int32_t lo, int32_t hi, float thr) {
+  while (lo < hi) {
+    const int32_t mid = (lo + hi) >> 1;
+    if (__ldg(base + mid) >= thr) hi = mid; else lo = mid + 1;
+  }
+  return lo;
+}
+
 // One lane GROUP (SG lanes, SG = 2^k >= min(count, 32)) per sampling row, one lane per draw; a warp carries 32/SG
 // rows, and a persistent grid strides over the live rows: with fanout 10 two rows share a warp (the kernel is
-// issue-bound: every instruction a lane group spares is throughput), and the per-block set-up
+// throughput-bound: a row's time does not depend on its length class, see bisect_clamped), and the per-block set-up
 // (jump tables, table wipe, parameter loads) is paid once per CTA instead of once per 8 rows.
 template <bool PHILOX, int CTAS>
 __global__ void __launch_bounds__(256, CTAS) k_sample(DevGraph g, SampleArgs a) {
@@ -368,7 +381,7 @@ __global__ void __launch_bounds__(256, CTAS) k_sample(DevGraph g, SampleArgs a) 
   // TMA-staged adjacency tiles: a row longer than the group's lanes but of at most kStageF * SG cumulative weights is copied
   // into the group's slice of shared memory by ONE cp.async.bulk (the elected lane issues it right after the row bounds are
   // known and the whole group goes on to derive its engine states; the draws then wait on the slice's mbarrier), and every
-  // inverse-CDF search of that row is a shared-memory binary search instead of an 8-ary descent through L2.
+  // inverse-CDF search of that row is a shared-memory binary search instead of a bisection through L2.
   constexpr int kStageF = 16;
   __shared__ __align__(128) float s_stage[256 * kStageF];
   __shared__ __align__(8) unsigned long long s_bar[32];
@@ -559,7 +572,7 @@ __global__ void __launch_bounds__(256, CTAS) k_sample(DevGraph g, SampleArgs a) 
         m = base + lo;
         wgt = __fsub_rn(srow[lo], lo > 0 ? srow[lo - 1] : 0.f);
       } else {
-        m = b + upper_bound_clamped(g.cum_w + b, 0, (int32_t)(e - b), thr);
+        m = b + bisect_clamped(g.cum_w + b, 0, (int32_t)(e - b), thr);
         float hi_v = __ldg(g.cum_w + m);
         float lo_v = m > base ? __ldg(g.cum_w + m - 1) : 0.f;
         wgt = __fsub_rn(hi_v, lo_v);
@@ -779,12 +792,14 @@ int hop(eu_ctx* c, const unsigned long long* seeds, int64_t rows_b, const int32_
     a.sg_log = 0;
     while ((1 << a.sg_log) < need) ++a.sg_log;
   }
-  // persistent grid: 8 CTAs per SM stride over the (live) rows.  EU_SAMPLE_CTAS = CTAs per SM (1..8; 6 also relaxes the
-  // register cap); read once (C++11 static initialisation is thread-safe: the ABI is re-entrant across ctxs)
+  // persistent grid: 8 CTAs per SM stride over the (live) rows.  EU_SAMPLE_CTAS = CTAs per SM (1..8); read once (C++11 static
+  // initialisation is thread-safe: the ABI is re-entrant across ctxs).  The minstd kernel is compiled for the occupancy the grid
+  // asks for: 32 registers at 7-8 CTAs per SM, 40 at 6, 48 at 5 or fewer.  The kernel spills at every one of these caps, and
+  // each step up removes some of its local-memory traffic.  The philox kernel keeps the 32- and 40-register builds.
   static const int stage_rows = [] { const char* e = getenv("EU_SAMPLE_STAGE"); return e ? (atoi(e) != 0 ? 1 : 0) : 1; }();
   a.stage = stage_rows;
   static const int grid_ctas = [] { const char* e = getenv("EU_SAMPLE_CTAS"); return e ? std::min(8, std::max(1, atoi(e))) : 8; }();
-  const int ctas = grid_ctas == 6 ? 6 : 8;
+  const int ctas = grid_ctas <= 5 ? 5 : grid_ctas == 6 ? 6 : 8;
   const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(ceil_div(rows * 32, (int64_t)(32 >> a.sg_log)), 256), kSMs * grid_ctas);
   if (c->rng == EU_RNG_PHILOX) {
     a.key = c->seed;
@@ -839,7 +854,10 @@ int hop(eu_ctx* c, const unsigned long long* seeds, int64_t rows_b, const int32_
     a.next_tabs = ntabs;
     a.next_cap_b = ng.cap_b;
   }
-  { EuProfScope ps(c, "k_sample<minstd>", rows); if (ctas == 6) k_sample<false, 6><<<blocks, 256, 0, s>>>(d, a); else k_sample<false, 8><<<blocks, 256, 0, s>>>(d, a); }
+  { EuProfScope ps(c, "k_sample<minstd>", rows);
+    if (ctas == 5) k_sample<false, 5><<<blocks, 256, 0, s>>>(d, a);
+    else if (ctas == 6) k_sample<false, 6><<<blocks, 256, 0, s>>>(d, a);
+    else k_sample<false, 8><<<blocks, 256, 0, s>>>(d, a); }
   EU_LAUNCHED();
   if (!raw && rows >= kRepeatMinRows) {
     EuProfScope ps(c, "k_copy_dups", rows);
