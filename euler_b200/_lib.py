@@ -53,6 +53,7 @@ class KgProblem(C.Structure):
 SHALLOW_MAX_SLOTS = 8   # EU_SHALLOW_MAX_SLOTS
 SHALLOW_MAX_WIDTH = 16384   # EU_SHALLOW_MAX_WIDTH
 SHALLOW_POOL_MAX_COUNT = 512   # EU_SHALLOW_POOL_MAX_COUNT
+NEIGHBOR_TOP_K_MAX = 16   # EU_NEIGHBOR_TOP_K_MAX
 
 
 class ShallowDense(C.Structure):
@@ -153,6 +154,7 @@ SIGNATURES = {
     "eu_random_walk_host": (C.c_int, [_P, _P, _I64, _P, _I32, _I32, _F, _F, _I64, _P]),
     "eu_get_dense_feature": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
     "eu_get_dense_feature_host": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
+    "eu_neighbor_top_k_feature": (C.c_int, [_P, _P, _I64, _P, _I32, _I32, _I32, _I32, _P]),
     "eu_get_full_neighbor": (C.c_int, [_P, _P, _I64, _P, _I32, _I64, _P, _P, _P, _P]),
     "eu_unique": (C.c_int, [_P, _P, _I64, _P, _P, _P]),
     "eu_full_neighbor_hop": (C.c_int, [_P, _P, _I64, _P, _I32, _I32, _I64, _P, _P, _P, _P, _P, _P, _P, _P]),

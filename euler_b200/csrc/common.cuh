@@ -109,6 +109,14 @@ __device__ __forceinline__ int64_t lookup_row(const DevGraph& g, unsigned long l
   }
 }
 
+// Dense slot `fid`'s columns of a feature row: [*off, *off + *width).  An unknown slot has none, so every fetch of it reads
+// zeros (Node::GetFloat32Feature skips it, node.cc:353-364; api.cc:71-73).
+__host__ __device__ __forceinline__ void dense_slot(const DevGraph& g, int32_t fid, int32_t* off, int32_t* width) {
+  const bool have = fid >= 0 && fid < g.n_slots;
+  *off = have ? g.slot_off[fid] : 0;
+  *width = have ? g.slot_dim[fid] : 0;
+}
+
 // Row `row`'s slice of ragged slot `fid` (ptr of S slots per row): [b, e) in the value array, b == e when the node / slot does
 // not exist
 __device__ __forceinline__ void ragged_slice(const int64_t* __restrict__ ptr, int32_t S, int64_t row, int32_t fid, int64_t* b, int64_t* e) {

@@ -5,7 +5,8 @@ embeddings, concatenated or added.  And SageEncoder / ShuffleSageEncoder (encode
 sample_fanout's sample tree with that input layer and the aggregators of aggregators.py.  And GCNEncoder / GenieEncoder
 (encoders.py:174-291), the full-neighbourhood encoders over get_multi_hop_neighbor's hops and the aggregators of
 sparse_aggregators.py.  And ScalableSageEncoder / ScalableGCNEncoder (encoders.py:294-408, 629-748), which train every layer
-from one hop over per-layer embedding stores (_ScalableStores).
+from one hop over per-layer embedding stores (_ScalableStores).  And LGCEncoder (encoders.py:872-922), LGCN's convolutions over
+each node's row and the k largest values of every feature column among its sampled neighbours.
 
 Callers size the table as the encoders do: SparseEmbedding(max_id + 1, dim) for values in [0, max_id] and
 default = max_id + 1 for nodes without values, so the table has max_id + 2 rows and the default row is the last one.
@@ -648,3 +649,65 @@ class ScalableGCNEncoder(GCNEncoder, _ScalableStores):
                 nb = self._store_rows(layer, neighbor)
         self._exchange(node, node_embeddings[:-1])
         return h.reshape(tuple(inputs.shape) + (self.dims[-1],))
+
+
+class LGCEncoder(torch.nn.Module):
+    """encoders.LGCEncoder (tf_euler/python/utils/encoders.py:872-922), "Large-Scale Learnable Graph Convolutional Networks"
+    (https://arxiv.org/pdf/1808.03965.pdf), with upstream's constructor arguments.  __call__(inputs) takes node ids of any
+    shape, flattened to [B], and returns f32[B, out_dim]:
+        1. neighbors = sample_neighbor(inputs, edge_type, nb_num), default_node -1
+        2. x = [the node's feature row; for every column, the k largest of that column over the nb_num neighbours'
+           rows, descending] -- f32[B, k + 1, feature_dim], slot feature_idx (an absent neighbour's row is zeros)
+        3. two tf.layers.conv1d over the k + 1 rows (channels last upstream, transposed for torch.nn.Conv1d): kernel size
+           k // 2 + 1, 'valid' padding, a bias, no activation; feature_dim -> hidden_dim -> out_dim, glorot-uniform kernels
+           and zero biases (TF's defaults); being torch's Conv1d they follow torch.backends.cudnn.allow_tf32 (on by
+           default, so TF32 products on an H100)
+        4. output row 0
+    fused=True (the default) builds x in one device op, ops.neighbor_top_k_feature, without the [B, nb_num, feature_dim]
+    neighbour rows; fused=False is the literal composition: two get_dense_feature calls, then cat, transpose and torch.topk.
+    The two give the same x, except where +0.0 and -0.0 tie: the op keeps the lower neighbour index first (tf.nn.top_k's
+    rule), torch.topk leaves the order of equal values open.  No gradient flows into x (graph data, as upstream).
+
+    Upstream quirks kept: for odd k the two valid convolutions read only rows 0 .. 2 (k // 2) of x, so the k-th largest
+    value never reaches the output (it is still selected); upstream's unused concat of the node and all neighbour rows
+    (`nbs`) is dropped.  feature_idx=-1, upstream's default, would ask get_dense_feature for slot -1, and a k outside
+    [1, nb_num] fails in tf.nn.top_k at run time: both raise ValueError at construction here."""
+
+    def __init__(self, edge_type=[0], feature_idx=-1, feature_dim=0, k=3, hidden_dim=128, nb_num=10, out_dim=64, fused=True,
+                 device=None):
+        super().__init__()
+        if feature_idx == -1:
+            raise ValueError('LGCEncoder needs a dense feature slot: feature_idx is -1')
+        if not 1 <= k <= nb_num:
+            raise ValueError('k must lie in [1, nb_num = %d], got %d' % (nb_num, k))
+        self.edge_type = edge_type
+        self.feature_idx = feature_idx
+        self.feature_dim = feature_dim
+        self.k = k
+        self.hidden_dim = hidden_dim
+        self.out_dim = out_dim
+        self.nb_num = nb_num
+        self.fused = fused
+        width = k // 2 + 1
+        self.conv1 = torch.nn.Conv1d(feature_dim, hidden_dim, width, device=device)
+        self.conv2 = torch.nn.Conv1d(hidden_dim, out_dim, width, device=device)
+        for conv in (self.conv1, self.conv2):
+            torch.nn.init.xavier_uniform_(conv.weight)    # TF's glorot: fans width * in and width * out, as torch counts them
+            torch.nn.init.zeros_(conv.bias)
+
+    def top_k_rows(self, nodes, neighbors):
+        """x of step 2, f32[B, k + 1, feature_dim], from the flat node ids and their neighbours i64[B, nb_num]"""
+        if self.fused:
+            return ops.neighbor_top_k_feature(nodes, neighbors, self.feature_idx, self.feature_dim, self.k)
+        node_feats, = ops.get_dense_feature(nodes, [self.feature_idx], [self.feature_dim])
+        neighbor_feats, = ops.get_dense_feature(neighbors.reshape(-1), [self.feature_idx], [self.feature_dim])
+        neighbor_feats = neighbor_feats.reshape(-1, self.nb_num, self.feature_dim)
+        topk = torch.topk(neighbor_feats.transpose(1, 2), self.k)[0].transpose(1, 2)
+        return torch.cat([node_feats.reshape(-1, 1, self.feature_dim), topk], 1)
+
+    def forward(self, inputs):
+        nodes = inputs.reshape(-1)
+        neighbors = ops.sample_neighbor(nodes, self.edge_type, self.nb_num)[0]
+        x = self.top_k_rows(nodes, neighbors)
+        out = self.conv2(self.conv1(x.transpose(1, 2)))
+        return out[:, :, 0]

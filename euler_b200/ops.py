@@ -336,6 +336,26 @@ def get_dense_feature(nodes, feature_names, dimensions, thread_num=1):
     return outs
 
 
+def neighbor_top_k_feature(nodes, neighbors, feature_name, dimension, k):
+    """LGCEncoder's input block (encoders.py:895-922) in one device op: nodes i64 of any shape (flattened to [B]), neighbors
+    i64[B, count] (sample_neighbor's rows), the dense slot feature_name (a name, or an int slot id) read dimension columns
+    wide.  Returns f32[B, k + 1, dimension]: row 0 is get_dense_feature(nodes), rows 1 .. k the k largest values of each
+    column over the node's neighbours, descending; equal values keep the lower neighbour index first (tf.nn.top_k's rule),
+    NaN ranks above every number.  It equals cat(get_dense_feature(nodes), the first k rows of a stable descending sort of
+    get_dense_feature(neighbors) per column) to the bit.  No gradient (the rows are graph data).  1 <= k <= count and
+    k <= NEIGHBOR_TOP_K_MAX (16), or EulerError."""
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    neighbors = _t(neighbors, torch.int64)
+    B = nodes.numel()
+    if neighbors.dim() != 2 or neighbors.shape[0] != B:
+        raise EulerError("neighbor_top_k_feature: neighbors must be [B, count] for B = %d nodes, got %s" % (B, tuple(neighbors.shape)))
+    k, dim = int(k), int(dimension)
+    out = torch.empty((B, max(k, 0) + 1, max(dim, 0)), dtype=torch.float32, device=nodes.device)   # bad sizes: the library refuses
+    _call("eu_neighbor_top_k_feature", nodes, B, neighbors, neighbors.shape[1], _slot(feature_name, get_graph().dense_feature_id),
+          dim, k, out)
+    return out
+
+
 def _values_i64(total):
     return (torch.empty(total, dtype=torch.int64, device=_dev()),)
 

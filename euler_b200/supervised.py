@@ -66,3 +66,18 @@ class GeniePath(SuperviseModel):
 
     def embed(self, n_id):
         return self._encoder(n_id)
+
+
+class LGCN(SuperviseModel):
+    """examples/lgcn/lgcn.py:26-37: SuperviseModel over LGCEncoder(metapath, feature_idx, feature_dim, k, dim, nb_num,
+    out_dim) -- dim is the encoder's hidden_dim and metapath its edge_type list.  The embedding is out_dim wide, so out_fc
+    reads out_dim columns.  fused and device are passed to the encoder."""
+
+    def __init__(self, dim, metapath, label_idx, label_dim, feature_idx=-1, feature_dim=0, k=3, nb_num=10, out_dim=64,
+                 metric_name='f1', fused=True, device=None):
+        from .encoders import LGCEncoder
+        super().__init__(label_idx, label_dim, metric_name, dim=out_dim, device=device)
+        self._encoder = LGCEncoder(metapath, feature_idx, feature_dim, k, dim, nb_num, out_dim, fused=fused, device=device)
+
+    def embed(self, n_id):
+        return self._encoder(n_id)

@@ -264,6 +264,22 @@ int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid
                          float* out);
 int eu_get_dense_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim,
                               float* out);
+/* LGCEncoder's input block (tf_euler/python/utils/encoders.py:895-922, "Large-Scale Learnable Graph Convolutional
+ * Networks"), fused from the ids: nodes i64[B], neighbors i64[B, count] (sample_neighbor's rows), out f32[B, k + 1, dim]:
+ *   out[b, 0, :]      = eu_get_dense_feature(nodes[b], fid, dim) exactly (zeros past the slot's stored width, clipped before
+ *                       it, a zero row for an absent id or an unknown slot)
+ *   out[b, 1 + j, d]  = for j < k, the j-th largest of the count values feature(neighbors[b, i])[d], each read under the same
+ *                       rule (an absent neighbour, such as sample_neighbor's -1, gives 0.0), in descending order.
+ * Ties: equal values keep the lower neighbour index first, tf.nn.top_k's rule (TF's TopKV2), so +0.0 / -0.0 ties are
+ * determined to the bit; NaN ranks above every number (torch.sort's order), NaNs among themselves by index.  The result is
+ * bit-exact against a stable descending sort of the fetched rows.  No [B, count, dim] intermediate; no host
+ * synchronisation and no scratch: capturable in a CUDA graph.  No backward pass (the input is graph data).
+ * k < 1 or k > count (tf.nn.top_k refuses k above the row length): EU_ERR_INVALID; k above EU_NEIGHBOR_TOP_K_MAX (each
+ * column's k candidates are held in registers): EU_ERR_UNSUPPORTED.  Negative B or dim, or a NULL pointer that is needed:
+ * EU_ERR_INVALID.  out is not written on any refusal; B = 0 or dim = 0 does nothing.  Device pointers. */
+#define EU_NEIGHBOR_TOP_K_MAX 16
+int eu_neighbor_top_k_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_t* neighbors, int32_t count, int32_t fid,
+                              int32_t dim, int32_t k, float* out);
 /* tf_euler.get_sparse_feature, one feature (tf_euler/kernels/get_sparse_feature_op.cc:52-130 over Node::GetUint64Feature
  * node.cc:366-379): the uint64 values of slot `fid` for every node, CSR-style: node i owns out_values[out_ptr[i], out_ptr[i+1]).
  * A node without values (absent node, unknown slot, empty slot) owns exactly ONE entry = default_value (the kernel's
