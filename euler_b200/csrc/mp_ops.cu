@@ -12,7 +12,11 @@
 //   sorted indices (what SageDataFlow / fixed-fanout blocks produce, sage_dataflow.py:43-46):
 //     warp per OUTPUT row, its edges found by binary search, accumulated left to right -> the
 //     reference's summation order, bit-exact, no atomics;
-//   unsorted indices: vector atomics (red.global.add.v4.f32), order-free, within 1e-5 relative.
+//   unsorted indices: vector atomics (red.global.add.v4.f32), order-free, within 1e-5 relative.  The f32 atomic add flushes
+//     subnormal inputs and results to zero (PTX atom / red .add.f32), which adds an absolute error below 2 * 2^-126 per
+//     update: a sum that is itself subnormal can come back as zero.  max is exact there too, but
+//     order-free: among equal zeros +0.0 wins (the reference keeps whichever of +0.0 / -0.0 comes first); -0.0 still beats
+//     every negative value.  NaN never wins and values at or below -1e9 leave the initial -1e9, on both paths.
 #include <stdlib.h>
 
 #include <cooperative_groups.h>
@@ -133,9 +137,11 @@ __global__ void k_fill_if(float* __restrict__ out, int64_t n, float v, const int
 }
 
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {
-  // total order trick: non-negative floats compare like signed ints, negative like reversed unsigned
+  // total order trick: floats with the sign bit clear compare like signed ints, with it set like reversed unsigned.  The branch
+  // is chosen on the sign bit, not on v >= 0 (true for -0.0, whose int bits INT_MIN would then never win): -0.0 beats every
+  // negative value and loses to +0.0.
   if (v != v) return;  // NaN never wins `upd > out`
-  if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+  if (__float_as_int(v) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
   else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 

@@ -643,7 +643,10 @@ def unique(ids):
 
 def sage_mean_aggregate(neighbor_ids, count, dim):
     """Fused get_dense_feature + scatter_mean for fixed-fanout blocks (SAGEConv's neighbor mean,
-    tf_euler/python/convolution/sage_conv.py:33-38 over sage_dataflow.py:43-46 blocks)."""
+    tf_euler/python/convolution/sage_conv.py:33-38 over sage_dataflow.py:43-46 blocks).  Each neighbor contributes columns
+    [0, min(dim, feat_dim)) of its whole stored feature row (every slot, concatenated), zeros beyond, and an id not in the
+    graph contributes zeros.  That equals get_dense_feature(neighbor_ids, [0], [dim]) followed by scatter_mean only when the
+    graph has one dense slot or dim <= slot 0's width."""
     ids = _t(neighbor_ids, torch.int64).reshape(-1)
     rows = ids.numel() // int(count)
     out = torch.empty((rows, int(dim)), dtype=torch.float32, device=ids.device)
@@ -740,12 +743,16 @@ def gather(params, indices):
 
 
 def scatter_add(updates, indices, size=None):
-    """mp_ops.scatter_add = MPScatterAdd (mp_ops.py:28)."""
+    """mp_ops.scatter_add = MPScatterAdd (mp_ops.py:28).  Bit for bit the reference's sums on a non-decreasing index; on any
+    other index the sums are order-free float atomics, which flush subnormal updates and partial sums to zero."""
     return _ScatterAdd.apply(_f32(updates), _t(indices, torch.int32).reshape(-1), int(size))
 
 
 def scatter_max(updates, indices, size=None):
-    """mp_ops.scatter_max = MPScatterMax (mp_ops.py:29); output initialised to -1e9."""
+    """mp_ops.scatter_max = MPScatterMax (mp_ops.py:29); output initialised to -1e9 and raised by strict `upd > out`: NaN never
+    wins and values at or below -1e9 leave -1e9.  Bit for bit the reference's result on a non-decreasing index; on any other
+    index too, except among equal zeros, where +0.0 wins over -0.0 in any order (the reference keeps the first of them).
+    -0.0 beats every negative value on both paths."""
     return _ScatterMax.apply(_f32(updates), _t(indices, torch.int32).reshape(-1), int(size))
 
 
