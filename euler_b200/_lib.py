@@ -178,6 +178,9 @@ SIGNATURES = {
     "eu_dna_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P, _P]),
     "eu_adjacency_mean": (C.c_int, [_P, _P, _I64, _P, _P, _I64, _I64, _I32, _P]),
     "eu_adjacency_mean_backward": (C.c_int, [_P, _P, _P, _P, _I64, _I64, _I64, _I32, _P]),
+    "eu_graph_adjacency": (C.c_int, [_P, _P, _I32, _P, _I64, _I64, _I64, _I64, _P, _P, _P, _P, _P]),
+    "eu_graph_node_ids": (C.c_int, [_P, _P]),
+    "eu_graph_node_rows": (C.c_int, [_P, _P, _I64, _P]),
     "eu_sparse_embedding_lookup": (C.c_int, [_P, _P, _I64, _I32, _I64, _P, _I64, _I32, _I32, _P]),
     "eu_sparse_embedding_lookup_backward": (C.c_int, [_P, _P, _P, _I64, _I32, _I64, _I64, _I32, _I32, _P]),
     "eu_sparse_embedding_lookup_backward_sparse": (C.c_int, [_P, _P, _P, _I64, _I32, _I64, _I64, _I32, _I32, _P, _P, _P]),

@@ -109,6 +109,15 @@ __device__ __forceinline__ int64_t lookup_row(const DevGraph& g, unsigned long l
   }
 }
 
+// the row i of listed entry e: the last i in [lo, hi] with ptr[i] <= e (rows before it may be empty)
+__device__ __forceinline__ int64_t hop_row_of(const long long* __restrict__ ptr, int64_t lo, int64_t hi, int64_t e) {
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (ptr[mid] <= e) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
 // Dense slot `fid`'s columns of a feature row: [*off, *off + *width).  An unknown slot has none, so every fetch of it reads
 // zeros (Node::GetFloat32Feature skips it, node.cc:353-364; api.cc:71-73).
 __host__ __device__ __forceinline__ void dense_slot(const DevGraph& g, int32_t fid, int32_t* off, int32_t* width) {

@@ -28,15 +28,6 @@ static constexpr int kHopThreads = 256;
 static constexpr int kHopPerThread = 4;
 static constexpr int kHopTile = kHopThreads * kHopPerThread;   // entries per CTA tile
 
-// the row i of listed entry e: the last i in [lo, hi] with ptr[i] <= e (rows before it may be empty)
-__device__ __forceinline__ int64_t hop_row_of(const long long* __restrict__ ptr, int64_t lo, int64_t hi, int64_t e) {
-  while (lo < hi) {
-    const int64_t mid = (lo + hi + 1) >> 1;
-    if (ptr[mid] <= e) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 // V = E (+ n when the frontier is appended) virtual items; items [0, E) are the listing, [E, V) the frontier
 __global__ void __launch_bounds__(kHopThreads) k_hop_fill(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t n,
                                                           ETList et, const long long* __restrict__ ptr, int64_t E, int64_t V,

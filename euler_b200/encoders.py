@@ -16,6 +16,7 @@ Upstream quirk: ShallowEncoder's use_hash_embedding=True names layers.HashEmbedd
 """
 import functools
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -403,6 +404,135 @@ class GCNEncoder(torch.nn.Module):
         out = self._layers([self.node_encoder(node) for node in nodes], adjs)
         return out.reshape(tuple(inputs.shape) + (self.dims[-1],))
 
+    @torch.no_grad()
+    def infer(self, ids=None, chunk_rows=1 << 20):
+        """forward(ids) for many ids at once, computed layer by layer over the whole graph: f32[len(ids), dims[-1]], or
+        every node in engine-row order (ops.graph_node_ids()) when ids is None.  The encoder draws nothing, so a node's
+        layer-l value depends only on its neighbours' layer-(l-1) values and each layer is one pass over the graph's edges
+        (ops.graph_adjacency) instead of one L-hop neighbourhood per batch.  Equals forward(ids) up to float rounding (the
+        neighbour sums run in listing order, forward's in its column order; the GEMMs have other shapes).  An id that is
+        not a node is encoded as forward encodes it: its node-encoder row, then every layer with no neighbours.
+
+        The plan (infer_plan) keeps, per layer below the last, one table of every node for each distinct metapath window;
+        the last layer runs at hop 0 on the requested rows only.  Peak memory is the node-encoder table, the tables of two
+        consecutive layers, the metapath's adjacencies (12 B per listed entry) and one chunk of chunk_rows rows: f32 tables
+        of 128 columns over 10M nodes are 5.1 GB each.  chunk_rows does not change the result's bits."""
+        return self._infer(ids, chunk_rows)
+
+    def _infer(self, ids, chunk_rows, each_layer=None):
+        """infer's device inputs: the metapath's whole-graph adjacencies, the requested rows and the node-encoder table over
+        every node and every absent id, all with one column numbering; then _infer_layers"""
+        if chunk_rows < 1:
+            raise ValueError('chunk_rows must be at least 1, got %d' % chunk_rows)
+        L, n = self.num_layers, ops.get_graph().num_nodes
+        hops = [_hop_key(t) for t in self.metapath]
+        built = {}
+        for h in (range(L) if L > 1 else []):
+            if hops[h] not in built:
+                built[hops[h]] = ops.graph_adjacency(self.metapath[h])
+        if ids is None:
+            if hops[0] not in built:
+                built[hops[0]] = ops.graph_adjacency(self.metapath[0])
+            final, absent_ids = built[hops[0]], []
+        else:
+            ids = ops._t(ids, torch.int64).reshape(-1)
+            rows = ops.graph_node_rows(ids)
+            final = ops.graph_adjacency(self.metapath[0], rows=rows)
+            absent_ids = [ids[rows < 0]]
+        # one numbering for every table: the n engine rows, then the distinct absent ids (none on most graphs)
+        absent = torch.unique(torch.cat([a[3] for a in list(built.values()) + [final]] + absent_ids))
+        N = n + absent.numel()
+
+        def renumber(adj, n_rows):
+            indptr, cols, _, extra = adj
+            if extra.numel():
+                mapped = n + torch.searchsorted(absent, extra)
+                cols = torch.where(cols < n, cols, mapped[(cols - n).clamp(min=0)])
+            if n_rows > indptr.numel() - 1:   # absent ids list nothing
+                indptr = torch.cat([indptr, indptr[-1:].expand(n_rows - indptr.numel() + 1)])
+            return indptr, cols
+
+        adjs = {key: renumber(adj, N) for key, adj in built.items()}
+        if ids is None:
+            final, self_cols = adjs[hops[0]], None
+            final = (final[0][:n + 1], final[1])
+        else:
+            final = renumber(final, 0)
+            self_cols = torch.where(rows >= 0, rows, n + torch.searchsorted(absent, ids))
+        node_ids = torch.cat([ops.graph_node_ids(), absent])
+        table = None
+        for a in range(0, N, chunk_rows):
+            rows_a = self.node_encoder(node_ids[a:a + chunk_rows])
+            if table is None:
+                table = rows_a.new_empty((N, rows_a.shape[1]))
+            table[a:a + rows_a.shape[0]] = rows_a
+        return self._infer_layers(table, [adjs.get(k) for k in hops], final, self_cols, chunk_rows, each_layer)
+
+    def _infer_layers(self, table, adjs, final, self_cols, chunk_rows, each_layer=None):
+        """infer's layer / hop plan over the node-encoder table [N, dims[0]] (row r = column r of the adjacencies):
+        adjs[h] = (indptr i64[N+1], cols) of metapath hop h over all N rows (used when L > 1), final = (indptr i64[B+1], cols)
+        of hop 0 at the B requested rows, whose own rows are self_cols (None: rows 0 .. B-1).  each_layer(layer, rows) gets
+        the requested rows' hop-0 values before layer 0 (layer = -1) and after every layer.  Plain torch around the
+        aggregators: with fused=False it runs on CPU tensors and in float64."""
+        L = self.num_layers
+        hops = [_hop_key(t) for t in self.metapath]
+        B = final[0].numel() - 1
+
+        def at_requested(t):
+            return t[:B] if self_cols is None else t[self_cols]
+
+        tables = {(): table}   # metapath window -> the table of every row at the hops of that window
+        if each_layer:
+            each_layer(-1, at_requested(table))
+        for layer, plan in enumerate(infer_plan(self.metapath)):
+            tables = {win: self._infer_layer(layer, tables[win[:-1]], tables[win[1:]], adjs[h[0]], None, chunk_rows)
+                      for win, h in plan.items()}
+            if each_layer:
+                each_layer(layer, at_requested(tables[tuple(hops[:layer + 1])]))
+        out = self._infer_layer(L - 1, tables[tuple(hops[:L - 1])], tables[tuple(hops[1:])], final, self_cols, chunk_rows)
+        if each_layer:
+            each_layer(L - 1, out)
+        return out
+
+    def _infer_layer(self, layer, self_table, neigh_table, adj, self_cols, chunk_rows):
+        """aggregator `layer` (and the residual) at every row of adj, chunk_rows rows at a time; row i's own row is
+        self_table[self_cols[i]] (self_cols None: self_table[i])"""
+        indptr, cols = adj
+        R = indptr.numel() - 1
+        starts = list(range(0, R, chunk_rows)) + [R]
+        offs = indptr[torch.as_tensor(starts, device=indptr.device)].tolist()
+        out = None
+        for a, b, oa, ob in zip(starts[:-1], starts[1:], offs[:-1], offs[1:]):
+            own = self_table[a:b] if self_cols is None else self_table[self_cols[a:b]]
+            h = self.aggregators[layer]((own, neigh_table, (indptr[a:b + 1] - oa, cols[oa:ob])))
+            h = own + h if self.use_residual else h
+            if out is None:
+                out = h.new_empty((R, h.shape[1]))
+            out[a:b] = h
+        return out if out is not None else self_table.new_empty((0, self.dims[layer + 1]))
+
+
+def _hop_key(types):
+    """one metapath hop's edge-type list as a hashable key (the order is kept: it is the listing order)"""
+    return tuple((types.reshape(-1) if torch.is_tensor(types) else np.asarray(types).reshape(-1)).tolist())
+
+
+def infer_plan(metapath):
+    """The tables GCNEncoder.infer builds for a metapath of L hops: per layer l < L - 1, {window: hops}, one table per
+    distinct window.  Layer l's table at hop h (h = 0 .. L-1-l) is built from layer l-1's tables at hops h and h + 1 over
+    metapath[h] (layer -1's is the node-encoder table, window ()), so it depends on metapath[h .. h+l]: its window is those
+    type lists, and hops whose windows are equal share one table.  The last layer runs at hop 0 only, at the requested
+    rows, so it has no table here."""
+    L = len(metapath)
+    keys = [_hop_key(t) for t in metapath]
+    plan = []
+    for layer in range(L - 1):
+        tables = {}
+        for h in range(L - layer):
+            tables.setdefault(tuple(keys[h:h + layer + 1]), []).append(h)
+        plan.append(tables)
+    return plan
+
 
 class GenieEncoder(GCNEncoder):
     """encoders.GenieEncoder (encoders.py:236-291), GeniePath's encoder: GCNEncoder's layers ('attention' by default), then
@@ -433,12 +563,25 @@ class GenieEncoder(GCNEncoder):
         hidden = [self.node_encoder(node) for node in nodes]
         h_t = [self.depth_fc[0](hidden[0])]
         self._layers(hidden, adjs, lambda layer, h: h_t.append(self.depth_fc[layer + 1](h)))
+        return self._steps(h_t).reshape(tuple(inputs.shape) + (self.dim,))
+
+    def _steps(self, h_t):
+        """the LSTM over the L + 1 depth_fc outputs from a zero state; upstream's output at the first step"""
         zero = h_t[0].new_zeros((h_t[0].shape[0], self.dim))
         state, outputs = (zero, zero), []
         for x in h_t:
             out, state = self.lstm_cell(x, state)
             outputs.append(out)
-        return outputs[0].reshape(tuple(inputs.shape) + (self.dim,))
+        return outputs[0]
+
+    @torch.no_grad()
+    def infer(self, ids=None, chunk_rows=1 << 20):
+        """forward(ids) computed layer by layer over the whole graph, as GCNEncoder.infer: every layer's hop-0 rows at the
+        requested ids through depth_fc, then the LSTM steps, returning the first step's output as forward does.
+        f32[len(ids), dim], or every node in engine-row order when ids is None."""
+        h_t = []
+        self._infer(ids, chunk_rows, lambda layer, rows: h_t.append(self.depth_fc[layer + 1](rows)))
+        return self._steps(h_t)
 
 
 def _exchange_composed(store, grad_store, ids, rows):

@@ -531,6 +531,54 @@ def get_multi_hop_neighbor(nodes, edge_types, sampler=None):
     return nodes_list, adj_list
 
 
+def graph_node_ids():
+    """The node ids of the graph in engine-row order, i64[n]: row r of graph_adjacency is the node graph_node_ids()[r]."""
+    out = torch.empty(get_graph().num_nodes, dtype=torch.int64, device=_dev())
+    _call("eu_graph_node_ids", out)
+    return out
+
+
+def graph_node_rows(nodes):
+    """The engine row of every node id, i64 of nodes' size; -1 for an id that is not a node."""
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    out = torch.empty_like(nodes)
+    _call("eu_graph_node_rows", nodes, nodes.numel(), out)
+    return out
+
+
+def graph_adjacency(edge_types, rows=None, weights=False):
+    """The adjacency of the resident graph with engine rows as columns, in one device op (include/euler_b200.h,
+    eu_graph_adjacency).  rows: None (every row), a range(r0, r1) of engine rows, or a tensor of engine rows (-1 lists
+    nothing).  Row i lists its node's neighbours as get_full_neighbor(node, edge_types) does, each as its engine row.
+    Returns (indptr i64[R+1], cols i64[nnz], weights f32[nnz] or None, extra_ids i64[X]): a listed id that is not a node
+    has column n + k with extra_ids[k] that id, k in first-occurrence order over this call's listing, so a chunked build
+    numbers each chunk's absent ids on its own.  Two host syncs, three when some listed id is not a node."""
+    et = get_edge_type_id(edge_types)
+    n = get_graph().num_nodes
+    if rows is None:
+        rows = range(n)
+    if isinstance(rows, range):
+        if rows.step != 1 or not 0 <= rows.start <= rows.stop <= n:
+            raise EulerError("graph_adjacency: rows must be a range of step 1 within [0, %d]" % n)
+        row_list, r0, r1 = None, rows.start, rows.stop
+    else:
+        row_list = _t(rows, torch.int64).reshape(-1)
+        r0, r1 = 0, row_list.numel()
+    dev = _dev()
+    counts = torch.zeros(2, dtype=torch.int64, device=dev)
+    indptr = torch.empty(r1 - r0 + 1, dtype=torch.int64, device=dev)
+    _call("eu_graph_adjacency", et, len(et), row_list, r0, r1, 0, 0, indptr, None, None, None, counts)
+    nnz, absent = torch.stack([indptr[-1], counts[0]]).tolist()
+    cols = torch.empty(nnz, dtype=torch.int64, device=dev)
+    w = torch.empty(nnz, dtype=torch.float32, device=dev) if weights else None
+    extra = torch.empty(absent, dtype=torch.int64, device=dev)
+    if nnz:
+        _call("eu_graph_adjacency", et, len(et), row_list, r0, r1, nnz, absent, indptr, cols, w, extra, counts)
+    if absent:
+        extra = extra[:int(counts[1].item())]
+    return indptr, cols, w, extra
+
+
 def sample_neighbor_layerwise(nodes, edge_types, count, default_node=-1, weight_func=''):
     """neighbor_ops.sample_neighbor_layerwise (neighbor_ops.py:72-77): nodes [batch, n] -> (neighbors i64[batch, count],
     adj f32[batch, n, count]); adj is the dense view of the reference's SparseTensor (1.0 where neighbors[b, k] is a neighbor of

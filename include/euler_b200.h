@@ -854,6 +854,30 @@ int eu_adjacency_mean(eu_ctx* c, const float* x_neigh, int64_t m, const int64_t*
                       int64_t nnz, int32_t dim, float* out);
 int eu_adjacency_mean_backward(eu_ctx* c, const float* grad_out, const int64_t* indptr, const int64_t* cols, int64_t n,
                                int64_t nnz, int64_t m, int32_t dim, float* grad_x);
+/* The adjacency of the resident graph, with engine rows as columns (layer-by-layer inference of GCNEncoder and
+ * GenieEncoder: every layer one pass over the graph's edges).  Output row i lists engine row r0 + i, or rows[r0 + i] when
+ * rows (i64, device) is given -- a value outside [0, n) lists nothing -- for i in [0, r1 - r0): eu_get_full_neighbor's
+ * listing of that row's node (the K types in the order given, repeats repeat, multi-edges kept; an unknown type lists
+ * nothing), each neighbour id replaced by its engine row (arithmetic on synthetic and sharded layouts, the id table
+ * otherwise).  A listed id that is not a node of the graph gets column n + k (n = eu_graph_num_nodes), k numbering the
+ * distinct such ids in first-occurrence order over THIS call's listing: each call, and so each chunk of a chunked build,
+ * numbers its own; out_extra[k] is the id.
+ * Two calls, like eu_get_full_neighbor:
+ *   cap = 0:             out_ptr i64[r1 - r0 + 1] and counts[0] = the listed entries whose id is not a node
+ *   cap = nnz = out_ptr[r1 - r0], extra_cap = counts[0]:   out_ptr again, out_cols i64[nnz], out_w f32[nnz] (optional:
+ *                        cum_w differences as eu_get_full_neighbor's weights), out_extra i64[extra_cap] (the first
+ *                        counts[1] hold the distinct absent ids)
+ * counts is i64[2] on the device.  No host synchronisation; entries are spread over threads by entry (a hub row does not
+ * serialise), the first call reads every listed id once more to count the absent ones.  ctx scratch: the scan temp, and
+ * O(extra_cap) for the absent ids.  r0 > r1, r1 > n without rows, K outside [0, 32], a NULL pointer that is needed:
+ * EU_ERR_INVALID; 2^31 rows or absent entries or more: EU_ERR_UNSUPPORTED.  Device pointers.
+ * eu_graph_node_ids: the node ids in engine-row order, out i64[n].
+ * eu_graph_node_rows: the engine row of every id, -1 for ids that are not nodes, out i64[B]. */
+int eu_graph_adjacency(eu_ctx* c, const int32_t* etypes, int32_t K, const int64_t* rows, int64_t r0, int64_t r1, int64_t cap,
+                       int64_t extra_cap, int64_t* out_ptr, int64_t* out_cols, float* out_w, int64_t* out_extra,
+                       int64_t* counts);
+int eu_graph_node_ids(eu_ctx* c, int64_t* out);
+int eu_graph_node_rows(eu_ctx* c, const int64_t* nodes, int64_t B, int64_t* out);
 /* The per-layer embedding stores of ScalableSageEncoder / ScalableGCNEncoder (tf_euler/python/utils/encoders.py:294-408,
  * 629-748): a store f32[n_rows, dim] and its gradient store f32[n_rows, dim], updated in place with fixed meanings for
  * repeated ids.  ids i64[M] must lie in [0, n_rows).
