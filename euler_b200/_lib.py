@@ -148,6 +148,7 @@ SIGNATURES = {
     "eu_sage_mean_aggregate_host": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
     "eu_sample_node": (C.c_int, [_P, _I32, _P, _I32, _P]),
     "eu_sample_node_host": (C.c_int, [_P, _I32, _P, _I32, _P]),
+    "eu_sample_n_with_types": (C.c_int, [_P, _P, _I64, _I32, _P]),
     "eu_build_alias_table": (C.c_int, [_P, _I64, _P, _P, _P]),
     "eu_graph_load_inspect": (C.c_int, [C.c_char_p, C.c_int, C.c_int, _P, _P, _P, _P, _I64, _P, _P]),
     "eu_random_walk": (C.c_int, [_P, _P, _I64, _P, _I32, _I32, _F, _F, _I64, _P]),

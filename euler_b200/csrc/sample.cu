@@ -712,10 +712,67 @@ __global__ void k_sample_node(NodeSamplerDev s, int32_t count, int32_t upd, unsi
   }
 }
 
-__global__ void k_advance_engine(EuRngState* rng, unsigned long long uniforms) {
+__device__ __forceinline__ void advance_engine(EuRngState* rng, unsigned long long uniforms) {
   rng->x = modmul(rng->x, modpow_a(2ull * uniforms));
   rng->draws += uniforms;
   rng->calls += 1;
+}
+
+__global__ void k_advance_engine(EuRngState* rng, unsigned long long uniforms) { advance_engine(rng, uniforms); }
+
+// ---------------------------------------------------------------------------- per-row typed node draws
+// sample_n_with_types: Graph::SampleNode(types[i], count) for every row i in order (graph.cc:221-245).  k_check_types ORs
+// what is wrong with the rows' types into one flag; the draw and the engine advance read it and do nothing once it is set,
+// so a refused call leaves `out` and the engine as they were, and the host reads the flag back in the call's one sync.
+enum : unsigned { kTypeAbsent = 1u, kTypeRange = 2u, kTypeEmpty = 4u };
+
+__global__ void k_check_types(const int32_t* __restrict__ types, int64_t n, int32_t n_types, unsigned int empty_types,
+                              unsigned int* flag) {
+  unsigned bad = 0;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t t = __ldg(types + i);
+    if (t == INT32_MIN) bad |= kTypeAbsent;             // get_node_type of an id that is not a node
+    else if (t < 0 || t >= n_types) bad |= kTypeRange;
+    else if ((empty_types >> t) & 1u) bad |= kTypeEmpty;
+  }
+  bad = __reduce_or_sync(0xffffffffu, bad);
+  if (bad && (threadIdx.x & 31) == 0) atomicOr(flag, bad);
+}
+
+// Draw e = i * count + j of the call is row i's draw j: two uniforms, the alias pick of node_samplers_[types[i]].  Under
+// minstd it starts at uniform 2e of the call, i.e. engine step 4e; a thread jumps there once and then strides by `jump` =
+// A^(4 * grid threads).
+template <bool PHILOX>
+__global__ void __launch_bounds__(256) k_sample_n_with_types(NodeSamplerDev s, const int32_t* __restrict__ types, int64_t n,
+                                                              int32_t count, uint32_t jump, unsigned long long key,
+                                                              const EuRngState* __restrict__ rng,
+                                                              const unsigned int* __restrict__ flag, long long* __restrict__ out) {
+  if (*flag) return;
+  const int64_t total = n * count, stride = (int64_t)gridDim.x * blockDim.x;
+  int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= total) return;
+  uint32_t x = PHILOX ? 0u : modmul(rng->x, modpow_a(4ull * (unsigned long long)e));
+  const uint32_t salt = PHILOX ? (uint32_t)rng->calls : 0u;
+  for (; e < total; e += stride) {
+    const int64_t i = e / count;
+    const int32_t j = (int32_t)(e - i * count);
+    const int32_t t = __ldg(types + i);
+    double u0, u1;
+    if (PHILOX) {
+      philox_uniform2(0x5A4E570000000000ull ^ (unsigned long long)i, (uint32_t)j, salt, key, u0, u1);
+    } else {
+      uint32_t y = x;
+      u0 = minstd_uniform(y);
+      u1 = minstd_uniform(y);
+      x = modmul(x, jump);
+    }
+    const long long col = alias_next(s.prob[t], s.alias[t], s.n[t], u0, u1);
+    out[e] = (long long)__ldg(s.ids[t] + col);
+  }
+}
+
+__global__ void k_advance_engine_unless(EuRngState* rng, unsigned long long uniforms, const unsigned int* flag) {
+  if (*flag == 0) advance_engine(rng, uniforms);
 }
 
 // ---------------------------------------------------------------------------- host side
@@ -1043,6 +1100,55 @@ int eu_sample_node(eu_ctx* c, int32_t count, const int32_t* types, int32_t n_typ
   EU_LAUNCHED();
   k_advance_engine<<<1, 1, 0, c->stream>>>(c->d_rng, (unsigned long long)upd * (unsigned long long)count);
   EU_LAUNCHED();
+  return EU_OK;
+}
+
+// The engine op API_SAMPLE_N_WITH_TYPES (euler/core/kernels/sample_n_with_types_op.cc) loops over the rows calling
+// SampleNode({types[i]}, count), which api.cc:32-37 sends to the scalar overload Graph::SampleNode(int, count).
+int eu_sample_n_with_types(eu_ctx* c, const int32_t* types, int64_t n, int32_t count, int64_t* out) {
+  if (!c || n < 0 || count < 0 || (n > 0 && count > 0 && (!types || !out))) {
+    set_error("eu_sample_n_with_types: bad argument");
+    return EU_ERR_INVALID;
+  }
+  if (n == 0 || count == 0) return EU_OK;
+  eu_graph* g = c->g;
+  EU_CUDA(cudaSetDevice(g->device));
+  int rc = graph_build_sampler(g);
+  if (rc) return rc;
+  const int32_t NT = g->d.n_node_types;
+  if (NT > EU_MAX_ETYPES) { set_error("more than %d node types", EU_MAX_ETYPES); return EU_ERR_UNSUPPORTED; }
+  NodeSamplerDev s{};
+  unsigned int empty_types = 0;
+  s.n_types = NT;
+  for (int t = 0; t < NT; ++t) {
+    s.ids[t] = g->samplers[t].ids; s.prob[t] = g->samplers[t].prob; s.alias[t] = g->samplers[t].alias;
+    s.n[t] = g->samplers[t].n;
+    // graph.cc:236 returns nothing for a type of total weight 0 (its normalised sampler sums to NaN here, so the raw sum decides)
+    if (!(g->type_sums[t] > 0.f)) empty_types |= 1u << t;
+  }
+  if ((rc = ctx_misc(c, 256))) return rc;
+  unsigned int* flag = (unsigned int*)c->d_misc;
+  cudaStream_t st = c->stream;
+  EU_CUDA(cudaMemsetAsync(flag, 0, sizeof(unsigned int), st));
+  k_check_types<<<(unsigned)std::min<int64_t>(ceil_div(n, 256), kSMs * 8), 256, 0, st>>>(types, n, NT, empty_types, flag);
+  EU_LAUNCHED();
+  const int64_t total = n * (int64_t)count;
+  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(total, 256), kSMs * 8);
+  const uint32_t jump = modpow_a(4ull * (unsigned long long)blocks * 256ull);
+  { EuProfScope ps(c, "k_sample_n_with_types", n);
+    if (c->rng == EU_RNG_PHILOX)
+      k_sample_n_with_types<true><<<blocks, 256, 0, st>>>(s, types, n, count, jump, c->seed, c->d_rng, flag, (long long*)out);
+    else
+      k_sample_n_with_types<false><<<blocks, 256, 0, st>>>(s, types, n, count, jump, c->seed, c->d_rng, flag, (long long*)out); }
+  EU_LAUNCHED();
+  k_advance_engine_unless<<<1, 1, 0, st>>>(c->d_rng, 2ull * (unsigned long long)total, flag);
+  EU_LAUNCHED();
+  unsigned int bad = 0;
+  EU_CUDA(cudaMemcpyAsync(&bad, flag, sizeof(bad), cudaMemcpyDeviceToHost, st));
+  EU_CUDA(cudaStreamSynchronize(st));
+  if (bad & kTypeAbsent) { set_error("sample_n_with_types: a source is not a node of the graph (type INT32_MIN)"); return EU_ERR_INVALID; }
+  if (bad & kTypeRange) { set_error("sample_n_with_types: a node type is outside [0, %d)", NT); return EU_ERR_INVALID; }
+  if (bad & kTypeEmpty) { set_error("sample_n_with_types: a listed node type has total weight 0"); return EU_ERR_STATE; }
   return EU_OK;
 }
 

@@ -311,6 +311,33 @@ def sample_node(count, node_type, condition=''):
     return out
 
 
+def get_node_type(nodes):
+    """the node type of every node (base._LIB_OP.get_node_type, euler::GetNodeType api.cc:50-61): i32[B], INT32_MIN for an
+    id that is not a node"""
+    nodes = _t(nodes, torch.int64).reshape(-1)
+    out = torch.empty(nodes.numel(), dtype=torch.int32, device=nodes.device)
+    _call("eu_get_node_type", nodes, nodes.numel(), out)
+    return out
+
+
+def sample_n_with_types(count, types):
+    """base._LIB_OP.sample_n_with_types (kernel tf_euler/kernels/sample_n_with_types_op.cc): row i of the i64[n, count]
+    result is `count` nodes drawn from node type types[i], the rows drawn in order from this thread's engine.  A type that
+    is INT32_MIN (an absent source) or out of range raises EulerError, and so does a type of total weight 0 (upstream
+    aborts); a refused call draws nothing."""
+    types = _t(types, torch.int32).reshape(-1)
+    count = int(count)
+    out = torch.empty((types.numel(), count), dtype=torch.int64, device=types.device)
+    _call("eu_sample_n_with_types", types, types.numel(), count, out)
+    return out
+
+
+def sample_node_with_src(src_nodes, count):
+    """sample_ops.sample_node_with_src (sample_ops.py:75-87): for every source node, `count` nodes of its type,
+    i64[len(src_nodes), count]"""
+    return sample_n_with_types(count, get_node_type(src_nodes))
+
+
 def random_walk(nodes, edge_types, p=1.0, q=1.0, default_node=-1):
     """walk_ops.random_walk (walk_ops.py:29-43).  edge_types: list of L 1-D type lists.
     Returns i64[B, L+1]."""

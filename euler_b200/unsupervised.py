@@ -14,7 +14,7 @@ Upstream's neg_condition (sample_node with an index query) is not supported.
 
 DGI (examples/dgi/dgi.py) is the one model here over a GraphSAGE encoder: encoders.ShuffleSageEncoder with ShallowEncoder's
 feature inputs, a bilinear decoder against the batch's readout, and the same rank metrics (composed_metric).  The
-unsupervised GraphSage / GCN models are not provided by this module.
+unsupervised GraphSage / GCN models are solution.UnsuperviseSolution over two encoders.
 """
 import torch
 import torch.nn.functional as F
@@ -60,15 +60,20 @@ def composed_metric(pos_logits, neg_logits, name):
     raise ValueError("metric must be one of %s, got %r" % (SKIPGRAM_METRICS, name))
 
 
+def xent_loss(logits, neg_logits):
+    """solution/losses.py's xent_loss: the mean sigmoid cross entropy of logits against ones and neg_logits against zeros,
+    over every entry of both"""
+    true_xent = F.binary_cross_entropy_with_logits(logits, torch.ones_like(logits), reduction='none')
+    negative_xent = F.binary_cross_entropy_with_logits(neg_logits, torch.zeros_like(neg_logits), reduction='none')
+    return torch.cat([true_xent.reshape(-1, 1), negative_xent.reshape(-1, 1)], 0).mean()
+
+
 def composed_skipgram_loss(emb, pos_emb, neg_emb, metric='mrr'):
     """PosNegLogits + xent_loss + the metric, literally (solution/logits.py, solution/losses.py): emb [B, 1, dim], pos_emb
     [B, P, dim], neg_emb [B, K, dim] -> (loss, metric)."""
     logit = torch.matmul(emb, pos_emb.transpose(1, 2))
     neg_logit = torch.matmul(emb, neg_emb.transpose(1, 2))
-    true_xent = F.binary_cross_entropy_with_logits(logit, torch.ones_like(logit), reduction='none')
-    negative_xent = F.binary_cross_entropy_with_logits(neg_logit, torch.zeros_like(neg_logit), reduction='none')
-    loss = torch.cat([true_xent.reshape(-1, 1), negative_xent.reshape(-1, 1)], 0).mean()
-    return loss, composed_metric(logit.detach(), neg_logit.detach(), metric)
+    return xent_loss(logit, neg_logit), composed_metric(logit.detach(), neg_logit.detach(), metric)
 
 
 class UnsuperviseModel(torch.nn.Module):
@@ -205,10 +210,7 @@ class DGI(torch.nn.Module):
         logits = torch.matmul(self.kernel(embedding), embedding_pos.transpose(1, 2))
         neg_logits = torch.matmul(self.kernel(embedding_negs), embedding_pos.transpose(1, 2))
         metric = composed_metric(logits.detach(), neg_logits.detach(), self.metric_name)
-        true_xent = F.binary_cross_entropy_with_logits(logits, torch.ones_like(logits), reduction='none')
-        negative_xent = F.binary_cross_entropy_with_logits(neg_logits, torch.zeros_like(neg_logits), reduction='none')
-        loss = torch.cat([true_xent.reshape(-1, 1), negative_xent.reshape(-1, 1)], 0).mean()
-        return loss, metric
+        return xent_loss(logits, neg_logits), metric
 
     def forward(self, inputs, generator=None):
         src = inputs.unsqueeze(-1)

@@ -249,6 +249,16 @@ int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, co
 int eu_sample_node(eu_ctx* c, int32_t count, const int32_t* types, int32_t n_types, int64_t* out);
 int eu_sample_node_host(eu_ctx* c, int32_t count, const int32_t* types, int32_t n_types,
                         int64_t* out);
+/* tf_euler.sample_n_with_types -- TF op SampleNWithTypes (tf_euler/kernels/sample_n_with_types_op.cc, engine op
+ * euler/core/kernels/sample_n_with_types_op.cc): row i of out i64[n, count] is SampleNode({types[i]}, count), the rows drawn
+ * in order from the ctx's one engine (Graph::SampleNode(int, count), graph.cc:221-245: 2 uniforms per draw).  Under
+ * EU_RNG_MINSTD row i's draw j starts at uniform 2 (i count + j) of the call, and the engine then advances by 2 n count
+ * uniforms, so a following sampling op continues the reference's stream; EU_RNG_PHILOX keys draw (i, j) on the call counter.
+ * types i32[n] and out are device pointers.  Refused, with out and the engine untouched: a row whose type is INT32_MIN (its
+ * source is not a node, as eu_get_node_type reports it) or outside [0, n_node_types) -> EU_ERR_INVALID (upstream indexes
+ * node_samplers_ with it); a type whose total node weight is 0 -> EU_ERR_STATE (upstream aborts on the short result).  The
+ * check is read back in the call's one stream synchronisation.  n = 0 or count = 0 returns at once. */
+int eu_sample_n_with_types(eu_ctx* c, const int32_t* types, int64_t n, int32_t count, int64_t* out);
 /* tf_euler.random_walk -- TF op RandomWalk (tf_euler/ops/walk_ops.cc:77-107, kernel
  * tf_euler/kernels/random_walk_op.cc:83-289).  etypes i32[L,K] (host); out i64[B,L+1].
  * EU_RNG_MINSTD: the reference's walks bit for bit (serial engine stream, sequential f32 prefix of the biased weights).
