@@ -220,6 +220,8 @@ SIGNATURES = {
     "eu_skipgram_loss_backward": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P]),
     "eu_skipgram_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P, _P, _P,
                                                    _P, _P]),
+    "eu_gae_loss": (C.c_int, [_P, _I64, _I32, _I32, _P, _P, _P, _F, _P, _P, _P]),
+    "eu_gae_loss_backward": (C.c_int, [_P, _P, _I64, _I32, _I32, _P, _P, _P, _F, _P, _P, _P]),
     "eu_kg_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "eu_kg_loss_backward": (C.c_int, [_P, _P, _P, _P, _P]),
     "eu_kg_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),

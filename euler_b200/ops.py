@@ -1661,6 +1661,80 @@ def skipgram_xent_loss(src, pos, negs, target, context, metric='mrr', sparse_gra
     return loss, skipgram_metric(rank, metric)
 
 
+# ------------------------------------------------------------------------------------ graph auto-encoder step
+class _GaeLoss(torch.autograd.Function):
+    """eu_gae_loss / eu_gae_loss_backward over the sets (src, pos, negs) of mu, log_var (or None) and noise (or None).  Saves
+    the inputs and the [B, 2K] logits; the reparameterised rows are never written."""
+
+    @staticmethod
+    def forward(ctx, radius, emb, pos, neg, lv_e, lv_p, lv_n, nz_e, nz_p, nz_n):
+        B, K, D = pos.shape
+        mu, lv, nz = [emb, pos, neg], [lv_e, lv_p, lv_n], [nz_e, nz_p, nz_n]
+        lv, nz = (lv if lv_e is not None else None), (nz if nz_e is not None else None)
+        logits = torch.empty((B, 2 * K), dtype=torch.float32, device=emb.device)
+        loss = torch.empty((), dtype=torch.float32, device=emb.device)
+        correct = torch.empty((), dtype=torch.int64, device=emb.device)
+        _call("eu_gae_loss", B, K, D, mu, lv, nz, radius, logits, loss, correct)
+        ctx.save_for_backward(emb, pos, neg, lv_e, lv_p, lv_n, nz_e, nz_p, nz_n, logits)
+        ctx.radius = radius
+        ctx.mark_non_differentiable(correct, logits)
+        return loss, correct, logits
+
+    @staticmethod
+    def backward(ctx, g_loss, g_correct, g_logits):
+        emb, pos, neg, lv_e, lv_p, lv_n, nz_e, nz_p, nz_n, logits = ctx.saved_tensors
+        B, K, D = pos.shape
+        var, noisy = lv_e is not None, nz_e is not None
+        mu = [emb, pos, neg]
+        g = g_loss.to(device=emb.device, dtype=torch.float32).reshape(1).contiguous()
+        g_mu = [torch.empty_like(t, memory_format=torch.contiguous_format) for t in mu]
+        g_lv = [torch.empty_like(t, memory_format=torch.contiguous_format) for t in mu] if var else None
+        _call("eu_gae_loss_backward", g, B, K, D, mu, [lv_e, lv_p, lv_n] if var else None,
+              [nz_e, nz_p, nz_n] if noisy else None, ctx.radius, logits, g_mu, g_lv)
+        return (None, *g_mu, *(g_lv or [None] * 3), None, None, None)
+
+
+def gae_loss(emb, pos, neg, log_var=None, noise=None, radius=1.0, return_logits=False):
+    """The reconstruction loss and accuracy of BaseGraphAutoEncoder.__call__ (mp_utils/base_gae.py) and, with log_var, of
+    VariationalGraphAutoEncoder.__call__ (examples/gae/gae.py), in one fused device op over encoder rows:
+        emb f32[B, D] (or [B, 1, D])   the source rows        pos, neg f32[B, K, D]   positive and negative context rows, K >= 1
+        log_var                        None (GAE), or the three sets' log-variance rows (same shapes as emb, pos, neg)
+        noise                          None (z = mu: VGAE's train=False), or three sets of unit-normal draws (same shapes);
+                                       the op forms z = mu + radius * noise * sqrt(exp(log_var)) itself
+    Returns (loss, correct) or, with return_logits, (loss, correct, logits f32[B, 2K]): loss is the mean sigmoid cross entropy
+    over the 2BK logits <z_src, z_ctx> (positives first, labelled 1), plus the mean KL -0.5 (log_var - exp(log_var) - mu^2 + 1)
+    over the B D (2K + 1) elements with log_var; correct (int64) counts floor(sigmoid(logit) + 0.5) == label, so the batch's
+    acc is correct / (2BK).  Gradients reach emb, pos, neg and log_var, never noise.  Deterministic, no atomics, and neither
+    pass synchronises with the host (include/euler_b200.h, eu_gae_loss)."""
+    if radius is None or not math.isfinite(float(radius)):
+        raise EulerError("gae_loss: radius must be finite, got %r" % (radius,))
+    if noise is not None and log_var is None:
+        raise EulerError("gae_loss: noise needs log_var")
+    _check_f32("gae_loss", (('emb', emb), ('pos', pos), ('neg', neg)))
+    if emb.dim() == 3 and emb.shape[1] == 1:
+        emb = emb.reshape(emb.shape[0], emb.shape[2])
+    if emb.dim() != 2 or pos.dim() != 3 or pos.shape[0] != emb.shape[0] or pos.shape[1] < 1 or pos.shape[2] != emb.shape[1] \
+            or neg.shape != pos.shape:
+        raise EulerError("gae_loss: need emb [B, D] and pos, neg [B, K >= 1, D]; got %s, %s and %s"
+                         % (tuple(emb.shape), tuple(pos.shape), tuple(neg.shape)))
+    sets = [emb, pos, neg]
+    extra = []
+    for name, group in (('log_var', log_var), ('noise', noise)):
+        if group is None:
+            extra.append([None] * 3)
+            continue
+        group = list(group)
+        _check_f32("gae_loss", [(name, t) for t in group])
+        group = [t.reshape(t.shape[0], t.shape[2]) if i == 0 and t.dim() == 3 and t.shape[1] == 1 else t
+                 for i, t in enumerate(group)]
+        if len(group) != 3 or any(t.shape != s.shape for t, s in zip(group, sets)):
+            raise EulerError("gae_loss: %s must be three sets shaped as emb, pos and neg" % name)
+        extra.append([_t(t, torch.float32) for t in group])
+    sets = [_t(t, torch.float32) for t in sets]
+    loss, correct, logits = _GaeLoss.apply(float(radius), *sets, *extra[0], *extra[1])
+    return (loss, correct, logits) if return_logits else (loss, correct)
+
+
 # ------------------------------------------------------------------------------------ knowledge-graph embedding step
 KG_MODELS = {'transe': 0, 'transh': 1, 'transr': 2, 'transd': 3, 'distmult': 4}
 KG_CORRUPT = {'front': 1, 'tail': 2, 'both': 3}

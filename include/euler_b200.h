@@ -515,6 +515,35 @@ int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const in
                                      int32_t dim, const float* logits, int64_t* rows_target, float* values_target,
                                      int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context);
 
+/* The reconstruction step of the graph auto-encoders GAE and VGAE (tf_euler/python/mp_utils/base_gae.py, examples/gae/gae.py),
+ * fused, over encoder rows.  Three sets of f32 row-major device rows, each 4-byte aligned (16-byte alignment and D % 4 == 0
+ * take vector loads, with the same bits): set 0 the sources [B, D], set 1 the positives [B, K, D], set 2 the negatives
+ * [B, K, D].  mu[s] are the rows; for the variational form log_var[s] (same shapes) and optionally noise[s] (unit-normal
+ * draws, same shapes) are given too, and the op forms z = mu + (radius noise) sqrt(exp(log_var)) itself, element by element in
+ * f32, without writing it; noise NULL gives z = mu (VGAE's train=False), log_var NULL the plain GAE (z = mu, no KL).  The
+ * pointer arrays mu, log_var, noise (three entries each) are host arrays.  Outputs, device pointers:
+ *   logits f32[B, 2K] (may be NULL): row b is <z_src[b], z_pos[b, k]> for k < K, then <z_src[b], z_neg[b, k]>, each dot in
+ *                         eu_skipgram_loss's fixed order (per-lane fma sums over 4-column chunks, then a fixed butterfly);
+ *   loss f32[1]:          the mean over the 2BK logits of max(x, 0) - x z + log1p(exp(-|x|)), z = 1 for the positives (f32
+ *                         terms summed in f64, one division), plus, in the variational form, the mean over the B D (2K + 1)
+ *                         elements of kl = -0.5 (log_var - exp(log_var) - mu^2 + 1) (f32 elements summed in f64, one division),
+ *                         the two f32 means added in f32 (B = 0: NaN);
+ *   correct i64[1]:       #{floor(sigmoid(x) + 0.5) == z} over the 2BK logits, sigmoid(x) = 1 / (1 + exp(-x)) in f32.
+ * The backward pass takes grad_loss (a device f32 scalar, read on the device) and the forward's logits, and writes dense
+ * gradients of the same shapes as the inputs: grad_mu[s] = dL/dz (+ grad kl / (B D (2K + 1)) mu in the variational form),
+ * grad_log_var[s] (required with log_var) = dL/dz (radius noise) 0.5 sqrt(exp(log_var)) + grad (exp(log_var) - 1) / (2 B D
+ * (2K + 1)); none goes to noise.  dL/dz_ctx[b, j] = c_bj z_src[b] and dL/dz_src[b] = sum over j of c_bj z_ctx[b, j] (fma from
+ * +0 in j order) with c_bj = (sigmoid(x_bj) - z) grad / 2BK.  Every element is written by one thread: no atomics, the same
+ * bits on every run, and neither pass synchronises with the host, so both can be captured in a CUDA graph (once the ctx
+ * scratch, O(B K) f64, has grown to the batch outside the capture).
+ * B < 0, K < 1, D < 1, a non-finite radius, noise without log_var, or a NULL pointer that is needed: EU_ERR_INVALID with
+ * nothing written; K >= 2^29 or B (2K + 1) >= 2^34: EU_ERR_UNSUPPORTED. */
+int eu_gae_loss(eu_ctx* c, int64_t B, int32_t K, int32_t D, const float* const* mu, const float* const* log_var,
+                const float* const* noise, float radius, float* logits, float* loss, int64_t* correct);
+int eu_gae_loss_backward(eu_ctx* c, const float* grad_loss, int64_t B, int32_t K, int32_t D, const float* const* mu,
+                         const float* const* log_var, const float* const* noise, float radius, const float* logits,
+                         float* const* grad_mu, float* const* grad_log_var);
+
 /* The knowledge-graph embedding step of TransE / TransH / TransR / TransD (examples/TransX) and DistMult (examples/distmult),
  * fused: the mapped id rows of each triple and of its corrupted triples, the scores, the margin loss and the rank.
  * Triple b: src_b, dst_b (entity ids), rel_b (relation id), neg[b, 0 .. K-1] (entity ids); ids are table rows.
