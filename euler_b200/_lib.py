@@ -54,6 +54,8 @@ SHALLOW_MAX_SLOTS = 8   # EU_SHALLOW_MAX_SLOTS
 SHALLOW_MAX_WIDTH = 16384   # EU_SHALLOW_MAX_WIDTH
 SHALLOW_POOL_MAX_COUNT = 512   # EU_SHALLOW_POOL_MAX_COUNT
 NEIGHBOR_TOP_K_MAX = 16   # EU_NEIGHBOR_TOP_K_MAX
+METRIC_AUC_MAX_THRESHOLDS = 16384   # EU_METRIC_AUC_MAX_THRESHOLDS
+METRIC_F1, METRIC_ACC = 0, 1   # EU_METRIC_F1, EU_METRIC_ACC
 
 
 class ShallowDense(C.Structure):
@@ -222,6 +224,8 @@ SIGNATURES = {
                                                    _P, _P]),
     "eu_gae_loss": (C.c_int, [_P, _I64, _I32, _I32, _P, _P, _P, _F, _P, _P, _P]),
     "eu_gae_loss_backward": (C.c_int, [_P, _P, _I64, _I32, _I32, _P, _P, _P, _F, _P, _P, _P]),
+    "eu_metric_auc_update": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
+    "eu_metric_count_update": (C.c_int, [_P, _I32, _P, _P, _I64, _P, _P, _P]),
     "eu_kg_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "eu_kg_loss_backward": (C.c_int, [_P, _P, _P, _P, _P]),
     "eu_kg_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),

@@ -11,28 +11,33 @@ fused=True (the default) computes the step after the encoders -- the logits, the
 the reparameterisation and the KL term -- in one device op, ops.gae_loss; fused=False is the literal torch composition of
 base_gae.py / gae.py (composed_gae_loss), which consumes the same draws and the same noise.
 
+streaming=True makes acc upstream's streaming tf.metrics.accuracy: the device module model.metric
+(metrics.StreamingAccuracy), whose value covers every batch since construction or model.metric.reset().  The fused path adds
+ops.gae_loss's correct count of the 2BK predictions to it (no second pass); fused=False adds the composed predictions.
+
 Departures from upstream: the encoder is injected (examples/gae builds GNN(BaseGNNNet), which this package does not have);
-acc is the batch's own value, where upstream's is the streaming tf.metrics.accuracy; VGAE returns the mu rows as its
-embedding, where upstream returns the tuple (mu, log_var, emb) in that slot.
+by default acc is the batch's own value, where upstream's is the streaming tf.metrics.accuracy (streaming=True gives that);
+VGAE returns the mu rows as its embedding, where upstream returns the tuple (mu, log_var, emb) in that slot.
 """
 import math
 
 import torch
 
-from . import ops
+from . import metrics, ops
 from .encoders import ShallowEncoder
 from .solution import acc_score
 from .unsupervised import xent_loss
 
 
-def composed_gae_loss(emb, emb_pos, emb_negs):
-    """base_gae.py's step after the encoders, literally: emb [B, 1, dim], emb_pos and emb_negs [B, K, dim] -> (loss, acc)"""
+def composed_gae_loss(emb, emb_pos, emb_negs, metric=acc_score):
+    """base_gae.py's step after the encoders, literally: emb [B, 1, dim], emb_pos and emb_negs [B, K, dim] -> (loss, acc),
+    acc = metric(label, predict) (acc_score, or a streaming metrics.StreamingAccuracy)"""
     logits = torch.matmul(emb, emb_pos.transpose(1, 2))
     neg_logits = torch.matmul(emb, emb_negs.transpose(1, 2))
     loss = xent_loss(logits, neg_logits)
     predict, neg_predict = torch.sigmoid(logits.detach()), torch.sigmoid(neg_logits.detach())
     label = torch.cat([torch.ones_like(predict), torch.zeros_like(neg_predict)], 2)
-    return loss, acc_score(label, torch.cat([predict, neg_predict], 2))
+    return loss, metric(label, torch.cat([predict, neg_predict], 2))
 
 
 def kl(mu, log_var):
@@ -47,9 +52,9 @@ def _fused_acc(correct, logits_count):
 class BaseGraphAutoEncoder(torch.nn.Module):
     """BaseGraphAutoEncoder(node_type, edge_type, max_id, num_negs=20): num_negs positives per input from sample_neighbor over
     edge_type (default node max_id + 1) and num_negs negatives per input from sample_node of node_type.  A subclass provides
-    embed(n_id) -> [B, n, dim] rows."""
+    embed(n_id) -> [B, n, dim] rows.  streaming=True makes acc the streaming model.metric (see the top of the file)."""
 
-    def __init__(self, node_type, edge_type, max_id, num_negs=20, fused=True):
+    def __init__(self, node_type, edge_type, max_id, num_negs=20, fused=True, *, streaming=False):
         super().__init__()
         if int(num_negs) < 1:
             raise ValueError("num_negs must be at least 1, got %r" % (num_negs,))
@@ -58,6 +63,9 @@ class BaseGraphAutoEncoder(torch.nn.Module):
         self.max_id = max_id
         self.num_negs = int(num_negs)
         self.fused = fused
+        self.streaming = bool(streaming)
+        if self.streaming:
+            self.metric = metrics.StreamingAccuracy()
 
     def to_sample(self, inputs):
         batch_size = inputs.numel()
@@ -69,12 +77,20 @@ class BaseGraphAutoEncoder(torch.nn.Module):
     def embed(self, n_id):
         raise NotImplementedError
 
+    def fused_acc(self, correct, logits_count):
+        """acc from the fused op's correct count of logits_count predictions"""
+        return self.metric.add_counts(correct, logits_count) if self.streaming else _fused_acc(correct, logits_count)
+
+    def composed_metric(self):
+        """the acc of the composed step: acc_score, or the streaming metric"""
+        return self.metric if self.streaming else acc_score
+
     def loss_and_acc(self, emb, emb_pos, emb_negs):
         """the step after the encoders: (loss, acc), fused or composed"""
         if self.fused:
             loss, correct = ops.gae_loss(emb, emb_pos, emb_negs)
-            return loss, _fused_acc(correct, 2 * emb_pos.shape[0] * emb_pos.shape[1])
-        return composed_gae_loss(emb, emb_pos, emb_negs)
+            return loss, self.fused_acc(correct, 2 * emb_pos.shape[0] * emb_pos.shape[1])
+        return composed_gae_loss(emb, emb_pos, emb_negs, self.composed_metric())
 
     def embedding(self, rows):
         """the returned embedding of embed(inputs)'s result"""
@@ -99,8 +115,8 @@ def _rows(encoder, n_id):
 class GraphAutoEncoder(BaseGraphAutoEncoder):
     """GraphAutoEncoder (examples/gae/gae.py) over the node encoder `encoder`: embed(n_id) = encoder(n_id) as [B, n, dim]."""
 
-    def __init__(self, encoder, node_type, edge_type, max_id, num_negs=5, fused=True):
-        super().__init__(node_type, edge_type, max_id, num_negs, fused=fused)
+    def __init__(self, encoder, node_type, edge_type, max_id, num_negs=5, fused=True, *, streaming=False):
+        super().__init__(node_type, edge_type, max_id, num_negs, fused=fused, streaming=streaming)
         if not callable(encoder):
             raise ValueError("encoder must map node ids to rows, got %r" % (encoder,))
         self.encoder = encoder
@@ -129,8 +145,8 @@ class VariationalGraphAutoEncoder(BaseGraphAutoEncoder):
     is None and emb = mu.  The loss adds mean(kl) over src, pos and negs; the returned embedding is the mu rows."""
 
     def __init__(self, radius, encoder, node_type, edge_type, max_id, num_negs=5, train=True, generator=None, fused=True,
-                 dim=None, device=None):
-        super().__init__(node_type, edge_type, max_id, num_negs, fused=fused)
+                 dim=None, device=None, *, streaming=False):
+        super().__init__(node_type, edge_type, max_id, num_negs, fused=fused, streaming=streaming)
         if not callable(encoder):
             raise ValueError("encoder must map node ids to rows, got %r" % (encoder,))
         self.radius = float(radius)
@@ -163,9 +179,9 @@ class VariationalGraphAutoEncoder(BaseGraphAutoEncoder):
         if self.fused:
             loss, correct = ops.gae_loss(mu, mu_p, mu_n, log_var=(lv, lv_p, lv_n),
                                          noise=None if nz is None else (nz, nz_p, nz_n), radius=self.radius)
-            return loss, _fused_acc(correct, 2 * mu_p.shape[0] * mu_p.shape[1])
+            return loss, self.fused_acc(correct, 2 * mu_p.shape[0] * mu_p.shape[1])
         loss, acc = composed_gae_loss(self.reparameterize(mu, lv, nz), self.reparameterize(mu_p, lv_p, nz_p),
-                                      self.reparameterize(mu_n, lv_n, nz_n))
+                                      self.reparameterize(mu_n, lv_n, nz_n), self.composed_metric())
         kls = torch.cat([self.kl(mu, lv), self.kl(mu_p, lv_p), self.kl(mu_n, lv_n)], 0)
         return loss + torch.mean(kls), acc
 

@@ -1735,6 +1735,76 @@ def gae_loss(emb, pos, neg, log_var=None, noise=None, radius=1.0, return_logits=
     return (loss, correct, logits) if return_logits else (loss, correct)
 
 
+# ------------------------------------------------------------------------------------ streaming metrics
+def _metric_tensors(op, named, dev):
+    """raise unless every (name, tensor, dtype, shape) of named is a contiguous tensor of that dtype and shape on dev"""
+    for nm, t, dtype, shape in named:
+        if not torch.is_tensor(t) or t.dtype != dtype or tuple(t.shape) != shape or t.device != dev or not t.is_contiguous():
+            raise EulerError("%s: %s must be a contiguous %s tensor of shape %s on %s" % (op, nm, dtype, shape, dev))
+
+
+def _metric_batch(op, labels, predictions):
+    """labels and predictions flattened: float32 tensors of one numel on one CUDA device"""
+    _check_f32(op, (('labels', labels), ('predictions', predictions)))
+    if labels.numel() != predictions.numel():
+        raise EulerError("%s: labels (%d elements) and predictions (%d) must have one numel"
+                         % (op, labels.numel(), predictions.numel()))
+    if predictions.device.type != 'cuda' or labels.device != predictions.device:
+        raise EulerError("%s: labels and predictions must be on one CUDA device" % op)
+    return labels.detach().reshape(-1).contiguous(), predictions.detach().reshape(-1).contiguous()
+
+
+def metric_auc_update(labels, predictions, tp, fn, tn, fp, refused, value):
+    """One step of tf.metrics.auc(labels, predictions, num_thresholds=T) (TF 1.x metrics_impl.py, trapezoidal ROC) on the
+    device: the batch's per-threshold counts are added to the state tp, fn, tn, fp (f32[T] each, 2 <= T <= 16384), and value
+    (an f32 scalar) becomes the AUC of the new state.  labels and predictions are float32 with one numel; a label is positive
+    when nonzero (NaN included) and predictions must lie in [0, 1].  A batch with a prediction outside [0, 1] or NaN is not
+    counted (TF raises at that step): the state is untouched, refused (an int64 scalar) += 1, and value reads NaN while
+    refused > 0.  No host synchronisation (include/euler_b200.h, eu_metric_auc_update); returns value."""
+    op = "metric_auc_update"
+    labels, predictions = _metric_batch(op, labels, predictions)
+    T = tp.shape[0] if torch.is_tensor(tp) and tp.dim() == 1 else -1
+    if not 2 <= T <= _lib.METRIC_AUC_MAX_THRESHOLDS:
+        raise EulerError("%s: the state must be f32[T] with 2 <= T <= %d" % (op, _lib.METRIC_AUC_MAX_THRESHOLDS))
+    dev = predictions.device
+    _metric_tensors(op, [(nm, t, torch.float32, (T,)) for nm, t in (('tp', tp), ('fn', fn), ('tn', tn), ('fp', fp))]
+                    + [('refused', refused, torch.int64, ()), ('value', value, torch.float32, ())], dev)
+    _call("eu_metric_auc_update", labels, predictions, labels.numel(), T, tp, fn, tn, fp, refused, value)
+    return value
+
+
+_COUNT_KINDS = {'f1': (_lib.METRIC_F1, 3), 'acc': (_lib.METRIC_ACC, 2)}
+
+
+def metric_count_update(kind, state, value, labels=None, predictions=None, correct=None, total=None):
+    """One step of utils/metrics.py's f1_score (kind 'f1': state f32[3] = tp, fn, fp) or acc_score (kind 'acc': state
+    f32[2] = total, count) with TF 1.x tf.metrics semantics, on the device: the batch's counts are added to state and value
+    (an f32 scalar) becomes the metric of the new state.  The batch is either labels and predictions (float32, one numel;
+    predictions are floor(p + 0.5) in float32) or, for 'acc' only, correct (an int64 device scalar, e.g. gae_loss's count)
+    over total predictions (a host int).  No host synchronisation (include/euler_b200.h, eu_metric_count_update); returns
+    value."""
+    op = "metric_count_update"
+    if kind not in _COUNT_KINDS:
+        raise EulerError("%s: kind must be one of %s, got %r" % (op, sorted(_COUNT_KINDS), kind))
+    code, width = _COUNT_KINDS[kind]
+    if correct is None:
+        if total is not None:
+            raise EulerError("%s: total goes with correct" % op)
+        labels, predictions = _metric_batch(op, labels, predictions)
+        dev, n = predictions.device, labels.numel()
+    else:
+        if kind != 'acc' or labels is not None or predictions is not None:
+            raise EulerError("%s: correct counts are taken for 'acc' only, without labels and predictions" % op)
+        if not torch.is_tensor(correct) or correct.dtype != torch.int64 or correct.numel() != 1 or correct.device.type != 'cuda':
+            raise EulerError("%s: correct must be an int64 CUDA scalar" % op)
+        if total is None or int(total) < 0:
+            raise EulerError("%s: total must be a count >= 0, got %r" % (op, total))
+        dev, n, correct = correct.device, int(total), correct.detach().reshape(()).contiguous()
+    _metric_tensors(op, [('state', state, torch.float32, (width,)), ('value', value, torch.float32, ())], dev)
+    _call("eu_metric_count_update", code, labels, predictions, n, correct, state, value)
+    return value
+
+
 # ------------------------------------------------------------------------------------ knowledge-graph embedding step
 KG_MODELS = {'transe': 0, 'transh': 1, 'transr': 2, 'transd': 3, 'distmult': 4}
 KG_CORRUPT = {'front': 1, 'tail': 2, 'both': 3}

@@ -8,15 +8,18 @@ are their submodules and solution.parameters() lists every trainable tensor.  __
 (embedding, loss, metric_name, metric).
 
 The step after the encoders is plain torch: PosNegLogits + xent_loss + the rank metric are unsupervised.py's composition
-(the rows already exist as encoder outputs, so a fused id-table op has nothing to save there).  Metrics are each batch's
-own value, where upstream's f1 / acc are streaming tf.metrics: 'f1' and 'acc' for SuperviseSolution, 'mrr', 'hit1', 'hit3',
-'hit10' and 'mr' for UnsuperviseSolution.  'auc' (tf.metrics.auc, a streaming histogram) is not provided.
+(the rows already exist as encoder outputs, so a fused id-table op has nothing to save there).  By default metrics are
+each batch's own value, where upstream's f1 / acc are streaming tf.metrics: 'f1' and 'acc' for SuperviseSolution, 'mrr',
+'hit1', 'hit3', 'hit10' and 'mr' for UnsuperviseSolution (per batch upstream too).  SuperviseSolution(..., streaming=True)
+takes upstream's streaming metrics instead -- 'f1', 'acc' or 'auc' (tf.metrics.auc at 5000 thresholds, applied to
+sigmoid(logit) with its own sigmoid, as upstream) -- as the device module solution.metric (euler_b200/metrics.py), whose
+value covers every batch since construction or solution.metric.reset().  Without streaming, 'auc' is refused.
 SuperviseSampleSolution / UnsuperviseSampleSolution, which parse text sample files on the host, are not provided either.
 """
 import torch
 import torch.nn.functional as F
 
-from . import ops
+from . import metrics, ops
 from .convolution import l2_normalize
 from .ops import SKIPGRAM_METRICS
 from .supervised import f1_score
@@ -77,14 +80,14 @@ def acc_score(labels, predict):
 SUPERVISED_METRICS = {'f1': f1_score, 'acc': acc_score}
 
 
-def _metric(name, metrics):
-    """the metric function of `name` among `metrics`; auc, upstream's streaming tf.metrics.auc, is refused with its reason"""
+def _metric(name, known):
+    """the metric function of `name` among `known`; auc, upstream's streaming tf.metrics.auc, is refused with its reason"""
     if name == 'auc':
         raise NotImplementedError("metric 'auc' is tf.metrics.auc, a streaming histogram over the session's batches, and is "
-                                  "not provided; use one of %s" % (sorted(metrics),))
-    if name not in metrics:
-        raise ValueError("metric_name must be one of %s, got %r" % (sorted(metrics), name))
-    return metrics[name]
+                                  "not provided; use one of %s" % (sorted(known),))
+    if name not in known:
+        raise ValueError("metric_name must be one of %s, got %r" % (sorted(known), name))
+    return known[name]
 
 
 # ------------------------------------------------------------------------------------ samplers
@@ -119,13 +122,19 @@ class SamplePosWithTypes(object):
 # ------------------------------------------------------------------------------------ solutions
 class SuperviseSolution(torch.nn.Module):
     """base_supervise.SuperviseSolution: label = get_label_fn(inputs), embedding = encoder_fn(inputs),
-    logit = logit_fn(embedding); loss_fn(label, logit) and the metric of (label, sigmoid(logit))."""
+    logit = logit_fn(embedding); loss_fn(label, logit) and the metric of (label, sigmoid(logit)).  streaming=True takes the
+    streaming metric solution.metric ('f1', 'acc' or 'auc'; see the top of the file)."""
 
-    def __init__(self, get_label_fn, encoder_fn, logit_fn, metric_name='f1', loss_fn=sigmoid_loss):
+    def __init__(self, get_label_fn, encoder_fn, logit_fn, metric_name='f1', loss_fn=sigmoid_loss, *, streaming=False):
         super().__init__()
         self.get_label_fn = get_label_fn
         self.metric_name = metric_name
-        self.metric_class = _metric(metric_name, SUPERVISED_METRICS)
+        self.streaming = bool(streaming)
+        if self.streaming:
+            self.metric = metrics.get(metric_name)
+            self.metric_class = None
+        else:
+            self.metric_class = _metric(metric_name, SUPERVISED_METRICS)
         self.encoder = encoder_fn
         self.logit_fn = logit_fn
         self.loss_fn = loss_fn
@@ -137,7 +146,7 @@ class SuperviseSolution(torch.nn.Module):
         label = self.get_label_fn(inputs)
         embedding = self.embed(inputs)
         logit = self.logit_fn(embedding)
-        metric = self.metric_class(label, torch.sigmoid(logit.detach()))
+        metric = (self.metric if self.streaming else self.metric_class)(label, torch.sigmoid(logit.detach()))
         loss = self.loss_fn(label, logit)
         return embedding, loss, self.metric_name, metric
 

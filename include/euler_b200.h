@@ -544,6 +544,40 @@ int eu_gae_loss_backward(eu_ctx* c, const float* grad_loss, int64_t B, int32_t K
                          const float* const* log_var, const float* const* noise, float radius, const float* logits,
                          float* const* grad_mu, float* const* grad_log_var);
 
+/* The streaming metrics of tf_euler/python/utils/metrics.py (auc_score, f1_score, acc_score), TF 1.x tf.metrics semantics:
+ * each call adds one batch's counts to f32 state the caller owns (device) and writes the value of the new state (device f32
+ * scalar), as the metric's update op returns it.  Every per-batch count is an exact integer, rounded once to f32 and added to
+ * the state with one f32 add: TF's float reduce_sum gives the same counts for batches below 2^24 elements.  Labels and
+ * predictions are f32[N] device arrays; a label is positive when nonzero (NaN included).  Neither call synchronises with the
+ * host (once the ctx scratch, O(T), has grown) and neither uses float atomics: the bits depend on the inputs only, and both
+ * can be captured in a CUDA graph.
+ *
+ * eu_metric_auc_update: tf.metrics.auc(labels, predictions, num_thresholds=T), trapezoidal ROC.  Thresholds t[0] =
+ * fl32(-1e-7), t[i] = fl32(i / (T - 1)) for 0 < i < T - 1 (computed in double), t[T-1] = fl32(1 + 1e-7); prediction p is
+ * positive at threshold i iff p > t[i] in f32.  The state is tp, fn, tn, fp f32[T].  Each prediction is bucketed once and
+ * counted in integer histograms; prefix sums give the per-threshold counts.  The value, with eps = 1e-6,
+ *   rec[i] = (tp + eps) / ((tp + fn) + eps),  fpr[i] = fp / ((fp + tn) + eps),
+ *   auc = sum over i < T - 1 of (fpr[i] - fpr[i+1]) ((rec[i] + rec[i+1]) / 2),
+ * each op one round-to-nearest f32 op, is summed in this fixed order: lane j of 1024 adds the terms j, j + 1024, .. from +0
+ * left to right, then the 1024 lane sums are added by a tree (lane j += lane j + s for s = 512, 256, .., 1); the result is
+ * lane 0.  A batch with a prediction outside [0, 1] or NaN (TF asserts) is not counted: the state is untouched and
+ * *refused (device i64) += 1.  The value is NaN while *refused > 0.  N = 0 counts nothing and rewrites the value.
+ * T < 2 or T > EU_METRIC_AUC_MAX_THRESHOLDS, N < 0, or a NULL pointer that is needed: EU_ERR_INVALID, before any device work.
+ *
+ * eu_metric_count_update: kind EU_METRIC_F1 (state f32[3] = tp, fn, fp; predictions floor(p + 0.5) in f32 cast to bool,
+ * NaN true; value p = tp / ((1e-7 + tp) + fp), r = tp / ((1e-7 + tp) + fn), f1 = ((2 p) r) / ((p + r) + 1e-7)) or
+ * EU_METRIC_ACC (state f32[2] = total, count; total += #{floor(p + 0.5) == label}, count += N; value total / count, 0 while
+ * count is 0).  With correct (a device i64 scalar) instead of labels and predictions, for EU_METRIC_ACC only, total +=
+ * *correct and count += N: a count the caller already has, e.g. eu_gae_loss's, with no second pass.
+ * An unknown kind, N < 0, a NULL pointer that is needed, or correct with labels, predictions or EU_METRIC_F1: EU_ERR_INVALID,
+ * before any device work. */
+#define EU_METRIC_AUC_MAX_THRESHOLDS 16384
+enum { EU_METRIC_F1 = 0, EU_METRIC_ACC = 1 };
+int eu_metric_auc_update(eu_ctx* c, const float* labels, const float* predictions, int64_t N, int32_t T, float* tp, float* fn,
+                         float* tn, float* fp, int64_t* refused, float* value);
+int eu_metric_count_update(eu_ctx* c, int32_t kind, const float* labels, const float* predictions, int64_t N,
+                           const int64_t* correct, float* state, float* value);
+
 /* The knowledge-graph embedding step of TransE / TransH / TransR / TransD (examples/TransX) and DistMult (examples/distmult),
  * fused: the mapped id rows of each triple and of its corrupted triples, the scores, the margin loss and the rank.
  * Triple b: src_b, dst_b (entity ids), rel_b (relation id), neg[b, 0 .. K-1] (entity ids); ids are table rows.
