@@ -13,3 +13,4 @@ from .ops import (adjacency_mean, agnn_attention_aggregate, context, dna_attenti
                   initialize_graph, neighbor_top_k_feature, random_walk, relation_mean_aggregate, sage_mean_aggregate, sample_fanout, sample_fanout_batched, sample_fanout_with_feature,
                   sample_edge, sample_neighbor, sample_neighbor_api, sample_neighbor_layerwise, sample_neighbor_layerwise_coo, sample_n_with_types, sample_node, sample_node_with_src, scatter_, scatter_add, scatter_max, scatter_mean,
                   scatter_softmax, seed, set_graph, shallow_encode, shallow_encode_pool, skipgram_xent_loss, sparse_feature_embedding, sparse_get_adj, sparse_get_adj_coo, store_accumulate, store_exchange, unique)
+from . import optimizers  # noqa: F401,E402  (tf_euler.utils.optimizers: get, MomentumOptimizer, AdagradOptimizer, AdamOptimizer)

@@ -56,6 +56,7 @@ SHALLOW_POOL_MAX_COUNT = 512   # EU_SHALLOW_POOL_MAX_COUNT
 NEIGHBOR_TOP_K_MAX = 16   # EU_NEIGHBOR_TOP_K_MAX
 METRIC_AUC_MAX_THRESHOLDS = 16384   # EU_METRIC_AUC_MAX_THRESHOLDS
 METRIC_F1, METRIC_ACC = 0, 1   # EU_METRIC_F1, EU_METRIC_ACC
+OPTIM_DENSE = -1   # EU_OPTIM_DENSE
 
 
 class ShallowDense(C.Structure):
@@ -226,6 +227,9 @@ SIGNATURES = {
     "eu_gae_loss_backward": (C.c_int, [_P, _P, _I64, _I32, _I32, _P, _P, _P, _F, _P, _P, _P]),
     "eu_metric_auc_update": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
     "eu_metric_count_update": (C.c_int, [_P, _I32, _P, _P, _I64, _P, _P, _P]),
+    "eu_optim_momentum": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _I64, _F, _F]),
+    "eu_optim_adagrad": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _I64, _F]),
+    "eu_optim_adam": (C.c_int, [_P, _P, _P, _P, _I64, _I32, _P, _P, _I64, _P, _F, _F, _F, _F]),
     "eu_kg_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "eu_kg_loss_backward": (C.c_int, [_P, _P, _P, _P, _P]),
     "eu_kg_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),

@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libeuler_b200.so")
-SOURCES = ["graph.cu", "loader.cu", "sample.cu", "walk.cu", "neighbor.cu", "unique.cu", "full_hop.cu", "mp_ops.cu", "gat.cu", "relation.cu", "dna.cu", "segment.cu", "adjacency.cu", "graph_adjacency.cu", "store.cu", "top_k.cu", "embedding.cu", "graph_label.cu", "readout.cu", "skipgram.cu", "gae.cu", "metrics.cu", "kg.cu", "features.cu", "edges.cu", "layerwise.cu", "shard.cu", "p2p.cu", "capi.cu", "host_abi.cu"]
+SOURCES = ["graph.cu", "loader.cu", "sample.cu", "walk.cu", "neighbor.cu", "unique.cu", "full_hop.cu", "mp_ops.cu", "gat.cu", "relation.cu", "dna.cu", "segment.cu", "adjacency.cu", "graph_adjacency.cu", "store.cu", "top_k.cu", "embedding.cu", "graph_label.cu", "readout.cu", "skipgram.cu", "gae.cu", "metrics.cu", "optim.cu", "kg.cu", "features.cu", "edges.cu", "layerwise.cu", "shard.cu", "p2p.cu", "capi.cu", "host_abi.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "--expt-relaxed-constexpr"]
 

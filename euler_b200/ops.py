@@ -1805,6 +1805,70 @@ def metric_count_update(kind, state, value, labels=None, predictions=None, corre
     return value
 
 
+# ------------------------------------------------------------------------------------ optimizers
+def _optim_args(op, var, slots, grad):
+    """the library's (N, D, values, rows, R) for one update of var and its slots (same shape, float32, contiguous, on the
+    graph's device): a dense grad of var's shape is taken as f32[N, D] over var's elements; a sparse COO grad of var's shape
+    with one sparse dimension (coalesced here when it is not) as its rows i64[R] and values f32[R, D], D the elements of a row
+    of var.  Raises EulerError before any device work."""
+    dev = _dev()
+    for nm, t in (('var', var),) + slots:
+        if not torch.is_tensor(t) or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous() or t.is_sparse:
+            raise EulerError("%s: %s must be a contiguous float32 tensor on %s" % (op, nm, dev))
+        if t.shape != var.shape:
+            raise EulerError("%s: %s has shape %s, var %s" % (op, nm, tuple(t.shape), tuple(var.shape)))
+    if not torch.is_tensor(grad) or grad.dtype != torch.float32 or grad.device != dev or grad.shape != var.shape:
+        raise EulerError("%s: grad must be a float32 tensor of var's shape %s on %s" % (op, tuple(var.shape), dev))
+    grad = grad.detach()
+    if not grad.is_sparse:
+        n = var.numel()
+        D = 4 if n % 4 == 0 else 1   # element-wise: a row width of 4 lets an aligned update take float4s
+        return n // D, D, grad.contiguous(), None, _lib.OPTIM_DENSE
+    if grad.layout != torch.sparse_coo or grad.sparse_dim() != 1 or var.dim() < 1:
+        raise EulerError("%s: a sparse grad must be a COO tensor with one sparse dimension (rows of var)" % op)
+    if not grad.is_coalesced():
+        grad = grad.coalesce()
+    N = var.shape[0]
+    D = var.numel() // N if N else math.prod(var.shape[1:])
+    rows = grad._indices()[0].contiguous()
+    return N, D, grad._values().reshape(rows.numel(), D).contiguous(), rows, rows.numel()
+
+
+def optim_momentum_(var, accum, grad, lr, momentum):
+    """One step of TF 1.x MomentumOptimizer (non-Nesterov) on var in place, no autograd: accum = accum * momentum + g,
+    var = var - lr * accum, each op one f32 rounding.  A dense grad updates every element (apply_momentum); a sparse COO grad
+    (sparse_apply_momentum) only its rows, after coalesce() when it is not coalesced.  var, accum: contiguous float32 of one
+    shape on the graph's device.  No host synchronisation for a dense or coalesced grad (include/euler_b200.h,
+    eu_optim_momentum); shape, dtype and device mismatches raise EulerError and write nothing.  Returns var."""
+    N, D, g, rows, R = _optim_args("optim_momentum_", var, (('accum', accum),), grad)
+    _call("eu_optim_momentum", var, accum, N, D, g, rows, R, float(lr), float(momentum))
+    return var
+
+
+def optim_adagrad_(var, accum, grad, lr):
+    """One step of TF 1.x AdagradOptimizer on var in place, no autograd: accum = accum + g * g, var = var - (lr * g) *
+    (1 / sqrt(accum)), each op one f32 rounding.  Dense grads update every element (apply_adagrad), sparse COO grads their
+    rows only (sparse_apply_adagrad), as optim_momentum_ (include/euler_b200.h, eu_optim_adagrad).  Returns var."""
+    N, D, g, rows, R = _optim_args("optim_adagrad_", var, (('accum', accum),), grad)
+    _call("eu_optim_adagrad", var, accum, N, D, g, rows, R, float(lr))
+    return var
+
+
+def optim_adam_(var, m, v, grad, powers, lr, beta1, beta2, epsilon):
+    """One step of TF 1.x AdamOptimizer on var in place, no autograd, with alpha = (lr * sqrt(1 - powers[1])) /
+    (1 - powers[0]) computed on the device from powers (float32[2]: beta1_power, beta2_power, on var's device).  A dense grad
+    runs ApplyAdam: m = m + (g - m) * (1 - b1), v = v + (g * g - v) * (1 - b2), var = var - (m * alpha) / (sqrt(v) + eps).  A
+    sparse COO grad (coalesced first when it is not) runs _apply_sparse_shared over EVERY row: m = m * b1 and v = v * b2, plus
+    g * (1 - b1) and (g * g) * (1 - b2) on the grad's rows, then var = var - (alpha * m) / (sqrt(v) + eps).  Each op is one f32
+    rounding.  The powers are not advanced here: the caller multiplies each by its beta once per step, after every variable
+    (TF's _finish).  Checks and synchronisation as optim_momentum_ (include/euler_b200.h, eu_optim_adam).  Returns var."""
+    op = "optim_adam_"
+    N, D, g, rows, R = _optim_args(op, var, (('m', m), ('v', v)), grad)
+    _metric_tensors(op, [('powers', powers, torch.float32, (2,))], var.device)
+    _call("eu_optim_adam", var, m, v, N, D, g, rows, R, powers, float(lr), float(beta1), float(beta2), float(epsilon))
+    return var
+
+
 # ------------------------------------------------------------------------------------ knowledge-graph embedding step
 KG_MODELS = {'transe': 0, 'transh': 1, 'transr': 2, 'transd': 3, 'distmult': 4}
 KG_CORRUPT = {'front': 1, 'tail': 2, 'both': 3}

@@ -578,6 +578,33 @@ int eu_metric_auc_update(eu_ctx* c, const float* labels, const float* prediction
 int eu_metric_count_update(eu_ctx* c, int32_t kind, const float* labels, const float* predictions, int64_t N,
                            const int64_t* correct, float* state, float* value);
 
+/* tf_euler's optimizers (utils/optimizers.py: sgd and momentum = MomentumOptimizer(lr, 0 / 0.9), AdagradOptimizer,
+ * AdamOptimizer) as TF 1.x applies them, in place over var f32[N, D] and its slot tables (accum, or m and v) of the same
+ * shape, on the ctx's stream.  All arithmetic is f32, each op rounded once in the order written, no FMA contraction;
+ * rsqrt(a) = 1 / sqrt(a).
+ * The gradient is dense (R = EU_OPTIM_DENSE: grad f32[N, D]) or sparse (R >= 0: rows i64[R], sorted and unique in [0, N),
+ * as a coalesced COO gradient has them, and grad f32[R, D]; TF sums duplicate IndexedSlices first).
+ *   Momentum (non-Nesterov): accum = accum * momentum + g; var = var - lr * accum.  Sparse: the R rows only.
+ *   Adagrad: accum = accum + g * g; var = var - (lr * g) * rsqrt(accum).  Sparse: the R rows only.
+ *   Adam, dense (ApplyAdam): m = m + (g - m) * (1 - b1); v = v + (g * g - v) * (1 - b2);
+ *     var = var - (m * alpha) / (sqrt(v) + eps).
+ *   Adam, sparse (_apply_sparse_shared), EVERY row: m = m * b1, then on the R rows m = m + g * (1 - b1); v = v * b2, then on
+ *     the R rows v = v + (g * g) * (1 - b2); var = var - (alpha * m) / (sqrt(v) + eps).
+ *   alpha = (lr * sqrt(1 - beta2_power)) / (1 - beta1_power), computed on the device from powers (device f32[2]:
+ *   beta1_power, beta2_power).  The caller multiplies each power by its beta once after every variable of a step (TF's
+ *   _finish).
+ * Sparse Adam is one pass over the table (24 N D + 4 R (D + 2) bytes); sparse Momentum and Adagrad touch the R rows only.
+ * A sparse row outside [0, N) is never written.  No host synchronisation and no float atomics: every call can be captured
+ * in a CUDA graph.  N < 0, D < 1, R < EU_OPTIM_DENSE, R > N, or a NULL pointer that is needed: EU_ERR_INVALID, before any
+ * device work.  Device pointers. */
+#define EU_OPTIM_DENSE (-1)
+int eu_optim_momentum(eu_ctx* c, float* var, float* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                      int64_t R, float lr, float momentum);
+int eu_optim_adagrad(eu_ctx* c, float* var, float* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                     int64_t R, float lr);
+int eu_optim_adam(eu_ctx* c, float* var, float* m, float* v, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                  int64_t R, const float* powers, float lr, float beta1, float beta2, float epsilon);
+
 /* The knowledge-graph embedding step of TransE / TransH / TransR / TransD (examples/TransX) and DistMult (examples/distmult),
  * fused: the mapped id rows of each triple and of its corrupted triples, the scores, the margin loss and the rank.
  * Triple b: src_b, dst_b (entity ids), rel_b (relation id), neg[b, 0 .. K-1] (entity ids); ids are table rows.
