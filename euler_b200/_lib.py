@@ -12,6 +12,9 @@ SO_PATH = os.path.join(_HERE, "lib", "libeuler_b200.so")
 EU_RNG_MINSTD = 0
 EU_RNG_PHILOX = 1
 
+# eu_feat_dtype: the storage type of a graph's dense node feature table, by name
+FEAT_DTYPES = {"float32": 0, "bfloat16": 1}
+
 
 class EulerError(RuntimeError):
     pass
@@ -92,7 +95,15 @@ SIGNATURES = {
                                              C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "eu_graph_create_rmat_hetero": (C.c_int, [_I64, _I64, _I32, _I32, C.c_double, C.c_double, C.c_double, _U64, _I32, _U64,
                                               C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
+    "eu_graph_create_dtype": (C.c_int, [C.POINTER(GraphDesc), C.c_int, _I32, C.POINTER(_P)]),
+    "eu_graph_create_rmat_dtype": (C.c_int, [_I64, _I64, C.c_double, C.c_double, C.c_double, _U64, _I32, _U64,
+                                             C.c_int, _I32, C.POINTER(_P)]),
+    "eu_graph_create_rmat_shard_dtype": (C.c_int, [_I64, _I64, C.c_double, C.c_double, C.c_double, _U64, _I32, _U64,
+                                                   C.c_int, C.c_int, C.c_int, _I32, C.POINTER(_P)]),
+    "eu_graph_create_rmat_hetero_dtype": (C.c_int, [_I64, _I64, _I32, _I32, C.c_double, C.c_double, C.c_double, _U64, _I32,
+                                                    _U64, C.c_int, C.c_int, C.c_int, _I32, C.POINTER(_P)]),
     "eu_graph_load": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
+    "eu_graph_load_dtype": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, _I32, C.POINTER(_P)]),
     "eu_graph_load_ex": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "eu_graph_set_edges": (C.c_int, [_P, _P]),
     "eu_graph_num_edge_records": (_I64, [_P]),
@@ -109,6 +120,7 @@ SIGNATURES = {
     "eu_graph_num_edge_types": (_I32, [_P]),
     "eu_graph_num_node_types": (_I32, [_P]),
     "eu_graph_feat_dim": (_I32, [_P]),
+    "eu_graph_feat_dtype": (_I32, [_P]),
     "eu_graph_hbm_bytes": (_I64, [_P]),
     "eu_graph_export": (C.c_int, [_P] * 9),
     "eu_graph_edge_type_id": (_I32, [_P, C.c_char_p]),

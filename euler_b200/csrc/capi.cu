@@ -294,8 +294,14 @@ bool InitQueryProxy(const char* conf) {
   int device = kv.count("device") ? atoi(kv["device"].c_str()) : 0;
   uint64_t seed = kv.count("seed") ? strtoull(kv["seed"].c_str(), nullptr, 10) : 1;
   eu_rng_kind rng = (kv.count("rng") && kv["rng"] == "philox") ? EU_RNG_PHILOX : EU_RNG_MINSTD;
+  // feature_dtype: the dense node feature table's storage type (eu_graph_load_dtype); float32 when absent
+  const std::string fdt = kv.count("feature_dtype") ? kv["feature_dtype"] : "float32";
+  if (fdt != "float32" && fdt != "bfloat16") {
+    fprintf(stderr, "[euler_b200] ERROR InitQueryProxy: feature_dtype=%s is not float32 or bfloat16\n", fdt.c_str());
+    return true;
+  }
   eu_graph* g = nullptr;
-  int rc = eu_graph_load(kv["data_path"].c_str(), 0, 1, device, &g);
+  int rc = eu_graph_load_dtype(kv["data_path"].c_str(), 0, 1, device, 1, fdt == "bfloat16" ? EU_FEAT_BF16 : EU_FEAT_F32, &g);
   if (rc != EU_OK) {
     fprintf(stderr, "[euler_b200] ERROR InitQueryProxy: graph load failed: %s\n", eu_last_error());
     return true;

@@ -6,6 +6,7 @@
 //   * Philox4x32-10 keyed on (node id, draw) for the throughput mode
 //   * inverse-CDF pick equivalent to RandomSelect (euler/common/compact_weighted_collection.h:30-52)
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -42,9 +43,11 @@ struct DevGraph {
   unsigned long long id_stride;   // 1, or the shard count for a shard's rows (ids congruent mod shards)
   const HashSlot* htab;
   unsigned long long hmask;       // capacity-1 (capacity is a power of two)
-  // dense f32 features: row-major [n, feat_dim]; slot s occupies columns [slot_off[s], +slot_dim[s])
+  // dense features: row-major [n, feat_dim] of feat_dtype (EU_FEAT_F32: float, EU_FEAT_BF16: __nv_bfloat16), read only
+  // through feat_cols / feat_ld / feat_ld4; slot s occupies columns [slot_off[s], +slot_dim[s])
   int32_t feat_dim;
-  const float* feat;
+  int32_t feat_dtype;             // fills the padding after feat_dim: every other member keeps its offset
+  const void* feat;
   int32_t n_slots;
   int32_t slot_off[EU_MAX_FEAT_SLOTS];
   int32_t slot_dim[EU_MAX_FEAT_SLOTS];
@@ -125,6 +128,34 @@ __host__ __device__ __forceinline__ void dense_slot(const DevGraph& g, int32_t f
   *off = have ? g.slot_off[fid] : 0;
   *width = have ? g.slot_dim[fid] : 0;
 }
+
+// ---------------------------------------------------------------------------------- dense feature storage
+// The one place that knows how a dense feature table is stored.  A kernel that reads rows is instantiated for its storage
+// type T (float or __nv_bfloat16), takes the table as feat_cols<T>(g) and loads columns with feat_ld (one) or feat_ld4 (four
+// consecutive, one 16-byte f32 / 8-byte bf16 load: the address must be aligned to four elements).  Both return f32;
+// widening bf16 is exact (its bits are the upper half of the f32's).  A bf16 table is written only through feat_st, the
+// device's round to nearest even: NaN becomes the canonical NaN, +-Inf stays, a finite value becomes +-Inf only where the
+// rounding says so, and subnormals round like any other value.
+template <typename T>
+__host__ __device__ __forceinline__ const T* feat_cols(const DevGraph& g) { return static_cast<const T*>(g.feat); }
+
+template <typename T> __device__ __forceinline__ float feat_ld(const T* p);
+template <> __device__ __forceinline__ float feat_ld<float>(const float* p) { return __ldg(p); }
+template <> __device__ __forceinline__ float feat_ld<__nv_bfloat16>(const __nv_bfloat16* p) {
+  return __uint_as_float((uint32_t)__ldg(reinterpret_cast<const unsigned short*>(p)) << 16);
+}
+
+template <typename T> __device__ __forceinline__ float4 feat_ld4(const T* p);
+template <> __device__ __forceinline__ float4 feat_ld4<float>(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+template <> __device__ __forceinline__ float4 feat_ld4<__nv_bfloat16>(const __nv_bfloat16* p) {
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));   // columns 0..3: the low and high halves of x, then of y
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xFFFF0000u));
+}
+
+template <typename T> __device__ __forceinline__ T feat_st(float v);
+template <> __device__ __forceinline__ float feat_st<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 feat_st<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
 // Row `row`'s slice of ragged slot `fid` (ptr of S slots per row): [b, e) in the value array, b == e when the node / slot does
 // not exist

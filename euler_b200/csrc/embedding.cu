@@ -173,7 +173,8 @@ __device__ __forceinline__ void shallow_slot(const DevGraph& g, const ShallowDev
 
 // G lanes per node r: the id columns, the dense slots (k_feature's rule: the stored columns, zeros past them, zeros for an
 // absent node or an unknown slot), then the sparse slots.  The group syncs between parts: a part may map columns to lanes
-// differently from the one before it, and ADD reads what the previous part wrote.
+// differently from the one before it, and ADD reads what the previous part wrote.  T: the dense table's storage type.
+template <typename T>
 __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, int G) {
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t r = tid >> (31 - __clz(G));
@@ -193,9 +194,9 @@ __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, i
     const int32_t fid = p.dense_fid[j];
     const bool have = fid >= 0 && fid < g.n_slots && row >= 0;
     const int sdim = have ? g.slot_dim[fid] : 0;
-    const float* f = g.feat + (have ? row * (int64_t)g.feat_dim + g.slot_off[fid] : 0);
+    const T* f = feat_cols<T>(g) + (have ? row * (int64_t)g.feat_dim + g.slot_off[fid] : 0);
     float* oj = od + p.dense_off[j];
-    for (int d = sub; d < p.dense_dim[j]; d += G) oj[d] = d < sdim ? __ldg(f + d) : 0.f;
+    for (int d = sub; d < p.dense_dim[j]; d += G) oj[d] = d < sdim ? feat_ld(f + d) : 0.f;
   }
   for (int s = 0; s < p.n_sparse; ++s) {
     __syncwarp(gm);
@@ -248,6 +249,7 @@ __device__ __forceinline__ void shallow_pool_slot(const DevGraph& g, const Shall
 // G lanes per output row r, the pool of the `count` ShallowEncoder rows (CONCAT) of nodes[r * count ..]: k_shallow_fwd's
 // parts and rules, each column summed over the segment's nodes in a register, in node order, and divided once by pool_den
 // (fl(count); 0: the sum).  The group looks every node's graph row up once, into its `count` slots of shared memory.
+template <typename T>
 __global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev p, int count, float pool_den, int G) {
   extern __shared__ int64_t pool_rows[];
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -271,10 +273,10 @@ __global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev 
     const int32_t fid = p.dense_fid[k];
     const bool known = fid >= 0 && fid < g.n_slots;
     const int sdim = known ? g.slot_dim[fid] : 0;
-    const float* f = g.feat + (known ? g.slot_off[fid] : 0);
+    const T* f = feat_cols<T>(g) + (known ? g.slot_off[fid] : 0);
     float* oj = o + p.dense_off[k];
     for (int d = sub; d < p.dense_dim[k]; d += G)
-      oj[d] = finish(pool_column(count, [&](int j) { return d < sdim && rows[j] >= 0 ? __ldg(f + rows[j] * (int64_t)g.feat_dim + d) : 0.f; }));
+      oj[d] = finish(pool_column(count, [&](int j) { return d < sdim && rows[j] >= 0 ? feat_ld(f + rows[j] * (int64_t)g.feat_dim + d) : 0.f; }));
   }
   for (int s = 0; s < p.n_sparse; ++s) {
     if (p.vec_mask >> s & 1) shallow_pool_slot<true>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
@@ -769,7 +771,9 @@ int eu_shallow_encode(eu_ctx* c, const eu_shallow_problem* p, float* out, float*
   d.dense_out = dense_out;
   const int G = shallow_lanes(&d, out);
   EuProfScope ps(c, "shallow_fwd", p->M);
-  k_shallow_fwd<<<(unsigned)ceil_div(p->M * G, 256), 256, 0, c->stream>>>(c->g->d, d, G);
+  const unsigned blocks = (unsigned)ceil_div(p->M * G, 256);
+  if (c->g->d.feat_dtype == EU_FEAT_BF16) k_shallow_fwd<__nv_bfloat16><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+  else k_shallow_fwd<float><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -813,8 +817,10 @@ int eu_shallow_encode_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t count
   while ((256 / G) * (size_t)count * sizeof(int64_t) > 48 * 1024) G *= 2;
   const int64_t R = p->M / count;
   EuProfScope ps(c, "shallow_pool", p->M);
-  k_shallow_pool<<<(unsigned)ceil_div(R * G, 256), 256, (256 / G) * (size_t)count * sizeof(int64_t), c->stream>>>(c->g->d, d, count,
-                                                                                                              gr.pool_den, G);
+  const unsigned blocks = (unsigned)ceil_div(R * G, 256);
+  const size_t smem = (256 / G) * (size_t)count * sizeof(int64_t);
+  if (c->g->d.feat_dtype == EU_FEAT_BF16) k_shallow_pool<__nv_bfloat16><<<blocks, 256, smem, c->stream>>>(c->g->d, d, count, gr.pool_den, G);
+  else k_shallow_pool<float><<<blocks, 256, smem, c->stream>>>(c->g->d, d, count, gr.pool_den, G);
   EU_LAUNCHED();
   return EU_OK;
 }

@@ -146,8 +146,10 @@ __global__ void k_iota_ids(unsigned long long* ids, int32_t* ntype, float* nw, i
   nw[r] = 1.0f;
 }
 
-// feat[row, d] = U(-1,1) from a hash of (global node index, d): identical on every shard layout
-__global__ void k_fill_feat(float* feat, int64_t n_local, int32_t dim, unsigned long long seed, unsigned long long base_id,
+// feat[row, d] = U(-1,1) from a hash of (global node index, d): identical on every shard layout.  A bf16 table holds that f32
+// value rounded (feat_st).
+template <typename T>
+__global__ void k_fill_feat(T* feat, int64_t n_local, int32_t dim, unsigned long long seed, unsigned long long base_id,
                             unsigned long long stride) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t total = n_local * (int64_t)dim;
@@ -156,8 +158,13 @@ __global__ void k_fill_feat(float* feat, int64_t n_local, int32_t dim, unsigned 
     const unsigned long long row = (unsigned long long)(i / dim), col = (unsigned long long)(i % dim);
     const unsigned long long gi = (base_id + row * stride - 1) * (unsigned long long)dim + col;
     unsigned long long h = mix64(seed ^ (gi * 0x9E3779B97F4A7C15ull));
-    feat[i] = (float)((double)(h >> 11) * (2.0 / 9007199254740992.0) - 1.0);
+    feat[i] = feat_st<T>((float)((double)(h >> 11) * (2.0 / 9007199254740992.0) - 1.0));
   }
+}
+
+__global__ void k_feat_round(const float* __restrict__ src, int64_t n, __nv_bfloat16* __restrict__ dst) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += step) dst[i] = feat_st<__nv_bfloat16>(src[i]);
 }
 
 // adj_sorted: lets the node2vec step classify neighbors by merging sorted lists in parallel
@@ -213,6 +220,43 @@ static int upload(eu_graph* g, const T** dst, const T* src, int64_t count) {
   if (rc) return rc;
   if (count > 0) EU_CUDA(cudaMemcpy(p, src, sizeof(T) * (size_t)count, cudaMemcpyHostToDevice));
   *dst = p;
+  return EU_OK;
+}
+
+static bool feat_dtype_ok(int32_t dtype) { return dtype == EU_FEAT_F32 || dtype == EU_FEAT_BF16; }
+
+// The host f32 table [count] into a device table of d.feat_dtype.  bf16: f32 chunks go up through one device buffer and are
+// rounded there (k_feat_round), so the peak is the bf16 table plus one chunk and the device's rounding is the only one.
+static int upload_feat(eu_graph* g, const float* src, int64_t count) {
+  DevGraph& d = g->d;
+  if (d.feat_dtype == EU_FEAT_F32) {
+    const float* p = nullptr;
+    const int rc = upload(g, &p, src, count);
+    d.feat = p;
+    return rc;
+  }
+  __nv_bfloat16* p = nullptr;
+  int rc = g->alloc(&p, count);
+  if (rc) return rc;
+  d.feat = p;
+  if (count == 0) return EU_OK;
+  constexpr int64_t kChunk = (int64_t)1 << 24;   // f32 elements per chunk: 64 MB
+  const int64_t chunk = std::min(count, kChunk);
+  float* stage = nullptr;
+  EU_CUDA(cudaMalloc(&stage, sizeof(float) * (size_t)chunk));
+  cudaError_t e = cudaSuccess;
+  for (int64_t off = 0; off < count && e == cudaSuccess; off += chunk) {   // one stream: a chunk is rounded before the next lands
+    const int64_t m = std::min(chunk, count - off);
+    e = cudaMemcpy(stage, src + off, sizeof(float) * (size_t)m, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+      k_feat_round<<<(unsigned)std::min<int64_t>(ceil_div(m, 256), kSMs * 8), 256>>>(stage, m, p + off);
+      g_launches++;
+      e = cudaGetLastError();
+    }
+  }
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  cudaFree(stage);
+  if (e != cudaSuccess) { set_error("feature upload: %s", cudaGetErrorString(e)); return EU_ERR_CUDA; }
   return EU_OK;
 }
 
@@ -350,7 +394,12 @@ const char* eu_version(void) { return "euler_b200 0.1 (sm_90a)"; }
 uint64_t eu_launch_count(void) { return eu::g_launches.load(); }
 
 int eu_graph_create(const eu_graph_desc* desc, int device, eu_graph** out) {
+  return eu_graph_create_dtype(desc, device, EU_FEAT_F32, out);
+}
+
+int eu_graph_create_dtype(const eu_graph_desc* desc, int device, int32_t feat_dtype, eu_graph** out) {
   if (!desc || !out) { set_error("null argument"); return EU_ERR_INVALID; }
+  if (!feat_dtype_ok(feat_dtype)) { set_error("eu_graph_create: unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; }
   if (desc->n_nodes < 0 || desc->n_edge_types < 1 || desc->n_edge_types > EU_MAX_ETYPES ||
       !desc->ids || !desc->grp_ptr || (!desc->cum_w && !desc->w && desc->grp_ptr[desc->n_nodes * desc->n_edge_types] > 0) ||
       (desc->cum_w && desc->n_edge_types > 1 && !desc->grp_cum)) {
@@ -401,7 +450,8 @@ int eu_graph_create(const eu_graph_desc* desc, int device, eu_graph** out) {
     d.grp_cum = gc;
   }
   d.feat_dim = desc->feat ? desc->feat_dim : 0;
-  if (d.feat_dim > 0) TRY(upload(g, &d.feat, desc->feat, n * (int64_t)d.feat_dim));
+  d.feat_dtype = feat_dtype;
+  if (d.feat_dim > 0) TRY(upload_feat(g, desc->feat, n * (int64_t)d.feat_dim));
   if (d.feat_dim > 0) {
     if (desc->n_feat_slots > 0) {
       if (desc->n_feat_slots > EU_MAX_FEAT_SLOTS || !desc->feat_slot_dims) { set_error("bad feature slots"); eu_graph_destroy(g); return EU_ERR_INVALID; }
@@ -454,7 +504,8 @@ int eu_graph_create(const eu_graph_desc* desc, int device, eu_graph** out) {
 // of the shards is exactly the unsharded graph.
 static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
                        int32_t feat_dim, uint64_t feat_seed, int device, int shard_index, int shard_number,
-                       int T, int NT, eu_graph** out) {
+                       int T, int NT, int32_t feat_dtype, eu_graph** out) {
+  if (!feat_dtype_ok(feat_dtype)) { set_error("eu_graph_create_rmat: unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; }
   if (!out || n_nodes <= 0 || n_edges < 0 || shard_number < 1 || shard_index < 0 || shard_index >= shard_number ||
       T < 1 || T > EU_MAX_ETYPES || NT < 1 || NT > EU_MAX_ETYPES || (double)n_nodes * (double)n_nodes * T >= 9.2e18) {
     set_error("eu_graph_create_rmat: bad sizes"); return EU_ERR_INVALID;
@@ -544,12 +595,20 @@ static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, dou
   d.grp_cum = gcum;
   d.dense_ids = 1; d.id_base = (unsigned long long)base_id; d.id_stride = (unsigned long long)N;
   d.feat_dim = feat_dim;
+  d.feat_dtype = feat_dtype;
   if (feat_dim > 0) {
-    float* feat = nullptr;
-    TRY(g->alloc(&feat, n_local * (int64_t)feat_dim));
-    k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
+    if (feat_dtype == EU_FEAT_BF16) {
+      __nv_bfloat16* feat = nullptr;
+      TRY(g->alloc(&feat, n_local * (int64_t)feat_dim));
+      k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
+      d.feat = feat;
+    } else {
+      float* feat = nullptr;
+      TRY(g->alloc(&feat, n_local * (int64_t)feat_dim));
+      k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
+      d.feat = feat;
+    }
     g_launches++;
-    d.feat = feat;
     d.n_slots = 1; d.slot_off[0] = 0; d.slot_dim[0] = feat_dim;
     g->dense_feature_names.push_back("feat0");
   }
@@ -565,20 +624,40 @@ static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, dou
 int eu_graph_create_rmat(int64_t n_nodes, int64_t n_edges, double a, double b, double c,
                          uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                          eu_graph** out) {
-  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, out);
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, EU_FEAT_F32, out);
 }
 
 int eu_graph_create_rmat_hetero(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
                                 double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                 int shard_index, int shard_number, eu_graph** out) {
   return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, n_edge_types,
-                     n_node_types, out);
+                     n_node_types, EU_FEAT_F32, out);
 }
 
 int eu_graph_create_rmat_shard(int64_t n_nodes, int64_t n_edges, double a, double b, double c,
                                uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                int shard_index, int shard_number, eu_graph** out) {
-  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, out);
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, EU_FEAT_F32,
+                     out);
+}
+
+int eu_graph_create_rmat_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed, int32_t feat_dim,
+                               uint64_t feat_seed, int device, int32_t feat_dtype, eu_graph** out) {
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, feat_dtype, out);
+}
+
+int eu_graph_create_rmat_shard_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
+                                     int32_t feat_dim, uint64_t feat_seed, int device, int shard_index, int shard_number,
+                                     int32_t feat_dtype, eu_graph** out) {
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, feat_dtype,
+                     out);
+}
+
+int eu_graph_create_rmat_hetero_dtype(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
+                                      double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
+                                      int shard_index, int shard_number, int32_t feat_dtype, eu_graph** out) {
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, n_edge_types,
+                     n_node_types, feat_dtype, out);
 }
 
 int eu_graph_destroy(eu_graph* g) {
@@ -594,6 +673,7 @@ int64_t eu_graph_num_edges(const eu_graph* g) { return g ? g->d.E : -1; }
 int32_t eu_graph_num_edge_types(const eu_graph* g) { return g ? g->d.T : -1; }
 int32_t eu_graph_num_node_types(const eu_graph* g) { return g ? g->d.n_node_types : -1; }
 int32_t eu_graph_feat_dim(const eu_graph* g) { return g ? g->d.feat_dim : -1; }
+int32_t eu_graph_feat_dtype(const eu_graph* g) { return g ? g->d.feat_dtype : -1; }
 int64_t eu_graph_hbm_bytes(const eu_graph* g) { return g ? g->hbm_bytes : -1; }
 
 int eu_graph_export(const eu_graph* g, uint64_t* ids, int32_t* node_type, float* node_w,
@@ -610,7 +690,17 @@ int eu_graph_export(const eu_graph* g, uint64_t* ids, int32_t* node_type, float*
   DL(nbr, d.nbr, d.E);
   DL(cum_w, d.cum_w, d.E);
   DL(grp_cum, d.grp_cum, d.n * d.T);
-  DL(feat, d.feat, d.n * (int64_t)d.feat_dim);
+  const int64_t nf = d.n * (int64_t)d.feat_dim;
+  if (d.feat_dtype == EU_FEAT_F32) {
+    DL(feat, feat_cols<float>(d), nf);
+  } else if (feat && d.feat && nf > 0) {   // widened on the host: the bf16 bits become the f32's upper half
+    std::vector<uint16_t> h((size_t)nf);
+    EU_CUDA(cudaMemcpy(h.data(), d.feat, sizeof(uint16_t) * (size_t)nf, cudaMemcpyDeviceToHost));
+    for (int64_t i = 0; i < nf; ++i) {
+      const uint32_t u = (uint32_t)h[i] << 16;
+      memcpy(feat + i, &u, sizeof(u));
+    }
+  }
 #undef DL
   return EU_OK;
 }

@@ -33,8 +33,8 @@ __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpre
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 
 // ---------------------------------------------------------------------------- feature fetch
-// out[i, 0:dim] = feat[row(ids[i]), 0:min(feat_dim,dim)], zeros elsewhere / for unknown ids.
-template <bool VEC>
+// out[i, 0:dim] = feat[row(ids[i]), 0:min(feat_dim,dim)], zeros elsewhere / for unknown ids.  T: the table's storage type.
+template <typename T, bool VEC>
 __global__ void __launch_bounds__(256) k_feature(DevGraph g, const unsigned long long* __restrict__ ids,
                                                  int64_t M, int32_t dim, int G, int32_t soff, int32_t sdim,
                                                  float* __restrict__ out) {
@@ -47,15 +47,15 @@ __global__ void __launch_bounds__(256) k_feature(DevGraph g, const unsigned long
     const int64_t row = sdim > 0 ? lookup_row(g, ids[i]) : -1;
     const int32_t fd = sdim;  // stored width of this slot
     float* o = out + i * (int64_t)dim;
-    const float* f = row >= 0 ? g.feat + row * (int64_t)g.feat_dim + soff : nullptr;
+    const T* f = row >= 0 ? feat_cols<T>(g) + row * (int64_t)g.feat_dim + soff : nullptr;
     if (VEC) {
       for (int32_t d = sub * 4; d < dim; d += G * 4) {
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (f && d < fd) v = ldg4(f + d);  // VEC requires fd % 4 == 0 so a float4 never straddles fd
+        if (f && d < fd) v = feat_ld4(f + d);  // VEC requires fd % 4 == 0 so a float4 never straddles fd
         st4(o + d, v);
       }
     } else {
-      for (int32_t d = sub; d < dim; d += G) o[d] = (f && d < fd) ? __ldg(f + d) : 0.f;
+      for (int32_t d = sub; d < dim; d += G) o[d] = (f && d < fd) ? feat_ld(f + d) : 0.f;
     }
   }
 }
@@ -246,13 +246,13 @@ __global__ void __launch_bounds__(256) k_sage_classify(DevGraph g, const unsigne
 // per lane are accumulated.
 // NV float4 per lane: rows of up to NV * 128 floats.  FULL: the width is exactly NV * 128 (128 / 256: no column guards, the
 // width is a compile-time constant); otherwise any multiple of 4 up to NV * 128 (e.g. 64 of configs[4]) with guarded columns.
-template <int NV, bool FULL>
+template <typename T, int NV, bool FULL>
 __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned long long* __restrict__ ids,
                                                    int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
                                                    int32_t count, bool mean, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int32_t fd = FULL ? NV * 128 : g.feat_dim;    // == dim, a multiple of 4, <= NV * 128 (checked by the launcher)
-  const float* __restrict__ feat = g.feat + lane * 4;
+  const T* __restrict__ feat = feat_cols<T>(g) + lane * 4;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t n = list ? (int64_t)__ldg(n_list) : rows;
   // grid-stride, one warp per output row (the launcher may cap the grid: EU_SAGE_CTAS CTAs per SM)
@@ -277,9 +277,9 @@ __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned lo
           const int j = __ffs(valid) - 1;
           valid &= valid - 1;
           const int32_t row = __shfl_sync(0xffffffffu, my, j);
-          const float* p = feat + (int64_t)row * fd;
+          const T* p = feat + (int64_t)row * fd;
 #pragma unroll
-          for (int t = 0; t < NV; ++t) v[q][t] = (FULL || lane * 4 + t * 128 < fd) ? ldg4(p + t * 128) : make_float4(0.f, 0.f, 0.f, 0.f);
+          for (int t = 0; t < NV; ++t) v[q][t] = (FULL || lane * 4 + t * 128 < fd) ? feat_ld4(p + t * 128) : make_float4(0.f, 0.f, 0.f, 0.f);
           n = q + 1;
         }
       }
@@ -307,6 +307,7 @@ __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned lo
 }
 
 // generic width fallback: one warp per representative, scalar columns
+template <typename T>
 __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const unsigned long long* __restrict__ ids,
                                                            int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
                                                            int32_t count, int32_t dim, bool mean, float* __restrict__ out) {
@@ -321,7 +322,7 @@ __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const uns
       float acc = 0.f;
       for (int32_t j = 0; j < count; ++j) {
         const int64_t row = lookup_row(g, __ldg(ids + r * count + j));
-        acc = __fadd_rn(acc, (row >= 0 && d < fd) ? __ldg(g.feat + row * (int64_t)fd + d) : 0.f);
+        acc = __fadd_rn(acc, (row >= 0 && d < fd) ? feat_ld(feat_cols<T>(g) + row * (int64_t)fd + d) : 0.f);
       }
       out[r * (int64_t)dim + d] = mean ? __fdiv_rn(acc, denom) : acc;
     }
@@ -407,6 +408,31 @@ static int scatter(eu_ctx* c, const float* upd, int64_t D, const int32_t* idx, i
   return EU_OK;
 }
 
+template <typename T>
+static int launch_feature(eu_ctx* c, const DevGraph& d, const int64_t* nodes, int64_t M, int32_t dim, int G, bool vec, unsigned blocks,
+                          int32_t soff, int32_t sdim, float* out) {
+  if (vec) k_feature<T, true><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
+  else k_feature<T, false><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+// the fused SAGE reduction over a table of T; v4: the float4 path's conditions hold (fanout_aggregate)
+template <typename T>
+static int launch_sage_mean(eu_ctx* c, const DevGraph& d, const unsigned long long* ids, int64_t rows, const int32_t* reps,
+                            const unsigned int* nrep, int32_t count, int32_t dim, bool mean, bool v4, unsigned blocks, float* out) {
+  cudaStream_t s = c->stream;
+  if (v4 && dim == 128) k_sage_mean<T, 1, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim == 256) k_sage_mean<T, 2, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 128) k_sage_mean<T, 1, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 256) k_sage_mean<T, 2, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 512) k_sage_mean<T, 4, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4) k_sage_mean<T, 8, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else k_sage_mean_generic<T><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, dim, mean, out);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
 }  // namespace eu
 
 using namespace eu;
@@ -424,10 +450,8 @@ int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid
   const int G = vec ? group_lanes(dim / 4) : (dim >= 32 ? 32 : 1);
   const unsigned blocks = capped_grid(ceil_div(M * G, 256), "EU_FEATURE_CTAS", 0);
   EuProfScope ps(c, "k_feature", M);
-  if (vec) k_feature<true><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
-  else k_feature<false><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
-  EU_LAUNCHED();
-  return EU_OK;
+  if (d.feat_dtype == EU_FEAT_BF16) return launch_feature<__nv_bfloat16>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
+  return launch_feature<float>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
 }
 
 int eu_gather(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx, int64_t E, float* out) {
@@ -478,16 +502,14 @@ static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int
   const int32_t* reps = dedup ? c->d_agg_rep : nullptr;
   const unsigned int* nrep = c->d_agg_nrep;
   { EuProfScope ps(c, mean ? "k_sage_mean" : "k_sage_add", rows);
-  // float4 path: one slot of the full stored width, a multiple of 4 floats up to 1024 (D = 64 of configs[4], 128, 256, ...)
-  const bool v4 = d.n < ((int64_t)1 << 31) && d.n_slots == 1 && dim == d.feat_dim && (dim & 3) == 0 && dim <= 1024 && aligned16(out) && aligned16(d.feat);
-  if (v4 && dim == 128) k_sage_mean<1, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim == 256) k_sage_mean<2, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 128) k_sage_mean<1, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 256) k_sage_mean<2, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 512) k_sage_mean<4, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4) k_sage_mean<8, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else k_sage_mean_generic<<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, dim, mean, out); }
-  EU_LAUNCHED();
+    // float4 path: one slot of the full stored width, a multiple of 4 floats up to 1024 (D = 64 of configs[4], 128, 256, ...),
+    // on a table aligned to four elements (16 bytes of f32, 8 of bf16)
+    const bool bf16 = d.feat_dtype == EU_FEAT_BF16;
+    const bool v4 = d.n < ((int64_t)1 << 31) && d.n_slots == 1 && dim == d.feat_dim && (dim & 3) == 0 && dim <= 1024 && aligned16(out) &&
+                    (bf16 ? ((uintptr_t)d.feat & 7) == 0 : aligned16(d.feat));
+    const int rc = bf16 ? launch_sage_mean<__nv_bfloat16>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out)
+                        : launch_sage_mean<float>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out);
+    if (rc) return rc; }
   if (!dedup) return EU_OK;
   { EuProfScope ps(c, "k_sage_broadcast", rows);
     const bool vec = (dim & 3) == 0 && aligned16(out);

@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(256) k_sym_reply_feature(DevGraph g, char* con
     for (int64_t k = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> sh; k < n_s; k += ((int64_t)gridDim.x * blockDim.x) >> sh) {
       const int64_t row = (int64_t)s * lay.cap + k;
       const int64_t gr = sdim > 0 ? lookup_row(g, ids[row]) : -1;
-      const float* f = gr >= 0 ? g.feat + gr * (int64_t)g.feat_dim + soff : nullptr;
+      const float* f = gr >= 0 ? feat_cols<float>(g) + gr * (int64_t)g.feat_dim + soff : nullptr;
       float* o = obase + (int64_t)src[row] * dim;
       for (int32_t d = sub * 4; d < dim; d += G * 4) {   // dim, sdim, soff multiples of 4 (checked by the launcher)
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -266,7 +266,7 @@ __global__ void __launch_bounds__(256) k_sym_reply_sage(DevGraph g, char* const*
   if (s_err) return;
   const int lane = threadIdx.x & 31;
   constexpr int32_t fd = NV * 128;
-  const float* __restrict__ feat = g.feat + lane * 4;
+  const float* __restrict__ feat = feat_cols<float>(g) + lane * 4;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t gps = (rows + kSageR - 1) / kSageR;   // destination groups per source
   for (int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; w < (int64_t)N * gps; w += nwarps) {
@@ -377,7 +377,7 @@ __global__ void __launch_bounds__(256) k_sym_reply_sage_generic(DevGraph g, char
       float acc = 0.f;
       for (int32_t e = e_lo; e < n_s && seg[e] < key_hi; ++e) {   // warp-uniform
         const int64_t row = lookup_row(g, sid[e]);
-        if (row >= 0 && col < fd && col < dim) acc = __fadd_rn(acc, __ldg(g.feat + row * (int64_t)fd + col));
+        if (row >= 0 && col < fd && col < dim) acc = __fadd_rn(acc, __ldg(feat_cols<float>(g) + row * (int64_t)fd + col));
       }
       if (col < dim) o[col] = acc;
     }
@@ -646,6 +646,7 @@ int eu_sym_get_dense_feature(eu_sym* s, const int64_t* ids, int64_t rows, int32_
   const SymLayout& L = s->lay;
   const DevGraph& d = c->g->d;
   const int N = s->world;
+  if (d.feat_dtype != EU_FEAT_F32) { set_error("eu_sym_get_dense_feature: the sharded feature paths read f32 tables only"); return EU_ERR_UNSUPPORTED; }
   if (rows > L.cap || rows > L.max_rows_f || dim > L.max_dim) { set_error("eu_sym_get_dense_feature: request exceeds the symmetric region"); return EU_ERR_INVALID; }
   const bool have = fid >= 0 && fid < d.n_slots;
   const int32_t soff = have ? d.slot_off[fid] : 0, sdim = have ? d.slot_dim[fid] : 0;
@@ -679,6 +680,7 @@ int eu_sym_sage_mean(eu_sym* s, const int64_t* nbr_ids, int64_t rows, int32_t co
   const DevGraph& d = c->g->d;
   const int N = s->world;
   const int64_t nid = rows * count;
+  if (d.feat_dtype != EU_FEAT_F32) { set_error("eu_sym_sage_mean: the sharded feature paths read f32 tables only"); return EU_ERR_UNSUPPORTED; }
   if (nid > L.cap || nid >= ((int64_t)1 << 31) || (int64_t)N * rows * dim > L.max_rows_f * (int64_t)L.max_dim) {
     set_error("eu_sym_sage_mean: %lld x %d ids / %d partial blocks exceed the symmetric region", (long long)rows, count, N);
     return EU_ERR_INVALID;

@@ -36,7 +36,7 @@ __device__ __forceinline__ void top_k_insert(float (&t)[KMAX], float v) {
 
 // out[b, 0, :] = the node's row, out[b, 1 + j, d] = the j-th of column d over the count neighbours (j < k <= KMAX).  The
 // slots start at -inf: a slot no value ranks above keeps -inf, which is the value it would have selected (k <= count).
-template <int KMAX, int C>
+template <typename T, int KMAX, int C>
 __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t B,
                                                            const unsigned long long* __restrict__ nbrs, int32_t count, int32_t soff,
                                                            int32_t width, int32_t dim, int32_t k, float* __restrict__ out) {
@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
   for (int64_t b = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; b < B; b += nwarps) {
     const unsigned long long* nb = nbrs + b * count;
     const int64_t self = w > 0 ? lookup_row(g, nodes[b]) : -1;
-    const float* fs = self >= 0 ? g.feat + self * (int64_t)g.feat_dim + soff : nullptr;
+    const T* fs = self >= 0 ? feat_cols<T>(g) + self * (int64_t)g.feat_dim + soff : nullptr;
     float* o = out + b * (int64_t)(k + 1) * dim;
     for (int32_t d0 = 0; d0 < dim; d0 += 32 * C) {
       float t[C][KMAX];
@@ -59,12 +59,12 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
         const int64_t mine = (w > 0 && lane < n) ? lookup_row(g, nb[j0 + lane]) : -1;
         for (int32_t j = 0; j < n; ++j) {
           const int64_t row = __shfl_sync(0xffffffffu, mine, j);
-          const float* f = g.feat + (row >= 0 ? row * (int64_t)g.feat_dim + soff : 0);
+          const T* f = feat_cols<T>(g) + (row >= 0 ? row * (int64_t)g.feat_dim + soff : 0);
           float v[C];
 #pragma unroll
           for (int c = 0; c < C; ++c) {
             const int32_t d = d0 + 32 * c + lane;
-            v[c] = (row >= 0 && d < w) ? __ldg(f + d) : 0.f;
+            v[c] = (row >= 0 && d < w) ? feat_ld(f + d) : 0.f;
           }
 #pragma unroll
           for (int c = 0; c < C; ++c) top_k_insert<KMAX>(t[c], v[c]);
@@ -74,7 +74,7 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
       for (int c = 0; c < C; ++c) {
         const int32_t d = d0 + 32 * c + lane;
         if (d >= dim) continue;
-        o[d] = (fs && d < w) ? __ldg(fs + d) : 0.f;
+        o[d] = (fs && d < w) ? feat_ld(fs + d) : 0.f;
 #pragma unroll
         for (int i = 0; i < KMAX; ++i)
           if (i < k) o[(int64_t)(1 + i) * dim + d] = t[c][i];
@@ -88,8 +88,13 @@ static int launch_top_k(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_
                         int32_t width, int32_t dim, int32_t k, float* out) {
   const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(B, 8), (int64_t)kSMs * 32);
   EuProfScope ps(c, "k_neighbor_top_k", B);
-  k_neighbor_top_k<KMAX, C><<<blocks, 256, 0, c->stream>>>(c->g->d, (const unsigned long long*)nodes, B,
-                                                             (const unsigned long long*)neighbors, count, soff, width, dim, k, out);
+  // a bf16 table widens exactly and order-preservingly (+-0 and NaN included): the selection is the f32 one's on the widened rows
+  if (c->g->d.feat_dtype == EU_FEAT_BF16)
+    k_neighbor_top_k<__nv_bfloat16, KMAX, C><<<blocks, 256, 0, c->stream>>>(c->g->d, (const unsigned long long*)nodes, B,
+                                                                            (const unsigned long long*)neighbors, count, soff, width, dim, k, out);
+  else
+    k_neighbor_top_k<float, KMAX, C><<<blocks, 256, 0, c->stream>>>(c->g->d, (const unsigned long long*)nodes, B,
+                                                                    (const unsigned long long*)neighbors, count, soff, width, dim, k, out);
   EU_LAUNCHED();
   return EU_OK;
 }

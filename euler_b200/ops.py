@@ -16,7 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import EulerError, check
-from .graph import Context, Graph
+from .graph import Context, Graph, feat_dtype_code
 
 _state = threading.local()
 _default = {"graph": None, "rng": "minstd", "seed": 1}
@@ -30,6 +30,11 @@ def initialize_graph(config):
         config = ';'.join('{}={}'.format(key, value) for key, value in config.items())
     if not isinstance(config, str):
         raise TypeError('Expect str or dict for graph config, got {}.'.format(type(config).__name__))
+    # feature_dtype=float32|bfloat16: the node feature table's storage type (Graph.load's feat_dtype), checked before the load
+    for item in config.split(';'):
+        key, eq, value = item.partition('=')
+        if key == 'feature_dtype' and eq:
+            feat_dtype_code(value)
     lib = _lib.load()
     ok = bool(lib.InitQueryProxy(config.encode()))
     h = lib.eu_default_graph()

@@ -292,6 +292,7 @@ class ShardedGraph:
 
     def get_dense_feature(self, nodes, fid, dim):
         ops, x = self.ops, self.xchg
+        _f32_features("ShardedGraph.get_dense_feature", getattr(ops, "graph", None), getattr(self.feature_ops, "graph", None))
         ids = ops.to_dev(nodes, _i64(ops)).reshape(-1)
         rows = ids.numel()
         if self.feature_ops is not None:     # replicated feature table: no exchange
@@ -417,6 +418,7 @@ class PeerShardedGraph:
 
     def get_dense_feature(self, nodes, fid, dim, clone=True, out=None):
         t = self.torch
+        _f32_features("PeerShardedGraph.get_dense_feature", self.graph, self.feature_graph)
         ids = nodes.to(device=self.dev, dtype=t.int64).reshape(-1).contiguous()
         if self.fctx is not None:      # replicated feature table: the single-GPU kernel, nothing crosses NVLink
             if out is None:
@@ -432,6 +434,7 @@ class PeerShardedGraph:
     def sage_mean(self, nbr_ids, rows, count, dim, out=None):
         """fused sharded mean aggregation of a fixed-fanout block (owners sum their rows; eu_sym_sage_mean)"""
         t = self.torch
+        _f32_features("PeerShardedGraph.sage_mean", self.graph, self.feature_graph)
         ids = nbr_ids.to(device=self.dev, dtype=t.int64).reshape(-1).contiguous()
         assert ids.numel() == rows * count
         if out is None:
@@ -459,6 +462,16 @@ class PeerShardedGraph:
 
 class EulerErrorSharded(RuntimeError):
     pass
+
+
+def _f32_features(what, *graphs):
+    """The sharded feature paths read float32 feature tables only: a bfloat16 graph is refused on every rank alike, before
+    any exchange or write."""
+    from ._lib import EulerError
+    for g in graphs:
+        if g is not None and getattr(g, "feat_dtype", "float32") != "float32":
+            raise EulerError("%s: the sharded feature paths read float32 feature tables only (this graph stores %s)"
+                             % (what, g.feat_dtype))
 
 
 def _i64(ops):

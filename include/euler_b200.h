@@ -92,6 +92,15 @@ typedef struct {
 } eu_graph_desc;
 
 int eu_graph_create(const eu_graph_desc* desc, int device, eu_graph** out);
+/* Storage type of the dense node feature table.  Every graph constructor stores f32; its *_dtype sibling takes one of
+ * these.  EU_FEAT_BF16 halves the table: each value is rounded to bfloat16 on the device (round to nearest even; NaN
+ * becomes a canonical NaN, +-Inf stays, a finite value becomes +-Inf only where the rounding says so), and every op that
+ * reads dense node features widens it exactly to f32, so its output is bit for bit the f32 op's on the rounded table.
+ * Host f32 arrays go up in bounded chunks and are rounded on the device: the peak is the bf16 table plus one chunk.  Edge
+ * features and ragged features are not affected.  An unknown dtype: EU_ERR_INVALID before any allocation.  The sharded
+ * feature paths (eu_sym_get_dense_feature, eu_sym_sage_mean) refuse a bf16 graph with EU_ERR_UNSUPPORTED. */
+typedef enum { EU_FEAT_F32 = 0, EU_FEAT_BF16 = 1 } eu_feat_dtype;
+int eu_graph_create_dtype(const eu_graph_desc* desc, int device, int32_t feat_dtype, eu_graph** out);
 /* Synthetic R-MAT graph generated, sorted and prefix-summed on the device (SURVEY.md section 8d "G-RMAT"):
  * ids 1..n, one node/edge type, n_edges directed edges with (a,b,c,d), adjacency sorted by dst,
  * weight = 1 + (hash(src,dst) % 100) / 10, feat ~ U(-1,1).  feat_dim may be 0. */
@@ -109,6 +118,16 @@ int eu_graph_create_rmat_shard(int64_t n_nodes, int64_t n_edges, double a, doubl
 int eu_graph_create_rmat_hetero(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
                                 double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                 int shard_index, int shard_number, eu_graph** out);
+/* The three R-MAT constructors with the feature table's storage type (eu_feat_dtype); a bf16 table holds the f32 values
+ * above, rounded on the device. */
+int eu_graph_create_rmat_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed, int32_t feat_dim,
+                               uint64_t feat_seed, int device, int32_t feat_dtype, eu_graph** out);
+int eu_graph_create_rmat_shard_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
+                                     int32_t feat_dim, uint64_t feat_seed, int device, int shard_index, int shard_number,
+                                     int32_t feat_dtype, eu_graph** out);
+int eu_graph_create_rmat_hetero_dtype(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
+                                      double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
+                                      int shard_index, int shard_number, int32_t feat_dtype, eu_graph** out);
 /* Euler 2.0 on-disk format (euler.meta + the Node and Edge partition files; SURVEY.md Appendix B), shard `shard_index` of
  * `shard_number` with the reference's file filter (graph.cc:90-98).  = Graph::Init, graph.h:53-56. */
 int eu_graph_load(const char* data_path, int shard_index, int shard_number, int device,
@@ -117,6 +136,9 @@ int eu_graph_load(const char* data_path, int shard_index, int shard_number, int 
  * files, when the directory has them, feed eu_sample_edge and the edge feature ops. */
 int eu_graph_load_ex(const char* data_path, int shard_index, int shard_number, int device, int load_edges,
                      eu_graph** out);
+/* eu_graph_load_ex with the node feature table's storage type (eu_feat_dtype) */
+int eu_graph_load_dtype(const char* data_path, int shard_index, int shard_number, int device, int load_edges,
+                        int32_t feat_dtype, eu_graph** out);
 /* Edge records (Edge files of the Euler format; euler/core/graph/edge.h): needed only by sample_edge and the edge feature ops.
  * HOST arrays; features use the node layout (dense slots concatenated per edge, ragged uint64 / binary slots).
  * sampler_order: edge rows in the order the reference's edge_map_ iterates (graph.cc:372-399); NULL = row order. */
@@ -158,8 +180,12 @@ int eu_graph_load_inspect(const char* data_path, int shard_index, int shard_numb
 int eu_build_alias_table(const float* weights, int64_t n, float* prob, int32_t* alias, float* sum);
 int32_t eu_graph_num_node_types(const eu_graph* g);
 int32_t eu_graph_feat_dim(const eu_graph* g);
+/* the eu_feat_dtype of the dense node feature table; -1 for a NULL graph */
+int32_t eu_graph_feat_dtype(const eu_graph* g);
+/* device bytes the graph holds (a bf16 feature table counts 2 bytes per element) */
 int64_t eu_graph_hbm_bytes(const eu_graph* g);
-/* Copy the device CSR back to caller-allocated HOST arrays (any pointer may be NULL). */
+/* Copy the device CSR back to caller-allocated HOST arrays (any pointer may be NULL).  feat is f32 whatever the table's
+ * storage type: a bf16 table comes back widened, exactly. */
 int eu_graph_export(const eu_graph* g, uint64_t* ids, int32_t* node_type, float* node_w,
                     int64_t* grp_ptr, uint64_t* nbr, float* cum_w, float* grp_cum, float* feat);
 /* type-name lookup from euler.meta (tf_euler/python/euler_ops/type_ops.py:31-64); -1 if unknown */
