@@ -92,3 +92,35 @@ def cuda_slot_graph(g):
     return euler_b200.Graph.from_csr(g["ids"], g["grp_ptr"], g["nbr"], n_edge_types=g["T"], node_type=g["node_type"],
                                      node_w=g["node_w"], cum_w=g["cum_w"], feat=g.get("feat"), u64_ptr=g["u64_ptr"], u64_val=g["u64_val"],
                                      n_u64_slots=g["S"])
+
+
+def composed_parts(nodes, id_table, dense, sparse):
+    """the single ops ShallowEncoder's row is made of, on the device: ([F.embedding(nodes, id_table)] or [],
+    get_dense_feature's slots, [sparse_feature_embedding per (name, table, default, combiner)])"""
+    import torch
+    import torch.nn.functional as F
+    import euler_b200
+    nd = torch.as_tensor(nodes, device="cuda")
+    idp = [F.embedding(nd, id_table)] if id_table is not None else []
+    dp = euler_b200.get_dense_feature(nd, [n for n, _ in dense], [d for _, d in dense]) if dense else []
+    sp = [euler_b200.sparse_feature_embedding(nd, n, t, dv, c) for n, t, dv, c in sparse]
+    return idp, dp, sp
+
+
+def pool_f32(rows, count, pool):
+    """shallow_encode_pool's defined order over shallow_encode's rows [R count, W], in float32 on the host: each column added
+    left to right from the segment's first row, mean divided once by fl(count)"""
+    x = rows.cpu().numpy().reshape(-1, count, rows.shape[1])
+    acc = x[:, 0].copy()
+    for j in range(1, count):
+        acc = acc + x[:, j]
+    return acc / np.float32(count) if pool == "mean" else acc
+
+
+def shallow_problem(nodes, id_table, dense, sparse, comb=0):
+    """the eu_shallow_problem of shallow_encode's arguments (names resolved on the installed graph), for raw library calls"""
+    import euler_b200
+    from euler_b200 import ops
+    g = euler_b200.get_graph()
+    res = [(g.sparse_feature_id(n), t, dv, ops._COMBINERS[c]) for n, t, dv, c in sparse]
+    return ops._shallow_problem(nodes, id_table, [(g.dense_feature_id(n) if isinstance(n, str) else n, d) for n, d in dense], res, comb)

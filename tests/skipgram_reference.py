@@ -115,3 +115,43 @@ def gen_pair_count(path_len, left, right):
     """gen_pair's pairs per walk of path_len nodes (gen_pair_op.cc): each node with the nodes up to `left` before and `right`
     after it"""
     return sum(min(i, left) + min(path_len - 1 - i, right) for i in range(path_len))
+
+
+# ------------------------------------------------------------------------------------ device helpers of the GPU tests
+def device_table(n_rows, dim, rng, offset=0, dyadic=True):
+    """a f32 table on the device whose data pointer is `offset` floats past a 16-byte boundary; dyadic: values k / 8,
+    |k| <= 8"""
+    import torch
+    v = rng.randint(-8, 9, size=n_rows * dim + offset) / 8.0 if dyadic else rng.randn(n_rows * dim + offset) * 0.3
+    t = torch.tensor(v, dtype=torch.float32).cuda()
+    return t[offset:].view(n_rows, dim)
+
+
+def pair_ids(rng, B, P, K, n_rows):
+    """random (src [B], pos [B, P], negs [B, K]), the last row named by a few src and pos entries"""
+    src = rng.randint(0, n_rows, size=B)
+    pos = rng.randint(0, n_rows, size=(B, P))
+    negs = rng.randint(0, n_rows, size=(B, K))
+    src[:3] = n_rows - 1            # the default row max_id + 1 of a table of max_id + 2 rows
+    pos[3:6, 0] = n_rows - 1
+    return src, pos, negs
+
+
+def device_forward(src, pos, negs, target, context):
+    """one eu_skipgram_loss: (logits, rank, loss)"""
+    import torch
+    from euler_b200 import ops
+    d = lambda a: torch.as_tensor(a, dtype=torch.int64).cuda().contiguous()   # noqa: E731
+    return ops._raw_skipgram(d(src).reshape(-1), d(pos), d(negs).reshape(len(src), -1), target, context)
+
+
+def device_grads(src, pos, negs, target, context, shared=False, sparse=False, g=None):
+    """(loss, the target table's gradient, the context table's or None when shared) of skipgram_xent_loss on copies of the
+    tables, the loss's upstream gradient g (default 1)"""
+    import torch
+    import euler_b200
+    T = target.clone().requires_grad_(True)
+    Cx = T if shared else context.clone().requires_grad_(True)
+    loss, _ = euler_b200.skipgram_xent_loss(src, pos, negs, T, Cx, sparse_grad=sparse)
+    loss.backward(None if g is None else torch.tensor(g, dtype=torch.float32, device="cuda"))
+    return loss, T.grad, (None if shared else Cx.grad)

@@ -4,6 +4,8 @@ import numpy as np
 import pytest
 import torch
 
+import kg_reference as kr
+
 pytestmark = pytest.mark.gpu
 
 MODELS = ('transe', 'transh', 'transr', 'transd', 'distmult')
@@ -26,53 +28,6 @@ def _dims(model, dim):
     return TRANSR_DIMS[dim] if model == 'transr' else (dim, dim)
 
 
-def _tables(model, n_ent, n_rel, ent_dim, rel_dim, rng, offset=0):
-    """random f32 tables on the device; offset shifts each data pointer off a 16-byte boundary"""
-    def t(rows, cols):
-        v = torch.tensor(rng.randn(rows * cols + offset) * 0.3, dtype=torch.float32).cuda()
-        return v[offset:].view(rows, cols)
-    tabs = [t(n_ent, ent_dim), t(n_rel, rel_dim)]
-    if model == 'transh':
-        tabs.append(t(n_rel, ent_dim))
-    elif model == 'transr':
-        tabs.append(t(n_rel, ent_dim * rel_dim))
-    elif model == 'transd':
-        tabs += [t(n_ent, ent_dim), t(n_rel, rel_dim)]
-    return tabs
-
-
-def _ids(rng, B, K, n_ent, n_rel):
-    d = lambda a: torch.as_tensor(a, dtype=torch.int64).cuda()   # noqa: E731
-    return (d(rng.randint(0, n_ent - 4, size=B)), d(rng.randint(0, n_ent - 4, size=B)),
-            d(rng.randint(0, n_ent - 4, size=(B, K))), d(rng.randint(0, n_rel - 1, size=B)))   # the last rows stay untouched
-
-
-def _raw(model, tabs, src, dst, neg, rel, l1, corrupt, margin, with_emb=False):
-    from euler_b200 import ops
-    m = ops.KG_MODELS[model]
-    slots = [None] * 4
-    for t, tb in zip(ops._KG_SLOTS[m], tabs):
-        slots[t] = tb
-    cfg = (m, l1, ops.KG_CORRUPT[corrupt], margin, tabs[0].shape[1], tabs[1].shape[1], False, with_emb)
-    return ops._raw_kg(*slots, src, dst, rel, neg, cfg)
-
-
-def _ref64(model, tabs, src, dst, neg, rel, l1, corrupt, margin):
-    from euler_b200.knowledge import composed_kg_scores
-    t64 = [t.detach().double().requires_grad_(True) for t in tabs]
-    pos, negs, emb = composed_kg_scores(model, t64, src, dst, neg, rel, l1=l1, corrupt=corrupt)
-    B = pos.shape[0]
-    loss = torch.clamp(margin + negs.reshape(B, -1).mean(-1, keepdim=True).reshape(-1, 1, 1) - pos, min=0).mean()
-    loss.backward()
-    return pos.reshape(B, 1), negs.reshape(B, -1), loss, [t.grad for t in t64], emb
-
-
-def _rel_err(a, b):
-    """the largest difference relative to b's largest entry"""
-    b = b.detach().double().cpu()
-    return float((a.detach().double().cpu() - b).abs().max() / max(1e-12, float(b.abs().max())))
-
-
 @pytest.mark.parametrize("dim", DIMS)
 @pytest.mark.parametrize("corrupt", CORRUPTS)
 @pytest.mark.parametrize("l1", (True, False))
@@ -80,59 +35,15 @@ def _rel_err(a, b):
 def test_against_float64(graph, model, l1, corrupt, dim):
     """scores and loss within 1e-6 of float64; ranks exact; every table's gradient within 1e-5 of float64 autograd, bit-identical
     run to run, zero on untouched rows, and the sparse COO equal to the dense rows"""
-    from euler_b200 import ops
     di = DIMS.index(dim)
     K = KS[(di + CORRUPTS.index(corrupt)) % len(KS)]
     ent_dim, rel_dim = _dims(model, dim)
     rng = np.random.RandomState(1000 * di + 10 * MODELS.index(model) + CORRUPTS.index(corrupt) + 5 * l1)
     n_ent, n_rel, B = 60, 8, 7 if K == 4097 else 33
-    tabs = _tables(model, n_ent, n_rel, ent_dim, rel_dim, rng, offset=di % 2)
-    src, dst, neg, rel = _ids(rng, B, K, n_ent, n_rel)
+    tabs = kr.tables(model, n_ent, n_rel, ent_dim, rel_dim, rng, offset=di % 2)
+    src, dst, neg, rel = kr.ids(rng, B, K, n_ent, n_rel)
     margin = 5.0    # every row active: the gate itself is covered by test_hinge_gate
-    scores, rank, loss, embs = _raw(model, tabs, src, dst, neg, rel, l1, corrupt, margin, with_emb=True)
-    pos64, neg64, loss64, grads64, emb64 = _ref64(model, tabs, src, dst, neg, rel, l1, corrupt, margin)
-    s64 = torch.cat([pos64, neg64], 1).detach()
-    assert _rel_err(scores, s64) <= 1e-6, (model, l1, corrupt, dim, K)
-    assert abs(float(loss) - float(loss64.detach())) <= 1e-6 * abs(float(loss64))
-    # dim 1: n(x) = sign(x) has the exact gradient 0 and TransH's projection is exactly 0; f32 leaves a cancellation residue
-    # of about eps |gy| / |x| there, so dim 1 is held to an absolute bound instead
-    def close(a, b, tol):
-        if dim > 1:
-            return _rel_err(a, b) <= tol
-        return float((a.detach().double().cpu() - b.detach().double().cpu()).abs().max()) <= 1e-4
-    for e, e64 in zip(embs, emb64):
-        assert close(e, e64, 1e-6)
-    sc = scores.cpu()
-    own = (sc[:, 1:] >= sc[:, :1]).sum(1)
-    assert torch.equal(rank.cpu().long(), own)
-    s64c = s64.cpu()
-    far = ((s64c[:, 1:] - s64c[:, :1]).abs() > 1e-5).all(1)
-    assert torch.equal(own[far], (s64c[far, 1:] >= s64c[far, :1]).sum(1))
-
-    t = [tb.clone().requires_grad_(True) for tb in tabs]
-    runs = []
-    for _ in range(2):
-        for x in t:
-            x.grad = None
-        l, _m = ops.kg_margin_loss(src, dst, neg, rel, t, model, l1=l1, corrupt=corrupt, margin=margin)
-        l.backward()
-        runs.append([x.grad.clone() for x in t])
-    touched_ent = torch.zeros(n_ent, dtype=torch.bool)
-    touched_ent[torch.cat([src, dst, neg.reshape(-1)]).cpu()] = True
-    touched_rel = torch.zeros(n_rel, dtype=torch.bool)
-    touched_rel[rel.cpu()] = True
-    for k, (g, g2, g64) in enumerate(zip(runs[0], runs[1], grads64)):
-        assert g.cpu().numpy().tobytes() == g2.cpu().numpy().tobytes(), (model, k)
-        assert close(g, g64, 1e-5), (model, l1, corrupt, dim, K, k, _rel_err(g, g64))
-        touched = touched_ent if g.shape[0] == n_ent else touched_rel
-        assert not g.cpu()[~touched].any()
-    for x in t:
-        x.grad = None
-    l, _m = ops.kg_margin_loss(src, dst, neg, rel, t, model, l1=l1, corrupt=corrupt, margin=margin, sparse_grad=True)
-    l.backward()
-    for x, g in zip(t, runs[0]):
-        assert x.grad.is_sparse and x.grad.coalesce()._nnz() == x.grad._nnz()   # one entry per distinct row
-        assert x.grad.to_dense().cpu().numpy().tobytes() == g.cpu().numpy().tobytes()
+    kr.check_against_float64(model, tabs, src, dst, neg, rel, l1, corrupt, margin, absolute=dim == 1)
 
 
 @pytest.mark.parametrize("model", MODELS)
@@ -141,18 +52,18 @@ def test_hinge_gate(graph, model):
     from euler_b200 import ops
     rng = np.random.RandomState(3)
     ent_dim, rel_dim = _dims(model, 32)
-    tabs = _tables(model, 40, 6, ent_dim, rel_dim, rng)
-    src, dst, neg, rel = _ids(rng, 50, 5, 40, 6)
-    scores = _raw(model, tabs, src, dst, neg, rel, True, 'both', 0.0)[0].cpu()
+    tabs = kr.tables(model, 40, 6, ent_dim, rel_dim, rng)
+    src, dst, neg, rel = kr.ids(rng, 50, 5, 40, 6)
+    scores = kr.raw(model, tabs, src, dst, neg, rel, True, 'both', 0.0)[0].cpu()
     h = (scores[:, 1:].mean(1) - scores[:, 0]).double()
     margin = float(-h.median()) + 1e-3   # about half the rows active, none at the boundary
     t = [tb.clone().requires_grad_(True) for tb in tabs]
     l, _ = ops.kg_margin_loss(src, dst, neg, rel, t, model, corrupt='both', margin=margin)
     l.backward()
-    _, _, loss64, g64, _ = _ref64(model, tabs, src, dst, neg, rel, True, 'both', margin)
+    _, _, loss64, g64, _ = kr.ref64(model, tabs, src, dst, neg, rel, True, 'both', margin)
     assert abs(float(l) - float(loss64)) <= 1e-6 * abs(float(loss64))
     for x, g in zip(t, g64):
-        assert _rel_err(x.grad, g) <= 1e-5
+        assert kr.rel_err(x.grad, g) <= 1e-5
     t = [tb.clone().requires_grad_(True) for tb in tabs]
     l, _ = ops.kg_margin_loss(src, dst, neg, rel, t, model, corrupt='both', margin=-1000.0)
     l.backward()
@@ -175,7 +86,7 @@ def test_hub_negative_exact_on_integer_gradients(graph):
     t = [ent.cuda().requires_grad_(True), relt.cuda().requires_grad_(True)]
     l, _ = ops.kg_margin_loss(src, dst, neg, rel, t, 'transe', l1=True, corrupt='both', margin=10.0)
     (l * float(B * 2 * K)).backward()    # cn = 1, cp = -2K: integer entries
-    _, _, _, g64, _ = _ref64('transe', [ent, relt], src.cpu(), dst.cpu(), neg.cpu(), rel.cpu(), True, 'both', 10.0)
+    _, _, _, g64, _ = kr.ref64('transe', [ent, relt], src.cpu(), dst.cpu(), neg.cpu(), rel.cpu(), True, 'both', 10.0)
     for x, g in zip(t, g64):
         want = (g * float(B * 2 * K)).numpy()
         assert np.array_equal(x.grad.cpu().numpy(), want.astype(np.float32))
@@ -191,15 +102,15 @@ def test_l2_zero_difference_has_zero_gradient(graph):
     hyper = torch.tensor([[0, 0, 0, 1.0]])
     src, dst, rel = torch.tensor([0]).cuda(), torch.tensor([1]).cuda(), torch.tensor([0]).cuda()
     neg = torch.tensor([[2, 3]]).cuda()
-    scores = _raw('transh', [x.cuda() for x in (ent, relt, hyper)], src, dst, neg, rel, False, 'both', 1.0)[0]
+    scores = kr.raw('transh', [x.cuda() for x in (ent, relt, hyper)], src, dst, neg, rel, False, 'both', 1.0)[0]
     assert float(scores[0, 0]) == 0.0
     t = [x.cuda().requires_grad_(True) for x in (ent, relt, hyper)]
     l, _ = ops.kg_margin_loss(src, dst, neg, rel, t, 'transh', l1=False, corrupt='both', margin=1.0)
     l.backward()
-    _, _, _, g64, _ = _ref64('transh', [ent, relt, hyper], src.cpu(), dst.cpu(), neg.cpu(), rel.cpu(), False, 'both', 1.0)
+    _, _, _, g64, _ = kr.ref64('transh', [ent, relt, hyper], src.cpu(), dst.cpu(), neg.cpu(), rel.cpu(), False, 'both', 1.0)
     for x, g in zip(t, g64):
         assert torch.isfinite(x.grad).all()
-        assert _rel_err(x.grad, g) <= 1e-5
+        assert kr.rel_err(x.grad, g) <= 1e-5
     assert dim == ent.shape[1]
 
 
@@ -207,8 +118,8 @@ def test_bad_arguments_raise(graph):
     import euler_b200
     from euler_b200 import ops
     rng = np.random.RandomState(9)
-    tabs = _tables('transe', 20, 4, 8, 8, rng)
-    src, dst, neg, rel = _ids(rng, 6, 3, 20, 4)
+    tabs = kr.tables('transe', 20, 4, 8, 8, rng)
+    src, dst, neg, rel = kr.ids(rng, 6, 3, 20, 4)
     bad = neg.clone()
     bad[2, 1] = 20
     with pytest.raises(euler_b200.EulerError):
@@ -217,7 +128,7 @@ def test_bad_arguments_raise(graph):
         ops.kg_margin_loss(src, dst, neg, rel + 4, tabs, 'transe')
     with pytest.raises(euler_b200.EulerError):
         ops.kg_margin_loss(src, dst, neg[:, :0], rel, tabs, 'transe')
-    big = _tables('transr', 20, 4, 256, 128, rng)
+    big = kr.tables('transr', 20, 4, 256, 128, rng)
     with pytest.raises(euler_b200.EulerError, match="not supported"):
         ops.kg_margin_loss(src, dst, neg, rel, big, 'transr')
     with pytest.raises(euler_b200.EulerError):
@@ -229,7 +140,7 @@ def test_empty_batch(graph, model):
     from euler_b200 import ops
     rng = np.random.RandomState(2)
     ent_dim, rel_dim = _dims(model, 4)
-    t = [x.clone().requires_grad_(True) for x in _tables(model, 10, 3, ent_dim, rel_dim, rng)]
+    t = [x.clone().requires_grad_(True) for x in kr.tables(model, 10, 3, ent_dim, rel_dim, rng)]
     e = torch.zeros(0, dtype=torch.int64).cuda()
     l, m = ops.kg_margin_loss(e, e, e.reshape(0, 2), e, t, model)
     assert torch.isnan(l)
@@ -282,6 +193,6 @@ def test_training_step_matches_composed(cls):
     assert abs(float(outs[0].loss) - float(outs[1].loss)) <= 1e-5 * max(1.0, abs(float(outs[1].loss)))
     assert abs(float(outs[0].metric) - float(outs[1].metric)) <= 1e-5 * max(1.0, abs(float(outs[1].metric)))
     for a, b in zip(outs[0].embedding, outs[1].embedding):
-        assert a.shape == b.shape and _rel_err(a, b) <= 1e-5
+        assert a.shape == b.shape and kr.rel_err(a, b) <= 1e-5
     for (n, p), (_, q) in zip(fused.named_parameters(), composed.named_parameters()):
-        assert _rel_err(p, q) <= 1e-5, n
+        assert kr.rel_err(p, q) <= 1e-5, n

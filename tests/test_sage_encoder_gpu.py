@@ -63,22 +63,12 @@ def _inputs(dim, off=0, combiners=("sum", "mean")):
     return id_table, sparse
 
 
-def _restated(rows, count, pool):
-    """the op's defined order over shallow_encode's rows, in float32 on the host: each column added left to right from the
-    segment's first row, mean divided once by fl(count)"""
-    x = rows.cpu().numpy().reshape(-1, count, rows.shape[1])
-    acc = x[:, 0].copy()
-    for j in range(1, count):
-        acc = acc + x[:, j]
-    return acc / np.float32(count) if pool == "mean" else acc
-
-
 def _check_forward(nodes, count, id_table, dense, sparse, what):
     import euler_b200
     rows = euler_b200.shallow_encode(nodes, id_table, dense, sparse, "concat")
     for pool in ("sum", "mean"):
         out = euler_b200.shallow_encode_pool(nodes, count, id_table, dense, sparse, pool)
-        want = _restated(rows, count, pool)
+        want = er.pool_f32(rows, count, pool)
         assert out.shape == want.shape and out.dtype == torch.float32
         assert out.cpu().numpy().tobytes() == want.tobytes(), (what, count, pool)
     mean = rows.view(-1, count, rows.shape[1]).mean(1)
@@ -126,14 +116,6 @@ def _raw(sym, p, *args):
     return getattr(_lib.load(), sym)(ops._ctx_on_stream()._h, C.byref(p), *args)
 
 
-def _problem(nodes, id_table, dense, sparse, comb=0):
-    import euler_b200
-    from euler_b200 import ops
-    g = euler_b200.get_graph()
-    res = [(g.sparse_feature_id(n), t, dv, ops._COMBINERS[c]) for n, t, dv, c in sparse]
-    return ops._shallow_problem(nodes, id_table, [(g.dense_feature_id(n) if isinstance(n, str) else n, d) for n, d in dense], res, comb)
-
-
 def test_raw_abi_unaligned_output_and_statuses(env):
     """the C entry point with an out pointer 4 bytes past a 16-byte boundary gives the same bits; the refusals' statuses"""
     import euler_b200
@@ -141,7 +123,7 @@ def test_raw_abi_unaligned_output_and_statuses(env):
     nodes = torch.as_tensor(env["nodes"], device="cuda")
     id_table, sparse = _inputs(16)
     dense = DENSE[:2]
-    p = _problem(nodes, id_table, dense, sparse)
+    p = er.shallow_problem(nodes, id_table, dense, sparse)
     W = 16 + 15 + 3 * 16
     buf = torch.empty(M // 10 * W + 1, device="cuda")
     assert _raw("eu_shallow_encode_pool", p, 10, 1, buf.data_ptr() + 4) == 0
@@ -156,7 +138,7 @@ def test_raw_abi_unaligned_output_and_statuses(env):
     assert _raw("eu_shallow_encode_pool", p, 10, 1, None) == INVALID
     assert _raw("eu_shallow_encode_pool", p, 640, 1, out.data_ptr()) == UNSUPPORTED    # beyond EU_SHALLOW_POOL_MAX_COUNT
     assert _lib.SHALLOW_POOL_MAX_COUNT == 512
-    p_add = _problem(nodes, id_table, [], sparse, comb=1)
+    p_add = er.shallow_problem(nodes, id_table, [], sparse, comb=1)
     assert _raw("eu_shallow_encode_pool", p_add, 10, 1, out.data_ptr()) == UNSUPPORTED
     grads = (C.c_void_p * 4)(*[torch.empty_like(t).data_ptr() for t in [id_table] + [s[1] for s in sparse]])
     assert _raw("eu_shallow_encode_pool_backward", p, 3, 1, out.data_ptr(), grads) == INVALID

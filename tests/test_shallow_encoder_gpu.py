@@ -4,7 +4,6 @@ the sparse COO gradients of shallow_encode and sparse_feature_embedding; and Sha
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 import embedding_reference as er
 
@@ -64,15 +63,6 @@ def _inputs(dim, off=0, combiners=("sum", "mean")):
     return id_table, sparse
 
 
-def _composed_parts(nodes, id_table, dense, sparse):
-    import euler_b200
-    nd = torch.as_tensor(nodes, device="cuda")
-    idp = [F.embedding(nd, id_table)] if id_table is not None else []
-    dp = euler_b200.get_dense_feature(nd, [n for n, _ in dense], [d for _, d in dense]) if dense else []
-    sp = [euler_b200.sparse_feature_embedding(nd, n, t, dv, c) for n, t, dv, c in sparse]
-    return idp, dp, sp
-
-
 @pytest.mark.parametrize("dim", (1, 3, 4, 16, 128))
 def test_concat_forward_bit_exact(env, dim):
     import euler_b200
@@ -81,11 +71,11 @@ def test_concat_forward_bit_exact(env, dim):
         id_table, sparse = _inputs(dim, off)
         for dense in (DENSE, DENSE[:1], []):
             out = euler_b200.shallow_encode(nodes, id_table, dense, sparse, "concat")
-            idp, dp, sp = _composed_parts(nodes, id_table, dense, sparse)
+            idp, dp, sp = er.composed_parts(nodes, id_table, dense, sparse)
             want = torch.cat(idp + dp + sp, 1)
             assert out.shape == want.shape and out.cpu().numpy().tobytes() == want.cpu().numpy().tobytes(), (dim, off, len(dense))
         out = euler_b200.shallow_encode(nodes, None, DENSE[:2], sparse[1:], "concat")   # no id table
-        idp, dp, sp = _composed_parts(nodes, None, DENSE[:2], sparse[1:])
+        idp, dp, sp = er.composed_parts(nodes, None, DENSE[:2], sparse[1:])
         assert out.cpu().numpy().tobytes() == torch.cat(dp + sp, 1).cpu().numpy().tobytes()
 
 
@@ -124,7 +114,7 @@ def test_add_forward_bit_exact_and_close_to_f64(env, dim):
     for off in (0, 1):
         id_table, sparse = _inputs(dim, off)
         emb, feats = euler_b200.shallow_encode(nodes, id_table, DENSE, sparse, "add")
-        idp, dp, sp = _composed_parts(nodes, id_table, DENSE, sparse)
+        idp, dp, sp = er.composed_parts(nodes, id_table, DENSE, sparse)
         want = idp[0]
         for x in sp:
             want = want + x    # the documented order: id + sparse_0 + sparse_1 + ..
@@ -141,7 +131,7 @@ def test_add_forward_bit_exact_and_close_to_f64(env, dim):
         err = np.abs(emb.cpu().numpy() - sum(parts))
         assert (err <= 1e-6 * mag + 1e-7).all(), float((err / (mag + 1e-30)).max())
     emb, feats = euler_b200.shallow_encode(nodes, None, [], sparse[:1], "add")   # one term: its bits
-    assert feats is None and torch.equal(emb, _composed_parts(nodes, None, [], sparse[:1])[2][0])
+    assert feats is None and torch.equal(emb, er.composed_parts(nodes, None, [], sparse[:1])[2][0])
 
 
 def test_bad_inputs_raise(env):

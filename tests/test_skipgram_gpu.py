@@ -22,38 +22,16 @@ def graph():
     return g
 
 
-def _table(n_rows, dim, rng, offset=0, dyadic=True):
-    """a table whose data pointer is `offset` floats past a 16-byte boundary; dyadic: values k / 8, |k| <= 8"""
-    v = rng.randint(-8, 9, size=n_rows * dim + offset) / 8.0 if dyadic else rng.randn(n_rows * dim + offset) * 0.3
-    t = torch.tensor(v, dtype=torch.float32).cuda()
-    return t[offset:].view(n_rows, dim)
-
-
-def _ids(rng, B, P, K, n_rows):
-    src = rng.randint(0, n_rows, size=B)
-    pos = rng.randint(0, n_rows, size=(B, P))
-    negs = rng.randint(0, n_rows, size=(B, K))
-    src[:3] = n_rows - 1            # the default row max_id + 1 of a table of max_id + 2 rows
-    pos[3:6, 0] = n_rows - 1
-    return src, pos, negs
-
-
-def _fwd(src, pos, negs, target, context):
-    from euler_b200 import ops
-    d = lambda a: torch.as_tensor(a, dtype=torch.int64).cuda().contiguous()   # noqa: E731
-    return ops._raw_skipgram(d(src).reshape(-1), d(pos), d(negs).reshape(len(src), -1), target, context)
-
-
 @pytest.mark.parametrize("dim", DIMS)
 @pytest.mark.parametrize("P,K", PK)
 def test_forward_logits_ranks_bit_exact(graph, dim, P, K):
     rng = np.random.RandomState(dim * 31 + P * 7 + K)
     n_rows, B = 300, 257
-    src, pos, negs = _ids(rng, B, P, K, n_rows)
+    src, pos, negs = sr.pair_ids(rng, B, P, K, n_rows)
     ctx = sr.context_ids(pos, negs)
     for off in (0, 1):
-        target, context = _table(n_rows, dim, rng, off), _table(n_rows, dim, rng, 3 - off)
-        logits, rank, loss = _fwd(src, pos, negs, target, context)
+        target, context = sr.device_table(n_rows, dim, rng, off), sr.device_table(n_rows, dim, rng, 3 - off)
+        logits, rank, loss = sr.device_forward(src, pos, negs, target, context)
         tn, cn = target.cpu().numpy(), context.cpu().numpy()
         x = logits.cpu().numpy()
         head = sr.logits_f32(tn, cn, src[:24], ctx[:24])          # the fixed order, literally, on the first rows
@@ -69,12 +47,12 @@ def test_metrics_exact_with_ties(graph, name):
     import euler_b200
     rng = np.random.RandomState(4)
     n_rows, dim, P, K = 50, 4, 2, 20
-    target = _table(n_rows, dim, rng)
+    target = sr.device_table(n_rows, dim, rng)
     target[:, 1:] = 0
     target[:, 0] = torch.tensor(rng.randint(-2, 3, size=n_rows), dtype=torch.float32)   # logits in a handful of values
-    src, pos, negs = _ids(rng, 999, P, K, n_rows)
+    src, pos, negs = sr.pair_ids(rng, 999, P, K, n_rows)
     loss, met = euler_b200.skipgram_xent_loss(src, pos, negs, target, target, metric=name)
-    x = _fwd(src, pos, negs, target, target)[0].cpu().numpy()
+    x = sr.device_forward(src, pos, negs, target, target)[0].cpu().numpy()
     rank = sr.rank_top_k_literal(x[:, :P], x[:, P:])
     assert len(np.unique(x)) <= 25 and (rank > 0).sum() > 100
     want = sr.metric(rank, name)
@@ -84,8 +62,8 @@ def test_metrics_exact_with_ties(graph, name):
 def test_out_of_range_ids_raise(graph):
     import euler_b200
     rng = np.random.RandomState(1)
-    t = _table(100, 8, rng)
-    src, pos, negs = _ids(rng, 64, 1, 5, 100)
+    t = sr.device_table(100, 8, rng)
+    src, pos, negs = sr.pair_ids(rng, 64, 1, 5, 100)
     for which, bad in (("src", -1), ("pos", 100), ("negs", 1 << 40)):
         s, p, n = src.copy(), pos.copy(), negs.copy()
         {"src": s, "pos": p, "negs": n}[which].flat[17] = bad
@@ -106,27 +84,18 @@ def test_empty_batch(graph):
     assert float(t.grad.abs().sum()) == 0 and float(c.grad.abs().sum()) == 0
 
 
-def _grads(src, pos, negs, target, context, shared=False, sparse=False, g=None):
-    import euler_b200
-    T = target.clone().requires_grad_(True)
-    Cx = T if shared else context.clone().requires_grad_(True)
-    loss, _ = euler_b200.skipgram_xent_loss(src, pos, negs, T, Cx, sparse_grad=sparse)
-    loss.backward(None if g is None else torch.tensor(g, dtype=torch.float32, device="cuda"))
-    return loss, T.grad, (None if shared else Cx.grad)
-
-
 @pytest.mark.parametrize("dim", (1, 3, 16, 128, 200))
 @pytest.mark.parametrize("P,K", ((1, 5), (3, 20), (1, 0)))
 def test_gradients_match_float64(graph, dim, P, K):
     rng = np.random.RandomState(dim + 10 * K + P)
     n_rows, B = 500, 3000
-    src, pos, negs = _ids(rng, B, P, K, n_rows)
+    src, pos, negs = sr.pair_ids(rng, B, P, K, n_rows)
     if K:
         negs[:, 0] = 7                                 # a hub negative over many chunks
     ctx = sr.context_ids(pos, negs)
     for off in (0, 1):
-        target, context = _table(n_rows, dim, rng, off, dyadic=False), _table(n_rows, dim, rng, off, dyadic=False)
-        _, gt, gc = _grads(src, pos, negs, target, context)
+        target, context = sr.device_table(n_rows, dim, rng, off, dyadic=False), sr.device_table(n_rows, dim, rng, off, dyadic=False)
+        _, gt, gc = sr.device_grads(src, pos, negs, target, context)
         wt, wc = sr.grads64(target.cpu().numpy(), context.cpu().numpy(), src, ctx, P)
         for got, want in ((gt, wt), (gc, wc)):
             got = got.cpu().numpy()
@@ -158,7 +127,7 @@ def test_integer_gradients_exact_through_many_chunks(graph, dim):
     target, context, src, pos, negs = _integer_setup(rng, dim, B, K, hub_reps=1500)
     ctx = sr.context_ids(pos, negs)
     N = B * (1 + K)
-    _, gt, gc = _grads(src, pos, negs, target, context, g=float(N))
+    _, gt, gc = sr.device_grads(src, pos, negs, target, context, g=float(N))
     wt, wc = sr.grads64(target.cpu().numpy(), context.cpu().numpy(), src, ctx, 1, g=N)
     wt, wc = np.round(wt), np.round(wc)               # the f64 coefficients are +-1 up to e^-128
     assert np.array_equal(gt.cpu().numpy(), wt) and np.array_equal(gc.cpu().numpy(), wc)
@@ -167,13 +136,13 @@ def test_integer_gradients_exact_through_many_chunks(graph, dim):
 
 def test_gradients_bit_identical_run_to_run(graph):
     rng = np.random.RandomState(9)
-    src, pos, negs = _ids(rng, 20000, 1, 5, 3000)
+    src, pos, negs = sr.pair_ids(rng, 20000, 1, 5, 3000)
     negs[:, 2] = 42
-    target, context = _table(3000, 64, rng, dyadic=False), _table(3000, 64, rng, dyadic=False)
+    target, context = sr.device_table(3000, 64, rng, dyadic=False), sr.device_table(3000, 64, rng, dyadic=False)
     for shared in (False, True):
         for sparse in (False, True):
-            a = _grads(src, pos, negs, target, context, shared, sparse)
-            b = _grads(src, pos, negs, target, context, shared, sparse)
+            a = sr.device_grads(src, pos, negs, target, context, shared, sparse)
+            b = sr.device_grads(src, pos, negs, target, context, shared, sparse)
             assert float(a[0].detach()) == float(b[0].detach())
             for x, y in zip(a[1:], b[1:]):
                 if x is None:
@@ -184,11 +153,11 @@ def test_gradients_bit_identical_run_to_run(graph):
 
 def test_shared_table_is_the_sum_of_both_gradients(graph):
     rng = np.random.RandomState(12)
-    src, pos, negs = _ids(rng, 5000, 3, 5, 700)
+    src, pos, negs = sr.pair_ids(rng, 5000, 3, 5, 700)
     negs[:, 1] = 5
-    t = _table(700, 32, rng)
-    _, g_sh, _ = _grads(src, pos, negs, t, t, shared=True)
-    _, gt, gc = _grads(src, pos, negs, t, t.clone())
+    t = sr.device_table(700, 32, rng)
+    _, g_sh, _ = sr.device_grads(src, pos, negs, t, t, shared=True)
+    _, gt, gc = sr.device_grads(src, pos, negs, t, t.clone())
     want = (gt.double() + gc.double())
     assert torch.allclose(g_sh.double(), want, rtol=1e-6, atol=1e-6 * float(want.abs().max()))
     wt, wc = sr.grads64(t.cpu().numpy(), t.cpu().numpy(), src, sr.context_ids(pos, negs), 3)
@@ -199,11 +168,11 @@ def test_shared_table_is_the_sum_of_both_gradients(graph):
 @pytest.mark.parametrize("dim", (3, 64))
 def test_sparse_gradient_is_the_coalesced_dense_one(graph, shared, dim):
     rng = np.random.RandomState(dim + shared)
-    src, pos, negs = _ids(rng, 4000, 1, 5, 100000)
+    src, pos, negs = sr.pair_ids(rng, 4000, 1, 5, 100000)
     negs[:, 0] = 99
-    target, context = _table(100000, dim, rng, dyadic=False), _table(100000, dim, rng, dyadic=False)
-    _, dt, dc = _grads(src, pos, negs, target, context, shared)
-    _, st, sc = _grads(src, pos, negs, target, context, shared, sparse=True)
+    target, context = sr.device_table(100000, dim, rng, dyadic=False), sr.device_table(100000, dim, rng, dyadic=False)
+    _, dt, dc = sr.device_grads(src, pos, negs, target, context, shared)
+    _, st, sc = sr.device_grads(src, pos, negs, target, context, shared, sparse=True)
     for d, s in ((dt, st), (dc, sc)):
         if d is None:
             assert s is None
