@@ -235,6 +235,10 @@ SIGNATURES = {
     "eu_skipgram_loss_backward": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P]),
     "eu_skipgram_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _P, _P, _P, _P, _P,
                                                    _P, _P]),
+    "eu_skipgram_loss_dtype": (C.c_int, [_P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _I32, _P, _P, _P]),
+    "eu_skipgram_loss_backward_dtype": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _I32, _P, _P, _P]),
+    "eu_skipgram_loss_backward_sparse_dtype": (C.c_int, [_P, _P, _P, _P, _P, _I64, _I32, _I32, _P, _P, _I64, _I32, _I32, _P, _P,
+                                                         _P, _P, _P, _P, _P]),
     "eu_gae_loss": (C.c_int, [_P, _I64, _I32, _I32, _P, _P, _P, _F, _P, _P, _P]),
     "eu_gae_loss_backward": (C.c_int, [_P, _P, _I64, _I32, _I32, _P, _P, _P, _F, _P, _P, _P]),
     "eu_metric_auc_update": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
@@ -242,6 +246,9 @@ SIGNATURES = {
     "eu_optim_momentum": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _I64, _F, _F]),
     "eu_optim_adagrad": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _I64, _F]),
     "eu_optim_adam": (C.c_int, [_P, _P, _P, _P, _I64, _I32, _P, _P, _I64, _P, _F, _F, _F, _F]),
+    "eu_optim_momentum_dtype": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _I64, _F, _F, _I32, _U64, _P, _I32]),
+    "eu_optim_adagrad_dtype": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _P, _I64, _F, _I32, _U64, _P, _I32]),
+    "eu_optim_adam_dtype": (C.c_int, [_P, _P, _P, _P, _I64, _I32, _P, _P, _I64, _P, _F, _F, _F, _F, _I32, _U64, _P, _I32]),
     "eu_kg_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "eu_kg_loss_backward": (C.c_int, [_P, _P, _P, _P, _P]),
     "eu_kg_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),

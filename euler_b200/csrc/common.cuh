@@ -157,6 +157,18 @@ template <typename T> __device__ __forceinline__ T feat_st(float v);
 template <> __device__ __forceinline__ float feat_st<float>(float v) { return v; }
 template <> __device__ __forceinline__ __nv_bfloat16 feat_st<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
+// A trained bf16 table (optim.cu) is written through sr_st instead: stochastic rounding with a 16-bit random integer r, added
+// to the low half of the f32 bits before they are truncated, so v rounds up with probability (its distance from the value
+// below) / ulp and the rounding is unbiased.  r = 0 truncates toward zero; r = 0x8000 rounds to nearest with ties away from
+// zero.  +-Inf stays; a NaN keeps its sign and upper payload and is made quiet; a finite value can carry into +-Inf only
+// from above the largest finite bf16.  Round to nearest would lose every update smaller than half an ulp.
+__device__ __forceinline__ __nv_bfloat16 sr_st(float v, uint32_t r) {
+  const uint32_t u = __float_as_uint(v);
+  const uint32_t h = (u & 0x7F800000u) == 0x7F800000u ? (u >> 16) | ((u & 0x007FFFFFu) ? 0x0040u : 0u)
+                                                      : (u + (r & 0xFFFFu)) >> 16;
+  return __ushort_as_bfloat16((unsigned short)h);
+}
+
 // Row `row`'s slice of ragged slot `fid` (ptr of S slots per row): [b, e) in the value array, b == e when the node / slot does
 // not exist
 __device__ __forceinline__ void ragged_slice(const int64_t* __restrict__ ptr, int32_t S, int64_t row, int32_t fid, int64_t* b, int64_t* e) {
@@ -271,6 +283,18 @@ __device__ __forceinline__ void philox_uniform2(unsigned long long id, uint32_t 
   unsigned long long b = ((unsigned long long)c[2] << 32) | c[3];
   u0 = (double)(a >> 11) * (1.0 / 9007199254740992.0);
   u1 = (double)(b >> 11) * (1.0 / 9007199254740992.0);
+}
+
+// the 128 bits of one Philox4x32-10 block: counter (element lo, element hi, step, tensor), key seed
+__device__ __forceinline__ uint4 philox_bits(unsigned long long seed, uint32_t step, uint32_t tensor, unsigned long long element) {
+  uint32_t c[4] = {(uint32_t)element, (uint32_t)(element >> 32), step, tensor};
+  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    philox_round(c, k0, k1);
+    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+  }
+  return make_uint4(c[0], c[1], c[2], c[3]);
 }
 
 // ---------------------------------------------------------------------------------- TMA bulk copy (sm_90+)

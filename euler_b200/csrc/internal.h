@@ -35,6 +35,8 @@ extern std::atomic<uint64_t> g_launches;
   } while (0)
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+// a table of eu_feat_dtype dtype takes 4-wide loads (16 bytes of f32, 8 of bf16) where p is aligned to four of its elements
+inline bool aligned4_elems(const void* p, int dtype) { return ((uintptr_t)p & (dtype == EU_FEAT_BF16 ? 7 : 15)) == 0; }
 
 struct ETList {           // an edge-type list passed by value to the full-neighbor kernels
   int32_t K;

@@ -27,6 +27,16 @@
 // row once: 24 N D + 4 R (D + 2) bytes.  Sparse Momentum and Adagrad touch the R rows only; dense forms are element-wise.
 // float4 when D % 4 == 0 and every pointer is 16-byte aligned, scalar otherwise; element indices are 64-bit.  No float
 // atomics and no host synchronisation.  A row outside [0, N) is never written.
+//
+// bf16 tables (T = __nv_bfloat16: var and every slot bf16, the gradient f32; the *_dtype entry points).  Each element is
+// widened exactly to f32, updated by the same upd / adam_decay in f32, and each value written (var and every slot) is rounded
+// to bf16 by sr_st (common.cuh), stochastic rounding.  Its 16 random bits are the low half of word w (0 var, 1 the first slot,
+// 2 the second) of philox_bits(seed, step, tensor, element): element is the flat index r D + col into var, step the low 32
+// bits of the device step counter (the caller advances it once per step, after every variable, as Adam's powers), tensor the
+// variable's index among the caller's.  A step is thus deterministic and can be captured in a CUDA graph.  The 4-wide form
+// needs var and the slots 8-byte aligned (one 8-byte load or store per tensor and element group of four).
+#include <type_traits>
+
 #include "internal.h"
 
 namespace eu {
@@ -73,62 +83,109 @@ __device__ __forceinline__ void adam_decay(const OptArgs& a, float alpha, float&
   w = __fsub_rn(w, __fdiv_rn(__fmul_rn(alpha, m), __fadd_rn(__fsqrt_rn(v), a.eps)));
 }
 
-// VW consecutive floats: one float4 or one float
+// the stochastic-rounding key of a bf16 update (see the top of the file); unused by f32 tables
+struct SrKey {
+  unsigned long long seed;
+  const int64_t* step;   // device step counter
+  uint32_t tensor;
+};
+
+template <typename T>
+constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
+
+// the random words of the elements [e, e + VW) of var: r[w][i] rounds tensor w (0 var, 1 slot 1, 2 slot 2) of element e + i
 template <int VW>
+__device__ __forceinline__ void sr_words(const SrKey& k, int64_t e, uint32_t (&r)[3][VW]) {
+  const uint32_t step = (uint32_t)__ldg(k.step);
+#pragma unroll
+  for (int i = 0; i < VW; ++i) {
+    const uint4 q = philox_bits(k.seed, step, k.tensor, (unsigned long long)(e + i));
+    r[0][i] = q.x; r[1][i] = q.y; r[2][i] = q.z;
+  }
+}
+
+// VW consecutive elements of a table of T, as f32: one float4 / one 8-byte bf16 load, or one element
+template <int VW, typename T = float>
 struct Vec {
   float x[VW];
-  __device__ __forceinline__ void load(const float* p) {
-    if (VW == 4) {
+  __device__ __forceinline__ void load(const T* p) {
+    if constexpr (kBf16<T>) {
+      if (VW == 4) {
+        const uint2 u = *reinterpret_cast<const uint2*>(p);
+        x[0] = __uint_as_float(u.x << 16); x[1] = __uint_as_float(u.x & 0xFFFF0000u);
+        x[VW > 2 ? 2 : 0] = __uint_as_float(u.y << 16); x[VW > 3 ? 3 : 0] = __uint_as_float(u.y & 0xFFFF0000u);
+      } else {
+        x[0] = __uint_as_float((uint32_t)*reinterpret_cast<const unsigned short*>(p) << 16);
+      }
+    } else if (VW == 4) {
       const float4 t = *reinterpret_cast<const float4*>(p);
       x[0] = t.x; x[1] = t.y; x[2] = t.z; x[3] = t.w;
     } else {
       x[0] = *p;
     }
   }
-  __device__ __forceinline__ void store(float* p) const {
-    if (VW == 4) *reinterpret_cast<float4*>(p) = make_float4(x[0], x[1], x[2], x[3]);
-    else *p = x[0];
+  // r: the elements' random words (bf16 only)
+  __device__ __forceinline__ void store(T* p, const uint32_t (&r)[VW]) const {
+    if constexpr (kBf16<T>) {
+      unsigned short h[VW];
+#pragma unroll
+      for (int i = 0; i < VW; ++i) h[i] = __bfloat16_as_ushort(sr_st(x[i], r[i]));
+      if (VW == 4) *reinterpret_cast<uint2*>(p) = make_uint2(h[0] | (uint32_t)h[VW > 1 ? 1 : 0] << 16,
+                                                              h[VW > 2 ? 2 : 0] | (uint32_t)h[VW > 3 ? 3 : 0] << 16);
+      else *reinterpret_cast<unsigned short*>(p) = h[0];
+    } else if (VW == 4) {
+      *reinterpret_cast<float4*>(p) = make_float4(x[0], x[1], x[2], x[3]);
+    } else {
+      *p = x[0];
+    }
   }
 };
 
 // dense form: element-wise over n = N D elements, VW per thread
-template <int K, int VW>
-__global__ void __launch_bounds__(kOptThreads) k_opt_dense(OptArgs a, float* __restrict__ var, float* __restrict__ s1,
-                                                           float* __restrict__ s2, const float* __restrict__ grad, int64_t n) {
+template <int K, int VW, typename T>
+__global__ void __launch_bounds__(kOptThreads) k_opt_dense(OptArgs a, T* __restrict__ var, T* __restrict__ s1,
+                                                           T* __restrict__ s2, const float* __restrict__ grad, int64_t n,
+                                                           SrKey sk) {
   const int64_t e = (blockIdx.x * (int64_t)kOptThreads + threadIdx.x) * VW;
   if (e >= n) return;
   const float alpha = K == kAdam ? adam_alpha(a) : 0.f;
-  Vec<VW> w, x, y, g;
+  Vec<VW, T> w, x, y;
+  Vec<VW> g;
   w.load(var + e);
   x.load(s1 + e);
   if (K == kAdam) y.load(s2 + e);
   g.load(grad + e);
 #pragma unroll
   for (int i = 0; i < VW; ++i) upd<K, false>(a, alpha, g.x[i], w.x[i], x.x[i], y.x[i]);
-  w.store(var + e);
-  x.store(s1 + e);
-  if (K == kAdam) y.store(s2 + e);
+  uint32_t r[3][VW] = {};
+  if constexpr (kBf16<T>) sr_words(sk, e, r);
+  w.store(var + e, r[0]);
+  x.store(s1 + e, r[1]);
+  if (K == kAdam) y.store(s2 + e, r[2]);
 }
 
 // sparse Momentum / Adagrad: element-wise over the R D gradient elements, VW per thread
-template <int K, int VW>
-__global__ void __launch_bounds__(kOptThreads) k_opt_rows(OptArgs a, float* __restrict__ var, float* __restrict__ s1,
+template <int K, int VW, typename T>
+__global__ void __launch_bounds__(kOptThreads) k_opt_rows(OptArgs a, T* __restrict__ var, T* __restrict__ s1,
                                                           int64_t N, int D, const float* __restrict__ grad,
-                                                          const int64_t* __restrict__ rows, int64_t R) {
+                                                          const int64_t* __restrict__ rows, int64_t R, SrKey sk) {
   const int64_t q = blockIdx.x * (int64_t)kOptThreads + threadIdx.x, per_row = D / VW;
   if (q >= R * per_row) return;
   const int64_t k = q / per_row, col = (q - k * per_row) * VW, r = __ldg(rows + k);
   if (r < 0 || r >= N) return;
   const int64_t e = r * D + col;
-  Vec<VW> w, x, g;
+  Vec<VW, T> w, x;
+  Vec<VW> g;
   float unused = 0.f;
   w.load(var + e);
   x.load(s1 + e);
   g.load(grad + k * D + col);
 #pragma unroll
   for (int i = 0; i < VW; ++i) upd<K, true>(a, 0.f, g.x[i], w.x[i], x.x[i], unused);
-  w.store(var + e);
-  x.store(s1 + e);
+  uint32_t rw[3][VW] = {};
+  if constexpr (kBf16<T>) sr_words(sk, e, rw);
+  w.store(var + e, rw[0]);
+  x.store(s1 + e, rw[1]);
 }
 
 // the first k in [0, R) with rows[k] >= r0 (R if none), by warp 0: each round the 32 lanes probe 32 evenly spaced rows of the
@@ -149,22 +206,22 @@ __device__ int64_t warp_lower_bound(const int64_t* __restrict__ rows, int64_t R,
 }
 
 // sparse Adam: CTA b owns the rows [b rpc, b rpc + nr) (rpc = rows_per_cta), nr D elements in passes of kChunk
-template <int VW>
-__global__ void __launch_bounds__(kOptThreads) k_adam_sparse(OptArgs a, float* __restrict__ var, float* __restrict__ m,
-                                                             float* __restrict__ v, int64_t N, int D,
+template <int VW, typename T>
+__global__ void __launch_bounds__(kOptThreads) k_adam_sparse(OptArgs a, T* __restrict__ var, T* __restrict__ m,
+                                                             T* __restrict__ v, int64_t N, int D,
                                                              const float* __restrict__ grad, const int64_t* __restrict__ rows,
-                                                             int64_t R, int rows_per_cta) {
+                                                             int64_t R, int rows_per_cta, SrKey sk) {
   constexpr int kItems = 16 / VW;   // vectors per thread per pass
   __shared__ int s_slot[kChunk];    // the CTA's row i -> its gradient row - lo, or -1
   __shared__ long long s_lo;
   const int64_t r0 = blockIdx.x * (int64_t)rows_per_cta;
   const int nr = (int)min((int64_t)rows_per_cta, N - r0);
   const int nq = nr * D / VW;   // vectors of the CTA (a vector never straddles two rows)
-  float* const vb = var + r0 * D;
-  float* const mb = m + r0 * D;
-  float* const sb = v + r0 * D;
+  T* const vb = var + r0 * D;
+  T* const mb = m + r0 * D;
+  T* const sb = v + r0 * D;
   const float alpha = adam_alpha(a);
-  Vec<VW> w[kItems], x[kItems], y[kItems];
+  Vec<VW, T> w[kItems], x[kItems], y[kItems];
   // the first pass's loads go out before the search, so the search's latency hides under them
 #pragma unroll
   for (int u = 0; u < kItems; ++u) {
@@ -214,18 +271,21 @@ __global__ void __launch_bounds__(kOptThreads) k_adam_sparse(OptArgs a, float* _
 #pragma unroll
         for (int i = 0; i < VW; ++i) adam_decay(a, alpha, w[u].x[i], x[u].x[i], y[u].x[i]);
       }
-      w[u].store(vb + (int64_t)e);
-      x[u].store(mb + (int64_t)e);
-      y[u].store(sb + (int64_t)e);
+      uint32_t r[3][VW] = {};
+      if constexpr (kBf16<T>) sr_words(sk, r0 * D + e, r);
+      w[u].store(vb + (int64_t)e, r[0]);
+      x[u].store(mb + (int64_t)e, r[1]);
+      y[u].store(sb + (int64_t)e, r[2]);
     }
   }
 }
 
 static bool a16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
-// the shared checks of the three entry points; *dense is set when R == EU_OPTIM_DENSE
-static int opt_check(const char* who, eu_ctx* c, const float* var, const float* s1, const float* s2, bool two_slots, int64_t N,
-                     int32_t D, const float* grad, const int64_t* rows, int64_t R, bool* dense) {
+// the shared checks of the entry points; *dense is set when R == EU_OPTIM_DENSE
+static int opt_check(const char* who, eu_ctx* c, const void* var, const void* s1, const void* s2, bool two_slots, int64_t N,
+                     int32_t D, const float* grad, const int64_t* rows, int64_t R, int32_t dtype, const int64_t* step,
+                     bool* dense) {
   *dense = R == EU_OPTIM_DENSE;
   const bool any = N > 0;
   if (!c || N < 0 || D < 1 || (R < 0 && !*dense) || (!*dense && R > N) || (any && (!var || !s1 || (two_slots && !s2))) ||
@@ -234,30 +294,109 @@ static int opt_check(const char* who, eu_ctx* c, const float* var, const float* 
               "when R > 0))", who);
     return EU_ERR_INVALID;
   }
+  if ((dtype != EU_FEAT_F32 && dtype != EU_FEAT_BF16) || (dtype == EU_FEAT_BF16 && !step)) {
+    set_error("%s: bad argument (dtype EU_FEAT_F32 or EU_FEAT_BF16, and a bf16 table needs the device step counter)", who);
+    return EU_ERR_INVALID;
+  }
   return EU_OK;
 }
 
-template <int K>
-static int launch_dense(eu_ctx* c, const OptArgs& a, float* var, float* s1, float* s2, const float* grad, int64_t n, bool vec) {
+// the 4-wide form: D % 4 == 0, var and the slots aligned to four elements, grad to 16 bytes
+static bool opt_vec(int32_t D, int32_t dtype, const void* var, const void* s1, const void* s2, const float* grad) {
+  return D % 4 == 0 && aligned4_elems(var, dtype) && aligned4_elems(s1, dtype) && (!s2 || aligned4_elems(s2, dtype)) && a16(grad);
+}
+
+template <int K, typename T>
+static int launch_dense(eu_ctx* c, const OptArgs& a, const SrKey& sk, T* var, T* s1, T* s2, const float* grad, int64_t n,
+                        bool vec) {
   if (n == 0) return EU_OK;
   const int vw = vec ? 4 : 1;
   const unsigned blocks = (unsigned)ceil_div(ceil_div(n, vw), kOptThreads);
-  if (vec) k_opt_dense<K, 4><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, s2, grad, n);
-  else k_opt_dense<K, 1><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, s2, grad, n);
+  if (vec) k_opt_dense<K, 4><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, s2, grad, n, sk);
+  else k_opt_dense<K, 1><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, s2, grad, n, sk);
   EU_LAUNCHED();
   return EU_OK;
 }
 
-template <int K>
-static int launch_rows(eu_ctx* c, const OptArgs& a, float* var, float* s1, int64_t N, int D, const float* grad,
+template <int K, typename T>
+static int launch_rows(eu_ctx* c, const OptArgs& a, const SrKey& sk, T* var, T* s1, int64_t N, int D, const float* grad,
                        const int64_t* rows, int64_t R, bool vec) {
   if (R == 0) return EU_OK;
   const int vw = vec ? 4 : 1;
   const unsigned blocks = (unsigned)ceil_div(R * (D / vw), kOptThreads);
-  if (vec) k_opt_rows<K, 4><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, N, D, grad, rows, R);
-  else k_opt_rows<K, 1><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, N, D, grad, rows, R);
+  if (vec) k_opt_rows<K, 4><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, N, D, grad, rows, R, sk);
+  else k_opt_rows<K, 1><<<blocks, kOptThreads, 0, c->stream>>>(a, var, s1, N, D, grad, rows, R, sk);
   EU_LAUNCHED();
   return EU_OK;
+}
+
+// Momentum (K = kMomentum) or Adagrad over a table of T
+template <int K, typename T>
+static int run_one_slot(eu_ctx* c, const OptArgs& a, const SrKey& sk, void* var, void* accum, int64_t N, int32_t D,
+                        const float* grad, const int64_t* rows, int64_t R, bool dense, bool vec) {
+  T* w = static_cast<T*>(var);
+  T* s1 = static_cast<T*>(accum);
+  return dense ? launch_dense<K>(c, a, sk, w, s1, (T*)nullptr, grad, N * D, vec) : launch_rows<K>(c, a, sk, w, s1, N, D, grad, rows, R, vec);
+}
+
+template <typename T>
+static int run_adam(eu_ctx* c, const OptArgs& a, const SrKey& sk, void* var, void* m, void* v, int64_t N, int32_t D,
+                    const float* grad, const int64_t* rows, int64_t R, bool dense, bool vec) {
+  T* w = static_cast<T*>(var);
+  T* s1 = static_cast<T*>(m);
+  T* s2 = static_cast<T*>(v);
+  if (dense) return launch_dense<kAdam>(c, a, sk, w, s1, s2, grad, N * D, vec);
+  if (N == 0) return EU_OK;
+  const int rows_per_cta = D >= kChunk ? 1 : kChunk / D;
+  const unsigned blocks = (unsigned)ceil_div(N, rows_per_cta);
+  if (vec) k_adam_sparse<4><<<blocks, kOptThreads, 0, c->stream>>>(a, w, s1, s2, N, D, grad, rows, R, rows_per_cta, sk);
+  else k_adam_sparse<1><<<blocks, kOptThreads, 0, c->stream>>>(a, w, s1, s2, N, D, grad, rows, R, rows_per_cta, sk);
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+static int momentum(const char* who, eu_ctx* c, void* var, void* accum, int64_t N, int32_t D, const float* grad,
+                    const int64_t* rows, int64_t R, float lr, float mom, int32_t dtype, const SrKey& sk) {
+  bool dense;
+  int rc;
+  if ((rc = opt_check(who, c, var, accum, nullptr, false, N, D, grad, rows, R, dtype, sk.step, &dense))) return rc;
+  EU_CUDA(cudaSetDevice(c->g->device));
+  const OptArgs a{lr, mom, 0.f, 0.f, 0.f, nullptr};
+  const bool vec = opt_vec(D, dtype, var, accum, nullptr, grad);
+  EuProfScope ps(c, "optim_momentum", dense ? N : R);
+  return dtype == EU_FEAT_BF16 ? run_one_slot<kMomentum, __nv_bfloat16>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec)
+                               : run_one_slot<kMomentum, float>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec);
+}
+
+static int adagrad(const char* who, eu_ctx* c, void* var, void* accum, int64_t N, int32_t D, const float* grad,
+                   const int64_t* rows, int64_t R, float lr, int32_t dtype, const SrKey& sk) {
+  bool dense;
+  int rc;
+  if ((rc = opt_check(who, c, var, accum, nullptr, false, N, D, grad, rows, R, dtype, sk.step, &dense))) return rc;
+  EU_CUDA(cudaSetDevice(c->g->device));
+  const OptArgs a{lr, 0.f, 0.f, 0.f, 0.f, nullptr};
+  const bool vec = opt_vec(D, dtype, var, accum, nullptr, grad);
+  EuProfScope ps(c, "optim_adagrad", dense ? N : R);
+  return dtype == EU_FEAT_BF16 ? run_one_slot<kAdagrad, __nv_bfloat16>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec)
+                               : run_one_slot<kAdagrad, float>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec);
+}
+
+static int adam(const char* who, eu_ctx* c, void* var, void* m, void* v, int64_t N, int32_t D, const float* grad,
+                const int64_t* rows, int64_t R, const float* powers, float lr, float beta1, float beta2, float epsilon,
+                int32_t dtype, const SrKey& sk) {
+  bool dense;
+  int rc;
+  if ((rc = opt_check(who, c, var, m, v, true, N, D, grad, rows, R, dtype, sk.step, &dense))) return rc;
+  if (!powers) {
+    set_error("%s: powers (device f32[2]: beta1_power, beta2_power) is needed", who);
+    return EU_ERR_INVALID;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  const OptArgs a{lr, 0.f, beta1, beta2, epsilon, powers};
+  const bool vec = opt_vec(D, dtype, var, m, v, grad);
+  EuProfScope ps(c, "optim_adam", N);
+  return dtype == EU_FEAT_BF16 ? run_adam<__nv_bfloat16>(c, a, sk, var, m, v, N, D, grad, rows, R, dense, vec)
+                               : run_adam<float>(c, a, sk, var, m, v, N, D, grad, rows, R, dense, vec);
 }
 
 }  // namespace eu
@@ -268,51 +407,37 @@ extern "C" {
 
 int eu_optim_momentum(eu_ctx* c, float* var, float* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
                       int64_t R, float lr, float momentum) {
-  bool dense;
-  int rc;
-  if ((rc = opt_check("eu_optim_momentum", c, var, accum, nullptr, false, N, D, grad, rows, R, &dense))) return rc;
-  EU_CUDA(cudaSetDevice(c->g->device));
-  const OptArgs a{lr, momentum, 0.f, 0.f, 0.f, nullptr};
-  const bool vec = D % 4 == 0 && a16(var) && a16(accum) && a16(grad);
-  EuProfScope ps(c, "optim_momentum", dense ? N : R);
-  return dense ? launch_dense<kMomentum>(c, a, var, accum, nullptr, grad, N * D, vec)
-               : launch_rows<kMomentum>(c, a, var, accum, N, D, grad, rows, R, vec);
+  return eu::momentum("eu_optim_momentum", c, var, accum, N, D, grad, rows, R, lr, momentum, EU_FEAT_F32, SrKey{0, nullptr, 0});
 }
 
 int eu_optim_adagrad(eu_ctx* c, float* var, float* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
                      int64_t R, float lr) {
-  bool dense;
-  int rc;
-  if ((rc = opt_check("eu_optim_adagrad", c, var, accum, nullptr, false, N, D, grad, rows, R, &dense))) return rc;
-  EU_CUDA(cudaSetDevice(c->g->device));
-  const OptArgs a{lr, 0.f, 0.f, 0.f, 0.f, nullptr};
-  const bool vec = D % 4 == 0 && a16(var) && a16(accum) && a16(grad);
-  EuProfScope ps(c, "optim_adagrad", dense ? N : R);
-  return dense ? launch_dense<kAdagrad>(c, a, var, accum, nullptr, grad, N * D, vec)
-               : launch_rows<kAdagrad>(c, a, var, accum, N, D, grad, rows, R, vec);
+  return eu::adagrad("eu_optim_adagrad", c, var, accum, N, D, grad, rows, R, lr, EU_FEAT_F32, SrKey{0, nullptr, 0});
 }
 
 int eu_optim_adam(eu_ctx* c, float* var, float* m, float* v, int64_t N, int32_t D, const float* grad, const int64_t* rows,
                   int64_t R, const float* powers, float lr, float beta1, float beta2, float epsilon) {
-  bool dense;
-  int rc;
-  if ((rc = opt_check("eu_optim_adam", c, var, m, v, true, N, D, grad, rows, R, &dense))) return rc;
-  if (!powers) {
-    set_error("eu_optim_adam: powers (device f32[2]: beta1_power, beta2_power) is needed");
-    return EU_ERR_INVALID;
-  }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  const OptArgs a{lr, 0.f, beta1, beta2, epsilon, powers};
-  const bool vec = D % 4 == 0 && a16(var) && a16(m) && a16(v) && a16(grad);
-  EuProfScope ps(c, "optim_adam", N);
-  if (dense) return launch_dense<kAdam>(c, a, var, m, v, grad, N * D, vec);
-  if (N == 0) return EU_OK;
-  const int rows_per_cta = D >= kChunk ? 1 : kChunk / D;
-  const unsigned blocks = (unsigned)ceil_div(N, rows_per_cta);
-  if (vec) k_adam_sparse<4><<<blocks, kOptThreads, 0, c->stream>>>(a, var, m, v, N, D, grad, rows, R, rows_per_cta);
-  else k_adam_sparse<1><<<blocks, kOptThreads, 0, c->stream>>>(a, var, m, v, N, D, grad, rows, R, rows_per_cta);
-  EU_LAUNCHED();
-  return EU_OK;
+  return eu::adam("eu_optim_adam", c, var, m, v, N, D, grad, rows, R, powers, lr, beta1, beta2, epsilon, EU_FEAT_F32,
+                  SrKey{0, nullptr, 0});
+}
+
+int eu_optim_momentum_dtype(eu_ctx* c, void* var, void* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                            int64_t R, float lr, float momentum, int32_t dtype, uint64_t seed, const int64_t* step,
+                            int32_t tensor) {
+  return eu::momentum("eu_optim_momentum_dtype", c, var, accum, N, D, grad, rows, R, lr, momentum, dtype,
+                      SrKey{seed, step, (uint32_t)tensor});
+}
+
+int eu_optim_adagrad_dtype(eu_ctx* c, void* var, void* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                           int64_t R, float lr, int32_t dtype, uint64_t seed, const int64_t* step, int32_t tensor) {
+  return eu::adagrad("eu_optim_adagrad_dtype", c, var, accum, N, D, grad, rows, R, lr, dtype, SrKey{seed, step, (uint32_t)tensor});
+}
+
+int eu_optim_adam_dtype(eu_ctx* c, void* var, void* m, void* v, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                        int64_t R, const float* powers, float lr, float beta1, float beta2, float epsilon, int32_t dtype,
+                        uint64_t seed, const int64_t* step, int32_t tensor) {
+  return eu::adam("eu_optim_adam_dtype", c, var, m, v, N, D, grad, rows, R, powers, lr, beta1, beta2, epsilon, dtype,
+                  SrKey{seed, step, (uint32_t)tensor});
 }
 
 }  // extern "C"

@@ -226,8 +226,8 @@ __device__ __forceinline__ float* distinct_out_row(float* out, const DistinctPla
 // A column's adds are fma(w, x, acc) in entry order whatever the lane mapping, and fma(1, x, acc) is __fadd_rn(acc, x).  The
 // gathered kind asks for one block per SM: under the default bound ptxas spilled around the scalar path's division subroutine.
 // The other kinds keep the default (a minimum of 0 emits none); one block per SM would raise them from 63 / 80 registers to
-// 70 / 82, and the float4 form would then fit two blocks per SM instead of three.
-template <bool VEC, bool GATHER>
+// 70 / 82, and the float4 form would then fit two blocks per SM instead of three.  T: the storage type of S.target.
+template <bool VEC, bool GATHER, typename T>
 __global__ void __launch_bounds__(256, GATHER ? 1 : 0) k_row_chunks(RowEntries S, const int32_t* __restrict__ perm, DistinctPlan P,
                                                                     int dim, int G, bool by_key, float* __restrict__ out) {
   const int lg = 31 - __clz(G);
@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(256, GATHER ? 1 : 0) k_row_chunks(RowEntries S
               w[q] = 1.f;
             } else {
               const int64_t t = en - S.n_src;
-              x[q] = row_load4<VEC>(S.target + row_of(__ldg(S.src + t / S.J), S.n_rows, &ignored) * dim, d, dim);
+              x[q] = row_load4<VEC>(static_cast<const T*>(S.target) + row_of(__ldg(S.src + t / S.J), S.n_rows, &ignored) * dim, d, dim);
               w[q] = __ldg(S.coef + t);
             }
           }
@@ -308,11 +308,12 @@ int sum_distinct_rows(eu_ctx* c, const RowEntries& S, const RowList& L, int dim,
   if (!L.E) return EU_OK;
   cudaStream_t s = c->stream;
   const bool vec = dim % 4 == 0 && (!S.node || S.ld % 4 == 0) && aligned16(out) && (!S.gt || aligned16(S.gt)) &&
-                   (!S.target || aligned16(S.target));
+                   (!S.target || aligned4_elems(S.target, S.target_dtype));
   const int G = group_lanes(ceil_div(dim, 4));
   const unsigned blocks = stride_grid((L.E + L.E / kSegChunk + 1) * G);   // >= one group per chunk, up to the grid cap
-  auto chunks = vec ? (S.node ? k_row_chunks<true, true> : k_row_chunks<true, false>)
-                    : (S.node ? k_row_chunks<false, true> : k_row_chunks<false, false>);
+  auto chunks = S.target_dtype == EU_FEAT_BF16 ? (vec ? k_row_chunks<true, false, __nv_bfloat16> : k_row_chunks<false, false, __nv_bfloat16>)
+                : vec ? (S.node ? k_row_chunks<true, true, float> : k_row_chunks<true, false, float>)
+                      : (S.node ? k_row_chunks<false, true, float> : k_row_chunks<false, false, float>);
   chunks<<<blocks, 256, 0, s>>>(S, L.ord.perm, L.P, dim, G, by_key, out);
   EU_LAUNCHED();
   k_row_combine<<<stride_grid(L.E * dim), 256, 0, s>>>(L.P, dim, by_key, out, rows);

@@ -155,15 +155,16 @@ size_t row_plan_bytes(int64_t E, int64_t n_rows, int64_t width);
 // L's stable order by key and its distinct-row plan, in buf (row_plan_bytes), once L->key is written; nothing when E = 0
 int plan_rows(eu_ctx* c, char* buf, RowList* L);
 
-// the columns [d, d + 4) of a row (fewer than 4 at the row's end): one float4 load (VEC) or up to four scalar loads
-template <bool VEC>
-__device__ __forceinline__ float4 row_load4(const float* __restrict__ row, int d, int dim) {
-  if (VEC) return __ldg(reinterpret_cast<const float4*>(row + d));
+// the columns [d, d + 4) of a row of f32 or bf16 (T) widened to f32 (fewer than 4 at the row's end): one 4-wide load (VEC:
+// 16 bytes of f32, 8 of bf16, so row + d is aligned to four elements) or up to four scalar loads
+template <bool VEC, typename T>
+__device__ __forceinline__ float4 row_load4(const T* __restrict__ row, int d, int dim) {
+  if (VEC) return feat_ld4<T>(row + d);
   float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-  v.x = __ldg(row + d);
-  if (d + 1 < dim) v.y = __ldg(row + d + 1);
-  if (d + 2 < dim) v.z = __ldg(row + d + 2);
-  if (d + 3 < dim) v.w = __ldg(row + d + 3);
+  v.x = feat_ld<T>(row + d);
+  if (d + 1 < dim) v.y = feat_ld<T>(row + d + 1);
+  if (d + 2 < dim) v.z = feat_ld<T>(row + d + 2);
+  if (d + 3 < dim) v.w = feat_ld<T>(row + d + 3);
   return v;
 }
 
@@ -177,7 +178,7 @@ __device__ __forceinline__ int64_t row_of(int64_t v, int64_t n_rows, int* bad) {
 // The values of an entry list ordered by row.  Entries e < n_src are stored rows gt[e, :], or, when node is given (the
 // gathered kind: every entry stored), rows gt[r * ld, :] with r = node[e] / group, each element divided by pool_den first
 // unless that is 0.  Entries e >= n_src have coef[t] * target[src_b, :], t = e - n_src, b = t / J (computed while they are
-// summed).  A list of stored rows only has n_src = its length.
+// summed; target is f32 or bf16, target_dtype, widened as it is read).  A list of stored rows only has n_src = its length.
 struct RowEntries {
   int64_t n_src = 0;
   const float* gt = nullptr;
@@ -188,8 +189,9 @@ struct RowEntries {
   int J = 1;
   const float* coef = nullptr;
   const int64_t* src = nullptr;
-  const float* target = nullptr;
+  const void* target = nullptr;
   int64_t n_rows = 0;
+  int target_dtype = EU_FEAT_F32;   // last: the other members keep their offsets
 };
 
 // The sums per distinct row of list L's entries S (nothing when L.E = 0): each 256-entry chunk adds its entries left to

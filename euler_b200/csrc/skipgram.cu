@@ -17,6 +17,9 @@
 //   loss = mean over the B J logits of max(x, 0) - x z + log1p(exp(-|x|)) (z = 1 for j < P): each term in f32, each row's
 //     terms added in j order in f64, the rows added in a fixed order in f64 (k_f64_mean), one division, rounded to f32.
 // An id outside [0, n_rows) is read as row 0 and flagged; the call returns EU_ERR_INVALID after its one synchronisation.
+// Tables are f32 or bf16 (T, an eu_feat_dtype): a bf16 element is widened exactly to f32 as it is read and every other step
+// is the f32 one, so a bf16 call gives the f32 call's bits on the widened tables.  The 4-wide loads (VEC) need dim % 4 == 0
+// and each table aligned to four elements (16 bytes of f32, 8 of bf16); the scalar path sums in the same order.
 //
 // Backward, with g the upstream gradient (a device scalar) and N = B J: gN = g / fl(N) once, and per logit
 //   c_bj = -gN / (1 + exp(x))  (j < P: (sigmoid(x) - 1) gN)      c_bj = gN / (1 + exp(-x))  (j >= P: sigmoid(x) gN).
@@ -61,10 +64,10 @@ __device__ __forceinline__ float sg_xent(float x, bool positive) {
 
 // G lanes per pair row b: the target row's first kSgRegs chunks of this lane in registers, kSgRows context rows in flight.
 // Lane 0 writes the logits; after them the group counts the rank and lane 0 adds the row's loss terms.
-template <bool VEC>
+template <bool VEC, typename T>
 __global__ void __launch_bounds__(256) k_sg_fwd(const int64_t* __restrict__ src, const int64_t* __restrict__ pos,
                                                 const int64_t* __restrict__ negs, int64_t B, int P, int K,
-                                                const float* __restrict__ target, const float* __restrict__ context, int64_t n_rows,
+                                                const T* __restrict__ target, const T* __restrict__ context, int64_t n_rows,
                                                 int dim, int G, float* logits, int32_t* __restrict__ rank,
                                                 double* __restrict__ rowloss, int* bad) {
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -74,7 +77,7 @@ __global__ void __launch_bounds__(256) k_sg_fwd(const int64_t* __restrict__ src,
   const unsigned gm = group_mask(G);
   const int J = P + K;
   const int nck = ((dim + 3) / 4 + G - 1) / G;   // chunks of the lane with the most
-  const float* tr = target + row_of(__ldg(src + b), n_rows, bad) * dim;
+  const T* tr = target + row_of(__ldg(src + b), n_rows, bad) * dim;
   float4 treg[kSgRegs];
 #pragma unroll
   for (int i = 0; i < kSgRegs; ++i) {
@@ -83,7 +86,7 @@ __global__ void __launch_bounds__(256) k_sg_fwd(const int64_t* __restrict__ src,
   }
   float* lrow = logits + b * J;
   for (int j0 = 0; j0 < J; j0 += kSgRows) {
-    const float* cr[kSgRows];
+    const T* cr[kSgRows];
 #pragma unroll
     for (int u = 0; u < kSgRows; ++u)
       cr[u] = j0 + u < J ? context + row_of(sg_ctx_id(pos, negs, b, P, K, j0 + u), n_rows, bad) * dim : nullptr;
@@ -158,10 +161,10 @@ __global__ void k_sg_keys(const int64_t* __restrict__ src, const int64_t* __rest
 }
 
 // G lanes per pair row b: gt[b, :] = sum over j of coef[b, j] * context[ctx_bj, :], fma from +0 in j order
-template <bool VEC>
+template <bool VEC, typename T>
 __global__ void __launch_bounds__(256) k_sg_target_rows(const int64_t* __restrict__ pos, const int64_t* __restrict__ negs, int64_t B,
                                                         int P, int K, const float* __restrict__ coef,
-                                                        const float* __restrict__ context, int64_t n_rows, int dim, int G,
+                                                        const T* __restrict__ context, int64_t n_rows, int dim, int G,
                                                         float* __restrict__ gt) {
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t b = tid >> (31 - __clz(G));
@@ -202,10 +205,10 @@ __global__ void __launch_bounds__(256) k_sg_target_rows(const int64_t* __restric
 }
 
 static int sg_check(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
-                    const float* target, const float* context, int64_t n_rows, int32_t dim, const char* who) {
+                    const void* target, const void* context, int64_t n_rows, int32_t dim, int32_t dtype, const char* who) {
   if (!c || B < 0 || P < 1 || K < 0 || n_rows < 1 || dim < 1 || !target || !context ||
-      (B > 0 && (!src || !pos || (K > 0 && !negs)))) {
-    set_error("%s: bad argument (B >= 0, P >= 1, K >= 0, n_rows and dim >= 1, tables and ids given)", who);
+      (B > 0 && (!src || !pos || (K > 0 && !negs))) || (dtype != EU_FEAT_F32 && dtype != EU_FEAT_BF16)) {
+    set_error("%s: bad argument (B >= 0, P >= 1, K >= 0, n_rows and dim >= 1, tables and ids given, a known table dtype)", who);
     return EU_ERR_INVALID;
   }
   if (n_rows >= ((int64_t)1 << 31) || !entries_fit(B * ((int64_t)P + K + 1))) {   // the longest list: one shared table's
@@ -218,7 +221,7 @@ static int sg_check(eu_ctx* c, const int64_t* src, const int64_t* pos, const int
 // The backward pass both output forms share.  shared: one list into the target outputs.  sparse: the COO of
 // each list, its distinct count read back; dense: the gradient tables, zeroed first.  One synchronisation at the end.
 static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B,
-                       int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows, int32_t dim,
+                       int32_t P, int32_t K, const void* target, const void* context, int64_t n_rows, int32_t dim, int32_t dtype,
                        const float* logits, bool shared, bool sparse, float* out_t, float* out_c, int64_t* rows_t,
                        int64_t* rows_c, int64_t* n_t, int64_t* n_c, const char* who) {
   cudaStream_t s = c->stream;
@@ -263,11 +266,18 @@ static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, co
   EuProfScope ps(c, "skipgram_bwd_sums", Lt.E + Lc.E);
   k_sg_coef<<<stride_grid(N), 256, 0, s>>>(logits, grad_loss, N, P, J, coef);
   EU_LAUNCHED();
-  const bool vec = dim % 4 == 0 && aligned16(context) && aligned16(gt);
+  const bool vec = dim % 4 == 0 && aligned4_elems(context, dtype) && aligned16(gt);
   const int G = group_lanes(ceil_div(dim, 4));
   const unsigned blocks = (unsigned)ceil_div(B * G, 256);
-  if (vec) k_sg_target_rows<true><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, context, n_rows, dim, G, gt);
-  else k_sg_target_rows<false><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, context, n_rows, dim, G, gt);
+  if (dtype == EU_FEAT_BF16) {
+    const __nv_bfloat16* cx = static_cast<const __nv_bfloat16*>(context);
+    if (vec) k_sg_target_rows<true><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
+    else k_sg_target_rows<false><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
+  } else {
+    const float* cx = static_cast<const float*>(context);
+    if (vec) k_sg_target_rows<true><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
+    else k_sg_target_rows<false><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
+  }
   EU_LAUNCHED();
   RowEntries R;   // the target list: the B src entries (gt rows), then the context entries; the context list: those only
   R.n_src = B;
@@ -276,6 +286,7 @@ static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, co
   R.coef = coef;
   R.src = src;
   R.target = target;
+  R.target_dtype = dtype;
   R.n_rows = n_rows;
   if ((rc = sum_distinct_rows(c, R, Lt, dim, !sparse, out_t, rows_t))) return rc;
   R.n_src = 0;
@@ -293,17 +304,11 @@ static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, co
   return EU_OK;
 }
 
-}  // namespace eu
-
-using namespace eu;
-
-extern "C" {
-
-int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
-                     const float* target, const float* context, int64_t n_rows, int32_t dim, float* logits, int32_t* rank,
-                     float* loss) {
-  const char* who = "eu_skipgram_loss";
-  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, who);
+// the forward pass of both table types
+static int sg_forward(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
+                      const void* target, const void* context, int64_t n_rows, int32_t dim, int32_t dtype, float* logits,
+                      int32_t* rank, float* loss, const char* who) {
+  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, dtype, who);
   if (rc) return rc;
   if (!loss || (B > 0 && (!logits || !rank))) {
     set_error("%s: bad argument (logits, rank and loss are required)", who);
@@ -313,11 +318,18 @@ int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const in
   EuProfScope ps(c, "skipgram_fwd", B);
   bool h_bad = false;
   rc = mean_loss(c, B, B * (int64_t)(P + K), loss, &h_bad, [&](int* bad, double* rowloss) -> int {
-    const bool vec = dim % 4 == 0 && aligned16(target) && aligned16(context);
+    const bool vec = dim % 4 == 0 && aligned4_elems(target, dtype) && aligned4_elems(context, dtype);
     const int G = group_lanes(ceil_div(dim, 4));   // one lane per 4-column chunk, both paths: the same order
     const unsigned blocks = (unsigned)ceil_div(B * G, 256);
-    if (vec) k_sg_fwd<true><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
-    else k_sg_fwd<false><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, target, context, n_rows, dim, G, logits, rank, rowloss, bad);
+    if (dtype == EU_FEAT_BF16) {
+      const __nv_bfloat16 *t = static_cast<const __nv_bfloat16*>(target), *cx = static_cast<const __nv_bfloat16*>(context);
+      if (vec) k_sg_fwd<true><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
+      else k_sg_fwd<false><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
+    } else {
+      const float *t = static_cast<const float*>(target), *cx = static_cast<const float*>(context);
+      if (vec) k_sg_fwd<true><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
+      else k_sg_fwd<false><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
+    }
     EU_LAUNCHED();
     return EU_OK;
   });
@@ -329,26 +341,25 @@ int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const in
   return EU_OK;
 }
 
-int eu_skipgram_loss_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
-                              int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
-                              int32_t dim, const float* logits, float* grad_target, float* grad_context) {
-  const char* who = "eu_skipgram_loss_backward";
-  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, who);
+static int sg_backward_dense(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                             int64_t B, int32_t P, int32_t K, const void* target, const void* context, int64_t n_rows,
+                             int32_t dim, int32_t dtype, const float* logits, float* grad_target, float* grad_context,
+                             const char* who) {
+  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, dtype, who);
   if (rc) return rc;
   if (!grad_loss || !grad_target || !grad_context || (B > 0 && !logits)) {
     set_error("%s: bad argument (grad_loss, logits and both gradient tables are required)", who);
     return EU_ERR_INVALID;
   }
-  return sg_backward(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, logits, grad_target == grad_context, false,
-                     grad_target, grad_context, nullptr, nullptr, nullptr, nullptr, who);
+  return sg_backward(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, dtype, logits, grad_target == grad_context,
+                     false, grad_target, grad_context, nullptr, nullptr, nullptr, nullptr, who);
 }
 
-int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
-                                     int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
-                                     int32_t dim, const float* logits, int64_t* rows_target, float* values_target,
-                                     int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context) {
-  const char* who = "eu_skipgram_loss_backward_sparse";
-  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, who);
+static int sg_backward_sparse(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                              int64_t B, int32_t P, int32_t K, const void* target, const void* context, int64_t n_rows,
+                              int32_t dim, int32_t dtype, const float* logits, int64_t* rows_target, float* values_target,
+                              int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context, const char* who) {
+  int rc = sg_check(c, src, pos, negs, B, P, K, target, context, n_rows, dim, dtype, who);
   if (rc) return rc;
   const bool shared = !rows_context;
   if (!grad_loss || !n_target || (B > 0 && (!logits || !rows_target || !values_target)) ||
@@ -356,8 +367,60 @@ int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const in
     set_error("%s: bad argument", who);
     return EU_ERR_INVALID;
   }
-  return sg_backward(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, logits, shared, true, values_target,
+  return sg_backward(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, dtype, logits, shared, true, values_target,
                      values_context, rows_target, rows_context, n_target, n_context, who);
+}
+
+}  // namespace eu
+
+using namespace eu;
+
+extern "C" {
+
+int eu_skipgram_loss(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
+                     const float* target, const float* context, int64_t n_rows, int32_t dim, float* logits, int32_t* rank,
+                     float* loss) {
+  return sg_forward(c, src, pos, negs, B, P, K, target, context, n_rows, dim, EU_FEAT_F32, logits, rank, loss, "eu_skipgram_loss");
+}
+
+int eu_skipgram_loss_dtype(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
+                           const void* target, const void* context, int64_t n_rows, int32_t dim, int32_t table_dtype,
+                           float* logits, int32_t* rank, float* loss) {
+  return sg_forward(c, src, pos, negs, B, P, K, target, context, n_rows, dim, table_dtype, logits, rank, loss,
+                    "eu_skipgram_loss_dtype");
+}
+
+int eu_skipgram_loss_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                              int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
+                              int32_t dim, const float* logits, float* grad_target, float* grad_context) {
+  return sg_backward_dense(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, EU_FEAT_F32, logits, grad_target,
+                           grad_context, "eu_skipgram_loss_backward");
+}
+
+int eu_skipgram_loss_backward_dtype(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                                    int64_t B, int32_t P, int32_t K, const void* target, const void* context, int64_t n_rows,
+                                    int32_t dim, int32_t table_dtype, const float* logits, float* grad_target,
+                                    float* grad_context) {
+  return sg_backward_dense(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, table_dtype, logits, grad_target,
+                           grad_context, "eu_skipgram_loss_backward_dtype");
+}
+
+int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                                     int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
+                                     int32_t dim, const float* logits, int64_t* rows_target, float* values_target,
+                                     int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context) {
+  return sg_backward_sparse(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, EU_FEAT_F32, logits, rows_target,
+                            values_target, n_target, rows_context, values_context, n_context, "eu_skipgram_loss_backward_sparse");
+}
+
+int eu_skipgram_loss_backward_sparse_dtype(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos,
+                                           const int64_t* negs, int64_t B, int32_t P, int32_t K, const void* target,
+                                           const void* context, int64_t n_rows, int32_t dim, int32_t table_dtype,
+                                           const float* logits, int64_t* rows_target, float* values_target, int64_t* n_target,
+                                           int64_t* rows_context, float* values_context, int64_t* n_context) {
+  return sg_backward_sparse(c, grad_loss, src, pos, negs, B, P, K, target, context, n_rows, dim, table_dtype, logits, rows_target,
+                            values_target, n_target, rows_context, values_context, n_context,
+                            "eu_skipgram_loss_backward_sparse_dtype");
 }
 
 }  // extern "C"

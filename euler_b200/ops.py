@@ -1586,16 +1586,43 @@ def skipgram_metric(rank, name):
     raise EulerError("skipgram metric must be one of %s, got %r" % (SKIPGRAM_METRICS, name))
 
 
+# the storage types of the skip-gram step's tables (eu_feat_dtype)
+_TABLE_DTYPES = {torch.float32: 0, torch.bfloat16: 1}
+
+
 def _raw_skipgram(src, pos, negs, target, context):
-    """one eu_skipgram_loss: (logits f32[B, P + K], rank i32[B], loss f32[])"""
+    """one eu_skipgram_loss (eu_skipgram_loss_dtype for bf16 tables): (logits f32[B, P + K], rank i32[B], loss f32[])"""
     B, P = pos.shape
     K = negs.shape[1]
     n_rows, dim = target.shape
     logits = torch.empty((B, P + K), dtype=torch.float32, device=target.device)
     rank = torch.empty(B, dtype=torch.int32, device=target.device)
     loss = torch.empty((), dtype=torch.float32, device=target.device)
-    _call("eu_skipgram_loss", src, pos, negs, B, P, K, target, context, n_rows, dim, logits, rank, loss)
+    if target.dtype == torch.bfloat16:
+        _call("eu_skipgram_loss_dtype", src, pos, negs, B, P, K, target, context, n_rows, dim, 1, logits, rank, loss)
+    else:
+        _call("eu_skipgram_loss", src, pos, negs, B, P, K, target, context, n_rows, dim, logits, rank, loss)
     return logits, rank, loss
+
+
+def _raw_skipgram_sparse_grads(src, pos, negs, target, context, logits, g, shared):
+    """one eu_skipgram_loss_backward_sparse(_dtype): [(rows i64[D], values f32[D, dim])] of the target table and, unless
+    shared, of the context table, coalesced; g is the loss's upstream gradient (a device f32[1])"""
+    B, P = pos.shape
+    K = negs.shape[1]
+    n_rows, dim = target.shape
+    shape_t, shape_c = (n_rows, dim), None if shared else (n_rows, dim)
+    rows_t, vals_t = _coo_buffers(B * (P + K + 1) if shared else B, shape_t, target.device)
+    rows_c, vals_c = _coo_buffers(B * (P + K), shape_c, target.device)
+    n_t, n_c = C.c_int64(), C.c_int64()
+    args = (g, src, pos, negs, B, P, K, target, context, n_rows, dim)
+    outs = (logits, rows_t, vals_t, C.byref(n_t), rows_c, vals_c, C.byref(n_c))
+    if target.dtype == torch.bfloat16:
+        _call("eu_skipgram_loss_backward_sparse_dtype", *args, 1, *outs)
+    else:
+        _call("eu_skipgram_loss_backward_sparse", *args, *outs)
+    grads = [(rows_t[:n_t.value], vals_t[:n_t.value])]
+    return grads if shared else grads + [(rows_c[:n_c.value], vals_c[:n_c.value])]
 
 
 class _SkipgramLoss(torch.autograd.Function):
@@ -1634,6 +1661,32 @@ class _SkipgramLoss(torch.autograd.Function):
         return _coo(rows_t, vals_t, n_t.value, shape_t), _coo(rows_c, vals_c, n_c.value, shape_c), None, None, None, None, None
 
 
+def _skipgram_args(op, src, pos, negs, target, context, metric):
+    """(src [B], pos [B, P], negs [B, K], target, context, shared) on the device, or EulerError: the checks of
+    skipgram_xent_loss"""
+    if metric not in SKIPGRAM_METRICS:
+        raise EulerError("%s: metric must be one of %s, got %r" % (op, SKIPGRAM_METRICS, metric))
+    shared = context is target
+    for nm, t in (('target', target), ('context', context)):
+        if not torch.is_tensor(t) or t.dtype not in _TABLE_DTYPES or t.dim() != 2:
+            raise EulerError("%s: %s must be a 2-D float32 or bfloat16 tensor" % (op, nm))
+    if target.dtype != context.dtype:
+        raise EulerError("%s: target (%s) and context (%s) must have one dtype" % (op, target.dtype, context.dtype))
+    if target.shape != context.shape:
+        raise EulerError("%s: target %s and context %s must have one shape" % (op, tuple(target.shape), tuple(context.shape)))
+    src = _t(src, torch.int64).reshape(-1)
+    B = src.numel()
+    pos, negs = _t(pos, torch.int64), _t(negs, torch.int64)
+    if pos.dim() == 1:
+        pos = pos.unsqueeze(1)
+    if pos.dim() != 2 or negs.dim() != 2 or pos.shape[0] != B or negs.shape[0] != B or pos.shape[1] < 1:
+        raise EulerError("%s: pos must be [B, P >= 1] and negs [B, K] with B = %d, got %s and %s"
+                         % (op, B, tuple(pos.shape), tuple(negs.shape)))
+    target = _t(target, target.dtype)
+    context = target if shared else _t(context, context.dtype)
+    return src, pos.contiguous(), negs.contiguous(), target, context, shared
+
+
 def skipgram_xent_loss(src, pos, negs, target, context, metric='mrr', sparse_grad=False):
     """The skip-gram step of UnsuperviseModel.__call__ (mp_utils/base.py:50-91; PosNegLogits, xent_loss, utils/metrics.py) in
     one fused device op, for id embeddings:
@@ -1645,25 +1698,32 @@ def skipgram_xent_loss(src, pos, negs, target, context, metric='mrr', sparse_gra
     top_k ranks them.  Ids index the tables directly, as tf.nn.embedding_lookup does; one outside [0, n_rows) raises.
     The gradient reaches the tables only: dense f32[n_rows, dim] gradients, or, with sparse_grad=True, coalesced sparse COO
     gradients of the rows the batch touches (as nn.Embedding(sparse=True) gives).  Deterministic, no atomics; the forward and the
-    backward synchronise once each."""
-    if metric not in SKIPGRAM_METRICS:
-        raise EulerError("skipgram_xent_loss: metric must be one of %s, got %r" % (SKIPGRAM_METRICS, metric))
-    shared = context is target
-    _check_f32("skipgram_xent_loss", (('target', target), ('context', context)), 2)
-    if target.shape != context.shape:
-        raise EulerError("skipgram_xent_loss: target %s and context %s must have one shape" % (tuple(target.shape), tuple(context.shape)))
-    src = _t(src, torch.int64).reshape(-1)
-    B = src.numel()
-    pos, negs = _t(pos, torch.int64), _t(negs, torch.int64)
-    if pos.dim() == 1:
-        pos = pos.unsqueeze(1)
-    if pos.dim() != 2 or negs.dim() != 2 or pos.shape[0] != B or negs.shape[0] != B or pos.shape[1] < 1:
-        raise EulerError("skipgram_xent_loss: pos must be [B, P >= 1] and negs [B, K] with B = %d, got %s and %s"
-                         % (B, tuple(pos.shape), tuple(negs.shape)))
-    target = _t(target, torch.float32)
-    context = target if shared else _t(context, torch.float32)
-    loss, rank = _SkipgramLoss.apply(target, context, src, pos.contiguous(), negs.contiguous(), shared, bool(sparse_grad))
+    backward synchronise once each.
+    bfloat16 tables (both of one dtype) are read widened exactly to f32, so the loss and metric are the f32 op's on the widened
+    tables.  They take no gradient through autograd, which would round their f32 gradient to nearest bf16: a bf16 table that
+    requires grad raises.  Train them with skipgram_xent_loss_sparse_grads and an optimizer's apply_sparse
+    (UnsuperviseModel.train_step)."""
+    src, pos, negs, target, context, shared = _skipgram_args("skipgram_xent_loss", src, pos, negs, target, context, metric)
+    if target.dtype == torch.bfloat16 and (target.requires_grad or context.requires_grad):
+        raise EulerError("skipgram_xent_loss: a bfloat16 table takes no autograd gradient (torch would round it to bf16); "
+                         "train it with skipgram_xent_loss_sparse_grads and an optimizer's apply_sparse")
+    loss, rank = _SkipgramLoss.apply(target, context, src, pos, negs, shared, bool(sparse_grad))
     return loss, skipgram_metric(rank, metric)
+
+
+def skipgram_xent_loss_sparse_grads(src, pos, negs, target, context, metric='mrr'):
+    """skipgram_xent_loss's forward and its sparse backward for an upstream gradient of 1, without autograd, for tables of
+    float32 or bfloat16 (read widened exactly to f32).  Returns (loss, metric, grads): grads is [(rows i64[D], values
+    f32[D, dim])], the coalesced f32 gradient of the target table, then of the context table unless it is the target
+    table -- the bits skipgram_xent_loss(..., sparse_grad=True).backward() gives f32 tables holding the widened values.  They
+    go to an optimizer's apply_sparse as they are, never rounded to bf16.  Synchronises twice (the forward, the backward)."""
+    src, pos, negs, target, context, shared = _skipgram_args("skipgram_xent_loss_sparse_grads", src, pos, negs, target, context,
+                                                             metric)
+    target, context = target.detach(), context.detach()
+    logits, rank, loss = _raw_skipgram(src, pos, negs, target, context)
+    g = torch.ones(1, dtype=torch.float32, device=target.device)
+    grads = _raw_skipgram_sparse_grads(src, pos, negs, target, context, logits, g, shared)
+    return loss, skipgram_metric(rank, metric), grads
 
 
 # ------------------------------------------------------------------------------------ graph auto-encoder step
@@ -1815,11 +1875,13 @@ def _optim_args(op, var, slots, grad):
     """the library's (N, D, values, rows, R) for one update of var and its slots (same shape, float32, contiguous, on the
     graph's device): a dense grad of var's shape is taken as f32[N, D] over var's elements; a sparse COO grad of var's shape
     with one sparse dimension (coalesced here when it is not) as its rows i64[R] and values f32[R, D], D the elements of a row
-    of var.  Raises EulerError before any device work."""
+    of var.  var and its slots may instead all be bfloat16 (the gradient stays float32).  Raises EulerError before any
+    device work."""
     dev = _dev()
+    dt = var.dtype if torch.is_tensor(var) and var.dtype == torch.bfloat16 else torch.float32
     for nm, t in (('var', var),) + slots:
-        if not torch.is_tensor(t) or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous() or t.is_sparse:
-            raise EulerError("%s: %s must be a contiguous float32 tensor on %s" % (op, nm, dev))
+        if not torch.is_tensor(t) or t.dtype != dt or t.device != dev or not t.is_contiguous() or t.is_sparse:
+            raise EulerError("%s: %s must be a contiguous %s tensor on %s" % (op, nm, dt, dev))
         if t.shape != var.shape:
             raise EulerError("%s: %s has shape %s, var %s" % (op, nm, tuple(t.shape), tuple(var.shape)))
     if not torch.is_tensor(grad) or grad.dtype != torch.float32 or grad.device != dev or grad.shape != var.shape:
@@ -1839,38 +1901,65 @@ def _optim_args(op, var, slots, grad):
     return N, D, grad._values().reshape(rows.numel(), D).contiguous(), rows, rows.numel()
 
 
-def optim_momentum_(var, accum, grad, lr, momentum):
+def _sr_args(op, var, seed, step, tensor):
+    """the trailing (dtype, seed, step, tensor) of an eu_optim_*_dtype call: step must be an int64 device scalar for bf16"""
+    if var.dtype != torch.bfloat16:
+        return 0, 0, None, 0
+    _metric_tensors(op, [('step', step, torch.int64, ())], var.device)
+    if not 0 <= int(seed) < 2 ** 64 or not 0 <= int(tensor) < 2 ** 31:
+        raise EulerError("%s: seed must lie in [0, 2^64) and tensor in [0, 2^31), got %r and %r" % (op, seed, tensor))
+    return 1, int(seed), step, int(tensor)
+
+
+def optim_momentum_(var, accum, grad, lr, momentum, seed=0, step=None, tensor=0):
     """One step of TF 1.x MomentumOptimizer (non-Nesterov) on var in place, no autograd: accum = accum * momentum + g,
     var = var - lr * accum, each op one f32 rounding.  A dense grad updates every element (apply_momentum); a sparse COO grad
     (sparse_apply_momentum) only its rows, after coalesce() when it is not coalesced.  var, accum: contiguous float32 of one
     shape on the graph's device.  No host synchronisation for a dense or coalesced grad (include/euler_b200.h,
-    eu_optim_momentum); shape, dtype and device mismatches raise EulerError and write nothing.  Returns var."""
-    N, D, g, rows, R = _optim_args("optim_momentum_", var, (('accum', accum),), grad)
-    _call("eu_optim_momentum", var, accum, N, D, g, rows, R, float(lr), float(momentum))
+    eu_optim_momentum); shape, dtype and device mismatches raise EulerError and write nothing.  Returns var.
+    var and accum may both be bfloat16 (grad stays float32): each value is widened exactly, updated in f32, and written back
+    by stochastic rounding keyed by (seed, step, tensor, element), step an int64 device scalar the caller advances once per
+    step (include/euler_b200.h, eu_optim_momentum_dtype)."""
+    op = "optim_momentum_"
+    N, D, g, rows, R = _optim_args(op, var, (('accum', accum),), grad)
+    if var.dtype == torch.bfloat16:
+        _call("eu_optim_momentum_dtype", var, accum, N, D, g, rows, R, float(lr), float(momentum), *_sr_args(op, var, seed, step, tensor))
+    else:
+        _call("eu_optim_momentum", var, accum, N, D, g, rows, R, float(lr), float(momentum))
     return var
 
 
-def optim_adagrad_(var, accum, grad, lr):
+def optim_adagrad_(var, accum, grad, lr, seed=0, step=None, tensor=0):
     """One step of TF 1.x AdagradOptimizer on var in place, no autograd: accum = accum + g * g, var = var - (lr * g) *
     (1 / sqrt(accum)), each op one f32 rounding.  Dense grads update every element (apply_adagrad), sparse COO grads their
-    rows only (sparse_apply_adagrad), as optim_momentum_ (include/euler_b200.h, eu_optim_adagrad).  Returns var."""
-    N, D, g, rows, R = _optim_args("optim_adagrad_", var, (('accum', accum),), grad)
-    _call("eu_optim_adagrad", var, accum, N, D, g, rows, R, float(lr))
+    rows only (sparse_apply_adagrad), as optim_momentum_ (include/euler_b200.h, eu_optim_adagrad).  Returns var.  bfloat16
+    var and accum as optim_momentum_."""
+    op = "optim_adagrad_"
+    N, D, g, rows, R = _optim_args(op, var, (('accum', accum),), grad)
+    if var.dtype == torch.bfloat16:
+        _call("eu_optim_adagrad_dtype", var, accum, N, D, g, rows, R, float(lr), *_sr_args(op, var, seed, step, tensor))
+    else:
+        _call("eu_optim_adagrad", var, accum, N, D, g, rows, R, float(lr))
     return var
 
 
-def optim_adam_(var, m, v, grad, powers, lr, beta1, beta2, epsilon):
+def optim_adam_(var, m, v, grad, powers, lr, beta1, beta2, epsilon, seed=0, step=None, tensor=0):
     """One step of TF 1.x AdamOptimizer on var in place, no autograd, with alpha = (lr * sqrt(1 - powers[1])) /
     (1 - powers[0]) computed on the device from powers (float32[2]: beta1_power, beta2_power, on var's device).  A dense grad
     runs ApplyAdam: m = m + (g - m) * (1 - b1), v = v + (g * g - v) * (1 - b2), var = var - (m * alpha) / (sqrt(v) + eps).  A
     sparse COO grad (coalesced first when it is not) runs _apply_sparse_shared over EVERY row: m = m * b1 and v = v * b2, plus
     g * (1 - b1) and (g * g) * (1 - b2) on the grad's rows, then var = var - (alpha * m) / (sqrt(v) + eps).  Each op is one f32
     rounding.  The powers are not advanced here: the caller multiplies each by its beta once per step, after every variable
-    (TF's _finish).  Checks and synchronisation as optim_momentum_ (include/euler_b200.h, eu_optim_adam).  Returns var."""
+    (TF's _finish).  Checks and synchronisation as optim_momentum_ (include/euler_b200.h, eu_optim_adam).  Returns var.
+    bfloat16 var, m and v as optim_momentum_; a sparse step rounds every row it writes."""
     op = "optim_adam_"
     N, D, g, rows, R = _optim_args(op, var, (('m', m), ('v', v)), grad)
     _metric_tensors(op, [('powers', powers, torch.float32, (2,))], var.device)
-    _call("eu_optim_adam", var, m, v, N, D, g, rows, R, powers, float(lr), float(beta1), float(beta2), float(epsilon))
+    hp = (float(lr), float(beta1), float(beta2), float(epsilon))
+    if var.dtype == torch.bfloat16:
+        _call("eu_optim_adam_dtype", var, m, v, N, D, g, rows, R, powers, *hp, *_sr_args(op, var, seed, step, tensor))
+    else:
+        _call("eu_optim_adam", var, m, v, N, D, g, rows, R, powers, *hp)
     return var
 
 

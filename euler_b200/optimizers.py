@@ -22,6 +22,14 @@ With fused=True (the default) each parameter's update is one device op (ops.opti
 that reads and writes each tensor once and never synchronises with the host, so a step can be captured in a CUDA graph.
 With fused=False the step runs TF's op sequence literally in torch, one torch op per TF op, on any device: the reference the
 fused ops are checked against.
+
+bfloat16 parameters (the skip-gram id tables of unsupervised.UnsuperviseModel(table_dtype=torch.bfloat16)) are trained by the
+fused ops only, with slots of the parameter's dtype.  Each value is widened exactly to f32 and updated in f32, and the var and
+every slot are written back by stochastic rounding keyed by (seed, the optimizer's step counter, the parameter's index in the
+optimizer, the element): one seed gives the same bits on every run.  The step counter (`sr_step`, int64 on the first bf16
+parameter's device) advances once per step, after every parameter, as Adam's powers do; state_dict() saves it.  Torch
+autograd would round a bf16 leaf's f32 gradient to nearest bf16, so a bf16 parameter takes its gradient through
+apply_sparse(param, rows, values) from f32 rows and values, never through .grad.  fused=False refuses bf16 parameters.
 """
 import math
 
@@ -64,9 +72,41 @@ def _rows(grad):
 
 
 class _TFOptimizer(torch.optim.Optimizer):
-    def __init__(self, params, defaults, fused):
+    def __init__(self, params, defaults, fused, seed):
+        self.fused = bool(fused)   # add_param_group reads it
+        if not isinstance(seed, int) or isinstance(seed, bool) or not 0 <= seed < 2 ** 64:
+            raise ValueError("seed must be an int in [0, 2^64), got %r" % (seed,))
+        self.seed = seed
+        self.sr_step = None   # the stochastic-rounding step counter, made with the first bf16 parameter
         super().__init__(params, defaults)
-        self.fused = bool(fused)
+
+    def add_param_group(self, param_group):
+        super().add_param_group(param_group)
+        bf16 = [p for p in self.param_groups[-1]['params'] if p.dtype == torch.bfloat16]
+        if bf16 and not self.fused:
+            self.param_groups.pop()
+            raise ValueError("a bfloat16 parameter is trained by the fused update only (fused=True)")
+        if bf16 and self.sr_step is None:
+            self.sr_step = torch.zeros((), dtype=torch.int64, device=bf16[0].device)
+
+    def _each(self):
+        """(index, param, group) of every parameter, in the order the parameters were given"""
+        i = 0
+        for group in self.param_groups:
+            for p in group['params']:
+                yield i, p, group
+                i += 1
+
+    def _update(self, i, p, grad, group):
+        state = self.state[p]
+        if not state:
+            self._init_state(p, state, group)
+        if self.fused:
+            self._fused(p, grad, state, group, dict(seed=self.seed, step=self.sr_step, tensor=i))
+        elif grad.is_sparse:
+            self._literal_sparse(p, *_rows(grad), state, group)
+        else:
+            self._literal_dense(p, grad, state, group)
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -74,40 +114,66 @@ class _TFOptimizer(torch.optim.Optimizer):
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        for group in self.param_groups:
-            for p in group['params']:
-                if p.grad is None:
-                    continue
-                state = self.state[p]
-                if not state:
-                    self._init_state(p, state, group)
-                if self.fused:
-                    self._fused(p, p.grad, state, group)
-                elif p.grad.is_sparse:
-                    self._literal_sparse(p, *_rows(p.grad), state, group)
-                else:
-                    self._literal_dense(p, p.grad, state, group)
+        for i, p, group in self._each():
+            if p.grad is not None:
+                self._update(i, p, p.grad, group)
         self._finish()
         return loss
 
+    @torch.no_grad()
+    def apply_sparse(self, param, rows, values):
+        """One step from sparse f32 gradients, without .grad: param, rows and values are one parameter, its rows i64[R]
+        (sorted and unique, as a coalesced gradient has them) and values f32[R, ...] of the parameter's row shape, or lists
+        of equal length with one entry per parameter.  The parameters not listed take no update this step, as a None .grad
+        in step().  The values are never rounded to the parameter's dtype: this is how a bfloat16 parameter is trained."""
+        if torch.is_tensor(param):
+            param, rows, values = [param], [rows], [values]
+        if not len(param) == len(rows) == len(values):
+            raise ValueError("apply_sparse: param, rows and values must have one length")
+        index = {id(p): (i, g) for i, p, g in self._each()}
+        for p in param:
+            if id(p) not in index:
+                raise ValueError("apply_sparse: a parameter is not one of this optimizer's")
+        for p, r, v in zip(param, rows, values):
+            if not torch.is_tensor(v) or v.dtype != torch.float32:
+                raise ValueError("apply_sparse: values must be float32, got %s" % getattr(v, 'dtype', type(v)))
+            i, group = index[id(p)]
+            grad = torch.sparse_coo_tensor(r.reshape(1, -1), v, tuple(p.shape), is_coalesced=True, check_invariants=False)
+            self._update(i, p, grad, group)
+        self._finish()
+
     def _finish(self):
-        pass
+        if self.sr_step is not None:
+            self.sr_step.add_(1)
+
+    def state_dict(self):
+        sd = super().state_dict()
+        if self.sr_step is not None:
+            sd['sr_step'] = self.sr_step.clone()
+        return sd
+
+    def load_state_dict(self, state_dict):
+        sd = dict(state_dict)
+        step = sd.pop('sr_step', None)
+        super().load_state_dict(sd)
+        if step is not None and self.sr_step is not None:
+            self.sr_step.copy_(step)
 
 
 class MomentumOptimizer(_TFOptimizer):
     """tf.train.MomentumOptimizer(learning_rate, momentum), non-Nesterov: accum = accum * momentum + g, var = var - lr *
     accum.  A sparse gradient updates its rows only.  Slot: state['momentum'], starting at zeros."""
 
-    def __init__(self, params, learning_rate, momentum, fused=True):
+    def __init__(self, params, learning_rate, momentum, fused=True, seed=0):
         _check("learning_rate", learning_rate, _finite_nonneg, "a finite number >= 0")
         _check("momentum", momentum, _finite_nonneg, "a finite number >= 0")
-        super().__init__(params, dict(lr=learning_rate, momentum=momentum), fused)
+        super().__init__(params, dict(lr=learning_rate, momentum=momentum), fused, seed)
 
     def _init_state(self, p, state, group):
         state['momentum'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
 
-    def _fused(self, p, grad, state, group):
-        ops.optim_momentum_(p, state['momentum'], grad, group['lr'], group['momentum'])
+    def _fused(self, p, grad, state, group, sr):
+        ops.optim_momentum_(p, state['momentum'], grad, group['lr'], group['momentum'], **sr)
 
     def _literal_dense(self, p, g, state, group):
         a = state['momentum']
@@ -125,18 +191,18 @@ class AdagradOptimizer(_TFOptimizer):
     """tf.train.AdagradOptimizer(learning_rate, initial_accumulator_value=0.1): accum = accum + g * g, var = var - (lr * g)
     * (1 / sqrt(accum)).  A sparse gradient updates its rows only.  Slot: state['accumulator']."""
 
-    def __init__(self, params, learning_rate, initial_accumulator_value=0.1, fused=True):
+    def __init__(self, params, learning_rate, initial_accumulator_value=0.1, fused=True, seed=0):
         _check("learning_rate", learning_rate, _finite_nonneg, "a finite number >= 0")
         _check("initial_accumulator_value", initial_accumulator_value, lambda x: math.isfinite(x) and x > 0,
                "a finite number > 0")
-        super().__init__(params, dict(lr=learning_rate, initial_accumulator_value=initial_accumulator_value), fused)
+        super().__init__(params, dict(lr=learning_rate, initial_accumulator_value=initial_accumulator_value), fused, seed)
 
     def _init_state(self, p, state, group):
         state['accumulator'] = torch.full_like(p, _f32(group['initial_accumulator_value']),
                                                memory_format=torch.contiguous_format)
 
-    def _fused(self, p, grad, state, group):
-        ops.optim_adagrad_(p, state['accumulator'], grad, group['lr'])
+    def _fused(self, p, grad, state, group, sr):
+        ops.optim_adagrad_(p, state['accumulator'], grad, group['lr'], **sr)
 
     def _literal_dense(self, p, g, state, group):
         a = state['accumulator']
@@ -158,12 +224,12 @@ class AdamOptimizer(_TFOptimizer):
     m) / (sqrt(v) + epsilon).  Slots: state['m'], state['v'], starting at zeros.  beta1 and beta2 are one per optimizer, as
     the power pair they advance (`beta_powers`, float32[2] on the first parameter's device)."""
 
-    def __init__(self, params, learning_rate=0.001, beta1=0.9, beta2=0.999, epsilon=1e-8, fused=True):
+    def __init__(self, params, learning_rate=0.001, beta1=0.9, beta2=0.999, epsilon=1e-8, fused=True, seed=0):
         _check("learning_rate", learning_rate, _finite_nonneg, "a finite number >= 0")
         for name, b in (("beta1", beta1), ("beta2", beta2)):
             _check(name, b, lambda x: 0 <= x < 1, "in [0, 1)")
         _check("epsilon", epsilon, _finite_nonneg, "a finite number >= 0")
-        super().__init__(params, dict(lr=learning_rate, beta1=beta1, beta2=beta2, epsilon=epsilon), fused)
+        super().__init__(params, dict(lr=learning_rate, beta1=beta1, beta2=beta2, epsilon=epsilon), fused, seed)
         dev = self.param_groups[0]['params'][0].device
         self.beta_powers = torch.tensor([_f32(beta1), _f32(beta2)], dtype=torch.float32, device=dev)
         self._betas = self.beta_powers.clone()
@@ -178,9 +244,9 @@ class AdamOptimizer(_TFOptimizer):
         state['m'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
         state['v'] = torch.zeros_like(p, memory_format=torch.contiguous_format)
 
-    def _fused(self, p, grad, state, group):
+    def _fused(self, p, grad, state, group, sr):
         ops.optim_adam_(p, state['m'], state['v'], grad, self.beta_powers, group['lr'], group['beta1'], group['beta2'],
-                        group['epsilon'])
+                        group['epsilon'], **sr)
 
     def _alpha(self, group):
         b1p, b2p = self.beta_powers[0], self.beta_powers[1]
@@ -202,6 +268,7 @@ class AdamOptimizer(_TFOptimizer):
 
     def _finish(self):
         self.beta_powers.mul_(self._betas)
+        super()._finish()
 
     def state_dict(self):
         sd = super().state_dict()

@@ -12,6 +12,11 @@ The encoders here are id tables, ShallowEncoder(max_id=max_id) with ids only: la
 max_id + 2 rows, so the default node max_id + 1 that random_walk and sample_neighbor pad with is a row of its own.
 Upstream's neg_condition (sample_node with an index query) is not supported.
 
+table_dtype=torch.bfloat16 stores the id tables (and, through the optimizer, their slots) in bfloat16: half the HBM.  Such
+tables take no autograd gradient (torch would round it to nearest bf16, losing most small updates); train_step(batch,
+optimizer) runs the fused forward and sparse backward and hands the f32 rows and values to the optimizer's apply_sparse,
+which writes the tables back by stochastic rounding.  It needs fused=True and one of optimizers.py's fused optimizers.
+
 DGI (examples/dgi/dgi.py) is the one model here over a GraphSAGE encoder: encoders.ShuffleSageEncoder with ShallowEncoder's
 feature inputs, a bilinear decoder against the batch's readout, and the same rank metrics (composed_metric).  The
 unsupervised GraphSage / GCN models are solution.UnsuperviseSolution over two encoders.
@@ -20,7 +25,8 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from .ops import SKIPGRAM_METRICS, gen_pair, random_walk, sample_neighbor, sample_node, skipgram_xent_loss
+from .ops import (SKIPGRAM_METRICS, gen_pair, random_walk, sample_neighbor, sample_node, skipgram_xent_loss,
+                  skipgram_xent_loss_sparse_grads)
 
 
 def _truncated_normal_(t, stddev):
@@ -33,9 +39,13 @@ class Embedding(torch.nn.Module):
     """layers.Embedding(max_id, dim) (utils/layers.py:119-149): a table f32[max_id + 1, dim] initialised truncated-normal with
     stddev 0.1; forward(ids) = tf.nn.embedding_lookup, shape ids.shape + (dim,)."""
 
-    def __init__(self, max_id, dim, device=None):
+    def __init__(self, max_id, dim, device=None, dtype=torch.float32):
         super().__init__()
-        self.embeddings = torch.nn.Parameter(_truncated_normal_(torch.empty(max_id + 1, dim, device=device), 0.1))
+        table = _truncated_normal_(torch.empty(max_id + 1, dim, device=device), 0.1)
+        if dtype == torch.float32:
+            self.embeddings = torch.nn.Parameter(table)
+        else:   # initialised in f32, rounded once to nearest; trained without autograd (UnsuperviseModel.train_step)
+            self.embeddings = torch.nn.Parameter(table.to(dtype), requires_grad=False)
 
     def forward(self, ids):
         return F.embedding(ids, self.embeddings)
@@ -79,18 +89,24 @@ def composed_skipgram_loss(emb, pos_emb, neg_emb, metric='mrr'):
 class UnsuperviseModel(torch.nn.Module):
     """UnsuperviseModel(node_type, edge_type, max_id, num_negs=20, metric_name='mrr') with id-table encoders of dim columns.
     to_sample: src = inputs, one positive from sample_neighbor(inputs, edge_type, 1, max_id + 1), num_negs negatives per row
-    from sample_node.  share_context: the context encoder is the target encoder (LINE's first order)."""
+    from sample_node.  share_context: the context encoder is the target encoder (LINE's first order).  table_dtype: float32, or
+    bfloat16 (fused only), trained by train_step."""
 
     def __init__(self, node_type, edge_type, max_id, dim, num_negs=20, metric_name='mrr', fused=True, sparse_grad=False,
-                 share_context=False, device=None):
+                 share_context=False, device=None, table_dtype=torch.float32):
         super().__init__()
         if metric_name not in SKIPGRAM_METRICS:
             raise ValueError("metric_name must be one of %s, got %r" % (SKIPGRAM_METRICS, metric_name))
+        if table_dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError("table_dtype must be torch.float32 or torch.bfloat16, got %r" % (table_dtype,))
+        if table_dtype == torch.bfloat16 and not fused:
+            raise ValueError("table_dtype=torch.bfloat16 needs fused=True: the composed step trains through autograd")
         self.node_type, self.edge_type, self.max_id = node_type, edge_type, max_id
         self.num_negs, self.metric_name = num_negs, metric_name
-        self.fused, self.sparse_grad = fused, sparse_grad
-        self.target_encoder = Embedding(max_id + 1, dim, device=device)
-        self.context_encoder = self.target_encoder if share_context else Embedding(max_id + 1, dim, device=device)
+        self.fused, self.sparse_grad, self.table_dtype = fused, sparse_grad, table_dtype
+        self.target_encoder = Embedding(max_id + 1, dim, device=device, dtype=table_dtype)
+        self.context_encoder = (self.target_encoder if share_context
+                                else Embedding(max_id + 1, dim, device=device, dtype=table_dtype))
 
     def embed(self, ids):
         return self.target_encoder(ids)
@@ -120,6 +136,22 @@ class UnsuperviseModel(torch.nn.Module):
         src, pos, negs = self.to_sample(inputs)
         loss, metric = self.loss_and_metric(src, pos, negs)
         return self.embed(inputs), loss, self.metric_name, metric
+
+    def train_step(self, batch, optimizer):
+        """One training step on the node ids `batch` without autograd: to_sample, the fused forward and sparse backward
+        (ops.skipgram_xent_loss_sparse_grads), then optimizer.apply_sparse with the tables' f32 rows and values.  The way to
+        train bf16 tables; f32 tables take the same step.  optimizer is one of optimizers.py's, fused, over these tables.
+        Returns (loss, metric)."""
+        if not self.fused:
+            raise ValueError("train_step runs the fused step: build the model with fused=True")
+        if not hasattr(optimizer, 'apply_sparse'):
+            raise ValueError("train_step needs one of euler_b200.optimizers' optimizers, got %s" % type(optimizer).__name__)
+        src, pos, negs = self.to_sample(batch)
+        target, context = self.target_encoder.embeddings, self.context_encoder.embeddings
+        loss, metric, grads = skipgram_xent_loss_sparse_grads(src, pos, negs, target, context, metric=self.metric_name)
+        tables = [target] if context is target else [target, context]
+        optimizer.apply_sparse(tables, [r for r, _ in grads], [v for _, v in grads])
+        return loss, metric
 
 
 def pairs_per_walk(walk_len, left_win_size, right_win_size):

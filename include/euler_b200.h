@@ -540,6 +540,23 @@ int eu_skipgram_loss_backward_sparse(eu_ctx* c, const float* grad_loss, const in
                                      int64_t B, int32_t P, int32_t K, const float* target, const float* context, int64_t n_rows,
                                      int32_t dim, const float* logits, int64_t* rows_target, float* values_target,
                                      int64_t* n_target, int64_t* rows_context, float* values_context, int64_t* n_context);
+/* The same three with the tables' storage type table_dtype (eu_feat_dtype; both tables have it).  Two rules make a bf16
+ * call exact: every read widens a bf16 element to f32 exactly, and all arithmetic stays f32 in the order above.  So a
+ * EU_FEAT_BF16 call gives bit for bit what the f32 call gives on the tables widened to f32; logits, rank, loss and the
+ * gradients stay f32.  The 4-wide loads need dim % 4 == 0 and the tables 8-byte aligned (bf16) or 16-byte aligned (f32);
+ * other tables take scalar loads with the same bits.  An unknown table_dtype: EU_ERR_INVALID. */
+int eu_skipgram_loss_dtype(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
+                           const void* target, const void* context, int64_t n_rows, int32_t dim, int32_t table_dtype,
+                           float* logits, int32_t* rank, float* loss);
+int eu_skipgram_loss_backward_dtype(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos, const int64_t* negs,
+                                    int64_t B, int32_t P, int32_t K, const void* target, const void* context, int64_t n_rows,
+                                    int32_t dim, int32_t table_dtype, const float* logits, float* grad_target,
+                                    float* grad_context);
+int eu_skipgram_loss_backward_sparse_dtype(eu_ctx* c, const float* grad_loss, const int64_t* src, const int64_t* pos,
+                                           const int64_t* negs, int64_t B, int32_t P, int32_t K, const void* target,
+                                           const void* context, int64_t n_rows, int32_t dim, int32_t table_dtype,
+                                           const float* logits, int64_t* rows_target, float* values_target, int64_t* n_target,
+                                           int64_t* rows_context, float* values_context, int64_t* n_context);
 
 /* The reconstruction step of the graph auto-encoders GAE and VGAE (tf_euler/python/mp_utils/base_gae.py, examples/gae/gae.py),
  * fused, over encoder rows.  Three sets of f32 row-major device rows, each 4-byte aligned (16-byte alignment and D % 4 == 0
@@ -630,6 +647,27 @@ int eu_optim_adagrad(eu_ctx* c, float* var, float* accum, int64_t N, int32_t D, 
                      int64_t R, float lr);
 int eu_optim_adam(eu_ctx* c, float* var, float* m, float* v, int64_t N, int32_t D, const float* grad, const int64_t* rows,
                   int64_t R, const float* powers, float lr, float beta1, float beta2, float epsilon);
+/* The same three over var and slots of storage type dtype (eu_feat_dtype; the gradient stays f32).  EU_FEAT_F32 is the call
+ * above (seed, step and tensor unused).  EU_FEAT_BF16 keeps the skip-gram tables' two rules -- every read widens bf16 to f32
+ * exactly, all arithmetic stays f32 in the order above -- so the only new rounding is the store: each value written (var
+ * and every slot) is rounded to bf16 by stochastic rounding.  A 16-bit random integer r is added to the low half of the f32
+ * bits, which are then truncated: the value rounds up with probability (distance to the bf16 below) / ulp, so a small update
+ * survives on average where round to nearest would drop every update below half an ulp.  +-Inf stays; a NaN stays a NaN
+ * (its sign and upper payload kept, made quiet).  r is the low 16 bits of word w (0 var, 1 accum or m, 2 v) of the
+ * Philox4x32-10 block with key seed and counter (element lo, element hi, *step mod 2^32, tensor): element is the flat index
+ * into var (row r, column d: r D + d, for dense and sparse gradients alike), step a device i64 counter the caller advances
+ * once per step after every variable (as Adam's powers; read on the device, so a step can be captured in a CUDA graph), and
+ * tensor the variable's index among those the caller updates with one seed.  Sparse Adam rounds every row it writes, the
+ * decay-only rows included.  The 4-wide form needs D % 4 == 0, var and slots 8-byte aligned and grad 16-byte aligned.  An
+ * unknown dtype, or EU_FEAT_BF16 without step: EU_ERR_INVALID, before any device work. */
+int eu_optim_momentum_dtype(eu_ctx* c, void* var, void* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                            int64_t R, float lr, float momentum, int32_t dtype, uint64_t seed, const int64_t* step,
+                            int32_t tensor);
+int eu_optim_adagrad_dtype(eu_ctx* c, void* var, void* accum, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                           int64_t R, float lr, int32_t dtype, uint64_t seed, const int64_t* step, int32_t tensor);
+int eu_optim_adam_dtype(eu_ctx* c, void* var, void* m, void* v, int64_t N, int32_t D, const float* grad, const int64_t* rows,
+                        int64_t R, const float* powers, float lr, float beta1, float beta2, float epsilon, int32_t dtype,
+                        uint64_t seed, const int64_t* step, int32_t tensor);
 
 /* The knowledge-graph embedding step of TransE / TransH / TransR / TransD (examples/TransX) and DistMult (examples/distmult),
  * fused: the mapped id rows of each triple and of its corrupted triples, the scores, the margin loss and the rank.
