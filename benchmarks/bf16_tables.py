@@ -1,15 +1,25 @@
 #!/usr/bin/env python
-"""DeepWalk's training step on float32 against bfloat16 id tables (unsupervised.DeepWalk(table_dtype=...), train_step), at one
-shape, in one run on one GPU.
+"""A training step on float32 against bfloat16 id tables, at one shape, in one run on one GPU: DeepWalk's
+(unsupervised.DeepWalk(table_dtype=...), train_step; the default) or a knowledge-graph model's (knowledge.TransE, TransR,
+TransD or DistMult(table_dtype=...), train_step).
 
-    python benchmarks/bf16_tables.py [--nodes N] [--edges E] [--dim D] [--batch B] [--optimizer NAME] [--steps K] [--warmup W]
+    python benchmarks/bf16_tables.py [--model deepwalk] [--nodes N] [--edges E] [--dim D] [--batch B] [--optimizer NAME]
+                                     [--steps K] [--warmup W]
+    python benchmarks/bf16_tables.py --model {transe,transr,transd,distmult} [--nodes N] [--triples T] [--relations R]
+                                     [--dim D] [--rel-dim D] [--batch B] [--negs K] [--lr LR] [--optimizer NAME] [--steps K]
+                                     [--warmup W]
 
-A step is train_step: the walks, pairs and negatives drawn on the device, the fused skip-gram forward, its sparse backward,
-and the optimizer's fused update of both tables and their slots (bf16: stochastic rounding on every store).  Both arms
-draw the same ids (the sampler is reseeded before each step of each arm) and start from the same tables (the f32 arm
-holds the bf16 arm's widened values).  The arms alternate round by round, timed with device events.  Reported per arm:
-ms per step, the tables' and slots' bytes, and the mean loss of the timed steps; the card's name, power limit and max SM
-clock are read in the same run.  One JSON line on stdout.  It needs a GPU: without one it fails."""
+DeepWalk: a step is train_step: the walks, pairs and negatives drawn on the device, the fused skip-gram forward, its sparse
+backward, and the optimizer's fused update of both tables and their slots (bf16: stochastic rounding on every store), on an
+R-MAT graph.  A knowledge-graph step is train_step on B triples from sample_edge: the relation ids from the edge feature
+'id', K negatives per triple from sample_node, the fused margin loss ('both' corruptions, L1) and its sparse backward, and
+the optimizer's update of every table and slot.  Its graph is built from a seed: N entities and T triples, uniform
+endpoints, relations of Zipf-like frequency (exponent 1.1) over R relation ids (Graph.from_csr + set_edges).  Defaults:
+10M entities, 10M triples, 1 000 relations, B = 8192, K = 64, dim 128 (TransR 128 x 32), Adam at lr 0.001.
+Both arms draw the same ids (the sampler is reseeded before each step of each arm) and start from the same tables (the
+f32 arm holds the bf16 arm's widened values).  The arms alternate round by round, timed with device events.  Reported per
+arm: ms per step, the tables' and slots' bytes, and the mean loss of the timed steps; the card's name, power limit and max
+SM clock are read in the same run.  One JSON line on stdout.  It needs a GPU: without one it fails."""
 import argparse
 import os
 import sys
@@ -23,41 +33,91 @@ from full_dataflow import emit, gpu_info  # noqa: E402
 import full_dataflow  # noqa: E402
 
 
+KG_MODELS = {"transe": "TransE", "transr": "TransR", "transd": "TransD", "distmult": "DistMult"}
+
+
 def parse(argv=None):
     p = argparse.ArgumentParser()
+    p.add_argument("--model", default="deepwalk", choices=["deepwalk"] + sorted(KG_MODELS))
     p.add_argument("--nodes", type=int, default=10_000_000)
     p.add_argument("--edges", type=int, default=100_000_000)
+    p.add_argument("--triples", type=int, default=10_000_000)
+    p.add_argument("--relations", type=int, default=1000)
     p.add_argument("--dim", type=int, default=128)
-    p.add_argument("--batch", type=int, default=512)
+    p.add_argument("--rel-dim", type=int, default=32, help="TransR's relation dim")
+    p.add_argument("--batch", type=int, default=None, help="default 512 (DeepWalk), 8192 (knowledge graph)")
+    p.add_argument("--negs", type=int, default=64)
+    p.add_argument("--lr", type=float, default=None, help="default 0.01 (DeepWalk), 0.001 (knowledge graph)")
     p.add_argument("--optimizer", default="adam")
     p.add_argument("--steps", type=int, default=20)
     p.add_argument("--warmup", type=int, default=3)
-    return p.parse_args(argv)
+    args = p.parse_args(argv)
+    kg = args.model != "deepwalk"
+    if args.batch is None:
+        args.batch = 8192 if kg else 512
+    if args.lr is None:
+        args.lr = 0.001 if kg else 0.01
+    return args
+
+
+def kg_graph(n_ent, n_tri, n_rel, seed=11):
+    """the knowledge graph of the module docstring: entities of node type 0, triples of edge type 0 whose relation id is
+    the dense edge feature 'id'"""
+    import numpy as np
+    import euler_b200 as eb
+    rng = np.random.RandomState(seed)
+    p = 1.0 / np.arange(1, n_rel + 1) ** 1.1
+    rel = rng.choice(n_rel, size=n_tri, p=p / p.sum())
+    src, dst = rng.randint(0, n_ent, n_tri), rng.randint(0, n_ent, n_tri)
+    order = np.lexsort((dst, src))
+    src, dst, rel = src[order], dst[order], rel[order]
+    ptr = np.zeros(n_ent + 1, np.int64)
+    np.add.at(ptr, src + 1, 1)
+    g = eb.Graph.from_csr(np.arange(n_ent), np.cumsum(ptr), dst, w=np.ones(n_tri, np.float32))
+    g.set_edges(src, dst, np.zeros(n_tri, np.int32), dense=rel.reshape(-1, 1).astype(np.float32), dense_names=['id'])
+    return g
 
 
 def run(args):
     import numpy as np
     import torch
     import euler_b200 as eb
-    from euler_b200 import optimizers, unsupervised as un
+    from euler_b200 import knowledge, optimizers, unsupervised as un
     torch.cuda.set_device(0)
-    eb.set_graph(eb.Graph.rmat(args.nodes, args.edges, seed=11), rng="philox", seed=1)
+    kg = args.model != "deepwalk"
+    if kg:
+        eb.set_graph(kg_graph(args.nodes, args.triples, args.relations), rng="philox", seed=1)
+    else:
+        eb.set_graph(eb.Graph.rmat(args.nodes, args.edges, seed=11), rng="philox", seed=1)
     models = {}
     for name, dt in (("bf16", torch.bfloat16), ("f32", torch.float32)):
         torch.manual_seed(3)
-        models[name] = un.DeepWalk(0, [0], args.nodes, args.dim, walk_len=3, num_negs=5, device="cuda", table_dtype=dt)
+        if kg:
+            rel_dim = args.rel_dim if args.model == "transr" else args.dim
+            models[name] = getattr(knowledge, KG_MODELS[args.model])(
+                0, 0, args.nodes - 1, args.relations - 1, args.dim, rel_dim, num_negs=args.negs, margin=1.0, l1=True,
+                corrupt='both', device="cuda", table_dtype=dt)
+        else:
+            models[name] = un.DeepWalk(0, [0], args.nodes, args.dim, walk_len=3, num_negs=5, device="cuda", table_dtype=dt)
     with torch.no_grad():
         for p16, p32 in zip(models["bf16"].parameters(), models["f32"].parameters()):
             p32.copy_(p16.float())
-    opts = {k: optimizers.get(args.optimizer)(list(m.parameters()), 0.01, **({"seed": 5} if k == "bf16" else {}))
+    opts = {k: optimizers.get(args.optimizer)(list(m.parameters()), args.lr, **({"seed": 5} if k == "bf16" else {}))
             for k, m in models.items()}
-    batches = [torch.from_numpy(np.random.RandomState(100 + i).randint(1, args.nodes + 1, size=args.batch)).cuda()
-               for i in range(args.warmup + args.steps)]
+    if kg:   # the triples of each step, drawn once: both arms train on the same edges
+        batches = []
+        for i in range(args.warmup + args.steps):
+            eb.seed(100 + i)
+            batches.append(eb.sample_edge(args.batch, 0))
+    else:
+        batches = [torch.from_numpy(np.random.RandomState(100 + i).randint(1, args.nodes + 1, size=args.batch)).cuda()
+                   for i in range(args.warmup + args.steps)]
     losses = {k: [] for k in models}
 
     def step(k, i):
         eb.seed(1000 + i)
-        losses[k].append(models[k].train_step(batches[i], opts[k])[0])
+        out = models[k].train_step(batches[i], opts[k])
+        losses[k].append(out.loss if kg else out[0])
 
     for i in range(args.warmup):
         for k in models:
@@ -90,8 +150,13 @@ def run(args):
         return sum(p.numel() * p.element_size() for p in ps) + sum(
             t.numel() * t.element_size() for p in ps for t in opts[k].state[p].values() if torch.is_tensor(t))
 
-    out = {"workload": "deepwalk_train_step", "nodes": args.nodes, "edges": args.edges, "dim": args.dim, "batch": args.batch,
-           "optimizer": args.optimizer, "gpu": gpu_info(0)}
+    if kg:
+        out = {"workload": "%s_train_step" % args.model, "entities": args.nodes, "triples": args.triples,
+               "relations": args.relations, "dim": args.dim, "rel_dim": args.rel_dim if args.model == "transr" else args.dim,
+               "batch": args.batch, "negs": args.negs, "optimizer": args.optimizer, "lr": args.lr, "gpu": gpu_info(0)}
+    else:
+        out = {"workload": "deepwalk_train_step", "nodes": args.nodes, "edges": args.edges, "dim": args.dim, "batch": args.batch,
+               "optimizer": args.optimizer, "gpu": gpu_info(0)}
     for k, (ms, n) in tot.items():
         out[k] = {"ms_per_step": ms / n, "steps": n, "table_and_slot_bytes": state_bytes(k),
                   "mean_loss": float(np.mean([float(x) for x in losses[k]]))}

@@ -252,6 +252,9 @@ SIGNATURES = {
     "eu_kg_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "eu_kg_loss_backward": (C.c_int, [_P, _P, _P, _P, _P]),
     "eu_kg_loss_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
+    "eu_kg_loss_dtype": (C.c_int, [_P, _P, _I32, _P, _P, _P, _P, _P, _P]),
+    "eu_kg_loss_backward_dtype": (C.c_int, [_P, _P, _I32, _P, _P, _P]),
+    "eu_kg_loss_backward_sparse_dtype": (C.c_int, [_P, _P, _I32, _P, _P, _P, _P, _P]),
     "eu_graph_set_edge_dense_feature_name": (C.c_int, [_P, _I32, C.c_char_p]),
     "InitQueryProxy": (C.c_bool, [C.c_char_p]),
     "eu_default_graph": (_P, []),

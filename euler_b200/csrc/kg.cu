@@ -44,6 +44,11 @@
 // sums in chunk order): no atomics, the same bits on every run.  Entity entries are listed src (B), dst
 // (B), then negatives (b, k); relation entries by triple.  Scratch is O(B (2 + K) dim) (TransR: plus B ent_dim rel_dim), never
 // O(n_rows).  An id outside its table is read as row 0 and flagged: EU_ERR_INVALID after the call's one synchronisation.
+//
+// Tables are f32 or bf16 (Tab, an eu_feat_dtype; one type for all of a call's tables).  Every read of a table element widens
+// bf16 to f32 exactly (row_load4, feat_ld; TransR's M is staged widened) and every other step is the f32 one, so a bf16 call
+// gives the f32 call's bits on the widened tables: scores, rank, loss, embeddings and gradients alike, all of them f32.  The
+// 4-wide loads (VEC) need both dims % 4 == 0 and each table aligned to four elements (16 bytes of f32, 8 of bf16).
 #include <atomic>
 
 #include "segment.cuh"
@@ -66,7 +71,7 @@ struct KgArgs {
   float margin;
   int64_t B;
   const int64_t *src, *dst, *rel, *neg;
-  const float *ent, *relt, *eaux, *raux;
+  const void *ent, *relt, *eaux, *raux;   // of the kernels' table type Tab
   int64_t n_ent, n_rel;
   int ent_dim, rel_dim;   // rel_dim is also the width of a mapped entity row and of every score
   int ldm;                // TransR: the row stride of the staged M (rel_dim rounded up to 4, plus 4 against bank conflicts)
@@ -135,13 +140,14 @@ __device__ __forceinline__ float kg_wsum(float x) {
   return x;
 }
 
-template <bool VEC>
-__device__ __forceinline__ KgRow kg_load(const float* __restrict__ row, int dim) {
+// a table row widened to f32
+template <bool VEC, typename Tab>
+__device__ __forceinline__ KgRow kg_load(const Tab* __restrict__ row, int dim) {
   KgRow r;
 #pragma unroll
   for (int i = 0; i < kKgCh; ++i) {
     const int d = kg_col(i);
-    r.v[i] = d < dim ? row_load4<VEC>(row, d, dim) : make_float4(0.f, 0.f, 0.f, 0.f);
+    r.v[i] = d < dim ? row_load4<VEC, Tab>(row, d, dim) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
   return r;
 }
@@ -249,9 +255,9 @@ struct KgMap {
 };
 
 // the mapped row of entity table row `row`; TransR uses the warp's row buffer w
-template <int M, bool VEC>
+template <int M, bool VEC, typename Tab>
 __device__ __forceinline__ void kg_map(const KgArgs& A, int64_t row, const KgSmem& S, float* w, KgMap& m) {
-  m.e = kg_load<VEC>(A.ent + row * A.ent_dim, A.ent_dim);
+  m.e = kg_load<VEC>(static_cast<const Tab*>(A.ent) + row * A.ent_dim, A.ent_dim);
   m.dot = 0.f;
   m.n.inv = 1.f;
   m.n.act = false;
@@ -264,7 +270,7 @@ __device__ __forceinline__ void kg_map(const KgArgs& A, int64_t row, const KgSme
     m.y = kg_zero();
     kg_each(A.ent_dim, [&](int i, int c) { kg_c(m.y.v[i], c) = __fmaf_rn(-m.dot, kg_c(h.v[i], c), kg_c(m.e.v[i], c)); });
   } else if (M == KG_TRANSD) {
-    m.t = kg_load<VEC>(A.eaux + row * A.ent_dim, A.ent_dim);
+    m.t = kg_load<VEC>(static_cast<const Tab*>(A.eaux) + row * A.ent_dim, A.ent_dim);
     const KgRow rt = kg_lds(S.a, A.ent_dim);
     m.dot = kg_dot(m.e, m.t, A.ent_dim);
     m.y = kg_zero();
@@ -341,24 +347,24 @@ __device__ __forceinline__ void kg_entity_back(const KgArgs& A, const KgMap& m, 
 }
 
 // The triple's own rows into shared memory: r = n(relation row), a = h (TransH) or rt (TransD), M (TransR), then the mapped
-// s and d.  Every thread of the block calls it.
-template <int M, bool VEC>
+// s and d.  Every thread of the block calls it.  M is staged widened to f32.
+template <int M, bool VEC, typename Tab>
 __device__ __forceinline__ void kg_stage(const KgArgs& A, int64_t b, const KgSmem& S, int* bad) {
   const int warp = threadIdx.x >> 5;
   const int64_t rb = row_of(__ldg(A.rel + b), A.n_rel, bad);
   if (M == KG_TRANSR) {
-    const float* mr = A.raux + rb * (int64_t)A.ent_dim * A.rel_dim;
+    const Tab* mr = static_cast<const Tab*>(A.raux) + rb * (int64_t)A.ent_dim * A.rel_dim;
     for (int t = threadIdx.x; t < A.ent_dim * A.ldm; t += blockDim.x) {
       const int i = t / A.ldm, j = t - i * A.ldm;
-      S.m[t] = j < A.rel_dim ? __ldg(mr + (int64_t)i * A.rel_dim + j) : 0.f;
+      S.m[t] = j < A.rel_dim ? feat_ld<Tab>(mr + (int64_t)i * A.rel_dim + j) : 0.f;
     }
   }
   if (warp == 0) {
-    KgRow r = kg_load<VEC>(A.relt + rb * A.rel_dim, A.rel_dim);
+    KgRow r = kg_load<VEC>(static_cast<const Tab*>(A.relt) + rb * A.rel_dim, A.rel_dim);
     kg_norm(r, A.rel_dim);
     kg_sts(S.r, r, A.rel_dim);
   } else if (warp == 1 && (M == KG_TRANSH || M == KG_TRANSD)) {
-    KgRow a = kg_load<VEC>(A.raux + rb * A.ent_dim, A.ent_dim);
+    KgRow a = kg_load<VEC>(static_cast<const Tab*>(A.raux) + rb * A.ent_dim, A.ent_dim);
     if (M == KG_TRANSH) kg_norm(a, A.ent_dim);
     kg_sts(S.a, a, A.ent_dim);
   }
@@ -366,7 +372,7 @@ __device__ __forceinline__ void kg_stage(const KgArgs& A, int64_t b, const KgSme
   if (warp < 2) {
     const int64_t id = __ldg((warp == 0 ? A.src : A.dst) + b);
     KgMap m;
-    kg_map<M, VEC>(A, row_of(id, A.n_ent, bad), S, S.w + warp * 2 * kKgMaxDim, m);
+    kg_map<M, VEC, Tab>(A, row_of(id, A.n_ent, bad), S, S.w + warp * 2 * kKgMaxDim, m);
     kg_sts(warp == 0 ? S.s : S.d, m.y, A.rel_dim);
   }
   __syncthreads();
@@ -374,7 +380,7 @@ __device__ __forceinline__ void kg_stage(const KgArgs& A, int64_t b, const KgSme
 
 // ---------------------------------------------------------------------------- forward
 // One block per (triple b, tile of kKgTile negatives); tile 0 also writes the true triple's score and the embeddings
-template <int M, bool VEC>
+template <int M, bool VEC, typename Tab>
 __global__ void __launch_bounds__(kKgThreads) k_kg_fwd(KgArgs A, int tiles, float* __restrict__ scores, float* emb_s,
                                                         float* emb_r, float* emb_d, int* bad) {
   extern __shared__ float4 kg_sm4[];
@@ -382,7 +388,7 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_fwd(KgArgs A, int tiles, floa
   const int64_t b = blockIdx.x / tiles;
   const int tile = (int)(blockIdx.x - b * tiles);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  kg_stage<M, VEC>(A, b, S, bad);
+  kg_stage<M, VEC, Tab>(A, b, S, bad);
   const int D = A.rel_dim;
   const KgRow s = kg_lds(S.s, D), d = kg_lds(S.d, D), r = kg_lds(S.r, D);
   float* srow = scores + b * (1 + (int64_t)A.C * A.K);
@@ -401,7 +407,7 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_fwd(KgArgs A, int tiles, floa
   const int k1 = min(A.K, (tile + 1) * kKgTile);
   for (int k = tile * kKgTile + warp; k < k1; k += kKgWarps) {
     KgMap m;
-    kg_map<M, VEC>(A, row_of(__ldg(A.neg + b * A.K + k), A.n_ent, bad), S, wbuf, m);
+    kg_map<M, VEC, Tab>(A, row_of(__ldg(A.neg + b * A.K + k), A.n_ent, bad), S, wbuf, m);
     if (A.front) {
       const float x = kg_score<M>(A.l1, m.y, r, d, D);
       if (lane == 0) srow[1 + k] = x;
@@ -453,7 +459,7 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_rows(const float* __restrict_
 // The gradient of a mapped row y from its DistMult / TransX terms is assembled by the callers below.
 
 // One block per (triple, tile), a warp per negative: the entity entries 2B + b K + k, F / T [b, k], U [b, 2 + k], sc [b, 2 + k]
-template <int M, bool VEC>
+template <int M, bool VEC, typename Tab>
 __global__ void __launch_bounds__(kKgThreads) k_kg_bwd_neg(KgArgs A, int tiles, const float2* __restrict__ coef, float* F, float* T,
                                                             float* U, float2* sc, float* Gent, float* Gea, int* bad) {
   extern __shared__ float4 kg_sm4[];
@@ -461,7 +467,7 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_bwd_neg(KgArgs A, int tiles, 
   const int64_t b = blockIdx.x / tiles;
   const int tile = (int)(blockIdx.x - b * tiles);
   const int warp = threadIdx.x >> 5;
-  kg_stage<M, VEC>(A, b, S, bad);
+  kg_stage<M, VEC, Tab>(A, b, S, bad);
   const int D = A.rel_dim;
   const KgRow s = kg_lds(S.s, D), d = kg_lds(S.d, D), r = kg_lds(S.r, D);
   const float cn = coef[b].y;
@@ -470,7 +476,7 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_bwd_neg(KgArgs A, int tiles, 
   const int k1 = min(A.K, (tile + 1) * kKgTile);
   for (int k = tile * kKgTile + warp; k < k1; k += kKgWarps) {
     KgMap m;
-    kg_map<M, VEC>(A, row_of(__ldg(A.neg + b * A.K + k), A.n_ent, bad), S, wbuf, m);
+    kg_map<M, VEC, Tab>(A, row_of(__ldg(A.neg + b * A.K + k), A.n_ent, bad), S, wbuf, m);
     KgRow gy = kg_zero();
     const int64_t bk = b * A.K + k;
     if (M == KG_DISTMULT) {
@@ -508,7 +514,7 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_bwd_neg(KgArgs A, int tiles, 
 // One block per triple: SF, ST = F, T summed over k from +0 in f64; the src and dst entries (warps 0 and 1) and the relation entry
 // (warp 2).  TransX: Gp = the true triple's term; gy_s = Gp + ST, gy_d = -(Gp + SF), gr = (Gp + SF) + ST.  DistMult:
 // gy_s = fma(cp, r d, r ST), gy_d = fma(cp, s r, r SF), gr = fma(cp, s d, fma(d, SF, s ST)).
-template <int M, bool VEC>
+template <int M, bool VEC, typename Tab>
 __global__ void __launch_bounds__(kKgThreads, 1) k_kg_bwd_triple(KgArgs A, const float2* __restrict__ coef, const float* __restrict__ F,
                                                                const float* __restrict__ T, float* U, float2* sc, float* Gent,
                                                                float* Gea, float* Grel, int* bad) {
@@ -528,7 +534,7 @@ __global__ void __launch_bounds__(kKgThreads, 1) k_kg_bwd_triple(KgArgs A, const
     S.f[j] = (float)f;
     S.t[j] = (float)t;
   }
-  kg_stage<M, VEC>(A, b, S, bad);   // its barriers also publish S.f and S.t
+  kg_stage<M, VEC, Tab>(A, b, S, bad);   // its barriers also publish S.f and S.t
   if (warp > 2) return;
   const float cp = coef[b].x;
   const KgRow s = kg_lds(S.s, D), d = kg_lds(S.d, D), r = kg_lds(S.r, D);
@@ -561,14 +567,14 @@ __global__ void __launch_bounds__(kKgThreads, 1) k_kg_bwd_triple(KgArgs A, const
   }
   if (warp == 2) {
     const int64_t rb = row_of(__ldg(A.rel + b), A.n_rel, bad);
-    KgRow y = kg_load<VEC>(A.relt + rb * D, D);
+    KgRow y = kg_load<VEC>(static_cast<const Tab*>(A.relt) + rb * D, D);
     const KgNorm n = kg_norm(y, D);
     kg_stg(Grel + b * D, kg_norm_back(y, n, g, D), D);
     return;
   }
   KgMap m;
   float* wbuf = S.w + warp * 2 * kKgMaxDim;
-  kg_map<M, VEC>(A, row_of(__ldg((warp == 0 ? A.src : A.dst) + b), A.n_ent, bad), S, wbuf, m);
+  kg_map<M, VEC, Tab>(A, row_of(__ldg((warp == 0 ? A.src : A.dst) + b), A.n_ent, bad), S, wbuf, m);
   kg_entity_back<M>(A, m, g, S, wbuf, warp * A.B + b, Gent, Gea, U + (b * N + warp) * D, sc + b * N + warp);
 }
 
@@ -581,7 +587,7 @@ __device__ __forceinline__ int64_t kg_entity_of(const KgArgs& A, int64_t b, int 
 // TransH and TransD, one block per triple, a thread per column, entries n = 0 .. K + 1 in order from +0:
 //   TransH: gh_j = -(sum of alpha_n U_nj + beta_n e_nj), then through n() (warp 0);  TransD: grt_j = sum of delta_n U_nj;
 //   f64 fmas, rounded once
-template <int M, bool VEC>
+template <int M, bool VEC, typename Tab>
 __global__ void __launch_bounds__(kKgThreads) k_kg_bwd_raux(KgArgs A, const float* __restrict__ U, const float2* __restrict__ sc,
                                                              float* __restrict__ Graux) {
   __shared__ __align__(16) float sg[kKgMaxDim];
@@ -595,7 +601,8 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_bwd_raux(KgArgs A, const floa
         const float2 w = __ldg(sc + b * N + n);
         const float u = __ldg(U + (b * N + n) * D + j);
         acc = fma((double)w.x, (double)u, acc);
-        if (M == KG_TRANSH) acc = fma((double)w.y, (double)__ldg(A.ent + kg_entity_of(A, b, n, &ignored) * D + j), acc);
+        if (M == KG_TRANSH)
+          acc = fma((double)w.y, (double)feat_ld<Tab>(static_cast<const Tab*>(A.ent) + kg_entity_of(A, b, n, &ignored) * D + j), acc);
       }
     }
     if (M == KG_TRANSD && j < D) Graux[b * D + j] = (float)acc;
@@ -604,12 +611,14 @@ __global__ void __launch_bounds__(kKgThreads) k_kg_bwd_raux(KgArgs A, const floa
   if (M != KG_TRANSH) return;
   __syncthreads();
   if (threadIdx.x >= 32) return;
-  KgRow y = kg_load<VEC>(A.raux + row_of(__ldg(A.rel + b), A.n_rel, &ignored) * D, D);
+  KgRow y = kg_load<VEC>(static_cast<const Tab*>(A.raux) + row_of(__ldg(A.rel + b), A.n_rel, &ignored) * D, D);
   const KgNorm n = kg_norm(y, D);
   kg_stg(Graux + b * D, kg_norm_back(y, n, kg_lds(sg, D), D), D);
 }
 
-// TransR: gM[b, i, j] = sum over entries n of e_ni U_nj, f64 fma in n order, rounded once; a thread per element
+// TransR: gM[b, i, j] = sum over entries n of e_ni U_nj (e widened to f32, then exactly to f64), f64 fma in n order, rounded
+// once; a thread per element
+template <typename Tab>
 __global__ void __launch_bounds__(256) k_kg_bwd_mat(KgArgs A, int blocks_per, const float* __restrict__ U, float* __restrict__ Graux) {
   const int64_t b = blockIdx.x / blocks_per;
   const int64_t t = (blockIdx.x - b * blocks_per) * 256 + threadIdx.x;
@@ -620,7 +629,8 @@ __global__ void __launch_bounds__(256) k_kg_bwd_mat(KgArgs A, int blocks_per, co
   int ignored = 0;
   double acc = 0.0;
   for (int n = 0; n < N; ++n)
-    acc = fma((double)__ldg(A.ent + kg_entity_of(A, b, n, &ignored) * A.ent_dim + i), (double)__ldg(U + (b * N + n) * A.rel_dim + j), acc);
+    acc = fma((double)feat_ld<Tab>(static_cast<const Tab*>(A.ent) + kg_entity_of(A, b, n, &ignored) * A.ent_dim + i),
+              (double)__ldg(U + (b * N + n) * A.rel_dim + j), acc);
   Graux[b * W + t] = (float)acc;
 }
 
@@ -641,9 +651,13 @@ static int kg_aux_width(int model, int ent_dim, int rel_dim) {
   return model == KG_TRANSH ? ent_dim : model == KG_TRANSR ? ent_dim * rel_dim : model == KG_TRANSD ? rel_dim : 0;
 }
 
-static int kg_args(eu_ctx* c, const eu_kg_problem* p, KgArgs* A, const char* who) {
+static int kg_args(eu_ctx* c, const eu_kg_problem* p, int dtype, KgArgs* A, const char* who) {
   if (!c || !p) {
     set_error("%s: bad argument", who);
+    return EU_ERR_INVALID;
+  }
+  if (dtype != EU_FEAT_F32 && dtype != EU_FEAT_BF16) {
+    set_error("%s: unknown table dtype %d (EU_FEAT_F32 or EU_FEAT_BF16)", who, dtype);
     return EU_ERR_INVALID;
   }
   const int m = p->model;
@@ -688,20 +702,20 @@ static int kg_args(eu_ctx* c, const eu_kg_problem* p, KgArgs* A, const char* who
   return EU_OK;
 }
 
-static bool kg_vec(int model, const KgArgs& A) {
-  return A.ent_dim % 4 == 0 && A.rel_dim % 4 == 0 && aligned16(A.ent) && aligned16(A.relt) && (!A.eaux || aligned16(A.eaux)) &&
-         (model == KG_TRANSR || !A.raux || aligned16(A.raux));
+static bool kg_vec(int model, const KgArgs& A, int dtype) {
+  return A.ent_dim % 4 == 0 && A.rel_dim % 4 == 0 && aligned4_elems(A.ent, dtype) && aligned4_elems(A.relt, dtype) &&
+         (!A.eaux || aligned4_elems(A.eaux, dtype)) && (model == KG_TRANSR || !A.raux || aligned4_elems(A.raux, dtype));
 }
 
-template <int M, bool VEC>
+template <int M, bool VEC, typename Tab>
 static int kg_launch_fwd(eu_ctx* c, const KgArgs& A, float* scores, float* es, float* er, float* ed, int* bad) {
   const size_t sm = kg_smem_bytes(M, A.ent_dim, A.ldm);
   if constexpr (M == KG_TRANSR) {
     static std::atomic<unsigned long long> done{0};
-    if (int rc = kg_allow_smem(k_kg_fwd<M, VEC>, c->g->device, &done)) return rc;
+    if (int rc = kg_allow_smem(k_kg_fwd<M, VEC, Tab>, c->g->device, &done)) return rc;
   }
   const int tiles = (int)ceil_div(A.K, kKgTile);
-  k_kg_fwd<M, VEC><<<(unsigned)(A.B * tiles), kKgThreads, sm, c->stream>>>(A, tiles, scores, es, er, ed, bad);
+  k_kg_fwd<M, VEC, Tab><<<(unsigned)(A.B * tiles), kKgThreads, sm, c->stream>>>(A, tiles, scores, es, er, ed, bad);
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -712,45 +726,55 @@ struct KgBwd {
   float2* sc = nullptr;
 };
 
-template <int M, bool VEC>
+template <int M, bool VEC, typename Tab>
 static int kg_launch_bwd(eu_ctx* c, const KgArgs& A, const KgBwd& W, int* bad) {
   cudaStream_t s = c->stream;
   const size_t sm = kg_smem_bytes(M, A.ent_dim, A.ldm);
   if constexpr (M == KG_TRANSR) {
     static std::atomic<unsigned long long> done_neg{0}, done_triple{0};
-    if (int rc = kg_allow_smem(k_kg_bwd_neg<M, VEC>, c->g->device, &done_neg)) return rc;
-    if (int rc = kg_allow_smem(k_kg_bwd_triple<M, VEC>, c->g->device, &done_triple)) return rc;
+    if (int rc = kg_allow_smem(k_kg_bwd_neg<M, VEC, Tab>, c->g->device, &done_neg)) return rc;
+    if (int rc = kg_allow_smem(k_kg_bwd_triple<M, VEC, Tab>, c->g->device, &done_triple)) return rc;
   }
   const int tiles = (int)ceil_div(A.K, kKgTile);
-  k_kg_bwd_neg<M, VEC><<<(unsigned)(A.B * tiles), kKgThreads, sm, s>>>(A, tiles, W.coef, W.F, W.T, W.U, W.sc, W.Gent, W.Gea, bad);
+  k_kg_bwd_neg<M, VEC, Tab><<<(unsigned)(A.B * tiles), kKgThreads, sm, s>>>(A, tiles, W.coef, W.F, W.T, W.U, W.sc, W.Gent, W.Gea, bad);
   EU_LAUNCHED();
-  k_kg_bwd_triple<M, VEC><<<(unsigned)A.B, kKgThreads, sm, s>>>(A, W.coef, W.F, W.T, W.U, W.sc, W.Gent, W.Gea, W.Grel, bad);
+  k_kg_bwd_triple<M, VEC, Tab><<<(unsigned)A.B, kKgThreads, sm, s>>>(A, W.coef, W.F, W.T, W.U, W.sc, W.Gent, W.Gea, W.Grel, bad);
   EU_LAUNCHED();
   if constexpr (M == KG_TRANSH || M == KG_TRANSD) {
-    k_kg_bwd_raux<M, VEC><<<(unsigned)A.B, kKgThreads, 0, s>>>(A, W.U, W.sc, W.Graux);
+    k_kg_bwd_raux<M, VEC, Tab><<<(unsigned)A.B, kKgThreads, 0, s>>>(A, W.U, W.sc, W.Graux);
     EU_LAUNCHED();
   } else if constexpr (M == KG_TRANSR) {
     const int per = (int)ceil_div((int64_t)A.ent_dim * A.rel_dim, 256);
-    k_kg_bwd_mat<<<(unsigned)(A.B * per), 256, 0, s>>>(A, per, W.U, W.Graux);
+    k_kg_bwd_mat<Tab><<<(unsigned)(A.B * per), 256, 0, s>>>(A, per, W.U, W.Graux);
     EU_LAUNCHED();
   }
   return EU_OK;
 }
 
-template <int M>
-static int kg_dispatch_fwd(eu_ctx* c, const KgArgs& A, float* scores, float* es, float* er, float* ed, int* bad) {
-  return kg_vec(M, A) ? kg_launch_fwd<M, true>(c, A, scores, es, er, ed, bad) : kg_launch_fwd<M, false>(c, A, scores, es, er, ed, bad);
+template <int M, typename Tab>
+static int kg_dispatch_fwd(eu_ctx* c, const KgArgs& A, int dtype, float* scores, float* es, float* er, float* ed, int* bad) {
+  return kg_vec(M, A, dtype) ? kg_launch_fwd<M, true, Tab>(c, A, scores, es, er, ed, bad)
+                             : kg_launch_fwd<M, false, Tab>(c, A, scores, es, er, ed, bad);
 }
 template <int M>
-static int kg_dispatch_bwd(eu_ctx* c, const KgArgs& A, const KgBwd& W, int* bad) {
-  return kg_vec(M, A) ? kg_launch_bwd<M, true>(c, A, W, bad) : kg_launch_bwd<M, false>(c, A, W, bad);
+static int kg_dispatch_fwd(eu_ctx* c, const KgArgs& A, int dtype, float* scores, float* es, float* er, float* ed, int* bad) {
+  return dtype == EU_FEAT_BF16 ? kg_dispatch_fwd<M, __nv_bfloat16>(c, A, dtype, scores, es, er, ed, bad)
+                               : kg_dispatch_fwd<M, float>(c, A, dtype, scores, es, er, ed, bad);
+}
+template <int M, typename Tab>
+static int kg_dispatch_bwd(eu_ctx* c, const KgArgs& A, int dtype, const KgBwd& W, int* bad) {
+  return kg_vec(M, A, dtype) ? kg_launch_bwd<M, true, Tab>(c, A, W, bad) : kg_launch_bwd<M, false, Tab>(c, A, W, bad);
+}
+template <int M>
+static int kg_dispatch_bwd(eu_ctx* c, const KgArgs& A, int dtype, const KgBwd& W, int* bad) {
+  return dtype == EU_FEAT_BF16 ? kg_dispatch_bwd<M, __nv_bfloat16>(c, A, dtype, W, bad) : kg_dispatch_bwd<M, float>(c, A, dtype, W, bad);
 }
 
 // The backward pass both output forms share: out[t] is table t's dense gradient or COO values, rows[t] its COO rows
-static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, bool sparse, float* const* out,
-                       int64_t* const* rows, int64_t* counts, const char* who) {
+static int kg_backward(eu_ctx* c, const eu_kg_problem* p, int dtype, const float* grad_loss, const float* scores, bool sparse,
+                       float* const* out, int64_t* const* rows, int64_t* counts, const char* who) {
   KgArgs A;
-  int rc = kg_args(c, p, &A, who);
+  int rc = kg_args(c, p, dtype, &A, who);
   if (rc) return rc;
   const int model = p->model;
   const bool has[4] = {true, true, model == KG_TRANSD, model == KG_TRANSH || model == KG_TRANSR || model == KG_TRANSD};
@@ -825,11 +849,11 @@ static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss
     k_kg_rows<<<(unsigned)B, kKgThreads, 0, s>>>(scores, B, A.C * A.K, A.margin, nullptr, nullptr, grad_loss, W.coef);
     EU_LAUNCHED();
     switch (model) {
-      case KG_TRANSE: rc = kg_dispatch_bwd<KG_TRANSE>(c, A, W, bad); break;
-      case KG_TRANSH: rc = kg_dispatch_bwd<KG_TRANSH>(c, A, W, bad); break;
-      case KG_TRANSR: rc = kg_dispatch_bwd<KG_TRANSR>(c, A, W, bad); break;
-      case KG_TRANSD: rc = kg_dispatch_bwd<KG_TRANSD>(c, A, W, bad); break;
-      default: rc = kg_dispatch_bwd<KG_DISTMULT>(c, A, W, bad); break;
+      case KG_TRANSE: rc = kg_dispatch_bwd<KG_TRANSE>(c, A, dtype, W, bad); break;
+      case KG_TRANSH: rc = kg_dispatch_bwd<KG_TRANSH>(c, A, dtype, W, bad); break;
+      case KG_TRANSR: rc = kg_dispatch_bwd<KG_TRANSR>(c, A, dtype, W, bad); break;
+      case KG_TRANSD: rc = kg_dispatch_bwd<KG_TRANSD>(c, A, dtype, W, bad); break;
+      default: rc = kg_dispatch_bwd<KG_DISTMULT>(c, A, dtype, W, bad); break;
     }
     if (rc) return rc;
   }
@@ -856,17 +880,11 @@ static int kg_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss
   return EU_OK;
 }
 
-}  // namespace eu
-
-using namespace eu;
-
-extern "C" {
-
-int eu_kg_loss(eu_ctx* c, const eu_kg_problem* p, float* scores, int32_t* rank, float* loss, float* src_emb, float* rel_emb,
-               float* dst_emb) {
-  const char* who = "eu_kg_loss";
+// The forward pass of both table types
+static int kg_forward(eu_ctx* c, const eu_kg_problem* p, int dtype, float* scores, int32_t* rank, float* loss, float* src_emb,
+                      float* rel_emb, float* dst_emb, const char* who) {
   KgArgs A;
-  int rc = kg_args(c, p, &A, who);
+  int rc = kg_args(c, p, dtype, &A, who);
   if (rc) return rc;
   if (!loss || (A.B > 0 && (!scores || !rank)) || (src_emb && A.B > 0 && (!rel_emb || !dst_emb))) {
     set_error("%s: bad argument (scores, rank and loss are required; the embeddings all or none)", who);
@@ -878,11 +896,11 @@ int eu_kg_loss(eu_ctx* c, const eu_kg_problem* p, float* scores, int32_t* rank, 
   rc = mean_loss(c, A.B, A.B, loss, &h_bad, [&](int* bad, double* rowloss) -> int {
     int rc2;
     switch (p->model) {
-      case KG_TRANSE: rc2 = kg_dispatch_fwd<KG_TRANSE>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      case KG_TRANSH: rc2 = kg_dispatch_fwd<KG_TRANSH>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      case KG_TRANSR: rc2 = kg_dispatch_fwd<KG_TRANSR>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      case KG_TRANSD: rc2 = kg_dispatch_fwd<KG_TRANSD>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
-      default: rc2 = kg_dispatch_fwd<KG_DISTMULT>(c, A, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSE: rc2 = kg_dispatch_fwd<KG_TRANSE>(c, A, dtype, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSH: rc2 = kg_dispatch_fwd<KG_TRANSH>(c, A, dtype, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSR: rc2 = kg_dispatch_fwd<KG_TRANSR>(c, A, dtype, scores, src_emb, rel_emb, dst_emb, bad); break;
+      case KG_TRANSD: rc2 = kg_dispatch_fwd<KG_TRANSD>(c, A, dtype, scores, src_emb, rel_emb, dst_emb, bad); break;
+      default: rc2 = kg_dispatch_fwd<KG_DISTMULT>(c, A, dtype, scores, src_emb, rel_emb, dst_emb, bad); break;
     }
     if (rc2) return rc2;
     k_kg_rows<<<(unsigned)A.B, kKgThreads, 0, c->stream>>>(scores, A.B, A.C * A.K, A.margin, rank, rowloss, nullptr, nullptr);
@@ -897,13 +915,39 @@ int eu_kg_loss(eu_ctx* c, const eu_kg_problem* p, float* scores, int32_t* rank, 
   return EU_OK;
 }
 
+}  // namespace eu
+
+using namespace eu;
+
+extern "C" {
+
+int eu_kg_loss(eu_ctx* c, const eu_kg_problem* p, float* scores, int32_t* rank, float* loss, float* src_emb, float* rel_emb,
+               float* dst_emb) {
+  return kg_forward(c, p, EU_FEAT_F32, scores, rank, loss, src_emb, rel_emb, dst_emb, "eu_kg_loss");
+}
+
+int eu_kg_loss_dtype(eu_ctx* c, const eu_kg_problem* p, int32_t table_dtype, float* scores, int32_t* rank, float* loss,
+                     float* src_emb, float* rel_emb, float* dst_emb) {
+  return kg_forward(c, p, table_dtype, scores, rank, loss, src_emb, rel_emb, dst_emb, "eu_kg_loss_dtype");
+}
+
 int eu_kg_loss_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, float* const* grads) {
-  return kg_backward(c, p, grad_loss, scores, false, grads, nullptr, nullptr, "eu_kg_loss_backward");
+  return kg_backward(c, p, EU_FEAT_F32, grad_loss, scores, false, grads, nullptr, nullptr, "eu_kg_loss_backward");
+}
+
+int eu_kg_loss_backward_dtype(eu_ctx* c, const eu_kg_problem* p, int32_t table_dtype, const float* grad_loss, const float* scores,
+                              float* const* grads) {
+  return kg_backward(c, p, table_dtype, grad_loss, scores, false, grads, nullptr, nullptr, "eu_kg_loss_backward_dtype");
 }
 
 int eu_kg_loss_backward_sparse(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, int64_t* const* rows,
                                float* const* values, int64_t* counts) {
-  return kg_backward(c, p, grad_loss, scores, true, values, rows, counts, "eu_kg_loss_backward_sparse");
+  return kg_backward(c, p, EU_FEAT_F32, grad_loss, scores, true, values, rows, counts, "eu_kg_loss_backward_sparse");
+}
+
+int eu_kg_loss_backward_sparse_dtype(eu_ctx* c, const eu_kg_problem* p, int32_t table_dtype, const float* grad_loss,
+                                     const float* scores, int64_t* const* rows, float* const* values, int64_t* counts) {
+  return kg_backward(c, p, table_dtype, grad_loss, scores, true, values, rows, counts, "eu_kg_loss_backward_sparse_dtype");
 }
 
 }  // extern "C"

@@ -10,6 +10,12 @@ hinge and stable sort), which is also the reference the fused op is tested and m
 
 Tables are layers.Embedding(max_id + 1, dim): max_id + 2 rows, truncated-normal with stddev 0.1 (unsupervised.Embedding).
 
+table_dtype=torch.bfloat16 stores every table of a model (and, through the optimizer, their slots) in bfloat16: half the
+HBM.  Such tables take no autograd gradient (torch would round it to nearest bf16, losing most small updates);
+train_step(edges, optimizer) runs the fused forward and sparse backward (ops.kg_margin_loss_sparse_grads) and hands the f32
+rows and values to the optimizer's apply_sparse, which writes the tables back by stochastic rounding.  It needs fused=True
+and one of optimizers.py's fused optimizers; forward still gives the loss, metric and embeddings, without a gradient.
+
 One documented departure: upstream's norm_emb reshapes the relation rows to [-1, ent_dim] before normalising, which for TransR
 with rel_dim != ent_dim normalises chunks that span triples (and fails when B rel_dim % ent_dim != 0).  Here each relation row
 is normalised over its own rel_dim, and TransR's embeddings are [B, rel_dim], in both paths.  The two agree when the dims are
@@ -19,8 +25,8 @@ import collections
 
 import torch
 
-from .ops import KG_MODELS, SKIPGRAM_METRICS, get_edge_dense_feature, kg_margin_loss, sample_node
-from .unsupervised import Embedding, composed_metric
+from .ops import KG_MODELS, SKIPGRAM_METRICS, get_edge_dense_feature, kg_margin_loss, kg_margin_loss_sparse_grads, sample_node
+from .unsupervised import Embedding, check_table_dtype, composed_metric
 
 ModelOutput = collections.namedtuple('ModelOutput', ['embedding', 'loss', 'metric_name', 'metric'])
 
@@ -111,25 +117,27 @@ def composed_kg_scores(model, tables, src, dst, neg, rel, l1=True, corrupt='both
 
 
 class _KgModel(torch.nn.Module):
-    """What TransX and DistMult share: the tables, generate_triplets and forward."""
+    """What TransX and DistMult share: the tables, generate_triplets, forward and train_step.  table_dtype: float32, or
+    bfloat16 (fused only) for every table, trained by train_step."""
     model = None
     metrics = SKIPGRAM_METRICS
 
     def __init__(self, node_type, edge_type, node_max_id, edge_max_id, ent_dim, rel_dim, num_negs=5, margin=1., l1=True,
-                 metric_name='mrr', corrupt='both', fused=True, sparse_grad=False, device=None):
+                 metric_name='mrr', corrupt='both', fused=True, sparse_grad=False, device=None, table_dtype=torch.float32):
         super().__init__()
         if metric_name not in self.metrics:
             raise ValueError('Metric name :{} not in list {}'.format(metric_name, list(self.metrics)))
         if corrupt not in ('front', 'tail', 'both'):
             raise ValueError("corrupt must be 'front', 'tail' or 'both', got %r" % (corrupt,))
+        check_table_dtype(table_dtype, fused)
         self.node_type, self.edge_type = node_type, edge_type
         self.node_max_id, self.edge_max_id = node_max_id, edge_max_id
         self.ent_dim, self.rel_dim = ent_dim, rel_dim
         self.num_negs, self.margin, self.l1 = num_negs, margin, l1
         self.metric_name, self.corrupt = metric_name, corrupt
-        self.fused, self.sparse_grad = fused, sparse_grad
-        self.entity_encoder = Embedding(node_max_id + 1, ent_dim, device=device)
-        self.relation_encoder = Embedding(edge_max_id + 1, rel_dim, device=device)
+        self.fused, self.sparse_grad, self.table_dtype = fused, sparse_grad, table_dtype
+        self.entity_encoder = Embedding(node_max_id + 1, ent_dim, device=device, dtype=table_dtype)
+        self.relation_encoder = Embedding(edge_max_id + 1, rel_dim, device=device, dtype=table_dtype)
 
     def tables(self):
         """the tables in the order ops.kg_margin_loss takes them"""
@@ -160,6 +168,27 @@ class _KgModel(torch.nn.Module):
         loss, metric, emb = self.loss_and_metric(src, dst, neg, rel)
         return ModelOutput(embedding=emb, loss=loss, metric_name=self.metric_name, metric=metric)
 
+    def train_step(self, inputs, optimizer):
+        """One training step on the edges `inputs` without autograd: generate_triplets, the fused forward and sparse backward
+        (ops.kg_margin_loss_sparse_grads), then optimizer.apply_sparse with every table's f32 rows and values.  The way to
+        train bf16 tables; f32 tables take the same step.  optimizer is one of optimizers.py's, fused, over these tables.  An
+        id outside its table raises before the optimizer runs: no table or slot changes.  Returns forward's ModelOutput.
+        DistMult(l2_regular=True) is refused: its L2 term is a dense gradient of the whole tables, which a sparse step
+        cannot carry (train it through forward and autograd)."""
+        if not self.fused:
+            raise ValueError("train_step runs the fused step: build the model with fused=True")
+        if getattr(self, 'l2_regular', False):
+            raise ValueError("train_step is a sparse step: l2_regular's whole-table term needs forward and autograd")
+        if not hasattr(optimizer, 'apply_sparse'):
+            raise ValueError("train_step needs one of euler_b200.optimizers' optimizers, got %s" % type(optimizer).__name__)
+        src, dst, neg, rel = self.generate_triplets(inputs)
+        tables = self.tables()
+        loss, metric, grads, emb = kg_margin_loss_sparse_grads(
+            src, dst, neg, rel, tables, self.model, l1=self.l1, corrupt=self.corrupt, margin=self.margin,
+            metric=self.metric_name, with_embeddings=True)
+        optimizer.apply_sparse(tables, [r for r, _ in grads], [v for _, v in grads])
+        return ModelOutput(embedding=emb, loss=loss, metric_name=self.metric_name, metric=metric)
+
 
 class TransX(_KgModel):
     """TransX (examples/TransX/transX.py): TransE's scores on the entity and relation tables; metric_name mrr, mr or hit10."""
@@ -188,7 +217,7 @@ class TransH(TransX):
             raise ValueError('Entity dim and Relation dim should be equal in TransH')
         super().__init__(node_type, edge_type, node_max_id, edge_max_id, ent_dim, rel_dim, num_negs=num_negs, margin=margin,
                          l1=l1, metric_name=metric_name, corrupt=corrupt, device=device, **kwargs)
-        self.hyper_vector = Embedding(edge_max_id + 1, ent_dim, device=device)
+        self.hyper_vector = Embedding(edge_max_id + 1, ent_dim, device=device, dtype=self.table_dtype)
 
     def tables(self):
         return super().tables() + [self.hyper_vector.embeddings]
@@ -203,7 +232,7 @@ class TransR(TransX):
                  metric_name='mrr', corrupt='both', device=None, **kwargs):
         super().__init__(node_type, edge_type, node_max_id, edge_max_id, ent_dim, rel_dim, num_negs=num_negs, margin=margin,
                          l1=l1, metric_name=metric_name, corrupt=corrupt, device=device, **kwargs)
-        self.transfer_matrix = Embedding(edge_max_id + 1, ent_dim * rel_dim, device=device)
+        self.transfer_matrix = Embedding(edge_max_id + 1, ent_dim * rel_dim, device=device, dtype=self.table_dtype)
 
     def tables(self):
         return super().tables() + [self.transfer_matrix.embeddings]
@@ -219,8 +248,8 @@ class TransD(TransX):
             raise ValueError('Entity dim and Relation dim should be equal in TransD')
         super().__init__(node_type, edge_type, node_max_id, edge_max_id, ent_dim, rel_dim, num_negs=num_negs, margin=margin,
                          l1=l1, metric_name=metric_name, corrupt=corrupt, device=device, **kwargs)
-        self.entity_transfer = Embedding(node_max_id + 1, ent_dim, device=device)
-        self.relation_transfer = Embedding(edge_max_id + 1, rel_dim, device=device)
+        self.entity_transfer = Embedding(node_max_id + 1, ent_dim, device=device, dtype=self.table_dtype)
+        self.relation_transfer = Embedding(edge_max_id + 1, rel_dim, device=device, dtype=self.table_dtype)
 
     def tables(self):
         return super().tables() + [self.entity_transfer.embeddings, self.relation_transfer.embeddings]
@@ -230,13 +259,16 @@ class DistMult(_KgModel):
     """DistMult (examples/distmult/distmult.py): y = n(e), r = n(r), score sum s (r d).  metric_name is one of metrics.get's
     ranking metrics (mrr, hit1, hit3, hit10, mr); its acc / auc / f1 take labels, not score pairs, and raise ValueError.
     l2_regular adds regular_param * (sum E^2 + sum R^2) over both whole tables, a torch term in both paths (not with
-    sparse_grad).  The fused op needs ent_dim == rel_dim, which upstream's einsum needs too."""
+    sparse_grad, bfloat16 tables or train_step: it is a dense whole-table autograd gradient).  The fused op needs ent_dim ==
+    rel_dim, which upstream's einsum needs too."""
     model = 'distmult'
 
     def __init__(self, node_type, edge_type, node_max_id, edge_max_id, ent_dim, rel_dim, num_negs=5, margin=1, metric_name='mrr',
                  corrupt='both', l2_regular=False, regular_param=0.0001, **kwargs):
         if ent_dim != rel_dim:
             raise ValueError('Entity dim and Relation dim should be equal in DistMult')
+        if l2_regular and kwargs.get('table_dtype', torch.float32) == torch.bfloat16:
+            raise ValueError('l2_regular is a dense autograd gradient of the whole tables: it cannot train bfloat16 tables')
         super().__init__(node_type, edge_type, node_max_id, edge_max_id, ent_dim, rel_dim, num_negs=num_negs, margin=margin,
                          metric_name=metric_name, corrupt=corrupt, **kwargs)
         if l2_regular and self.sparse_grad:

@@ -1984,7 +1984,8 @@ def _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, 
 
 
 def _raw_kg(ent, relt, eaux, raux, src, dst, rel, neg, cfg):
-    """one eu_kg_loss: (scores f32[B, 1 + C K], rank i32[B], loss f32[], [src_emb, rel_emb, dst_emb] or None)"""
+    """one eu_kg_loss (eu_kg_loss_dtype for bf16 tables): (scores f32[B, 1 + C K], rank i32[B], loss f32[],
+    [src_emb, rel_emb, dst_emb] or None)"""
     model, l1, corrupt, margin, ent_dim, rel_dim, sparse_grad, with_emb = cfg
     B, K = neg.shape
     dev = ent.device
@@ -1993,8 +1994,28 @@ def _raw_kg(ent, relt, eaux, raux, src, dst, rel, neg, cfg):
     loss = torch.empty((), dtype=torch.float32, device=dev)
     embs = [torch.empty((B, rel_dim), dtype=torch.float32, device=dev) for _ in range(3)] if with_emb else None
     p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, (ent, relt, eaux, raux), ent_dim, rel_dim)
-    _call("eu_kg_loss", C.byref(p), scores, rank, loss, *(embs or [None] * 3))
+    if ent.dtype == torch.bfloat16:
+        _call("eu_kg_loss_dtype", C.byref(p), _TABLE_DTYPES[ent.dtype], scores, rank, loss, *(embs or [None] * 3))
+    else:
+        _call("eu_kg_loss", C.byref(p), scores, rank, loss, *(embs or [None] * 3))
     return scores, rank, loss, embs
+
+
+def _raw_kg_sparse_grads(slots, src, dst, rel, neg, cfg, scores, g):
+    """one eu_kg_loss_backward_sparse(_dtype) over the four table slots: per slot (rows i64[cap], values f32[cap, width]) or
+    (None, None), _coo_buffers' arrays, and the counts of their rows filled"""
+    model, l1, corrupt, margin, ent_dim, rel_dim, _, _ = cfg
+    B, K = neg.shape
+    p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, rel_dim)
+    entries = (B * (K + 2), B, B * (K + 2), B)
+    bufs = [_coo_buffers(e, _shape(t), slots[0].device) for e, t in zip(entries, slots)]
+    counts = (C.c_int64 * 4)()
+    outs = ([r for r, _ in bufs], [v for _, v in bufs], counts)
+    if slots[0].dtype == torch.bfloat16:
+        _call("eu_kg_loss_backward_sparse_dtype", C.byref(p), _TABLE_DTYPES[slots[0].dtype], g, scores, *outs)
+    else:
+        _call("eu_kg_loss_backward_sparse", C.byref(p), g, scores, *outs)
+    return bufs, list(counts)
 
 
 class _KgLoss(torch.autograd.Function):
@@ -2019,18 +2040,52 @@ class _KgLoss(torch.autograd.Function):
         slots = (ent, relt, eaux, raux)
         dev = ent.device
         g = g_loss.to(device=dev, dtype=torch.float32).reshape(1).contiguous()
-        p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, rel_dim)
         if not sparse_grad:
+            p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, slots, ent_dim, rel_dim)
             grads = [None if t is None else torch.empty_like(t) for t in slots]
             _call("eu_kg_loss_backward", C.byref(p), g, scores, grads)
             return tuple(grads) + (None,) * 5
-        B, K = neg.shape
-        entries = (B * (K + 2), B, B * (K + 2), B)
-        shapes = [_shape(t) for t in slots]
-        bufs = [_coo_buffers(e, sh, dev) for e, sh in zip(entries, shapes)]
-        counts = (C.c_int64 * 4)()
-        _call("eu_kg_loss_backward_sparse", C.byref(p), g, scores, [r for r, _ in bufs], [v for _, v in bufs], counts)
-        return tuple(_coo(r, v, counts[t], shapes[t]) for t, (r, v) in enumerate(bufs)) + (None,) * 5
+        bufs, counts = _raw_kg_sparse_grads(slots, src, dst, rel, neg, ctx.cfg, scores, g)
+        return tuple(_coo(r, v, counts[t], _shape(slots[t])) for t, (r, v) in enumerate(bufs)) + (None,) * 5
+
+
+def _kg_args(op, src, dst, neg, rel, tables, model, corrupt, metric):
+    """(model index, the four table slots, src, dst, rel [B], neg [B, K]) on the device, or EulerError: the checks of
+    kg_margin_loss"""
+    name = str(model).lower()
+    if name not in KG_MODELS:
+        raise EulerError("%s: model must be one of %s, got %r" % (op, sorted(KG_MODELS), model))
+    if corrupt not in KG_CORRUPT:
+        raise EulerError("%s: corrupt must be one of %s, got %r" % (op, sorted(KG_CORRUPT), corrupt))
+    if metric not in SKIPGRAM_METRICS:
+        raise EulerError("%s: metric must be one of %s, got %r" % (op, SKIPGRAM_METRICS, metric))
+    m = KG_MODELS[name]
+    want = _KG_SLOTS[m]
+    tables = list(tables)
+    if len(tables) != len(want):
+        raise EulerError("%s: %s takes %d tables, got %d" % (op, name, len(want), len(tables)))
+    for k, tb in enumerate(tables):
+        if not torch.is_tensor(tb) or tb.dtype not in _TABLE_DTYPES or tb.dim() != 2:
+            raise EulerError("%s: table %d must be a 2-D float32 or bfloat16 tensor" % (op, k))
+    if any(tb.dtype != tables[0].dtype for tb in tables):
+        raise EulerError("%s: the tables must have one dtype, got %s" % (op, [str(tb.dtype) for tb in tables]))
+    slots = [None] * 4
+    for t, tb in zip(want, tables):
+        slots[t] = _t(tb, tb.dtype)
+    ent_dim, rel_dim = slots[0].shape[1], slots[1].shape[1]
+    aux_w = {1: ent_dim, 2: ent_dim * rel_dim, 3: rel_dim}.get(m)
+    if (slots[2] is not None and tuple(slots[2].shape) != tuple(slots[0].shape)) or \
+       (slots[3] is not None and (slots[3].shape[0] != slots[1].shape[0] or slots[3].shape[1] != aux_w)):
+        raise EulerError("%s: the auxiliary tables of %s must match the entity / relation tables" % (op, name))
+    src = _t(src, torch.int64).reshape(-1)
+    dst = _t(dst, torch.int64).reshape(-1)
+    rel = _t(rel, torch.int64).reshape(-1)
+    neg = _t(neg, torch.int64)
+    B = src.numel()
+    if dst.numel() != B or rel.numel() != B or neg.dim() != 2 or neg.shape[0] != B:
+        raise EulerError("%s: src, dst, rel must have B = %d ids and neg be [B, K], got %s, %s, %s"
+                         % (op, B, dst.numel(), rel.numel(), tuple(neg.shape)))
+    return m, slots, src, dst, rel, neg
 
 
 def kg_margin_loss(src, dst, neg, rel, tables, model, l1=True, corrupt='both', margin=1.0, metric='mrr', sparse_grad=False,
@@ -2039,45 +2094,44 @@ def kg_margin_loss(src, dst, neg, rel, tables, model, l1=True, corrupt='both', m
     device op:
         src, dst [B] or [B, 1]   entity ids of the true triples      rel [B] or [B, 1]   their relation ids (int64)
         neg [B, K]               entity ids of the corruptions (K >= 1)
-        tables                   f32 tables by model: 'transe' / 'distmult' (entity, relation); 'transh' (entity, relation,
-                                 hyper); 'transr' (entity, relation, transfer_matrix [n_rel, ent_dim * rel_dim]); 'transd'
-                                 (entity, relation, entity_transfer, relation_transfer)
+        tables                   f32 or bf16 tables by model: 'transe' / 'distmult' (entity, relation); 'transh' (entity,
+                                 relation, hyper); 'transr' (entity, relation, transfer_matrix [n_rel, ent_dim * rel_dim]);
+                                 'transd' (entity, relation, entity_transfer, relation_transfer)
     Scores each triple and its corruptions ('front': (neg_k, r, d), 'tail': (s, r, neg_k), 'both': front then tail) on the
     mapped rows (include/euler_b200.h, eu_kg_loss), and returns (loss, metric): loss = mean_b max(margin + mean_k neg - pos, 0),
     metric the ranking metric `metric` (skipgram_metric: mrr, hit1, hit3, hit10, mr) of the true triple among its corruptions,
     ties ranked as TF's stable top_k ranks them.  with_embeddings=True appends the mapped (src, rel, dst) rows f32[B, rel_dim]
     (not differentiated).  The gradient reaches the tables only: dense, or with sparse_grad=True coalesced sparse COO gradients
-    of the rows the batch touches.  Deterministic, no atomics; the forward and the backward synchronise once each."""
-    name = str(model).lower()
-    if name not in KG_MODELS:
-        raise EulerError("kg_margin_loss: model must be one of %s, got %r" % (sorted(KG_MODELS), model))
-    if corrupt not in KG_CORRUPT:
-        raise EulerError("kg_margin_loss: corrupt must be one of %s, got %r" % (sorted(KG_CORRUPT), corrupt))
-    if metric not in SKIPGRAM_METRICS:
-        raise EulerError("kg_margin_loss: metric must be one of %s, got %r" % (SKIPGRAM_METRICS, metric))
-    m = KG_MODELS[name]
-    want = _KG_SLOTS[m]
-    tables = list(tables)
-    if len(tables) != len(want):
-        raise EulerError("kg_margin_loss: %s takes %d tables, got %d" % (name, len(want), len(tables)))
-    _check_f32("kg_margin_loss", [("table %d" % k, tb) for k, tb in enumerate(tables)], 2)
-    slots = [None] * 4
-    for t, tb in zip(want, tables):
-        slots[t] = _t(tb, torch.float32)
-    ent_dim, rel_dim = slots[0].shape[1], slots[1].shape[1]
-    aux_w = {1: ent_dim, 2: ent_dim * rel_dim, 3: rel_dim}.get(m)
-    if (slots[2] is not None and tuple(slots[2].shape) != tuple(slots[0].shape)) or \
-       (slots[3] is not None and (slots[3].shape[0] != slots[1].shape[0] or slots[3].shape[1] != aux_w)):
-        raise EulerError("kg_margin_loss: the auxiliary tables of %s must match the entity / relation tables" % name)
-    src = _t(src, torch.int64).reshape(-1)
-    dst = _t(dst, torch.int64).reshape(-1)
-    rel = _t(rel, torch.int64).reshape(-1)
-    neg = _t(neg, torch.int64)
-    B = src.numel()
-    if dst.numel() != B or rel.numel() != B or neg.dim() != 2 or neg.shape[0] != B:
-        raise EulerError("kg_margin_loss: src, dst, rel must have B = %d ids and neg be [B, K], got %s, %s, %s"
-                         % (B, dst.numel(), rel.numel(), tuple(neg.shape)))
-    cfg = (m, bool(l1), KG_CORRUPT[corrupt], float(margin), ent_dim, rel_dim, bool(sparse_grad), bool(with_embeddings))
+    of the rows the batch touches.  Deterministic, no atomics; the forward and the backward synchronise once each.
+    bfloat16 tables (all of one dtype) are read widened exactly to f32, so the loss, metric and embeddings are the f32 op's
+    on the widened tables.  They take no gradient through autograd, which would round their f32 gradient to nearest bf16: a
+    bf16 table that requires grad raises.  Train them with kg_margin_loss_sparse_grads and an optimizer's apply_sparse
+    (knowledge's train_step)."""
+    m, slots, src, dst, rel, neg = _kg_args("kg_margin_loss", src, dst, neg, rel, tables, model, corrupt, metric)
+    if slots[0].dtype == torch.bfloat16 and any(t is not None and t.requires_grad for t in slots):
+        raise EulerError("kg_margin_loss: a bfloat16 table takes no autograd gradient (torch would round it to bf16); "
+                         "train it with kg_margin_loss_sparse_grads and an optimizer's apply_sparse")
+    cfg = (m, bool(l1), KG_CORRUPT[corrupt], float(margin), slots[0].shape[1], slots[1].shape[1], bool(sparse_grad),
+           bool(with_embeddings))
     out = _KgLoss.apply(slots[0], slots[1], slots[2], slots[3], src, dst, rel, neg, cfg)
     res = (out[0], skipgram_metric(out[1], metric))
     return res + tuple(out[2:]) if with_embeddings else res
+
+
+def kg_margin_loss_sparse_grads(src, dst, neg, rel, tables, model, l1=True, corrupt='both', margin=1.0, metric='mrr',
+                                with_embeddings=False):
+    """kg_margin_loss's forward and its sparse backward for an upstream gradient of 1, without autograd, for tables of
+    float32 or bfloat16 (all of one dtype, read widened exactly to f32).  Returns (loss, metric, grads), plus the mapped
+    (src, rel, dst) rows f32[B, rel_dim] with with_embeddings=True: grads is one (rows i64[D], values f32[D, width]) per
+    table, in the order the model takes its tables -- the coalesced f32 gradient that kg_margin_loss(..., sparse_grad=True)
+    .backward() gives f32 tables holding the widened values.  They go to an optimizer's apply_sparse as they are, never
+    rounded to bf16.  Synchronises twice (the forward, the backward)."""
+    m, slots, src, dst, rel, neg = _kg_args("kg_margin_loss_sparse_grads", src, dst, neg, rel, tables, model, corrupt, metric)
+    slots = [None if t is None else t.detach() for t in slots]
+    cfg = (m, bool(l1), KG_CORRUPT[corrupt], float(margin), slots[0].shape[1], slots[1].shape[1], True, bool(with_embeddings))
+    scores, rank, loss, embs = _raw_kg(*slots, src, dst, rel, neg, cfg)
+    g = torch.ones(1, dtype=torch.float32, device=slots[0].device)
+    bufs, counts = _raw_kg_sparse_grads(slots, src, dst, rel, neg, cfg, scores, g)
+    grads = [(bufs[t][0][:counts[t]], bufs[t][1][:counts[t]]) for t in _KG_SLOTS[m]]
+    res = (loss, skipgram_metric(rank, metric), grads)
+    return res + (embs,) if with_embeddings else res

@@ -51,6 +51,14 @@ class Embedding(torch.nn.Module):
         return F.embedding(ids, self.embeddings)
 
 
+def check_table_dtype(table_dtype, fused):
+    """ValueError unless table_dtype is float32, or bfloat16 with fused=True (bf16 tables train without autograd)"""
+    if table_dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError("table_dtype must be torch.float32 or torch.bfloat16, got %r" % (table_dtype,))
+    if table_dtype == torch.bfloat16 and not fused:
+        raise ValueError("table_dtype=torch.bfloat16 needs fused=True: the composed step trains through autograd")
+
+
 def _stable_ranks(pos_logits, neg_logits):
     """metrics.py's rank of the last entry of concat([neg, pos], 2): top_k (stable: ties to the lower index) and its inverse"""
     scores = torch.cat([neg_logits, pos_logits], 2)
@@ -97,10 +105,7 @@ class UnsuperviseModel(torch.nn.Module):
         super().__init__()
         if metric_name not in SKIPGRAM_METRICS:
             raise ValueError("metric_name must be one of %s, got %r" % (SKIPGRAM_METRICS, metric_name))
-        if table_dtype not in (torch.float32, torch.bfloat16):
-            raise ValueError("table_dtype must be torch.float32 or torch.bfloat16, got %r" % (table_dtype,))
-        if table_dtype == torch.bfloat16 and not fused:
-            raise ValueError("table_dtype=torch.bfloat16 needs fused=True: the composed step trains through autograd")
+        check_table_dtype(table_dtype, fused)
         self.node_type, self.edge_type, self.max_id = node_type, edge_type, max_id
         self.num_negs, self.metric_name = num_negs, metric_name
         self.fused, self.sparse_grad, self.table_dtype = fused, sparse_grad, table_dtype

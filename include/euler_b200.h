@@ -713,13 +713,27 @@ typedef struct {
   const int64_t* dst;       /* [B] */
   const int64_t* rel;       /* [B] */
   const int64_t* neg;       /* [B, K] */
-  const float* table[4];    /* entity, relation, entity-side auxiliary, relation-side auxiliary */
+  const float* table[4];    /* entity, relation, entity-side auxiliary, relation-side auxiliary; with the _dtype calls'
+                               EU_FEAT_BF16 each points at bf16 storage of the same shape */
 } eu_kg_problem;
 int eu_kg_loss(eu_ctx* c, const eu_kg_problem* p, float* scores, int32_t* rank, float* loss, float* src_emb, float* rel_emb,
                float* dst_emb);
 int eu_kg_loss_backward(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, float* const* grads);
 int eu_kg_loss_backward_sparse(eu_ctx* c, const eu_kg_problem* p, const float* grad_loss, const float* scores, int64_t* const* rows,
                                float* const* values, int64_t* counts);
+/* The same three with the tables' storage type table_dtype (eu_feat_dtype; every table of the call has it, and table[t] is
+ * then read as that type).  The skip-gram tables' two rules make a bf16 call exact: every read widens a bf16 element to f32
+ * exactly (TransR's matrix is staged widened), and all arithmetic stays f32 in the order above.  So a EU_FEAT_BF16 call
+ * gives bit for bit what the f32 call gives on the tables widened to f32; scores, rank, loss, the embeddings and every
+ * gradient stay f32.  The 4-wide loads need both dims % 4 == 0 and each table 8-byte aligned (bf16) or 16-byte aligned
+ * (f32); other tables take scalar loads with the same bits.  EU_FEAT_F32 is the call above.  An unknown table_dtype:
+ * EU_ERR_INVALID, before any device work; every other bound and status as above. */
+int eu_kg_loss_dtype(eu_ctx* c, const eu_kg_problem* p, int32_t table_dtype, float* scores, int32_t* rank, float* loss,
+                     float* src_emb, float* rel_emb, float* dst_emb);
+int eu_kg_loss_backward_dtype(eu_ctx* c, const eu_kg_problem* p, int32_t table_dtype, const float* grad_loss, const float* scores,
+                              float* const* grads);
+int eu_kg_loss_backward_sparse_dtype(eu_ctx* c, const eu_kg_problem* p, int32_t table_dtype, const float* grad_loss,
+                                     const float* scores, int64_t* const* rows, float* const* values, int64_t* counts);
 
 /* tf_euler.sample_edge -- TF op SampleEdge (tf_euler/kernels/sample_edge_op.cc; Graph::SampleEdge graph.cc:277-301): `count`
  * edges of ONE type drawn by the alias method over the edge weights, out i64[count,3] = (src, dst, type).  Several types or
