@@ -1,13 +1,16 @@
 #!/usr/bin/env python
 """A training step on float32 against bfloat16 id tables, at one shape, in one run on one GPU: DeepWalk's
-(unsupervised.DeepWalk(table_dtype=...), train_step; the default) or a knowledge-graph model's (knowledge.TransE, TransR,
-TransD or DistMult(table_dtype=...), train_step).
+(unsupervised.DeepWalk(table_dtype=...), train_step; the default), a knowledge-graph model's (knowledge.TransE, TransR,
+TransD or DistMult(table_dtype=...), train_step) or a supervised SageEncoder's (encoders.SageEncoder(table_dtype=...),
+optimizers.minimize).
 
     python benchmarks/bf16_tables.py [--model deepwalk] [--nodes N] [--edges E] [--dim D] [--batch B] [--optimizer NAME]
                                      [--steps K] [--warmup W]
     python benchmarks/bf16_tables.py --model {transe,transr,transd,distmult} [--nodes N] [--triples T] [--relations R]
                                      [--dim D] [--rel-dim D] [--batch B] [--negs K] [--lr LR] [--optimizer NAME] [--steps K]
                                      [--warmup W]
+    python benchmarks/bf16_tables.py --model sage [--nodes N] [--edges E] [--dim D] [--batch B] [--lr LR] [--optimizer NAME]
+                                     [--steps K] [--warmup W]
 
 DeepWalk: a step is train_step: the walks, pairs and negatives drawn on the device, the fused skip-gram forward, its sparse
 backward, and the optimizer's fused update of both tables and their slots (bf16: stochastic rounding on every store), on an
@@ -16,6 +19,11 @@ R-MAT graph.  A knowledge-graph step is train_step on B triples from sample_edge
 the optimizer's update of every table and slot.  Its graph is built from a seed: N entities and T triples, uniform
 endpoints, relations of Zipf-like frequency (exponent 1.1) over R relation ids (Graph.from_csr + set_edges).  Defaults:
 10M entities, 10M triples, 1 000 relations, B = 8192, K = 64, dim 128 (TransR 128 x 32), Adam at lr 0.001.
+SageEncoder: a step is optimizers.minimize of a SuperviseModel over SageEncoder on the graph of benchmarks/sage_encoder.py
+(the 10M-node R-MAT with a 128-column dense slot and its two seeded uint64 slots): use_id at dim 128 and both slots at dim
+128 (tables of N + 2, 10^6 + 2 and 10^7 + 2 rows), fanout [15, 10], 'mean' (so the deepest hop is pooled), dim 128, and a
+label of 8 columns taken from the dense slot (each column's sign) -- the fanout, both encoder passes with the tables' sparse
+backward, and the optimizer's update of the dense parameters and every table and slot.  Defaults: B = 512, Adam at lr 0.001.
 Both arms draw the same ids (the sampler is reseeded before each step of each arm) and start from the same tables (the
 f32 arm holds the bf16 arm's widened values).  The arms alternate round by round, timed with device events.  Reported per
 arm: ms per step, the tables' and slots' bytes, and the mean loss of the timed steps; the card's name, power limit and max
@@ -38,7 +46,7 @@ KG_MODELS = {"transe": "TransE", "transr": "TransR", "transd": "TransD", "distmu
 
 def parse(argv=None):
     p = argparse.ArgumentParser()
-    p.add_argument("--model", default="deepwalk", choices=["deepwalk"] + sorted(KG_MODELS))
+    p.add_argument("--model", default="deepwalk", choices=["deepwalk", "sage"] + sorted(KG_MODELS))
     p.add_argument("--nodes", type=int, default=10_000_000)
     p.add_argument("--edges", type=int, default=100_000_000)
     p.add_argument("--triples", type=int, default=10_000_000)
@@ -52,11 +60,11 @@ def parse(argv=None):
     p.add_argument("--steps", type=int, default=20)
     p.add_argument("--warmup", type=int, default=3)
     args = p.parse_args(argv)
-    kg = args.model != "deepwalk"
+    kg = args.model not in ("deepwalk", "sage")
     if args.batch is None:
         args.batch = 8192 if kg else 512
     if args.lr is None:
-        args.lr = 0.001 if kg else 0.01
+        args.lr = 0.01 if args.model == "deepwalk" else 0.001
     return args
 
 
@@ -78,21 +86,57 @@ def kg_graph(n_ent, n_tri, n_rel, seed=11):
     return g
 
 
+def sage_model(args, dt):
+    """the supervised SageEncoder of the module docstring (f32 tables take sparse gradients, as the bf16 proxies do)"""
+    import torch
+    import torch.nn.functional as F
+    import euler_b200 as eb
+    from shallow_encoder import DENSE_DIM
+    from sparse_embedding import SLOTS
+    from euler_b200.encoders import SageEncoder
+    from euler_b200.supervised import SuperviseModel
+
+    class SupervisedSage(SuperviseModel):
+        def __init__(self):
+            super().__init__("feat0", 8, dim=args.dim, device="cuda")
+            self.encoder = SageEncoder([[0], [0]], [15, 10], args.dim, aggregator="mean", feature_idx="feat0",
+                                       feature_dim=DENSE_DIM, max_id=args.nodes, use_id=True,
+                                       sparse_feature_idx=[n for n, _ in SLOTS], sparse_feature_max_id=[m - 1 for _, m in SLOTS],
+                                       embedding_dim=args.dim, sparse_grad=dt == torch.float32, device="cuda", table_dtype=dt)
+
+        def embed(self, n_id):
+            return self.encoder(n_id)
+
+        def forward(self, inputs):
+            """SuperviseModel's loss, its labels in {0, 1}: the signs of the slot's first 8 columns"""
+            label = (eb.get_dense_feature(inputs, ["feat0"], [8])[0] > 0).float()
+            return F.binary_cross_entropy_with_logits(self.out_fc(self.embed(inputs)), label)
+
+    return SupervisedSage()
+
+
 def run(args):
     import numpy as np
     import torch
     import euler_b200 as eb
     from euler_b200 import knowledge, optimizers, unsupervised as un
     torch.cuda.set_device(0)
-    kg = args.model != "deepwalk"
+    kg = args.model not in ("deepwalk", "sage")
+    sage = args.model == "sage"
     if kg:
         eb.set_graph(kg_graph(args.nodes, args.triples, args.relations), rng="philox", seed=1)
+    elif sage:
+        import shallow_encoder
+        shallow_encoder.torch = torch
+        shallow_encoder.build_graph(args)
     else:
         eb.set_graph(eb.Graph.rmat(args.nodes, args.edges, seed=11), rng="philox", seed=1)
     models = {}
     for name, dt in (("bf16", torch.bfloat16), ("f32", torch.float32)):
         torch.manual_seed(3)
-        if kg:
+        if sage:
+            models[name] = sage_model(args, dt)
+        elif kg:
             rel_dim = args.rel_dim if args.model == "transr" else args.dim
             models[name] = getattr(knowledge, KG_MODELS[args.model])(
                 0, 0, args.nodes - 1, args.relations - 1, args.dim, rel_dim, num_negs=args.negs, margin=1.0, l1=True,
@@ -102,6 +146,7 @@ def run(args):
     with torch.no_grad():
         for p16, p32 in zip(models["bf16"].parameters(), models["f32"].parameters()):
             p32.copy_(p16.float())
+    torch.cuda.empty_cache()
     opts = {k: optimizers.get(args.optimizer)(list(m.parameters()), args.lr, **({"seed": 5} if k == "bf16" else {}))
             for k, m in models.items()}
     if kg:   # the triples of each step, drawn once: both arms train on the same edges
@@ -116,6 +161,9 @@ def run(args):
 
     def step(k, i):
         eb.seed(1000 + i)
+        if sage:
+            losses[k].append(optimizers.minimize(opts[k], models[k](batches[i]), models[k]).detach())
+            return
         out = models[k].train_step(batches[i], opts[k])
         losses[k].append(out.loss if kg else out[0])
 
@@ -146,7 +194,7 @@ def run(args):
         i += n
 
     def state_bytes(k):
-        ps = list(models[k].parameters())
+        ps = [p for p in models[k].parameters() if p.dim() == 2 and p.shape[0] > 10 ** 5] if sage else list(models[k].parameters())
         return sum(p.numel() * p.element_size() for p in ps) + sum(
             t.numel() * t.element_size() for p in ps for t in opts[k].state[p].values() if torch.is_tensor(t))
 
@@ -154,6 +202,10 @@ def run(args):
         out = {"workload": "%s_train_step" % args.model, "entities": args.nodes, "triples": args.triples,
                "relations": args.relations, "dim": args.dim, "rel_dim": args.rel_dim if args.model == "transr" else args.dim,
                "batch": args.batch, "negs": args.negs, "optimizer": args.optimizer, "lr": args.lr, "gpu": gpu_info(0)}
+    elif sage:
+        out = {"workload": "supervised_sage_minimize_step", "nodes": args.nodes, "edges": args.edges, "dim": args.dim,
+               "fanout": [15, 10], "aggregator": "mean", "batch": args.batch, "optimizer": args.optimizer, "lr": args.lr,
+               "gpu": gpu_info(0)}
     else:
         out = {"workload": "deepwalk_train_step", "nodes": args.nodes, "edges": args.edges, "dim": args.dim, "batch": args.batch,
                "optimizer": args.optimizer, "gpu": gpu_info(0)}

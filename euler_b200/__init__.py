@@ -12,5 +12,5 @@ from .ops import (adjacency_mean, agnn_attention_aggregate, context, dna_attenti
                   get_binary_feature, get_multi_hop_neighbor, get_node_type, get_node_type_id, get_sorted_full_neighbor, get_sparse_feature, get_top_k_neighbor, initialize_embedded_graph, kg_margin_loss, kg_margin_loss_sparse_grads,
                   initialize_graph, neighbor_top_k_feature, random_walk, relation_mean_aggregate, sage_mean_aggregate, sample_fanout, sample_fanout_batched, sample_fanout_with_feature,
                   sample_edge, sample_neighbor, sample_neighbor_api, sample_neighbor_layerwise, sample_neighbor_layerwise_coo, sample_n_with_types, sample_node, sample_node_with_src, scatter_, scatter_add, scatter_max, scatter_mean,
-                  scatter_softmax, seed, set_graph, shallow_encode, shallow_encode_pool, skipgram_xent_loss, skipgram_xent_loss_sparse_grads, sparse_feature_embedding, sparse_get_adj, sparse_get_adj_coo, store_accumulate, store_exchange, unique)
+                  scatter_softmax, seed, set_graph, shallow_encode, shallow_encode_pool, skipgram_xent_loss, skipgram_xent_loss_sparse_grads, sparse_feature_embedding, sparse_get_adj, sparse_get_adj_coo, store_accumulate, store_exchange, table_proxy, unique)
 from . import optimizers  # noqa: F401,E402  (tf_euler.utils.optimizers: get, MomentumOptimizer, AdagradOptimizer, AdamOptimizer)

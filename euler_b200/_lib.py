@@ -200,10 +200,13 @@ SIGNATURES = {
     "eu_sparse_embedding_lookup": (C.c_int, [_P, _P, _I64, _I32, _I64, _P, _I64, _I32, _I32, _P]),
     "eu_sparse_embedding_lookup_backward": (C.c_int, [_P, _P, _P, _I64, _I32, _I64, _I64, _I32, _I32, _P]),
     "eu_sparse_embedding_lookup_backward_sparse": (C.c_int, [_P, _P, _P, _I64, _I32, _I64, _I64, _I32, _I32, _P, _P, _P]),
+    "eu_sparse_embedding_lookup_dtype": (C.c_int, [_P, _P, _I64, _I32, _I64, _P, _I64, _I32, _I32, _I32, _P]),
     "eu_shallow_encode": (C.c_int, [_P, _P, _P, _P]),
     "eu_shallow_encode_backward": (C.c_int, [_P, _P, _P, _P]),
     "eu_shallow_encode_backward_sparse": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "eu_shallow_encode_dtype": (C.c_int, [_P, _P, _I32, _P, _P]),
     "eu_shallow_encode_pool": (C.c_int, [_P, _P, _I32, _I32, _P]),
+    "eu_shallow_encode_pool_dtype": (C.c_int, [_P, _P, _I32, _I32, _I32, _P]),
     "eu_shallow_encode_pool_backward": (C.c_int, [_P, _P, _I32, _I32, _P, _P]),
     "eu_shallow_encode_pool_backward_sparse": (C.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P]),
     "eu_store_exchange": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _I64, _P, _P]),

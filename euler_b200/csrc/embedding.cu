@@ -16,9 +16,16 @@
 //   acc = table[v_0]; acc = __fadd_rn(acc, table[v_k]) for k = 1 .. n-1   (from the first row, not from +0)
 //   out_i = acc (sum), __fdiv_rn(acc, fl(n)) (mean), __fdiv_rn(acc, __fsqrt_rn(fl(n))) (sqrtn)
 // A group of G lanes per node: the bag's values are loaded G at a time, one per lane, and broadcast by shuffle; kEmbUnroll
-// table rows are loaded ahead of the ordered adds (emb_bag_sum, which both forward kernels call).  float4 loads when
-// dim % 4 == 0 and table / out are 16-byte aligned, scalar otherwise: the same adds in the same order, so the bits do not
-// depend on the alignment.  No scratch, no synchronisation: the forward is capturable in a CUDA graph.
+// table rows are loaded ahead of the ordered adds (emb_bag_sum, which both forward kernels call).  4-wide loads when
+// dim % 4 == 0, the table is aligned to four elements (16 bytes of f32, 8 of bf16) and out to 16 bytes, scalar otherwise:
+// the same adds in the same order, so the bits do not depend on the alignment.  No scratch, no synchronisation: the
+// forward is capturable in a CUDA graph.
+//
+// Tables are f32 or bf16 (E; all tables of one problem share it).  Only the forward kernels read a table, through feat_ld /
+// feat_ld4, which widen bf16 to f32 exactly; every other step is the f32 one, so a bf16 call gives the f32 call's bits on
+// the widened tables.  The backward never dereferences a table: emb_backward, k_emb_lengths, k_emb_entries,
+// k_emb_scale_grad and segment.cuh's distinct-row sums read grad_out, the graph's bags, n_rows and dim only, so one
+// backward serves both dtypes.
 //
 // Backward, grad_table[v] = sum over the entries (i, k) with v_k = v of s_i(g_i), where s_i is the identity (sum),
 // __fdiv_rn(., fl(n_i)) (mean) or __fdiv_rn(., __fsqrt_rn(fl(n_i))) (sqrtn), elementwise.  The entries of every table are
@@ -45,7 +52,7 @@ template <> struct EmbVec<true> {
   using T = float4;
   static constexpr int W = 4;
   static __device__ __forceinline__ T zero(float z) { return make_float4(z, z, z, z); }
-  static __device__ __forceinline__ T load(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+  template <typename E> static __device__ __forceinline__ T load(const E* p) { return feat_ld4<E>(p); }
   static __device__ __forceinline__ T load_rw(const float* p) { return *reinterpret_cast<const float4*>(p); }   // written by this kernel
   static __device__ __forceinline__ void store(float* p, T v) { *reinterpret_cast<float4*>(p) = v; }
   static __device__ __forceinline__ T add(T a, T b) {
@@ -59,7 +66,7 @@ template <> struct EmbVec<false> {
   using T = float;
   static constexpr int W = 1;
   static __device__ __forceinline__ T zero(float z) { return z; }
-  static __device__ __forceinline__ T load(const float* p) { return __ldg(p); }
+  template <typename E> static __device__ __forceinline__ T load(const E* p) { return feat_ld<E>(p); }
   static __device__ __forceinline__ T load_rw(const float* p) { return *p; }
   static __device__ __forceinline__ void store(float* p, T v) { *p = v; }
   static __device__ __forceinline__ T add(T a, T b) { return __fadd_rn(a, b); }
@@ -69,9 +76,9 @@ template <> struct EmbVec<false> {
 // This lane's columns [d, d + W) of the sum of the bag [b, e) of the uint64 values (empty: the one entry dflt), whole-group
 // call (every lane of the group takes part in the shuffles; act: d < dim, an inactive lane loads nothing).  The sum starts
 // from the bag's first row (its bits, -0.0 and NaN payloads included) and adds the others left to right.
-template <bool VEC>
+template <bool VEC, typename E>
 __device__ __forceinline__ typename EmbVec<VEC>::T emb_bag_tile(const DevGraph& g, int64_t b, int64_t e, unsigned long long dflt,
-                                                                const float* __restrict__ table, int dim, int d, bool act, int G,
+                                                                const E* __restrict__ table, int dim, int d, bool act, int G,
                                                                 int sub, unsigned gm) {
   using V = EmbVec<VEC>;
   const bool empty = e == b;
@@ -99,9 +106,9 @@ __device__ __forceinline__ typename EmbVec<VEC>::T emb_bag_tile(const DevGraph& 
 // group's mask gm), W columns per lane and step, blocks of G * W columns with a group-uniform trip count (emb_bag_tile).
 // *n = the bag's entries (1 for the default); it is set before the first sink(d, acc) call, which hands over the lane's
 // columns [d, d + W) of the sum, for d < dim only.
-template <bool VEC, typename Sink>
+template <bool VEC, typename E, typename Sink>
 __device__ __forceinline__ void emb_bag_sum(const DevGraph& g, int64_t row, int32_t fid, unsigned long long dflt,
-                                            const float* __restrict__ table, int dim, int G, int sub, unsigned gm, int64_t* n_out,
+                                            const E* __restrict__ table, int dim, int G, int sub, unsigned gm, int64_t* n_out,
                                             Sink sink) {
   using V = EmbVec<VEC>;
   int64_t b, e;
@@ -109,15 +116,15 @@ __device__ __forceinline__ void emb_bag_sum(const DevGraph& g, int64_t row, int3
   *n_out = e == b ? 1 : e - b;
   for (int d0 = 0; d0 < dim; d0 += G * V::W) {
     const int d = d0 + sub * V::W;
-    const typename V::T acc = emb_bag_tile<VEC>(g, b, e, dflt, table, dim, d, d < dim, G, sub, gm);
+    const typename V::T acc = emb_bag_tile<VEC, E>(g, b, e, dflt, table, dim, d, d < dim, G, sub, gm);
     if (d < dim) sink(d, acc);
   }
 }
 
 // G lanes per node r (a power of two)
-template <bool VEC>
+template <bool VEC, typename E>
 __global__ void __launch_bounds__(256, 1) k_emb_fwd(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t M, int32_t fid,
-                                                 unsigned long long dflt, const float* __restrict__ table, int dim, int G, int comb,
+                                                 unsigned long long dflt, const E* __restrict__ table, int dim, int G, int comb,
                                                  float* __restrict__ out) {
   using V = EmbVec<VEC>;
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -127,7 +134,7 @@ __global__ void __launch_bounds__(256, 1) k_emb_fwd(DevGraph g, const unsigned l
   const unsigned gm = group_mask(G);
   float* o = out + r * (int64_t)dim;
   int64_t n;
-  emb_bag_sum<VEC>(g, lookup_row(g, __ldg(nodes + r)), fid, dflt, table, dim, G, sub, gm, &n,
+  emb_bag_sum<VEC, E>(g, lookup_row(g, __ldg(nodes + r)), fid, dflt, table, dim, G, sub, gm, &n,
                    [&](int d, typename V::T acc) { V::store(o + d, acc); });
   if (comb == EU_COMBINE_SUM) return;
   // mean / sqrtn: one division per column, in a pass of its own over the row this group just wrote (L1-resident), so that
@@ -142,30 +149,30 @@ struct ShallowDev {   // eu_shallow_problem, resolved for the device: column off
   const unsigned long long* nodes;
   int64_t M;
   int W, add;                      // out's width; EU_SHALLOW_ADD
-  const float* id_table;
+  const void* id_table;            // every table of the problem: f32, or bf16 (the kernels' E)
   int64_t n_id_rows;
   int id_dim;
   int n_dense, dense_w;            // dense_w: dense_out's width (ADD)
   int32_t dense_fid[EU_SHALLOW_MAX_SLOTS];
   int dense_dim[EU_SHALLOW_MAX_SLOTS], dense_off[EU_SHALLOW_MAX_SLOTS];
   int n_sparse;
-  unsigned vec_mask;               // bit s: slot s's table and out columns take float4 loads and stores
+  unsigned vec_mask;               // bit s: slot s's table and out columns take 4-wide loads and float4 stores
   int32_t sp_fid[EU_SHALLOW_MAX_SLOTS];
   int sp_dim[EU_SHALLOW_MAX_SLOTS], sp_comb[EU_SHALLOW_MAX_SLOTS], sp_off[EU_SHALLOW_MAX_SLOTS];
   unsigned long long sp_dflt[EU_SHALLOW_MAX_SLOTS];
-  const float* sp_table[EU_SHALLOW_MAX_SLOTS];
+  const void* sp_table[EU_SHALLOW_MAX_SLOTS];
   float* out;
   float* dense_out;
 };
 
 // slot s of node row `row` into o (its first column): stored (CONCAT, or the first term of ADD) or added to what o holds
-template <bool VEC>
+template <bool VEC, typename E>
 __device__ __forceinline__ void shallow_slot(const DevGraph& g, const ShallowDev& p, int s, int64_t row, float* o, bool first, int G,
                                              int sub, unsigned gm) {
   using V = EmbVec<VEC>;
   const int comb = p.sp_comb[s];
   int64_t n;
-  emb_bag_sum<VEC>(g, row, p.sp_fid[s], p.sp_dflt[s], p.sp_table[s], p.sp_dim[s], G, sub, gm, &n, [&](int d, typename V::T acc) {
+  emb_bag_sum<VEC, E>(g, row, p.sp_fid[s], p.sp_dflt[s], static_cast<const E*>(p.sp_table[s]), p.sp_dim[s], G, sub, gm, &n, [&](int d, typename V::T acc) {
     if (comb != EU_COMBINE_SUM) acc = V::div(acc, emb_den(n, comb));
     V::store(o + d, first ? acc : V::add(V::load_rw(o + d), acc));
   });
@@ -173,8 +180,9 @@ __device__ __forceinline__ void shallow_slot(const DevGraph& g, const ShallowDev
 
 // G lanes per node r: the id columns, the dense slots (k_feature's rule: the stored columns, zeros past them, zeros for an
 // absent node or an unknown slot), then the sparse slots.  The group syncs between parts: a part may map columns to lanes
-// differently from the one before it, and ADD reads what the previous part wrote.  T: the dense table's storage type.
-template <typename T>
+// differently from the one before it, and ADD reads what the previous part wrote.  T: the dense table's storage type, E the
+// id and sparse tables'.
+template <typename T, typename E>
 __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, int G) {
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t r = tid >> (31 - __clz(G));
@@ -185,8 +193,8 @@ __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, i
   float* o = p.out + r * (int64_t)p.W;
   if (p.id_table) {
     const bool ok = (long long)id >= 0 && (long long)id < p.n_id_rows;   // false only under capture (the check is skipped)
-    const float* t = p.id_table + (ok ? (int64_t)id : 0) * p.id_dim;
-    for (int d = sub; d < p.id_dim; d += G) o[d] = ok ? __ldg(t + d) : __int_as_float(0x7fc00000);
+    const E* t = static_cast<const E*>(p.id_table) + (ok ? (int64_t)id : 0) * p.id_dim;
+    for (int d = sub; d < p.id_dim; d += G) o[d] = ok ? feat_ld<E>(t + d) : __int_as_float(0x7fc00000);
   }
   const int64_t row = lookup_row(g, id);
   float* od = p.add ? p.dense_out + r * (int64_t)p.dense_w : o;
@@ -202,8 +210,8 @@ __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, i
     __syncwarp(gm);
     const bool first = !p.add || (s == 0 && !p.id_table);
     float* os = o + p.sp_off[s];
-    if (p.vec_mask >> s & 1) shallow_slot<true>(g, p, s, row, os, first, G, sub, gm);
-    else shallow_slot<false>(g, p, s, row, os, first, G, sub, gm);
+    if (p.vec_mask >> s & 1) shallow_slot<true, E>(g, p, s, row, os, first, G, sub, gm);
+    else shallow_slot<false, E>(g, p, s, row, os, first, G, sub, gm);
   }
 }
 
@@ -226,7 +234,7 @@ __device__ __forceinline__ float pool_column(int count, Load load) {
 
 // slot s of the segment's nodes (their graph rows in `rows`), pooled into o (the slot's first column of the output row):
 // per tile of G * W columns, each node's bag sum and combiner division (shallow_slot's), added across the nodes in registers
-template <bool VEC>
+template <bool VEC, typename E>
 __device__ __forceinline__ void shallow_pool_slot(const DevGraph& g, const ShallowDev& p, int s, const int64_t* rows, int count,
                                                   float pool_den, float* o, int G, int sub, unsigned gm) {
   using V = EmbVec<VEC>;
@@ -237,7 +245,7 @@ __device__ __forceinline__ void shallow_pool_slot(const DevGraph& g, const Shall
     for (int j = 0; j < count; ++j) {
       int64_t b, e;
       ragged_slice(g.u64_ptr, g.n_u64_slots, rows[j], p.sp_fid[s], &b, &e);
-      typename V::T x = emb_bag_tile<VEC>(g, b, e, p.sp_dflt[s], p.sp_table[s], dim, d, d < dim, G, sub, gm);
+      typename V::T x = emb_bag_tile<VEC, E>(g, b, e, p.sp_dflt[s], static_cast<const E*>(p.sp_table[s]), dim, d, d < dim, G, sub, gm);
       if (comb != EU_COMBINE_SUM) x = V::div(x, emb_den(e == b ? 1 : e - b, comb));
       acc = j == 0 ? x : V::add(acc, x);
     }
@@ -249,7 +257,7 @@ __device__ __forceinline__ void shallow_pool_slot(const DevGraph& g, const Shall
 // G lanes per output row r, the pool of the `count` ShallowEncoder rows (CONCAT) of nodes[r * count ..]: k_shallow_fwd's
 // parts and rules, each column summed over the segment's nodes in a register, in node order, and divided once by pool_den
 // (fl(count); 0: the sum).  The group looks every node's graph row up once, into its `count` slots of shared memory.
-template <typename T>
+template <typename T, typename E>
 __global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev p, int count, float pool_den, int G) {
   extern __shared__ int64_t pool_rows[];
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -267,7 +275,7 @@ __global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev 
     o[d] = finish(pool_column(count, [&](int j) {
       const long long id = (long long)__ldg(nodes + j);
       const bool ok = id >= 0 && id < p.n_id_rows;   // false only under capture (the check is skipped)
-      return ok ? __ldg(p.id_table + id * p.id_dim + d) : __int_as_float(0x7fc00000);
+      return ok ? feat_ld<E>(static_cast<const E*>(p.id_table) + id * p.id_dim + d) : __int_as_float(0x7fc00000);
     }));
   for (int k = 0; k < p.n_dense; ++k) {
     const int32_t fid = p.dense_fid[k];
@@ -279,8 +287,8 @@ __global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev 
       oj[d] = finish(pool_column(count, [&](int j) { return d < sdim && rows[j] >= 0 ? feat_ld(f + rows[j] * (int64_t)g.feat_dim + d) : 0.f; }));
   }
   for (int s = 0; s < p.n_sparse; ++s) {
-    if (p.vec_mask >> s & 1) shallow_pool_slot<true>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
-    else shallow_pool_slot<false>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
+    if (p.vec_mask >> s & 1) shallow_pool_slot<true, E>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
+    else shallow_pool_slot<false, E>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
   }
 }
 
@@ -662,13 +670,15 @@ static int shallow_id_check(eu_ctx* c, const eu_shallow_problem* p, const char* 
   return EU_OK;
 }
 
-// the lane group of a row whose widest part has `widest` columns, and the slots that take float4 loads and stores
-static int shallow_lanes(ShallowDev* d, const float* out) {
+// the lane group of a row whose widest part has `widest` columns, and the slots that take 4-wide loads and float4 stores (a
+// table aligned to four elements of table_dtype, the output to 16 bytes)
+static int shallow_lanes(ShallowDev* d, const float* out, int table_dtype) {
   int widest = d->id_dim;
   for (int j = 0; j < d->n_dense; ++j) widest = std::max(widest, d->dense_dim[j]);
   for (int k = 0; k < d->n_sparse; ++k) {
     widest = std::max(widest, d->sp_dim[k]);
-    if (d->sp_dim[k] % 4 == 0 && aligned16(d->sp_table[k]) && aligned16(out) && d->W % 4 == 0 && d->sp_off[k] % 4 == 0) d->vec_mask |= 1u << k;
+    if (d->sp_dim[k] % 4 == 0 && aligned4_elems(d->sp_table[k], table_dtype) && aligned16(out) && d->W % 4 == 0 && d->sp_off[k] % 4 == 0)
+      d->vec_mask |= 1u << k;
   }
   return group_lanes(ceil_div(widest, 4));
 }
@@ -712,6 +722,107 @@ static int shallow_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const
   return EU_OK;
 }
 
+// EU_ERR_INVALID unless table_dtype is an eu_feat_dtype
+static int table_dtype_check(int32_t table_dtype, const char* who) {
+  if (table_dtype != EU_FEAT_F32 && table_dtype != EU_FEAT_BF16) {
+    set_error("%s: unknown table dtype %d (EU_FEAT_F32 or EU_FEAT_BF16)", who, (int)table_dtype);
+    return EU_ERR_INVALID;
+  }
+  return EU_OK;
+}
+
+// eu_sparse_embedding_lookup(_dtype)
+static int emb_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const void* table, int64_t n_rows,
+                      int32_t dim, int32_t combiner, int32_t table_dtype, float* out, const char* who) {
+  int rc = table_dtype_check(table_dtype, who);
+  if (rc || (rc = emb_check(c, nodes, M, fid, default_value, table != nullptr, n_rows, dim, combiner, out, who))) return rc;
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (M == 0) return EU_OK;
+  const bool vec = dim % 4 == 0 && aligned4_elems(table, table_dtype) && aligned16(out);
+  const int G = group_lanes(ceil_div(dim, vec ? 4 : 1));
+  const unsigned blocks = (unsigned)ceil_div(M * G, 256);
+  const auto* nd = (const unsigned long long*)nodes;
+  const auto dflt = (unsigned long long)default_value;
+  EuProfScope ps(c, "emb_fwd", M);
+  if (table_dtype == EU_FEAT_BF16) {
+    const auto* t = static_cast<const __nv_bfloat16*>(table);
+    if (vec) k_emb_fwd<true><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
+    else k_emb_fwd<false><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
+  } else {
+    const auto* t = static_cast<const float*>(table);
+    if (vec) k_emb_fwd<true><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
+    else k_emb_fwd<false><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
+  }
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+// eu_shallow_encode(_dtype)
+static int shallow_encode(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, float* out, float* dense_out, const char* who) {
+  ShallowDev d;
+  EmbTables T;
+  int rc = table_dtype_check(table_dtype, who);
+  if (rc || (rc = shallow_resolve(c, p, &d, &T, who))) return rc;
+  if (p->M > 0 && ((d.W > 0 && !out) || (d.add && d.dense_w > 0 && !dense_out))) {
+    set_error("%s: bad argument (out%s is required)", who, d.add ? " and dense_out" : "");
+    return EU_ERR_INVALID;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (p->M == 0 || (d.W == 0 && d.dense_w == 0)) return EU_OK;
+  if ((rc = shallow_id_check(c, p, who))) return rc;
+  d.out = out;
+  d.dense_out = dense_out;
+  const int G = shallow_lanes(&d, out, table_dtype);
+  EuProfScope ps(c, "shallow_fwd", p->M);
+  const unsigned blocks = (unsigned)ceil_div(p->M * G, 256);
+  const bool bf16_feat = c->g->d.feat_dtype == EU_FEAT_BF16;
+  if (table_dtype == EU_FEAT_BF16) {
+    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, __nv_bfloat16><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+    else k_shallow_fwd<float, __nv_bfloat16><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+  } else {
+    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, float><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+    else k_shallow_fwd<float, float><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+  }
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+// eu_shallow_encode_pool(_dtype)
+static int shallow_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, int32_t count, int32_t pool, float* out,
+                        const char* who) {
+  ShallowDev d;
+  EmbTables T;
+  GradRows gr;
+  int rc = table_dtype_check(table_dtype, who);
+  if (rc || (rc = shallow_resolve(c, p, &d, &T, who)) || (rc = pool_check(p, count, pool, &gr, who))) return rc;
+  if (p->M > 0 && d.W > 0 && !out) {
+    set_error("%s: bad argument (out is required)", who);
+    return EU_ERR_INVALID;
+  }
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (p->M == 0 || d.W == 0) return EU_OK;
+  if ((rc = shallow_id_check(c, p, who))) return rc;
+  d.out = out;
+  // the group's graph rows live in shared memory: wider groups until a block's fit in the default 48 KB
+  int G = shallow_lanes(&d, out, table_dtype);
+  while ((256 / G) * (size_t)count * sizeof(int64_t) > 48 * 1024) G *= 2;
+  const int64_t R = p->M / count;
+  EuProfScope ps(c, "shallow_pool", p->M);
+  const unsigned blocks = (unsigned)ceil_div(R * G, 256);
+  const size_t smem = (256 / G) * (size_t)count * sizeof(int64_t);
+  const bool bf16_feat = c->g->d.feat_dtype == EU_FEAT_BF16;
+  cudaStream_t s = c->stream;
+  if (table_dtype == EU_FEAT_BF16) {
+    if (bf16_feat) k_shallow_pool<__nv_bfloat16, __nv_bfloat16><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
+    else k_shallow_pool<float, __nv_bfloat16><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
+  } else {
+    if (bf16_feat) k_shallow_pool<__nv_bfloat16, float><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
+    else k_shallow_pool<float, float><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
+  }
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
 }  // namespace eu
 
 using namespace eu;
@@ -720,21 +831,12 @@ extern "C" {
 
 int eu_sparse_embedding_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const float* table,
                                int64_t n_rows, int32_t dim, int32_t combiner, float* out) {
-  const char* who = "eu_sparse_embedding_lookup";
-  int rc = emb_check(c, nodes, M, fid, default_value, table != nullptr, n_rows, dim, combiner, out, who);
-  if (rc) return rc;
-  EU_CUDA(cudaSetDevice(c->g->device));
-  if (M == 0) return EU_OK;
-  const bool vec = dim % 4 == 0 && aligned16(table) && aligned16(out);
-  const int G = group_lanes(ceil_div(dim, vec ? 4 : 1));
-  const unsigned blocks = (unsigned)ceil_div(M * G, 256);
-  EuProfScope ps(c, "emb_fwd", M);
-  if (vec) k_emb_fwd<true><<<blocks, 256, 0, c->stream>>>(c->g->d, (const unsigned long long*)nodes, M, fid, (unsigned long long)default_value,
-                                                          table, dim, G, combiner, out);
-  else k_emb_fwd<false><<<blocks, 256, 0, c->stream>>>(c->g->d, (const unsigned long long*)nodes, M, fid, (unsigned long long)default_value,
-                                                       table, dim, G, combiner, out);
-  EU_LAUNCHED();
-  return EU_OK;
+  return emb_lookup(c, nodes, M, fid, default_value, table, n_rows, dim, combiner, EU_FEAT_F32, out, "eu_sparse_embedding_lookup");
+}
+
+int eu_sparse_embedding_lookup_dtype(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const void* table,
+                                     int64_t n_rows, int32_t dim, int32_t combiner, int32_t table_dtype, float* out) {
+  return emb_lookup(c, nodes, M, fid, default_value, table, n_rows, dim, combiner, table_dtype, out, "eu_sparse_embedding_lookup_dtype");
 }
 
 int eu_sparse_embedding_lookup_backward(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
@@ -755,27 +857,11 @@ int eu_sparse_embedding_lookup_backward_sparse(eu_ctx* c, const float* grad_out,
 }
 
 int eu_shallow_encode(eu_ctx* c, const eu_shallow_problem* p, float* out, float* dense_out) {
-  const char* who = "eu_shallow_encode";
-  ShallowDev d;
-  EmbTables T;
-  int rc = shallow_resolve(c, p, &d, &T, who);
-  if (rc) return rc;
-  if (p->M > 0 && ((d.W > 0 && !out) || (d.add && d.dense_w > 0 && !dense_out))) {
-    set_error("%s: bad argument (out%s is required)", who, d.add ? " and dense_out" : "");
-    return EU_ERR_INVALID;
-  }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  if (p->M == 0 || (d.W == 0 && d.dense_w == 0)) return EU_OK;
-  if ((rc = shallow_id_check(c, p, who))) return rc;
-  d.out = out;
-  d.dense_out = dense_out;
-  const int G = shallow_lanes(&d, out);
-  EuProfScope ps(c, "shallow_fwd", p->M);
-  const unsigned blocks = (unsigned)ceil_div(p->M * G, 256);
-  if (c->g->d.feat_dtype == EU_FEAT_BF16) k_shallow_fwd<__nv_bfloat16><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-  else k_shallow_fwd<float><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-  EU_LAUNCHED();
-  return EU_OK;
+  return shallow_encode(c, p, EU_FEAT_F32, out, dense_out, "eu_shallow_encode");
+}
+
+int eu_shallow_encode_dtype(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, float* out, float* dense_out) {
+  return shallow_encode(c, p, table_dtype, out, dense_out, "eu_shallow_encode_dtype");
 }
 
 int eu_shallow_encode_backward(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, float* const* grads) {
@@ -798,31 +884,11 @@ int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, co
 }
 
 int eu_shallow_encode_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, float* out) {
-  const char* who = "eu_shallow_encode_pool";
-  ShallowDev d;
-  EmbTables T;
-  GradRows gr;
-  int rc = shallow_resolve(c, p, &d, &T, who);
-  if (rc || (rc = pool_check(p, count, pool, &gr, who))) return rc;
-  if (p->M > 0 && d.W > 0 && !out) {
-    set_error("%s: bad argument (out is required)", who);
-    return EU_ERR_INVALID;
-  }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  if (p->M == 0 || d.W == 0) return EU_OK;
-  if ((rc = shallow_id_check(c, p, who))) return rc;
-  d.out = out;
-  // the group's graph rows live in shared memory: wider groups until a block's fit in the default 48 KB
-  int G = shallow_lanes(&d, out);
-  while ((256 / G) * (size_t)count * sizeof(int64_t) > 48 * 1024) G *= 2;
-  const int64_t R = p->M / count;
-  EuProfScope ps(c, "shallow_pool", p->M);
-  const unsigned blocks = (unsigned)ceil_div(R * G, 256);
-  const size_t smem = (256 / G) * (size_t)count * sizeof(int64_t);
-  if (c->g->d.feat_dtype == EU_FEAT_BF16) k_shallow_pool<__nv_bfloat16><<<blocks, 256, smem, c->stream>>>(c->g->d, d, count, gr.pool_den, G);
-  else k_shallow_pool<float><<<blocks, 256, smem, c->stream>>>(c->g->d, d, count, gr.pool_den, G);
-  EU_LAUNCHED();
-  return EU_OK;
+  return shallow_pool(c, p, EU_FEAT_F32, count, pool, out, "eu_shallow_encode_pool");
+}
+
+int eu_shallow_encode_pool_dtype(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, int32_t count, int32_t pool, float* out) {
+  return shallow_pool(c, p, table_dtype, count, pool, out, "eu_shallow_encode_pool_dtype");
 }
 
 int eu_shallow_encode_pool_backward(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, const float* grad_out,

@@ -22,7 +22,7 @@ import torch.nn.functional as F
 
 from . import _lib, ops
 from .ops import sparse_feature_embedding
-from .unsupervised import Embedding
+from .unsupervised import Embedding, check_table_dtype
 
 
 def _truncated_normal_(t, stddev):
@@ -38,14 +38,19 @@ class SparseEmbedding(torch.nn.Module):
     __call__(sparse) takes the (indices, values, dense_shape) triple ops.get_sparse_feature returns and restates
     tf.nn.embedding_lookup_sparse(table, sp_ids, None, combiner) in torch: the reference path, composed of a gather and a
     segment sum.  lookup(nodes, feature_name, default_value) goes from node ids to the same rows in one fused device op
-    (ops.sparse_feature_embedding)."""
+    (ops.sparse_feature_embedding).  dtype=torch.bfloat16 initialises the table in f32 and rounds it once to nearest; such a
+    table takes no autograd gradient (ShallowEncoder trains it through a proxy)."""
 
-    def __init__(self, max_id, dim, combiner='sum', device=None):
+    def __init__(self, max_id, dim, combiner='sum', device=None, dtype=torch.float32):
         super().__init__()
         if combiner not in ('sum', 'mean', 'sqrtn'):
             raise ValueError("combiner must be 'sum', 'mean' or 'sqrtn'")
         self.combiner = combiner
-        self.embeddings = torch.nn.Parameter(_truncated_normal_(torch.empty(max_id + 1, dim, device=device), 0.0002))
+        table = _truncated_normal_(torch.empty(max_id + 1, dim, device=device), 0.0002)
+        if dtype == torch.float32:
+            self.embeddings = torch.nn.Parameter(table)
+        else:
+            self.embeddings = torch.nn.Parameter(table.to(dtype), requires_grad=False)
 
     def forward(self, sparse):
         indices, values, dense_shape = sparse
@@ -97,11 +102,19 @@ class ShallowEncoder(torch.nn.Module):
     exactly as the composition does; 'add' computes (id + sparse_0 + ..) + Dense(features), which differs from upstream's
     add_n order id + Dense(features) + sparse_0 + .. only in float rounding.  sparse_grad=True gives the tables coalesced
     sparse COO gradients (use an optimizer that takes them, e.g. torch.optim.SGD or SparseAdam).  fused=False runs the literal
-    composition: Embedding, get_dense_feature, get_sparse_feature + SparseEmbedding.__call__, then cat or add_n."""
+    composition: Embedding, get_dense_feature, get_sparse_feature + SparseEmbedding.__call__, then cat or add_n.
+
+    table_dtype=torch.bfloat16 (fused only) stores the id table and every SparseEmbedding table in bfloat16, initialised in
+    f32 and rounded once to nearest: half the HBM, and the optimizer keeps its slots in bf16 too.  The rows are the f32
+    op's on the widened tables.  A bf16 table takes no autograd gradient; each has a proxy (ops.table_proxy, not a
+    parameter and not in the state_dict) that receives its f32 sparse gradient, and optimizers.minimize hands those to
+    the optimizer in the same step as the dense parameters."""
 
     def __init__(self, dim=None, feature_idx='f1', feature_dim=0, max_id=-1, sparse_feature_idx=-1, sparse_feature_max_id=-1,
-                 embedding_dim=16, use_hash_embedding=False, combiner='concat', fused=True, sparse_grad=False, device=None):
+                 embedding_dim=16, use_hash_embedding=False, combiner='concat', fused=True, sparse_grad=False, device=None,
+                 table_dtype=torch.float32):
         super().__init__()
+        check_table_dtype(table_dtype, fused)
         if combiner not in ['add', 'concat']:
             raise ValueError('combiner must be \'add\' or \'concat\'.')
         if combiner == 'add' and dim is None:
@@ -151,13 +164,15 @@ class ShallowEncoder(torch.nn.Module):
         self.embedding_dim = embedding_dim
         self.fused = fused
         self.sparse_grad = sparse_grad
+        self.table_dtype = table_dtype
+        self._proxies = {}   # table index (0: id, 1 + s: slot s) -> its proxy; plain attributes, not module state
 
         dims = list(embedding_dim) if embedding_num else []
         if use_id:
-            self.embedding = Embedding(max_id + 1, dims.pop(0), device=device)
+            self.embedding = Embedding(max_id + 1, dims.pop(0), device=device, dtype=table_dtype)
         if use_sparse_feature:
             self.sparse_embeddings = torch.nn.ModuleList(
-                [SparseEmbedding(m + 1, d, device=device) for m, d in zip(sparse_feature_max_id, dims)])
+                [SparseEmbedding(m + 1, d, device=device, dtype=table_dtype) for m, d in zip(sparse_feature_max_id, dims)])
         if dim:
             feat_w = sum(feature_dim) if use_feature else 0
             in_dim = feat_w if combiner == 'add' else feat_w + (sum(embedding_dim) if embedding_num else 0)
@@ -184,12 +199,29 @@ class ShallowEncoder(torch.nn.Module):
         return out.reshape(shape + (self.output_dim,))
 
     def _op_inputs(self):
-        """(id_table, dense, sparse) as ops.shallow_encode takes them"""
+        """(id_table, dense, sparse, proxies) as ops.shallow_encode takes them"""
         id_table = self.embedding.embeddings if self.use_id else None
         dense = list(zip(self.feature_idx, self.feature_dim)) if self.use_feature else []
         sparse = [(name, e.embeddings, dv, e.combiner) for name, e, dv in
                   zip(self.sparse_feature_idx, self.sparse_embeddings, self._default_values())] if self.use_sparse_feature else []
-        return id_table, dense, sparse
+        return id_table, dense, sparse, self._proxy_list([id_table] + [s[1] for s in sparse])
+
+    def _proxy_list(self, tables):
+        """one proxy per table (None for an absent or f32 table), made on the table's device at first use"""
+        out = []
+        for t, table in enumerate(tables):
+            q = None
+            if table is not None and table.dtype == torch.bfloat16:
+                q = self._proxies.get(t)
+                if q is None or q.device != table.device or tuple(q.shape) != tuple(table.shape):
+                    q = self._proxies[t] = ops.table_proxy(table)
+            out.append(q)
+        return out
+
+    def table_proxies(self):
+        """[(table, proxy)] of every bfloat16 table: what optimizers.minimize steps"""
+        id_table, _, sparse, proxies = self._op_inputs()
+        return [(t, q) for t, q in zip([id_table] + [s[1] for s in sparse], proxies) if q is not None]
 
     @property
     def poolable(self):
@@ -199,15 +231,15 @@ class ShallowEncoder(torch.nn.Module):
     def pooled(self, nodes, count, pool):
         """the 'sum' or 'mean' of this encoder's rows over consecutive segments of `count` nodes, f32[nodes.numel() / count,
         output_dim], in one device op that never writes the rows (ops.shallow_encode_pool); needs poolable"""
-        id_table, dense, sparse = self._op_inputs()
-        return ops.shallow_encode_pool(nodes, count, id_table, dense, sparse, pool, self.sparse_grad)
+        id_table, dense, sparse, proxies = self._op_inputs()
+        return ops.shallow_encode_pool(nodes, count, id_table, dense, sparse, pool, self.sparse_grad, proxies)
 
     def _fused(self, nodes):
-        id_table, dense, sparse = self._op_inputs()
+        id_table, dense, sparse, proxies = self._op_inputs()
         if self.combiner == 'concat':
-            emb = ops.shallow_encode(nodes, id_table, dense, sparse, 'concat', self.sparse_grad)
+            emb = ops.shallow_encode(nodes, id_table, dense, sparse, 'concat', self.sparse_grad, proxies)
             return self.dense(emb) if self.dim else emb
-        emb, feats = ops.shallow_encode(nodes, id_table, dense, sparse, 'add', self.sparse_grad)
+        emb, feats = ops.shallow_encode(nodes, id_table, dense, sparse, 'add', self.sparse_grad, proxies)
         if feats is None:
             return emb
         feats = self.dense(feats)
@@ -244,7 +276,8 @@ class SageEncoder(torch.nn.Module):
     node encoder can pool (ShallowEncoder.poolable, and a fanout within the op's bound): the aggregator then receives
     ops.shallow_encode_pool's [n, W] rows and the [n * fanout, W] matrix is never written, forward or backward.  Every other
     combination takes the composition.  fused=False is the literal composition everywhere: the node encoder's composed path
-    per hop, then upstream's layer / hop loop.  sparse_grad=True gives the node encoder's tables sparse COO gradients."""
+    per hop, then upstream's layer / hop loop.  sparse_grad=True gives the node encoder's tables sparse COO gradients.
+    table_dtype is the node encoder's (ShallowEncoder; bfloat16 trains with optimizers.minimize)."""
 
     @staticmethod
     def create_aggregators(in_dim, dim, num_layers, aggregator, **kwargs):
@@ -258,7 +291,7 @@ class SageEncoder(torch.nn.Module):
     def __init__(self, metapath, fanouts, dim, aggregator='mean', concat=False, shared_aggregators=None, feature_idx=-1,
                  feature_dim=0, max_id=-1, use_feature=None, use_id=None, sparse_feature_idx=-1, sparse_feature_max_id=-1,
                  embedding_dim=16, use_hash_embedding=False, use_residual=False, shared_node_encoder=None, fused=True,
-                 sparse_grad=False, device=None):
+                 sparse_grad=False, device=None, table_dtype=torch.float32):
         super().__init__()
         if len(metapath) != len(fanouts):
             raise ValueError('Len of metapath must be the same as fanouts.')
@@ -273,7 +306,8 @@ class SageEncoder(torch.nn.Module):
             self._node_encoder = ShallowEncoder(
                 feature_idx=feature_idx, feature_dim=feature_dim, max_id=max_id if use_id else -1,
                 sparse_feature_idx=sparse_feature_idx, sparse_feature_max_id=sparse_feature_max_id, embedding_dim=embedding_dim,
-                use_hash_embedding=use_hash_embedding, fused=fused, sparse_grad=sparse_grad, device=device)
+                use_hash_embedding=use_hash_embedding, fused=fused, sparse_grad=sparse_grad, device=device,
+                table_dtype=table_dtype)
         self.dims = [self._node_encoder.output_dim] + [dim] * self.num_layers
         if shared_aggregators is not None:
             self.aggregators = shared_aggregators
@@ -348,11 +382,12 @@ class GCNEncoder(torch.nn.Module):
 
     fused=True (the default) gives the aggregators their device paths (sparse_aggregators: ops.adjacency_mean for 'gcn' /
     'mean', ops.gat_attention_aggregate for 'attention') and the node encoder its fused op; fused=False is the literal
-    composition everywhere.  sparse_grad=True gives the node encoder's tables sparse COO gradients."""
+    composition everywhere.  sparse_grad=True gives the node encoder's tables sparse COO gradients.  table_dtype is the node
+    encoder's (ShallowEncoder; bfloat16 trains with optimizers.minimize, and infer reads the bf16 tables as they are)."""
 
     def __init__(self, metapath, dim, aggregator='mean', feature_idx=-1, feature_dim=0, max_id=-1, use_id=False,
                  sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
-                 use_residual=False, head_num=4, fused=True, sparse_grad=False, device=None):
+                 use_residual=False, head_num=4, fused=True, sparse_grad=False, device=None, table_dtype=torch.float32):
         super().__init__()
         from . import sparse_aggregators
         self.metapath = metapath
@@ -370,7 +405,7 @@ class GCNEncoder(torch.nn.Module):
             dim=dim if use_residual else None, feature_idx=feature_idx, feature_dim=feature_dim,
             max_id=max_id if use_id else -1, sparse_feature_idx=sparse_feature_idx, sparse_feature_max_id=sparse_feature_max_id,
             embedding_dim=embedding_dim, use_hash_embedding=use_hash_embedding, combiner='add' if use_residual else 'concat',
-            fused=fused, sparse_grad=sparse_grad, device=device)
+            fused=fused, sparse_grad=sparse_grad, device=device, table_dtype=table_dtype)
         aggregator_class = sparse_aggregators.get(aggregator)
         self.dims = [self._node_encoder.output_dim]
         aggs = []
@@ -547,10 +582,10 @@ class GenieEncoder(GCNEncoder):
 
     def __init__(self, metapath, dim, aggregator='attention', feature_idx=-1, feature_dim=0, max_id=-1, use_id=False,
                  sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
-                 use_residual=False, head_num=4, fused=True, sparse_grad=False, device=None):
+                 use_residual=False, head_num=4, fused=True, sparse_grad=False, device=None, table_dtype=torch.float32):
         super().__init__(metapath, dim, aggregator, feature_idx, feature_dim, max_id, use_id, sparse_feature_idx,
                          sparse_feature_max_id, embedding_dim, use_hash_embedding, use_residual, head_num, fused=fused,
-                         sparse_grad=sparse_grad, device=device)
+                         sparse_grad=sparse_grad, device=device, table_dtype=table_dtype)
         from .graph_pool import LSTMCell
         self.dim = dim
         self.depth_fc = torch.nn.ModuleList([Dense(d, dim, use_bias=True, device=device) for d in self.dims])
@@ -593,6 +628,12 @@ def _exchange_composed(store, grad_store, ids, rows):
     store.index_put_((keys,), rows.detach()[torch.as_tensor(list(last.values()), dtype=torch.int64, device=store.device)])
     grad_store.index_put_((keys,), torch.zeros((), dtype=grad_store.dtype, device=grad_store.device))
     return taken
+
+
+def _scalable_f32(table_dtype):
+    """the scalable encoders train their stores and node-encoder tables in f32 only (train_step steps them through .grad)"""
+    if table_dtype != torch.float32:
+        raise ValueError("the scalable encoders train float32 tables only, got table_dtype=%r" % (table_dtype,))
 
 
 class _ScalableStores(torch.nn.Module):
@@ -712,7 +753,8 @@ class ScalableSageEncoder(SageEncoder, _ScalableStores):
                  feature_idx=-1, feature_dim=0, max_id=-1, use_feature=True, use_id=False, sparse_feature_idx=-1,
                  sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False, shared_node_encoder=None,
                  use_residual=False, store_learning_rate=0.001, store_init_maxval=0.05, fused=True, sparse_grad=False,
-                 device=None, generator=None):
+                 device=None, generator=None, table_dtype=torch.float32):
+        _scalable_f32(table_dtype)
         super().__init__([edge_type] * num_layers, [fanout] * num_layers, dim, aggregator, concat, shared_aggregators,
                          feature_idx, feature_dim, max_id, use_feature, use_id, sparse_feature_idx, sparse_feature_max_id,
                          embedding_dim, use_hash_embedding, use_residual=use_residual,
@@ -766,7 +808,8 @@ class ScalableGCNEncoder(GCNEncoder, _ScalableStores):
     def __init__(self, edge_type, num_layers, dim, aggregator='mean', feature_idx=-1, feature_dim=0, max_id=-1, use_id=False,
                  sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
                  use_residual=False, store_learning_rate=0.001, store_init_maxval=0.05, head_num=4, fused=True,
-                 sparse_grad=False, device=None, generator=None):
+                 sparse_grad=False, device=None, generator=None, table_dtype=torch.float32):
+        _scalable_f32(table_dtype)
         super().__init__([edge_type] * num_layers, dim, aggregator, feature_idx, feature_dim, max_id, use_id,
                          sparse_feature_idx, sparse_feature_max_id, embedding_dim, use_hash_embedding, use_residual,
                          head_num, fused=fused, sparse_grad=sparse_grad, device=device)

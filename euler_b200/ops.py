@@ -1174,28 +1174,69 @@ def _shape(table):
     return None if table is None else tuple(table.shape)
 
 
+def table_proxy(table):
+    """The gradient proxy of a bfloat16 table: a float32 leaf of the table's shape that requires grad and owns no [n_rows, dim]
+    storage (one element, strides 0).  Given to sparse_feature_embedding, shallow_encode or shallow_encode_pool in the
+    table's place, it receives the table's f32 gradient as a sparse COO tensor in .grad, summed over every use in the graph
+    as autograd sums a sparse_grad=True table's; optimizers.minimize hands it to the optimizer, never rounded to bf16."""
+    return torch.zeros(1, dtype=torch.float32, device=table.device).as_strided(tuple(table.shape), (0, 0)).requires_grad_()
+
+
+def _check_tables(op, named, proxies=None):
+    """the storage dtype of the embedding tables named [(name, table)] (None entries skipped): raise unless all are 2-D
+    float32 or bfloat16 tensors of one dtype, no bf16 table requires grad, and proxies (None, or one entry per named table:
+    None or a gradient proxy) gives proxies to bf16 tables only, each a float32 leaf of its table's shape that requires grad"""
+    present = [(nm, t) for nm, t in named if t is not None]
+    for nm, t in present:
+        if not torch.is_tensor(t) or t.dtype not in _TABLE_DTYPES or t.dim() != 2:
+            raise EulerError("%s: %s must be a 2-D float32 or bfloat16 tensor" % (op, nm))
+    dtypes = {t.dtype for _, t in present}
+    if len(dtypes) > 1:
+        raise EulerError("%s: the tables must have one dtype, got %s" % (op, [str(t.dtype) for _, t in present]))
+    dt = dtypes.pop() if dtypes else torch.float32
+    if dt == torch.bfloat16 and any(t.requires_grad for _, t in present):
+        raise EulerError("%s: a bfloat16 table takes no autograd gradient (torch would round it to bf16); give it a gradient "
+                         "proxy (table_proxy) and train it with optimizers.minimize" % op)
+    proxies = [None] * len(named) if proxies is None else list(proxies)
+    if len(proxies) != len(named):
+        raise EulerError("%s: proxies needs one entry per table (%d), got %d" % (op, len(named), len(proxies)))
+    for (nm, t), q in zip(named, proxies):
+        if q is None:
+            continue
+        if t is None or t.dtype != torch.bfloat16:
+            raise EulerError("%s: a gradient proxy stands in for a bfloat16 table only (%s)" % (op, nm))
+        if not torch.is_tensor(q) or q.dtype != torch.float32 or tuple(q.shape) != tuple(t.shape) or not q.requires_grad \
+                or q.device != t.device:
+            raise EulerError("%s: the proxy of %s must be a float32 tensor of the table's shape %s on its device that requires "
+                             "grad" % (op, nm, tuple(t.shape)))
+    return dt, proxies
+
+
 # ------------------------------------------------------------------------------------ sparse-feature embedding
 _COMBINERS = {"sum": 0, "mean": 1, "sqrtn": 2}
 
 
 def _raw_embedding(nodes, fid, table, default_value, comb):
-    """one eu_sparse_embedding_lookup: out f32[M, dim]"""
+    """one eu_sparse_embedding_lookup (eu_sparse_embedding_lookup_dtype for a bf16 table): out f32[M, dim]"""
     n_rows, dim = table.shape
     out = torch.empty((nodes.numel(), dim), dtype=torch.float32, device=table.device)
-    _call("eu_sparse_embedding_lookup", nodes, nodes.numel(), fid, default_value, table, n_rows, dim, comb, out)
+    if table.dtype == torch.bfloat16:
+        _call("eu_sparse_embedding_lookup_dtype", nodes, nodes.numel(), fid, default_value, table, n_rows, dim, comb, 1, out)
+    else:
+        _call("eu_sparse_embedding_lookup", nodes, nodes.numel(), fid, default_value, table, n_rows, dim, comb, out)
     return out
 
 
 class _SparseEmbedding(torch.autograd.Function):
     """eu_sparse_embedding_lookup / eu_sparse_embedding_lookup_backward.  Saves only the node ids: the backward pass lists the
-    entries again from the graph."""
+    entries again from the graph.  The gradient goes to the table, or to its proxy when one is given (then sparse)."""
 
     @staticmethod
-    def forward(ctx, table, nodes, fid, default_value, comb, sparse_grad):
+    def forward(ctx, table, proxy, nodes, fid, default_value, comb, sparse_grad):
         out = _raw_embedding(nodes, fid, table, default_value, comb)
-        if ctx.needs_input_grad[0]:
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
             ctx.save_for_backward(nodes)
-        ctx.args = (fid, default_value, comb, table.shape, sparse_grad)
+        ctx.args = (fid, default_value, comb, table.shape, sparse_grad or proxy is not None)
         return out
 
     @staticmethod
@@ -1207,11 +1248,12 @@ class _SparseEmbedding(torch.autograd.Function):
         if not sparse_grad:
             g_t = torch.empty((n_rows, dim), dtype=torch.float32, device=grad.device)
             _call("eu_sparse_embedding_lookup_backward", *args, g_t)
-            return g_t, None, None, None, None, None
+            return g_t, None, None, None, None, None, None
         rows, vals = _coo_buffers(_sparse_entries(nodes, fid), (n_rows, dim), grad.device)
         n = C.c_int64()
         _call("eu_sparse_embedding_lookup_backward_sparse", *args, rows, vals, C.byref(n))
-        return _coo(rows, vals, n.value, (n_rows, dim)), None, None, None, None, None
+        g_t = _coo(rows, vals, n.value, (n_rows, dim))
+        return ((None, g_t) if ctx.needs_input_grad[1] else (g_t, None)) + (None,) * 5
 
 
 def _sparse_entries(nodes, fid):
@@ -1220,7 +1262,7 @@ def _sparse_entries(nodes, fid):
     return _ragged_lengths("eu_get_sparse_feature", nodes.numel(), nodes, nodes.numel(), int(fid), 0)[1]
 
 
-def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner='sum', sparse_grad=False):
+def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner='sum', sparse_grad=False, proxy=None):
     """SparseEmbedding over get_sparse_feature in one fused device op: row i is tf.nn.embedding_lookup_sparse(table, sp_ids,
     None, combiner) (layers.py:152-169) of the SparseTensor get_sparse_feature(nodes, [feature_name], [default_value]) returns,
     i.e. the rows of table f32[n_rows, dim] named by node i's uint64 values of the slot, in stored order, or the one row
@@ -1229,13 +1271,16 @@ def sparse_feature_embedding(nodes, feature_name, table, default_value, combiner
     the call raises otherwise, before any device work.  The gradient reaches table only (deterministic, no atomics): a dense
     f32[n_rows, dim] gradient, or, with sparse_grad=True, a coalesced sparse COO gradient of the rows the batch touches (as
     nn.Embedding(sparse=True) gives), the same values without an [n_rows, dim] buffer.  The forward does not synchronise; the
-    backward synchronises once (dense) or three times (sparse: sizing the COO, the entry count, the row count)."""
+    backward synchronises once (dense) or three times (sparse: sizing the COO, the entry count, the row count).
+    A bfloat16 table is read widened exactly to f32, so the output is the f32 op's on the widened table.  It takes no
+    gradient itself (one that requires grad raises); its gradient goes to `proxy` (table_proxy), a float32 leaf of the
+    table's shape, as the coalesced f32 sparse COO gradient the f32 table gets with sparse_grad=True."""
     if combiner not in _COMBINERS:
         raise EulerError("sparse_feature_embedding: combiner must be one of %s, got %r" % (sorted(_COMBINERS), combiner))
-    _check_f32("sparse_feature_embedding", (("table", table),), 2)
+    dt, (proxy,) = _check_tables("sparse_feature_embedding", [("table", table)], [proxy])
     fid = _slot(feature_name, get_graph().sparse_feature_id)
     nodes = _t(nodes, torch.int64).reshape(-1)
-    return _SparseEmbedding.apply(_t(table, torch.float32), nodes, fid, int(default_value), _COMBINERS[combiner], bool(sparse_grad))
+    return _SparseEmbedding.apply(_t(table, dt), proxy, nodes, fid, int(default_value), _COMBINERS[combiner], bool(sparse_grad))
 
 
 # ------------------------------------------------------------------------------------ ShallowEncoder's input row
@@ -1255,18 +1300,21 @@ def _shallow_problem(nodes, id_table, dense, sparse, comb):
         q = p.sparse[k]
         q.fid, q.dim, q.combiner, q.default_value = fid, table.shape[1], c, default
         q.n_rows, q.table = table.shape[0], table.data_ptr()
+    first = id_table if id_table is not None else (sparse[0][1] if sparse else None)
+    p.table_dtype = _TABLE_DTYPES[first.dtype] if first is not None else 0
     return p
 
 
-def _shallow_inputs(who, nodes, id_table, dense, sparse, comb, sparse_grad):
-    """shallow_encode's arguments checked and resolved: (nodes i64[M], _ShallowEncode's cfg, the id table, the slots' tables)"""
+def _shallow_inputs(who, nodes, id_table, dense, sparse, comb, sparse_grad, proxies):
+    """shallow_encode's arguments checked and resolved: (nodes i64[M], _ShallowEncode's cfg, the id table, the slots'
+    tables, the proxies in the table order (id table, slots): one per table, None where a table has none)"""
     g = get_graph()
     dense, sparse = list(dense), list(sparse)
     if len(dense) > _lib.SHALLOW_MAX_SLOTS or len(sparse) > _lib.SHALLOW_MAX_SLOTS:
         raise EulerError("%s: at most %d dense and %d sparse slots" % (who, _lib.SHALLOW_MAX_SLOTS, _lib.SHALLOW_MAX_SLOTS))
     tables = ([id_table] if id_table is not None else []) + [s[1] for s in sparse]
-    named = [("sparse table %d" % k, s[1]) for k, s in enumerate(sparse)]
-    _check_f32(who, ([("id_table", id_table)] if id_table is not None else []) + named, 2)
+    named = [("id_table", id_table)] + [("sparse table %d" % k, s[1]) for k, s in enumerate(sparse)]
+    dt, proxies = _check_tables(who, named, proxies)
     d_cfg = tuple((_slot(n, g.dense_feature_id), int(d)) for n, d in dense)
     s_cfg = []
     for s in sparse:
@@ -1281,9 +1329,27 @@ def _shallow_inputs(who, nodes, id_table, dense, sparse, comb, sparse_grad):
     dense_w = sum(d for _, d in d_cfg)
     W = (emb_dims[0] if emb_dims else 0) if comb == 1 else sum(emb_dims) + dense_w
     nodes = _t(nodes, torch.int64).reshape(-1)
-    id_t = _t(id_table, torch.float32) if id_table is not None else None
-    ts = [_t(s[1], torch.float32) for s in sparse]
-    return nodes, (d_cfg, tuple(s_cfg), comb, W, dense_w if comb == 1 else 0, bool(sparse_grad)), id_t, ts
+    id_t = _t(id_table, dt) if id_table is not None else None
+    ts = [_t(s[1], dt) for s in sparse]
+    # a proxy's gradient is the sparse COO one
+    sparse_grad = bool(sparse_grad) or any(q is not None for q in proxies)
+    return nodes, (d_cfg, tuple(s_cfg), comb, W, dense_w if comb == 1 else 0, sparse_grad), id_t, ts, proxies
+
+
+def _route_grads(ctx, first, grads):
+    """the backward's outputs for the tables at inputs first .. first + n - 1 and their proxies right after them: each
+    table's gradient goes to its proxy when the proxy needs it, else to the table"""
+    n = len(grads)
+    to_proxy = [ctx.needs_input_grad[first + n + t] for t in range(n)]
+    return tuple(None if p else g for g, p in zip(grads, to_proxy)) + tuple(g if p else None for g, p in zip(grads, to_proxy))
+
+
+def _shallow_call(sym, p, *args):
+    """eu_shallow_encode(_pool) over p, or its _dtype twin when the problem's tables are bf16"""
+    if p.table_dtype:
+        _call(sym + "_dtype", C.byref(p), p.table_dtype, *args)
+    else:
+        _call(sym, C.byref(p), *args)
 
 
 def _shallow_backward(sym, extra, nodes, cfg, grad, id_table, tables):
@@ -1308,19 +1374,20 @@ def _shallow_backward(sym, extra, nodes, cfg, grad, id_table, tables):
 
 
 class _ShallowEncode(torch.autograd.Function):
-    """eu_shallow_encode / eu_shallow_encode_backward(_sparse).  Saves the node ids only (and the tables, which are inputs):
-    the backward pass lists every table's entries again from the graph.  Inputs after the configuration: the id table (None
-    when absent), then one table per sparse slot."""
+    """eu_shallow_encode(_dtype) / eu_shallow_encode_backward(_sparse).  Saves the node ids only (and the tables, which are
+    inputs): the backward pass lists every table's entries again from the graph.  Inputs after the configuration: the id
+    table (None when absent), then one table per sparse slot, then one proxy (or None) per table in that order."""
 
     @staticmethod
-    def forward(ctx, nodes, cfg, id_table, *tables):
+    def forward(ctx, nodes, cfg, id_table, *tables_proxies):
+        tables = tables_proxies[:(len(tables_proxies) - 1) // 2]
         dense, sparse_cfg, comb, W, dense_w, sparse_grad = cfg
         sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
         M, dev = nodes.numel(), nodes.device
         out = torch.empty((M, W), dtype=torch.float32, device=dev)
         dense_out = torch.empty((M, dense_w), dtype=torch.float32, device=dev) if comb == 1 else None
         p = _shallow_problem(nodes, id_table, dense, sparse, comb)
-        _call("eu_shallow_encode", C.byref(p), out, dense_out)
+        _shallow_call("eu_shallow_encode", p, out, dense_out)
         ctx.save_for_backward(nodes, id_table, *tables)
         ctx.cfg = cfg
         if dense_out is None:
@@ -1331,10 +1398,11 @@ class _ShallowEncode(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad, *unused):
         nodes, id_table, *tables = ctx.saved_tensors
-        return (None, None) + _shallow_backward("eu_shallow_encode_backward", (), nodes, ctx.cfg, grad, id_table, tables)
+        grads = _shallow_backward("eu_shallow_encode_backward", (), nodes, ctx.cfg, grad, id_table, tables)
+        return (None, None) + _route_grads(ctx, 2, grads)
 
 
-def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat', sparse_grad=False):
+def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat', sparse_grad=False, proxies=None):
     """ShallowEncoder's input row (tf_euler/python/utils/encoders.py:134-171) in one fused device op, for node ids of any shape
     (flattened to M):
         id_table    f32[n_id_rows, id_dim] or None: row nodes[i] (tf.nn.embedding_lookup; an id outside the table raises)
@@ -1347,13 +1415,17 @@ def shallow_encode(nodes, id_table=None, dense=(), sparse=(), combiner='concat',
     The gradient reaches the tables only (features are not trainable), deterministic, no atomics: dense gradients, or with
     sparse_grad=True coalesced sparse COO gradients of the rows the batch touches.  The forward synchronises once to check the
     ids when an id table is given, and not at all under CUDA-graph capture (include/euler_b200.h); the backward once (dense)
-    or 2 + the slots (sparse)."""
+    or 2 + the slots (sparse).
+    The tables may instead all be bfloat16, read widened exactly to f32: the rows are the f32 op's on the widened tables.
+    A bf16 table takes no gradient itself (one that requires grad raises).  proxies (None, or one entry per table in the
+    order id table, then the slots: None or table_proxy(table)) are float32 leaves that take each bf16 table's gradient,
+    the coalesced f32 sparse COO gradient an f32 table holding the widened values gets with sparse_grad=True."""
     if combiner not in SHALLOW_COMBINERS:
         raise EulerError("shallow_encode: combiner must be one of %s, got %r" % (sorted(SHALLOW_COMBINERS), combiner))
     comb = SHALLOW_COMBINERS[combiner]
-    nodes, cfg, id_t, ts = _shallow_inputs("shallow_encode", nodes, id_table, dense, sparse, comb, sparse_grad)
+    nodes, cfg, id_t, ts, qs = _shallow_inputs("shallow_encode", nodes, id_table, dense, sparse, comb, sparse_grad, proxies)
     d_cfg = cfg[0]
-    res = _ShallowEncode.apply(nodes, cfg, id_t, *ts)
+    res = _ShallowEncode.apply(nodes, cfg, id_t, *ts, *qs)
     if comb == 0:
         return res
     out, feats = res
@@ -1364,16 +1436,18 @@ POOLS = {'sum': 0, 'mean': 1}
 
 
 class _ShallowEncodePool(torch.autograd.Function):
-    """eu_shallow_encode_pool / eu_shallow_encode_pool_backward(_sparse): _ShallowEncode's inputs ('concat'), with the
-    segment length and the pool code.  Saves the node ids only (and the tables, which are inputs)."""
+    """eu_shallow_encode_pool(_dtype) / eu_shallow_encode_pool_backward(_sparse): _ShallowEncode's inputs ('concat', the
+    proxies included), with the segment length and the pool code.  Saves the node ids only (and the tables, which are
+    inputs)."""
 
     @staticmethod
-    def forward(ctx, nodes, cfg, count, pool, id_table, *tables):
+    def forward(ctx, nodes, cfg, count, pool, id_table, *tables_proxies):
+        tables = tables_proxies[:(len(tables_proxies) - 1) // 2]
         dense, sparse_cfg, comb, W = cfg[:4]
         sparse = [(fid, t, dv, c) for (fid, dv, c), t in zip(sparse_cfg, tables)]
         out = torch.empty((nodes.numel() // max(count, 1), W), dtype=torch.float32, device=nodes.device)   # count < 1 is refused below
         p = _shallow_problem(nodes, id_table, dense, sparse, comb)
-        _call("eu_shallow_encode_pool", C.byref(p), count, pool, out)
+        _shallow_call("eu_shallow_encode_pool", p, count, pool, out)
         ctx.save_for_backward(nodes, id_table, *tables)
         ctx.cfg = (cfg, count, pool)
         return out
@@ -1382,11 +1456,11 @@ class _ShallowEncodePool(torch.autograd.Function):
     def backward(ctx, grad):
         nodes, id_table, *tables = ctx.saved_tensors
         cfg, count, pool = ctx.cfg
-        return (None, None, None, None) + _shallow_backward("eu_shallow_encode_pool_backward", (count, pool), nodes, cfg, grad,
-                                                            id_table, tables)
+        grads = _shallow_backward("eu_shallow_encode_pool_backward", (count, pool), nodes, cfg, grad, id_table, tables)
+        return (None, None, None, None) + _route_grads(ctx, 4, grads)
 
 
-def shallow_encode_pool(nodes, count, id_table=None, dense=(), sparse=(), pool='mean', sparse_grad=False):
+def shallow_encode_pool(nodes, count, id_table=None, dense=(), sparse=(), pool='mean', sparse_grad=False, proxies=None):
     """The 'concat' rows of shallow_encode pooled over consecutive segments of `count` nodes, in one fused device op: what
     SageEncoder's first layer needs of the deepest hop of sample_fanout (count = the last fanout).  nodes (any shape, M =
     R * count ids when flattened), id_table, dense and sparse are shallow_encode's; returns f32[R, W], row r the 'sum' or
@@ -1394,11 +1468,12 @@ def shallow_encode_pool(nodes, count, id_table=None, dense=(), sparse=(), pool='
     too, as reduce_mean(axis=1) counts them).  The [M, W] matrix is never written, in either direction.  Fixed order
     (include/euler_b200.h): each column is added left to right from the segment's first row, mean divides once by count.
     Gradients reach the tables only, as shallow_encode's (dense, or coalesced sparse COO with sparse_grad=True), with the
-    same synchronisations.  count is at least 1, divides M and is at most 512 (EU_SHALLOW_POOL_MAX_COUNT)."""
+    same synchronisations.  count is at least 1, divides M and is at most 512 (EU_SHALLOW_POOL_MAX_COUNT).  bfloat16
+    tables and their proxies as shallow_encode's."""
     if pool not in POOLS:
         raise EulerError("shallow_encode_pool: pool must be one of %s, got %r" % (sorted(POOLS), pool))
-    nodes, cfg, id_t, ts = _shallow_inputs("shallow_encode_pool", nodes, id_table, dense, sparse, 0, sparse_grad)
-    return _ShallowEncodePool.apply(nodes, cfg, int(count), POOLS[pool], id_t, *ts)
+    nodes, cfg, id_t, ts, qs = _shallow_inputs("shallow_encode_pool", nodes, id_table, dense, sparse, 0, sparse_grad, proxies)
+    return _ShallowEncodePool.apply(nodes, cfg, int(count), POOLS[pool], id_t, *ts, *qs)
 
 
 # ------------------------------------------------------------------------------------ embedding stores

@@ -109,14 +109,25 @@ class _TFOptimizer(torch.optim.Optimizer):
             self._literal_dense(p, grad, state, group)
 
     @torch.no_grad()
-    def step(self, closure=None):
+    def step(self, closure=None, sparse_grads=None):
+        """One step over every parameter with a gradient.  sparse_grads (optional) maps parameters to float32 sparse COO
+        gradients, which are used instead of their .grad (never rounded to the parameter's dtype: this is how a bfloat16
+        table trains beside dense parameters).  Adam's powers and the rounding step counter advance once."""
+        sparse_grads = {} if sparse_grads is None else sparse_grads
+        mine = {id(p) for _, p, _ in self._each()}
+        for p, g in sparse_grads.items():
+            if id(p) not in mine:
+                raise ValueError("step: a parameter of sparse_grads is not one of this optimizer's")
+            if not torch.is_tensor(g) or not g.is_sparse or g.dtype != torch.float32 or tuple(g.shape) != tuple(p.shape):
+                raise ValueError("step: sparse_grads must map each parameter to a float32 sparse COO gradient of its shape")
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
         for i, p, group in self._each():
-            if p.grad is not None:
-                self._update(i, p, p.grad, group)
+            grad = sparse_grads.get(p, p.grad)
+            if grad is not None:
+                self._update(i, p, grad, group)
         self._finish()
         return loss
 
@@ -280,6 +291,26 @@ class AdamOptimizer(_TFOptimizer):
         powers = sd.pop('beta_powers')
         super().load_state_dict(sd)
         self.beta_powers.copy_(powers)
+
+
+def minimize(optimizer, loss, module):
+    """One training step of a model whose node encoders may hold bfloat16 tables (encoders.ShallowEncoder(table_dtype=)):
+    clears every parameter's .grad and every table proxy's, runs loss.backward(), collects each bf16 table's f32 sparse
+    gradient from its proxy (every ShallowEncoder in module.modules(), a shared one once) and steps `optimizer` once with
+    them as sparse_grads.  Without a bf16 table it is zero_grad(); loss.backward(); step().  Returns loss."""
+    from .encoders import ShallowEncoder
+    encoders = [m for m in module.modules() if isinstance(m, ShallowEncoder)]
+    pairs = {}
+    for e in encoders:
+        for table, proxy in e.table_proxies():
+            pairs[id(table)] = (table, proxy)
+    optimizer.zero_grad()
+    for _, proxy in pairs.values():
+        proxy.grad = None
+    loss.backward()
+    sparse_grads = {table: proxy.grad for table, proxy in pairs.values() if proxy.grad is not None}
+    optimizer.step(sparse_grads=sparse_grads)
+    return loss
 
 
 OPTIMIZERS = {

@@ -59,19 +59,19 @@ class SuperviseModel(torch.nn.Module):
 
 class GeniePath(SuperviseModel):
     """examples/geniepath/geniepath.py:26-48: SuperviseModel over GenieEncoder(metapath, dim, 'attention', .., head_num).
-    fused, sparse_grad and device are passed to the encoder (see GCNEncoder); streaming to SuperviseModel."""
+    fused, sparse_grad, device and table_dtype are passed to the encoder (see GCNEncoder); streaming to SuperviseModel."""
 
     def __init__(self, dim, metapath, label_idx, label_dim, max_id=-1, feature_idx=-1, feature_dim=0, use_id=False,
                  sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
                  use_residual=False, head_num=4, metric_name='f1', fused=True, sparse_grad=False, device=None, *,
-                 streaming=False):
+                 streaming=False, table_dtype=torch.float32):
         from .encoders import GenieEncoder
         super().__init__(label_idx, label_dim, metric_name, dim=dim, device=device, streaming=streaming)
         self._encoder = GenieEncoder(
             metapath, dim, 'attention', feature_idx=feature_idx, feature_dim=feature_dim, max_id=max_id, use_id=use_id,
             sparse_feature_idx=sparse_feature_idx, sparse_feature_max_id=sparse_feature_max_id, embedding_dim=embedding_dim,
             use_hash_embedding=use_hash_embedding, use_residual=use_residual, head_num=head_num, fused=fused,
-            sparse_grad=sparse_grad, device=device)
+            sparse_grad=sparse_grad, device=device, table_dtype=table_dtype)
 
     def embed(self, n_id):
         return self._encoder(n_id)

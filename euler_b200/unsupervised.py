@@ -219,11 +219,13 @@ class DGI(torch.nn.Module):
     the batch's mean embedding, with sigmoid cross entropy (ones for the true rows, zeros for the shuffled ones) and
     composed_metric for the rank metric.  __call__(inputs, generator=None) returns upstream's
     (embedding, loss, metric_name, metric), the embedding from a second pass of the encoder with fresh samples, as upstream;
-    generator fixes the shuffles.  num_negs is kept and unused, as upstream.  fused / sparse_grad are SageEncoder's."""
+    generator fixes the shuffles.  num_negs is kept and unused, as upstream.  fused / sparse_grad / table_dtype are
+    SageEncoder's (bfloat16 tables train with optimizers.minimize)."""
 
     def __init__(self, node_type, edge_type, max_id, metapath, fanouts, dim, aggregator='mean', concat=False, feature_idx=-1,
                  feature_dim=0, use_feature=None, use_id=False, sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16,
-                 use_hash_embedding=False, use_residual=False, num_negs=5, metric='mrr', fused=True, sparse_grad=False, device=None):
+                 use_hash_embedding=False, use_residual=False, num_negs=5, metric='mrr', fused=True, sparse_grad=False, device=None,
+                 table_dtype=torch.float32):
         super().__init__()
         from .encoders import Dense, ShuffleSageEncoder   # encoders builds on Embedding above
         if metric not in SKIPGRAM_METRICS:
@@ -235,7 +237,7 @@ class DGI(torch.nn.Module):
             metapath, fanouts, dim, aggregator, concat, feature_idx=feature_idx, feature_dim=feature_dim, max_id=max_id,
             use_id=use_id, sparse_feature_idx=sparse_feature_idx, sparse_feature_max_id=sparse_feature_max_id,
             embedding_dim=embedding_dim, use_hash_embedding=use_hash_embedding, use_residual=use_residual, fused=fused,
-            sparse_grad=sparse_grad, device=device)
+            sparse_grad=sparse_grad, device=device, table_dtype=table_dtype)
 
     def target_encoder(self, inputs, generator=None):
         return self._target_encoder(inputs, generator)

@@ -357,6 +357,14 @@ int eu_sparse_embedding_lookup_backward(eu_ctx* c, const float* grad_out, const 
 int eu_sparse_embedding_lookup_backward_sparse(eu_ctx* c, const float* grad_out, const int64_t* nodes, int64_t M, int32_t fid,
                                                int64_t default_value, int64_t n_rows, int32_t dim, int32_t combiner, int64_t* rows,
                                                float* values, int64_t* n);
+/* The forward with the table's storage type table_dtype (eu_feat_dtype): table is then read as that type.  Every read widens a
+ * bf16 element to f32 exactly and all arithmetic stays f32 in the order above, so a EU_FEAT_BF16 call gives bit for bit what
+ * the f32 call gives on the table widened to f32.  The 4-wide loads need dim % 4 == 0, the table 8-byte aligned (bf16) or
+ * 16-byte aligned (f32) and out 16-byte aligned; otherwise scalar loads give the same bits.  EU_FEAT_F32 is the call above.
+ * An unknown table_dtype: EU_ERR_INVALID, before any device work; every other bound and status as above.  The backward
+ * entry points have no _dtype twin: they read grad_out, the graph's bags and the table's shape, never the table. */
+int eu_sparse_embedding_lookup_dtype(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const void* table,
+                                     int64_t n_rows, int32_t dim, int32_t combiner, int32_t table_dtype, float* out);
 
 /* ShallowEncoder's input row, fused (tf_euler/python/utils/encoders.py:32-171): per node an id embedding, the dense feature
  * slots and one SparseEmbedding per uint64 slot, concatenated or added.  Node i of nodes i64[M]:
@@ -403,14 +411,14 @@ typedef struct {
   int32_t reserved;         /* 0 */
   int64_t default_value;    /* in [0, n_rows) */
   int64_t n_rows;
-  const float* table;       /* f32[n_rows, dim] */
+  const float* table;       /* f32[n_rows, dim]; with the _dtype calls' EU_FEAT_BF16, bf16 storage of that shape */
 } eu_shallow_sparse;
 typedef struct {
   int32_t combiner;         /* EU_SHALLOW_CONCAT or EU_SHALLOW_ADD */
   int32_t id_dim;
   int64_t M;
   const int64_t* nodes;     /* [M] */
-  const float* id_table;    /* f32[n_id_rows, id_dim], or NULL */
+  const float* id_table;    /* f32[n_id_rows, id_dim], or NULL; with the _dtype calls' EU_FEAT_BF16, bf16 storage */
   int64_t n_id_rows;
   int32_t n_dense, n_sparse;
   eu_shallow_dense dense[EU_SHALLOW_MAX_SLOTS];
@@ -420,6 +428,14 @@ int eu_shallow_encode(eu_ctx* c, const eu_shallow_problem* p, float* out, float*
 int eu_shallow_encode_backward(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, float* const* grads);
 int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const float* grad_out, int64_t* const* rows,
                                       float* const* values, int64_t* counts);
+/* eu_shallow_encode with the tables' storage type table_dtype (eu_feat_dtype): the id table and every slot's table have it,
+ * and the problem's table pointers are then read as that type (the struct's layout is unchanged).  As for
+ * eu_sparse_embedding_lookup_dtype, every table read widens bf16 to f32 exactly and all arithmetic stays f32 in the order
+ * above, so a EU_FEAT_BF16 call gives the f32 call's bits on the widened tables, with f32 or bf16 dense features alike.  A
+ * slot's 4-wide loads need its table aligned to four elements (8 bytes of bf16, 16 of f32) and out 16-byte aligned.  An
+ * unknown table_dtype: EU_ERR_INVALID, before any device work; every other bound and status as eu_shallow_encode's.  The
+ * backward entry points serve both dtypes: they never dereference a table (only its rows and dim). */
+int eu_shallow_encode_dtype(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, float* out, float* dense_out);
 
 /* ShallowEncoder's rows pooled over fixed segments: what SageEncoder's first layer needs of the deepest hop of a fanout
  * (tf_euler/python/utils/encoders.py:475-491: the hop's rows reshaped to [R, count, W] reach the mean / gcn aggregator only
@@ -442,6 +458,8 @@ int eu_shallow_encode_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, co
 #define EU_SHALLOW_POOL_MAX_COUNT 512
 enum { EU_POOL_SUM = 0, EU_POOL_MEAN = 1 };
 int eu_shallow_encode_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, float* out);
+/* eu_shallow_encode_pool with the tables' storage type table_dtype, by eu_shallow_encode_dtype's rules. */
+int eu_shallow_encode_pool_dtype(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, int32_t count, int32_t pool, float* out);
 int eu_shallow_encode_pool_backward(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool, const float* grad_out,
                                     float* const* grads);
 int eu_shallow_encode_pool_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, int32_t count, int32_t pool,
