@@ -36,11 +36,13 @@ def sr_bits(x, r):
     return out
 
 
-def step(name, tables, grad, seed, step_no, tensor, lr, adam=None, momentum=0.0):
+def step(name, tables, grad, seed, step_no, tensor, lr, adam=None, momentum=0.0, rows=None):
     """One update of bf16 tables (uint16 bit arrays [N, D]: var, then its slots) in place: widen, the f32 update of
     optim_reference, then stochastic rounding of every element written -- the rows of a sparse Momentum / Adagrad gradient,
     every element otherwise -- with word w of philox_bits(seed, step_no, tensor, r D + d) for table w.  grad: a dense f32
-    array or (rows, values).  adam: an optim_reference.Adam whose powers are the step's (the caller calls finish())."""
+    array or (rows, values).  adam: an optim_reference.Adam whose powers are the step's (the caller calls finish()).
+    rows: None when the tables are whole, else int64[N], the row of the full table each given row is: row i then draws with
+    element rows[i] D + d, so a step can be restated on picked rows of a table too large to copy."""
     N, D = tables[0].shape
     f = [bf.widen(t).reshape(N, D) for t in tables]
     if name == 'adam':
@@ -49,8 +51,9 @@ def step(name, tables, grad, seed, step_no, tensor, lr, adam=None, momentum=0.0)
         ref.adagrad(f[0], f[1], grad, lr)
     else:
         ref.momentum(f[0], f[1], grad, lr, momentum)
-    rows = np.unique(grad[0]) if isinstance(grad, tuple) and name != 'adam' else np.arange(N)
-    elem = (rows[:, None] * D + np.arange(D)[None, :]).reshape(-1)
+    written = np.unique(grad[0]) if isinstance(grad, tuple) and name != 'adam' else np.arange(N)
+    glob = written if rows is None else np.asarray(rows, np.int64)[written]
+    elem = (glob.astype(np.int64)[:, None] * D + np.arange(D)[None, :]).reshape(-1)
     words = philox_bits(seed, step_no, tensor, elem)
     for w, (t, v) in enumerate(zip(tables, f)):
-        t[rows] = sr_bits(v[rows].reshape(-1), words[w]).reshape(len(rows), D)
+        t[written] = sr_bits(v[written].reshape(-1), words[w]).reshape(len(written), D)
