@@ -14,6 +14,8 @@ EU_RNG_PHILOX = 1
 
 # eu_feat_dtype: the storage type of a graph's dense node feature table, by name
 FEAT_DTYPES = {"float32": 0, "bfloat16": 1}
+# eu_feat_place: where that table lives, by name
+FEAT_PLACES = {"device": 0, "host": 1}
 
 
 class EulerError(RuntimeError):
@@ -31,6 +33,11 @@ class GraphDesc(C.Structure):
         ("n_u64_slots", C.c_int32), ("u64_ptr", C.c_void_p), ("u64_val", C.c_void_p),
         ("n_bin_slots", C.c_int32), ("bin_ptr", C.c_void_p), ("bin_val", C.c_void_p),
     ]
+
+
+class FeatStorage(C.Structure):
+    """eu_feat_storage"""
+    _fields_ = [("dtype", C.c_int32), ("place", C.c_int32), ("cache_rows", C.c_int64)]
 
 
 class EdgeDesc(C.Structure):
@@ -104,6 +111,14 @@ SIGNATURES = {
                                                     _U64, C.c_int, C.c_int, C.c_int, _I32, C.POINTER(_P)]),
     "eu_graph_load": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "eu_graph_load_dtype": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, _I32, C.POINTER(_P)]),
+    "eu_graph_create_storage": (C.c_int, [C.POINTER(GraphDesc), C.c_int, C.POINTER(FeatStorage), C.POINTER(_P)]),
+    "eu_graph_create_rmat_storage": (C.c_int, [_I64, _I64, C.c_double, C.c_double, C.c_double, _U64, _I32, _U64, C.c_int,
+                                               C.POINTER(FeatStorage), C.POINTER(_P)]),
+    "eu_graph_create_rmat_hetero_storage": (C.c_int, [_I64, _I64, _I32, _I32, C.c_double, C.c_double, C.c_double, _U64, _I32,
+                                                      _U64, C.c_int, C.c_int, C.c_int, C.POINTER(FeatStorage),
+                                                      C.POINTER(_P)]),
+    "eu_graph_load_storage": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(FeatStorage),
+                                        C.POINTER(_P)]),
     "eu_graph_load_ex": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     "eu_graph_set_edges": (C.c_int, [_P, _P]),
     "eu_graph_num_edge_records": (_I64, [_P]),
@@ -122,6 +137,10 @@ SIGNATURES = {
     "eu_graph_feat_dim": (_I32, [_P]),
     "eu_graph_feat_dtype": (_I32, [_P]),
     "eu_graph_hbm_bytes": (_I64, [_P]),
+    "eu_graph_feat_place": (_I32, [_P]),
+    "eu_graph_feat_cache_rows": (_I64, [_P]),
+    "eu_graph_host_bytes": (_I64, [_P]),
+    "eu_graph_export_feat_slots": (C.c_int, [_P, _P]),
     "eu_graph_export": (C.c_int, [_P] * 9),
     "eu_graph_edge_type_id": (_I32, [_P, C.c_char_p]),
     "eu_graph_node_type_id": (_I32, [_P, C.c_char_p]),

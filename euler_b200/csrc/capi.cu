@@ -300,8 +300,18 @@ bool InitQueryProxy(const char* conf) {
     fprintf(stderr, "[euler_b200] ERROR InitQueryProxy: feature_dtype=%s is not float32 or bfloat16\n", fdt.c_str());
     return true;
   }
+  // feature_place=device|host and feature_cache_rows=C: where the table lives (eu_feat_storage); device and 0 when absent
+  const std::string fpl = kv.count("feature_place") ? kv["feature_place"] : "device";
+  const std::string fcr = kv.count("feature_cache_rows") ? kv["feature_cache_rows"] : "0";
+  if ((fpl != "device" && fpl != "host") || fcr.empty() || fcr.find_first_not_of("0123456789") != std::string::npos) {
+    fprintf(stderr, "[euler_b200] ERROR InitQueryProxy: feature_place=%s / feature_cache_rows=%s: the place is device or host, "
+            "the rows an integer >= 0\n", fpl.c_str(), fcr.c_str());
+    return true;
+  }
+  const eu_feat_storage st{fdt == "bfloat16" ? EU_FEAT_BF16 : EU_FEAT_F32, fpl == "host" ? EU_FEAT_HOST : EU_FEAT_DEVICE,
+                           (int64_t)strtoll(fcr.c_str(), nullptr, 10)};
   eu_graph* g = nullptr;
-  int rc = eu_graph_load_dtype(kv["data_path"].c_str(), 0, 1, device, 1, fdt == "bfloat16" ? EU_FEAT_BF16 : EU_FEAT_F32, &g);
+  int rc = eu_graph_load_storage(kv["data_path"].c_str(), 0, 1, device, 1, &st, &g);
   if (rc != EU_OK) {
     fprintf(stderr, "[euler_b200] ERROR InitQueryProxy: graph load failed: %s\n", eu_last_error());
     return true;

@@ -59,6 +59,14 @@ struct DevGraph {
   int32_t n_bin_slots;
   const int64_t* bin_ptr;
   const unsigned char* bin_val;
+  // where the dense table lives (eu_feat_place: kFeatDevice / kFeatHost; appended so every member above keeps its offset).
+  // Host: feat is the device pointer of a mapped pinned host table holding every row, feat_cache [feat_cache_rows, feat_dim]
+  // of feat_dtype in HBM copies the rows of highest in-degree, and feat_slot[n] (HBM) maps a row to its cache row or -1.
+  // Read rows only through feat_row.
+  int32_t feat_place;
+  const void* feat_cache;
+  const int32_t* feat_slot;
+  int64_t feat_cache_rows;
 };
 
 // edge store (edges.cu): SoA edge arrays + (src, dst, type) -> row table + features with the node layout
@@ -138,6 +146,38 @@ __host__ __device__ __forceinline__ void dense_slot(const DevGraph& g, int32_t f
 // rounding says so, and subnormals round like any other value.
 template <typename T>
 __host__ __device__ __forceinline__ const T* feat_cols(const DevGraph& g) { return static_cast<const T*>(g.feat); }
+
+// eu_feat_place (include/euler_b200.h)
+enum : int { kFeatDevice = 0, kFeatHost = 1 };
+
+// Where a kernel finds row `row` (>= 0) of the table, for the table's placement P (kFeatDevice or kFeatHost, a template
+// argument like T, picked by the launcher from g.feat_place).  Device: the HBM table.  Host: the HBM cache row when the slot
+// map gives one, else the row of the mapped host table.  Both tiers hold the same bits, so what a kernel reads never depends
+// on the placement or the cache size.  feat_row(g, row, W, col) is column col of the row, with W the row width where the
+// kernel knows it at compile time (it must equal g.feat_dim).  The device forms are the expressions the kernels used before
+// placement existed, term for term, so the device instantiations compile to the same instructions.
+template <typename T, int P>
+__device__ __forceinline__ const T* feat_row(const DevGraph& g, int64_t row, int32_t W, int32_t col) {
+  if (P == kFeatHost) {
+    const int32_t s = __ldg(g.feat_slot + row);
+    if (s >= 0) return static_cast<const T*>(g.feat_cache) + col + (int64_t)s * W;
+  }
+  return feat_cols<T>(g) + col + row * (int64_t)W;
+}
+template <typename T, int P>
+__device__ __forceinline__ const T* feat_row(const DevGraph& g, int64_t row) {
+  if (P == kFeatHost) {
+    const int32_t s = __ldg(g.feat_slot + row);
+    if (s >= 0) return static_cast<const T*>(g.feat_cache) + (int64_t)s * g.feat_dim;
+  }
+  return feat_cols<T>(g) + row * (int64_t)g.feat_dim;
+}
+// column col of row `row` when ok, else the table's first element (which the caller must not read): a row that may be absent
+template <typename T, int P>
+__device__ __forceinline__ const T* feat_row_if(const DevGraph& g, bool ok, int64_t row, int32_t col) {
+  if (P == kFeatHost) return ok ? feat_row<T, P>(g, row) + col : feat_cols<T>(g);
+  return feat_cols<T>(g) + (ok ? row * (int64_t)g.feat_dim + col : 0);
+}
 
 template <typename T> __device__ __forceinline__ float feat_ld(const T* p);
 template <> __device__ __forceinline__ float feat_ld<float>(const float* p) { return __ldg(p); }

@@ -180,9 +180,9 @@ __device__ __forceinline__ void shallow_slot(const DevGraph& g, const ShallowDev
 
 // G lanes per node r: the id columns, the dense slots (k_feature's rule: the stored columns, zeros past them, zeros for an
 // absent node or an unknown slot), then the sparse slots.  The group syncs between parts: a part may map columns to lanes
-// differently from the one before it, and ADD reads what the previous part wrote.  T: the dense table's storage type, E the
-// id and sparse tables'.
-template <typename T, typename E>
+// differently from the one before it, and ADD reads what the previous part wrote.  T: the dense table's storage type and P its
+// placement, E the id and sparse tables' storage type.
+template <typename T, typename E, int P>
 __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, int G) {
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t r = tid >> (31 - __clz(G));
@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(256) k_shallow_fwd(DevGraph g, ShallowDev p, i
     const int32_t fid = p.dense_fid[j];
     const bool have = fid >= 0 && fid < g.n_slots && row >= 0;
     const int sdim = have ? g.slot_dim[fid] : 0;
-    const T* f = feat_cols<T>(g) + (have ? row * (int64_t)g.feat_dim + g.slot_off[fid] : 0);
+    const T* f = feat_row_if<T, P>(g, have, row, have ? g.slot_off[fid] : 0);
     float* oj = od + p.dense_off[j];
     for (int d = sub; d < p.dense_dim[j]; d += G) oj[d] = d < sdim ? feat_ld(f + d) : 0.f;
   }
@@ -257,7 +257,7 @@ __device__ __forceinline__ void shallow_pool_slot(const DevGraph& g, const Shall
 // G lanes per output row r, the pool of the `count` ShallowEncoder rows (CONCAT) of nodes[r * count ..]: k_shallow_fwd's
 // parts and rules, each column summed over the segment's nodes in a register, in node order, and divided once by pool_den
 // (fl(count); 0: the sum).  The group looks every node's graph row up once, into its `count` slots of shared memory.
-template <typename T, typename E>
+template <typename T, typename E, int P>
 __global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev p, int count, float pool_den, int G) {
   extern __shared__ int64_t pool_rows[];
   const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -281,10 +281,10 @@ __global__ void __launch_bounds__(256, 2) k_shallow_pool(DevGraph g, ShallowDev 
     const int32_t fid = p.dense_fid[k];
     const bool known = fid >= 0 && fid < g.n_slots;
     const int sdim = known ? g.slot_dim[fid] : 0;
-    const T* f = feat_cols<T>(g) + (known ? g.slot_off[fid] : 0);
+    const int32_t soff = known ? g.slot_off[fid] : 0;
     float* oj = o + p.dense_off[k];
     for (int d = sub; d < p.dense_dim[k]; d += G)
-      oj[d] = finish(pool_column(count, [&](int j) { return d < sdim && rows[j] >= 0 ? feat_ld(f + rows[j] * (int64_t)g.feat_dim + d) : 0.f; }));
+      oj[d] = finish(pool_column(count, [&](int j) { return d < sdim && rows[j] >= 0 ? feat_ld(feat_row<T, P>(g, rows[j], g.feat_dim, soff) + d) : 0.f; }));
   }
   for (int s = 0; s < p.n_sparse; ++s) {
     if (p.vec_mask >> s & 1) shallow_pool_slot<true, E>(g, p, s, rows, count, pool_den, o + p.sp_off[s], G, sub, gm);
@@ -757,6 +757,35 @@ static int emb_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, i
   return EU_OK;
 }
 
+// k_shallow_fwd / k_shallow_pool for the dense table at P, of bf16_feat's type, and tables of table_dtype
+template <int P>
+static int launch_shallow_fwd(eu_ctx* c, const ShallowDev& d, int G, unsigned blocks, int32_t table_dtype, bool bf16_feat) {
+  if (table_dtype == EU_FEAT_BF16) {
+    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, __nv_bfloat16, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+    else k_shallow_fwd<float, __nv_bfloat16, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+  } else {
+    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, float, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+    else k_shallow_fwd<float, float, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+  }
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
+template <int P>
+static int launch_shallow_pool(eu_ctx* c, const ShallowDev& d, int count, float pool_den, int G, unsigned blocks, size_t smem,
+                               int32_t table_dtype, bool bf16_feat) {
+  cudaStream_t s = c->stream;
+  if (table_dtype == EU_FEAT_BF16) {
+    if (bf16_feat) k_shallow_pool<__nv_bfloat16, __nv_bfloat16, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
+    else k_shallow_pool<float, __nv_bfloat16, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
+  } else {
+    if (bf16_feat) k_shallow_pool<__nv_bfloat16, float, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
+    else k_shallow_pool<float, float, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
+  }
+  EU_LAUNCHED();
+  return EU_OK;
+}
+
 // eu_shallow_encode(_dtype)
 static int shallow_encode(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, float* out, float* dense_out, const char* who) {
   ShallowDev d;
@@ -776,15 +805,8 @@ static int shallow_encode(eu_ctx* c, const eu_shallow_problem* p, int32_t table_
   EuProfScope ps(c, "shallow_fwd", p->M);
   const unsigned blocks = (unsigned)ceil_div(p->M * G, 256);
   const bool bf16_feat = c->g->d.feat_dtype == EU_FEAT_BF16;
-  if (table_dtype == EU_FEAT_BF16) {
-    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, __nv_bfloat16><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-    else k_shallow_fwd<float, __nv_bfloat16><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-  } else {
-    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, float><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-    else k_shallow_fwd<float, float><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-  }
-  EU_LAUNCHED();
-  return EU_OK;
+  if (c->g->d.feat_place == EU_FEAT_HOST) return launch_shallow_fwd<kFeatHost>(c, d, G, blocks, table_dtype, bf16_feat);
+  return launch_shallow_fwd<kFeatDevice>(c, d, G, blocks, table_dtype, bf16_feat);
 }
 
 // eu_shallow_encode_pool(_dtype)
@@ -811,16 +833,9 @@ static int shallow_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dt
   const unsigned blocks = (unsigned)ceil_div(R * G, 256);
   const size_t smem = (256 / G) * (size_t)count * sizeof(int64_t);
   const bool bf16_feat = c->g->d.feat_dtype == EU_FEAT_BF16;
-  cudaStream_t s = c->stream;
-  if (table_dtype == EU_FEAT_BF16) {
-    if (bf16_feat) k_shallow_pool<__nv_bfloat16, __nv_bfloat16><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
-    else k_shallow_pool<float, __nv_bfloat16><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
-  } else {
-    if (bf16_feat) k_shallow_pool<__nv_bfloat16, float><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
-    else k_shallow_pool<float, float><<<blocks, 256, smem, s>>>(c->g->d, d, count, gr.pool_den, G);
-  }
-  EU_LAUNCHED();
-  return EU_OK;
+  if (c->g->d.feat_place == EU_FEAT_HOST)
+    return launch_shallow_pool<kFeatHost>(c, d, count, gr.pool_den, G, blocks, smem, table_dtype, bf16_feat);
+  return launch_shallow_pool<kFeatDevice>(c, d, count, gr.pool_den, G, blocks, smem, table_dtype, bf16_feat);
 }
 
 }  // namespace eu

@@ -167,6 +167,39 @@ __global__ void k_feat_round(const float* __restrict__ src, int64_t n, __nv_bflo
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += step) dst[i] = feat_st<__nv_bfloat16>(src[i]);
 }
 
+// ---- the HBM cache of a host-placed feature table (eu_feat_storage)
+// deg[row] += 1 for every adjacency entry whose neighbour id is a row of this graph (ids without a row count for nothing)
+__global__ void k_in_degree(DevGraph g, unsigned long long* __restrict__ deg) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; e < g.E; e += step) {
+    const int64_t r = lookup_row(g, __ldg(g.nbr + e));
+    if (r >= 0) atomicAdd(deg + r, 1ull);
+  }
+}
+
+// the ranking's keys and values: ~deg sorts in-degree descending; the rows go in ascending and the radix sort is stable, so
+// ties keep row order
+__global__ void k_rank_keys(unsigned long long* __restrict__ deg, int64_t n, int32_t* __restrict__ rows) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += step) { deg[r] = ~deg[r]; rows[r] = (int32_t)r; }
+}
+
+// slot[order[i]] = i for the first C ranked rows (slot is all -1 before)
+__global__ void k_cache_slots(const int32_t* __restrict__ order, int64_t C, int32_t* __restrict__ slot) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < C; i += step) slot[order[i]] = (int32_t)i;
+}
+
+// cache[i, :] = host[order[i], :]: a gather of whole rows from the mapped table, bits unchanged
+template <typename T>
+__global__ void k_cache_fill(const T* __restrict__ host, const int32_t* __restrict__ order, int64_t C, int32_t W,
+                             T* __restrict__ cache) {
+  const int64_t total = C * (int64_t)W;
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += step)
+    cache[i] = host[(int64_t)__ldg(order + i / W) * W + i % W];
+}
+
 // adj_sorted: lets the node2vec step classify neighbors by merging sorted lists in parallel
 // (the reference's two-pointer merge, tf_euler/kernels/random_walk_op.cc:140-168, assumes sorted lists too).
 __global__ void k_check_adj_sorted(int64_t n_groups, const int64_t* grp_ptr, const unsigned long long* nbr, int* unsorted) {
@@ -225,20 +258,112 @@ static int upload(eu_graph* g, const T** dst, const T* src, int64_t count) {
 
 static bool feat_dtype_ok(int32_t dtype) { return dtype == EU_FEAT_F32 || dtype == EU_FEAT_BF16; }
 
-// The host f32 table [count] into a device table of d.feat_dtype.  bf16: f32 chunks go up through one device buffer and are
-// rounded there (k_feat_round), so the peak is the bf16 table plus one chunk and the device's rounding is the only one.
+int feat_storage_check(const eu_feat_storage* in, int64_t n, const char* who, eu_feat_storage* st) {
+  *st = in ? *in : eu_feat_storage{EU_FEAT_F32, EU_FEAT_DEVICE, 0};
+  if (!feat_dtype_ok(st->dtype)) { set_error("%s: unknown feature dtype %d", who, st->dtype); return EU_ERR_INVALID; }
+  if (st->place != EU_FEAT_DEVICE && st->place != EU_FEAT_HOST) {
+    set_error("%s: unknown feature place %d (EU_FEAT_DEVICE or EU_FEAT_HOST)", who, st->place);
+    return EU_ERR_INVALID;
+  }
+  if (st->cache_rows < 0 || st->cache_rows > n) {
+    set_error("%s: feature cache rows %lld outside [0, %lld]", who, (long long)st->cache_rows, (long long)n);
+    return EU_ERR_INVALID;
+  }
+  if (st->cache_rows > 0 && st->place != EU_FEAT_HOST) {
+    set_error("%s: a feature cache needs a host-placed table (the device table is in HBM already)", who);
+    return EU_ERR_INVALID;
+  }
+  if (st->place == EU_FEAT_HOST && n >= ((int64_t)1 << 31)) {
+    set_error("%s: a host-placed feature table holds fewer than 2^31 rows (the slot map is int32)", who);
+    return EU_ERR_UNSUPPORTED;
+  }
+  return EU_OK;
+}
+
+// The feature table [count] of d.feat_dtype, in HBM or (d.feat_place) in mapped pinned host memory: d.feat is what kernels
+// read, *fill what the build writes through (the same pointer).
+template <typename T>
+static int alloc_feat(eu_graph* g, int64_t count, T** fill) {
+  if (g->d.feat_place == EU_FEAT_HOST) {
+    T* host = nullptr;
+    const int rc = g->host_alloc(&host, fill, count);
+    g->feat_host = host;
+    if (rc) return rc;
+  } else {
+    const int rc = g->alloc(fill, count);
+    if (rc) return rc;
+  }
+  g->d.feat = *fill;
+  return EU_OK;
+}
+
+// Host placement: the slot map, and the HBM cache of the first C rows by (in-degree descending, row ascending).  Integer counts
+// and a stable radix sort: the same rows every build.  Needs the CSR, the id -> row table and the filled host table.
+static int build_feat_cache(eu_graph* g, int64_t C) {
+  DevGraph& d = g->d;
+  if (d.feat_place != EU_FEAT_HOST || d.feat_dim <= 0) return EU_OK;
+  const int64_t n = d.n;
+  int32_t* slot = nullptr;
+  int rc = g->alloc(&slot, n);
+  if (rc) return rc;
+  EU_CUDA(cudaMemset(slot, 0xFF, sizeof(int32_t) * (size_t)(n > 0 ? n : 1)));
+  d.feat_slot = slot;
+  d.feat_cache_rows = C;
+  if (C == 0) return EU_OK;
+  const size_t es = d.feat_dtype == EU_FEAT_BF16 ? 2 : 4;
+  void* cache = nullptr;
+  rc = es == 2 ? g->alloc((__nv_bfloat16**)&cache, C * (int64_t)d.feat_dim) : g->alloc((float**)&cache, C * (int64_t)d.feat_dim);
+  if (rc) return rc;
+  d.feat_cache = cache;
+  unsigned long long *deg = nullptr, *deg_sorted = nullptr;
+  int32_t *rows = nullptr, *order = nullptr;
+  void* tmp = nullptr;
+  size_t tmp_bytes = 0;
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, deg, deg_sorted, rows, order, n);
+  if (e == cudaSuccess) e = cudaMalloc(&deg, sizeof(unsigned long long) * (size_t)n);
+  if (e == cudaSuccess) e = cudaMalloc(&deg_sorted, sizeof(unsigned long long) * (size_t)n);
+  if (e == cudaSuccess) e = cudaMalloc(&rows, sizeof(int32_t) * (size_t)n);
+  if (e == cudaSuccess) e = cudaMalloc(&order, sizeof(int32_t) * (size_t)n);
+  if (e == cudaSuccess) e = cudaMalloc(&tmp, tmp_bytes > 0 ? tmp_bytes : 1);
+  if (e == cudaSuccess) e = cudaMemset(deg, 0, sizeof(unsigned long long) * (size_t)n);
+  const unsigned grid = kSMs * 8;
+  if (e == cudaSuccess && d.E > 0) { k_in_degree<<<grid, 256>>>(d, deg); g_launches++; e = cudaGetLastError(); }
+  if (e == cudaSuccess) { k_rank_keys<<<grid, 256>>>(deg, n, rows); g_launches++; e = cudaGetLastError(); }
+  if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, deg, deg_sorted, rows, order, n);
+  if (e == cudaSuccess) { k_cache_slots<<<grid, 256>>>(order, C, slot); g_launches++; e = cudaGetLastError(); }
+  if (e == cudaSuccess) {
+    if (es == 2) k_cache_fill<<<grid, 256>>>(feat_cols<__nv_bfloat16>(d), order, C, d.feat_dim, (__nv_bfloat16*)cache);
+    else k_cache_fill<<<grid, 256>>>(feat_cols<float>(d), order, C, d.feat_dim, (float*)cache);
+    g_launches++;
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  cudaFree(deg); cudaFree(deg_sorted); cudaFree(rows); cudaFree(order); cudaFree(tmp);
+  if (e != cudaSuccess) { set_error("feature cache build: %s", cudaGetErrorString(e)); return EU_ERR_CUDA; }
+  return EU_OK;
+}
+
+// The host f32 table [count] into a table of d.feat_dtype at d.feat_place.  bf16: f32 chunks go up through one device buffer
+// and are rounded there (k_feat_round, which writes a host-placed table through its mapped pointer), so the peak is the bf16
+// table plus one chunk and the device's rounding is the only one.
 static int upload_feat(eu_graph* g, const float* src, int64_t count) {
   DevGraph& d = g->d;
   if (d.feat_dtype == EU_FEAT_F32) {
-    const float* p = nullptr;
-    const int rc = upload(g, &p, src, count);
-    d.feat = p;
-    return rc;
+    if (d.feat_place == EU_FEAT_DEVICE) {
+      const float* p = nullptr;
+      const int rc = upload(g, &p, src, count);
+      d.feat = p;
+      return rc;
+    }
+    float* p = nullptr;
+    const int rc = alloc_feat(g, count, &p);
+    if (rc) return rc;
+    if (count > 0) memcpy(const_cast<void*>(g->feat_host), src, sizeof(float) * (size_t)count);
+    return EU_OK;
   }
   __nv_bfloat16* p = nullptr;
-  int rc = g->alloc(&p, count);
+  int rc = alloc_feat(g, count, &p);
   if (rc) return rc;
-  d.feat = p;
   if (count == 0) return EU_OK;
   constexpr int64_t kChunk = (int64_t)1 << 24;   // f32 elements per chunk: 64 MB
   const int64_t chunk = std::min(count, kChunk);
@@ -400,6 +525,17 @@ int eu_graph_create(const eu_graph_desc* desc, int device, eu_graph** out) {
 int eu_graph_create_dtype(const eu_graph_desc* desc, int device, int32_t feat_dtype, eu_graph** out) {
   if (!desc || !out) { set_error("null argument"); return EU_ERR_INVALID; }
   if (!feat_dtype_ok(feat_dtype)) { set_error("eu_graph_create: unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; }
+  const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0};
+  return eu_graph_create_storage(desc, device, &st, out);
+}
+
+int eu_graph_create_storage(const eu_graph_desc* desc, int device, const eu_feat_storage* storage, eu_graph** out) {
+  if (!desc || !out) { set_error("null argument"); return EU_ERR_INVALID; }
+  eu_feat_storage st{EU_FEAT_F32, EU_FEAT_DEVICE, 0};
+  if (desc->n_nodes >= 0) {
+    const int rc = feat_storage_check(storage, desc->n_nodes, "eu_graph_create", &st);
+    if (rc) return rc;
+  }
   if (desc->n_nodes < 0 || desc->n_edge_types < 1 || desc->n_edge_types > EU_MAX_ETYPES ||
       !desc->ids || !desc->grp_ptr || (!desc->cum_w && !desc->w && desc->grp_ptr[desc->n_nodes * desc->n_edge_types] > 0) ||
       (desc->cum_w && desc->n_edge_types > 1 && !desc->grp_cum)) {
@@ -450,7 +586,8 @@ int eu_graph_create_dtype(const eu_graph_desc* desc, int device, int32_t feat_dt
     d.grp_cum = gc;
   }
   d.feat_dim = desc->feat ? desc->feat_dim : 0;
-  d.feat_dtype = feat_dtype;
+  d.feat_dtype = st.dtype;
+  d.feat_place = st.place;
   if (d.feat_dim > 0) TRY(upload_feat(g, desc->feat, n * (int64_t)d.feat_dim));
   if (d.feat_dim > 0) {
     if (desc->n_feat_slots > 0) {
@@ -490,6 +627,7 @@ int eu_graph_create_dtype(const eu_graph_desc* desc, int device, int32_t feat_dt
   d.id_base = n > 0 ? desc->ids[0] : 0;
   d.id_stride = 1;
   TRY(build_hash(g));
+  TRY(build_feat_cache(g, st.cache_rows));
   if (desc->sampler_order) g->sampler_order.assign(desc->sampler_order, desc->sampler_order + n);
   for (int t = 0; t < T; ++t) g->edge_type_names.push_back(std::to_string(t));
   for (int t = 0; t < d.n_node_types; ++t) g->node_type_names.push_back(std::to_string(t));
@@ -504,18 +642,19 @@ int eu_graph_create_dtype(const eu_graph_desc* desc, int device, int32_t feat_dt
 // of the shards is exactly the unsharded graph.
 static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
                        int32_t feat_dim, uint64_t feat_seed, int device, int shard_index, int shard_number,
-                       int T, int NT, int32_t feat_dtype, eu_graph** out) {
-  if (!feat_dtype_ok(feat_dtype)) { set_error("eu_graph_create_rmat: unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; }
+                       int T, int NT, const eu_feat_storage* storage, eu_graph** out) {
+  eu_feat_storage st;
   if (!out || n_nodes <= 0 || n_edges < 0 || shard_number < 1 || shard_index < 0 || shard_index >= shard_number ||
       T < 1 || T > EU_MAX_ETYPES || NT < 1 || NT > EU_MAX_ETYPES || (double)n_nodes * (double)n_nodes * T >= 9.2e18) {
     set_error("eu_graph_create_rmat: bad sizes"); return EU_ERR_INVALID;
   }
   if ((double)n_nodes * (double)n_nodes >= 9.2e18) { set_error("n_nodes too large for 64-bit sort keys"); return EU_ERR_INVALID; }
-  int rc = check_device(device);
-  if (rc) return rc;
   const int64_t N = shard_number;
   const int64_t base_id = shard_index == 0 ? N : shard_index;           // first owned id (ids are 1..n; 0 is unusable)
   const int64_t n_local = n_nodes >= base_id ? (n_nodes - base_id) / N + 1 : 0;
+  int rc = feat_storage_check(storage, n_local, "eu_graph_create_rmat", &st);
+  if (rc) return rc;
+  if ((rc = check_device(device))) return rc;
   eu_graph* g = new eu_graph();
   g->device = device;
   DevGraph& d = g->d;
@@ -595,24 +734,24 @@ static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, dou
   d.grp_cum = gcum;
   d.dense_ids = 1; d.id_base = (unsigned long long)base_id; d.id_stride = (unsigned long long)N;
   d.feat_dim = feat_dim;
-  d.feat_dtype = feat_dtype;
-  if (feat_dim > 0) {
-    if (feat_dtype == EU_FEAT_BF16) {
+  d.feat_dtype = st.dtype;
+  d.feat_place = st.place;
+  if (feat_dim > 0) {   // a host-placed table is filled through its mapped pointer
+    if (st.dtype == EU_FEAT_BF16) {
       __nv_bfloat16* feat = nullptr;
-      TRY(g->alloc(&feat, n_local * (int64_t)feat_dim));
+      TRY(alloc_feat(g, n_local * (int64_t)feat_dim, &feat));
       k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
-      d.feat = feat;
     } else {
       float* feat = nullptr;
-      TRY(g->alloc(&feat, n_local * (int64_t)feat_dim));
+      TRY(alloc_feat(g, n_local * (int64_t)feat_dim, &feat));
       k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
-      d.feat = feat;
     }
     g_launches++;
     d.n_slots = 1; d.slot_off[0] = 0; d.slot_dim[0] = feat_dim;
     g->dense_feature_names.push_back("feat0");
   }
   TRY(build_hash(g));
+  TRY(build_feat_cache(g, st.cache_rows));
   for (int t = 0; t < T; ++t) g->edge_type_names.push_back(std::to_string(t));
   for (int t = 0; t < NT; ++t) g->node_type_names.push_back(std::to_string(t));
 #undef TRY
@@ -621,49 +760,72 @@ static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, dou
   return EU_OK;
 }
 
+// the storage descriptor of the *_dtype constructors (a table of that type in HBM), the dtype checked first
+#define EU_DTYPE_STORAGE(who)                                                                                           \
+  if (!feat_dtype_ok(feat_dtype)) { set_error(who ": unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; } \
+  const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0}
+
 int eu_graph_create_rmat(int64_t n_nodes, int64_t n_edges, double a, double b, double c,
                          uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                          eu_graph** out) {
-  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, EU_FEAT_F32, out);
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, nullptr, out);
 }
 
 int eu_graph_create_rmat_hetero(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
                                 double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                 int shard_index, int shard_number, eu_graph** out) {
   return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, n_edge_types,
-                     n_node_types, EU_FEAT_F32, out);
+                     n_node_types, nullptr, out);
 }
 
 int eu_graph_create_rmat_shard(int64_t n_nodes, int64_t n_edges, double a, double b, double c,
                                uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                int shard_index, int shard_number, eu_graph** out) {
-  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, EU_FEAT_F32,
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, nullptr,
                      out);
 }
 
 int eu_graph_create_rmat_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed, int32_t feat_dim,
                                uint64_t feat_seed, int device, int32_t feat_dtype, eu_graph** out) {
-  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, feat_dtype, out);
+  EU_DTYPE_STORAGE("eu_graph_create_rmat");
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, &st, out);
 }
 
 int eu_graph_create_rmat_shard_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
                                      int32_t feat_dim, uint64_t feat_seed, int device, int shard_index, int shard_number,
                                      int32_t feat_dtype, eu_graph** out) {
-  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, feat_dtype,
-                     out);
+  EU_DTYPE_STORAGE("eu_graph_create_rmat");
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, &st, out);
 }
 
 int eu_graph_create_rmat_hetero_dtype(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
                                       double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                       int shard_index, int shard_number, int32_t feat_dtype, eu_graph** out) {
+  EU_DTYPE_STORAGE("eu_graph_create_rmat");
   return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, n_edge_types,
-                     n_node_types, feat_dtype, out);
+                     n_node_types, &st, out);
+}
+#undef EU_DTYPE_STORAGE
+
+int eu_graph_create_rmat_storage(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
+                                 int32_t feat_dim, uint64_t feat_seed, int device, const eu_feat_storage* storage,
+                                 eu_graph** out) {
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, storage, out);
+}
+
+int eu_graph_create_rmat_hetero_storage(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types,
+                                        double a, double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed,
+                                        int device, int shard_index, int shard_number, const eu_feat_storage* storage,
+                                        eu_graph** out) {
+  return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, n_edge_types,
+                     n_node_types, storage, out);
 }
 
 int eu_graph_destroy(eu_graph* g) {
   if (!g) return EU_OK;
   cudaSetDevice(g->device);
   for (void* p : g->allocs) cudaFree(p);
+  for (void* p : g->host_allocs) cudaFreeHost(p);
   delete g;
   return EU_OK;
 }
@@ -674,7 +836,22 @@ int32_t eu_graph_num_edge_types(const eu_graph* g) { return g ? g->d.T : -1; }
 int32_t eu_graph_num_node_types(const eu_graph* g) { return g ? g->d.n_node_types : -1; }
 int32_t eu_graph_feat_dim(const eu_graph* g) { return g ? g->d.feat_dim : -1; }
 int32_t eu_graph_feat_dtype(const eu_graph* g) { return g ? g->d.feat_dtype : -1; }
+int32_t eu_graph_feat_place(const eu_graph* g) { return g ? g->d.feat_place : -1; }
+int64_t eu_graph_feat_cache_rows(const eu_graph* g) { return g ? g->d.feat_cache_rows : -1; }
 int64_t eu_graph_hbm_bytes(const eu_graph* g) { return g ? g->hbm_bytes : -1; }
+int64_t eu_graph_host_bytes(const eu_graph* g) { return g ? g->host_bytes : -1; }
+
+int eu_graph_export_feat_slots(const eu_graph* g, int32_t* slots) {
+  if (!g || (!slots && g->d.n > 0)) { set_error("eu_graph_export_feat_slots: bad argument"); return EU_ERR_INVALID; }
+  const DevGraph& d = g->d;
+  if (!d.feat_slot) {
+    for (int64_t r = 0; r < d.n; ++r) slots[r] = -1;
+    return EU_OK;
+  }
+  EU_CUDA(cudaSetDevice(g->device));
+  if (d.n > 0) EU_CUDA(cudaMemcpy(slots, d.feat_slot, sizeof(int32_t) * (size_t)d.n, cudaMemcpyDeviceToHost));
+  return EU_OK;
+}
 
 int eu_graph_export(const eu_graph* g, uint64_t* ids, int32_t* node_type, float* node_w,
                     int64_t* grp_ptr, uint64_t* nbr, float* cum_w, float* grp_cum, float* feat) {
@@ -691,7 +868,19 @@ int eu_graph_export(const eu_graph* g, uint64_t* ids, int32_t* node_type, float*
   DL(cum_w, d.cum_w, d.E);
   DL(grp_cum, d.grp_cum, d.n * d.T);
   const int64_t nf = d.n * (int64_t)d.feat_dim;
-  if (d.feat_dtype == EU_FEAT_F32) {
+  if (d.feat_place == EU_FEAT_HOST) {   // the pinned table holds every row (the cache only copies some): read it in place
+    if (feat && nf > 0) {
+      if (d.feat_dtype == EU_FEAT_F32) {
+        memcpy(feat, g->feat_host, sizeof(float) * (size_t)nf);
+      } else {
+        const uint16_t* h = static_cast<const uint16_t*>(g->feat_host);
+        for (int64_t i = 0; i < nf; ++i) {
+          const uint32_t u = (uint32_t)h[i] << 16;
+          memcpy(feat + i, &u, sizeof(u));
+        }
+      }
+    }
+  } else if (d.feat_dtype == EU_FEAT_F32) {
     DL(feat, feat_cols<float>(d), nf);
   } else if (feat && d.feat && nf > 0) {   // widened on the host: the bf16 bits become the f32's upper half
     std::vector<uint16_t> h((size_t)nf);

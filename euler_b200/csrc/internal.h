@@ -34,6 +34,8 @@ extern std::atomic<uint64_t> g_launches;
     }                                                                              \
   } while (0)
 
+static_assert((int)kFeatDevice == (int)EU_FEAT_DEVICE && (int)kFeatHost == (int)EU_FEAT_HOST, "eu_feat_place");
+
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // a table of eu_feat_dtype dtype takes 4-wide loads (16 bytes of f32, 8 of bf16) where p is aligned to four of its elements
 inline bool aligned4_elems(const void* p, int dtype) { return ((uintptr_t)p & (dtype == EU_FEAT_BF16 ? 7 : 15)) == 0; }
@@ -58,6 +60,10 @@ struct eu_graph {
   eu::DevGraph d{};
   std::vector<void*> allocs;
   int64_t hbm_bytes = 0;
+  // mapped pinned host memory (a host-placed feature table: d.feat is its device pointer, feat_host the host one)
+  std::vector<void*> host_allocs;
+  int64_t host_bytes = 0;
+  const void* feat_host = nullptr;
   // global node sampler (Graph::BuildGlobalSampler, graph.cc:333-370); built lazily
   bool sampler_built = false;
   std::vector<eu::TypeSampler> samplers;
@@ -98,6 +104,26 @@ struct eu_graph {
     allocs.push_back(q);
     hbm_bytes += (int64_t)bytes;
     *p = (T*)q;
+    return EU_OK;
+  }
+  // count elements of mapped pinned host memory: *host for the host, *dev for kernels
+  template <typename T>
+  int host_alloc(T** host, T** dev, int64_t count) {
+    const size_t bytes = (size_t)(count > 0 ? count : 1) * sizeof(T);
+    void* q = nullptr;
+    cudaError_t e = cudaHostAlloc(&q, bytes, cudaHostAllocMapped);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      eu::set_error("cudaHostAlloc(%zu, mapped) -> %s", bytes, cudaGetErrorString(e));
+      return EU_ERR_CUDA;
+    }
+    host_allocs.push_back(q);
+    host_bytes += (int64_t)bytes;
+    void* qd = nullptr;
+    e = cudaHostGetDevicePointer(&qd, q, 0);
+    if (e != cudaSuccess) { eu::set_error("cudaHostGetDevicePointer -> %s", cudaGetErrorString(e)); return EU_ERR_CUDA; }
+    *host = (T*)q;
+    *dev = (T*)qd;
     return EU_OK;
   }
 };
@@ -202,6 +228,9 @@ int sparse_entry_ptr(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, vo
 int agg_reserve(eu_ctx* c, int64_t rows, int64_t table_slots);   // the fused SAGE aggregation's dedup scratch
 int refuse_growth_in_capture(eu_ctx* c, const char* what);   // EU_ERR_STATE if the ctx stream is being captured
 int graph_build_sampler(eu_graph* g);
+// graph.cu: *st = the storage descriptor `in` (null: f32 in HBM) once it is valid for a table of n rows; else EU_ERR_INVALID /
+// EU_ERR_UNSUPPORTED naming `who`, before anything is allocated
+int feat_storage_check(const eu_feat_storage* in, int64_t n, const char* who, eu_feat_storage* st);
 int graph_build_labels(eu_graph* g);   // graph_label.cu: the label table (EU_ERR_STATE without a graph_label slot)
 // graph_label.cu: Graph::GetGraphLabel's list (graph.cc:439-457) from the binary slot `fid` (S slots per row) of the rows
 // visited in node_map_ order (`order`, empty = row order); row_label (may be null) gets each row's label index, or L for a

@@ -255,8 +255,8 @@ struct LoadInspect {
   std::vector<std::string> labels;      // then Graph::GetGraphLabel's list
 };
 
-static int load_impl(const char* data_path, int shard_index, int shard_number, int device, int load_edges, int32_t feat_dtype,
-                     eu_graph** out, LoadInspect* inspect) {
+static int load_impl(const char* data_path, int shard_index, int shard_number, int device, int load_edges,
+                     const eu_feat_storage* storage, eu_graph** out, LoadInspect* inspect) {
   if (!data_path || (!out && !inspect) || shard_number <= 0 || shard_index < 0 || shard_index >= shard_number) {
     set_error("eu_graph_load: bad argument (shard %d of %d)", shard_index, shard_number);
     return EU_ERR_INVALID;
@@ -452,7 +452,7 @@ static int load_impl(const char* data_path, int shard_index, int shard_number, i
       }
     return EU_OK;
   }
-  int rc = eu_graph_create_dtype(&d, device, feat_dtype, out);
+  int rc = eu_graph_create_storage(&d, device, storage, out);
   if (rc) return rc;
   eu_graph* g = *out;
   g->edge_type_names.assign(T, "");
@@ -485,14 +485,25 @@ extern "C" int eu_graph_load_dtype(const char* data_path, int shard_index, int s
                                    int32_t feat_dtype, eu_graph** out) {
   if (!out) { set_error("eu_graph_load: bad argument (null out)"); return EU_ERR_INVALID; }
   if (feat_dtype != EU_FEAT_F32 && feat_dtype != EU_FEAT_BF16) { set_error("eu_graph_load: unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; }
-  return load_impl(data_path, shard_index, shard_number, device, load_edges, feat_dtype, out, nullptr);
+  const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0};
+  return load_impl(data_path, shard_index, shard_number, device, load_edges, &st, out, nullptr);
+}
+
+// the descriptor is checked here against every row count (C <= n waits for the files: eu_graph_create_storage checks it)
+extern "C" int eu_graph_load_storage(const char* data_path, int shard_index, int shard_number, int device, int load_edges,
+                                     const eu_feat_storage* storage, eu_graph** out) {
+  if (!out) { set_error("eu_graph_load: bad argument (null out)"); return EU_ERR_INVALID; }
+  eu_feat_storage st;
+  const int rc = feat_storage_check(storage, storage ? storage->cache_rows : 0, "eu_graph_load", &st);
+  if (rc) return rc;
+  return load_impl(data_path, shard_index, shard_number, device, load_edges, &st, out, nullptr);
 }
 
 extern "C" int eu_graph_load_inspect(const char* data_path, int shard_index, int shard_number, int64_t* n_nodes, int64_t* n_edges,
                                      int32_t* n_edge_types, int32_t* n_node_types, int64_t cap, int64_t* order_ids,
                                      int32_t* order_types) {
   LoadInspect li;
-  const int rc = load_impl(data_path, shard_index, shard_number, 0, 0, EU_FEAT_F32, nullptr, &li);
+  const int rc = load_impl(data_path, shard_index, shard_number, 0, 0, nullptr, nullptr, &li);
   if (rc) return rc;
   if (n_nodes) *n_nodes = li.n_nodes;
   if (n_edges) *n_edges = li.n_edges;
@@ -509,7 +520,7 @@ extern "C" int eu_graph_load_inspect(const char* data_path, int shard_index, int
 extern "C" int eu_graph_labels_inspect(const char* data_path, int64_t cap, int64_t* n_labels, int64_t* n_bytes, int64_t* ptr,
                                        uint8_t* bytes) {
   LoadInspect li;
-  const int rc = load_impl(data_path, 0, 1, 0, 0, EU_FEAT_F32, nullptr, &li);
+  const int rc = load_impl(data_path, 0, 1, 0, 0, nullptr, nullptr, &li);
   if (rc) return rc;
   if (!li.has_labels || li.labels.empty()) { set_error("graph label set is empty! (%s has no binary feature graph_label)", data_path); return EU_ERR_STATE; }
   int64_t total = 0;

@@ -33,8 +33,9 @@ __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpre
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 
 // ---------------------------------------------------------------------------- feature fetch
-// out[i, 0:dim] = feat[row(ids[i]), 0:min(feat_dim,dim)], zeros elsewhere / for unknown ids.  T: the table's storage type.
-template <typename T, bool VEC>
+// out[i, 0:dim] = feat[row(ids[i]), 0:min(feat_dim,dim)], zeros elsewhere / for unknown ids.  T: the table's storage type, P
+// its placement.
+template <typename T, bool VEC, int P>
 __global__ void __launch_bounds__(256) k_feature(DevGraph g, const unsigned long long* __restrict__ ids,
                                                  int64_t M, int32_t dim, int G, int32_t soff, int32_t sdim,
                                                  float* __restrict__ out) {
@@ -47,7 +48,7 @@ __global__ void __launch_bounds__(256) k_feature(DevGraph g, const unsigned long
     const int64_t row = sdim > 0 ? lookup_row(g, ids[i]) : -1;
     const int32_t fd = sdim;  // stored width of this slot
     float* o = out + i * (int64_t)dim;
-    const T* f = row >= 0 ? feat_cols<T>(g) + row * (int64_t)g.feat_dim + soff : nullptr;
+    const T* f = row >= 0 ? feat_row<T, P>(g, row) + soff : nullptr;
     if (VEC) {
       for (int32_t d = sub * 4; d < dim; d += G * 4) {
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -246,13 +247,12 @@ __global__ void __launch_bounds__(256) k_sage_classify(DevGraph g, const unsigne
 // per lane are accumulated.
 // NV float4 per lane: rows of up to NV * 128 floats.  FULL: the width is exactly NV * 128 (128 / 256: no column guards, the
 // width is a compile-time constant); otherwise any multiple of 4 up to NV * 128 (e.g. 64 of configs[4]) with guarded columns.
-template <typename T, int NV, bool FULL>
+template <typename T, int NV, bool FULL, int P>
 __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned long long* __restrict__ ids,
                                                    int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
                                                    int32_t count, bool mean, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int32_t fd = FULL ? NV * 128 : g.feat_dim;    // == dim, a multiple of 4, <= NV * 128 (checked by the launcher)
-  const T* __restrict__ feat = feat_cols<T>(g) + lane * 4;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t n = list ? (int64_t)__ldg(n_list) : rows;
   // grid-stride, one warp per output row (the launcher may cap the grid: EU_SAGE_CTAS CTAs per SM)
@@ -277,7 +277,7 @@ __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned lo
           const int j = __ffs(valid) - 1;
           valid &= valid - 1;
           const int32_t row = __shfl_sync(0xffffffffu, my, j);
-          const T* p = feat + (int64_t)row * fd;
+          const T* p = feat_row<T, P>(g, row, fd, lane * 4);
 #pragma unroll
           for (int t = 0; t < NV; ++t) v[q][t] = (FULL || lane * 4 + t * 128 < fd) ? feat_ld4(p + t * 128) : make_float4(0.f, 0.f, 0.f, 0.f);
           n = q + 1;
@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned lo
 }
 
 // generic width fallback: one warp per representative, scalar columns
-template <typename T>
+template <typename T, int P>
 __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const unsigned long long* __restrict__ ids,
                                                            int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
                                                            int32_t count, int32_t dim, bool mean, float* __restrict__ out) {
@@ -322,7 +322,7 @@ __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const uns
       float acc = 0.f;
       for (int32_t j = 0; j < count; ++j) {
         const int64_t row = lookup_row(g, __ldg(ids + r * count + j));
-        acc = __fadd_rn(acc, (row >= 0 && d < fd) ? feat_ld(feat_cols<T>(g) + row * (int64_t)fd + d) : 0.f);
+        acc = __fadd_rn(acc, (row >= 0 && d < fd) ? feat_ld(feat_row<T, P>(g, row, fd, 0) + d) : 0.f);
       }
       out[r * (int64_t)dim + d] = mean ? __fdiv_rn(acc, denom) : acc;
     }
@@ -408,27 +408,27 @@ static int scatter(eu_ctx* c, const float* upd, int64_t D, const int32_t* idx, i
   return EU_OK;
 }
 
-template <typename T>
+template <typename T, int P>
 static int launch_feature(eu_ctx* c, const DevGraph& d, const int64_t* nodes, int64_t M, int32_t dim, int G, bool vec, unsigned blocks,
                           int32_t soff, int32_t sdim, float* out) {
-  if (vec) k_feature<T, true><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
-  else k_feature<T, false><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
+  if (vec) k_feature<T, true, P><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
+  else k_feature<T, false, P><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
   EU_LAUNCHED();
   return EU_OK;
 }
 
-// the fused SAGE reduction over a table of T; v4: the float4 path's conditions hold (fanout_aggregate)
-template <typename T>
+// the fused SAGE reduction over a table of T placed at P; v4: the float4 path's conditions hold (fanout_aggregate)
+template <typename T, int P>
 static int launch_sage_mean(eu_ctx* c, const DevGraph& d, const unsigned long long* ids, int64_t rows, const int32_t* reps,
                             const unsigned int* nrep, int32_t count, int32_t dim, bool mean, bool v4, unsigned blocks, float* out) {
   cudaStream_t s = c->stream;
-  if (v4 && dim == 128) k_sage_mean<T, 1, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim == 256) k_sage_mean<T, 2, true><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 128) k_sage_mean<T, 1, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 256) k_sage_mean<T, 2, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 512) k_sage_mean<T, 4, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4) k_sage_mean<T, 8, false><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else k_sage_mean_generic<T><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, dim, mean, out);
+  if (v4 && dim == 128) k_sage_mean<T, 1, true, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim == 256) k_sage_mean<T, 2, true, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 128) k_sage_mean<T, 1, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 256) k_sage_mean<T, 2, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 512) k_sage_mean<T, 4, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4) k_sage_mean<T, 8, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else k_sage_mean_generic<T, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, dim, mean, out);
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -450,8 +450,12 @@ int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid
   const int G = vec ? group_lanes(dim / 4) : (dim >= 32 ? 32 : 1);
   const unsigned blocks = capped_grid(ceil_div(M * G, 256), "EU_FEATURE_CTAS", 0);
   EuProfScope ps(c, "k_feature", M);
-  if (d.feat_dtype == EU_FEAT_BF16) return launch_feature<__nv_bfloat16>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
-  return launch_feature<float>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
+  const bool host = d.feat_place == EU_FEAT_HOST;
+  if (d.feat_dtype == EU_FEAT_BF16)
+    return host ? launch_feature<__nv_bfloat16, kFeatHost>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out)
+                : launch_feature<__nv_bfloat16, kFeatDevice>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
+  return host ? launch_feature<float, kFeatHost>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out)
+              : launch_feature<float, kFeatDevice>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
 }
 
 int eu_gather(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx, int64_t E, float* out) {
@@ -507,8 +511,11 @@ static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int
     const bool bf16 = d.feat_dtype == EU_FEAT_BF16;
     const bool v4 = d.n < ((int64_t)1 << 31) && d.n_slots == 1 && dim == d.feat_dim && (dim & 3) == 0 && dim <= 1024 && aligned16(out) &&
                     (bf16 ? ((uintptr_t)d.feat & 7) == 0 : aligned16(d.feat));
-    const int rc = bf16 ? launch_sage_mean<__nv_bfloat16>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out)
-                        : launch_sage_mean<float>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out);
+    const bool host = d.feat_place == EU_FEAT_HOST;
+    const int rc = bf16 ? (host ? launch_sage_mean<__nv_bfloat16, kFeatHost>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out)
+                                : launch_sage_mean<__nv_bfloat16, kFeatDevice>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out))
+                        : (host ? launch_sage_mean<float, kFeatHost>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out)
+                                : launch_sage_mean<float, kFeatDevice>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out));
     if (rc) return rc; }
   if (!dedup) return EU_OK;
   { EuProfScope ps(c, "k_sage_broadcast", rows);

@@ -647,6 +647,7 @@ int eu_sym_get_dense_feature(eu_sym* s, const int64_t* ids, int64_t rows, int32_
   const DevGraph& d = c->g->d;
   const int N = s->world;
   if (d.feat_dtype != EU_FEAT_F32) { set_error("eu_sym_get_dense_feature: the sharded feature paths read f32 tables only"); return EU_ERR_UNSUPPORTED; }
+  if (d.feat_place != EU_FEAT_DEVICE) { set_error("eu_sym_get_dense_feature: the sharded feature paths read tables held in HBM only"); return EU_ERR_UNSUPPORTED; }
   if (rows > L.cap || rows > L.max_rows_f || dim > L.max_dim) { set_error("eu_sym_get_dense_feature: request exceeds the symmetric region"); return EU_ERR_INVALID; }
   const bool have = fid >= 0 && fid < d.n_slots;
   const int32_t soff = have ? d.slot_off[fid] : 0, sdim = have ? d.slot_dim[fid] : 0;
@@ -681,6 +682,7 @@ int eu_sym_sage_mean(eu_sym* s, const int64_t* nbr_ids, int64_t rows, int32_t co
   const int N = s->world;
   const int64_t nid = rows * count;
   if (d.feat_dtype != EU_FEAT_F32) { set_error("eu_sym_sage_mean: the sharded feature paths read f32 tables only"); return EU_ERR_UNSUPPORTED; }
+  if (d.feat_place != EU_FEAT_DEVICE) { set_error("eu_sym_sage_mean: the sharded feature paths read tables held in HBM only"); return EU_ERR_UNSUPPORTED; }
   if (nid > L.cap || nid >= ((int64_t)1 << 31) || (int64_t)N * rows * dim > L.max_rows_f * (int64_t)L.max_dim) {
     set_error("eu_sym_sage_mean: %lld x %d ids / %d partial blocks exceed the symmetric region", (long long)rows, count, N);
     return EU_ERR_INVALID;

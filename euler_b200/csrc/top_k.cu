@@ -36,7 +36,7 @@ __device__ __forceinline__ void top_k_insert(float (&t)[KMAX], float v) {
 
 // out[b, 0, :] = the node's row, out[b, 1 + j, d] = the j-th of column d over the count neighbours (j < k <= KMAX).  The
 // slots start at -inf: a slot no value ranks above keeps -inf, which is the value it would have selected (k <= count).
-template <typename T, int KMAX, int C>
+template <typename T, int KMAX, int C, int P>
 __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t B,
                                                            const unsigned long long* __restrict__ nbrs, int32_t count, int32_t soff,
                                                            int32_t width, int32_t dim, int32_t k, float* __restrict__ out) {
@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
   for (int64_t b = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5; b < B; b += nwarps) {
     const unsigned long long* nb = nbrs + b * count;
     const int64_t self = w > 0 ? lookup_row(g, nodes[b]) : -1;
-    const T* fs = self >= 0 ? feat_cols<T>(g) + self * (int64_t)g.feat_dim + soff : nullptr;
+    const T* fs = self >= 0 ? feat_row<T, P>(g, self) + soff : nullptr;
     float* o = out + b * (int64_t)(k + 1) * dim;
     for (int32_t d0 = 0; d0 < dim; d0 += 32 * C) {
       float t[C][KMAX];
@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
         const int64_t mine = (w > 0 && lane < n) ? lookup_row(g, nb[j0 + lane]) : -1;
         for (int32_t j = 0; j < n; ++j) {
           const int64_t row = __shfl_sync(0xffffffffu, mine, j);
-          const T* f = feat_cols<T>(g) + (row >= 0 ? row * (int64_t)g.feat_dim + soff : 0);
+          const T* f = feat_row_if<T, P>(g, row >= 0, row, soff);
           float v[C];
 #pragma unroll
           for (int c = 0; c < C; ++c) {
@@ -89,12 +89,19 @@ static int launch_top_k(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_
   const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(B, 8), (int64_t)kSMs * 32);
   EuProfScope ps(c, "k_neighbor_top_k", B);
   // a bf16 table widens exactly and order-preservingly (+-0 and NaN included): the selection is the f32 one's on the widened rows
-  if (c->g->d.feat_dtype == EU_FEAT_BF16)
-    k_neighbor_top_k<__nv_bfloat16, KMAX, C><<<blocks, 256, 0, c->stream>>>(c->g->d, (const unsigned long long*)nodes, B,
-                                                                            (const unsigned long long*)neighbors, count, soff, width, dim, k, out);
-  else
-    k_neighbor_top_k<float, KMAX, C><<<blocks, 256, 0, c->stream>>>(c->g->d, (const unsigned long long*)nodes, B,
-                                                                    (const unsigned long long*)neighbors, count, soff, width, dim, k, out);
+  const auto* nd = (const unsigned long long*)nodes;
+  const auto* nb = (const unsigned long long*)neighbors;
+  const DevGraph& g = c->g->d;
+  if (g.feat_place == EU_FEAT_HOST) {
+    if (g.feat_dtype == EU_FEAT_BF16)
+      k_neighbor_top_k<__nv_bfloat16, KMAX, C, kFeatHost><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
+    else
+      k_neighbor_top_k<float, KMAX, C, kFeatHost><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
+  } else if (g.feat_dtype == EU_FEAT_BF16) {
+    k_neighbor_top_k<__nv_bfloat16, KMAX, C, kFeatDevice><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
+  } else {
+    k_neighbor_top_k<float, KMAX, C, kFeatDevice><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
+  }
   EU_LAUNCHED();
   return EU_OK;
 }

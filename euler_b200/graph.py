@@ -32,6 +32,22 @@ def feat_dtype_code(feat_dtype):
         raise EulerError("feat_dtype must be one of %s, got %r" % (sorted(_lib.FEAT_DTYPES), feat_dtype)) from None
 
 
+def feat_storage(feat_dtype="float32", feat_place="device", feat_cache_rows=0):
+    """eu_feat_storage of a storage type, a place ('device' or 'host') and a number of HBM cache rows; EulerError for an
+    unknown type or place, a negative or non-integer row count, or a cache beside a device-placed table, before any
+    allocation.  Rows beyond the graph's are refused by the constructor, also before any allocation."""
+    dt = feat_dtype_code(feat_dtype)
+    try:
+        place = _lib.FEAT_PLACES[feat_place]
+    except (KeyError, TypeError):
+        raise EulerError("feat_place must be one of %s, got %r" % (sorted(_lib.FEAT_PLACES), feat_place)) from None
+    if isinstance(feat_cache_rows, bool) or not isinstance(feat_cache_rows, (int, np.integer)) or feat_cache_rows < 0:
+        raise EulerError("feat_cache_rows must be an integer >= 0, got %r" % (feat_cache_rows,))
+    if feat_cache_rows > 0 and feat_place != "host":
+        raise EulerError("feat_cache_rows > 0 needs feat_place='host' (a device-placed table is in HBM already)")
+    return _lib.FeatStorage(dt, place, int(feat_cache_rows))
+
+
 class Graph:
     def __init__(self, handle, device):
         self._h = handle
@@ -42,11 +58,13 @@ class Graph:
     def from_csr(cls, ids, grp_ptr, nbr, n_edge_types=1, cum_w=None, grp_cum=None, w=None,
                  node_type=None, node_w=None, n_node_types=1, feat=None, feat_slot_dims=None,
                  sampler_order=None, device=0, u64_ptr=None, u64_val=None, n_u64_slots=0, bin_ptr=None, bin_val=None,
-                 n_bin_slots=0, binary_feature_names=None, feat_dtype="float32"):
+                 n_bin_slots=0, binary_feature_names=None, feat_dtype="float32", feat_place="device", feat_cache_rows=0):
         """binary_feature_names: one name per binary slot (default bin_0, bin_1, ...); a slot named 'graph_label' holds each
         node's graph label for sample_graph_label / get_graph_by_label.  feat_dtype: the dense table's storage type,
-        'float32' or 'bfloat16' (each value rounded to nearest even on the device; every op reads it widened to f32)."""
-        dt = feat_dtype_code(feat_dtype)
+        'float32' or 'bfloat16' (each value rounded to nearest even on the device; every op reads it widened to f32).
+        feat_place 'host': the table sits in mapped pinned host memory and kernels read it in place, with copies of its
+        feat_cache_rows rows of highest in-degree in HBM; every op returns the bits it returns on the device-placed graph."""
+        st = feat_storage(feat_dtype, feat_place, feat_cache_rows)
         ids = _np(ids, np.uint64)
         keep = [ids, _np(node_type, np.int32), _np(node_w, np.float32), _np(grp_ptr, np.int64),
                 _np(nbr, np.uint64), _np(cum_w, np.float32), _np(grp_cum, np.float32),
@@ -68,19 +86,21 @@ class Graph:
         if n_bin_slots and bin_ptr is not None:
             d.n_bin_slots, d.bin_ptr, d.bin_val = int(n_bin_slots), _ptr(keep[13]), _ptr(keep[14] if len(keep[14]) else np.zeros(1, np.uint8))
         h = C.c_void_p()
-        check(_lib.load().eu_graph_create_dtype(C.byref(d), device, dt, C.byref(h)))
+        check(_lib.load().eu_graph_create_storage(C.byref(d), device, C.byref(st), C.byref(h)))
         g = cls(h, device)
         for k, name in enumerate(binary_feature_names or ()):
             check(_lib.load().eu_graph_set_binary_feature_name(h, k, str(name).encode()))
         return g
 
     @classmethod
-    def rmat(cls, n_nodes, n_edges, a=0.57, b=0.19, c=0.19, seed=42, feat_dim=0, feat_seed=7, device=0, feat_dtype="float32"):
-        """feat_dtype 'bfloat16': the f32 features rounded to bfloat16 on the device."""
-        dt = feat_dtype_code(feat_dtype)
+    def rmat(cls, n_nodes, n_edges, a=0.57, b=0.19, c=0.19, seed=42, feat_dim=0, feat_seed=7, device=0, feat_dtype="float32",
+             feat_place="device", feat_cache_rows=0):
+        """feat_dtype 'bfloat16': the f32 features rounded to bfloat16 on the device.  feat_place / feat_cache_rows: as
+        from_csr."""
+        st = feat_storage(feat_dtype, feat_place, feat_cache_rows)
         h = C.c_void_p()
-        check(_lib.load().eu_graph_create_rmat_dtype(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed,
-                                                     device, dt, C.byref(h)))
+        check(_lib.load().eu_graph_create_rmat_storage(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed,
+                                                       device, C.byref(st), C.byref(h)))
         return cls(h, device)
 
     @classmethod
@@ -95,23 +115,26 @@ class Graph:
 
     @classmethod
     def rmat_hetero(cls, n_nodes, n_edges, n_edge_types, n_node_types, shard_index=0, shard_number=1, a=0.57, b=0.19,
-                    c=0.19, seed=44, feat_dim=0, feat_seed=7, device=0, feat_dtype="float32"):
-        """Heterogeneous R-MAT graph (edge type = hash(edge) % T, node type = id % NT), optionally one shard of it."""
-        dt = feat_dtype_code(feat_dtype)
+                    c=0.19, seed=44, feat_dim=0, feat_seed=7, device=0, feat_dtype="float32", feat_place="device",
+                    feat_cache_rows=0):
+        """Heterogeneous R-MAT graph (edge type = hash(edge) % T, node type = id % NT), optionally one shard of it.
+        feat_place / feat_cache_rows: as from_csr."""
+        st = feat_storage(feat_dtype, feat_place, feat_cache_rows)
         h = C.c_void_p()
-        check(_lib.load().eu_graph_create_rmat_hetero_dtype(n_nodes, n_edges, n_edge_types, n_node_types, a, b, c, seed,
-                                                            feat_dim, feat_seed, device, shard_index, shard_number, dt,
-                                                            C.byref(h)))
+        check(_lib.load().eu_graph_create_rmat_hetero_storage(n_nodes, n_edges, n_edge_types, n_node_types, a, b, c, seed,
+                                                              feat_dim, feat_seed, device, shard_index, shard_number,
+                                                              C.byref(st), C.byref(h)))
         return cls(h, device)
 
     @classmethod
-    def load(cls, data_path, shard_index=0, shard_number=1, device=0, load_edges=True, feat_dtype="float32"):
+    def load(cls, data_path, shard_index=0, shard_number=1, device=0, load_edges=True, feat_dtype="float32",
+             feat_place="device", feat_cache_rows=0):
         """Graph::Init (graph.h:53-56); load_edges=False = load_data_type 'node'; feat_dtype: the node feature table's
-        storage type ('float32' or 'bfloat16')"""
-        dt = feat_dtype_code(feat_dtype)
+        storage type ('float32' or 'bfloat16'); feat_place / feat_cache_rows: as from_csr"""
+        st = feat_storage(feat_dtype, feat_place, feat_cache_rows)
         h = C.c_void_p()
-        check(_lib.load().eu_graph_load_dtype(str(data_path).encode(), shard_index, shard_number, device, int(load_edges),
-                                              dt, C.byref(h)))
+        check(_lib.load().eu_graph_load_storage(str(data_path).encode(), shard_index, shard_number, device, int(load_edges),
+                                                C.byref(st), C.byref(h)))
         return cls(h, device)
 
     def close(self):
@@ -153,8 +176,30 @@ class Graph:
         return {v: k for k, v in _lib.FEAT_DTYPES.items()}[code]
 
     @property
+    def feat_place(self):
+        """'device' or 'host': where the dense node feature table lives"""
+        code = _lib.load().eu_graph_feat_place(self._h)
+        return {v: k for k, v in _lib.FEAT_PLACES.items()}[code]
+
+    @property
+    def feat_cache_rows(self):
+        """rows of a host-placed table copied into HBM (0 for a device-placed one)"""
+        return _lib.load().eu_graph_feat_cache_rows(self._h)
+
+    @property
     def hbm_bytes(self):
         return _lib.load().eu_graph_hbm_bytes(self._h)
+
+    @property
+    def host_bytes(self):
+        """pinned host bytes: the host-placed feature table (0 for a device-placed one)"""
+        return _lib.load().eu_graph_host_bytes(self._h)
+
+    def feat_cache_slots(self):
+        """int32[n]: each row's HBM cache row, or -1 (all -1 for a device-placed table)"""
+        out = np.zeros(self.num_nodes, np.int32)
+        check(_lib.load().eu_graph_export_feat_slots(self._h, _ptr(out)))
+        return out
 
     def edge_type_id(self, name):
         return _lib.load().eu_graph_edge_type_id(self._h, str(name).encode())

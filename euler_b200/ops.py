@@ -16,7 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import EulerError, check
-from .graph import Context, Graph, feat_dtype_code
+from .graph import Context, Graph, feat_dtype_code, feat_storage
 
 _state = threading.local()
 _default = {"graph": None, "rng": "minstd", "seed": 1}
@@ -30,11 +30,21 @@ def initialize_graph(config):
         config = ';'.join('{}={}'.format(key, value) for key, value in config.items())
     if not isinstance(config, str):
         raise TypeError('Expect str or dict for graph config, got {}.'.format(type(config).__name__))
-    # feature_dtype=float32|bfloat16: the node feature table's storage type (Graph.load's feat_dtype), checked before the load
+    # feature_dtype=float32|bfloat16: the node feature table's storage type (Graph.load's feat_dtype); feature_place=device|host
+    # and feature_cache_rows=C: where it lives and how many of its rows are cached in HBM (Graph.load's feat_place and
+    # feat_cache_rows).  All are checked before the load.
+    opts = {}
     for item in config.split(';'):
         key, eq, value = item.partition('=')
-        if key == 'feature_dtype' and eq:
-            feat_dtype_code(value)
+        if key in ('feature_dtype', 'feature_place', 'feature_cache_rows') and eq:
+            opts[key] = value
+    if 'feature_dtype' in opts:
+        feat_dtype_code(opts['feature_dtype'])
+    if 'feature_place' in opts or 'feature_cache_rows' in opts:
+        rows = opts.get('feature_cache_rows', '0')
+        if not rows.isdigit():
+            raise EulerError("feature_cache_rows must be an integer >= 0, got %r" % rows)
+        feat_storage(opts.get('feature_dtype', 'float32'), opts.get('feature_place', 'device'), int(rows))
     lib = _lib.load()
     ok = bool(lib.InitQueryProxy(config.encode()))
     h = lib.eu_default_graph()

@@ -465,13 +465,16 @@ class EulerErrorSharded(RuntimeError):
 
 
 def _f32_features(what, *graphs):
-    """The sharded feature paths read float32 feature tables only: a bfloat16 graph is refused on every rank alike, before
-    any exchange or write."""
+    """The sharded feature paths read float32 feature tables held in HBM only: a bfloat16 or host-placed graph is refused on
+    every rank alike, before any exchange or write."""
     from ._lib import EulerError
     for g in graphs:
         if g is not None and getattr(g, "feat_dtype", "float32") != "float32":
             raise EulerError("%s: the sharded feature paths read float32 feature tables only (this graph stores %s)"
                              % (what, g.feat_dtype))
+        if g is not None and getattr(g, "feat_place", "device") != "device":
+            raise EulerError("%s: the sharded feature paths read feature tables held in HBM only (this graph's is placed on "
+                             "the %s)" % (what, g.feat_place))
 
 
 def _i64(ops):

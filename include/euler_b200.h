@@ -128,6 +128,33 @@ int eu_graph_create_rmat_shard_dtype(int64_t n_nodes, int64_t n_edges, double a,
 int eu_graph_create_rmat_hetero_dtype(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
                                       double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                       int shard_index, int shard_number, int32_t feat_dtype, eu_graph** out);
+/* Where the dense node feature table lives.  EU_FEAT_DEVICE (every constructor above): in HBM.  EU_FEAT_HOST: the whole table
+ * [n, feat_dim] sits in mapped pinned host memory (cudaHostAllocMapped) and kernels read it in place over the host link;
+ * cache_rows = C (0 <= C <= n) rows are also copied once, at build time, into an HBM cache [C, feat_dim], and an int32 slot map
+ * [n] in HBM sends each row to its cache row or to -1.  The cached rows are the C first by (in-degree descending, row
+ * ascending), where a row's in-degree counts the adjacency entries, over all rows and edge types, whose neighbour id is that
+ * row's (ids without a row count for nothing).  Row r is read from the cache when its slot is >= 0 and from the host table
+ * otherwise; both hold the same bits (the table is never written after the build), so every op's output is bit for bit the
+ * one it gives on the same graph held in HBM, whatever C is.  The storage type rules above hold for both places: a bf16 host
+ * table is rounded on the device.
+ * Refusals, before any allocation: an unknown dtype or place, C < 0, C > n, or C > 0 with EU_FEAT_DEVICE: EU_ERR_INVALID; a
+ * host table of 2^31 rows or more: EU_ERR_UNSUPPORTED.  A failed pinned allocation returns EU_ERR_CUDA and frees what was
+ * allocated.  The sharded feature paths (eu_sym_get_dense_feature, eu_sym_sage_mean) refuse a host-placed graph with
+ * EU_ERR_UNSUPPORTED, as they refuse bf16.  A NULL storage descriptor is {EU_FEAT_F32, EU_FEAT_DEVICE, 0}. */
+typedef enum { EU_FEAT_DEVICE = 0, EU_FEAT_HOST = 1 } eu_feat_place;
+typedef struct {
+  int32_t dtype;        /* eu_feat_dtype */
+  int32_t place;        /* eu_feat_place */
+  int64_t cache_rows;   /* rows cached in HBM; 0 unless place is EU_FEAT_HOST */
+} eu_feat_storage;
+int eu_graph_create_storage(const eu_graph_desc* desc, int device, const eu_feat_storage* storage, eu_graph** out);
+int eu_graph_create_rmat_storage(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
+                                 int32_t feat_dim, uint64_t feat_seed, int device, const eu_feat_storage* storage,
+                                 eu_graph** out);
+int eu_graph_create_rmat_hetero_storage(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types,
+                                        double a, double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed,
+                                        int device, int shard_index, int shard_number, const eu_feat_storage* storage,
+                                        eu_graph** out);
 /* Euler 2.0 on-disk format (euler.meta + the Node and Edge partition files; SURVEY.md Appendix B), shard `shard_index` of
  * `shard_number` with the reference's file filter (graph.cc:90-98).  = Graph::Init, graph.h:53-56. */
 int eu_graph_load(const char* data_path, int shard_index, int shard_number, int device,
@@ -139,6 +166,9 @@ int eu_graph_load_ex(const char* data_path, int shard_index, int shard_number, i
 /* eu_graph_load_ex with the node feature table's storage type (eu_feat_dtype) */
 int eu_graph_load_dtype(const char* data_path, int shard_index, int shard_number, int device, int load_edges,
                         int32_t feat_dtype, eu_graph** out);
+/* eu_graph_load_ex with the node feature table's storage descriptor (eu_feat_storage) */
+int eu_graph_load_storage(const char* data_path, int shard_index, int shard_number, int device, int load_edges,
+                          const eu_feat_storage* storage, eu_graph** out);
 /* Edge records (Edge files of the Euler format; euler/core/graph/edge.h): needed only by sample_edge and the edge feature ops.
  * HOST arrays; features use the node layout (dense slots concatenated per edge, ragged uint64 / binary slots).
  * sampler_order: edge rows in the order the reference's edge_map_ iterates (graph.cc:372-399); NULL = row order. */
@@ -182,8 +212,17 @@ int32_t eu_graph_num_node_types(const eu_graph* g);
 int32_t eu_graph_feat_dim(const eu_graph* g);
 /* the eu_feat_dtype of the dense node feature table; -1 for a NULL graph */
 int32_t eu_graph_feat_dtype(const eu_graph* g);
-/* device bytes the graph holds (a bf16 feature table counts 2 bytes per element) */
+/* the eu_feat_place of the dense node feature table, and the rows its HBM cache holds; -1 for a NULL graph */
+int32_t eu_graph_feat_place(const eu_graph* g);
+int64_t eu_graph_feat_cache_rows(const eu_graph* g);
+/* device bytes the graph holds (a bf16 feature table counts 2 bytes per element; a host-placed table counts only its cache
+ * and slot map) */
 int64_t eu_graph_hbm_bytes(const eu_graph* g);
+/* pinned host bytes the graph holds: the host-placed feature table, 0 otherwise; -1 for a NULL graph */
+int64_t eu_graph_host_bytes(const eu_graph* g);
+/* Copy the feature rows' cache slots to the HOST array slots[n]: a row's HBM cache row, or -1.  A device-placed table has no
+ * cache: every slot is -1. */
+int eu_graph_export_feat_slots(const eu_graph* g, int32_t* slots);
 /* Copy the device CSR back to caller-allocated HOST arrays (any pointer may be NULL).  feat is f32 whatever the table's
  * storage type: a bf16 table comes back widened, exactly. */
 int eu_graph_export(const eu_graph* g, uint64_t* ids, int32_t* node_type, float* node_w,
