@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """A training step on float32 against bfloat16 id tables, at one shape, in one run on one GPU: DeepWalk's
 (unsupervised.DeepWalk(table_dtype=...), train_step; the default), a knowledge-graph model's (knowledge.TransE, TransR,
-TransD or DistMult(table_dtype=...), train_step) or a supervised SageEncoder's (encoders.SageEncoder(table_dtype=...),
-optimizers.minimize).
+TransD or DistMult(table_dtype=...), train_step), a supervised SageEncoder's (encoders.SageEncoder(table_dtype=...),
+optimizers.minimize) or a ScalableSageEncoder's over f32 against bf16 embedding stores (store_dtype=..., train_step).
 
     python benchmarks/bf16_tables.py [--model deepwalk] [--nodes N] [--edges E] [--dim D] [--batch B] [--optimizer NAME]
                                      [--steps K] [--warmup W]
@@ -11,6 +11,8 @@ optimizers.minimize).
                                      [--warmup W]
     python benchmarks/bf16_tables.py --model sage [--nodes N] [--edges E] [--dim D] [--batch B] [--lr LR] [--optimizer NAME]
                                      [--steps K] [--warmup W]
+    python benchmarks/bf16_tables.py --model scalable [--nodes N] [--edges E] [--dim D] [--batch B] [--lr LR] [--steps K]
+                                     [--warmup W] [--no-part-b]
 
 DeepWalk: a step is train_step: the walks, pairs and negatives drawn on the device, the fused skip-gram forward, its sparse
 backward, and the optimizer's fused update of both tables and their slots (bf16: stochastic rounding on every store), on an
@@ -27,7 +29,18 @@ backward, and the optimizer's update of the dense parameters and every table and
 Both arms draw the same ids (the sampler is reseeded before each step of each arm) and start from the same tables (the
 f32 arm holds the bf16 arm's widened values).  The arms alternate round by round, timed with device events.  Reported per
 arm: ms per step, the tables' and slots' bytes, and the mean loss of the timed steps; the card's name, power limit and max
-SM clock are read in the same run.  One JSON line on stdout.  It needs a GPU: without one it fails."""
+SM clock are read in the same run.  One JSON line on stdout.  It needs a GPU: without one it fails.
+
+ScalableSageEncoder (--model scalable), part A: the configuration of benchmarks/scalable_encoder.py -- the 10M-node /
+100M-edge R-MAT with its 128-column dense slot, 2 layers at dim 128, fanout 10, 'mean', batch 8192, a Linear(128, 16) head
+on seeded labels and SGD at lr 0.01 -- with f32 stores against bf16 stores (store_dtype=torch.bfloat16).  A step is
+forward(training=True), the loss and train_step; the f32 arm starts from the bf16 arm's widened stores, both arms draw the
+same seeds and the sampler is reseeded per step.  Reported per arm: ms per step, the two store ops alone (store_exchange over
+the batch, store_accumulate over the hop with count 10 and 'mean'), the store pair's bytes and the mean loss; all timed
+arms alternate round by round.  Part B: the headline graph, the 50M-node / 500M-edge R-MAT with bf16 features of 256
+columns, and the same 2-layer encoder over them.  The store pair's bytes, and the f32 initialisation each bf16 store is rounded from, are computed from the
+shapes and compared with the free device memory after the graph is built: each arm that fits runs on its own, and an arm that
+does not is reported as not fitting from that arithmetic, never by attempting the allocation."""
 import argparse
 import os
 import sys
@@ -46,7 +59,7 @@ KG_MODELS = {"transe": "TransE", "transr": "TransR", "transd": "TransD", "distmu
 
 def parse(argv=None):
     p = argparse.ArgumentParser()
-    p.add_argument("--model", default="deepwalk", choices=["deepwalk", "sage"] + sorted(KG_MODELS))
+    p.add_argument("--model", default="deepwalk", choices=["deepwalk", "sage", "scalable"] + sorted(KG_MODELS))
     p.add_argument("--nodes", type=int, default=10_000_000)
     p.add_argument("--edges", type=int, default=100_000_000)
     p.add_argument("--triples", type=int, default=10_000_000)
@@ -59,12 +72,13 @@ def parse(argv=None):
     p.add_argument("--optimizer", default="adam")
     p.add_argument("--steps", type=int, default=20)
     p.add_argument("--warmup", type=int, default=3)
+    p.add_argument("--no-part-b", action="store_true", help="--model scalable: skip the 50M-node part")
     args = p.parse_args(argv)
-    kg = args.model not in ("deepwalk", "sage")
+    kg = args.model not in ("deepwalk", "sage", "scalable")
     if args.batch is None:
-        args.batch = 8192 if kg else 512
+        args.batch = 8192 if kg or args.model == "scalable" else 512
     if args.lr is None:
-        args.lr = 0.01 if args.model == "deepwalk" else 0.001
+        args.lr = 0.01 if args.model in ("deepwalk", "scalable") else 0.001
     return args
 
 
@@ -115,12 +129,176 @@ def sage_model(args, dt):
     return SupervisedSage()
 
 
+SCALABLE_LABELS = 16
+SCALABLE_FANOUT = 10
+
+
+def store_pair_bytes(n_nodes, dim, dt):
+    """one layer's store and gradient store, [n_nodes + 2, dim] each"""
+    return 2 * (n_nodes + 2) * dim * (2 if dt == "bf16" else 4)
+
+
+def init_peak_bytes(n_nodes, dim, dt):
+    """the most the stores of a 2-layer encoder hold while they are built: a bf16 store is rounded from an f32 one, which
+    lives until the bf16 copy exists, and its gradient store comes after"""
+    row = (n_nodes + 2) * dim
+    return 4 * row + 2 * row if dt == "bf16" else 2 * 4 * row
+
+
+def scalable_arms(args, n_nodes, feature, dts, steps, warmup, store_ops=True):
+    """ScalableSageEncoder train steps (and the store ops alone) for each store dtype of dts on the installed graph, the f32
+    arm from the bf16 arm's widened stores; {dt: {...}} of ms per step, store-op ms, store bytes and mean loss"""
+    import numpy as np
+    import torch
+    import euler_b200 as eb
+    from euler_b200.encoders import ScalableSageEncoder
+    fid, fdim = feature
+    labels = (torch.rand(args.batch, SCALABLE_LABELS, generator=torch.Generator().manual_seed(3)) < 0.5).float().cuda()
+    encs, heads, opts = {}, {}, {}
+    for k in dts:
+        torch.manual_seed(0)
+        encs[k] = ScalableSageEncoder([0], SCALABLE_FANOUT, 2, args.dim, aggregator="mean", feature_idx=[fid], feature_dim=[fdim],
+                                      max_id=n_nodes, device="cuda", generator=torch.Generator(device="cuda").manual_seed(1),
+                                      store_dtype=torch.bfloat16 if k == "bf16" else torch.float32, store_seed=5)
+        heads[k] = torch.nn.Linear(args.dim, SCALABLE_LABELS).cuda()
+        opts[k] = torch.optim.SGD(list(encs[k].parameters()) + list(heads[k].parameters()), lr=args.lr)
+    if "bf16" in encs and "f32" in encs:
+        with torch.no_grad():
+            for a, b in zip(encs["f32"].stores, encs["bf16"].stores):
+                a.copy_(b.float())
+    torch.cuda.empty_cache()
+    batches = [torch.from_numpy(np.random.RandomState(100 + i).randint(1, n_nodes + 1, size=args.batch)).cuda()
+               for i in range(warmup + steps)]
+    losses = {k: [] for k in encs}
+    nxt = {k: 0 for k in encs}
+
+    def train(k):
+        i = nxt[k] % len(batches)
+        nxt[k] += 1
+        eb.seed(1000 + i)                      # the sampler reseeded per step: both arms draw the same hop
+        enc = encs[k]
+        loss = torch.nn.functional.binary_cross_entropy_with_logits(heads[k](enc(batches[i], training=True)), labels)
+        enc.train_step(loss, opts[k])
+        losses[k].append(loss.detach())
+
+    eb.seed(7)
+    node, neighbor = eb.sample_fanout(batches[0], [[0]], [SCALABLE_FANOUT], default_node=n_nodes + 1)[0]
+    gen = torch.Generator(device="cuda").manual_seed(4)
+    rows = torch.randn(node.numel(), args.dim, device="cuda", generator=gen)
+    grad = torch.randn(node.numel(), args.dim, device="cuda", generator=gen)
+    counter = torch.zeros((), dtype=torch.int64, device="cuda")
+
+    def ops_of(k):
+        store, gs = encs[k].stores[0], encs[k].gradient_stores[0]
+        sr = dict(seed=5, step=counter, tensor=0) if k == "bf16" else {}
+
+        def run():
+            eb.store_exchange(store, gs, node, rows)
+            eb.store_accumulate(gs, neighbor, grad, SCALABLE_FANOUT, "mean", **sr)
+        return run
+
+    arms = {("step", k): (lambda k=k: train(k)) for k in encs}
+    if store_ops:
+        arms.update({("store_ops", k): ops_of(k) for k in encs})
+    for _ in range(warmup):
+        for fn in arms.values():
+            fn()
+    torch.cuda.synchronize()
+    for k in losses:
+        losses[k].clear()
+    rounds = max(1, min(5, steps))
+    per = -(-steps // rounds)
+    tot = {a: [0.0, 0] for a in arms}
+    for _ in range(rounds):
+        for a, fn in arms.items():
+            torch.cuda.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(per):
+                fn()
+            e1.record()
+            torch.cuda.synchronize()
+            tot[a][0] += e0.elapsed_time(e1)
+            tot[a][1] += per
+    out = {}
+    for k in encs:
+        ms, n = tot[("step", k)]
+        out[k] = {"ms_per_step": ms / n, "steps": n, "store_pair_bytes": sum(t.numel() * t.element_size()
+                                                                             for t in encs[k].stores + encs[k].gradient_stores),
+                  "mean_loss": float(np.mean([float(x) for x in losses[k]]))}
+        if store_ops:
+            ms, n = tot[("store_ops", k)]
+            out[k]["store_ops_ms"] = ms / n
+    return out
+
+
+def run_scalable(args):
+    import torch
+    import euler_b200 as eb
+    torch.cuda.set_device(0)
+    import shallow_encoder
+    shallow_encoder.torch = torch
+    from shallow_encoder import DENSE_DIM
+    out = {"workload": "scalable_sage_train_step", "gpu": gpu_info(0), "dim": args.dim, "fanout": SCALABLE_FANOUT, "layers": 2,
+           "aggregator": "mean", "batch": args.batch, "optimizer": "sgd", "lr": args.lr}
+    g = shallow_encoder.build_graph(args)
+    a = scalable_arms(args, args.nodes, ("feat0", DENSE_DIM), ("bf16", "f32"), args.steps, args.warmup)
+    a["bf16_over_f32_time"] = a["bf16"]["ms_per_step"] / a["f32"]["ms_per_step"]
+    a["bf16_over_f32_store_ops_time"] = a["bf16"]["store_ops_ms"] / a["f32"]["store_ops_ms"]
+    out["part_a"] = dict(graph="rmat %d nodes / %d edges, feat_dim %d f32" % (args.nodes, args.edges, DENSE_DIM), **a)
+    g.close()
+    del g
+    import gc
+    gc.collect()
+    torch.cuda.empty_cache()
+    if not args.no_part_b:
+        out["part_b"] = scalable_part_b(args)
+    emit(out)
+
+
+def scalable_part_b(args):
+    """the headline graph: fit from the arithmetic, then the arms that fit"""
+    import gc
+    import time
+    import torch
+    import euler_b200 as eb
+    n, E = 50_000_000, 500_000_000
+    D = 256
+    res = {"graph": "rmat %d nodes / %d edges, feat_dim %d bf16" % (n, E, D)}
+    t0 = time.time()
+    g = eb.Graph.rmat(n, E, seed=11, feat_dim=D, feat_dtype="bfloat16")
+    torch.cuda.synchronize()
+    eb.set_graph(g, rng="philox", seed=5)
+    free, total = torch.cuda.mem_get_info()
+    spare = 2 << 30                      # the step's own buffers: batch, hop, plan scratch, the head
+    res.update(build_s=round(time.time() - t0, 1), graph_hbm_bytes=g.hbm_bytes, free_after_graph_bytes=free, device_bytes=total)
+    fits = []
+    for dt in ("bf16", "f32"):
+        need = max(store_pair_bytes(n, args.dim, dt), init_peak_bytes(n, args.dim, dt)) + spare
+        ok = need <= free
+        res[dt] = {"store_pair_bytes": store_pair_bytes(n, args.dim, dt), "init_peak_bytes": init_peak_bytes(n, args.dim, dt),
+                   "needed_bytes": need, "fits": ok}
+        if ok:
+            fits.append(dt)
+        else:
+            res[dt]["result"] = "does not fit: %.1f GB needed beside the graph, %.1f GB free" % (need / 1e9, free / 1e9)
+    for dt in fits:                      # one arm at a time: the two pairs together are not the question here
+        r = scalable_arms(args, n, (0, D), (dt,), max(1, args.steps // 2), min(args.warmup, 2), store_ops=False)[dt]
+        res[dt].update(r)
+        gc.collect()
+        torch.cuda.empty_cache()
+    g.close()
+    return res
+
+
 def run(args):
     import numpy as np
     import torch
     import euler_b200 as eb
     from euler_b200 import knowledge, optimizers, unsupervised as un
     torch.cuda.set_device(0)
+    if args.model == "scalable":
+        return run_scalable(args)
     kg = args.model not in ("deepwalk", "sage")
     sage = args.model == "sage"
     if kg:

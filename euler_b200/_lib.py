@@ -230,6 +230,8 @@ SIGNATURES = {
     "eu_shallow_encode_pool_backward_sparse": (C.c_int, [_P, _P, _I32, _I32, _P, _P, _P, _P]),
     "eu_store_exchange": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _I64, _P, _P]),
     "eu_store_accumulate": (C.c_int, [_P, _P, _I64, _I32, _P, _I64, _I32, _I32, _P]),
+    "eu_store_exchange_dtype": (C.c_int, [_P, _P, _P, _I64, _I32, _P, _I64, _P, _P, _I32]),
+    "eu_store_accumulate_dtype": (C.c_int, [_P, _P, _I64, _I32, _P, _I64, _I32, _I32, _P, _I32, _U64, _P, _I32]),
     "eu_gather_host": (C.c_int, [_P, _P, _I64, _I64, _P, _I64, _P]),
     "eu_scatter_add_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),
     "eu_scatter_max_host": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),

@@ -23,6 +23,16 @@
 // Both calls check the ids (one flag, one read-back) before anything is written; under CUDA-graph capture the check is
 // skipped, and an id outside the table is then routed to a virtual row n_rows that is never read or written (its taken
 // rows are NaN).  No other host synchronisation.
+//
+// bf16 stores (T = __nv_bfloat16, the *_dtype entry points: store and grad_store both bf16; rows, taken and grad stay f32).
+// Every read widens a stored element exactly to f32; only the writes round.  The exchange's store row is an overwrite, so it
+// is rounded to nearest even (feat_st); taken is the gradient row as it was, widened; the cleared row is exact zeros.  The
+// accumulation adds the same f32 sum S_v to the widened stored value with the same __fadd_rn and writes it by stochastic
+// rounding (sr_st), its 16 random bits the low half of word 0 of philox_bits(seed, *step, tensor, v dim + f), so an add
+// smaller than half an ulp is kept on average.  step is a device counter read on the device: a captured graph replays with
+// the live value.  The 4-wide path needs the bf16 tables aligned to four elements (8 bytes) and rows / taken to 16 bytes.
+#include <type_traits>
+
 #include "segment.cuh"
 
 namespace eu {
@@ -39,26 +49,57 @@ __global__ void k_store_keys(const int64_t* __restrict__ ids, int64_t M, int64_t
   }
 }
 
-// columns [d, d + 4) of a row (fewer at its end): one float4 store (VEC) or up to four scalar stores
-template <bool VEC>
-__device__ __forceinline__ void row_store4(float* __restrict__ row, int d, int dim, float4 v) {
+// columns [d, d + 4) of a row of T (fewer at its end), each value rounded to nearest by feat_st: one 4-wide store (VEC: a
+// float4, or 8 bytes of bf16) or up to four scalar stores
+template <bool VEC, typename T>
+__device__ __forceinline__ void row_store4(T* __restrict__ row, int d, int dim, float4 v) {
   if (VEC) {
-    *reinterpret_cast<float4*>(row + d) = v;
+    if constexpr (std::is_same<T, float>::value) {
+      *reinterpret_cast<float4*>(row + d) = v;
+    } else {
+      const uint32_t lo = __bfloat16_as_ushort(feat_st<T>(v.x)) | (uint32_t)__bfloat16_as_ushort(feat_st<T>(v.y)) << 16;
+      const uint32_t hi = __bfloat16_as_ushort(feat_st<T>(v.z)) | (uint32_t)__bfloat16_as_ushort(feat_st<T>(v.w)) << 16;
+      *reinterpret_cast<uint2*>(row + d) = make_uint2(lo, hi);
+    }
     return;
   }
-  row[d] = v.x;
-  if (d + 1 < dim) row[d + 1] = v.y;
-  if (d + 2 < dim) row[d + 2] = v.z;
-  if (d + 3 < dim) row[d + 3] = v.w;
+  row[d] = feat_st<T>(v.x);
+  if (d + 1 < dim) row[d + 1] = feat_st<T>(v.y);
+  if (d + 2 < dim) row[d + 2] = feat_st<T>(v.z);
+  if (d + 3 < dim) row[d + 3] = feat_st<T>(v.w);
+}
+
+// one element of a table of T, widened to f32, through the read-write path (the table is written by the same kernel)
+__device__ __forceinline__ float store_ld(const float* p) { return *p; }
+__device__ __forceinline__ float store_ld(const __nv_bfloat16* p) {
+  return __uint_as_float((uint32_t)*reinterpret_cast<const unsigned short*>(p) << 16);
+}
+
+// columns [d, d + 4) of a row of T widened to f32 through the read-write path (0 past the row's end): one 4-wide load (VEC)
+// or up to four scalar loads
+template <bool VEC, typename T>
+__device__ __forceinline__ float4 store_ld4(const T* row, int d, int dim) {
+  if constexpr (std::is_same<T, float>::value) {
+    return VEC ? *reinterpret_cast<const float4*>(row + d) : make_float4(row[d], d + 1 < dim ? row[d + 1] : 0.f,
+                                                                         d + 2 < dim ? row[d + 2] : 0.f, d + 3 < dim ? row[d + 3] : 0.f);
+  } else {
+    if (VEC) {
+      const uint2 u = *reinterpret_cast<const uint2*>(row + d);
+      return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                         __uint_as_float(u.y & 0xFFFF0000u));
+    }
+    return make_float4(store_ld(row + d), d + 1 < dim ? store_ld(row + d + 1) : 0.f, d + 2 < dim ? store_ld(row + d + 2) : 0.f,
+                       d + 3 < dim ? store_ld(row + d + 3) : 0.f);
+  }
 }
 
 // G lanes per distinct id p of the plan (segment [start[p], start[p + 1]) of the stable order perm), 4 columns per lane and
 // step.  The group reads the gradient row before it clears it; the stores' rows are written but never read here, so the
-// loads of grad_store and rows go through the read-write path.
-template <bool VEC>
+// loads of grad_store and rows go through the read-write path.  T: the stores' type.
+template <bool VEC, typename T>
 __global__ void __launch_bounds__(256) k_store_exchange(DistinctPlan P, const int32_t* __restrict__ perm, int64_t n_rows, int dim,
-                                                        int G, const float* __restrict__ rows, float* __restrict__ store,
-                                                        float* __restrict__ grad_store, float* __restrict__ taken) {
+                                                        int G, const float* __restrict__ rows, T* __restrict__ store,
+                                                        T* __restrict__ grad_store, float* __restrict__ taken) {
   const int lg = 31 - __clz(G);
   const int sub = (int)(threadIdx.x & (G - 1));
   const int64_t D = __ldg(P.nd);
@@ -69,14 +110,13 @@ __global__ void __launch_bounds__(256) k_store_exchange(DistinctPlan P, const in
     const int64_t v = __ldg(P.key + p);
     const int64_t k0 = __ldg(P.start + p), k1 = __ldg(P.start + p + 1);
     const bool real = v < n_rows;   // false only under capture: the virtual row of the ids outside the table
-    float* s = store + v * dim;
-    float* gs = grad_store + v * dim;
+    T* s = store + v * dim;
+    T* gs = grad_store + v * dim;
     const float* last = rows + (int64_t)__ldg(perm + k1 - 1) * dim;
     for (int d = sub * 4; d < dim; d += G * 4) {
       float4 g = nan4;
       if (real) {
-        g = VEC ? *reinterpret_cast<const float4*>(gs + d) : make_float4(gs[d], d + 1 < dim ? gs[d + 1] : 0.f,
-                                                                          d + 2 < dim ? gs[d + 2] : 0.f, d + 3 < dim ? gs[d + 3] : 0.f);
+        g = store_ld4<VEC>(gs, d, dim);
         row_store4<VEC>(s, d, dim, row_load4<VEC>(last, d, dim));
         row_store4<VEC>(gs, d, dim, make_float4(0.f, 0.f, 0.f, 0.f));
       }
@@ -85,13 +125,24 @@ __global__ void __launch_bounds__(256) k_store_exchange(DistinctPlan P, const in
   }
 }
 
-// grad_store[key[p]] = __fadd_rn(grad_store[key[p]], vals[p]) elementwise, for the distinct ids p < *nd (not the virtual row)
-__global__ void k_store_add(DistinctPlan P, int64_t n_rows, int dim, const float* __restrict__ vals, float* __restrict__ grad_store) {
+// grad_store[key[p]] = __fadd_rn(grad_store[key[p]], vals[p]) elementwise, for the distinct ids p < *nd (not the virtual row).
+// T = bf16: the stored value is widened, and the sum written by stochastic rounding keyed (seed, *step, tensor, element);
+// the f32 kernel never reads the key, which follows its parameters so theirs keep their offsets.
+template <typename T>
+__global__ void k_store_add(DistinctPlan P, int64_t n_rows, int dim, const float* __restrict__ vals, T* __restrict__ grad_store,
+                            unsigned long long seed, const int64_t* __restrict__ step, uint32_t tensor) {
   const int64_t D = __ldg(P.nd);
+  uint32_t s32 = 0;
+  if constexpr (!std::is_same<T, float>::value) s32 = (uint32_t)__ldg(step);
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D * dim; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t p = t / dim, f = t - p * dim;
     const int64_t v = __ldg(P.key + p);
-    if (v < n_rows) grad_store[v * dim + f] = __fadd_rn(grad_store[v * dim + f], __ldg(vals + t));
+    if (v < n_rows) {
+      const int64_t e = v * dim + f;
+      const float x = __fadd_rn(store_ld(grad_store + e), __ldg(vals + t));
+      if constexpr (std::is_same<T, float>::value) grad_store[e] = x;
+      else grad_store[e] = sr_st(x, philox_bits(seed, s32, tensor, (unsigned long long)e).x);
+    }
   }
 }
 
@@ -141,17 +192,16 @@ static int store_plan(eu_ctx* c, const int64_t* ids, int64_t M, int64_t n_rows, 
   return plan_rows(c, m + o_plan, L);
 }
 
-}  // namespace eu
+static bool store_dtype_ok(int32_t dtype) { return dtype == EU_FEAT_F32 || dtype == EU_FEAT_BF16; }
 
-using namespace eu;
-
-extern "C" {
-
-int eu_store_exchange(eu_ctx* c, float* store, float* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
-                      const float* rows, float* taken) {
-  const char* who = "eu_store_exchange";
+static int store_exchange(eu_ctx* c, void* store, void* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
+                          const float* rows, float* taken, int32_t dtype, const char* who) {
   int rc = store_check(c, store && grad_store && (M == 0 || (ids && rows && taken)), n_rows, dim, M, who);
   if (rc) return rc;
+  if (!store_dtype_ok(dtype)) {
+    set_error("%s: unknown store dtype %d (EU_FEAT_F32 or EU_FEAT_BF16)", who, (int)dtype);
+    return EU_ERR_INVALID;
+  }
   EU_CUDA(cudaSetDevice(c->g->device));
   if (M == 0) return EU_OK;
   RowList L;
@@ -161,23 +211,35 @@ int eu_store_exchange(eu_ctx* c, float* store, float* grad_store, int64_t n_rows
     EuProfScope ps(c, "store_exchange_plan", M);
     if ((rc = store_plan(c, ids, M, n_rows, dim, false, 0, &L, &node, &vals, who))) return rc;
   }
-  const bool vec = dim % 4 == 0 && aligned16(store) && aligned16(grad_store) && aligned16(rows) && aligned16(taken);
+  const bool vec = dim % 4 == 0 && aligned4_elems(store, dtype) && aligned4_elems(grad_store, dtype) && aligned16(rows) &&
+                   aligned16(taken);
   const int G = group_lanes(ceil_div(dim, 4));
   EuProfScope ps(c, "store_exchange", M);
-  auto k = vec ? k_store_exchange<true> : k_store_exchange<false>;
-  k<<<stride_grid(M * G), 256, 0, c->stream>>>(L.P, L.ord.perm, n_rows, dim, G, rows, store, grad_store, taken);
+  if (dtype == EU_FEAT_BF16) {
+    auto k = vec ? k_store_exchange<true, __nv_bfloat16> : k_store_exchange<false, __nv_bfloat16>;
+    k<<<stride_grid(M * G), 256, 0, c->stream>>>(L.P, L.ord.perm, n_rows, dim, G, rows, (__nv_bfloat16*)store,
+                                                 (__nv_bfloat16*)grad_store, taken);
+  } else {
+    auto k = vec ? k_store_exchange<true, float> : k_store_exchange<false, float>;
+    k<<<stride_grid(M * G), 256, 0, c->stream>>>(L.P, L.ord.perm, n_rows, dim, G, rows, (float*)store, (float*)grad_store, taken);
+  }
   EU_LAUNCHED();
   return EU_OK;
 }
 
-int eu_store_accumulate(eu_ctx* c, float* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M, int32_t count,
-                        int32_t pool, const float* grad) {
-  const char* who = "eu_store_accumulate";
+static int store_accumulate(eu_ctx* c, void* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M, int32_t count,
+                            int32_t pool, const float* grad, int32_t dtype, uint64_t seed, const int64_t* step, int32_t tensor,
+                            const char* who) {
   int rc = store_check(c, grad_store && (M == 0 || (ids && grad)), n_rows, dim, M, who);
   if (rc) return rc;
   if (count < 1 || M % count || (pool != EU_POOL_SUM && pool != EU_POOL_MEAN)) {
     set_error("%s: count = %d must be at least 1 and divide M = %lld, pool must be EU_POOL_SUM or EU_POOL_MEAN", who, (int)count,
               (long long)M);
+    return EU_ERR_INVALID;
+  }
+  if (!store_dtype_ok(dtype) || (dtype == EU_FEAT_BF16 && !step)) {
+    set_error("%s: bad argument (dtype EU_FEAT_F32 or EU_FEAT_BF16, and a bf16 gradient store needs the device step counter)",
+              who);
     return EU_ERR_INVALID;
   }
   EU_CUDA(cudaSetDevice(c->g->device));
@@ -198,9 +260,41 @@ int eu_store_accumulate(eu_ctx* c, float* grad_store, int64_t n_rows, int32_t di
   R.group = count;
   R.pool_den = pool == EU_POOL_MEAN ? (float)count : 0.f;
   if ((rc = sum_distinct_rows(c, R, L, dim, false, vals, nullptr))) return rc;
-  k_store_add<<<stride_grid(M * dim), 256, 0, c->stream>>>(L.P, n_rows, dim, vals, grad_store);
+  if (dtype == EU_FEAT_BF16)
+    k_store_add<__nv_bfloat16><<<stride_grid(M * dim), 256, 0, c->stream>>>(L.P, n_rows, dim, vals, (__nv_bfloat16*)grad_store,
+                                                                            seed, step, (uint32_t)tensor);
+  else
+    k_store_add<float><<<stride_grid(M * dim), 256, 0, c->stream>>>(L.P, n_rows, dim, vals, (float*)grad_store, 0, nullptr, 0);
   EU_LAUNCHED();
   return EU_OK;
+}
+
+}  // namespace eu
+
+using namespace eu;
+
+extern "C" {
+
+int eu_store_exchange(eu_ctx* c, float* store, float* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
+                      const float* rows, float* taken) {
+  return store_exchange(c, store, grad_store, n_rows, dim, ids, M, rows, taken, EU_FEAT_F32, "eu_store_exchange");
+}
+
+int eu_store_accumulate(eu_ctx* c, float* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M, int32_t count,
+                        int32_t pool, const float* grad) {
+  return store_accumulate(c, grad_store, n_rows, dim, ids, M, count, pool, grad, EU_FEAT_F32, 0, nullptr, 0, "eu_store_accumulate");
+}
+
+int eu_store_exchange_dtype(eu_ctx* c, void* store, void* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
+                            const float* rows, float* taken, int32_t dtype) {
+  return store_exchange(c, store, grad_store, n_rows, dim, ids, M, rows, taken, dtype, "eu_store_exchange_dtype");
+}
+
+int eu_store_accumulate_dtype(eu_ctx* c, void* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
+                              int32_t count, int32_t pool, const float* grad, int32_t dtype, uint64_t seed, const int64_t* step,
+                              int32_t tensor) {
+  return store_accumulate(c, grad_store, n_rows, dim, ids, M, count, pool, grad, dtype, seed, step, tensor,
+                          "eu_store_accumulate_dtype");
 }
 
 }  // extern "C"

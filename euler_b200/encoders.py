@@ -631,9 +631,20 @@ def _exchange_composed(store, grad_store, ids, rows):
 
 
 def _scalable_f32(table_dtype):
-    """the scalable encoders train their stores and node-encoder tables in f32 only (train_step steps them through .grad)"""
+    """the scalable encoders train their node-encoder tables in f32 only (train_step steps them through .grad)"""
     if table_dtype != torch.float32:
         raise ValueError("the scalable encoders train float32 tables only, got table_dtype=%r" % (table_dtype,))
+
+
+def _scalable_store_args(store_dtype, store_seed, fused):
+    """the stores' dtype and stochastic-rounding seed, checked before anything is allocated: float32, or bfloat16 with the
+    fused store ops (the literal composition would round every accumulation to nearest)"""
+    if store_dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError("store_dtype must be torch.float32 or torch.bfloat16, got %r" % (store_dtype,))
+    if store_dtype == torch.bfloat16 and not fused:
+        raise ValueError("store_dtype=torch.bfloat16 needs fused=True")
+    if not isinstance(store_seed, (int, np.integer)) or not 0 <= int(store_seed) < 2 ** 64:
+        raise ValueError("store_seed must be an integer in [0, 2^64), got %r" % (store_seed,))
 
 
 class _ScalableStores(torch.nn.Module):
@@ -649,18 +660,30 @@ class _ScalableStores(torch.nn.Module):
       3. train_step(loss, optimizer) adds d(loss + store_loss) / d(each layer's neighbour store rows) into gradient_stores
          (every id gets the fixed-order sum of its entries, added with one rounding), computes d loss / d params for
          `optimizer` and d store_loss / d params for store_optimizer from the same parameters, then steps both.
+
+    store_dtype=torch.bfloat16 keeps every store and gradient store in bfloat16, half the bytes (fused only).  Each store is
+    initialised in f32 exactly as an f32 one and rounded once to nearest; the gradient stores are zeros.  Reads widen
+    exactly, so the forward is the f32 encoder's on the widened stores; the exchange rounds the written store rows to
+    nearest, and each accumulation is written by stochastic rounding keyed by (store_seed, store_sr_step, layer, element).
+    store_sr_step, an int64 device counter (a non-persistent buffer), advances once per train_step, after every layer.
     """
 
-    def _init_stores(self, widths, max_id, store_learning_rate, store_init_maxval, generator, device):
+    def _init_stores(self, widths, max_id, store_learning_rate, store_init_maxval, generator, device,
+                     store_dtype=torch.float32, store_seed=0):
         self.max_id = max_id
         self.store_learning_rate = store_learning_rate
         self.store_init_maxval = store_init_maxval
+        self.store_dtype = store_dtype
+        self.store_seed = int(store_seed)
         self._n_stores = len(widths)
         for l, w in enumerate(widths):
             # upstream's tables are LOCAL_VARIABLES, which its Saver does not checkpoint: non-persistent buffers
             store = torch.empty((max_id + 2, w), device=device).uniform_(0, store_init_maxval, generator=generator)
-            self.register_buffer('store_%d' % l, store, persistent=False)
-            self.register_buffer('gradient_store_%d' % l, torch.zeros((max_id + 2, w), device=device), persistent=False)
+            self.register_buffer('store_%d' % l, store.to(store_dtype), persistent=False)
+            del store   # a bf16 store's f32 initialisation is freed before its gradient store is made
+            self.register_buffer('gradient_store_%d' % l, torch.zeros((max_id + 2, w), dtype=store_dtype, device=device),
+                                 persistent=False)
+        self.register_buffer('store_sr_step', torch.zeros((), dtype=torch.int64, device=device), persistent=False)
         self.store_optimizer = torch.optim.Adam(self.parameters(), lr=store_learning_rate)
         self.store_loss = None
         self._neigh_rows = []
@@ -710,15 +733,19 @@ class _ScalableStores(torch.nn.Module):
         store_grads = [None] * len(params)
         if self.store_loss.requires_grad:
             store_grads = torch.autograd.grad(self.store_loss, params, retain_graph=True, allow_unused=True)
+        bf16 = self.store_dtype == torch.bfloat16
         if neigh:
             grads = torch.autograd.grad(loss + self.store_loss, [r for _, _, r, _, _ in neigh], retain_graph=True, allow_unused=True)
             for (l, neighbor, _, count, pool), g in zip(neigh, grads):
                 if g is None:
                     continue
                 if self.fused:
-                    ops.store_accumulate(self.gradient_stores[l], neighbor, g, count, pool or 'sum')
+                    sr = dict(seed=self.store_seed, step=self.store_sr_step, tensor=l) if bf16 else {}
+                    ops.store_accumulate(self.gradient_stores[l], neighbor, g, count, pool or 'sum', **sr)
                 else:
                     self.gradient_stores[l].index_add_(0, neighbor, g)
+        if bf16:
+            self.store_sr_step.add_(1)
         optimizer.zero_grad()
         loss.backward()
         optimizer.step()
@@ -735,6 +762,7 @@ class ScalableSageEncoder(SageEncoder, _ScalableStores):
     aggregates the hop's node-encoder rows, layer l >= 1 the neighbours' rows of stores[l - 1] (f32[max_id + 2, dims[l]],
     initialised uniform(0, store_init_maxval) from `generator`; gradient_stores alike, zeros).  The step's order and
     train_step are _ScalableStores'; store_optimizer is torch.optim.Adam(self.parameters(), store_learning_rate).
+    store_dtype=torch.bfloat16 (with store_seed) keeps the stores in bfloat16, by _ScalableStores' rules.
 
     fused=True (the default): layer 0 pools the hop through ShallowEncoder.pooled by SageEncoder's rule; layers >= 1 read
     the stores through ops.shallow_encode_pool(neighbor, fanout, id_table=store) when the aggregator has forward_pooled
@@ -753,15 +781,17 @@ class ScalableSageEncoder(SageEncoder, _ScalableStores):
                  feature_idx=-1, feature_dim=0, max_id=-1, use_feature=True, use_id=False, sparse_feature_idx=-1,
                  sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False, shared_node_encoder=None,
                  use_residual=False, store_learning_rate=0.001, store_init_maxval=0.05, fused=True, sparse_grad=False,
-                 device=None, generator=None, table_dtype=torch.float32):
+                 device=None, generator=None, table_dtype=torch.float32, store_dtype=torch.float32, store_seed=0):
         _scalable_f32(table_dtype)
+        _scalable_store_args(store_dtype, store_seed, fused)
         super().__init__([edge_type] * num_layers, [fanout] * num_layers, dim, aggregator, concat, shared_aggregators,
                          feature_idx, feature_dim, max_id, use_feature, use_id, sparse_feature_idx, sparse_feature_max_id,
                          embedding_dim, use_hash_embedding, use_residual=use_residual,
                          shared_node_encoder=shared_node_encoder, fused=fused, sparse_grad=sparse_grad, device=device)
         self.edge_type = edge_type
         self.fanout = fanout
-        self._init_stores(self.dims[1:-1], max_id, store_learning_rate, store_init_maxval, generator, device)
+        self._init_stores(self.dims[1:-1], max_id, store_learning_rate, store_init_maxval, generator, device, store_dtype,
+                          store_seed)
 
     def _pools_store(self, aggregator):
         return self.fused and hasattr(aggregator, 'forward_pooled') and 1 <= self.fanout <= _lib.SHALLOW_POOL_MAX_COUNT
@@ -797,7 +827,8 @@ class ScalableGCNEncoder(GCNEncoder, _ScalableStores):
     `generator`; gradient_stores alike, zeros), each layer's output plus its input under use_residual.  The step's order and
     train_step are _ScalableStores'.  fused=True reads the stores through ops.shallow_encode and updates them through
     ops.store_exchange / ops.store_accumulate, the aggregators taking their own fused paths; fused=False is the literal
-    composition (store[ids], index_put_ keep-last, index_add_).
+    composition (store[ids], index_put_ keep-last, index_add_).  store_dtype=torch.bfloat16 (with store_seed) keeps the
+    stores in bfloat16, by _ScalableStores' rules.
 
     Differences from upstream:
       - an aggregator whose output is stored must be dim wide, the stores' width; 'attention' with dim % head_num != 0 is
@@ -808,8 +839,10 @@ class ScalableGCNEncoder(GCNEncoder, _ScalableStores):
     def __init__(self, edge_type, num_layers, dim, aggregator='mean', feature_idx=-1, feature_dim=0, max_id=-1, use_id=False,
                  sparse_feature_idx=-1, sparse_feature_max_id=-1, embedding_dim=16, use_hash_embedding=False,
                  use_residual=False, store_learning_rate=0.001, store_init_maxval=0.05, head_num=4, fused=True,
-                 sparse_grad=False, device=None, generator=None, table_dtype=torch.float32):
+                 sparse_grad=False, device=None, generator=None, table_dtype=torch.float32, store_dtype=torch.float32,
+                 store_seed=0):
         _scalable_f32(table_dtype)
+        _scalable_store_args(store_dtype, store_seed, fused)
         super().__init__([edge_type] * num_layers, dim, aggregator, feature_idx, feature_dim, max_id, use_id,
                          sparse_feature_idx, sparse_feature_max_id, embedding_dim, use_hash_embedding, use_residual,
                          head_num, fused=fused, sparse_grad=sparse_grad, device=device)
@@ -818,7 +851,8 @@ class ScalableGCNEncoder(GCNEncoder, _ScalableStores):
         self.dim = dim
         self.edge_type = edge_type
         self.fused = fused
-        self._init_stores([dim] * (num_layers - 1), max_id, store_learning_rate, store_init_maxval, generator, device)
+        self._init_stores([dim] * (num_layers - 1), max_id, store_learning_rate, store_init_maxval, generator, device,
+                          store_dtype, store_seed)
 
     def forward(self, inputs, training=False):
         if not training:

@@ -1488,11 +1488,16 @@ def shallow_encode_pool(nodes, count, id_table=None, dense=(), sparse=(), pool='
 
 # ------------------------------------------------------------------------------------ embedding stores
 def _store_table(op, named):
-    """the tables a store op updates in place: float32 2-D, contiguous, on the graph's device"""
-    _check_f32(op, named, 2)
+    """the tables a store op updates in place: 2-D, contiguous, on the graph's device, all float32 or all bfloat16; returns
+    that dtype"""
+    dt = named[0][1].dtype if torch.is_tensor(named[0][1]) else None
     for nm, t in named:
+        if not torch.is_tensor(t) or t.dtype not in (torch.float32, torch.bfloat16) or t.dtype != dt or t.dim() != 2:
+            raise EulerError("%s: %s must be 2-D float32 or bfloat16 tensors of one dtype"
+                             % (op, " and ".join(nm for nm, _ in named)))
         if not t.is_contiguous() or t.device != _dev():
             raise EulerError("%s: %s must be contiguous on %s" % (op, nm, _dev()))
+    return dt
 
 
 def store_exchange(store, grad_store, ids, rows):
@@ -1500,9 +1505,11 @@ def store_exchange(store, grad_store, ids, rows):
     and in one device op, for ids i64[M] (any shape) in [0, n_rows) and rows f32[M, dim]:
         store[ids[i]] = rows[i]   the LAST occurrence of a repeated id wins
         taken[i] = grad_store[ids[i]] as it was before the call, for every i; then grad_store[ids[i]] = 0
-    store and grad_store are f32[n_rows, dim].  Returns taken f32[M, dim].  No autograd: rows is read detached.  An id
-    outside the tables raises before either is written (one host synchronisation; none under CUDA-graph capture)."""
-    _store_table("store_exchange", (("store", store), ("grad_store", grad_store)))
+    store and grad_store are f32[n_rows, dim], or both bfloat16: the store row is then rounded to nearest even and taken is
+    the gradient row widened exactly (include/euler_b200.h, eu_store_exchange_dtype).  Returns taken f32[M, dim].  No
+    autograd: rows is read detached.  An id outside the tables raises before either is written (one host synchronisation;
+    none under CUDA-graph capture)."""
+    dt = _store_table("store_exchange", (("store", store), ("grad_store", grad_store)))
     _check_f32("store_exchange", (("rows", rows),), 2)
     ids = _t(ids, torch.int64).reshape(-1)
     n_rows, dim = store.shape
@@ -1511,21 +1518,28 @@ def store_exchange(store, grad_store, ids, rows):
                          % (tuple(store.shape), tuple(grad_store.shape), tuple(rows.shape), ids.numel()))
     rows = _t(rows.detach(), torch.float32)
     taken = torch.empty((ids.numel(), dim), dtype=torch.float32, device=store.device)
-    _call("eu_store_exchange", store, grad_store, n_rows, dim, ids, ids.numel(), rows, taken)
+    if dt == torch.bfloat16:
+        _call("eu_store_exchange_dtype", store, grad_store, n_rows, dim, ids, ids.numel(), rows, taken, 1)
+    else:
+        _call("eu_store_exchange", store, grad_store, n_rows, dim, ids, ids.numel(), rows, taken)
     return taken
 
 
-def store_accumulate(grad_store, ids, grad, count=1, pool='mean'):
+def store_accumulate(grad_store, ids, grad, count=1, pool='mean', seed=0, step=None, tensor=0):
     """The gradient-store update of ScalableSageEncoder / ScalableGCNEncoder (tf.scatter_add, encoders.py:382-389), in place
     and in one device op: grad_store[ids[e]] += grad[e // count] (divided by count under pool='mean'), for ids i64[M] (any
     shape) in [0, n_rows), grad f32[M / count, dim] and grad_store f32[n_rows, dim].  That is the gradient of
     shallow_encode_pool(ids, count, id_table=store, pool=pool) (count = 1: of shallow_encode(ids, id_table=store)), summed per
     distinct id in that op's fixed order and added to the stored row with one rounding: deterministic, no atomics.  No
-    autograd.  An id outside the table raises before it is written (one host synchronisation; none under capture)."""
+    autograd.  An id outside the table raises before it is written (one host synchronisation; none under capture).
+    grad_store may be bfloat16 (grad stays float32): the same sum is added to the widened row in f32 and written back by
+    stochastic rounding keyed by (seed, step, tensor, element), step an int64 device scalar the caller advances once per
+    step, as optim_momentum_'s (include/euler_b200.h, eu_store_accumulate_dtype)."""
+    op = "store_accumulate"
     if pool not in POOLS:
         raise EulerError("store_accumulate: pool must be one of %s, got %r" % (sorted(POOLS), pool))
-    _store_table("store_accumulate", (("grad_store", grad_store),))
-    _check_f32("store_accumulate", (("grad", grad),), 2)
+    dt = _store_table(op, (("grad_store", grad_store),))
+    _check_f32(op, (("grad", grad),), 2)
     ids = _t(ids, torch.int64).reshape(-1)
     n_rows, dim = grad_store.shape
     count = int(count)
@@ -1533,7 +1547,11 @@ def store_accumulate(grad_store, ids, grad, count=1, pool='mean'):
         raise EulerError("store_accumulate: need count >= 1 dividing M = %d and grad [M / count, %d]; got count %d, grad %s"
                          % (ids.numel(), dim, count, tuple(grad.shape)))
     grad = _t(grad.detach(), torch.float32)
-    _call("eu_store_accumulate", grad_store, n_rows, dim, ids, ids.numel(), count, POOLS[pool], grad)
+    if dt == torch.bfloat16:
+        _call("eu_store_accumulate_dtype", grad_store, n_rows, dim, ids, ids.numel(), count, POOLS[pool], grad,
+              *_sr_args(op, grad_store, seed, step, tensor))
+    else:
+        _call("eu_store_accumulate", grad_store, n_rows, dim, ids, ids.numel(), count, POOLS[pool], grad)
 
 
 # ------------------------------------------------------------------------------------ graph-level minibatches

@@ -1137,6 +1137,24 @@ int eu_store_exchange(eu_ctx* c, float* store, float* grad_store, int64_t n_rows
                       const float* rows, float* taken);
 int eu_store_accumulate(eu_ctx* c, float* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M, int32_t count,
                         int32_t pool, const float* grad);
+/* The same two over a store pair of storage type dtype (eu_feat_dtype; store and grad_store both have it; rows, taken and
+ * grad stay f32).  EU_FEAT_F32 is the call above (seed, step and tensor unused).  With EU_FEAT_BF16 every read widens a
+ * stored element exactly to f32 and only the writes round:
+ *   exchange:    store[v] = the round to nearest even of rows[the last i with that id] (an overwrite: no seed); taken[i] =
+ *                the pre-clear gradient row widened, f32; the cleared rows are exact zeros.
+ *   accumulate:  grad_store[v] = SR(__fadd_rn(widen(grad_store[v]), S_v)), S_v the f32 call's sum, SR the stochastic
+ *                rounding of eu_optim_*_dtype: the low 16 bits of word 0 of Philox4x32-10 with counter (element lo,
+ *                element hi, *step mod 2^32, tensor) and key seed, element = v * dim + f (64-bit), are added to the low half
+ *                of the f32 bits, which are then dropped.  step is a device int64 read on the device, so a captured graph
+ *                replays with the live counter.  Rows no id names keep their bits.
+ * The 4-wide path needs dim % 4 == 0, the bf16 tables 8-byte aligned and rows / taken 16-byte aligned; otherwise scalar
+ * accesses give the same bits.  An unknown dtype, or eu_store_accumulate_dtype with EU_FEAT_BF16 and no step:
+ * EU_ERR_INVALID before any device work; every other bound and status as above. */
+int eu_store_exchange_dtype(eu_ctx* c, void* store, void* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
+                            const float* rows, float* taken, int32_t dtype);
+int eu_store_accumulate_dtype(eu_ctx* c, void* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
+                              int32_t count, int32_t pool, const float* grad, int32_t dtype, uint64_t seed, const int64_t* step,
+                              int32_t tensor);
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx,
                    int64_t E, float* out);
 int eu_scatter_add_host(eu_ctx* c, const float* updates, int64_t D, const int32_t* idx, int64_t E,
