@@ -6,14 +6,17 @@ is no Python/CPU fallback: if the library is missing or no CUDA device is presen
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(_HERE, "lib", "libeuler_b200.so")
 
 EU_RNG_MINSTD = 0
 EU_RNG_PHILOX = 1
 
-# eu_feat_dtype: the storage type of a graph's dense node feature table, by name
+# eu_feat_dtype: the storage type of a graph's dense node feature table or of an embedding table, by name and by torch dtype
 FEAT_DTYPES = {"float32": 0, "bfloat16": 1}
+TORCH_DTYPES = {getattr(torch, name): code for name, code in FEAT_DTYPES.items()}
 # eu_feat_place: where that table lives, by name
 FEAT_PLACES = {"device": 0, "host": 1}
 

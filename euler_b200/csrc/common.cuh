@@ -9,6 +9,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #define EU_WARP 32
 #define EU_MAX_ETYPES 32
@@ -140,10 +141,8 @@ __host__ __device__ __forceinline__ void dense_slot(const DevGraph& g, int32_t f
 // ---------------------------------------------------------------------------------- dense feature storage
 // The one place that knows how a dense feature table is stored.  A kernel that reads rows is instantiated for its storage
 // type T (float or __nv_bfloat16), takes the table as feat_cols<T>(g) and loads columns with feat_ld (one) or feat_ld4 (four
-// consecutive, one 16-byte f32 / 8-byte bf16 load: the address must be aligned to four elements).  Both return f32;
-// widening bf16 is exact (its bits are the upper half of the f32's).  A bf16 table is written only through feat_st, the
-// device's round to nearest even: NaN becomes the canonical NaN, +-Inf stays, a finite value becomes +-Inf only where the
-// rounding says so, and subnormals round like any other value.
+// consecutive), which widen to f32 (f32 / bf16 elements, below).  A bf16 table is written only through feat_st, the device's
+// round to nearest even.
 template <typename T>
 __host__ __device__ __forceinline__ const T* feat_cols(const DevGraph& g) { return static_cast<const T*>(g.feat); }
 
@@ -177,36 +176,6 @@ template <typename T, int P>
 __device__ __forceinline__ const T* feat_row_if(const DevGraph& g, bool ok, int64_t row, int32_t col) {
   if (P == kFeatHost) return ok ? feat_row<T, P>(g, row) + col : feat_cols<T>(g);
   return feat_cols<T>(g) + (ok ? row * (int64_t)g.feat_dim + col : 0);
-}
-
-template <typename T> __device__ __forceinline__ float feat_ld(const T* p);
-template <> __device__ __forceinline__ float feat_ld<float>(const float* p) { return __ldg(p); }
-template <> __device__ __forceinline__ float feat_ld<__nv_bfloat16>(const __nv_bfloat16* p) {
-  return __uint_as_float((uint32_t)__ldg(reinterpret_cast<const unsigned short*>(p)) << 16);
-}
-
-template <typename T> __device__ __forceinline__ float4 feat_ld4(const T* p);
-template <> __device__ __forceinline__ float4 feat_ld4<float>(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-template <> __device__ __forceinline__ float4 feat_ld4<__nv_bfloat16>(const __nv_bfloat16* p) {
-  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));   // columns 0..3: the low and high halves of x, then of y
-  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
-                     __uint_as_float(u.y & 0xFFFF0000u));
-}
-
-template <typename T> __device__ __forceinline__ T feat_st(float v);
-template <> __device__ __forceinline__ float feat_st<float>(float v) { return v; }
-template <> __device__ __forceinline__ __nv_bfloat16 feat_st<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-
-// A trained bf16 table (optim.cu) is written through sr_st instead: stochastic rounding with a 16-bit random integer r, added
-// to the low half of the f32 bits before they are truncated, so v rounds up with probability (its distance from the value
-// below) / ulp and the rounding is unbiased.  r = 0 truncates toward zero; r = 0x8000 rounds to nearest with ties away from
-// zero.  +-Inf stays; a NaN keeps its sign and upper payload and is made quiet; a finite value can carry into +-Inf only
-// from above the largest finite bf16.  Round to nearest would lose every update smaller than half an ulp.
-__device__ __forceinline__ __nv_bfloat16 sr_st(float v, uint32_t r) {
-  const uint32_t u = __float_as_uint(v);
-  const uint32_t h = (u & 0x7F800000u) == 0x7F800000u ? (u >> 16) | ((u & 0x007FFFFFu) ? 0x0040u : 0u)
-                                                      : (u + (r & 0xFFFFu)) >> 16;
-  return __ushort_as_bfloat16((unsigned short)h);
 }
 
 // Row `row`'s slice of ragged slot `fid` (ptr of S slots per row): [b, e) in the value array, b == e when the node / slot does
@@ -335,6 +304,102 @@ __device__ __forceinline__ uint4 philox_bits(unsigned long long seed, uint32_t s
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
   return make_uint4(c[0], c[1], c[2], c[3]);
+}
+
+// ---------------------------------------------------------------------------------- f32 / bf16 elements
+// The one place that knows how an element of an f32 or bf16 table (T = float or __nv_bfloat16) is read and written.  Reads
+// return f32: widening bf16 is exact (its bits are the upper half of the f32's).  The 4-wide forms move four consecutive
+// elements as one 16-byte f32 / 8-byte bf16 access, so the address must be aligned to four elements.  An f32 value is stored
+// as it is; a bf16 one is rounded.
+//   feat_ld, feat_ld4   loads through the read-only data cache (__ldg), for tables the kernel does not write
+//   rw_ld, rw_ld4       plain loads, for kernels that write the table they read (the stores, the optimizers)
+//   feat_st, rn_st4     round to nearest even: NaN becomes the canonical NaN, +-Inf stays, a finite value becomes +-Inf only
+//                       where the rounding says so, and subnormals round like any other value
+//   sr_st, sr_st4       stochastic rounding from given random words (SrKey), for trained tables
+__device__ __forceinline__ float bf16_bits_f32(uint32_t h) { return __uint_as_float(h << 16); }
+// four bf16 elements as the two words of one 8-byte access: columns 0..3 are the low and high halves of x, then of y
+__device__ __forceinline__ float4 bf16x4_f32(uint2 u) {
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xFFFF0000u));
+}
+__device__ __forceinline__ uint2 bf16x4_bits(__nv_bfloat16 a, __nv_bfloat16 b, __nv_bfloat16 c, __nv_bfloat16 d) {
+  return make_uint2(__bfloat16_as_ushort(a) | (uint32_t)__bfloat16_as_ushort(b) << 16,
+                    __bfloat16_as_ushort(c) | (uint32_t)__bfloat16_as_ushort(d) << 16);
+}
+
+template <typename T> __device__ __forceinline__ float feat_ld(const T* p);
+template <> __device__ __forceinline__ float feat_ld<float>(const float* p) { return __ldg(p); }
+template <> __device__ __forceinline__ float feat_ld<__nv_bfloat16>(const __nv_bfloat16* p) {
+  return bf16_bits_f32(__ldg(reinterpret_cast<const unsigned short*>(p)));
+}
+template <typename T> __device__ __forceinline__ float4 feat_ld4(const T* p);
+template <> __device__ __forceinline__ float4 feat_ld4<float>(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+template <> __device__ __forceinline__ float4 feat_ld4<__nv_bfloat16>(const __nv_bfloat16* p) {
+  return bf16x4_f32(__ldg(reinterpret_cast<const uint2*>(p)));
+}
+
+__device__ __forceinline__ float rw_ld(const float* p) { return *p; }
+__device__ __forceinline__ float rw_ld(const __nv_bfloat16* p) { return bf16_bits_f32(*reinterpret_cast<const unsigned short*>(p)); }
+__device__ __forceinline__ float4 rw_ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ float4 rw_ld4(const __nv_bfloat16* p) { return bf16x4_f32(*reinterpret_cast<const uint2*>(p)); }
+
+template <typename T> __device__ __forceinline__ T feat_st(float v);
+template <> __device__ __forceinline__ float feat_st<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 feat_st<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+__device__ __forceinline__ void rn_st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void rn_st4(__nv_bfloat16* p, float4 v) {
+  *reinterpret_cast<uint2*>(p) = bf16x4_bits(feat_st<__nv_bfloat16>(v.x), feat_st<__nv_bfloat16>(v.y), feat_st<__nv_bfloat16>(v.z),
+                                             feat_st<__nv_bfloat16>(v.w));
+}
+
+// Stochastic rounding with a 16-bit random integer r (the low half of a random word), added to the low half of the f32 bits
+// before they are truncated, so v rounds up with probability (its distance from the value below) / ulp and the rounding is
+// unbiased.  r = 0 truncates toward zero; r = 0x8000 rounds to nearest with ties away from zero.  +-Inf stays; a NaN keeps
+// its sign and upper payload and is made quiet; a finite value can carry into +-Inf only from above the largest finite bf16.
+// Round to nearest would lose every update smaller than half an ulp.
+__device__ __forceinline__ __nv_bfloat16 sr_st(float v, uint32_t r) {
+  const uint32_t u = __float_as_uint(v);
+  const uint32_t h = (u & 0x7F800000u) == 0x7F800000u ? (u >> 16) | ((u & 0x007FFFFFu) ? 0x0040u : 0u)
+                                                      : (u + (r & 0xFFFFu)) >> 16;
+  return __ushort_as_bfloat16((unsigned short)h);
+}
+__device__ __forceinline__ void sr_st(float* p, float v, uint32_t) { *p = v; }
+__device__ __forceinline__ void sr_st(__nv_bfloat16* p, float v, uint32_t r) {
+  *reinterpret_cast<unsigned short*>(p) = __bfloat16_as_ushort(sr_st(v, r));
+}
+__device__ __forceinline__ void sr_st4(float* p, float4 v, const uint32_t (&)[4]) { rn_st4(p, v); }
+__device__ __forceinline__ void sr_st4(__nv_bfloat16* p, float4 v, const uint32_t (&r)[4]) {
+  *reinterpret_cast<uint2*>(p) = bf16x4_bits(sr_st(v.x, r[0]), sr_st(v.y, r[1]), sr_st(v.z, r[2]), sr_st(v.w, r[3]));
+}
+
+// The key of the random words that round a trained bf16 table: element e's words at a step are the four of philox_bits(seed,
+// step, tensor, e), with step the low 32 bits of the device counter *step, read on the device (a captured CUDA graph replays
+// with the live count) and once per thread.  An f32 table never reads it.
+struct SrKey {
+  unsigned long long seed;
+  const int64_t* step;   // device step counter
+  uint32_t tensor;
+};
+__device__ __forceinline__ uint4 sr_bits(const SrKey& k, uint32_t step, unsigned long long e) {
+  return philox_bits(k.seed, step, k.tensor, e);
+}
+// the words of the elements [e, e + VW) of a table updated with up to three tensors: r[w][i] rounds tensor w of element e + i
+template <int VW>
+__device__ __forceinline__ void sr_words(const SrKey& k, int64_t e, uint32_t (&r)[3][VW]) {
+  const uint32_t step = (uint32_t)__ldg(k.step);
+#pragma unroll
+  for (int i = 0; i < VW; ++i) {
+    const uint4 q = sr_bits(k, step, (unsigned long long)(e + i));
+    r[0][i] = q.x; r[1][i] = q.y; r[2][i] = q.z;
+  }
+}
+
+// the host's widening of n bf16 bit patterns h to f32
+inline void bf16_bits_f32_host(const uint16_t* h, int64_t n, float* out) {
+  for (int64_t i = 0; i < n; ++i) {
+    const uint32_t u = (uint32_t)h[i] << 16;
+    memcpy(out + i, &u, sizeof(u));
+  }
 }
 
 // ---------------------------------------------------------------------------------- TMA bulk copy (sm_90+)

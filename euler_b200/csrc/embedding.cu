@@ -722,19 +722,10 @@ static int shallow_backward_sparse(eu_ctx* c, const eu_shallow_problem* p, const
   return EU_OK;
 }
 
-// EU_ERR_INVALID unless table_dtype is an eu_feat_dtype
-static int table_dtype_check(int32_t table_dtype, const char* who) {
-  if (table_dtype != EU_FEAT_F32 && table_dtype != EU_FEAT_BF16) {
-    set_error("%s: unknown table dtype %d (EU_FEAT_F32 or EU_FEAT_BF16)", who, (int)table_dtype);
-    return EU_ERR_INVALID;
-  }
-  return EU_OK;
-}
-
 // eu_sparse_embedding_lookup(_dtype)
 static int emb_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int64_t default_value, const void* table, int64_t n_rows,
                       int32_t dim, int32_t combiner, int32_t table_dtype, float* out, const char* who) {
-  int rc = table_dtype_check(table_dtype, who);
+  int rc = dtype_check(table_dtype, who, "table");
   if (rc || (rc = emb_check(c, nodes, M, fid, default_value, table != nullptr, n_rows, dim, combiner, out, who))) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   if (M == 0) return EU_OK;
@@ -744,44 +735,11 @@ static int emb_lookup(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, i
   const auto* nd = (const unsigned long long*)nodes;
   const auto dflt = (unsigned long long)default_value;
   EuProfScope ps(c, "emb_fwd", M);
-  if (table_dtype == EU_FEAT_BF16) {
-    const auto* t = static_cast<const __nv_bfloat16*>(table);
-    if (vec) k_emb_fwd<true><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
-    else k_emb_fwd<false><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
-  } else {
-    const auto* t = static_cast<const float*>(table);
-    if (vec) k_emb_fwd<true><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
-    else k_emb_fwd<false><<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, t, dim, G, combiner, out);
-  }
-  EU_LAUNCHED();
-  return EU_OK;
-}
-
-// k_shallow_fwd / k_shallow_pool for the dense table at P, of bf16_feat's type, and tables of table_dtype
-template <int P>
-static int launch_shallow_fwd(eu_ctx* c, const ShallowDev& d, int G, unsigned blocks, int32_t table_dtype, bool bf16_feat) {
-  if (table_dtype == EU_FEAT_BF16) {
-    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, __nv_bfloat16, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-    else k_shallow_fwd<float, __nv_bfloat16, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-  } else {
-    if (bf16_feat) k_shallow_fwd<__nv_bfloat16, float, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-    else k_shallow_fwd<float, float, P><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
-  }
-  EU_LAUNCHED();
-  return EU_OK;
-}
-
-template <int P>
-static int launch_shallow_pool(eu_ctx* c, const ShallowDev& d, int count, float pool_den, int G, unsigned blocks, size_t smem,
-                               int32_t table_dtype, bool bf16_feat) {
-  cudaStream_t s = c->stream;
-  if (table_dtype == EU_FEAT_BF16) {
-    if (bf16_feat) k_shallow_pool<__nv_bfloat16, __nv_bfloat16, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
-    else k_shallow_pool<float, __nv_bfloat16, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
-  } else {
-    if (bf16_feat) k_shallow_pool<__nv_bfloat16, float, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
-    else k_shallow_pool<float, float, P><<<blocks, 256, smem, s>>>(c->g->d, d, count, pool_den, G);
-  }
+  with_dtype(table_dtype, [&](auto e) {
+    using E = typename decltype(e)::type;
+    auto k = vec ? k_emb_fwd<true, E> : k_emb_fwd<false, E>;
+    k<<<blocks, 256, 0, c->stream>>>(c->g->d, nd, M, fid, dflt, static_cast<const E*>(table), dim, G, combiner, out);
+  });
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -790,7 +748,7 @@ static int launch_shallow_pool(eu_ctx* c, const ShallowDev& d, int count, float 
 static int shallow_encode(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dtype, float* out, float* dense_out, const char* who) {
   ShallowDev d;
   EmbTables T;
-  int rc = table_dtype_check(table_dtype, who);
+  int rc = dtype_check(table_dtype, who, "table");
   if (rc || (rc = shallow_resolve(c, p, &d, &T, who))) return rc;
   if (p->M > 0 && ((d.W > 0 && !out) || (d.add && d.dense_w > 0 && !dense_out))) {
     set_error("%s: bad argument (out%s is required)", who, d.add ? " and dense_out" : "");
@@ -804,9 +762,13 @@ static int shallow_encode(eu_ctx* c, const eu_shallow_problem* p, int32_t table_
   const int G = shallow_lanes(&d, out, table_dtype);
   EuProfScope ps(c, "shallow_fwd", p->M);
   const unsigned blocks = (unsigned)ceil_div(p->M * G, 256);
-  const bool bf16_feat = c->g->d.feat_dtype == EU_FEAT_BF16;
-  if (c->g->d.feat_place == EU_FEAT_HOST) return launch_shallow_fwd<kFeatHost>(c, d, G, blocks, table_dtype, bf16_feat);
-  return launch_shallow_fwd<kFeatDevice>(c, d, G, blocks, table_dtype, bf16_feat);
+  with_feat(c->g->d, [&](auto t, auto p) {
+    with_dtype(table_dtype, [&](auto e) {
+      k_shallow_fwd<typename decltype(t)::type, typename decltype(e)::type, decltype(p)::value><<<blocks, 256, 0, c->stream>>>(c->g->d, d, G);
+    });
+  });
+  EU_LAUNCHED();
+  return EU_OK;
 }
 
 // eu_shallow_encode_pool(_dtype)
@@ -815,7 +777,7 @@ static int shallow_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dt
   ShallowDev d;
   EmbTables T;
   GradRows gr;
-  int rc = table_dtype_check(table_dtype, who);
+  int rc = dtype_check(table_dtype, who, "table");
   if (rc || (rc = shallow_resolve(c, p, &d, &T, who)) || (rc = pool_check(p, count, pool, &gr, who))) return rc;
   if (p->M > 0 && d.W > 0 && !out) {
     set_error("%s: bad argument (out is required)", who);
@@ -832,10 +794,14 @@ static int shallow_pool(eu_ctx* c, const eu_shallow_problem* p, int32_t table_dt
   EuProfScope ps(c, "shallow_pool", p->M);
   const unsigned blocks = (unsigned)ceil_div(R * G, 256);
   const size_t smem = (256 / G) * (size_t)count * sizeof(int64_t);
-  const bool bf16_feat = c->g->d.feat_dtype == EU_FEAT_BF16;
-  if (c->g->d.feat_place == EU_FEAT_HOST)
-    return launch_shallow_pool<kFeatHost>(c, d, count, gr.pool_den, G, blocks, smem, table_dtype, bf16_feat);
-  return launch_shallow_pool<kFeatDevice>(c, d, count, gr.pool_den, G, blocks, smem, table_dtype, bf16_feat);
+  with_feat(c->g->d, [&](auto t, auto p) {
+    with_dtype(table_dtype, [&](auto e) {
+      k_shallow_pool<typename decltype(t)::type, typename decltype(e)::type, decltype(p)::value><<<blocks, 256, smem, c->stream>>>(
+          c->g->d, d, count, gr.pool_den, G);
+    });
+  });
+  EU_LAUNCHED();
+  return EU_OK;
 }
 
 }  // namespace eu

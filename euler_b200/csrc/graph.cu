@@ -256,11 +256,9 @@ static int upload(eu_graph* g, const T** dst, const T* src, int64_t count) {
   return EU_OK;
 }
 
-static bool feat_dtype_ok(int32_t dtype) { return dtype == EU_FEAT_F32 || dtype == EU_FEAT_BF16; }
-
 int feat_storage_check(const eu_feat_storage* in, int64_t n, const char* who, eu_feat_storage* st) {
   *st = in ? *in : eu_feat_storage{EU_FEAT_F32, EU_FEAT_DEVICE, 0};
-  if (!feat_dtype_ok(st->dtype)) { set_error("%s: unknown feature dtype %d", who, st->dtype); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(st->dtype, who, "feature")) return rc;
   if (st->place != EU_FEAT_DEVICE && st->place != EU_FEAT_HOST) {
     set_error("%s: unknown feature place %d (EU_FEAT_DEVICE or EU_FEAT_HOST)", who, st->place);
     return EU_ERR_INVALID;
@@ -310,9 +308,8 @@ static int build_feat_cache(eu_graph* g, int64_t C) {
   d.feat_slot = slot;
   d.feat_cache_rows = C;
   if (C == 0) return EU_OK;
-  const size_t es = d.feat_dtype == EU_FEAT_BF16 ? 2 : 4;
   void* cache = nullptr;
-  rc = es == 2 ? g->alloc((__nv_bfloat16**)&cache, C * (int64_t)d.feat_dim) : g->alloc((float**)&cache, C * (int64_t)d.feat_dim);
+  rc = with_dtype(d.feat_dtype, [&](auto t) { return g->alloc((typename decltype(t)::type**)&cache, C * (int64_t)d.feat_dim); });
   if (rc) return rc;
   d.feat_cache = cache;
   unsigned long long *deg = nullptr, *deg_sorted = nullptr;
@@ -332,8 +329,10 @@ static int build_feat_cache(eu_graph* g, int64_t C) {
   if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, deg, deg_sorted, rows, order, n);
   if (e == cudaSuccess) { k_cache_slots<<<grid, 256>>>(order, C, slot); g_launches++; e = cudaGetLastError(); }
   if (e == cudaSuccess) {
-    if (es == 2) k_cache_fill<<<grid, 256>>>(feat_cols<__nv_bfloat16>(d), order, C, d.feat_dim, (__nv_bfloat16*)cache);
-    else k_cache_fill<<<grid, 256>>>(feat_cols<float>(d), order, C, d.feat_dim, (float*)cache);
+    with_dtype(d.feat_dtype, [&](auto t) {
+      using T = typename decltype(t)::type;
+      k_cache_fill<<<grid, 256>>>(feat_cols<T>(d), order, C, d.feat_dim, (T*)cache);
+    });
     g_launches++;
     e = cudaGetLastError();
   }
@@ -524,7 +523,7 @@ int eu_graph_create(const eu_graph_desc* desc, int device, eu_graph** out) {
 
 int eu_graph_create_dtype(const eu_graph_desc* desc, int device, int32_t feat_dtype, eu_graph** out) {
   if (!desc || !out) { set_error("null argument"); return EU_ERR_INVALID; }
-  if (!feat_dtype_ok(feat_dtype)) { set_error("eu_graph_create: unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(feat_dtype, "eu_graph_create", "feature")) return rc;
   const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0};
   return eu_graph_create_storage(desc, device, &st, out);
 }
@@ -737,15 +736,14 @@ static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, dou
   d.feat_dtype = st.dtype;
   d.feat_place = st.place;
   if (feat_dim > 0) {   // a host-placed table is filled through its mapped pointer
-    if (st.dtype == EU_FEAT_BF16) {
-      __nv_bfloat16* feat = nullptr;
-      TRY(alloc_feat(g, n_local * (int64_t)feat_dim, &feat));
-      k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
-    } else {
-      float* feat = nullptr;
-      TRY(alloc_feat(g, n_local * (int64_t)feat_dim, &feat));
-      k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
-    }
+    rc = with_dtype(st.dtype, [&](auto t) {
+      typename decltype(t)::type* feat = nullptr;
+      const int arc = alloc_feat(g, n_local * (int64_t)feat_dim, &feat);
+      if (arc == EU_OK)
+        k_fill_feat<<<kSMs * 8, 256>>>(feat, n_local, feat_dim, feat_seed, (unsigned long long)base_id, (unsigned long long)N);
+      return arc;
+    });
+    TRY(rc);
     g_launches++;
     d.n_slots = 1; d.slot_off[0] = 0; d.slot_dim[0] = feat_dim;
     g->dense_feature_names.push_back("feat0");
@@ -759,11 +757,6 @@ static int rmat_create(int64_t n_nodes, int64_t n_edges, double a, double b, dou
   *out = g;
   return EU_OK;
 }
-
-// the storage descriptor of the *_dtype constructors (a table of that type in HBM), the dtype checked first
-#define EU_DTYPE_STORAGE(who)                                                                                           \
-  if (!feat_dtype_ok(feat_dtype)) { set_error(who ": unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; } \
-  const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0}
 
 int eu_graph_create_rmat(int64_t n_nodes, int64_t n_edges, double a, double b, double c,
                          uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
@@ -787,25 +780,27 @@ int eu_graph_create_rmat_shard(int64_t n_nodes, int64_t n_edges, double a, doubl
 
 int eu_graph_create_rmat_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed, int32_t feat_dim,
                                uint64_t feat_seed, int device, int32_t feat_dtype, eu_graph** out) {
-  EU_DTYPE_STORAGE("eu_graph_create_rmat");
+  if (int rc = dtype_check(feat_dtype, "eu_graph_create_rmat", "feature")) return rc;
+  const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0};
   return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, 0, 1, 1, 1, &st, out);
 }
 
 int eu_graph_create_rmat_shard_dtype(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
                                      int32_t feat_dim, uint64_t feat_seed, int device, int shard_index, int shard_number,
                                      int32_t feat_dtype, eu_graph** out) {
-  EU_DTYPE_STORAGE("eu_graph_create_rmat");
+  if (int rc = dtype_check(feat_dtype, "eu_graph_create_rmat", "feature")) return rc;
+  const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0};
   return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, 1, 1, &st, out);
 }
 
 int eu_graph_create_rmat_hetero_dtype(int64_t n_nodes, int64_t n_edges, int32_t n_edge_types, int32_t n_node_types, double a,
                                       double b, double c, uint64_t seed, int32_t feat_dim, uint64_t feat_seed, int device,
                                       int shard_index, int shard_number, int32_t feat_dtype, eu_graph** out) {
-  EU_DTYPE_STORAGE("eu_graph_create_rmat");
+  if (int rc = dtype_check(feat_dtype, "eu_graph_create_rmat", "feature")) return rc;
+  const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0};
   return rmat_create(n_nodes, n_edges, a, b, c, seed, feat_dim, feat_seed, device, shard_index, shard_number, n_edge_types,
                      n_node_types, &st, out);
 }
-#undef EU_DTYPE_STORAGE
 
 int eu_graph_create_rmat_storage(int64_t n_nodes, int64_t n_edges, double a, double b, double c, uint64_t seed,
                                  int32_t feat_dim, uint64_t feat_seed, int device, const eu_feat_storage* storage,
@@ -870,25 +865,15 @@ int eu_graph_export(const eu_graph* g, uint64_t* ids, int32_t* node_type, float*
   const int64_t nf = d.n * (int64_t)d.feat_dim;
   if (d.feat_place == EU_FEAT_HOST) {   // the pinned table holds every row (the cache only copies some): read it in place
     if (feat && nf > 0) {
-      if (d.feat_dtype == EU_FEAT_F32) {
-        memcpy(feat, g->feat_host, sizeof(float) * (size_t)nf);
-      } else {
-        const uint16_t* h = static_cast<const uint16_t*>(g->feat_host);
-        for (int64_t i = 0; i < nf; ++i) {
-          const uint32_t u = (uint32_t)h[i] << 16;
-          memcpy(feat + i, &u, sizeof(u));
-        }
-      }
+      if (d.feat_dtype == EU_FEAT_F32) memcpy(feat, g->feat_host, sizeof(float) * (size_t)nf);
+      else bf16_bits_f32_host(static_cast<const uint16_t*>(g->feat_host), nf, feat);
     }
   } else if (d.feat_dtype == EU_FEAT_F32) {
     DL(feat, feat_cols<float>(d), nf);
-  } else if (feat && d.feat && nf > 0) {   // widened on the host: the bf16 bits become the f32's upper half
+  } else if (feat && d.feat && nf > 0) {   // widened on the host
     std::vector<uint16_t> h((size_t)nf);
     EU_CUDA(cudaMemcpy(h.data(), d.feat, sizeof(uint16_t) * (size_t)nf, cudaMemcpyDeviceToHost));
-    for (int64_t i = 0; i < nf; ++i) {
-      const uint32_t u = (uint32_t)h[i] << 16;
-      memcpy(feat + i, &u, sizeof(u));
-    }
+    bf16_bits_f32_host(h.data(), nf, feat);
   }
 #undef DL
   return EU_OK;

@@ -3,8 +3,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string.h>
+
 #include <atomic>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/euler_b200.h"
@@ -39,6 +42,34 @@ static_assert((int)kFeatDevice == (int)EU_FEAT_DEVICE && (int)kFeatHost == (int)
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // a table of eu_feat_dtype dtype takes 4-wide loads (16 bytes of f32, 8 of bf16) where p is aligned to four of its elements
 inline bool aligned4_elems(const void* p, int dtype) { return ((uintptr_t)p & (dtype == EU_FEAT_BF16 ? 7 : 15)) == 0; }
+
+// ---- the storage type of a table or feature row (eu_feat_dtype)
+inline bool dtype_ok(int32_t dtype) { return dtype == EU_FEAT_F32 || dtype == EU_FEAT_BF16; }
+// EU_OK for an eu_feat_dtype code, else EU_ERR_INVALID with "<who>: unknown <noun> dtype <dtype>"; a table's or a store's
+// text also names the codes, a graph's feature text does not
+inline int dtype_check(int32_t dtype, const char* who, const char* noun) {
+  if (dtype_ok(dtype)) return EU_OK;
+  set_error("%s: unknown %s dtype %d%s", who, noun, (int)dtype, strcmp(noun, "feature") ? " (EU_FEAT_F32 or EU_FEAT_BF16)" : "");
+  return EU_ERR_INVALID;
+}
+
+template <typename T>
+struct TypeTag { using type = T; };
+// f(TypeTag<T>{}) with T the element type of a checked eu_feat_dtype code: float or __nv_bfloat16
+template <typename F>
+auto with_dtype(int32_t dtype, F&& f) {
+  if (dtype == EU_FEAT_BF16) return f(TypeTag<__nv_bfloat16>{});
+  return f(TypeTag<float>{});
+}
+// f(TypeTag<T>{}, std::integral_constant<int, P>{}) for the graph's dense feature table: T its element type, P its placement
+// (kFeatDevice or kFeatHost)
+template <typename F>
+auto with_feat(const DevGraph& g, F&& f) {
+  return with_dtype(g.feat_dtype, [&](auto t) {
+    if (g.feat_place == EU_FEAT_HOST) return f(t, std::integral_constant<int, kFeatHost>{});
+    return f(t, std::integral_constant<int, kFeatDevice>{});
+  });
+}
 
 struct ETList {           // an edge-type list passed by value to the full-neighbor kernels
   int32_t K;

@@ -656,10 +656,7 @@ static int kg_args(eu_ctx* c, const eu_kg_problem* p, int dtype, KgArgs* A, cons
     set_error("%s: bad argument", who);
     return EU_ERR_INVALID;
   }
-  if (dtype != EU_FEAT_F32 && dtype != EU_FEAT_BF16) {
-    set_error("%s: unknown table dtype %d (EU_FEAT_F32 or EU_FEAT_BF16)", who, dtype);
-    return EU_ERR_INVALID;
-  }
+  if (int rc = dtype_check(dtype, who, "table")) return rc;
   const int m = p->model;
   if (m < KG_TRANSE || m > KG_DISTMULT || p->corrupt < 1 || p->corrupt > 3 || p->B < 0 || p->K < 1 || p->ent_dim < 1 ||
       p->rel_dim < 1 || p->n_ent < 1 || p->n_rel < 1 || !p->table[0] || !p->table[1] || (p->B > 0 && (!p->src || !p->dst || !p->rel || !p->neg))) {
@@ -751,23 +748,20 @@ static int kg_launch_bwd(eu_ctx* c, const KgArgs& A, const KgBwd& W, int* bad) {
   return EU_OK;
 }
 
-template <int M, typename Tab>
-static int kg_dispatch_fwd(eu_ctx* c, const KgArgs& A, int dtype, float* scores, float* es, float* er, float* ed, int* bad) {
-  return kg_vec(M, A, dtype) ? kg_launch_fwd<M, true, Tab>(c, A, scores, es, er, ed, bad)
-                             : kg_launch_fwd<M, false, Tab>(c, A, scores, es, er, ed, bad);
-}
 template <int M>
 static int kg_dispatch_fwd(eu_ctx* c, const KgArgs& A, int dtype, float* scores, float* es, float* er, float* ed, int* bad) {
-  return dtype == EU_FEAT_BF16 ? kg_dispatch_fwd<M, __nv_bfloat16>(c, A, dtype, scores, es, er, ed, bad)
-                               : kg_dispatch_fwd<M, float>(c, A, dtype, scores, es, er, ed, bad);
-}
-template <int M, typename Tab>
-static int kg_dispatch_bwd(eu_ctx* c, const KgArgs& A, int dtype, const KgBwd& W, int* bad) {
-  return kg_vec(M, A, dtype) ? kg_launch_bwd<M, true, Tab>(c, A, W, bad) : kg_launch_bwd<M, false, Tab>(c, A, W, bad);
+  return with_dtype(dtype, [&](auto t) {
+    using Tab = typename decltype(t)::type;
+    return kg_vec(M, A, dtype) ? kg_launch_fwd<M, true, Tab>(c, A, scores, es, er, ed, bad)
+                               : kg_launch_fwd<M, false, Tab>(c, A, scores, es, er, ed, bad);
+  });
 }
 template <int M>
 static int kg_dispatch_bwd(eu_ctx* c, const KgArgs& A, int dtype, const KgBwd& W, int* bad) {
-  return dtype == EU_FEAT_BF16 ? kg_dispatch_bwd<M, __nv_bfloat16>(c, A, dtype, W, bad) : kg_dispatch_bwd<M, float>(c, A, dtype, W, bad);
+  return with_dtype(dtype, [&](auto t) {
+    using Tab = typename decltype(t)::type;
+    return kg_vec(M, A, dtype) ? kg_launch_bwd<M, true, Tab>(c, A, W, bad) : kg_launch_bwd<M, false, Tab>(c, A, W, bad);
+  });
 }
 
 // The backward pass both output forms share: out[t] is table t's dense gradient or COO values, rows[t] its COO rows

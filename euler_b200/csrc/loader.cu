@@ -484,7 +484,7 @@ extern "C" int eu_graph_load_ex(const char* data_path, int shard_index, int shar
 extern "C" int eu_graph_load_dtype(const char* data_path, int shard_index, int shard_number, int device, int load_edges,
                                    int32_t feat_dtype, eu_graph** out) {
   if (!out) { set_error("eu_graph_load: bad argument (null out)"); return EU_ERR_INVALID; }
-  if (feat_dtype != EU_FEAT_F32 && feat_dtype != EU_FEAT_BF16) { set_error("eu_graph_load: unknown feature dtype %d", feat_dtype); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(feat_dtype, "eu_graph_load", "feature")) return rc;
   const eu_feat_storage st{feat_dtype, EU_FEAT_DEVICE, 0};
   return load_impl(data_path, shard_index, shard_number, device, load_edges, &st, out, nullptr);
 }

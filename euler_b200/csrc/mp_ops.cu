@@ -408,15 +408,6 @@ static int scatter(eu_ctx* c, const float* upd, int64_t D, const int32_t* idx, i
   return EU_OK;
 }
 
-template <typename T, int P>
-static int launch_feature(eu_ctx* c, const DevGraph& d, const int64_t* nodes, int64_t M, int32_t dim, int G, bool vec, unsigned blocks,
-                          int32_t soff, int32_t sdim, float* out) {
-  if (vec) k_feature<T, true, P><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
-  else k_feature<T, false, P><<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
-  EU_LAUNCHED();
-  return EU_OK;
-}
-
 // the fused SAGE reduction over a table of T placed at P; v4: the float4 path's conditions hold (fanout_aggregate)
 template <typename T, int P>
 static int launch_sage_mean(eu_ctx* c, const DevGraph& d, const unsigned long long* ids, int64_t rows, const int32_t* reps,
@@ -450,12 +441,14 @@ int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid
   const int G = vec ? group_lanes(dim / 4) : (dim >= 32 ? 32 : 1);
   const unsigned blocks = capped_grid(ceil_div(M * G, 256), "EU_FEATURE_CTAS", 0);
   EuProfScope ps(c, "k_feature", M);
-  const bool host = d.feat_place == EU_FEAT_HOST;
-  if (d.feat_dtype == EU_FEAT_BF16)
-    return host ? launch_feature<__nv_bfloat16, kFeatHost>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out)
-                : launch_feature<__nv_bfloat16, kFeatDevice>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
-  return host ? launch_feature<float, kFeatHost>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out)
-              : launch_feature<float, kFeatDevice>(c, d, nodes, M, dim, G, vec, blocks, soff, sdim, out);
+  with_feat(d, [&](auto t, auto p) {
+    using T = typename decltype(t)::type;
+    constexpr int P = decltype(p)::value;
+    auto k = vec ? k_feature<T, true, P> : k_feature<T, false, P>;
+    k<<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
+  });
+  EU_LAUNCHED();
+  return EU_OK;
 }
 
 int eu_gather(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx, int64_t E, float* out) {
@@ -508,14 +501,11 @@ static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int
   { EuProfScope ps(c, mean ? "k_sage_mean" : "k_sage_add", rows);
     // float4 path: one slot of the full stored width, a multiple of 4 floats up to 1024 (D = 64 of configs[4], 128, 256, ...),
     // on a table aligned to four elements (16 bytes of f32, 8 of bf16)
-    const bool bf16 = d.feat_dtype == EU_FEAT_BF16;
     const bool v4 = d.n < ((int64_t)1 << 31) && d.n_slots == 1 && dim == d.feat_dim && (dim & 3) == 0 && dim <= 1024 && aligned16(out) &&
-                    (bf16 ? ((uintptr_t)d.feat & 7) == 0 : aligned16(d.feat));
-    const bool host = d.feat_place == EU_FEAT_HOST;
-    const int rc = bf16 ? (host ? launch_sage_mean<__nv_bfloat16, kFeatHost>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out)
-                                : launch_sage_mean<__nv_bfloat16, kFeatDevice>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out))
-                        : (host ? launch_sage_mean<float, kFeatHost>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out)
-                                : launch_sage_mean<float, kFeatDevice>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out));
+                    aligned4_elems(d.feat, d.feat_dtype);
+    const int rc = with_feat(d, [&](auto t, auto p) {
+      return launch_sage_mean<typename decltype(t)::type, decltype(p)::value>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out);
+    });
     if (rc) return rc; }
   if (!dedup) return EU_OK;
   { EuProfScope ps(c, "k_sage_broadcast", rows);

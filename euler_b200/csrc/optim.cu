@@ -30,10 +30,10 @@
 //
 // bf16 tables (T = __nv_bfloat16: var and every slot bf16, the gradient f32; the *_dtype entry points).  Each element is
 // widened exactly to f32, updated by the same upd / adam_decay in f32, and each value written (var and every slot) is rounded
-// to bf16 by sr_st (common.cuh), stochastic rounding.  Its 16 random bits are the low half of word w (0 var, 1 the first slot,
-// 2 the second) of philox_bits(seed, step, tensor, element): element is the flat index r D + col into var, step the low 32
-// bits of the device step counter (the caller advances it once per step, after every variable, as Adam's powers), tensor the
-// variable's index among the caller's.  A step is thus deterministic and can be captured in a CUDA graph.  The 4-wide form
+// to bf16 by sr_st (common.cuh), stochastic rounding.  Its random word is word w (0 var, 1 the first slot, 2 the second) of
+// SrKey{seed, step, tensor}'s for the element: element is the flat index r D + col into var, step the device step counter
+// (the caller advances it once per step, after every variable, as Adam's powers), tensor the variable's index among the
+// caller's.  A step is thus deterministic and can be captured in a CUDA graph.  The 4-wide form
 // needs var and the slots 8-byte aligned (one 8-byte load or store per tensor and element group of four).
 #include <type_traits>
 
@@ -83,61 +83,25 @@ __device__ __forceinline__ void adam_decay(const OptArgs& a, float alpha, float&
   w = __fsub_rn(w, __fdiv_rn(__fmul_rn(alpha, m), __fadd_rn(__fsqrt_rn(v), a.eps)));
 }
 
-// the stochastic-rounding key of a bf16 update (see the top of the file); unused by f32 tables
-struct SrKey {
-  unsigned long long seed;
-  const int64_t* step;   // device step counter
-  uint32_t tensor;
-};
-
 template <typename T>
 constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
 
-// the random words of the elements [e, e + VW) of var: r[w][i] rounds tensor w (0 var, 1 slot 1, 2 slot 2) of element e + i
-template <int VW>
-__device__ __forceinline__ void sr_words(const SrKey& k, int64_t e, uint32_t (&r)[3][VW]) {
-  const uint32_t step = (uint32_t)__ldg(k.step);
-#pragma unroll
-  for (int i = 0; i < VW; ++i) {
-    const uint4 q = philox_bits(k.seed, step, k.tensor, (unsigned long long)(e + i));
-    r[0][i] = q.x; r[1][i] = q.y; r[2][i] = q.z;
-  }
-}
-
-// VW consecutive elements of a table of T, as f32: one float4 / one 8-byte bf16 load, or one element
+// VW consecutive elements of a table of T, as f32: one float4 / one 8-byte bf16 access, or one element
 template <int VW, typename T = float>
 struct Vec {
   float x[VW];
   __device__ __forceinline__ void load(const T* p) {
-    if constexpr (kBf16<T>) {
-      if (VW == 4) {
-        const uint2 u = *reinterpret_cast<const uint2*>(p);
-        x[0] = __uint_as_float(u.x << 16); x[1] = __uint_as_float(u.x & 0xFFFF0000u);
-        x[VW > 2 ? 2 : 0] = __uint_as_float(u.y << 16); x[VW > 3 ? 3 : 0] = __uint_as_float(u.y & 0xFFFF0000u);
-      } else {
-        x[0] = __uint_as_float((uint32_t)*reinterpret_cast<const unsigned short*>(p) << 16);
-      }
-    } else if (VW == 4) {
-      const float4 t = *reinterpret_cast<const float4*>(p);
+    if constexpr (VW == 4) {
+      const float4 t = rw_ld4(p);
       x[0] = t.x; x[1] = t.y; x[2] = t.z; x[3] = t.w;
     } else {
-      x[0] = *p;
+      x[0] = rw_ld(p);
     }
   }
   // r: the elements' random words (bf16 only)
   __device__ __forceinline__ void store(T* p, const uint32_t (&r)[VW]) const {
-    if constexpr (kBf16<T>) {
-      unsigned short h[VW];
-#pragma unroll
-      for (int i = 0; i < VW; ++i) h[i] = __bfloat16_as_ushort(sr_st(x[i], r[i]));
-      if (VW == 4) *reinterpret_cast<uint2*>(p) = make_uint2(h[0] | (uint32_t)h[VW > 1 ? 1 : 0] << 16,
-                                                              h[VW > 2 ? 2 : 0] | (uint32_t)h[VW > 3 ? 3 : 0] << 16);
-      else *reinterpret_cast<unsigned short*>(p) = h[0];
-    } else if (VW == 4) {
-      *reinterpret_cast<float4*>(p) = make_float4(x[0], x[1], x[2], x[3]);
-    } else {
-      *p = x[0];
-    }
+    if constexpr (VW == 4) sr_st4(p, make_float4(x[0], x[1], x[2], x[3]), r);
+    else sr_st(p, x[0], r[0]);
   }
 };
 
@@ -294,7 +258,7 @@ static int opt_check(const char* who, eu_ctx* c, const void* var, const void* s1
               "when R > 0))", who);
     return EU_ERR_INVALID;
   }
-  if ((dtype != EU_FEAT_F32 && dtype != EU_FEAT_BF16) || (dtype == EU_FEAT_BF16 && !step)) {
+  if (!dtype_ok(dtype) || (dtype == EU_FEAT_BF16 && !step)) {
     set_error("%s: bad argument (dtype EU_FEAT_F32 or EU_FEAT_BF16, and a bf16 table needs the device step counter)", who);
     return EU_ERR_INVALID;
   }
@@ -364,8 +328,9 @@ static int momentum(const char* who, eu_ctx* c, void* var, void* accum, int64_t 
   const OptArgs a{lr, mom, 0.f, 0.f, 0.f, nullptr};
   const bool vec = opt_vec(D, dtype, var, accum, nullptr, grad);
   EuProfScope ps(c, "optim_momentum", dense ? N : R);
-  return dtype == EU_FEAT_BF16 ? run_one_slot<kMomentum, __nv_bfloat16>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec)
-                               : run_one_slot<kMomentum, float>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec);
+  return with_dtype(dtype, [&](auto t) {
+    return run_one_slot<kMomentum, typename decltype(t)::type>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec);
+  });
 }
 
 static int adagrad(const char* who, eu_ctx* c, void* var, void* accum, int64_t N, int32_t D, const float* grad,
@@ -377,8 +342,9 @@ static int adagrad(const char* who, eu_ctx* c, void* var, void* accum, int64_t N
   const OptArgs a{lr, 0.f, 0.f, 0.f, 0.f, nullptr};
   const bool vec = opt_vec(D, dtype, var, accum, nullptr, grad);
   EuProfScope ps(c, "optim_adagrad", dense ? N : R);
-  return dtype == EU_FEAT_BF16 ? run_one_slot<kAdagrad, __nv_bfloat16>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec)
-                               : run_one_slot<kAdagrad, float>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec);
+  return with_dtype(dtype, [&](auto t) {
+    return run_one_slot<kAdagrad, typename decltype(t)::type>(c, a, sk, var, accum, N, D, grad, rows, R, dense, vec);
+  });
 }
 
 static int adam(const char* who, eu_ctx* c, void* var, void* m, void* v, int64_t N, int32_t D, const float* grad,
@@ -395,8 +361,9 @@ static int adam(const char* who, eu_ctx* c, void* var, void* m, void* v, int64_t
   const OptArgs a{lr, 0.f, beta1, beta2, epsilon, powers};
   const bool vec = opt_vec(D, dtype, var, m, v, grad);
   EuProfScope ps(c, "optim_adam", N);
-  return dtype == EU_FEAT_BF16 ? run_adam<__nv_bfloat16>(c, a, sk, var, m, v, N, D, grad, rows, R, dense, vec)
-                               : run_adam<float>(c, a, sk, var, m, v, N, D, grad, rows, R, dense, vec);
+  return with_dtype(dtype, [&](auto t) {
+    return run_adam<typename decltype(t)::type>(c, a, sk, var, m, v, N, D, grad, rows, R, dense, vec);
+  });
 }
 
 }  // namespace eu

@@ -311,10 +311,13 @@ int sum_distinct_rows(eu_ctx* c, const RowEntries& S, const RowList& L, int dim,
                    (!S.target || aligned4_elems(S.target, S.target_dtype));
   const int G = group_lanes(ceil_div(dim, 4));
   const unsigned blocks = stride_grid((L.E + L.E / kSegChunk + 1) * G);   // >= one group per chunk, up to the grid cap
-  auto chunks = S.target_dtype == EU_FEAT_BF16 ? (vec ? k_row_chunks<true, false, __nv_bfloat16> : k_row_chunks<false, false, __nv_bfloat16>)
-                : vec ? (S.node ? k_row_chunks<true, true, float> : k_row_chunks<true, false, float>)
-                      : (S.node ? k_row_chunks<false, true, float> : k_row_chunks<false, false, float>);
-  chunks<<<blocks, 256, 0, s>>>(S, L.ord.perm, L.P, dim, G, by_key, out);
+  with_dtype(S.target_dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    auto chunks = vec ? k_row_chunks<true, false, T> : k_row_chunks<false, false, T>;
+    if constexpr (std::is_same<T, float>::value)   // a list of the gathered kind is f32
+      if (S.node) chunks = vec ? k_row_chunks<true, true, float> : k_row_chunks<false, true, float>;
+    chunks<<<blocks, 256, 0, s>>>(S, L.ord.perm, L.P, dim, G, by_key, out);
+  });
   EU_LAUNCHED();
   k_row_combine<<<stride_grid(L.E * dim), 256, 0, s>>>(L.P, dim, by_key, out, rows);
   EU_LAUNCHED();

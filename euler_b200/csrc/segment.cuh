@@ -156,15 +156,16 @@ size_t row_plan_bytes(int64_t E, int64_t n_rows, int64_t width);
 int plan_rows(eu_ctx* c, char* buf, RowList* L);
 
 // the columns [d, d + 4) of a row of f32 or bf16 (T) widened to f32 (fewer than 4 at the row's end): one 4-wide load (VEC:
-// 16 bytes of f32, 8 of bf16, so row + d is aligned to four elements) or up to four scalar loads
-template <bool VEC, typename T>
+// 16 bytes of f32, 8 of bf16, so row + d is aligned to four elements) or up to four scalar loads, through the read-only
+// cache, or (RW) plain loads of a row the kernel writes
+template <bool VEC, typename T, bool RW = false>
 __device__ __forceinline__ float4 row_load4(const T* __restrict__ row, int d, int dim) {
-  if (VEC) return feat_ld4<T>(row + d);
+  if (VEC) return RW ? rw_ld4(row + d) : feat_ld4<T>(row + d);
   float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-  v.x = feat_ld<T>(row + d);
-  if (d + 1 < dim) v.y = feat_ld<T>(row + d + 1);
-  if (d + 2 < dim) v.z = feat_ld<T>(row + d + 2);
-  if (d + 3 < dim) v.w = feat_ld<T>(row + d + 3);
+  v.x = RW ? rw_ld(row + d) : feat_ld<T>(row + d);
+  if (d + 1 < dim) v.y = RW ? rw_ld(row + d + 1) : feat_ld<T>(row + d + 1);
+  if (d + 2 < dim) v.z = RW ? rw_ld(row + d + 2) : feat_ld<T>(row + d + 2);
+  if (d + 3 < dim) v.w = RW ? rw_ld(row + d + 3) : feat_ld<T>(row + d + 3);
   return v;
 }
 

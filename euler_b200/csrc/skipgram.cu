@@ -207,7 +207,7 @@ __global__ void __launch_bounds__(256) k_sg_target_rows(const int64_t* __restric
 static int sg_check(eu_ctx* c, const int64_t* src, const int64_t* pos, const int64_t* negs, int64_t B, int32_t P, int32_t K,
                     const void* target, const void* context, int64_t n_rows, int32_t dim, int32_t dtype, const char* who) {
   if (!c || B < 0 || P < 1 || K < 0 || n_rows < 1 || dim < 1 || !target || !context ||
-      (B > 0 && (!src || !pos || (K > 0 && !negs))) || (dtype != EU_FEAT_F32 && dtype != EU_FEAT_BF16)) {
+      (B > 0 && (!src || !pos || (K > 0 && !negs))) || !dtype_ok(dtype)) {
     set_error("%s: bad argument (B >= 0, P >= 1, K >= 0, n_rows and dim >= 1, tables and ids given, a known table dtype)", who);
     return EU_ERR_INVALID;
   }
@@ -269,15 +269,11 @@ static int sg_backward(eu_ctx* c, const float* grad_loss, const int64_t* src, co
   const bool vec = dim % 4 == 0 && aligned4_elems(context, dtype) && aligned16(gt);
   const int G = group_lanes(ceil_div(dim, 4));
   const unsigned blocks = (unsigned)ceil_div(B * G, 256);
-  if (dtype == EU_FEAT_BF16) {
-    const __nv_bfloat16* cx = static_cast<const __nv_bfloat16*>(context);
-    if (vec) k_sg_target_rows<true><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
-    else k_sg_target_rows<false><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
-  } else {
-    const float* cx = static_cast<const float*>(context);
-    if (vec) k_sg_target_rows<true><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
-    else k_sg_target_rows<false><<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, cx, n_rows, dim, G, gt);
-  }
+  with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    auto k = vec ? k_sg_target_rows<true, T> : k_sg_target_rows<false, T>;
+    k<<<blocks, 256, 0, s>>>(pos, negs, B, P, K, coef, static_cast<const T*>(context), n_rows, dim, G, gt);
+  });
   EU_LAUNCHED();
   RowEntries R;   // the target list: the B src entries (gt rows), then the context entries; the context list: those only
   R.n_src = B;
@@ -321,15 +317,12 @@ static int sg_forward(eu_ctx* c, const int64_t* src, const int64_t* pos, const i
     const bool vec = dim % 4 == 0 && aligned4_elems(target, dtype) && aligned4_elems(context, dtype);
     const int G = group_lanes(ceil_div(dim, 4));   // one lane per 4-column chunk, both paths: the same order
     const unsigned blocks = (unsigned)ceil_div(B * G, 256);
-    if (dtype == EU_FEAT_BF16) {
-      const __nv_bfloat16 *t = static_cast<const __nv_bfloat16*>(target), *cx = static_cast<const __nv_bfloat16*>(context);
-      if (vec) k_sg_fwd<true><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
-      else k_sg_fwd<false><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
-    } else {
-      const float *t = static_cast<const float*>(target), *cx = static_cast<const float*>(context);
-      if (vec) k_sg_fwd<true><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
-      else k_sg_fwd<false><<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, t, cx, n_rows, dim, G, logits, rank, rowloss, bad);
-    }
+    with_dtype(dtype, [&](auto t) {
+      using T = typename decltype(t)::type;
+      auto k = vec ? k_sg_fwd<true, T> : k_sg_fwd<false, T>;
+      k<<<blocks, 256, 0, c->stream>>>(src, pos, negs, B, P, K, static_cast<const T*>(target), static_cast<const T*>(context), n_rows,
+                                       dim, G, logits, rank, rowloss, bad);
+    });
     EU_LAUNCHED();
     return EU_OK;
   });

@@ -28,9 +28,9 @@
 // Every read widens a stored element exactly to f32; only the writes round.  The exchange's store row is an overwrite, so it
 // is rounded to nearest even (feat_st); taken is the gradient row as it was, widened; the cleared row is exact zeros.  The
 // accumulation adds the same f32 sum S_v to the widened stored value with the same __fadd_rn and writes it by stochastic
-// rounding (sr_st), its 16 random bits the low half of word 0 of philox_bits(seed, *step, tensor, v dim + f), so an add
-// smaller than half an ulp is kept on average.  step is a device counter read on the device: a captured graph replays with
-// the live value.  The 4-wide path needs the bf16 tables aligned to four elements (8 bytes) and rows / taken to 16 bytes.
+// rounding (sr_st), its random word the first of SrKey{seed, step, tensor}'s for element v dim + f (common.cuh), so an add
+// smaller than half an ulp is kept on average.  The 4-wide path needs the bf16 tables aligned to four elements (8 bytes) and
+// rows / taken to 16 bytes.
 #include <type_traits>
 
 #include "segment.cuh"
@@ -49,48 +49,18 @@ __global__ void k_store_keys(const int64_t* __restrict__ ids, int64_t M, int64_t
   }
 }
 
-// columns [d, d + 4) of a row of T (fewer at its end), each value rounded to nearest by feat_st: one 4-wide store (VEC: a
-// float4, or 8 bytes of bf16) or up to four scalar stores
+// columns [d, d + 4) of a row of T (fewer at its end), each value rounded to nearest: one 4-wide store (VEC) or up to four
+// scalar stores
 template <bool VEC, typename T>
 __device__ __forceinline__ void row_store4(T* __restrict__ row, int d, int dim, float4 v) {
   if (VEC) {
-    if constexpr (std::is_same<T, float>::value) {
-      *reinterpret_cast<float4*>(row + d) = v;
-    } else {
-      const uint32_t lo = __bfloat16_as_ushort(feat_st<T>(v.x)) | (uint32_t)__bfloat16_as_ushort(feat_st<T>(v.y)) << 16;
-      const uint32_t hi = __bfloat16_as_ushort(feat_st<T>(v.z)) | (uint32_t)__bfloat16_as_ushort(feat_st<T>(v.w)) << 16;
-      *reinterpret_cast<uint2*>(row + d) = make_uint2(lo, hi);
-    }
+    rn_st4(row + d, v);
     return;
   }
   row[d] = feat_st<T>(v.x);
   if (d + 1 < dim) row[d + 1] = feat_st<T>(v.y);
   if (d + 2 < dim) row[d + 2] = feat_st<T>(v.z);
   if (d + 3 < dim) row[d + 3] = feat_st<T>(v.w);
-}
-
-// one element of a table of T, widened to f32, through the read-write path (the table is written by the same kernel)
-__device__ __forceinline__ float store_ld(const float* p) { return *p; }
-__device__ __forceinline__ float store_ld(const __nv_bfloat16* p) {
-  return __uint_as_float((uint32_t)*reinterpret_cast<const unsigned short*>(p) << 16);
-}
-
-// columns [d, d + 4) of a row of T widened to f32 through the read-write path (0 past the row's end): one 4-wide load (VEC)
-// or up to four scalar loads
-template <bool VEC, typename T>
-__device__ __forceinline__ float4 store_ld4(const T* row, int d, int dim) {
-  if constexpr (std::is_same<T, float>::value) {
-    return VEC ? *reinterpret_cast<const float4*>(row + d) : make_float4(row[d], d + 1 < dim ? row[d + 1] : 0.f,
-                                                                         d + 2 < dim ? row[d + 2] : 0.f, d + 3 < dim ? row[d + 3] : 0.f);
-  } else {
-    if (VEC) {
-      const uint2 u = *reinterpret_cast<const uint2*>(row + d);
-      return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
-                         __uint_as_float(u.y & 0xFFFF0000u));
-    }
-    return make_float4(store_ld(row + d), d + 1 < dim ? store_ld(row + d + 1) : 0.f, d + 2 < dim ? store_ld(row + d + 2) : 0.f,
-                       d + 3 < dim ? store_ld(row + d + 3) : 0.f);
-  }
 }
 
 // G lanes per distinct id p of the plan (segment [start[p], start[p + 1]) of the stable order perm), 4 columns per lane and
@@ -116,7 +86,7 @@ __global__ void __launch_bounds__(256) k_store_exchange(DistinctPlan P, const in
     for (int d = sub * 4; d < dim; d += G * 4) {
       float4 g = nan4;
       if (real) {
-        g = store_ld4<VEC>(gs, d, dim);
+        g = row_load4<VEC, T, true>(gs, d, dim);
         row_store4<VEC>(s, d, dim, row_load4<VEC>(last, d, dim));
         row_store4<VEC>(gs, d, dim, make_float4(0.f, 0.f, 0.f, 0.f));
       }
@@ -132,6 +102,7 @@ template <typename T>
 __global__ void k_store_add(DistinctPlan P, int64_t n_rows, int dim, const float* __restrict__ vals, T* __restrict__ grad_store,
                             unsigned long long seed, const int64_t* __restrict__ step, uint32_t tensor) {
   const int64_t D = __ldg(P.nd);
+  const SrKey sk{seed, step, tensor};
   uint32_t s32 = 0;
   if constexpr (!std::is_same<T, float>::value) s32 = (uint32_t)__ldg(step);
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < D * dim; t += (int64_t)gridDim.x * blockDim.x) {
@@ -139,9 +110,9 @@ __global__ void k_store_add(DistinctPlan P, int64_t n_rows, int dim, const float
     const int64_t v = __ldg(P.key + p);
     if (v < n_rows) {
       const int64_t e = v * dim + f;
-      const float x = __fadd_rn(store_ld(grad_store + e), __ldg(vals + t));
+      const float x = __fadd_rn(rw_ld(grad_store + e), __ldg(vals + t));
       if constexpr (std::is_same<T, float>::value) grad_store[e] = x;
-      else grad_store[e] = sr_st(x, philox_bits(seed, s32, tensor, (unsigned long long)e).x);
+      else grad_store[e] = sr_st(x, sr_bits(sk, s32, (unsigned long long)e).x);
     }
   }
 }
@@ -192,16 +163,11 @@ static int store_plan(eu_ctx* c, const int64_t* ids, int64_t M, int64_t n_rows, 
   return plan_rows(c, m + o_plan, L);
 }
 
-static bool store_dtype_ok(int32_t dtype) { return dtype == EU_FEAT_F32 || dtype == EU_FEAT_BF16; }
-
 static int store_exchange(eu_ctx* c, void* store, void* grad_store, int64_t n_rows, int32_t dim, const int64_t* ids, int64_t M,
                           const float* rows, float* taken, int32_t dtype, const char* who) {
   int rc = store_check(c, store && grad_store && (M == 0 || (ids && rows && taken)), n_rows, dim, M, who);
   if (rc) return rc;
-  if (!store_dtype_ok(dtype)) {
-    set_error("%s: unknown store dtype %d (EU_FEAT_F32 or EU_FEAT_BF16)", who, (int)dtype);
-    return EU_ERR_INVALID;
-  }
+  if ((rc = dtype_check(dtype, who, "store"))) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   if (M == 0) return EU_OK;
   RowList L;
@@ -215,14 +181,11 @@ static int store_exchange(eu_ctx* c, void* store, void* grad_store, int64_t n_ro
                    aligned16(taken);
   const int G = group_lanes(ceil_div(dim, 4));
   EuProfScope ps(c, "store_exchange", M);
-  if (dtype == EU_FEAT_BF16) {
-    auto k = vec ? k_store_exchange<true, __nv_bfloat16> : k_store_exchange<false, __nv_bfloat16>;
-    k<<<stride_grid(M * G), 256, 0, c->stream>>>(L.P, L.ord.perm, n_rows, dim, G, rows, (__nv_bfloat16*)store,
-                                                 (__nv_bfloat16*)grad_store, taken);
-  } else {
-    auto k = vec ? k_store_exchange<true, float> : k_store_exchange<false, float>;
-    k<<<stride_grid(M * G), 256, 0, c->stream>>>(L.P, L.ord.perm, n_rows, dim, G, rows, (float*)store, (float*)grad_store, taken);
-  }
+  with_dtype(dtype, [&](auto t) {
+    using T = typename decltype(t)::type;
+    auto k = vec ? k_store_exchange<true, T> : k_store_exchange<false, T>;
+    k<<<stride_grid(M * G), 256, 0, c->stream>>>(L.P, L.ord.perm, n_rows, dim, G, rows, (T*)store, (T*)grad_store, taken);
+  });
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -237,7 +200,7 @@ static int store_accumulate(eu_ctx* c, void* grad_store, int64_t n_rows, int32_t
               (long long)M);
     return EU_ERR_INVALID;
   }
-  if (!store_dtype_ok(dtype) || (dtype == EU_FEAT_BF16 && !step)) {
+  if (!dtype_ok(dtype) || (dtype == EU_FEAT_BF16 && !step)) {
     set_error("%s: bad argument (dtype EU_FEAT_F32 or EU_FEAT_BF16, and a bf16 gradient store needs the device step counter)",
               who);
     return EU_ERR_INVALID;
@@ -260,11 +223,10 @@ static int store_accumulate(eu_ctx* c, void* grad_store, int64_t n_rows, int32_t
   R.group = count;
   R.pool_den = pool == EU_POOL_MEAN ? (float)count : 0.f;
   if ((rc = sum_distinct_rows(c, R, L, dim, false, vals, nullptr))) return rc;
-  if (dtype == EU_FEAT_BF16)
-    k_store_add<__nv_bfloat16><<<stride_grid(M * dim), 256, 0, c->stream>>>(L.P, n_rows, dim, vals, (__nv_bfloat16*)grad_store,
-                                                                            seed, step, (uint32_t)tensor);
-  else
-    k_store_add<float><<<stride_grid(M * dim), 256, 0, c->stream>>>(L.P, n_rows, dim, vals, (float*)grad_store, 0, nullptr, 0);
+  with_dtype(dtype, [&](auto t) {   // an f32 store never reads the key
+    using T = typename decltype(t)::type;
+    k_store_add<T><<<stride_grid(M * dim), 256, 0, c->stream>>>(L.P, n_rows, dim, vals, (T*)grad_store, seed, step, (uint32_t)tensor);
+  });
   EU_LAUNCHED();
   return EU_OK;
 }

@@ -92,16 +92,9 @@ static int launch_top_k(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_
   const auto* nd = (const unsigned long long*)nodes;
   const auto* nb = (const unsigned long long*)neighbors;
   const DevGraph& g = c->g->d;
-  if (g.feat_place == EU_FEAT_HOST) {
-    if (g.feat_dtype == EU_FEAT_BF16)
-      k_neighbor_top_k<__nv_bfloat16, KMAX, C, kFeatHost><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
-    else
-      k_neighbor_top_k<float, KMAX, C, kFeatHost><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
-  } else if (g.feat_dtype == EU_FEAT_BF16) {
-    k_neighbor_top_k<__nv_bfloat16, KMAX, C, kFeatDevice><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
-  } else {
-    k_neighbor_top_k<float, KMAX, C, kFeatDevice><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
-  }
+  with_feat(g, [&](auto t, auto p) {
+    k_neighbor_top_k<typename decltype(t)::type, KMAX, C, decltype(p)::value><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
+  });
   EU_LAUNCHED();
   return EU_OK;
 }

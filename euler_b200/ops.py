@@ -1192,18 +1192,24 @@ def table_proxy(table):
     return torch.zeros(1, dtype=torch.float32, device=table.device).as_strided(tuple(table.shape), (0, 0)).requires_grad_()
 
 
+def _table_dtype(op, named, mixed=None):
+    """the storage dtype of the tables named [(name, table)], float32 when there are none: raises EulerError unless each is a
+    2-D float32 or bfloat16 tensor, then unless all have one dtype (mixed(dtypes): that error's text, where the op words it)"""
+    for nm, t in named:
+        if not torch.is_tensor(t) or t.dtype not in _lib.TORCH_DTYPES or t.dim() != 2:
+            raise EulerError("%s: %s must be a 2-D float32 or bfloat16 tensor" % (op, nm))
+    dtypes = [t.dtype for _, t in named]
+    if len(set(dtypes)) > 1:
+        raise EulerError(mixed(dtypes) if mixed else "%s: the tables must have one dtype, got %s" % (op, [str(d) for d in dtypes]))
+    return dtypes[0] if dtypes else torch.float32
+
+
 def _check_tables(op, named, proxies=None):
     """the storage dtype of the embedding tables named [(name, table)] (None entries skipped): raise unless all are 2-D
     float32 or bfloat16 tensors of one dtype, no bf16 table requires grad, and proxies (None, or one entry per named table:
     None or a gradient proxy) gives proxies to bf16 tables only, each a float32 leaf of its table's shape that requires grad"""
     present = [(nm, t) for nm, t in named if t is not None]
-    for nm, t in present:
-        if not torch.is_tensor(t) or t.dtype not in _TABLE_DTYPES or t.dim() != 2:
-            raise EulerError("%s: %s must be a 2-D float32 or bfloat16 tensor" % (op, nm))
-    dtypes = {t.dtype for _, t in present}
-    if len(dtypes) > 1:
-        raise EulerError("%s: the tables must have one dtype, got %s" % (op, [str(t.dtype) for _, t in present]))
-    dt = dtypes.pop() if dtypes else torch.float32
+    dt = _table_dtype(op, present)
     if dt == torch.bfloat16 and any(t.requires_grad for _, t in present):
         raise EulerError("%s: a bfloat16 table takes no autograd gradient (torch would round it to bf16); give it a gradient "
                          "proxy (table_proxy) and train it with optimizers.minimize" % op)
@@ -1311,7 +1317,7 @@ def _shallow_problem(nodes, id_table, dense, sparse, comb):
         q.fid, q.dim, q.combiner, q.default_value = fid, table.shape[1], c, default
         q.n_rows, q.table = table.shape[0], table.data_ptr()
     first = id_table if id_table is not None else (sparse[0][1] if sparse else None)
-    p.table_dtype = _TABLE_DTYPES[first.dtype] if first is not None else 0
+    p.table_dtype = _lib.TORCH_DTYPES[first.dtype] if first is not None else 0
     return p
 
 
@@ -1489,12 +1495,13 @@ def shallow_encode_pool(nodes, count, id_table=None, dense=(), sparse=(), pool='
 # ------------------------------------------------------------------------------------ embedding stores
 def _store_table(op, named):
     """the tables a store op updates in place: 2-D, contiguous, on the graph's device, all float32 or all bfloat16; returns
-    that dtype"""
-    dt = named[0][1].dtype if torch.is_tensor(named[0][1]) else None
-    for nm, t in named:
-        if not torch.is_tensor(t) or t.dtype not in (torch.float32, torch.bfloat16) or t.dtype != dt or t.dim() != 2:
+    that dtype.  Each table is checked whole before the next."""
+    for i, (nm, t) in enumerate(named):
+        try:
+            dt = _table_dtype(op, named[:i + 1])
+        except EulerError:
             raise EulerError("%s: %s must be 2-D float32 or bfloat16 tensors of one dtype"
-                             % (op, " and ".join(nm for nm, _ in named)))
+                             % (op, " and ".join(nm for nm, _ in named))) from None
         if not t.is_contiguous() or t.device != _dev():
             raise EulerError("%s: %s must be contiguous on %s" % (op, nm, _dev()))
     return dt
@@ -1689,10 +1696,6 @@ def skipgram_metric(rank, name):
     raise EulerError("skipgram metric must be one of %s, got %r" % (SKIPGRAM_METRICS, name))
 
 
-# the storage types of the skip-gram step's tables (eu_feat_dtype)
-_TABLE_DTYPES = {torch.float32: 0, torch.bfloat16: 1}
-
-
 def _raw_skipgram(src, pos, negs, target, context):
     """one eu_skipgram_loss (eu_skipgram_loss_dtype for bf16 tables): (logits f32[B, P + K], rank i32[B], loss f32[])"""
     B, P = pos.shape
@@ -1770,11 +1773,8 @@ def _skipgram_args(op, src, pos, negs, target, context, metric):
     if metric not in SKIPGRAM_METRICS:
         raise EulerError("%s: metric must be one of %s, got %r" % (op, SKIPGRAM_METRICS, metric))
     shared = context is target
-    for nm, t in (('target', target), ('context', context)):
-        if not torch.is_tensor(t) or t.dtype not in _TABLE_DTYPES or t.dim() != 2:
-            raise EulerError("%s: %s must be a 2-D float32 or bfloat16 tensor" % (op, nm))
-    if target.dtype != context.dtype:
-        raise EulerError("%s: target (%s) and context (%s) must have one dtype" % (op, target.dtype, context.dtype))
+    _table_dtype(op, (('target', target), ('context', context)),
+                 lambda d: "%s: target (%s) and context (%s) must have one dtype" % (op, d[0], d[1]))
     if target.shape != context.shape:
         raise EulerError("%s: target %s and context %s must have one shape" % (op, tuple(target.shape), tuple(context.shape)))
     src = _t(src, torch.int64).reshape(-1)
@@ -2098,7 +2098,7 @@ def _raw_kg(ent, relt, eaux, raux, src, dst, rel, neg, cfg):
     embs = [torch.empty((B, rel_dim), dtype=torch.float32, device=dev) for _ in range(3)] if with_emb else None
     p = _kg_problem(model, l1, corrupt, margin, src, dst, rel, neg, (ent, relt, eaux, raux), ent_dim, rel_dim)
     if ent.dtype == torch.bfloat16:
-        _call("eu_kg_loss_dtype", C.byref(p), _TABLE_DTYPES[ent.dtype], scores, rank, loss, *(embs or [None] * 3))
+        _call("eu_kg_loss_dtype", C.byref(p), _lib.TORCH_DTYPES[ent.dtype], scores, rank, loss, *(embs or [None] * 3))
     else:
         _call("eu_kg_loss", C.byref(p), scores, rank, loss, *(embs or [None] * 3))
     return scores, rank, loss, embs
@@ -2115,7 +2115,7 @@ def _raw_kg_sparse_grads(slots, src, dst, rel, neg, cfg, scores, g):
     counts = (C.c_int64 * 4)()
     outs = ([r for r, _ in bufs], [v for _, v in bufs], counts)
     if slots[0].dtype == torch.bfloat16:
-        _call("eu_kg_loss_backward_sparse_dtype", C.byref(p), _TABLE_DTYPES[slots[0].dtype], g, scores, *outs)
+        _call("eu_kg_loss_backward_sparse_dtype", C.byref(p), _lib.TORCH_DTYPES[slots[0].dtype], g, scores, *outs)
     else:
         _call("eu_kg_loss_backward_sparse", C.byref(p), g, scores, *outs)
     return bufs, list(counts)
@@ -2167,11 +2167,7 @@ def _kg_args(op, src, dst, neg, rel, tables, model, corrupt, metric):
     tables = list(tables)
     if len(tables) != len(want):
         raise EulerError("%s: %s takes %d tables, got %d" % (op, name, len(want), len(tables)))
-    for k, tb in enumerate(tables):
-        if not torch.is_tensor(tb) or tb.dtype not in _TABLE_DTYPES or tb.dim() != 2:
-            raise EulerError("%s: table %d must be a 2-D float32 or bfloat16 tensor" % (op, k))
-    if any(tb.dtype != tables[0].dtype for tb in tables):
-        raise EulerError("%s: the tables must have one dtype, got %s" % (op, [str(tb.dtype) for tb in tables]))
+    _table_dtype(op, [("table %d" % k, tb) for k, tb in enumerate(tables)])
     slots = [None] * 4
     for t, tb in zip(want, tables):
         slots[t] = _t(tb, tb.dtype)
