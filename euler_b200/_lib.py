@@ -206,6 +206,14 @@ SIGNATURES = {
     "eu_scatter_mean": (C.c_int, [_P, _P, _I64, _P, _I64, _I64, _P]),
     "eu_sage_mean_aggregate": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
     "eu_sage_add_aggregate": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
+    "eu_get_dense_feature_out_dtype": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32, _P]),
+    "eu_get_dense_feature_host_out_dtype": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32, _P]),
+    "eu_sage_mean_aggregate_out_dtype": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32, _P]),
+    "eu_sage_mean_aggregate_host_out_dtype": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32, _P]),
+    "eu_sage_add_aggregate_out_dtype": (C.c_int, [_P, _P, _I64, _I32, _I32, _I32, _P]),
+    "eu_neighbor_top_k_feature_out_dtype": (C.c_int, [_P, _P, _I64, _P, _I32, _I32, _I32, _I32, _I32, _P]),
+    "eu_sample_fanout_with_feature_out_dtype": (C.c_int, [_P, _P, _I64, _P, _I32, _P, _I32, _I64, _P, _P, _P, _P, _I32, _P, _P, _I32,
+                                                          _P, _I32, _P, _P, _P, _P]),
     "eu_gat_aggregate": (C.c_int, [_P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P]),
     "eu_gat_aggregate_backward": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _I32, _P, _P, _P]),
     "eu_agnn_aggregate": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I64, _I64, _I64, _I32, _P, _P, _P]),

@@ -207,30 +207,55 @@ int eu_random_walk_host(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_
   return io.finish();
 }
 
-int eu_get_dense_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, float* out) {
-  if (!c || M < 0 || dim < 0 || (M > 0 && (!nodes || !out))) { set_error("eu_get_dense_feature_host: bad argument"); return EU_ERR_INVALID; }
+// bytes of one output element of a checked eu_feat_dtype code
+static int64_t out_elem_bytes(int32_t dtype) { return dtype == EU_FEAT_BF16 ? 2 : 4; }
+
+static int dense_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, int32_t out_dtype, void* out,
+                              const char* who) {
+  if (!c || M < 0 || dim < 0 || (M > 0 && (!nodes || !out))) { set_error("%s: bad argument", who); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(out_dtype, who, "output")) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   HostIO io{c};
-  const int64_t o_nodes = io.in(nodes, 8 * M), o_out = io.out(out, 4 * M * dim);
+  const int64_t o_nodes = io.in(nodes, 8 * M), o_out = io.out(out, out_elem_bytes(out_dtype) * M * dim);
   int rc;
   if ((rc = io.begin()) || (rc = io.upload())) return rc;
-  if ((rc = eu_get_dense_feature(c, io.dev<const int64_t>(o_nodes), M, fid, dim, io.dev<float>(o_out)))) return rc;
+  if ((rc = out_dtype == EU_FEAT_F32
+                ? eu_get_dense_feature(c, io.dev<const int64_t>(o_nodes), M, fid, dim, io.dev<float>(o_out))
+                : eu_get_dense_feature_out_dtype(c, io.dev<const int64_t>(o_nodes), M, fid, dim, out_dtype, io.dev<void>(o_out)))) return rc;
   if ((rc = io.download())) return rc;
   return io.finish();
 }
 
 // eu_sage_mean_aggregate with host buffers: only the neighbor ids go up and only the [rows, dim] means come down -- the
 // rows*count feature rows the unfused composition (get_dense_feature_host + scatter_mean) would move never leave HBM.
-int eu_sage_mean_aggregate_host(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out) {
-  if (!c || rows < 0 || count < 0 || dim <= 0 || (rows > 0 && (!nbr_ids || !out))) { set_error("eu_sage_mean_aggregate_host: bad argument"); return EU_ERR_INVALID; }
+static int sage_mean_aggregate_host(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, int32_t out_dtype,
+                                    void* out, const char* who) {
+  if (!c || rows < 0 || count < 0 || dim <= 0 || (rows > 0 && (!nbr_ids || !out))) { set_error("%s: bad argument", who); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(out_dtype, who, "output")) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   HostIO io{c};
-  const int64_t o_ids = io.in(nbr_ids, 8 * rows * count), o_out = io.out(out, 4 * rows * dim);
+  const int64_t o_ids = io.in(nbr_ids, 8 * rows * count), o_out = io.out(out, out_elem_bytes(out_dtype) * rows * dim);
   int rc;
   if ((rc = io.begin()) || (rc = io.upload())) return rc;
-  if ((rc = eu_sage_mean_aggregate(c, io.dev<const int64_t>(o_ids), rows, count, dim, io.dev<float>(o_out)))) return rc;
+  if ((rc = out_dtype == EU_FEAT_F32
+                ? eu_sage_mean_aggregate(c, io.dev<const int64_t>(o_ids), rows, count, dim, io.dev<float>(o_out))
+                : eu_sage_mean_aggregate_out_dtype(c, io.dev<const int64_t>(o_ids), rows, count, dim, out_dtype, io.dev<void>(o_out)))) return rc;
   if ((rc = io.download())) return rc;
   return io.finish();
+}
+
+int eu_get_dense_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, float* out) {
+  return dense_feature_host(c, nodes, M, fid, dim, EU_FEAT_F32, out, "eu_get_dense_feature_host");
+}
+int eu_get_dense_feature_host_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, int32_t out_dtype, void* out) {
+  return dense_feature_host(c, nodes, M, fid, dim, out_dtype, out, "eu_get_dense_feature_host_out_dtype");
+}
+int eu_sage_mean_aggregate_host(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out) {
+  return sage_mean_aggregate_host(c, nbr_ids, rows, count, dim, EU_FEAT_F32, out, "eu_sage_mean_aggregate_host");
+}
+int eu_sage_mean_aggregate_host_out_dtype(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, int32_t out_dtype,
+                                          void* out) {
+  return sage_mean_aggregate_host(c, nbr_ids, rows, count, dim, out_dtype, out, "eu_sage_mean_aggregate_host_out_dtype");
 }
 
 int eu_gather_host(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_t* idx, int64_t E, float* out) {

@@ -34,11 +34,11 @@ __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<floa
 
 // ---------------------------------------------------------------------------- feature fetch
 // out[i, 0:dim] = feat[row(ids[i]), 0:min(feat_dim,dim)], zeros elsewhere / for unknown ids.  T: the table's storage type, P
-// its placement.
-template <typename T, bool VEC, int P>
+// its placement, O the output's element type (float, or __nv_bfloat16: each value rounded once at the store).
+template <typename T, typename O, bool VEC, int P>
 __global__ void __launch_bounds__(256) k_feature(DevGraph g, const unsigned long long* __restrict__ ids,
                                                  int64_t M, int32_t dim, int G, int32_t soff, int32_t sdim,
-                                                 float* __restrict__ out) {
+                                                 O* __restrict__ out) {
   const int sh = 31 - __clz(G);   // G is a power of two
   const int sub = (int)(threadIdx.x & (G - 1));
   const int64_t stride = ((int64_t)gridDim.x * blockDim.x) >> sh;
@@ -47,16 +47,16 @@ __global__ void __launch_bounds__(256) k_feature(DevGraph g, const unsigned long
   for (int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> sh; i < M; i += stride) {
     const int64_t row = sdim > 0 ? lookup_row(g, ids[i]) : -1;
     const int32_t fd = sdim;  // stored width of this slot
-    float* o = out + i * (int64_t)dim;
+    O* o = out + i * (int64_t)dim;
     const T* f = row >= 0 ? feat_row<T, P>(g, row) + soff : nullptr;
     if (VEC) {
       for (int32_t d = sub * 4; d < dim; d += G * 4) {
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         if (f && d < fd) v = feat_ld4(f + d);  // VEC requires fd % 4 == 0 so a float4 never straddles fd
-        st4(o + d, v);
+        rn_st4(o + d, v);
       }
     } else {
-      for (int32_t d = sub; d < dim; d += G) o[d] = (f && d < fd) ? feat_ld(f + d) : 0.f;
+      for (int32_t d = sub; d < dim; d += G) o[d] = feat_st<O>((f && d < fd) ? feat_ld(f + d) : 0.f);
     }
   }
 }
@@ -247,10 +247,11 @@ __global__ void __launch_bounds__(256) k_sage_classify(DevGraph g, const unsigne
 // per lane are accumulated.
 // NV float4 per lane: rows of up to NV * 128 floats.  FULL: the width is exactly NV * 128 (128 / 256: no column guards, the
 // width is a compile-time constant); otherwise any multiple of 4 up to NV * 128 (e.g. 64 of configs[4]) with guarded columns.
-template <typename T, int NV, bool FULL, int P>
+// O: the output's element type; the sum and the division are f32 whatever it is, and a bf16 output is rounded once at the store.
+template <typename T, typename O, int NV, bool FULL, int P>
 __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned long long* __restrict__ ids,
                                                    int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
-                                                   int32_t count, bool mean, float* __restrict__ out) {
+                                                   int32_t count, bool mean, O* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int32_t fd = FULL ? NV * 128 : g.feat_dim;    // == dim, a multiple of 4, <= NV * 128 (checked by the launcher)
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -296,21 +297,21 @@ __global__ void __launch_bounds__(256) k_sage_mean(DevGraph g, const unsigned lo
     }
   }
   const float denom = __fadd_rn((float)count, 1e-7f);
-  float* o = out + r * (int64_t)fd + lane * 4;
+  O* o = out + r * (int64_t)fd + lane * 4;
 #pragma unroll
   for (int t = 0; t < NV; ++t) {
     float4 a = acc[t];
     if (mean) { a.x = __fdiv_rn(a.x, denom); a.y = __fdiv_rn(a.y, denom); a.z = __fdiv_rn(a.z, denom); a.w = __fdiv_rn(a.w, denom); }
-    if (FULL || lane * 4 + t * 128 < fd) st4(o + t * 128, a);
+    if (FULL || lane * 4 + t * 128 < fd) rn_st4(o + t * 128, a);
   }
   }
 }
 
 // generic width fallback: one warp per representative, scalar columns
-template <typename T, int P>
+template <typename T, typename O, int P>
 __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const unsigned long long* __restrict__ ids,
                                                            int64_t rows, const int32_t* __restrict__ list, const unsigned int* __restrict__ n_list,
-                                                           int32_t count, int32_t dim, bool mean, float* __restrict__ out) {
+                                                           int32_t count, int32_t dim, bool mean, O* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int32_t fd = g.feat_dim;
   const float denom = __fadd_rn((float)count, 1e-7f);
@@ -324,18 +325,20 @@ __global__ void __launch_bounds__(256) k_sage_mean_generic(DevGraph g, const uns
         const int64_t row = lookup_row(g, __ldg(ids + r * count + j));
         acc = __fadd_rn(acc, (row >= 0 && d < fd) ? feat_ld(feat_row<T, P>(g, row, fd, 0) + d) : 0.f);
       }
-      out[r * (int64_t)dim + d] = mean ? __fdiv_rn(acc, denom) : acc;
+      out[r * (int64_t)dim + d] = feat_st<O>(mean ? __fdiv_rn(acc, denom) : acc);
     }
   }
 }
 
 // G lanes per row (G a power of two): a duplicate gets its representative's output, a row without a neighbor gets +0.0 (what
 // the reduction writes for it: it starts at +0.0 and adds nothing); representatives are already done.  Then every slot the
-// representatives claimed is freed.
-template <bool VEC>
+// representatives claimed is freed.  O: the output's element type.  A bf16 representative row goes through feat_ld / rn_st4
+// unchanged: it was rounded by the same rounding, which maps a widened bf16 value to its own bits (NaN to the same canonical
+// NaN).
+template <typename O, bool VEC>
 __global__ void __launch_bounds__(256) k_sage_broadcast(const int32_t* __restrict__ src, int64_t rows, int32_t dim, int G,
                                                         const uint32_t* __restrict__ rep_slot, const unsigned int* __restrict__ n_rep,
-                                                        unsigned long long* tab, float* out) {
+                                                        unsigned long long* tab, O* out) {
   const int sh = 31 - __clz(G);
   const int sub = (int)(threadIdx.x & (G - 1));
   const int64_t gtid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -343,12 +346,12 @@ __global__ void __launch_bounds__(256) k_sage_broadcast(const int32_t* __restric
   for (int64_t r = gtid >> sh; r < rows; r += nthreads >> sh) {
     const int64_t s = __ldg(src + r);
     if (s == r) continue;
-    float* o = out + r * (int64_t)dim;
-    const float* f = s >= 0 ? out + s * (int64_t)dim : nullptr;   // a representative's row: not written by this kernel
+    O* o = out + r * (int64_t)dim;
+    const O* f = s >= 0 ? out + s * (int64_t)dim : nullptr;   // a representative's row: not written by this kernel
     if (VEC) {
-      for (int32_t d = sub * 4; d < dim; d += G * 4) st4(o + d, f ? ldg4(f + d) : make_float4(0.f, 0.f, 0.f, 0.f));
+      for (int32_t d = sub * 4; d < dim; d += G * 4) rn_st4(o + d, f ? feat_ld4(f + d) : make_float4(0.f, 0.f, 0.f, 0.f));
     } else {
-      for (int32_t d = sub; d < dim; d += G) o[d] = f ? __ldg(f + d) : 0.f;
+      for (int32_t d = sub; d < dim; d += G) o[d] = feat_st<O>(f ? feat_ld(f + d) : 0.f);
     }
   }
   const int64_t n = (int64_t)__ldg(n_rep);
@@ -408,18 +411,19 @@ static int scatter(eu_ctx* c, const float* upd, int64_t D, const int32_t* idx, i
   return EU_OK;
 }
 
-// the fused SAGE reduction over a table of T placed at P; v4: the float4 path's conditions hold (fanout_aggregate)
-template <typename T, int P>
+// the fused SAGE reduction over a table of T placed at P into an output of O; v4: the float4 path's conditions hold
+// (fanout_aggregate)
+template <typename T, typename O, int P>
 static int launch_sage_mean(eu_ctx* c, const DevGraph& d, const unsigned long long* ids, int64_t rows, const int32_t* reps,
-                            const unsigned int* nrep, int32_t count, int32_t dim, bool mean, bool v4, unsigned blocks, float* out) {
+                            const unsigned int* nrep, int32_t count, int32_t dim, bool mean, bool v4, unsigned blocks, O* out) {
   cudaStream_t s = c->stream;
-  if (v4 && dim == 128) k_sage_mean<T, 1, true, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim == 256) k_sage_mean<T, 2, true, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 128) k_sage_mean<T, 1, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 256) k_sage_mean<T, 2, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4 && dim <= 512) k_sage_mean<T, 4, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else if (v4) k_sage_mean<T, 8, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
-  else k_sage_mean_generic<T, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, dim, mean, out);
+  if (v4 && dim == 128) k_sage_mean<T, O, 1, true, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim == 256) k_sage_mean<T, O, 2, true, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 128) k_sage_mean<T, O, 1, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 256) k_sage_mean<T, O, 2, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4 && dim <= 512) k_sage_mean<T, O, 4, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else if (v4) k_sage_mean<T, O, 8, false, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, mean, out);
+  else k_sage_mean_generic<T, O, P><<<blocks, 256, 0, s>>>(d, ids, rows, reps, nrep, count, dim, mean, out);
   EU_LAUNCHED();
   return EU_OK;
 }
@@ -430,22 +434,27 @@ using namespace eu;
 
 extern "C" {
 
-int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, float* out) {
-  if (!c || M < 0 || dim < 0 || (M > 0 && (!nodes || (dim > 0 && !out)))) { set_error("eu_get_dense_feature: bad argument"); return EU_ERR_INVALID; }
+static int dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, int32_t out_dtype, void* out,
+                         const char* who) {
+  if (!c || M < 0 || dim < 0 || (M > 0 && (!nodes || (dim > 0 && !out)))) { set_error("%s: bad argument", who); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(out_dtype, who, "output")) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   if (M == 0 || dim == 0) return EU_OK;
   const DevGraph& d = c->g->d;
   int32_t soff, sdim;
   dense_slot(d, fid, &soff, &sdim);
-  const bool vec = (dim % 4 == 0) && (d.feat_dim % 4 == 0) && (soff % 4 == 0) && (sdim % 4 == 0) && aligned16(out);
+  const bool vec = (dim % 4 == 0) && (d.feat_dim % 4 == 0) && (soff % 4 == 0) && (sdim % 4 == 0) && aligned4_elems(out, out_dtype);
   const int G = vec ? group_lanes(dim / 4) : (dim >= 32 ? 32 : 1);
   const unsigned blocks = capped_grid(ceil_div(M * G, 256), "EU_FEATURE_CTAS", 0);
   EuProfScope ps(c, "k_feature", M);
   with_feat(d, [&](auto t, auto p) {
-    using T = typename decltype(t)::type;
-    constexpr int P = decltype(p)::value;
-    auto k = vec ? k_feature<T, true, P> : k_feature<T, false, P>;
-    k<<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, out);
+    with_dtype(out_dtype, [&](auto o) {
+      using T = typename decltype(t)::type;
+      using O = typename decltype(o)::type;
+      constexpr int P = decltype(p)::value;
+      auto k = vec ? k_feature<T, O, true, P> : k_feature<T, O, false, P>;
+      k<<<blocks, 256, 0, c->stream>>>(d, (const unsigned long long*)nodes, M, dim, G, soff, sdim, (O*)out);
+    });
   });
   EU_LAUNCHED();
   return EU_OK;
@@ -465,6 +474,13 @@ int eu_gather(eu_ctx* c, const float* params, int64_t N, int64_t D, const int32_
   return EU_OK;
 }
 
+int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, float* out) {
+  return dense_feature(c, nodes, M, fid, dim, EU_FEAT_F32, out, "eu_get_dense_feature");
+}
+int eu_get_dense_feature_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, int32_t out_dtype, void* out) {
+  return dense_feature(c, nodes, M, fid, dim, out_dtype, out, "eu_get_dense_feature_out_dtype");
+}
+
 int eu_scatter_add(eu_ctx* c, const float* u, int64_t D, const int32_t* idx, int64_t E, int64_t size, float* out) {
   return scatter<OP_ADD>(c, u, D, idx, E, size, out);
 }
@@ -475,8 +491,10 @@ int eu_scatter_mean(eu_ctx* c, const float* u, int64_t D, const int32_t* idx, in
   return scatter<OP_MEAN>(c, u, D, idx, E, size, out);
 }
 
-static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, bool mean, float* out) {
-  if (!c || rows < 0 || count < 0 || dim <= 0 || (rows > 0 && (!nbr_ids || !out))) { set_error("eu_sage_mean_aggregate: bad argument"); return EU_ERR_INVALID; }
+static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, bool mean, int32_t out_dtype,
+                            void* out, const char* who) {
+  if (!c || rows < 0 || count < 0 || dim <= 0 || (rows > 0 && (!nbr_ids || !out))) { set_error("%s: bad argument", who); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(out_dtype, who, "output")) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   if (rows == 0) return EU_OK;
   cudaStream_t s = c->stream;
@@ -500,31 +518,46 @@ static int fanout_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int
   const unsigned int* nrep = c->d_agg_nrep;
   { EuProfScope ps(c, mean ? "k_sage_mean" : "k_sage_add", rows);
     // float4 path: one slot of the full stored width, a multiple of 4 floats up to 1024 (D = 64 of configs[4], 128, 256, ...),
-    // on a table aligned to four elements (16 bytes of f32, 8 of bf16)
-    const bool v4 = d.n < ((int64_t)1 << 31) && d.n_slots == 1 && dim == d.feat_dim && (dim & 3) == 0 && dim <= 1024 && aligned16(out) &&
-                    aligned4_elems(d.feat, d.feat_dtype);
+    // on a table and an output aligned to four elements (16 bytes of f32, 8 of bf16)
+    const bool v4 = d.n < ((int64_t)1 << 31) && d.n_slots == 1 && dim == d.feat_dim && (dim & 3) == 0 && dim <= 1024 &&
+                    aligned4_elems(out, out_dtype) && aligned4_elems(d.feat, d.feat_dtype);
     const int rc = with_feat(d, [&](auto t, auto p) {
-      return launch_sage_mean<typename decltype(t)::type, decltype(p)::value>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks, out);
+      return with_dtype(out_dtype, [&](auto o) {
+        using O = typename decltype(o)::type;
+        return launch_sage_mean<typename decltype(t)::type, O, decltype(p)::value>(c, d, ids, rows, reps, nrep, count, dim, mean, v4, blocks,
+                                                                                   (O*)out);
+      });
     });
     if (rc) return rc; }
   if (!dedup) return EU_OK;
   { EuProfScope ps(c, "k_sage_broadcast", rows);
-    const bool vec = (dim & 3) == 0 && aligned16(out);
+    const bool vec = (dim & 3) == 0 && aligned4_elems(out, out_dtype);
     const int G = vec ? group_lanes(dim / 4) : (dim >= 32 ? 32 : 1);
     const unsigned bb = capped_grid(ceil_div(rows * G, 256), "EU_SAGE_CTAS", 0);
-    if (vec) k_sage_broadcast<true><<<bb, 256, 0, s>>>(c->d_agg_src, rows, dim, G, c->d_agg_slot, nrep, c->d_agg_tab, out);
-    else k_sage_broadcast<false><<<bb, 256, 0, s>>>(c->d_agg_src, rows, dim, G, c->d_agg_slot, nrep, c->d_agg_tab, out); }
+    with_dtype(out_dtype, [&](auto o) {
+      using O = typename decltype(o)::type;
+      auto k = vec ? k_sage_broadcast<O, true> : k_sage_broadcast<O, false>;
+      k<<<bb, 256, 0, s>>>(c->d_agg_src, rows, dim, G, c->d_agg_slot, nrep, c->d_agg_tab, (O*)out);
+    }); }
   EU_LAUNCHED();
   return EU_OK;
 }
 
 int eu_sage_mean_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out) {
-  return fanout_aggregate(c, nbr_ids, rows, count, dim, true, out);
+  return fanout_aggregate(c, nbr_ids, rows, count, dim, true, EU_FEAT_F32, out, "eu_sage_mean_aggregate");
+}
+int eu_sage_mean_aggregate_out_dtype(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, int32_t out_dtype,
+                                     void* out) {
+  return fanout_aggregate(c, nbr_ids, rows, count, dim, true, out_dtype, out, "eu_sage_mean_aggregate_out_dtype");
 }
 // the scatter_add variant over the same fixed-fanout blocks (aggr='add': GCN / the per-relation sums of configs[4]):
 // get_dense_feature + scatter_add over edge_src = repeat(range(rows), count), fused
 int eu_sage_add_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out) {
-  return fanout_aggregate(c, nbr_ids, rows, count, dim, false, out);
+  return fanout_aggregate(c, nbr_ids, rows, count, dim, false, EU_FEAT_F32, out, "eu_sage_mean_aggregate");
+}
+int eu_sage_add_aggregate_out_dtype(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, int32_t out_dtype,
+                                    void* out) {
+  return fanout_aggregate(c, nbr_ids, rows, count, dim, false, out_dtype, out, "eu_sage_add_aggregate_out_dtype");
 }
 
 }  // extern "C"

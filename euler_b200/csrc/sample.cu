@@ -992,12 +992,11 @@ int eu_sample_fanout(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* 
   return eu_sample_fanout_batched(c, nodes, 1, B, etypes, K, counts, L, default_node, out_ids, out_w, out_t);
 }
 
-int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K, const int32_t* counts,
-                                  int32_t L, int64_t default_node, int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t,
-                                  int64_t* const* eng_ids, int32_t n_dense, const int32_t* dense_fids, const int32_t* dense_dims,
-                                  float* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids, int64_t* const* sparse_ptr,
-                                  int64_t* sparse_total, int64_t* sparse_max_len) {
-  const char* who = "eu_sample_fanout_with_feature";
+static int fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K, const int32_t* counts,
+                               int32_t L, int64_t default_node, int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t,
+                               int64_t* const* eng_ids, int32_t n_dense, const int32_t* dense_fids, const int32_t* dense_dims,
+                               int32_t dense_dtype, void* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids,
+                               int64_t* const* sparse_ptr, int64_t* sparse_total, int64_t* sparse_max_len, const char* who) {
   if (!c || B < 0 || L < 0 || (L > 0 && (!counts || !out_ids || !out_w || !out_t || !eng_ids)) || (K > 0 && !etypes) || n_dense < 0 ||
       n_sparse < 0 || (n_dense > 0 && (!dense_fids || !dense_dims || !out_dense)) ||
       (n_sparse > 0 && (!sparse_fids || !sparse_ptr || !sparse_total || !sparse_max_len))) {
@@ -1006,6 +1005,7 @@ int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, co
   }
   for (int l = 0; l < L; ++l)
     if (counts[l] < 1) { set_error("%s: counts must be positive", who); return EU_ERR_INVALID; }
+  if (int rc = dtype_check(dense_dtype, who, "output")) return rc;
   EU_CUDA(cudaSetDevice(c->g->device));
   std::vector<int64_t> rows(L + 1, B);
   for (int l = 0; l < L; ++l) rows[l + 1] = rows[l] * counts[l];
@@ -1036,8 +1036,12 @@ int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, co
   if (n_sparse > 0) EU_CUDA(cudaMemsetAsync(m, 0, 16 * (size_t)NS, c->stream));
   for (int l = 0; l <= L; ++l) {
     const int64_t* ids = l == 0 ? nodes : eng_ids[l - 1];
-    for (int j = 0; j < n_dense; ++j)
-      if ((rc = eu_get_dense_feature(c, ids, rows[l], dense_fids[j], dense_dims[j], out_dense[l * n_dense + j]))) return rc;
+    for (int j = 0; j < n_dense; ++j) {
+      void* o = out_dense[l * n_dense + j];
+      rc = dense_dtype == EU_FEAT_F32 ? eu_get_dense_feature(c, ids, rows[l], dense_fids[j], dense_dims[j], (float*)o)
+                                      : eu_get_dense_feature_out_dtype(c, ids, rows[l], dense_fids[j], dense_dims[j], dense_dtype, o);
+      if (rc) return rc;
+    }
     for (int j = 0; j < n_sparse; ++j) {
       const int k = l * n_sparse + j;
       if ((rc = sparse_entry_ptr(c, ids, rows[l], sparse_fids[j], m + o_tmp, tmp, sparse_ptr[k]))) return rc;
@@ -1051,6 +1055,26 @@ int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, co
   EU_CUDA(cudaStreamSynchronize(c->stream));
   for (int k = 0; k < NS; ++k) { sparse_total[k] = st[2 * k]; sparse_max_len[k] = st[2 * k + 1]; }
   return EU_OK;
+}
+
+int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K, const int32_t* counts,
+                                  int32_t L, int64_t default_node, int64_t* const* out_ids, float* const* out_w, int32_t* const* out_t,
+                                  int64_t* const* eng_ids, int32_t n_dense, const int32_t* dense_fids, const int32_t* dense_dims,
+                                  float* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids, int64_t* const* sparse_ptr,
+                                  int64_t* sparse_total, int64_t* sparse_max_len) {
+  return fanout_with_feature(c, nodes, B, etypes, K, counts, L, default_node, out_ids, out_w, out_t, eng_ids, n_dense, dense_fids,
+                             dense_dims, EU_FEAT_F32, (void* const*)out_dense, n_sparse, sparse_fids, sparse_ptr, sparse_total,
+                             sparse_max_len, "eu_sample_fanout_with_feature");
+}
+int eu_sample_fanout_with_feature_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K,
+                                            const int32_t* counts, int32_t L, int64_t default_node, int64_t* const* out_ids,
+                                            float* const* out_w, int32_t* const* out_t, int64_t* const* eng_ids, int32_t n_dense,
+                                            const int32_t* dense_fids, const int32_t* dense_dims, int32_t dense_dtype,
+                                            void* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids,
+                                            int64_t* const* sparse_ptr, int64_t* sparse_total, int64_t* sparse_max_len) {
+  return fanout_with_feature(c, nodes, B, etypes, K, counts, L, default_node, out_ids, out_w, out_t, eng_ids, n_dense, dense_fids,
+                             dense_dims, dense_dtype, out_dense, n_sparse, sparse_fids, sparse_ptr, sparse_total, sparse_max_len,
+                             "eu_sample_fanout_with_feature_out_dtype");
 }
 
 int eu_sample_node(eu_ctx* c, int32_t count, const int32_t* types, int32_t n_types, int64_t* out) {

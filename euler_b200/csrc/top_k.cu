@@ -35,11 +35,12 @@ __device__ __forceinline__ void top_k_insert(float (&t)[KMAX], float v) {
 }
 
 // out[b, 0, :] = the node's row, out[b, 1 + j, d] = the j-th of column d over the count neighbours (j < k <= KMAX).  The
-// slots start at -inf: a slot no value ranks above keeps -inf, which is the value it would have selected (k <= count).
-template <typename T, int KMAX, int C, int P>
+// slots start at -inf: a slot no value ranks above keeps -inf, which is the value it would have selected (k <= count).  The
+// selection is f32; O, the output's element type, only decides how each selected value is stored (a bf16 one rounded once).
+template <typename T, typename O, int KMAX, int C, int P>
 __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const unsigned long long* __restrict__ nodes, int64_t B,
                                                            const unsigned long long* __restrict__ nbrs, int32_t count, int32_t soff,
-                                                           int32_t width, int32_t dim, int32_t k, float* __restrict__ out) {
+                                                           int32_t width, int32_t dim, int32_t k, O* __restrict__ out) {
   const int lane = (int)(threadIdx.x & 31);
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int32_t w = min(width, dim);   // columns read from the graph; the rest are zeros
@@ -47,7 +48,7 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
     const unsigned long long* nb = nbrs + b * count;
     const int64_t self = w > 0 ? lookup_row(g, nodes[b]) : -1;
     const T* fs = self >= 0 ? feat_row<T, P>(g, self) + soff : nullptr;
-    float* o = out + b * (int64_t)(k + 1) * dim;
+    O* o = out + b * (int64_t)(k + 1) * dim;
     for (int32_t d0 = 0; d0 < dim; d0 += 32 * C) {
       float t[C][KMAX];
 #pragma unroll
@@ -74,10 +75,10 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
       for (int c = 0; c < C; ++c) {
         const int32_t d = d0 + 32 * c + lane;
         if (d >= dim) continue;
-        o[d] = (fs && d < w) ? feat_ld(fs + d) : 0.f;
+        o[d] = feat_st<O>((fs && d < w) ? feat_ld(fs + d) : 0.f);
 #pragma unroll
         for (int i = 0; i < KMAX; ++i)
-          if (i < k) o[(int64_t)(1 + i) * dim + d] = t[c][i];
+          if (i < k) o[(int64_t)(1 + i) * dim + d] = feat_st<O>(t[c][i]);
       }
     }
   }
@@ -85,7 +86,7 @@ __global__ void __launch_bounds__(256, 4) k_neighbor_top_k(DevGraph g, const uns
 
 template <int KMAX, int C>
 static int launch_top_k(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_t* neighbors, int32_t count, int32_t soff,
-                        int32_t width, int32_t dim, int32_t k, float* out) {
+                        int32_t width, int32_t dim, int32_t k, int32_t out_dtype, void* out) {
   const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(B, 8), (int64_t)kSMs * 32);
   EuProfScope ps(c, "k_neighbor_top_k", B);
   // a bf16 table widens exactly and order-preservingly (+-0 and NaN included): the selection is the f32 one's on the widened rows
@@ -93,10 +94,38 @@ static int launch_top_k(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_
   const auto* nb = (const unsigned long long*)neighbors;
   const DevGraph& g = c->g->d;
   with_feat(g, [&](auto t, auto p) {
-    k_neighbor_top_k<typename decltype(t)::type, KMAX, C, decltype(p)::value><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff, width, dim, k, out);
+    with_dtype(out_dtype, [&](auto o) {
+      using O = typename decltype(o)::type;
+      k_neighbor_top_k<typename decltype(t)::type, O, KMAX, C, decltype(p)::value><<<blocks, 256, 0, c->stream>>>(g, nd, B, nb, count, soff,
+                                                                                                                width, dim, k, (O*)out);
+    });
   });
   EU_LAUNCHED();
   return EU_OK;
+}
+
+static int neighbor_top_k(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_t* neighbors, int32_t count, int32_t fid, int32_t dim,
+                          int32_t k, int32_t out_dtype, void* out, const char* who) {
+  if (!c || B < 0 || dim < 0 || (B > 0 && (!nodes || !neighbors || (dim > 0 && !out)))) {
+    set_error("%s: bad argument", who);
+    return EU_ERR_INVALID;
+  }
+  if (k < 1 || k > count) {
+    set_error("%s: k = %d must lie in [1, count = %d]", who, k, count);
+    return EU_ERR_INVALID;
+  }
+  if (k > EU_NEIGHBOR_TOP_K_MAX) {
+    set_error("%s: k = %d is above the bound %d", who, k, EU_NEIGHBOR_TOP_K_MAX);
+    return EU_ERR_UNSUPPORTED;
+  }
+  if (int rc = dtype_check(out_dtype, who, "output")) return rc;
+  EU_CUDA(cudaSetDevice(c->g->device));
+  if (B == 0 || dim == 0) return EU_OK;
+  int32_t soff, width;
+  dense_slot(c->g->d, fid, &soff, &width);
+  if (k <= 4) return launch_top_k<4, 4>(c, nodes, B, neighbors, count, soff, width, dim, k, out_dtype, out);
+  if (k <= 8) return launch_top_k<8, 2>(c, nodes, B, neighbors, count, soff, width, dim, k, out_dtype, out);
+  return launch_top_k<EU_NEIGHBOR_TOP_K_MAX, 1>(c, nodes, B, neighbors, count, soff, width, dim, k, out_dtype, out);
 }
 
 }  // namespace eu
@@ -107,25 +136,11 @@ extern "C" {
 
 int eu_neighbor_top_k_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_t* neighbors, int32_t count, int32_t fid,
                               int32_t dim, int32_t k, float* out) {
-  if (!c || B < 0 || dim < 0 || (B > 0 && (!nodes || !neighbors || (dim > 0 && !out)))) {
-    set_error("eu_neighbor_top_k_feature: bad argument");
-    return EU_ERR_INVALID;
-  }
-  if (k < 1 || k > count) {
-    set_error("eu_neighbor_top_k_feature: k = %d must lie in [1, count = %d]", k, count);
-    return EU_ERR_INVALID;
-  }
-  if (k > EU_NEIGHBOR_TOP_K_MAX) {
-    set_error("eu_neighbor_top_k_feature: k = %d is above the bound %d", k, EU_NEIGHBOR_TOP_K_MAX);
-    return EU_ERR_UNSUPPORTED;
-  }
-  EU_CUDA(cudaSetDevice(c->g->device));
-  if (B == 0 || dim == 0) return EU_OK;
-  int32_t soff, width;
-  dense_slot(c->g->d, fid, &soff, &width);
-  if (k <= 4) return launch_top_k<4, 4>(c, nodes, B, neighbors, count, soff, width, dim, k, out);
-  if (k <= 8) return launch_top_k<8, 2>(c, nodes, B, neighbors, count, soff, width, dim, k, out);
-  return launch_top_k<EU_NEIGHBOR_TOP_K_MAX, 1>(c, nodes, B, neighbors, count, soff, width, dim, k, out);
+  return neighbor_top_k(c, nodes, B, neighbors, count, fid, dim, k, EU_FEAT_F32, out, "eu_neighbor_top_k_feature");
+}
+int eu_neighbor_top_k_feature_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_t* neighbors, int32_t count, int32_t fid,
+                                        int32_t dim, int32_t k, int32_t out_dtype, void* out) {
+  return neighbor_top_k(c, nodes, B, neighbors, count, fid, dim, k, out_dtype, out, "eu_neighbor_top_k_feature_out_dtype");
 }
 
 }  // extern "C"

@@ -308,6 +308,15 @@ int eu_sample_fanout_with_feature(eu_ctx* c, const int64_t* nodes, int64_t B, co
                                   int64_t* const* eng_ids, int32_t n_dense, const int32_t* dense_fids, const int32_t* dense_dims,
                                   float* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids, int64_t* const* sparse_ptr,
                                   int64_t* sparse_total, int64_t* sparse_max_len);
+/* eu_sample_fanout_with_feature with every out_dense[k] of dense_dtype (an eu_feat_dtype code; the rule of
+ * eu_get_dense_feature_out_dtype).  The hops, weights, types, engine ids, sparse outputs and the draws the engine consumes are
+ * exactly the f32 call's.  An unknown dense_dtype: EU_ERR_INVALID before any draw or write. */
+int eu_sample_fanout_with_feature_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t B, const int32_t* etypes, int32_t K,
+                                            const int32_t* counts, int32_t L, int64_t default_node, int64_t* const* out_ids,
+                                            float* const* out_w, int32_t* const* out_t, int64_t* const* eng_ids, int32_t n_dense,
+                                            const int32_t* dense_fids, const int32_t* dense_dims, int32_t dense_dtype,
+                                            void* const* out_dense, int32_t n_sparse, const int32_t* sparse_fids,
+                                            int64_t* const* sparse_ptr, int64_t* sparse_total, int64_t* sparse_max_len);
 /* tf_euler.sample_node -- TF op SampleNode (tf_euler/ops/sample_ops.cc:22-37, kernel
  * tf_euler/kernels/sample_node_op.cc:39-96; euler::SampleNode api.cc:32-37).  types i32[n_types]
  * (host); a single -1 means all types.  out i64[count]. */
@@ -339,6 +348,21 @@ int eu_get_dense_feature(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid
                          float* out);
 int eu_get_dense_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim,
                               float* out);
+/* Output dtype of the graph-feature ops.  Each *_out_dtype twin below takes an eu_feat_dtype code `out_dtype` and an output
+ * `void* out` of that element type (f32 or bf16, same shape as the f32 call), and is otherwise its f32 sibling: same
+ * arguments, statuses and synchronisation (the device twins never synchronise the host and are capturable).
+ * Exactness: with out_dtype = EU_FEAT_BF16 the output is, bit for bit, the f32 call's output converted on the device
+ * (torch's .to(torch.bfloat16) of it): every value is computed in f32 exactly as the f32 call computes it (sums and
+ * divisions included) and rounded once, at the store, to nearest even -- NaN becomes the canonical NaN, +-Inf stays, a
+ * finite value becomes +-Inf only where the rounding says so, and subnormals round like any other value.  This holds for
+ * either table dtype, either placement and any cache size.  On a bf16 table, eu_get_dense_feature_out_dtype and the rows of
+ * eu_neighbor_top_k_feature_out_dtype return the stored bits unchanged.  Every output offset is 64-bit: a bf16 output may
+ * pass 2^31 elements.  An unknown out_dtype: EU_ERR_INVALID ("<entry point>: unknown output dtype <code> (EU_FEAT_F32 or
+ * EU_FEAT_BF16)") before anything is enqueued or written.  The _host twins stage out_dtype-sized elements; their buffers may
+ * be pageable or page-locked as for every _host call.  The sharded entry points have no twin. */
+int eu_get_dense_feature_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, int32_t out_dtype, void* out);
+int eu_get_dense_feature_host_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t M, int32_t fid, int32_t dim, int32_t out_dtype,
+                                        void* out);
 /* LGCEncoder's input block (tf_euler/python/utils/encoders.py:895-922, "Large-Scale Learnable Graph Convolutional
  * Networks"), fused from the ids: nodes i64[B], neighbors i64[B, count] (sample_neighbor's rows), out f32[B, k + 1, dim]:
  *   out[b, 0, :]      = eu_get_dense_feature(nodes[b], fid, dim) exactly (zeros past the slot's stored width, clipped before
@@ -355,6 +379,10 @@ int eu_get_dense_feature_host(eu_ctx* c, const int64_t* nodes, int64_t M, int32_
 #define EU_NEIGHBOR_TOP_K_MAX 16
 int eu_neighbor_top_k_feature(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_t* neighbors, int32_t count, int32_t fid,
                               int32_t dim, int32_t k, float* out);
+/* eu_neighbor_top_k_feature into out of out_dtype (see eu_get_dense_feature_out_dtype): the selection is the f32 one, each
+ * selected value rounded at the store.  The k and argument refusals come first, then the dtype's. */
+int eu_neighbor_top_k_feature_out_dtype(eu_ctx* c, const int64_t* nodes, int64_t B, const int64_t* neighbors, int32_t count, int32_t fid,
+                                        int32_t dim, int32_t k, int32_t out_dtype, void* out);
 /* tf_euler.get_sparse_feature, one feature (tf_euler/kernels/get_sparse_feature_op.cc:52-130 over Node::GetUint64Feature
  * node.cc:366-379): the uint64 values of slot `fid` for every node, CSR-style: node i owns out_values[out_ptr[i], out_ptr[i+1]).
  * A node without values (absent node, unknown slot, empty slot) owns exactly ONE entry = default_value (the kernel's
@@ -933,6 +961,15 @@ int eu_sage_mean_aggregate_host(eu_ctx* c, const int64_t* nbr_ids, int64_t rows,
 /* the same block with aggr = 'add' (scatter_add, tf_euler/kernels/scatter_op.cc:44-55): out[r,:] = sum_j x(nbr_ids[r*count+j]),
  * x as above */
 int eu_sage_add_aggregate(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, float* out);
+/* the three above into out of out_dtype (the rule of eu_get_dense_feature_out_dtype): sums and the (count + 1e-7) division in
+ * f32 as the f32 calls do them, each value rounded once at the store; a repeated segment's copies and the zero rows of
+ * segments without a neighbour are the same bits as its own row / +0.0 */
+int eu_sage_mean_aggregate_out_dtype(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, int32_t out_dtype,
+                                     void* out);
+int eu_sage_mean_aggregate_host_out_dtype(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim,
+                                          int32_t out_dtype, void* out);
+int eu_sage_add_aggregate_out_dtype(eu_ctx* c, const int64_t* nbr_ids, int64_t rows, int32_t count, int32_t dim, int32_t out_dtype,
+                                    void* out);
 /* GATConv's attention aggregation (tf_euler/python/convolution/gat_conv.py:53-78, aggr = 'add', after its `fc`), fused.
  * H = heads, C = head_dim; inputs h_src f32[n_src, H*C] (heads concatenated per row), s_dst f32[n_dst, H] and
  * s_src f32[n_src, H] (the per-node scores att_i(x), att_j(x)), dst / src i32[E] (edge_index[0] / [1]).  For head h:
