@@ -20,23 +20,12 @@ device memory one call needs above its inputs per arm (torch's allocator peak pl
 fresh process per arm), the per-kernel times of the fused op (eu_ctx_profile), and the card's name and power limit read in
 the same run.  One JSON line on stdout; nothing is written to the tree."""
 import argparse
-import ctypes as C
-import json
-import os
-import subprocess
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+from harness import block_edges
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from gat_aggregate import block_edges, device_used  # noqa: E402
 
 DIMS = (32, 128)
 BATCHES_128 = (2048, 1024, 512, 256)
@@ -92,12 +81,8 @@ def batch_for(args, D):
 
 def in_child(args, flag, value):
     """this script with `flag value` in a fresh process: its one JSON line"""
-    cmd = [sys.executable, os.path.abspath(__file__), flag, value, "--nodes", str(args.nodes), "--edges", str(args.edges),
-           "--batch", str(args.batch)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise SystemExit("%s %s failed:\n%s" % (flag, value, r.stderr[-2000:]))
-    return json.loads(r.stdout.strip().splitlines()[-1])
+    return harness.in_fresh_process(__file__, [flag, value, "--nodes", str(args.nodes), "--edges", str(args.edges),
+                                               "--batch", str(args.batch)])
 
 
 def dim_inputs(n_dst, n_src, D):
@@ -142,7 +127,7 @@ def make_arms(ops, x, nd, ns, beta, g, dst, src, n_dst, n_src):
 
 
 def memory_of_arm(args, D, batch, arm):
-    """In a process of its own: the device memory one call of `arm` needs above its inputs, as gat_aggregate.memory_of_arm
+    """In a process of its own: the device memory one call of `arm` needs above its inputs, as gat_aggregate.py
     measures it (torch's allocator peak + the device memory allocated outside it, i.e. the library's ctx scratch, on
     Contexts that have done nothing else; kernels and Contexts set up first by every arm on a tiny block)."""
     import gc
@@ -160,16 +145,8 @@ def memory_of_arm(args, D, batch, arm):
     fn = make_arms(ops, x, nd, ns, beta, g, dst, src, n_dst, n_src)[arm]
     torch.cuda.synchronize()
     torch.cuda.empty_cache()
-    alloc0 = torch.cuda.memory_allocated()
-    other0 = device_used() - torch.cuda.memory_reserved()
-    torch.cuda.reset_peak_memory_stats()
-    r = fn()
-    torch.cuda.synchronize()
-    out = {"torch_peak_bytes": int(torch.cuda.max_memory_allocated() - alloc0),
-           "op_scratch_bytes": int(device_used() - torch.cuda.memory_reserved() - other0)}
-    del r
-    out["total_bytes"] = out["torch_peak_bytes"] + out["op_scratch_bytes"]
-    return out
+    peak, scratch = harness.memory_of(fn)
+    return {"torch_peak_bytes": peak, "op_scratch_bytes": scratch, "total_bytes": peak + scratch}
 
 
 def gate(ops, arms, x, nd, ns, beta, g, dst, src, n_dst, D):
@@ -222,46 +199,25 @@ def run(args):
         arms = make_arms(ops, x, nd, ns, beta, g, dst, src, n_dst, n_src)
         worst = gate(ops, arms, x, nd, ns, beta, g, dst, src, n_dst, D)
 
-        for fn in arms.values():
-            for _ in range(args.warmup):
-                fn()
-        torch.cuda.synchronize()
-        rounds = max(1, min(5, args.steps))
-        per = -(-args.steps // rounds)
-        tot = {k: [0.0, 0] for k in arms}
-        for _ in range(rounds):
-            for k, fn in arms.items():
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(per):
-                    fn()
-                e1.record()
-                torch.cuda.synchronize()
-                tot[k][0] += e0.elapsed_time(e1)
-                tot[k][1] += per
-        arm_out = {k: {"ms_per_call": v[0] / v[1], "edges_per_sec": E / (v[0] / v[1] * 1e-3), "calls": v[1],
-                       "memory": memory[D][k]} for k, v in tot.items()}
+        rounds, per = harness.rounds_of(args.steps)
+        ms = harness.time_arms(arms, rounds, args.warmup, per)
+        arm_out = {k: {"ms_per_call": float(np.mean(v)), "edges_per_sec": E / (float(np.mean(v)) * 1e-3), "calls": rounds * per,
+                       "memory": memory[D][k]} for k, v in ms.items()}
         # per-kernel times of the fused op, in a separate pass (the events bracket every kernel).  Autograd runs the backward
         # pass on its own thread, hence on another Context: both entry points are called here directly, on this thread's.
         torch.cuda.synchronize()
         ctx = ops._ctx_on_stream()
-        lib.eu_ctx_profile(ctx._h, 1)
         gx, gnd, gns, gb = (torch.empty_like(t) for t in (x, nd, ns, beta))
-        for _ in range(3):
-            _, alpha, cos = ops._raw_agnn(x, nd, ns, beta, dst, src, n_dst, True)
-            _lib.check(lib.eu_agnn_aggregate_backward(ctx._h, g.data_ptr(), x.data_ptr(), nd.data_ptr(), ns.data_ptr(), beta.data_ptr(),
-                                                      alpha.data_ptr(), cos.data_ptr(), dst.data_ptr(), src.data_ptr(), E, n_dst,
-                                                      n_src, D, gx.data_ptr(), gnd.data_ptr(), gns.data_ptr(), gb.data_ptr()))
-        del alpha, cos, gx, gnd, gns, gb
-        buf = C.create_string_buffer(1 << 16)
-        lib.eu_ctx_profile_read(ctx._h, buf, len(buf))
-        lib.eu_ctx_profile(ctx._h, 0)
-        kern = {}
-        for line in buf.value.decode().splitlines():
-            parts = line.split(",")
-            if len(parts) == 4 and parts[0].startswith("agnn_"):
-                kern[parts[0]] = {"launches": int(parts[2]), "ms_per_launch": float(parts[3]) / max(int(parts[2]), 1)}
+
+        def fused_passes():
+            for _ in range(3):
+                _, alpha, cos = ops._raw_agnn(x, nd, ns, beta, dst, src, n_dst, True)
+                _lib.check(lib.eu_agnn_aggregate_backward(ctx._h, g.data_ptr(), x.data_ptr(), nd.data_ptr(), ns.data_ptr(),
+                                                          beta.data_ptr(), alpha.data_ptr(), cos.data_ptr(), dst.data_ptr(),
+                                                          src.data_ptr(), E, n_dst, n_src, D, gx.data_ptr(), gnd.data_ptr(),
+                                                          gns.data_ptr(), gb.data_ptr()))
+        kern = harness.kernel_times(lib, ctx, "agnn_", fused_passes)
+        del gx, gnd, gns, gb
         results.append({"dim": D, "block": block, "arms": arm_out, "kernels": kern, "setup_s": round(t_setup, 2),
                         "composition_peak_estimate_bytes": choice[D]["composition_peak_estimate_bytes"],
                         "free_bytes_at_choice": choice[D]["free_bytes_at_choice"],
@@ -282,19 +238,17 @@ def run(args):
            "parity_gate": {"passed": True, "what": "per D: fused forward bit-exact vs the composition fed the op's cos on the "
                                                    "stably sorted edge list; fused gradients within 1e-4 (floor 1e-4 x largest; "
                                                    "grad_beta: 1e-4 x sum |du * cos|) of autograd through the composition"},
-           "gpu": gpu_info(0)}
-    emit(out)
+           "gpu": harness.gpu_info(0)}
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     a = parse()
     if a.memory_arm:
         D, batch, arm = a.memory_arm.split(",")
-        emit(memory_of_arm(a, int(D), int(batch), arm))
+        harness.emit(memory_of_arm(a, int(D), int(batch), arm))
     elif a.choose_batch:
-        emit(batch_for(a, a.choose_batch))
+        harness.emit(batch_for(a, a.choose_batch))
     else:
         run(a)

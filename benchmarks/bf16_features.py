@@ -20,22 +20,14 @@ lowest free memory seen during it (sampled every 20 ms), then one batch-8192 [15
 does not fit is reported with what was seen, not retried smaller.
 The card's name, power limit and max SM clock are read in the same run.  One JSON line on stdout; it needs a GPU."""
 import argparse
-import os
-import sys
 import threading
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+import harness
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-import bf16_reference as br  # noqa: E402
-from full_dataflow import emit, gpu_info  # noqa: E402
+import bf16_reference as br
 
 D, FEAT_SEED, GRAPH_SEED = 256, 7, 42
 WORKLOADS = [(1024, [25, 10]), (8192, [15, 10]), (16384, [15, 10])]
@@ -75,24 +67,6 @@ def hop2(graph, batch, fanout, seed):
     return ids[2]
 
 
-def time_arms(arms, rounds, iters):
-    """ms per call of each arm, the arms alternating round by round"""
-    for fn in arms.values():
-        fn()
-    torch.cuda.synchronize()
-    tot = {k: 0.0 for k in arms}
-    for _ in range(rounds):
-        for k, fn in arms.items():
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(iters):
-                fn()
-            e1.record()
-            e1.synchronize()
-            tot[k] += e0.elapsed_time(e1)
-    return {k: v / (rounds * iters) for k, v in tot.items()}
-
-
 def part_a(args):
     import euler_b200
     t0 = time.time()
@@ -130,7 +104,7 @@ def part_a(args):
                 else:
                     arms[name] = (lambda c=ctx, o=o: euler_b200._lib.check(euler_b200._lib.load().eu_sage_mean_aggregate(
                         c._h, ids.data_ptr(), R, count, D, o.data_ptr())), ctx)
-            ms = time_arms({k: v[0] for k, v in arms.items()}, args.rounds, args.iters)
+            ms = {k: float(np.mean(v)) for k, v in harness.time_arms({k: v[0] for k, v in arms.items()}, args.rounds, 1, args.iters).items()}
             for name in graphs:
                 s = 4 if name == "float32" else 2
                 nbytes = M * (s + 4) * D if op == "get_dense_feature" else R * (count * s * D + 4 * D)
@@ -178,19 +152,13 @@ def part_b(args):
     euler_b200.set_graph(g, rng="minstd", seed=5)
     seeds = torch.randint(1, n + 1, (8192,), generator=torch.Generator().manual_seed(5)).cuda()
 
+    last = {}
+
     def step():
-        ids, _, _ = euler_b200.sample_fanout(seeds, [[0], [0]], [15, 10])
-        return ids, euler_b200.sage_mean_aggregate(ids[2], 10, D)
-    step()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(args.rounds):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        ids, agg = step()
-        e1.record()
-        e1.synchronize()
-        times.append(e0.elapsed_time(e1))
+        last["ids"], _, _ = euler_b200.sample_fanout(seeds, [[0], [0]], [15, 10])
+        return euler_b200.sage_mean_aggregate(last["ids"][2], 10, D)
+    times = harness.time_arms({"step": step}, args.rounds, 1)["step"]
+    ids = last["ids"]
     out["fanout_mean_step_ms"] = {"min": round(min(times), 3), "median": round(float(np.median(times)), 3), "steps": len(times)}
     pick = ids[2][torch.randint(0, ids[2].numel(), (4096,), generator=torch.Generator().manual_seed(6)).cuda()]
     got = euler_b200.get_dense_feature(pick, [0], [D])[0].cpu().numpy()
@@ -207,17 +175,14 @@ def main():
     args = parse()
     if not torch.cuda.is_available():
         raise SystemExit("bf16_features.py needs a GPU")
-    res = {"benchmark": "bf16_features", "gpu": gpu_info(torch.cuda.current_device())}
+    res = {"benchmark": "bf16_features", "gpu": harness.gpu_info(torch.cuda.current_device())}
     if "A" in args.part:
         res["A"] = part_a(args)
     if "B" in args.part:
         res["B"] = part_b(args)
-    emit(res)
+    harness.emit(res)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    import full_dataflow
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     main()

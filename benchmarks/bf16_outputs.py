@@ -25,19 +25,12 @@ Reported per table and arm:
 The card's name, power limit and max SM clock are read in the same run.  One JSON line on stdout; it needs a GPU."""
 import argparse
 import ctypes
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
 
 NODES, EDGES, D, BATCH, COUNTS = 10_000_000, 100_000_000, 256, 8192, [15, 10]
 ARMS = ("f32", "f32+cast", "bf16")
@@ -152,26 +145,14 @@ def run_table(eb, dtype, args):
     e2e = {a: [] for a in ARMS}
     for _ in range(args.rounds):
         for arm in ARMS:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(args.iters):
-                graphs[arm].replay()
-            e1.record()
-            e1.synchronize()
-            dev[arm].append(e0.elapsed_time(e1) / args.iters)
-            torch.cuda.synchronize()
+            dev[arm] += harness.time_arms({arm: graphs[arm].replay}, 1, 0, args.iters)[arm]
             t0 = time.perf_counter()
             for _ in range(args.host_iters):
                 host(arm)
             e2e[arm].append((time.perf_counter() - t0) * 1e3 / args.host_iters)
     for arm in ARMS:
-        torch.cuda.synchronize()
-        base = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        outs = device_step(eb, seeds, arm)
-        torch.cuda.synchronize()
-        res[arm].update(device_ms=spread(dev[arm]), e2e_ms=spread(e2e[arm]), peak_alloc_bytes=torch.cuda.max_memory_allocated() - base)
-        del outs
+        res[arm].update(device_ms=spread(dev[arm]), e2e_ms=spread(e2e[arm]),
+                        peak_alloc_bytes=harness.memory_of(lambda: device_step(eb, seeds, arm))[0])
     del graphs
     for key in ("device_ms", "e2e_ms"):
         res["bf16_over_f32_" + key] = round(res["bf16"][key]["median"] / res["f32"][key]["median"], 3)
@@ -187,17 +168,14 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bf16_outputs.py needs a GPU")
     import euler_b200 as eb
-    out = {"benchmark": "bf16_outputs", "gpu": gpu_info(torch.cuda.current_device()),
+    out = {"benchmark": "bf16_outputs", "gpu": harness.gpu_info(torch.cuda.current_device()),
            "workload": "rmat %d nodes / %d edges, D = %d, batch %d, fanout %s" % (NODES, EDGES, D, BATCH, COUNTS),
            "rounds": args.rounds, "iters": args.iters, "host_iters": args.host_iters, "tables": []}
     for dtype in ("float32", "bfloat16"):
         out["tables"].append(run_table(eb, dtype, args))
-    emit(out)
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    import full_dataflow
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     main()

@@ -42,18 +42,8 @@ columns, and the same 2-layer encoder over them.  The store pair's bytes, and th
 shapes and compared with the free device memory after the graph is built: each arm that fits runs on its own, and an arm that
 does not is reported as not fitting from that arithmetic, never by attempting the allocation."""
 import argparse
-import os
-import sys
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-
-
+import harness
 KG_MODELS = {"transe": "TransE", "transr": "TransR", "transd": "TransD", "distmult": "DistMult"}
 
 
@@ -105,8 +95,7 @@ def sage_model(args, dt):
     import torch
     import torch.nn.functional as F
     import euler_b200 as eb
-    from shallow_encoder import DENSE_DIM
-    from sparse_embedding import SLOTS
+    from harness import DENSE_DIM, SLOTS
     from euler_b200.encoders import SageEncoder
     from euler_b200.supervised import SuperviseModel
 
@@ -206,29 +195,15 @@ def scalable_arms(args, n_nodes, feature, dts, steps, warmup, store_ops=True):
     torch.cuda.synchronize()
     for k in losses:
         losses[k].clear()
-    rounds = max(1, min(5, steps))
-    per = -(-steps // rounds)
-    tot = {a: [0.0, 0] for a in arms}
-    for _ in range(rounds):
-        for a, fn in arms.items():
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(per):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            tot[a][0] += e0.elapsed_time(e1)
-            tot[a][1] += per
+    rounds, per = harness.rounds_of(steps)
+    ms = harness.time_arms(arms, rounds, 0, per)
     out = {}
     for k in encs:
-        ms, n = tot[("step", k)]
-        out[k] = {"ms_per_step": ms / n, "steps": n, "store_pair_bytes": sum(t.numel() * t.element_size()
-                                                                             for t in encs[k].stores + encs[k].gradient_stores),
+        out[k] = {"ms_per_step": float(np.mean(ms[("step", k)])), "steps": rounds * per,
+                  "store_pair_bytes": sum(t.numel() * t.element_size() for t in encs[k].stores + encs[k].gradient_stores),
                   "mean_loss": float(np.mean([float(x) for x in losses[k]]))}
         if store_ops:
-            ms, n = tot[("store_ops", k)]
-            out[k]["store_ops_ms"] = ms / n
+            out[k]["store_ops_ms"] = float(np.mean(ms[("store_ops", k)]))
     return out
 
 
@@ -236,12 +211,10 @@ def run_scalable(args):
     import torch
     import euler_b200 as eb
     torch.cuda.set_device(0)
-    import shallow_encoder
-    shallow_encoder.torch = torch
-    from shallow_encoder import DENSE_DIM
-    out = {"workload": "scalable_sage_train_step", "gpu": gpu_info(0), "dim": args.dim, "fanout": SCALABLE_FANOUT, "layers": 2,
+    from harness import DENSE_DIM
+    out = {"workload": "scalable_sage_train_step", "gpu": harness.gpu_info(0), "dim": args.dim, "fanout": SCALABLE_FANOUT, "layers": 2,
            "aggregator": "mean", "batch": args.batch, "optimizer": "sgd", "lr": args.lr}
-    g = shallow_encoder.build_graph(args)
+    g = harness.build_graph(args)
     a = scalable_arms(args, args.nodes, ("feat0", DENSE_DIM), ("bf16", "f32"), args.steps, args.warmup)
     a["bf16_over_f32_time"] = a["bf16"]["ms_per_step"] / a["f32"]["ms_per_step"]
     a["bf16_over_f32_store_ops_time"] = a["bf16"]["store_ops_ms"] / a["f32"]["store_ops_ms"]
@@ -253,7 +226,7 @@ def run_scalable(args):
     torch.cuda.empty_cache()
     if not args.no_part_b:
         out["part_b"] = scalable_part_b(args)
-    emit(out)
+    harness.emit(out)
 
 
 def scalable_part_b(args):
@@ -304,9 +277,7 @@ def run(args):
     if kg:
         eb.set_graph(kg_graph(args.nodes, args.triples, args.relations), rng="philox", seed=1)
     elif sage:
-        import shallow_encoder
-        shallow_encoder.torch = torch
-        shallow_encoder.build_graph(args)
+        harness.build_graph(args)
     else:
         eb.set_graph(eb.Graph.rmat(args.nodes, args.edges, seed=11), rng="philox", seed=1)
     models = {}
@@ -351,23 +322,16 @@ def run(args):
     torch.cuda.synchronize()
     for k in losses:
         losses[k].clear()
-    rounds = max(1, min(5, args.steps))
-    per = -(-args.steps // rounds)
+    rounds, per = harness.rounds_of(args.steps)
     tot = {k: [0.0, 0] for k in models}
     i = args.warmup
     for _ in range(rounds):
         n = min(per, args.warmup + args.steps - i)
         if n <= 0:
             break
-        for k in models:
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for j in range(n):
-                step(k, i + j)
-            e1.record()
-            torch.cuda.synchronize()
-            tot[k][0] += e0.elapsed_time(e1)
+        ms = harness.time_arms({k: (lambda k=k, seq=iter(range(i, i + n)): step(k, next(seq))) for k in models}, 1, 0, n)
+        for k, v in ms.items():
+            tot[k][0] += v[0] * n
             tot[k][1] += n
         i += n
 
@@ -379,23 +343,21 @@ def run(args):
     if kg:
         out = {"workload": "%s_train_step" % args.model, "entities": args.nodes, "triples": args.triples,
                "relations": args.relations, "dim": args.dim, "rel_dim": args.rel_dim if args.model == "transr" else args.dim,
-               "batch": args.batch, "negs": args.negs, "optimizer": args.optimizer, "lr": args.lr, "gpu": gpu_info(0)}
+               "batch": args.batch, "negs": args.negs, "optimizer": args.optimizer, "lr": args.lr, "gpu": harness.gpu_info(0)}
     elif sage:
         out = {"workload": "supervised_sage_minimize_step", "nodes": args.nodes, "edges": args.edges, "dim": args.dim,
                "fanout": [15, 10], "aggregator": "mean", "batch": args.batch, "optimizer": args.optimizer, "lr": args.lr,
-               "gpu": gpu_info(0)}
+               "gpu": harness.gpu_info(0)}
     else:
         out = {"workload": "deepwalk_train_step", "nodes": args.nodes, "edges": args.edges, "dim": args.dim, "batch": args.batch,
-               "optimizer": args.optimizer, "gpu": gpu_info(0)}
+               "optimizer": args.optimizer, "gpu": harness.gpu_info(0)}
     for k, (ms, n) in tot.items():
         out[k] = {"ms_per_step": ms / n, "steps": n, "table_and_slot_bytes": state_bytes(k),
                   "mean_loss": float(np.mean([float(x) for x in losses[k]]))}
     out["bf16_over_f32_time"] = out["bf16"]["ms_per_step"] / out["f32"]["ms_per_step"]
-    emit(out)
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

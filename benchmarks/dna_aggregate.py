@@ -21,23 +21,12 @@ edges/s and the device memory one call needs above its inputs per arm (torch's a
 scratch, measured in a fresh process per arm), the per-kernel times of the fused op (eu_ctx_profile), and the card's name,
 power limit and SM clock read in the same run.  One JSON line on stdout; nothing is written to the tree."""
 import argparse
-import ctypes as C
-import json
-import os
-import subprocess
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+from harness import block_edges
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from gat_aggregate import block_edges, device_used  # noqa: E402
 
 CONFIGS = ((32, 1), (128, 1), (128, 4))
 GROUPS = 8
@@ -105,12 +94,8 @@ def batch_for(args, dim, H):
 
 def in_child(args, flag, value):
     """this script with `flag value` in a fresh process: its one JSON line"""
-    cmd = [sys.executable, os.path.abspath(__file__), flag, value, "--nodes", str(args.nodes), "--edges", str(args.edges),
-           "--batch", str(args.batch)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise SystemExit("%s %s failed:\n%s" % (flag, value, r.stderr[-2000:]))
-    return json.loads(r.stdout.strip().splitlines()[-1])
+    return harness.in_fresh_process(__file__, [flag, value, "--nodes", str(args.nodes), "--edges", str(args.edges),
+                                               "--batch", str(args.batch)])
 
 
 def inputs(n_dst, n_src, dim, H):
@@ -168,16 +153,8 @@ def memory_of_arm(args, dim, H, batch, arm):
     fn = make_arms(ops, conv, xt, xs, lins, g, dst, src, n_dst, n_src, H)[arm]
     torch.cuda.synchronize()
     torch.cuda.empty_cache()
-    alloc0 = torch.cuda.memory_allocated()
-    other0 = device_used() - torch.cuda.memory_reserved()
-    torch.cuda.reset_peak_memory_stats()
-    r = fn()
-    torch.cuda.synchronize()
-    out = {"torch_peak_bytes": int(torch.cuda.max_memory_allocated() - alloc0),
-           "op_scratch_bytes": int(device_used() - torch.cuda.memory_reserved() - other0)}
-    del r
-    out["total_bytes"] = out["torch_peak_bytes"] + out["op_scratch_bytes"]
-    return out
+    peak, scratch = harness.memory_of(fn)
+    return {"torch_peak_bytes": peak, "op_scratch_bytes": scratch, "total_bytes": peak + scratch}
 
 
 def gate(arms, dim, H):
@@ -203,29 +180,6 @@ def gate(arms, dim, H):
     return worst
 
 
-def time_arms(arms, steps, warmup):
-    import torch
-    for fn in arms.values():
-        for _ in range(warmup):
-            fn()
-    torch.cuda.synchronize()
-    rounds = max(1, min(5, steps))
-    per = -(-steps // rounds)
-    tot = {k: [0.0, 0] for k in arms}
-    for _ in range(rounds):
-        for k, fn in arms.items():
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(per):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            tot[k][0] += e0.elapsed_time(e1)
-            tot[k][1] += per
-    return {k: (v[0] / v[1], v[1]) for k, v in tot.items()}
-
-
 def kernel_times(lib, ops, xt, xs, lins, g, dst, src, n_dst, n_src, H):
     """per-kernel times of the fused op on this thread's Context (autograd's backward runs on another thread: both entry
     points are called here directly)"""
@@ -237,24 +191,17 @@ def kernel_times(lib, ops, xt, xs, lins, g, dst, src, n_dst, n_src, H):
     n0, n1 = (t.reshape(-1).contiguous() for t in conv.gcn_norm(torch.stack([dst, src]), (n_dst, n_src)))
     torch.cuda.synchronize()
     ctx = ops._ctx_on_stream()
-    lib.eu_ctx_profile(ctx._h, 1)
     gq, gk, gv = (torch.empty_like(t) for t in (q, k, v))
     E, dim = dst.numel(), q.shape[1]
-    for _ in range(3):
-        _, alpha = ops._raw_dna(q, k, v, n0, n1, dst, src, n_dst, H, True)
-        _lib.check(lib.eu_dna_aggregate_backward(ctx._h, g.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), n0.data_ptr(),
-                                                 n1.data_ptr(), alpha.data_ptr(), dst.data_ptr(), src.data_ptr(), E, n_dst, n_src,
-                                                 H, dim // H, gq.data_ptr(), gk.data_ptr(), gv.data_ptr()))
-    torch.cuda.synchronize()
-    buf = C.create_string_buffer(1 << 16)
-    lib.eu_ctx_profile_read(ctx._h, buf, len(buf))
-    lib.eu_ctx_profile(ctx._h, 0)
-    kern = {}
-    for line in buf.value.decode().splitlines():
-        parts = line.split(",")
-        if len(parts) == 4 and parts[0].startswith("dna_"):
-            kern[parts[0]] = {"launches": int(parts[2]), "ms_per_launch": float(parts[3]) / max(int(parts[2]), 1)}
-    return kern
+
+    def fused_passes():
+        for _ in range(3):
+            _, alpha = ops._raw_dna(q, k, v, n0, n1, dst, src, n_dst, H, True)
+            _lib.check(lib.eu_dna_aggregate_backward(ctx._h, g.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), n0.data_ptr(),
+                                                     n1.data_ptr(), alpha.data_ptr(), dst.data_ptr(), src.data_ptr(), E, n_dst,
+                                                     n_src, H, dim // H, gq.data_ptr(), gk.data_ptr(), gv.data_ptr()))
+        torch.cuda.synchronize()
+    return harness.kernel_times(lib, ctx, "dna_", fused_passes)
 
 
 def block_info(dst, n_dst, n_src, indeg, batch):
@@ -295,10 +242,11 @@ def run(args):
                 res["gate_worst_grad_diff_over_floor"] = gate(arms, dim, H)
             else:
                 arms = {k: fn for k, fn in arms.items() if k.startswith("fused")}
-            times = time_arms(arms, args.steps, args.warmup)
-            arm_out = {k: {"ms_per_call": ms, "edges_per_sec": E / (ms * 1e-3), "calls": n,
+            rounds, per = harness.rounds_of(args.steps)
+            times = {k: float(np.mean(v)) for k, v in harness.time_arms(arms, rounds, args.warmup, per).items()}
+            arm_out = {k: {"ms_per_call": ms, "edges_per_sec": E / (ms * 1e-3), "calls": rounds * per,
                            "memory": memory[(dim, H)].get(k) if batch == (b or args.batch) else None}
-                       for k, (ms, n) in times.items()}
+                       for k, ms in times.items()}
             entry = {"block": block_info(dst, n_dst, n_src, indeg, batch), "arms": arm_out, "setup_s": round(t_setup, 2)}
             if with_comp:
                 entry["speedup_fwd"] = arm_out["composition_fwd"]["ms_per_call"] / arm_out["fused_fwd"]["ms_per_call"]
@@ -322,20 +270,18 @@ def run(args):
            "parity_gate": {"passed": True, "what": "per configuration at the comparison batch: fused forward within 1e-4 (floor "
                                                    "1e-4 x largest) of the composition; fused gradients within 1e-3 (floor 1e-3 "
                                                    "x largest) of autograd through the composition"},
-           "gpu": gpu_info(0)}
-    emit(out)
+           "gpu": harness.gpu_info(0)}
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     a = parse()
     if a.memory_arm:
         d, h, batch, arm = a.memory_arm.split(",")
-        emit(memory_of_arm(a, int(d), int(h), int(batch), arm))
+        harness.emit(memory_of_arm(a, int(d), int(h), int(batch), arm))
     elif a.choose_batch:
         d, h = a.choose_batch.split(",")
-        emit(batch_for(a, int(d), int(h)))
+        harness.emit(batch_for(a, int(d), int(h)))
     else:
         run(a)

@@ -13,18 +13,13 @@ restatement of gcn_dataflow.py / neighbor_dataflow.py, and the composition with 
 metric = block entries/s: edge_index columns of all hops (listed edges + self loops) per second.  One JSON line on stdout;
 nothing is written to the tree."""
 import argparse
-import json
 import os
-import subprocess
-import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from bench import FEAT_SEED, GRAPH_SEED, Clocks  # noqa: E402
+from bench import FEAT_SEED, GRAPH_SEED, Clocks
 
 FULL_METAPATH = [[0], [0]]
 
@@ -69,17 +64,6 @@ def np_unique_first(x):
     rank = np.empty_like(order)
     rank[order] = np.arange(len(order))
     return vals[order], rank[inv]
-
-
-def gpu_info(index):
-    """card name, power limit and max SM clock, read in the measuring run"""
-    try:
-        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-        name, power, mhz = [x.strip() for x in out.split(",")]
-        return {"name": name, "power_limit": power, "sm_max_clock": mhz}
-    except Exception as e:                      # noqa: BLE001
-        return {"unavailable": str(e)}
 
 
 def run_full(args):
@@ -136,17 +120,12 @@ def run_full(args):
 
     def timed(fn, first, n):
         """n steps on seed sets first.. ; returns (ms, entries, per-hop sizes)"""
-        torch.cuda.synchronize()
-        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        ev0.record()
-        entries, hops = 0, []
-        for i in range(first, first + n):
-            blocks = fn(dev_seeds[i % n_sb])
-            hops.append([(int(ei.shape[1]), int(nid.numel())) for nid, _, ei in blocks])
-            entries += sum(h[0] for h in hops[-1])
-        ev1.record()
-        torch.cuda.synchronize()
-        return ev0.elapsed_time(ev1), entries, hops
+        hops, seq = [], iter(range(first, first + n))
+
+        def step():
+            hops.append([(int(ei.shape[1]), int(nid.numel())) for nid, _, ei in fn(dev_seeds[next(seq) % n_sb])])
+        ms = harness.time_arms({"step": step}, 1, 0, n)["step"][0] * n
+        return ms, sum(h[0] for hop in hops for h in hop), hops
 
     arms = {"fused": fused_step, "composition": composed_step}
     for fn in arms.values():
@@ -154,8 +133,7 @@ def run_full(args):
         # rounds (a growth synchronises and reallocates), then the warm-up steps
         timed(fn, 0, n_sb)
         timed(fn, 0, max(args.warmup, 1))
-    rounds = max(1, min(5, args.steps))
-    per = -(-args.steps // rounds)
+    rounds, per = harness.rounds_of(args.steps)
     tot = {k: [0.0, 0, 0] for k in arms}
     per_round, hop_sizes = [], []
     clocks = Clocks(local)
@@ -190,20 +168,10 @@ def run_full(args):
                            "ms_per_step": tot["composition"][0] / tot["composition"][2],
                            "what": "get_full_neighbor + torch repeat_interleave / cat + unique, once per hop"},
            "speedup_vs_composition": rate["fused"] / rate["composition"], "rounds": per_round, "hops": hops,
-           "parity_gate": gate, "clocks": clk, "gpu": gpu_info(local), "graph_build_s": round(t_graph, 2)}
-    emit(out)
-
-
-_REAL_STDOUT = None
-
-
-def emit(out):
-    """the ONE JSON line goes to the process's real stdout; everything else any library printed went to stderr"""
-    os.write(_REAL_STDOUT if _REAL_STDOUT is not None else 1, (json.dumps(out) + "\n").encode())
+           "parity_gate": gate, "clocks": clk, "gpu": harness.gpu_info(local), "graph_build_s": round(t_graph, 2)}
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    _REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run_full(parse())

@@ -14,21 +14,12 @@ fused=False step's on the same draws; a mismatch aborts.  tests/test_gae_gpu.py 
 Reported per arm: ms per call and torch's allocator peak above the inputs; the card's name, power limit and max SM clock read
 in the same run.  One JSON line on stdout.  It needs a GPU: without one it fails rather than measure anything else."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+from harness import timed
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-import shallow_encoder  # noqa: E402
-from shallow_encoder import timed  # noqa: E402
 
 FEAT, DIMS, FANOUTS, NEGS, BATCH = 128, (32, 128), [10, 10], 10, 1024
 MODELS, ENCODERS = ("gae", "vgae"), ("sage", "gcn")
@@ -119,7 +110,6 @@ def run(args):
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("benchmarks/gae_step.py needs a GPU; nothing is measured without one")
-    shallow_encoder.torch = torch
     import euler_b200 as eb
     torch.cuda.set_device(0)
     t0 = time.time()
@@ -144,13 +134,11 @@ def run(args):
                         (lambda m=m, opt=opt: step(eb, m, opt, seeds))
                 step_res.update(timed(pair, args.steps, args.warmup))   # the two arms alternate round by round
                 del pair, m, opt
-    emit({"metric": "gae_step_sage_d32_fused_ms", "value": step_res["step_gae_sage_d32_fused"]["ms_per_call"], "gate": "passed",
-          "gpu": gpu_info(0), "batch": BATCH, "fanouts": FANOUTS, "dims": list(DIMS), "num_negs": NEGS, "setup_s": setup_s,
-          "steps": step_res, "loss_alone": loss_res})
+    harness.emit({"metric": "gae_step_sage_d32_fused_ms", "value": step_res["step_gae_sage_d32_fused"]["ms_per_call"], "gate": "passed",
+                  "gpu": harness.gpu_info(0), "batch": BATCH, "fanouts": FANOUTS, "dims": list(DIMS), "num_negs": NEGS, "setup_s": setup_s,
+                  "steps": step_res, "loss_alone": loss_res})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

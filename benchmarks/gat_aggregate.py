@@ -17,23 +17,12 @@ in a fresh process per arm), the per-kernel times of the fused op (eu_ctx_profil
 forward arms on the same block without its largest target (what that one target costs), and the card's name and power
 limit read in the same run.  One JSON line on stdout; nothing is written to the tree."""
 import argparse
-import ctypes as C
-import json
-import os
-import subprocess
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from bench import GRAPH_SEED  # noqa: E402
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
+from harness import block_edges
 
 SHAPES = [(1, 32), (8, 8)]
 
@@ -58,21 +47,6 @@ def composition(ops, F, h, sd, ss, dst, src, n_dst):
 
 
 ARMS = ("fused_fwd", "composition_fwd", "fused_fwd_bwd", "composition_fwd_bwd")
-
-
-def block_edges(args, self_loops=False):
-    """the benchmark block: (dst, src) int32 on the device, its sizes and each target's edge count"""
-    import torch
-    import euler_b200 as eb
-    from euler_b200.dataflow import GCNDataFlow
-    graph = eb.Graph.rmat(args.nodes, args.edges, seed=GRAPH_SEED, device=0)
-    eb.set_graph(graph)
-    seeds = torch.from_numpy(np.random.RandomState(7000).randint(1, args.nodes + 1, size=args.batch).astype(np.int64)).cuda()
-    blk = GCNDataFlow([[0], [0]], add_self_loops=self_loops)(seeds)[0]
-    ei = blk.edge_index.to(torch.int32)
-    n_dst, n_src = blk.size
-    dst, src = ei[0].contiguous(), ei[1].contiguous()
-    return dst, src, n_dst, n_src, torch.bincount(dst.long(), minlength=n_dst)
 
 
 def shape_inputs(n_dst, n_src, H, Cd):
@@ -110,12 +84,6 @@ def make_arms(ops, F, h, sd, ss, g, dst, src, n_dst, n_src):
     return dict(zip(ARMS, (fused_fwd, comp_fwd, fused_fb, comp_fb)))
 
 
-def device_used():
-    import torch
-    free, total = torch.cuda.mem_get_info()
-    return total - free
-
-
 def memory_of_arm(args, hc, arm):
     """In a process of its own: the device memory one call of `arm` needs above its inputs.  torch_peak = the torch caching
     allocator's peak (torch.cuda.max_memory_allocated); op_scratch = device memory allocated outside torch's allocator, which is
@@ -140,26 +108,14 @@ def memory_of_arm(args, hc, arm):
     fn = make_arms(ops, F, h, sd, ss, g, dst, src, n_dst, n_src)[arm]
     torch.cuda.synchronize()
     torch.cuda.empty_cache()
-    alloc0 = torch.cuda.memory_allocated()
-    other0 = device_used() - torch.cuda.memory_reserved()
-    torch.cuda.reset_peak_memory_stats()
-    r = fn()
-    torch.cuda.synchronize()
-    out = {"torch_peak_bytes": int(torch.cuda.max_memory_allocated() - alloc0),
-           "op_scratch_bytes": int(device_used() - torch.cuda.memory_reserved() - other0)}
-    del r
-    out["total_bytes"] = out["torch_peak_bytes"] + out["op_scratch_bytes"]
-    return out
+    peak, scratch = harness.memory_of(fn)
+    return {"torch_peak_bytes": peak, "op_scratch_bytes": scratch, "total_bytes": peak + scratch}
 
 
 def measure_memory(args, hc, arm):
     """memory_of_arm in a fresh process (scratch only grows, so each arm needs its own)"""
-    cmd = [sys.executable, os.path.abspath(__file__), "--memory-arm", "%d,%d,%s" % (hc[0], hc[1], arm), "--nodes", str(args.nodes),
-           "--edges", str(args.edges), "--batch", str(args.batch)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise SystemExit("memory measurement of %s at %s failed:\n%s" % (arm, hc, r.stderr[-2000:]))
-    return json.loads(r.stdout.strip().splitlines()[-1])
+    return harness.in_fresh_process(__file__, ["--memory-arm", "%d,%d,%s" % (hc[0], hc[1], arm), "--nodes", str(args.nodes),
+                                               "--edges", str(args.edges), "--batch", str(args.batch)])
 
 
 def run(args):
@@ -195,46 +151,24 @@ def run(args):
                                  "max abs diff %g" % (nm, H, Cd, float((x - y).abs().max())))
         del fg, cg
 
-        for fn in arms.values():
-            for _ in range(args.warmup):
-                fn()
-        torch.cuda.synchronize()
-        rounds = max(1, min(5, args.steps))
-        per = -(-args.steps // rounds)
-        tot = {k: [0.0, 0] for k in arms}
-        for _ in range(rounds):
-            for k, fn in arms.items():
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(per):
-                    fn()
-                e1.record()
-                torch.cuda.synchronize()
-                tot[k][0] += e0.elapsed_time(e1)
-                tot[k][1] += per
-        arm_out = {k: {"ms_per_call": v[0] / v[1], "edges_per_sec": E / (v[0] / v[1] * 1e-3), "calls": v[1],
-                       "memory": memory["%d,%d" % (H, Cd)][k]} for k, v in tot.items()}
+        rounds, per = harness.rounds_of(args.steps)
+        ms = harness.time_arms(arms, rounds, args.warmup, per)
+        arm_out = {k: {"ms_per_call": float(np.mean(v)), "edges_per_sec": E / (float(np.mean(v)) * 1e-3), "calls": rounds * per,
+                       "memory": memory["%d,%d" % (H, Cd)][k]} for k, v in ms.items()}
         # per-kernel times of the fused op, in a separate pass (the events bracket every kernel).  Autograd runs the backward
         # pass on its own thread, hence on another Context: both entry points are called here directly, on this thread's.
         torch.cuda.synchronize()
         ctx = ops._ctx_on_stream()
-        lib.eu_ctx_profile(ctx._h, 1)
         gh, gsd, gss = torch.empty_like(h), torch.empty_like(sd), torch.empty_like(ss)
-        for _ in range(3):
-            _, alpha = ops._raw_gat(h, sd, ss, dst, src, n_dst, True)
-            _lib.check(lib.eu_gat_aggregate_backward(ctx._h, g.data_ptr(), h.data_ptr(), alpha.data_ptr(), sd.data_ptr(), ss.data_ptr(),
-                                                     dst.data_ptr(), src.data_ptr(), E, n_dst, n_src, H, Cd, gh.data_ptr(),
-                                                     gsd.data_ptr(), gss.data_ptr()))
-        del alpha, gh, gsd, gss
-        buf = C.create_string_buffer(1 << 16)
-        lib.eu_ctx_profile_read(ctx._h, buf, len(buf))
-        lib.eu_ctx_profile(ctx._h, 0)
-        kern = {}
-        for line in buf.value.decode().splitlines():
-            parts = line.split(",")
-            if len(parts) == 4 and parts[0].startswith("gat_"):
-                kern[parts[0]] = {"launches": int(parts[2]), "ms_per_launch": float(parts[3]) / max(int(parts[2]), 1)}
+
+        def fused_passes():
+            for _ in range(3):
+                _, alpha = ops._raw_gat(h, sd, ss, dst, src, n_dst, True)
+                _lib.check(lib.eu_gat_aggregate_backward(ctx._h, g.data_ptr(), h.data_ptr(), alpha.data_ptr(), sd.data_ptr(),
+                                                         ss.data_ptr(), dst.data_ptr(), src.data_ptr(), E, n_dst, n_src, H, Cd,
+                                                         gh.data_ptr(), gsd.data_ptr(), gss.data_ptr()))
+        kern = harness.kernel_times(lib, ctx, "gat_", fused_passes)
+        del gh, gsd, gss
         # what the largest target costs: it stays on one lane group (its sums run in edge order), so it sets the kernel's
         # critical path; the same block without that target's edges, forward only
         keep = dst != int(indeg.argmax())
@@ -244,16 +178,8 @@ def run(args):
         for k, fn in (("fused_fwd", lambda: ops.gat_attention_aggregate(h, sd, ss, kei, (n_dst, n_src))),
                       ("composition_fwd", lambda: composition(ops, F, h, sd, ss, kd, ks, n_dst))):
             with torch.no_grad():
-                for _ in range(args.warmup):
-                    fn()
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(args.steps):
-                    fn()
-                e1.record()
-                torch.cuda.synchronize()
-            no_hub[k] = {"ms_per_call": e0.elapsed_time(e1) / args.steps, "edges": kd.numel()}
+                ms = harness.time_arms({k: fn}, 1, args.warmup, args.steps)[k][0]
+            no_hub[k] = {"ms_per_call": ms, "edges": kd.numel()}
         del kd, ks, kei, keep
         results.append({"heads": H, "head_dim": Cd, "arms": arm_out, "kernels": kern, "without_largest_target": no_hub,
                         "speedup_fwd": arm_out["composition_fwd"]["ms_per_call"] / arm_out["fused_fwd"]["ms_per_call"],
@@ -270,17 +196,15 @@ def run(args):
            "block": block, "shapes": results,
            "parity_gate": {"passed": True, "what": "per (H, C): fused forward bit-exact vs the composition; fused gradients within "
                                                    "1e-4 (floor 1e-4 x largest) of autograd through the composition"},
-           "gpu": gpu_info(0), "setup_s": round(t_setup, 2)}
-    emit(out)
+           "gpu": harness.gpu_info(0), "setup_s": round(t_setup, 2)}
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     a = parse()
     if a.memory_arm:
         H, Cd, arm = a.memory_arm.split(",")
-        emit(memory_of_arm(a, (int(H), int(Cd)), arm))
+        harness.emit(memory_of_arm(a, (int(H), int(Cd)), arm))
     else:
         run(a)

@@ -20,21 +20,12 @@ Reported per arm: ms per call and torch's allocator peak above the inputs; the [
 shapes; the card's name, power limit and max SM clock read in the same run.  One JSON line on stdout.  It needs a GPU:
 without one it fails rather than measure anything else."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+from harness import DENSE_DIM, build_graph, timed
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from shallow_encoder import DENSE_DIM, build_graph, timed  # noqa: E402
-import shallow_encoder  # noqa: E402
 
 METAPATH = [[0], [0]]
 GATE_SEEDS = 256
@@ -97,7 +88,6 @@ def run(args):
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("benchmarks/gcn_encoder.py needs a GPU; nothing is measured without one")
-    shallow_encoder.torch = torch
     import euler_b200 as eb
     torch.cuda.set_device(0)
     t0 = time.time()
@@ -137,14 +127,12 @@ def run(args):
     for (a, f), enc in encs.items():
         arms["encoder_%s_%s_fwd_bwd" % (a, "fused" if f else "composed")] = (lambda e: lambda: encoder_step(e, seeds))(enc)
     res = timed(arms, args.steps, args.warmup)
-    emit({"metric": "gcn_encoder_adjacency_mean_fwd_ms", "value": res["adj_fused_fwd"]["ms_per_call"], "gate": "passed",
-          "gpu": gpu_info(0), "batch": args.batch, "dim": args.dim, "setup_s": setup_s, "arms": res,
-          "shapes": {"hop1_rows": n, "hop2_nodes": m, "hop1_entries": nnz, "message_bytes": nnz * args.dim * 4,
+    harness.emit({"metric": "gcn_encoder_adjacency_mean_fwd_ms", "value": res["adj_fused_fwd"]["ms_per_call"], "gate": "passed",
+                  "gpu": harness.gpu_info(0), "batch": args.batch, "dim": args.dim, "setup_s": setup_s, "arms": res,
+                  "shapes": {"hop1_rows": n, "hop2_nodes": m, "hop1_entries": nnz, "message_bytes": nnz * args.dim * 4,
                      "seed_entries": int(adjs[0][1].numel()), "gate_seeds": GATE_SEEDS}})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

@@ -15,20 +15,12 @@ mismatch aborts.  Then:
   (d) 'attention' (4 heads): the gate on 1024 ids and infer() once, timed.
 The card's name, power limit and max SM clock are read in the same run.  One JSON line on stdout.  It needs a GPU."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+from harness import DENSE_DIM, build_graph
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from shallow_encoder import DENSE_DIM, build_graph  # noqa: E402
 
 METAPATH = [[0], [0]]
 
@@ -67,34 +59,20 @@ def gate(enc, args, ids, what):
 
 
 def event_ms(fn, reps):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def outside_torch():
-    """device bytes in use that torch's allocator does not hold (the library's graph and ctx scratch)"""
-    free, total = torch.cuda.mem_get_info()
-    return total - free - torch.cuda.memory_reserved()
+    return harness.time_arms({"call": fn}, 1, 0, reps)["call"][0]
 
 
 def measure_infer(enc, args):
-    torch.cuda.synchronize()
-    a0, o0 = torch.cuda.memory_allocated(), outside_torch()
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.time()
-    out = enc.infer(chunk_rows=args.chunk_rows)
-    torch.cuda.synchronize()
-    first_s = time.time() - t0
-    res = {"first_call_s": first_s, "torch_peak_bytes": int(torch.cuda.max_memory_allocated() - a0),
-           "scratch_growth_bytes": int(outside_torch() - o0), "rows": int(out.shape[0])}
-    del out
-    return res
+    first = {}
+
+    def call():
+        t0 = time.time()
+        out = enc.infer(chunk_rows=args.chunk_rows)
+        torch.cuda.synchronize()
+        first.update(first_call_s=time.time() - t0, rows=int(out.shape[0]))
+        return out
+    peak, scratch = harness.memory_of(call)
+    return {"first_call_s": first["first_call_s"], "torch_peak_bytes": peak, "scratch_growth_bytes": scratch, "rows": first["rows"]}
 
 
 def run(args):
@@ -137,13 +115,11 @@ def run(args):
     att = make_encoder(args, "attention")
     gates["attention"] = gate(att, args, gate_ids[:1024], "attention")
     res["infer_attention"] = measure_infer(att, args)
-    emit({"metric": "gcn_infer_all_nodes_ms", "value": res["infer_gcn"]["ms_per_call"], "gate": "passed", "gate_err": gates,
-          "gpu": gpu_info(0), "nodes": args.nodes, "edges": args.edges, "dim": args.dim, "batch": args.batch,
-          "chunk_rows": args.chunk_rows, "setup_s": setup_s, "arms": res})
+    harness.emit({"metric": "gcn_infer_all_nodes_ms", "value": res["infer_gcn"]["ms_per_call"], "gate": "passed", "gate_err": gates,
+                  "gpu": harness.gpu_info(0), "nodes": args.nodes, "edges": args.edges, "dim": args.dim, "batch": args.batch,
+                  "chunk_rows": args.chunk_rows, "setup_s": setup_s, "arms": res})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

@@ -17,18 +17,12 @@ torch allocator's peak above the inputs per arm (the library's own ctx scratch i
 ms per call, and the card's name and power limit read in the same run.  One JSON line on stdout; nothing is written to the
 tree."""
 import argparse
-import os
 import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
 
 DIMS = (64, 128)
 
@@ -85,17 +79,9 @@ def main(args):
     n_labels = len(ops.graph_labels())
     build_s = time.time() - t0
     B = args.batch
-    ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
 
     def timed(fn, n):
-        torch.cuda.synchronize()
-        a, b = ev(), ev()
-        a.record()
-        for _ in range(n):
-            fn()
-        b.record()
-        torch.cuda.synchronize()
-        return a.elapsed_time(b) / n
+        return harness.time_arms({"call": fn}, 1, 0, n)["call"][0]
 
     # ---- batch construction alone
     labels = ops.sample_graph_label(B)
@@ -159,23 +145,15 @@ def main(args):
         for n, fn in runs.items():
             for _ in range(args.warmup):
                 fn()
-            torch.cuda.synchronize()
-            base = torch.cuda.memory_allocated()
-            torch.cuda.reset_peak_memory_stats()
-            fn()
-            torch.cuda.synchronize()
-            mem[n] = (torch.cuda.max_memory_allocated() - base) / 2 ** 20
-        times = {n: [] for n in names}
-        for _ in range(3):                                   # alternate the arms in rounds
-            for n, fn in runs.items():
-                times[n].append(timed(fn, args.steps))
+            mem[n] = harness.memory_of(fn)[0] / 2 ** 20
+        times = harness.time_arms(runs, 3, 0, args.steps)      # alternate the arms in rounds
         for (m, fu, bw) in names:
             key = "D%d_%s_%s_%s" % (D, "attention_pool" if m == "logits" else "set2set_step", "fused" if fu else "composition",
                                     "fwd_bwd" if bw else "fwd")
             results[key] = {"ms_median": float(np.median(times[(m, fu, bw)])), "ms_all": times[(m, fu, bw)],
                             "peak_alloc_MiB": mem[(m, fu, bw)]}
-    emit({"bench": "graph_readout", "gpu": gpu_info(0), "graphs": args.graphs, "nodes": int(len(ids)), "labels": n_labels,
-          "batch": B, "batch_rows": nnz, "graph_build_s": build_s, "gate": gate, "construct": construct, "readout": results})
+    harness.emit({"bench": "graph_readout", "gpu": harness.gpu_info(0), "graphs": args.graphs, "nodes": int(len(ids)), "labels": n_labels,
+                  "batch": B, "batch_rows": nnz, "graph_build_s": build_s, "gate": gate, "construct": construct, "readout": results})
     print("%-48s %10s %12s" % ("arm", "ms", "peak MiB"), file=sys.stderr)
     for k, v in results.items():
         print("%-48s %10.3f %12.1f" % (k, v["ms_median"], v["peak_alloc_MiB"]), file=sys.stderr)
@@ -184,4 +162,5 @@ def main(args):
 
 
 if __name__ == "__main__":
+    harness.divert_stdout()
     main(parse())

@@ -17,20 +17,13 @@ table on the host (102.4 GB pinned) and a 10 % cache: one batch-8192 [15, 10] fa
 rows checked against the oracle's R-MAT feature rows (oracle/pyoracle.py).
 The card's name, power limit and max SM clock are read in the same run.  One JSON line on stdout; it needs a GPU."""
 import argparse
-import os
 import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+import harness
+import numpy as np
+import torch
 
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
 
 D, FEAT_SEED, GRAPH_SEED = 256, 7, 42
 CACHE_FRACTIONS = (0.0, 0.01, 0.10, 0.25)
@@ -80,23 +73,6 @@ def reads(slots, n, seeds, hop1, hop2):
     return int(ids.size), int((slots[ids - 1] >= 0).sum())
 
 
-def time_pair(fns, rounds, iters):
-    for fn in fns.values():
-        fn()
-    torch.cuda.synchronize()
-    tot = {k: 0.0 for k in fns}
-    for _ in range(rounds):
-        for k, fn in fns.items():
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(iters):
-                fn()
-            e1.record()
-            e1.synchronize()
-            tot[k] += e0.elapsed_time(e1)
-    return {k: v / (rounds * iters) for k, v in tot.items()}
-
-
 def part_a(args):
     import euler_b200
     n, E = args.nodes, 10 * args.nodes
@@ -124,8 +100,9 @@ def part_a(args):
                 if not torch.equal(bits(a), bits(b)):
                     raise SystemExit("CHECK FAILED: host-placed %s C=%d differs from the device arm" % (dt, C))
             rows, hits = reads(gh.feat_cache_slots(), n, seeds, hop1, hop2)
-            ms = time_pair({"device": lambda: step(gd, seeds, hop1, hop2), "host": lambda: step(gh, seeds, hop1, hop2)},
-                           args.rounds, args.iters)
+            ms = harness.time_arms({"device": lambda: step(gd, seeds, hop1, hop2), "host": lambda: step(gh, seeds, hop1, hop2)},
+                                   args.rounds, 1, args.iters)
+            ms = {k: float(np.mean(v)) for k, v in ms.items()}
             out["arms"].append({"dtype": dt, "cache_rows": C, "cache_fraction": frac, "check": "bit-exact",
                                 "device_ms": round(ms["device"], 3), "host_ms": round(ms["host"], 3),
                                 "host_over_device": round(ms["host"] / ms["device"], 2),
@@ -156,14 +133,7 @@ def part_b():
     res = {"graph": "rmat 100M / 1B, D = 256, f32 on the host, 10 % cache", "build_s": round(time.time() - t0, 1),
            "hbm_bytes": g.hbm_bytes, "host_bytes": g.host_bytes, "free_device_bytes": torch.cuda.mem_get_info()[0]}
     seeds, hop1, hop2 = sample(g)
-    step(g, seeds, hop1, hop2)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    step(g, seeds, hop1, hop2)
-    e1.record()
-    e1.synchronize()
-    res["step_feature_ms"] = round(e0.elapsed_time(e1), 3)
+    res["step_feature_ms"] = round(harness.time_arms({"step": lambda: step(g, seeds, hop1, hop2)}, 1, 1)["step"][0], 3)
     pick = hop2[torch.randperm(hop2.numel(), generator=torch.Generator().manual_seed(1))[:4096].cuda()]
     got = euler_b200.get_dense_feature(pick, [0], [D])[0].cpu().numpy()
     want = po.rmat_feat_rows(pick.cpu().numpy(), n, D, FEAT_SEED)
@@ -175,11 +145,12 @@ def part_b():
 
 def main(argv=None):
     args = parse(argv)
-    out = {"benchmark": "host_features", "gpu": gpu_info(0), "part_a": part_a(args)}
+    out = {"benchmark": "host_features", "gpu": harness.gpu_info(0), "part_a": part_a(args)}
     if args.full:
         out["part_b"] = part_b()
-    emit(out)
+    harness.emit(out)
 
 
 if __name__ == "__main__":
+    harness.divert_stdout()
     main()

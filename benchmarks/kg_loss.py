@@ -21,18 +21,10 @@ ctx scratch is reported beside: the growth of the device's used memory outside t
 fit is reported "not run" with its largest tiled tensor estimated from the shapes.  The card's name and power limit are read
 in the same run.  One JSON line on stdout."""
 import argparse
-import json
-import os
-import sys
 
+import harness
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-
-from full_dataflow import gpu_info  # noqa: E402
 
 MODELS = ('transe', 'transh', 'transr', 'transd', 'distmult')
 SEED = 20201
@@ -126,39 +118,20 @@ def gate(ids, n_ent, n_rel):
     return out
 
 
-def time_arms(arms, steps, warmup):
+def measure(arms, steps, warmup):
     """arms: name -> thunk.  Alternate the arms round by round; median ms per call and the allocator peak above the inputs."""
     import torch
-    res = {name: {"ms": [], "peak_mb": None} for name in arms}
+    res = {}
     for name, fn in arms.items():
         try:
-            torch.cuda.synchronize()
-            free0 = torch.cuda.mem_get_info()[0]
-            base = torch.cuda.memory_allocated()
-            reserved0 = torch.cuda.memory_reserved()
-            torch.cuda.reset_peak_memory_stats()
-            fn()
-            torch.cuda.synchronize()
-            res[name]["peak_mb"] = round((torch.cuda.max_memory_allocated() - base) / 2**20, 1)
-            outside = (free0 - torch.cuda.mem_get_info()[0]) - (torch.cuda.memory_reserved() - reserved0)
-            res[name]["ctx_scratch_mb"] = round(max(0, outside) / 2**20, 1)
+            peak, outside = harness.memory_of(fn)
+            res[name] = {"peak_mb": round(peak / 2**20, 1), "ctx_scratch_mb": round(max(0, outside) / 2**20, 1)}
         except torch.OutOfMemoryError:
             res[name] = {"not_run": "out of memory"}
             torch.cuda.empty_cache()
-    live = [n for n in arms if "not_run" not in res[n]]
-    for _ in range(warmup):
-        for n in live:
-            arms[n]()
-    for _ in range(steps):
-        for n in live:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            arms[n]()
-            e1.record()
-            torch.cuda.synchronize()
-            res[n]["ms"].append(e0.elapsed_time(e1))
-    for n in live:
-        res[n]["ms_median"] = round(float(np.median(res[n].pop("ms"))), 3)
+    live = {n: fn for n, fn in arms.items() if "not_run" not in res[n]}
+    for n, ms in harness.time_arms(live, steps, warmup).items():
+        res[n]["ms_median"] = round(float(np.median(ms)), 3)
     return res
 
 
@@ -166,7 +139,7 @@ def main(argv=None):
     import torch
     args = parse(argv)
     only = set(args.only.split(","))
-    out = {"gpu": gpu_info(torch.cuda.current_device())}
+    out = {"gpu": harness.gpu_info(torch.cuda.current_device())}
     g, n_ent, n_rel = fb15k_graph()
     torch.manual_seed(SEED)
     w1 = graph_ids(1200, 1)
@@ -177,7 +150,7 @@ def main(argv=None):
             tabs = make_tables(model, n_ent, n_rel, 50, 50)
             arms = {"%s_%s" % (kind, arm): (lambda kind=kind, arm=arm: call(kind, model, tabs, w1, arm, 0.5, "mrr"))
                     for arm in ("fwd", "fwd_bwd") for kind in ("fused", "composed")}
-            r[model] = time_arms(arms, args.steps, args.warmup)
+            r[model] = measure(arms, args.steps, args.warmup)
             del tabs
             torch.cuda.empty_cache()
         out["W1"] = r
@@ -197,7 +170,7 @@ def main(argv=None):
                 est = B * K * 128 * 128 * 4 / 2**30
                 arms = {k: v for k, v in arms.items() if k.startswith("fused")}
                 r["transr_composed"] = "not run: the tiled [B, K, ent_dim * rel_dim] matrix alone is %.1f GB" % est
-            r[model] = time_arms(arms, args.steps, args.warmup)
+            r[model] = measure(arms, args.steps, args.warmup)
             del tabs
             torch.cuda.empty_cache()
         out["W2"] = r
@@ -212,12 +185,13 @@ def main(argv=None):
                 est = 128 * 14951 * 100 * 100 * 4 / 2**30
                 arms = {k: v for k, v in arms.items() if k.startswith("fused")}
                 r["transr_composed"] = "not run: the tiled [B, K, ent_dim * rel_dim] matrix alone is %.1f GB" % est
-            r[model] = time_arms(arms, args.steps, args.warmup)
+            r[model] = measure(arms, args.steps, args.warmup)
             del tabs
             torch.cuda.empty_cache()
         out["W3"] = r
-    print(json.dumps(out))
+    harness.emit(out)
 
 
 if __name__ == "__main__":
+    harness.divert_stdout()
     main()

@@ -14,18 +14,13 @@ blocks, and compares the adjacency of sample_neighbor_layerwise_coo bit-exactly 
 builder (tf_euler/kernels/sparse_get_adj_op.cc:84-117) over the oracle's listing on the exported CSR; a mismatch aborts.
 metric = edge_index columns of all hops per second.  One JSON line on stdout; nothing is written to the tree."""
 import argparse
-import json
 import os
-import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from bench import GRAPH_SEED, Clocks  # noqa: E402
-from full_dataflow import gpu_info  # noqa: E402
+from bench import GRAPH_SEED, Clocks
 
 METAPATH = [[0], [0]]
 WORKLOADS = [{"name": "example", "batch": 512, "fanouts": [400, 400]},
@@ -125,20 +120,14 @@ def run(args):
             """n steps on seed sets first.. with the engine seeded by engine_seed: both arms draw the same neighbors and build
             the same blocks.  Returns (ms, edge_index columns, per-hop sizes)"""
             eb.seed(engine_seed)
-            torch.cuda.synchronize()
-            ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            ev0.record()
-            cols, hops = 0, []
-            for i in range(first, first + n):
-                blocks = step(flow, dev_seeds[i % n_sb])
-                hops.append([(int(ei.shape[1]), int(nid.numel())) for nid, _, ei in blocks])
-                cols += sum(h[0] for h in hops[-1])
-            ev1.record()
-            torch.cuda.synchronize()
-            return ev0.elapsed_time(ev1), cols, hops
+            hops, seq = [], iter(range(first, first + n))
 
-        rounds = max(1, min(5, args.steps))
-        per = -(-args.steps // rounds)
+            def call():
+                hops.append([(int(ei.shape[1]), int(nid.numel())) for nid, _, ei in step(flow, dev_seeds[next(seq) % n_sb])])
+            ms = harness.time_arms({"step": call}, 1, 0, n)["step"][0] * n
+            return ms, sum(h[0] for hop in hops for h in hop), hops
+
+        rounds, per = harness.rounds_of(args.steps)
         for flow in arms.values():
             timed(flow, 0, max(args.warmup, 1), 0)
             for r in range(rounds):       # the timed steps once: scratch and the caching allocator reach their size
@@ -205,21 +194,11 @@ def run(args):
                                   "LayerwiseDataFlow metapath %s with self loops, 1 GPU; value = the %s workload"
                                   % (args.nodes // 10**6, args.edges // 10**6, METAPATH, head["workload"]),
                       "nodes": args.nodes, "edges": args.edges},
-           "workloads": results, "parity_gate": gates or {"passed": None, "skipped": "--no-gate"}, "gpu": gpu_info(local),
+           "workloads": results, "parity_gate": gates or {"passed": None, "skipped": "--no-gate"}, "gpu": harness.gpu_info(local),
            "graph_build_s": round(t_graph, 2)}
-    emit(out)
-
-
-_REAL_STDOUT = None
-
-
-def emit(out):
-    """the ONE JSON line goes to the process's real stdout; everything else any library printed went to stderr"""
-    os.write(_REAL_STDOUT if _REAL_STDOUT is not None else 1, (json.dumps(out) + "\n").encode())
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    _REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

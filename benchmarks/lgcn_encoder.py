@@ -18,22 +18,13 @@ rows at the wide width; a mismatch aborts.  The arms of a graph alternate in rou
 per call and torch's allocator peak above the inputs; the card's name, power limit and SM clock read in the same run.  One
 JSON line on stdout."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from bench import GRAPH_SEED  # noqa: E402
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-import shallow_encoder  # noqa: E402
-from shallow_encoder import DENSE_DIM, build_graph, timed  # noqa: E402
+from bench import GRAPH_SEED
+from harness import DENSE_DIM, build_graph, timed
 
 LABEL_DIM, HIDDEN, OUT = 16, 128, 64
 
@@ -101,7 +92,6 @@ def run(args):
     global torch
     import torch
     import euler_b200 as eb
-    shallow_encoder.torch = torch          # its timing loop reads the module's torch
     torch.cuda.set_device(0)
     t0 = time.time()
     _g = build_graph(args)
@@ -114,13 +104,11 @@ def run(args):
     args.nodes_now = args.wide_nodes
     wide_res = measure(eb, args, 0, args.wide_dim, 2048)
     wide_res["graph"] = {"nodes": args.wide_nodes, "edges": args.wide_edges}
-    emit({"metric": "lgcn_top_k_op_ms", "value": head["arms"]["op_fused"]["ms_per_call"], "gate": "passed", "gpu": gpu_info(0),
-          "batch": args.batch, "nb_num": args.nb_num, "k": args.k, "setup_s": setup_s,
-          "graph": {"nodes": args.nodes, "edges": args.edges}, "headline": head, "wide": wide_res})
+    harness.emit({"metric": "lgcn_top_k_op_ms", "value": head["arms"]["op_fused"]["ms_per_call"], "gate": "passed", "gpu": harness.gpu_info(0),
+                  "batch": args.batch, "nb_num": args.nb_num, "k": args.k, "setup_s": setup_s,
+                  "graph": {"nodes": args.nodes, "edges": args.edges}, "headline": head, "wide": wide_res})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

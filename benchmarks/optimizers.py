@@ -16,18 +16,9 @@ pass from its algorithmic bytes 24 N D + 4 R (D + 2) (var, m and v read and writ
 read once) and that rate over the H100 SXM's 3.35 TB/s; the card's name, power limit and max SM clock read in the same run.
 One JSON line on stdout.  It needs a GPU: without one it fails rather than measure anything else."""
 import argparse
-import os
-import sys
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-import shallow_encoder  # noqa: E402
-from shallow_encoder import timed  # noqa: E402
+import harness
+from harness import timed
 
 TABLES = [(10_000_000, 128), (20_000_000, 64)]
 HBM_BYTES_PER_S = 3.35e12
@@ -99,7 +90,7 @@ def run(args):
         raise SystemExit("benchmarks/optimizers.py needs a GPU")
     eb.set_graph(eb.Graph.rmat(1000, 5000, seed=1), rng="minstd", seed=1)
     gen = torch.Generator(device="cuda").manual_seed(0)
-    out = {"metric": "ms_per_step", "gpu": gpu_info(0), "steps": args.steps, "warmup": args.warmup, "sparse": [], "dense": {}}
+    out = {"metric": "ms_per_step", "gpu": harness.gpu_info(0), "steps": args.steps, "warmup": args.warmup, "sparse": [], "dense": {}}
     for N, D in TABLES:
         rows = deepwalk_rows(N, gen)
         R = rows.numel()
@@ -125,13 +116,10 @@ def run(args):
     dgrads = [torch.randn(p.shape, generator=gen, device="cuda") for p in dense]
     out["dense"] = {"params": len(dense), "elements": int(sum(p.numel() for p in dense)),
                     "adam": compare('adam', lambda: [torch.nn.Parameter(p.clone()) for p in dense], dgrads, args)}
-    emit(out)
+    harness.emit(out)
 
 
 if __name__ == "__main__":
     import torch
-    shallow_encoder.torch = torch
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

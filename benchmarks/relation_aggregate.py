@@ -24,24 +24,12 @@ reported per block: E, P (the distinct (target, relation) pairs), targets, the l
 scratch, measured in a fresh process per arm), and the card's name and power limit read in the same run.  One JSON line on
 stdout; nothing is written to the tree."""
 import argparse
-import ctypes as C
-import json
-import os
-import subprocess
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from bench import C5_ETYPES, C5_NTYPES, C5_SEED  # noqa: E402
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from gat_aggregate import device_used  # noqa: E402
+from bench import C5_ETYPES, C5_NTYPES, C5_SEED
 
 SHAPES = [(16, 32), (128, 128)]
 MODES = {"e_id": C5_ETYPES, "wn18": 18}
@@ -178,7 +166,7 @@ def gate(arms, x, W, g, dst, src, rel, n_dst, R, with_comp, what):
 
 
 def memory_of_arm(args, mode, F, D, batch, arm):
-    """In a process of its own: the device memory one call of `arm` needs above its inputs, as gat_aggregate.memory_of_arm
+    """In a process of its own: the device memory one call of `arm` needs above its inputs, as gat_aggregate.py
     measures it (torch's allocator peak + the device memory allocated outside it, i.e. the library's ctx scratch, on Contexts
     that have done nothing else; the kernels and Contexts are set up first by every arm on a tiny block)."""
     import gc
@@ -195,48 +183,13 @@ def memory_of_arm(args, mode, F, D, batch, arm):
     fn = make_arms(x, W, g, dst, src, rel, n_dst, n_src)[arm]
     torch.cuda.synchronize()
     torch.cuda.empty_cache()
-    alloc0 = torch.cuda.memory_allocated()
-    other0 = device_used() - torch.cuda.memory_reserved()
-    torch.cuda.reset_peak_memory_stats()
-    r = fn()
-    torch.cuda.synchronize()
-    out = {"torch_peak_bytes": int(torch.cuda.max_memory_allocated() - alloc0),
-           "op_scratch_bytes": int(device_used() - torch.cuda.memory_reserved() - other0)}
-    del r
-    out["total_bytes"] = out["torch_peak_bytes"] + out["op_scratch_bytes"]
-    return out
+    peak, scratch = harness.memory_of(fn)
+    return {"torch_peak_bytes": peak, "op_scratch_bytes": scratch, "total_bytes": peak + scratch}
 
 
 def measure_memory(args, mode, F, D, batch, arm):
-    cmd = [sys.executable, os.path.abspath(__file__), "--memory-arm", "%s,%d,%d,%d,%s" % (mode, F, D, batch, arm),
-           "--nodes", str(args.nodes), "--edges", str(args.edges)]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise SystemExit("memory measurement of %s at %s %s failed:\n%s" % (arm, mode, (F, D), r.stderr[-2000:]))
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
-def time_arms(arms, names, steps, warmup):
-    import torch
-    for k in names:
-        for _ in range(warmup):
-            arms[k]()
-    torch.cuda.synchronize()
-    rounds = max(1, min(5, steps))
-    per = -(-steps // rounds)
-    tot = {k: [0.0, 0] for k in names}
-    for _ in range(rounds):
-        for k in names:
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(per):
-                arms[k]()
-            e1.record()
-            torch.cuda.synchronize()
-            tot[k][0] += e0.elapsed_time(e1)
-            tot[k][1] += per
-    return {k: v[0] / v[1] for k, v in tot.items()}
+    return harness.in_fresh_process(__file__, ["--memory-arm", "%s,%d,%d,%d,%s" % (mode, F, D, batch, arm),
+                                               "--nodes", str(args.nodes), "--edges", str(args.edges)])
 
 
 def kernel_times(x, W, g, dst, src, rel, n_dst, n_src, R):
@@ -247,22 +200,16 @@ def kernel_times(x, W, g, dst, src, rel, n_dst, n_src, R):
     lib = _lib.load()
     torch.cuda.synchronize()
     ctx = ops._ctx_on_stream()
-    lib.eu_ctx_profile(ctx._h, 1)
     gx, gW = torch.empty_like(x), torch.empty_like(W)
     F, D = x.shape[1], W.shape[1]
-    for _ in range(3):
-        ops._raw_relation(x, W, rel, dst, src, n_dst)
-        _lib.check(lib.eu_relation_aggregate_backward(ctx._h, g.data_ptr(), x.data_ptr(), W.data_ptr(), rel.data_ptr(), dst.data_ptr(),
-                                                      src.data_ptr(), dst.numel(), n_dst, n_src, R, D, F, gx.data_ptr(), gW.data_ptr()))
-    buf = C.create_string_buffer(1 << 16)
-    lib.eu_ctx_profile_read(ctx._h, buf, len(buf))
-    lib.eu_ctx_profile(ctx._h, 0)
-    kern = {}
-    for line in buf.value.decode().splitlines():
-        parts = line.split(",")
-        if len(parts) == 4 and parts[0].startswith("rel_"):
-            kern[parts[0]] = {"launches": int(parts[2]), "ms_per_launch": float(parts[3]) / max(int(parts[2]), 1)}
-    return kern
+
+    def fused_passes():
+        for _ in range(3):
+            ops._raw_relation(x, W, rel, dst, src, n_dst)
+            _lib.check(lib.eu_relation_aggregate_backward(ctx._h, g.data_ptr(), x.data_ptr(), W.data_ptr(), rel.data_ptr(),
+                                                          dst.data_ptr(), src.data_ptr(), dst.numel(), n_dst, n_src, R, D, F,
+                                                          gx.data_ptr(), gW.data_ptr()))
+    return harness.kernel_times(lib, ctx, "rel_", fused_passes)
 
 
 def run_block(args, mode, F, D, batch, with_comp, memory):
@@ -281,7 +228,8 @@ def run_block(args, mode, F, D, batch, with_comp, memory):
     what = "%s (F, D) = (%d, %d) batch %d" % (mode, F, D, batch)
     info["gate"] = gate(arms, x, W, g, dst, src, rel, n_dst, R, with_comp, what)
     names = list(ARMS) if with_comp else ["fused_fwd", "fused_fwd_bwd"]
-    ms = time_arms(arms, names, args.steps, args.warmup)
+    rounds, per = harness.rounds_of(args.steps)
+    ms = {k: float(np.mean(v)) for k, v in harness.time_arms({k: arms[k] for k in names}, rounds, args.warmup, per).items()}
     info["arms"] = {k: {"ms_per_call": ms[k], "edges_per_sec": E / (ms[k] * 1e-3),
                         "memory": memory.get((mode, F, D, batch, k))} for k in names}
     info["kernels"] = kernel_times(x, W, g, dst, src, rel, n_dst, n_src, R)
@@ -351,17 +299,15 @@ def run(args):
            "parity_gate": {"passed": True, "what": "per block timed: fused forward within 1e-5 (floor 1e-5 x largest) of float64, "
                                                    "within 1e-4 of relation_aggregate where it runs; fused gradients within 1e-4 "
                                                    "of float64"},
-           "gpu": gpu_info(0), "plan_s": round(t_plan, 2)}
-    emit(out)
+           "gpu": harness.gpu_info(0), "plan_s": round(t_plan, 2)}
+    harness.emit(out)
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     a = parse()
     if a.memory_arm:
         mode, F, D, batch, arm = a.memory_arm.split(",")
-        emit(memory_of_arm(a, mode, int(F), int(D), int(batch), arm))
+        harness.emit(memory_of_arm(a, mode, int(F), int(D), int(batch), arm))
     else:
         run(a)

@@ -3,31 +3,17 @@
   C3  node2vec biased walk p=0.5 q=2.0 walk_len=80 batch=4096 on RMAT 10M/100M   (+ p=q=1 deepwalk path)
   C4  50M nodes / 500M edges, D=256 on ONE 80 GB GPU: 2-hop [15,10] batch=8192 (the 1-GPU point of configs[3])
   C5  heterogeneous 3 node types / 5 edge types, 50M nodes: per-edge-type sample_neighbor + scatter_add, D=64
-Usage: python benchmarks/run_configs.py [c3] [c4] [c5] [--small]"""
-import json
-import os
-import sys
+Usage: python benchmarks/run_configs.py [c3] [c4] [c5] [--small]
+One JSON line per config on stdout, each with the card's name, power limit and max SM clock read in the same run."""
+import argparse
 import time
 
+import harness
 import numpy as np
-import torch
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import euler_b200 as eb  # noqa: E402
 
 
 def timeit(fn, iters, warm=2):
-    for _ in range(warm):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
+    return harness.time_arms({"call": fn}, 1, warm, iters)["call"][0]
 
 
 def c3(small):
@@ -47,7 +33,7 @@ def c3(small):
         ms1 = timeit(lambda: eb.random_walk(seeds, et, 1.0, 1.0), 5, warm=1)
         out["deepwalk_%s_ms" % rng] = ms1
         out["deepwalk_%s_walker_steps_per_s" % rng] = 4096 * 80 / (ms1 * 1e-3)
-    print(json.dumps(out))
+    harness.emit(dict(out, gpu=harness.gpu_info(0)))
     g.close()
 
 
@@ -75,10 +61,10 @@ def c4(small):
     ids, a0, a1 = step()
     edges = B * 15 + B * 150
     ok = bool(((ids[2] >= -1) & (ids[2] <= n)).all().item()) and bool(torch.isfinite(a1).all().item())
-    print(json.dumps({"config": "C4 on one GPU", "nodes": n, "edges": E, "feat_dim": D, "hbm_graph_gb": g.hbm_bytes / 1e9,
-                      "graph_build_s": build_s, "batch": B, "fanout": counts, "ms_per_step_single_lane": ms,
-                      "sampled_edges_per_s_single_lane": edges / (ms * 1e-3), "outputs_in_range": ok,
-                      "valid_fraction_hop2": float((ids[2] != -1).float().mean().item())}))
+    harness.emit({"config": "C4 on one GPU", "nodes": n, "edges": E, "feat_dim": D, "hbm_graph_gb": g.hbm_bytes / 1e9,
+                  "graph_build_s": build_s, "batch": B, "fanout": counts, "ms_per_step_single_lane": ms,
+                  "sampled_edges_per_s_single_lane": edges / (ms * 1e-3), "outputs_in_range": ok,
+                  "valid_fraction_hop2": float((ids[2] != -1).float().mean().item()), "gpu": harness.gpu_info(0)})
     g.close()
 
 
@@ -100,15 +86,20 @@ def c5(small):
     ms = timeit(step, 20, warm=3)
     outs = step()
     types = eb.sample_neighbor(seeds, list(range(T)), count)[2]
-    print(json.dumps({"config": "C5 hetero on one GPU", "nodes": n, "edges": E, "edge_types": T, "node_types": NT, "feat_dim": D,
-                      "batch": B, "count": count, "ms_per_step": ms, "sampled_edges_per_s": B * count * T / (ms * 1e-3),
-                      "agg_finite": bool(all(torch.isfinite(o).all().item() for o in outs)),
-                      "types_seen_all_mode": sorted(set(types.unique().tolist()))}))
+    harness.emit({"config": "C5 hetero on one GPU", "nodes": n, "edges": E, "edge_types": T, "node_types": NT, "feat_dim": D,
+                  "batch": B, "count": count, "ms_per_step": ms, "sampled_edges_per_s": B * count * T / (ms * 1e-3),
+                  "agg_finite": bool(all(torch.isfinite(o).all().item() for o in outs)),
+                  "types_seen_all_mode": sorted(set(types.unique().tolist())), "gpu": harness.gpu_info(0)})
     g.close()
 
 
 if __name__ == "__main__":
-    small = "--small" in sys.argv
-    which = [a for a in sys.argv[1:] if not a.startswith("--")] or ["c3", "c4", "c5"]
-    for w in which:
-        {"c3": c3, "c4": c4, "c5": c5}[w](small)
+    p = argparse.ArgumentParser()
+    p.add_argument("configs", nargs="*", choices=["c3", "c4", "c5"], help="default: all three")
+    p.add_argument("--small", action="store_true")
+    args = p.parse_args()
+    harness.divert_stdout()
+    import torch
+    import euler_b200 as eb
+    for w in args.configs or ["c3", "c4", "c5"]:
+        {"c3": c3, "c4": c4, "c5": c5}[w](args.small)

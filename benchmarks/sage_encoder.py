@@ -18,22 +18,11 @@ memory in use outside torch's allocator) over the run; the bytes the [M, W] matr
 card's name, power limit and max SM clock read in the same run.  One JSON line on stdout.  It needs a GPU: without one it
 fails rather than measure anything else."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from shallow_encoder import DENSE_DIM, DIM, build_graph, timed  # noqa: E402
-import shallow_encoder  # noqa: E402
-from sparse_embedding import SLOTS  # noqa: E402
+import harness
+import numpy as np
+from harness import DENSE_DIM, DIM, SLOTS, build_graph, timed
 
 
 def parse(argv=None):
@@ -95,17 +84,11 @@ def gate(eb, args, fanout, seeds):
             raise SystemExit("GATE FAILED: parameter %d's gradient is %.3g of its largest entry from the composition's" % (t, err))
 
 
-def outside_torch():
-    free, total = torch.cuda.mem_get_info()
-    return total - free - torch.cuda.memory_reserved()
-
-
 def run(args):
     global torch
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("benchmarks/sage_encoder.py needs a GPU; nothing is measured without one")
-    shallow_encoder.torch = torch
     import euler_b200 as eb
     torch.cuda.set_device(0)
     sh = shapes(args)
@@ -122,37 +105,38 @@ def run(args):
     dense = [("feat0", DENSE_DIM)]
     torch.cuda.synchronize()
     setup_s = time.time() - t0
-    scratch0 = outside_torch()
-    gate(eb, args, fanout, seeds)
+    res = {}
 
-    def pooled(sg=False):
-        return eb.shallow_encode_pool(deep, fanout[-1], id_table, dense, sparse, "mean", sparse_grad=sg)
+    def gated_run():
+        gate(eb, args, fanout, seeds)
 
-    def composed(sg=False):
-        return eb.shallow_encode(deep, id_table, dense, sparse, "concat", sparse_grad=sg).view(-1, fanout[-1], sh["row_width"]).mean(1)
+        def pooled(sg=False):
+            return eb.shallow_encode_pool(deep, fanout[-1], id_table, dense, sparse, "mean", sparse_grad=sg)
 
-    def fwd_bwd(fn, sg):
-        out = fn(sg)
-        torch.autograd.grad(out, params, torch.ones_like(out))
+        def composed(sg=False):
+            return eb.shallow_encode(deep, id_table, dense, sparse, "concat", sparse_grad=sg).view(-1, fanout[-1], sh["row_width"]).mean(1)
 
-    encs = {(f, s): make_encoder(eb, args, fanout, f, s) for f in (True, False) for s in (False, True)}
-    arms = {
-        "hop_pooled_fwd": pooled, "hop_composed_fwd": composed,
-        "hop_pooled_fwd_bwd_dense": lambda: fwd_bwd(pooled, False), "hop_composed_fwd_bwd_dense": lambda: fwd_bwd(composed, False),
-        "hop_pooled_fwd_bwd_sparse": lambda: fwd_bwd(pooled, True), "hop_composed_fwd_bwd_sparse": lambda: fwd_bwd(composed, True),
-        "encoder_fused_fwd_bwd_dense": lambda: encoder_step(eb, encs[True, False], seeds),
-        "encoder_composed_fwd_bwd_dense": lambda: encoder_step(eb, encs[False, False], seeds),
-        "encoder_fused_fwd_bwd_sparse": lambda: encoder_step(eb, encs[True, True], seeds),
-        "encoder_composed_fwd_bwd_sparse": lambda: encoder_step(eb, encs[False, True], seeds),
-    }
-    res = timed(arms, args.steps, args.warmup)
-    emit({"metric": "sage_encoder_deepest_hop_fwd_ms", "value": res["hop_pooled_fwd"]["ms_per_call"], "gate": "passed",
-          "gpu": gpu_info(0), "batch": args.batch, "dim": args.dim, "shapes": sh, "setup_s": setup_s, "arms": res,
-          "ctx_scratch_growth_bytes": int(max(0, outside_torch() - scratch0))})
+        def fwd_bwd(fn, sg):
+            out = fn(sg)
+            torch.autograd.grad(out, params, torch.ones_like(out))
+
+        encs = {(f, s): make_encoder(eb, args, fanout, f, s) for f in (True, False) for s in (False, True)}
+        arms = {
+            "hop_pooled_fwd": pooled, "hop_composed_fwd": composed,
+            "hop_pooled_fwd_bwd_dense": lambda: fwd_bwd(pooled, False), "hop_composed_fwd_bwd_dense": lambda: fwd_bwd(composed, False),
+            "hop_pooled_fwd_bwd_sparse": lambda: fwd_bwd(pooled, True), "hop_composed_fwd_bwd_sparse": lambda: fwd_bwd(composed, True),
+            "encoder_fused_fwd_bwd_dense": lambda: encoder_step(eb, encs[True, False], seeds),
+            "encoder_composed_fwd_bwd_dense": lambda: encoder_step(eb, encs[False, False], seeds),
+            "encoder_fused_fwd_bwd_sparse": lambda: encoder_step(eb, encs[True, True], seeds),
+            "encoder_composed_fwd_bwd_sparse": lambda: encoder_step(eb, encs[False, True], seeds),
+        }
+        res.update(timed(arms, args.steps, args.warmup))
+    scratch_growth = harness.memory_of(gated_run)[1]      # the library's ctx scratch over the gate and every arm
+    harness.emit({"metric": "sage_encoder_deepest_hop_fwd_ms", "value": res["hop_pooled_fwd"]["ms_per_call"], "gate": "passed",
+                  "gpu": harness.gpu_info(0), "batch": args.batch, "dim": args.dim, "shapes": sh, "setup_s": setup_s, "arms": res,
+                  "ctx_scratch_growth_bytes": max(0, scratch_growth)})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

@@ -20,21 +20,12 @@ Reported per arm: ms per call, torch's allocator peak above the inputs, and the 
 card's name, power limit and max SM clock read in the same run.  One JSON line on stdout.  It needs a GPU: without one it
 fails rather than measure anything else."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+from harness import DENSE_DIM, build_graph, timed
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from shallow_encoder import DENSE_DIM, build_graph, timed  # noqa: E402
-import shallow_encoder  # noqa: E402
 
 LABELS = 16
 
@@ -83,7 +74,6 @@ def run(args):
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("benchmarks/scalable_encoder.py needs a GPU; nothing is measured without one")
-    shallow_encoder.torch = torch
     import euler_b200 as eb
     from euler_b200.encoders import SageEncoder, ScalableSageEncoder
     torch.cuda.set_device(0)
@@ -135,13 +125,11 @@ def run(args):
 
     arms = {"scalable_sage_step": scal_step, "sage_step": sage_step, "store_ops": store_ops, "store_ops_torch": store_ops_torch}
     res = timed(arms, args.steps, args.warmup)
-    emit({"metric": "scalable_sage_step_ms", "value": res["scalable_sage_step"]["ms_per_call"], "gate": "passed",
-          "gpu": gpu_info(0), "batch": args.batch, "dim": args.dim, "fanout": args.fanout, "shapes": sh, "setup_s": setup_s,
-          "arms": res})
+    harness.emit({"metric": "scalable_sage_step_ms", "value": res["scalable_sage_step"]["ms_per_call"], "gate": "passed",
+                  "gpu": harness.gpu_info(0), "batch": args.batch, "dim": args.dim, "fanout": args.fanout, "shapes": sh, "setup_s": setup_s,
+                  "arms": res})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

@@ -19,23 +19,12 @@ The arms alternate in rounds in one process.  Then a large-vocabulary case: slot
 per second and torch's allocator peak above the inputs; the card's name, power limit and SM clock read in the same run.
 Anything not run is reported as "not measured".  One JSON line on stdout."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from bench import GRAPH_SEED  # noqa: E402
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-from sparse_embedding import SLOTS, slot_arrays  # noqa: E402
-
-DENSE_DIM, DIM = 128, 16
+from harness import DENSE_DIM, DIM, SLOTS, build_graph, timed
 
 
 def parse(argv=None):
@@ -48,20 +37,6 @@ def parse(argv=None):
     p.add_argument("--warmup", type=int, default=3)
     p.add_argument("--big-rows", type=int, default=100_000_000, help="rows of the large-vocabulary slot table (0: skip)")
     return p.parse_args(argv)
-
-
-def build_graph(args):
-    import euler_b200 as eb
-    g0 = eb.Graph.rmat(args.nodes, args.edges, seed=GRAPH_SEED, feat_dim=DENSE_DIM, device=0)
-    csr = g0.export(with_feat=True)
-    g0.close()
-    ptr, vals = slot_arrays(args.nodes)
-    g = eb.Graph.from_csr(csr["ids"], csr["grp_ptr"], csr["nbr"], n_edge_types=csr["T"], cum_w=csr["cum_w"], grp_cum=csr["grp_cum"],
-                          node_type=csr["node_type"], node_w=csr["node_w"], feat=csr["feat"], feat_slot_dims=[DENSE_DIM],
-                          u64_ptr=ptr, u64_val=vals, n_u64_slots=2)
-    del csr
-    eb.set_graph(g, rng="philox", seed=5)
-    return g
 
 
 def composed(eb, F, nodes, id_table, tables, sparse_grad):
@@ -119,34 +94,6 @@ def gate(eb, F, hops, id_table, tables):
             raise SystemExit("GATE FAILED: table %d's sparse gradient differs from its dense one" % t)
 
 
-def timed(arms, steps, warmup):
-    peak = {}
-    for k, fn in arms.items():
-        for _ in range(warmup):
-            fn()
-        torch.cuda.synchronize()
-        a0 = torch.cuda.memory_allocated()
-        torch.cuda.reset_peak_memory_stats()
-        fn()
-        torch.cuda.synchronize()
-        peak[k] = int(torch.cuda.max_memory_allocated() - a0)
-    rounds = max(1, min(5, steps))
-    per = -(-steps // rounds)
-    tot = {k: [0.0, 0] for k in arms}
-    for _ in range(rounds):
-        for k, fn in arms.items():
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(per):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            tot[k][0] += e0.elapsed_time(e1)
-            tot[k][1] += per
-    return {k: {"ms_per_call": v[0] / v[1], "calls": v[1], "torch_peak_bytes": peak[k]} for k, v in tot.items()}
-
-
 def run(args):
     global torch
     import torch
@@ -175,13 +122,11 @@ def run(args):
         big = timed({k: arms[k] for k in big}, max(1, args.steps // 4), 1)
         big["table_bytes"] = args.big_rows * DIM * 4
         del big_tables, arms
-    emit({"metric": "shallow_encoder_fwd_rows_per_sec", "value": res["fused_fwd"]["rows_per_sec"], "gate": "passed",
-          "gpu": gpu_info(0), "batch": args.batch, "fanout": fanout, "rows": rows, "row_width": DIM + DENSE_DIM + DIM * len(SLOTS),
-          "setup_s": setup_s, "arms": res, "large_vocabulary": {"rows": args.big_rows, "dim": DIM, "arms": big}})
+    harness.emit({"metric": "shallow_encoder_fwd_rows_per_sec", "value": res["fused_fwd"]["rows_per_sec"], "gate": "passed",
+                  "gpu": harness.gpu_info(0), "batch": args.batch, "fanout": fanout, "rows": rows, "row_width": DIM + DENSE_DIM + DIM * len(SLOTS),
+                  "setup_s": setup_s, "arms": res, "large_vocabulary": {"rows": args.big_rows, "dim": DIM, "arms": big}})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

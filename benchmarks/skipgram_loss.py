@@ -17,21 +17,13 @@ library's ctx scratch took (the growth of the device's used memory outside torch
 (walk -> pairs -> negatives -> loss -> backward -> SGD) is timed fused and composed.  The card's name, power limit and SM
 clock are read in the same run.  One JSON line on stdout."""
 import argparse
-import json
 import os
 import shutil
-import subprocess
-import sys
 import tempfile
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-
-from bench import GRAPH_SEED  # noqa: E402
-from full_dataflow import gpu_info  # noqa: E402
+import harness
+from bench import GRAPH_SEED
 
 ARMS = ("fwd", "fwd_bwd", "fwd_bwd_sparse")
 
@@ -104,16 +96,8 @@ def mem_arm(args):
     ids = tuple(x.cuda() for x in saved["ids"])
     eb.set_graph(eb.Graph.rmat(1000, 5000, seed=1), rng="minstd", seed=1)   # a ctx; the ids index the tables only
     t, c = tables(saved["n_rows"], int(dim), arm != "fwd")
-    torch.cuda.synchronize()
-    free0 = torch.cuda.mem_get_info()[0]
-    res0 = torch.cuda.memory_reserved()
-    a0 = torch.cuda.memory_allocated()
-    torch.cuda.reset_peak_memory_stats()
-    run_arm(kind, arm, ids, t, c)
-    torch.cuda.synchronize()
-    peak = torch.cuda.max_memory_allocated() - a0
-    outside = (free0 - torch.cuda.mem_get_info()[0]) - (torch.cuda.memory_reserved() - res0)
-    print(json.dumps({"torch_peak_bytes": int(peak), "ctx_scratch_bytes": int(max(outside, 0))}))
+    peak, outside = harness.memory_of(lambda: run_arm(kind, arm, ids, t, c))
+    harness.emit({"torch_peak_bytes": peak, "ctx_scratch_bytes": max(outside, 0)})
 
 
 def main(args):
@@ -130,7 +114,7 @@ def main(args):
     n = pair.shape[0] * pair.shape[1]
     ids = (pair[:, :, 0].reshape(n, 1).contiguous(), pair[:, :, 1].reshape(n, 1).contiguous(),
            eb.sample_node(n * args.negs, 0).reshape(n, args.negs))
-    out = {"what": "skip-gram step (loss + mrr), fused eu_skipgram_loss vs torch composition", "gpu": gpu_info(0),
+    out = {"what": "skip-gram step (loss + mrr), fused eu_skipgram_loss vs torch composition", "gpu": harness.gpu_info(0),
            "pairs": n, "K": args.negs, "nodes": args.nodes, "rows_touched": int(torch.unique(torch.cat([x.reshape(-1) for x in ids])).numel()),
            "results": {}}
     tmp = tempfile.mkdtemp(prefix="skipgram_bench_")
@@ -152,25 +136,17 @@ def main(args):
         assert abs(float(lf) - l64) <= 1e-6 * l64, ("loss gate", dim, gate)
         assert abs(float(mf) - float(mc)) <= 1e-4, ("metric gate", dim, gate)
         del gtf, gcf
-        ms = {(k, a): [] for k in ("fused", "composed") for a in ARMS}
-        for r in range(args.warmup + args.steps):
-            for key in ms:
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                run_arm(key[0], key[1], ids, t, c)
-                e1.record()
-                torch.cuda.synchronize()
-                if r >= args.warmup:
-                    ms[key].append(e0.elapsed_time(e1))
+        ms = harness.time_arms({(k, a): (lambda k=k, a=a: run_arm(k, a, ids, t, c)) for k in ("fused", "composed") for a in ARMS},
+                               args.steps, args.warmup)
         t.grad = c.grad = None
         del t, c
         torch.cuda.empty_cache()
         res = {}
         for (k, a), v in ms.items():
-            mem = subprocess.run([sys.executable, __file__, "--mem-arm", "%s:%s:%d" % (k, a, dim), "--ids", ids_path],
-                                 capture_output=True, text=True, timeout=600)
-            m = json.loads(mem.stdout.strip().splitlines()[-1]) if mem.returncode == 0 else {"error": mem.stderr[-500:]}
+            try:
+                m = harness.in_fresh_process(__file__, ["--mem-arm", "%s:%s:%d" % (k, a, dim), "--ids", ids_path])
+            except SystemExit as e:
+                m = {"error": str(e)[-500:]}
             res["%s_%s" % (k, a)] = {"ms_median": float(np.median(v)), "ms_min": float(np.min(v)), "ms_max": float(np.max(v)), **m}
         for a in ARMS:
             res["speedup_" + a] = res["composed_" + a]["ms_median"] / res["fused_" + a]["ms_median"]
@@ -200,10 +176,11 @@ def main(args):
         torch.cuda.empty_cache()
     out["deepwalk_step_dim128"] = step
     shutil.rmtree(tmp, ignore_errors=True)
-    print(json.dumps(out))
+    harness.emit(out)
 
 
 if __name__ == "__main__":
+    harness.divert_stdout()
     a = parse()
     if a.mem_arm:
         mem_arm(a)

@@ -14,21 +14,12 @@ the gate allows for the rounding of either; tests/test_solution_gpu.py checks th
 Reported per arm: ms per step and torch's allocator peak above the inputs; the card's name, power limit and max SM clock read in
 the same run.  One JSON line on stdout.  It needs a GPU: without one it fails rather than measure anything else."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
+import harness
+import numpy as np
+from harness import timed
 
-import numpy as np  # noqa: E402
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-import shallow_encoder  # noqa: E402
-from shallow_encoder import timed  # noqa: E402
 
 FEAT, DIM, FANOUTS, NEGS, BATCHES = 128, 128, [10, 10], 5, (512, 2048)
 
@@ -86,7 +77,6 @@ def run(args):
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("benchmarks/solution_step.py needs a GPU; nothing is measured without one")
-    shallow_encoder.torch = torch
     import euler_b200 as eb
     torch.cuda.set_device(0)
     t0 = time.time()
@@ -105,13 +95,11 @@ def run(args):
             arms["step_b%d_%s" % (B, "fused" if f else "composed")] = (lambda s=sols[f], x=seeds[B]: step(eb, s[0], s[1], x))
     arms["sample_node_with_src_2048x5"] = lambda: eb.sample_node_with_src(seeds[2048], NEGS)
     res = timed(arms, args.steps, args.warmup)
-    emit({"metric": "unsupervised_sage_step_b2048_fused_ms", "value": res["step_b2048_fused"]["ms_per_call"], "gate": "passed",
-          "gpu": gpu_info(0), "batches": list(BATCHES), "fanouts": FANOUTS, "dim": DIM, "num_negs": NEGS, "setup_s": setup_s,
-          "arms": res})
+    harness.emit({"metric": "unsupervised_sage_step_b2048_fused_ms", "value": res["step_b2048_fused"]["ms_per_call"], "gate": "passed",
+                  "gpu": harness.gpu_info(0), "batches": list(BATCHES), "fanouts": FANOUTS, "dim": DIM, "num_negs": NEGS, "setup_s": setup_s,
+                  "arms": res})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

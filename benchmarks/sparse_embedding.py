@@ -17,23 +17,13 @@ float64 on 4096 hop-2 rows; a mismatch aborts.  The arms alternate in rounds in 
 call, embedded rows per second, torch's allocator peak above the inputs, the algorithmic bytes (entries * dim * 4 read,
 rows * dim * 4 written), and the card's name, power limit and SM clock read in the same run.  One JSON line on stdout."""
 import argparse
-import os
-import sys
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+import harness
+import numpy as np
 
-import numpy as np  # noqa: E402
-
-from bench import GRAPH_SEED  # noqa: E402
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-
-SLOTS = (("u64_0", 10 ** 6), ("u64_1", 10 ** 7))   # name, max_id + 1 (the default value; the table has one more row)
+from bench import GRAPH_SEED
+from harness import SLOTS, slot_arrays
 
 
 def parse(argv=None):
@@ -45,25 +35,6 @@ def parse(argv=None):
     p.add_argument("--steps", type=int, default=20)
     p.add_argument("--warmup", type=int, default=3)
     return p.parse_args(argv)
-
-
-def slot_arrays(n, seed=2024):
-    """u64_ptr [n * 2 + 1] and u64_val of the two seeded slots"""
-    rng = np.random.RandomState(seed)
-    la = rng.randint(1, 9, size=n)
-    la[rng.rand(n) < 0.2] = 0
-    big = rng.rand(n) < 0.001
-    la[big] = rng.randint(300, 2001, size=int(big.sum()))
-    lb = rng.randint(1, 5, size=n)
-    lens = np.stack([la, lb], axis=1).reshape(-1).astype(np.int64)
-    ptr = np.zeros(2 * n + 1, np.int64)
-    np.cumsum(lens, out=ptr[1:])
-    slot = np.repeat(np.tile(np.arange(2, dtype=np.int8), n), lens)
-    vals = np.empty(int(ptr[-1]), np.uint64)
-    na, nb = int((slot == 0).sum()), int((slot == 1).sum())
-    vals[slot == 0] = (rng.zipf(1.2, size=na) - 1) % SLOTS[0][1]
-    vals[slot == 1] = rng.randint(0, SLOTS[1][1], size=nb)
-    return ptr, vals
 
 
 def build_graph(args):
@@ -181,44 +152,18 @@ def run(args):
             gen = torch.Generator(device="cuda").manual_seed(dim)
             tables = [(torch.randn(m + 1, dim, device="cuda", generator=gen) * 0.01).requires_grad_(True) for _, m in SLOTS]
             gate(eb, er, ids, ptr, vals, hops, tables, combiner)
-            arms = make_arms(eb, F, seeds, fanout, hops, tables, combiner)
-            peak = {}
-            for k, fn in arms.items():
-                for _ in range(args.warmup):
-                    fn()
-                torch.cuda.synchronize()
-                a0 = torch.cuda.memory_allocated()
-                torch.cuda.reset_peak_memory_stats()
-                fn()
-                torch.cuda.synchronize()
-                peak[k] = int(torch.cuda.max_memory_allocated() - a0)
-            rounds = max(1, min(5, args.steps))
-            per = -(-args.steps // rounds)
-            tot = {k: [0.0, 0] for k in arms}
-            for _ in range(rounds):
-                for k, fn in arms.items():
-                    torch.cuda.synchronize()
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                    for _ in range(per):
-                        fn()
-                    e1.record()
-                    torch.cuda.synchronize()
-                    tot[k][0] += e0.elapsed_time(e1)
-                    tot[k][1] += per
+            res = harness.timed(make_arms(eb, F, seeds, fanout, hops, tables, combiner), args.steps, args.warmup)
             alg = 4 * dim * (sum(entries.values()) + rows * len(SLOTS))
-            results.append({"dim": dim, "combiner": combiner, "algorithmic_fwd_bytes": alg, "arms": {
-                k: {"ms_per_call": v[0] / v[1], "rows_per_sec": rows * len(SLOTS) / (v[0] / v[1] * 1e-3), "calls": v[1],
-                    "torch_peak_bytes": peak[k]} for k, v in tot.items()}})
-            del tables, arms
+            for v in res.values():
+                v["rows_per_sec"] = rows * len(SLOTS) / (v["ms_per_call"] * 1e-3)
+            results.append({"dim": dim, "combiner": combiner, "algorithmic_fwd_bytes": alg, "arms": res})
+            del tables
     head = [r for r in results if r["dim"] == 64 and r["combiner"] == "sum"][0]["arms"]
-    emit({"metric": "sparse_embedding_lookup_rows_per_sec", "value": head["lookup_fused_fwd"]["rows_per_sec"],
-          "gate": "passed", "gpu": gpu_info(0), "batch": args.batch, "fanout": fanout, "rows_per_slot": rows,
-          "entries_per_slot": entries, "setup_s": setup_s, "results": results})
+    harness.emit({"metric": "sparse_embedding_lookup_rows_per_sec", "value": head["lookup_fused_fwd"]["rows_per_sec"],
+                  "gate": "passed", "gpu": harness.gpu_info(0), "batch": args.batch, "fanout": fanout, "rows_per_slot": rows,
+                  "entries_per_slot": entries, "setup_s": setup_s, "results": results})
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())

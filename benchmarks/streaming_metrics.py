@@ -18,18 +18,9 @@ Then one SuperviseModel step (forward, backward, SGD) over SageEncoder([[0], [0]
 Reported per arm: us per call and torch's allocator peak above the inputs; the card's name, power limit and max SM clock read
 in the same run.  One JSON line on stdout.  It needs a GPU: without one it fails rather than measure anything else."""
 import argparse
-import os
-import sys
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, HERE)
-
-from full_dataflow import emit, gpu_info  # noqa: E402
-import full_dataflow  # noqa: E402
-import shallow_encoder  # noqa: E402
-from shallow_encoder import timed  # noqa: E402
+import harness
+from harness import timed
 
 WORKLOADS = [(61952, 5000), (61952, 200), (20480, 5000), (20480, 200), (1 << 20, 5000), (1 << 20, 200)]
 LITERAL_MAX = 400_000_000
@@ -85,14 +76,13 @@ def composed_update(lab, p, thr, st):
 def run(args):
     global torch
     import torch
-    shallow_encoder.torch = torch
     assert torch.cuda.is_available(), "streaming_metrics.py needs a GPU"
     import euler_b200 as eb
     from euler_b200 import ops
     dev = torch.device("cuda", 0)
     g = eb.Graph.rmat(args.nodes, args.edges, seed=42, feat_dim=128, device=0)
     eb.set_graph(g, rng="minstd", seed=5)
-    out = {"gpu": gpu_info(0), "workloads": []}
+    out = {"gpu": harness.gpu_info(0), "workloads": []}
     gen = torch.Generator(device=dev).manual_seed(1)
     for N, T in WORKLOADS:
         x = torch.randn(N, generator=gen, device=dev)
@@ -125,7 +115,7 @@ def run(args):
             r["us_per_call"] = r.pop("ms_per_call") * 1000.0
         out["workloads"].append({"N": N, "T": T, "arms": res, "literal_skipped": "literal" not in names})
     out["supervise_step"] = model_step(args, eb, dev)
-    emit(out)
+    harness.emit(out)
 
 
 def model_step(args, eb, dev):
@@ -164,7 +154,5 @@ def model_step(args, eb, dev):
 
 
 if __name__ == "__main__":
-    sys.stdout.flush()
-    full_dataflow._REAL_STDOUT = os.dup(1)
-    os.dup2(2, 1)
+    harness.divert_stdout()
     run(parse())
